@@ -1,13 +1,17 @@
 #!/usr/bin/env python
-"""bench.py -- decode tokens/s of the B200 hot path (BASELINE.json metric) + roofline + CPU baseline.
+"""bench.py -- decode tokens/s of the H100 hot path (BASELINE.json metric) + roofline + CPU baseline.
 
-  python bench.py [--gpus N --steps K --warmup W] [--impl reference]
+  python bench.py [--gpus N --steps K --warmup W] [--impl reference] [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 A "step" = one full decode step (all layers: 4 GEMMs + rope/append + paged attention + norms, lm_head, greedy argmax)
 for a batch of synthetic sequences under ONE CUDA graph.  Default workload = the configuration BASELINE.json's metric is
-quoted on: Llama-3-8B INT4-AWQ(g128), batch 32, context 2048, one B200.  N > 1 = the reference's tensor-parallel split
+quoted on: Llama-3-8B INT4-AWQ(g128), batch 32, context 2048, one H100.  N > 1 = the reference's tensor-parallel split
 (strong scaling: the same batch, weights/heads sharded, NCCL all-reduce after the row-parallel GEMMs).
+
+--dump-outputs DIR writes what the last timed step computed -- logits.npy (float32 [batch, vocab], gathered over the vocab shards
+under TP) and next_ids.npy (float64 [batch], the greedy tokens) -- so that two builds can be compared output for output: the weights, KV cache, page tables and
+token ids are generated from fixed seeds, so the same arguments give the same inputs on every run.
 """
 import argparse
 import json
@@ -41,6 +45,8 @@ def parse():
     ap.add_argument("--program", type=int, default=int(os.environ.get("B200_PROGRAM", "0")))  # record the step into a decode program (persistent kernel between attention calls)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--comm", default=os.environ.get("B200_COMM", "peer"), choices=["peer", "nccl"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32 / float64, <= 64 MB in all)")
     return ap.parse_args()
 
 
@@ -50,7 +56,27 @@ def peaks():
             p = json.load(f)
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:  # noqa: BLE001
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
+
+
+DUMP_BUDGET = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes each array as out_dir/<name>.npy, smallest first. An array that does not fit in what is left of DUMP_BUDGET is
+    replaced by a fixed, seeded sample of its flattened elements (<name>.npy) plus the sampled flat indices (<name>_index.npy)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    left = DUMP_BUDGET
+    for name, a in sorted(arrays.items(), key=lambda kv: kv[1].nbytes):
+        if a.nbytes > left:
+            n = max(1, left // (a.itemsize + 8))
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=min(n, a.size), replace=False))
+            np.save(os.path.join(out_dir, f"{name}_index.npy"), idx.astype(np.float64))
+            a = a.reshape(-1)[idx]
+            left -= idx.size * 8
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+        left -= a.nbytes
 
 
 def model_cfg(args):
@@ -231,12 +257,10 @@ def main():
         t = torch.tensor([diff, rms_diff, -agree], device=dev, dtype=torch.float64)
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         # The two arms round differently by construction: ours sums the W partials in fp32 and rounds once, NCCL's fp16 ring
-        # rounds after every hop, and the difference accumulates over 2 x layers all-reduces (measured at TP8: max |d| 0.08 on
-        # logits of rms 1.28 over 4 M elements; rms |d| 0.010 for the 32-layer model, 0.022 for the 80-layer one). The criterion
-        # is therefore the RMS difference -- <= 1 % of the logit rms for 32 layers, scaled by sqrt(layers / 32) because the
-        # per-all-reduce rounding differences add up like a random walk -- plus agreement of the sampled tokens; the max is
-        # reported. Exact parity of the sharded step is the job of tests/test_gpu_tp.py and tools/tp_check.py (vs the UNSHARDED
-        # oracle: max logit error 0.003 at TP8, profiles/r02_tp8_parity.txt).
+        # rounds after every hop, and the difference accumulates over 2 x layers all-reduces. The criterion is therefore the
+        # RMS difference -- <= 1 % of the logit rms for 32 layers, scaled by sqrt(layers / 32) because the per-all-reduce
+        # rounding differences add up like a random walk -- plus agreement of the sampled tokens; the max is reported. Exact
+        # parity of the sharded step is the job of tests/test_gpu_tp.py and tools/tp_check.py (vs the UNSHARDED oracle).
         parity_check = {"against": "nccl all_reduce + all_gather + torch.argmax", "max_abs_logit_diff": t[0].item(),
                         "rms_logit_diff": t[1].item(), "logit_rms": rms, "token_agreement": -t[2].item(),
                         "rms_tolerance": 1e-2 * rms * (cfg.layers / 32.0) ** 0.5,
@@ -257,44 +281,56 @@ def main():
         model.replay()
     barrier()
     sampler = ClockSampler(local_rank) if rank == 0 else None
-    st, en = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    st.record()
-    for _ in range(args.steps):
-        model.replay()
-    en.record()
-    barrier()
-    ms = st.elapsed_time(en) / args.steps
+    try:
+        st, en = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        st.record()
+        for _ in range(args.steps):
+            model.replay()
+        en.record()
+        barrier()
+        ms = st.elapsed_time(en) / args.steps
+        if args.dump_outputs:
+            # the outputs of the last timed replay (the later e2e / attention timings do not feed them back); under TP the
+            # vocab shards are gathered into the full [batch, vocab] logits (every rank takes part, rank 0 writes)
+            logits = model.logits
+            if tp > 1:
+                shards = torch.empty(tp, *model.logits.shape, dtype=model.logits.dtype, device=dev)
+                dist.all_gather_into_tensor(shards, model.logits)
+                logits = shards.permute(1, 0, 2).reshape(args.batch, -1)[:, : cfg.vocab]
+            if rank == 0:
+                dumped = {"logits": logits.float().cpu().numpy(), "next_ids": model.next_ids.cpu().numpy().astype("float64")}
 
-    # ---- end to end ("e2e"): host buffers -> H2D -> step -> D2H, every step, through the public call
-    for _ in range(3):
-        model.upload_inputs(); model.replay(); model.download_outputs()
-    barrier()
-    st.record()
-    for _ in range(args.steps):
-        model.upload_inputs()
-        model.replay()
-        model.download_outputs()
-        torch.cuda.current_stream(dev).synchronize()   # the caller needs the sampled tokens before the next step
-    en.record()
-    barrier()
-    ms_e2e = st.elapsed_time(en) / args.steps
+        # ---- end to end ("e2e"): host buffers -> H2D -> step -> D2H, every step, through the public call
+        for _ in range(3):
+            model.upload_inputs(); model.replay(); model.download_outputs()
+        barrier()
+        st.record()
+        for _ in range(args.steps):
+            model.upload_inputs()
+            model.replay()
+            model.download_outputs()
+            torch.cuda.current_stream(dev).synchronize()   # the caller needs the sampled tokens before the next step
+        en.record()
+        barrier()
+        ms_e2e = st.elapsed_time(en) / args.steps
 
-    # ---- dominant kernel (paged decode attention): average launch duration, CUDA events on the launching stream,
-    #      each launch reads a different layer's 268 MB of K/V (> L2), same inputs as inside the step
-    n_attn = 0
-    for _ in range(3):
-        ops.paged_decode_attn(model.q, model.layers[0]["kv"], model.page_list, model.seq_lens, model.ctx, model.attn_ws,
-                              out=model.attn)
-    torch.cuda.synchronize(dev)
-    st.record()
-    for _ in range(max(1, args.steps // 5)):
-        for L in model.layers:
-            ops.paged_decode_attn(model.q, L["kv"], model.page_list, model.seq_lens, model.ctx, model.attn_ws, out=model.attn)
-            n_attn += 1
-    en.record()
-    barrier()
-    attn_ms = st.elapsed_time(en) / n_attn
-    clocks = sampler.stop() if sampler else None
+        # ---- dominant kernel (paged decode attention): average launch duration, CUDA events on the launching stream,
+        #      each launch reads a different layer's 268 MB of K/V (> L2), same inputs as inside the step
+        n_attn = 0
+        for _ in range(3):
+            ops.paged_decode_attn(model.q, model.layers[0]["kv"], model.page_list, model.seq_lens, model.ctx, model.attn_ws,
+                                  out=model.attn)
+        torch.cuda.synchronize(dev)
+        st.record()
+        for _ in range(max(1, args.steps // 5)):
+            for L in model.layers:
+                ops.paged_decode_attn(model.q, L["kv"], model.page_list, model.seq_lens, model.ctx, model.attn_ws, out=model.attn)
+                n_attn += 1
+        en.record()
+        barrier()
+        attn_ms = st.elapsed_time(en) / n_attn
+    finally:
+        clocks = sampler.stop() if sampler else None   # never leave the nvidia-smi sampler running
 
     if tp > 1:
         t = torch.tensor([ms, ms_e2e, attn_ms], device=dev, dtype=torch.float64)
@@ -307,13 +343,6 @@ def main():
         attn_bytes = ab["kv"] / cfg.layers
         achieved = attn_bytes / (attn_ms * 1e-3) / 1e9
         step_gbs = ab["total"] / (ms * 1e-3) / 1e9
-        traffic = None
-        tfile = os.path.join(ROOT, "profiles", "attn_traffic_bytes.json")
-        if os.path.exists(tfile):
-            try:
-                traffic = json.load(open(tfile)).get(f"b{args.batch}_ctx{args.ctx}_tp{tp}")   # from an `ncu --set full` capture (profiles/README.md), not measured in this run
-            except Exception:  # noqa: BLE001
-                traffic = None
         line = {
             "metric": METRIC, "value": args.batch / (ms * 1e-3), "unit": UNIT, "n_gpus": tp, "steps": args.steps,
             "warmup": max(args.warmup, 3), "ms_per_step": ms, "higher_is_better": True, "scaling": "strong",
@@ -332,8 +361,7 @@ def main():
             "launches_per_step": launches_per_step,
             "clocks": clocks,
             "roofline": {"kernel": "paged_decode_attn_kernel", "bound": "hbm", "achieved": achieved, "peak": peak,
-                         "unit": "GB/s", "frac": achieved / peak, "traffic": traffic, "traffic_source": ("ncu --set full capture, profiles/r01_ncu_attn_b32_s2048_summary.txt" if traffic else None),
-                         "peak_source": peak_src,
+                         "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src,
                          "bytes_per_launch": attn_bytes, "us_per_launch": attn_ms * 1e3},
             "step_roofline": {"algorithmic_bytes_per_gpu": ab["total"], "achieved_gbs": step_gbs, "frac": step_gbs / peak,
                               "roofline_tokens_per_s": args.batch / (ab["total"] / (peak * 1e9)), "split": ab},
@@ -342,6 +370,8 @@ def main():
             cb = cpu_arm(args, cfg)
             line["cpu_baseline"] = {k: cb[k] for k in ("value", "unit", "cores", "kind", "sample")}
         print(json.dumps(line))
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, dumped)
     if tp > 1:
         # Teardown: process groups whose collectives were captured in CUDA graphs hang in destroy_process_group
         # (observed: NCCL watchdog stuck in CudaEventDestroy). Drop the graph, sync, and leave without the destructor.

@@ -1,5 +1,5 @@
 /*
- * b200_decode_ops.h -- C ABI of libb200_decode.so: the B200-native (sm_100a) decode hot path of rtp-llm.
+ * b200_decode_ops.h -- C ABI of libb200_decode.so: the Hopper-native (H100, sm_90a) decode hot path of rtp-llm.
  *
  * This is the drop-in boundary.  Every entry point takes plain device pointers, sizes and a cudaStream_t (passed as
  * void*), returns 0 on success or a negative B200_E* code (message via b200_last_error()), never synchronises the
@@ -21,7 +21,7 @@ extern "C" {
 #define B200_OK 0
 #define B200_EINVAL (-1)      /* bad argument (shape, alignment, unsupported configuration) */
 #define B200_ECUDA (-2)       /* a CUDA runtime / driver call failed */
-#define B200_EUNSUPPORTED (-3) /* not an sm_100 device, or feature outside the built scope */
+#define B200_EUNSUPPORTED (-3) /* not an sm_90 device, or feature outside the built scope */
 
 /* weight formats of b200_wo_gemm */
 #define B200_FMT_F16 0   /* W stored [N][K] (K contiguous), element type = activation type */
@@ -37,7 +37,7 @@ extern "C" {
 /* Last error message of the calling thread ("" if none). */
 const char* b200_last_error(void);
 
-/* 0 if device `device` is sm_100 (B200) and the library's kernels can run there, else B200_EUNSUPPORTED. */
+/* 0 if device `device` is sm_90 (H100) and the library's kernels can run there, else B200_EUNSUPPORTED. */
 int b200_device_check(int device);
 
 /* Library-wide switch: launch the kernels of the decode chain (norms, rope, attention, GEMMs) with programmatic dependent
@@ -259,7 +259,7 @@ int b200_peer_argmax(const void* logits, int is_bf16, int rows, int vocab_local,
 
 /* ------------------------------------------------------------------------------------------------ decode programs */
 
-/* A decode program is a recorded sequence of the op calls above, replayed with far fewer launches -- the B200 counterpart
+/* A decode program is a recorded sequence of the op calls above, replayed with far fewer launches -- this library's counterpart
  * of the reference's CUDA-graph capture of the decode step (rtp_llm/cpp/cuda_graph/cuda_graph_runner.cc: capture once per
  * batch size, replay every step).  Between b200_program_begin and b200_program_end every op call of the CALLING THREAD is
  * appended to the program instead of being launched (arguments are checked and launch shapes planned at record time;

@@ -113,7 +113,7 @@ def load() -> ctypes.CDLL:
                 _build.build()
             except Exception as e:  # noqa: BLE001
                 raise B200Error(f"{LIB_PATH} is missing and could not be built ({e}): run `python -m rtp_llm_b200.build` "
-                                "(nvcc, sm_100a). There is no fallback path.") from e
+                                "(nvcc, sm_90a). There is no fallback path.") from e
         else:
             _rebuild_if_stale()
         lib = ctypes.CDLL(LIB_PATH)

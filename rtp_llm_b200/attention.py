@@ -63,7 +63,7 @@ class B200DecodeAttnOp:
               and _tokens_per_block(c) in (16, 32, 64, 128))
         kv_dtype = str(getattr(c, "kv_cache_dtype", "BASE"))
         return ok and "FP8" not in kv_dtype.upper() and torch.cuda.is_available() and \
-            torch.cuda.get_device_capability()[0] == 10
+            torch.cuda.get_device_capability() == (9, 0)
 
     def prepare(self, attn_inputs) -> B200AttnParams:
         block_ids = attn_inputs.kv_cache_kernel_block_id_device

@@ -1,5 +1,5 @@
-"""Build libb200_decode.so (hand-written sm_100a CUDA + the C ABI) in-tree with nvcc. No JIT cache: the .so travels
-with the repo snapshot to the GPU box."""
+"""Build libb200_decode.so (hand-written sm_90a CUDA + the C ABI) in-tree with nvcc. No JIT cache: the library is built
+once, next to its sources, and loaded from there."""
 import os
 import subprocess
 import sys
@@ -11,7 +11,7 @@ OBJDIR = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libb200_decode.so")
 # translation units compile in parallel (the persistent-kernel instantiations dominate the build time)
 SOURCES = ["c_api.cu", "gemm_cluster.cu", "gemm_cluster_rs.cu", "segment_f16.cu", "segment_bf16.cu"]
-NVCC_FLAGS = ["-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3",
+NVCC_FLAGS = ["-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3",
               "-Xcompiler", "-fPIC", "-DB200_BUILD"]
 if os.environ.get("B200_DEV"):           # developer build: clock64 timeline + ablation switches in the cluster GEMM (tools/gemm_trace.py)
     NVCC_FLAGS.append("-DB200_GEMM_DEV")  # goes to its own library (lib_dev.so, loaded through B200_LIB_PATH), never the product one
@@ -94,7 +94,7 @@ def build_testref(force: bool = False) -> str:
     if not force and not _newer(TESTREF_LIB, [TESTREF_SRC, os.path.join(CSRC, "ptx.cuh")]):
         return TESTREF_LIB
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    subprocess.check_call([nvcc, "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-O2", "-shared", "-Xcompiler", "-fPIC",
+    subprocess.check_call([nvcc, "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-shared", "-Xcompiler", "-fPIC",
                            "-o", TESTREF_LIB, TESTREF_SRC, "-lcudart"])
     return TESTREF_LIB
 

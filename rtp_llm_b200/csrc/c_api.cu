@@ -62,10 +62,10 @@ int num_sms() {
     static int sms[16] = {};
     int dev = 0;
     cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 16) return 148;
+    if (dev < 0 || dev >= 16) return 132;
     if (!sms[dev]) {
         cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev);
-        if (sms[dev] <= 0) sms[dev] = 148;
+        if (sms[dev] <= 0) sms[dev] = 132;   // no device (host-only planning): an H100 SXM
     }
     return sms[dev];
 }
@@ -147,10 +147,10 @@ void attn_split(int units, int max_tiles, int* nsplit, int* tiles_per_split, int
     int best_c = max_tiles;
     double best = 1e30;
     const int sms = num_sms();
-    // Model fitted to measurements on B200 (profiles/r01_kernel_bench.txt, tools/tp8_shapes.py; within ~10 % for 32..256
-    // (sequence, kv-head) units): a CTA has ~3 us of fixed time, streams its 32 KB tiles at min(60 GB/s -- what its 96 KB ring
-    // sustains --, HBM / resident CTAs), CTAs beyond 2*SMs are back-filled (fractional waves), a split adds ~3 us of merge.
-    const double slots = 2.0 * sms, hbm = 6.2e12, r_cta = 60e9, fixed = 3e-6, merge = 3e-6, tile_bytes = 32768.0 * head_dim / 128.0;
+    // Cost model (not refitted on H100; hbm = what an H100 SXM's 3.35 TB/s HBM3 sustains in practice): a CTA has ~3 us of
+    // fixed time, streams its 32 KB tiles at min(60 GB/s -- what its 96 KB ring sustains --, HBM / resident CTAs), CTAs
+    // beyond 2*SMs are back-filled (fractional waves), a split adds ~3 us of merge.
+    const double slots = 2.0 * sms, hbm = 3.0e12, r_cta = 60e9, fixed = 3e-6, merge = 3e-6, tile_bytes = 32768.0 * head_dim / 128.0;
     const bool cluster_ok = env_int("B200_ATTN_CLUSTER", 1) != 0;
     for (int c = 1; c <= max_tiles; ++c) {
         const int ns = (max_tiles + c - 1) / c;
@@ -358,8 +358,8 @@ int b200_device_check(int device) {
     cudaDeviceProp prop;
     cudaError_t e = cudaGetDeviceProperties(&prop, device);
     if (e != cudaSuccess) return fail(B200_EUNSUPPORTED, "no CUDA device %d: %s", device, cudaGetErrorString(e));
-    if (prop.major != 10) return fail(B200_EUNSUPPORTED, "device %d is sm_%d%d, this library is sm_100a only", device,
-                                      prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(B200_EUNSUPPORTED, "device %d is sm_%d%d, this library is sm_90a only", device, prop.major, prop.minor);
     if (!encode_fn()) return fail(B200_EUNSUPPORTED, "driver lacks cuTensorMapEncodeTiled");
     return B200_OK;
 }
@@ -716,7 +716,7 @@ int wo_gemm_impl(int fmt, int is_bf16, const void* x, int B, int K, int N, const
 
     // ---- weight-only INT8 / INT4 at decode batches: inside a decode program the GEMM is an op of the persistent kernel
     // (uniform split-K merged through L2). A stand-alone call uses the cluster kernel below (split-K merged through DSMEM):
-    // measured on B200 at B=32 (profiles/r02_gemm_paths.txt) the cluster kernel is faster for every Llama-3-8B shape;
+    // the cluster kernel has no grid-wide barrier, so it is the default outside a program;
     // B200_GEMM_PERSISTENT=1 routes stand-alone calls through the persistent kernel too (experiments / tests).
     const bool seg_capable = (fmt == B200_FMT_INT8 || fmt == B200_FMT_INT4) && bpad <= 64;   // INT8G / FP16: cluster kernel only
     const bool streamk = seg_capable && !rs && (recording_fused(kOpGemm) || env_int("B200_GEMM_PERSISTENT", 0));
@@ -780,13 +780,11 @@ int wo_gemm_impl(int fmt, int is_bf16, const void* x, int B, int K, int N, const
     p.k_blocks = K / kGemmBK;
     p.use_pdl = use_pdl ? 1 : 0;
     p.silu_mul = silu_mul ? 1 : 0;
-    p.dbg = 0;
 #ifdef B200_GEMM_DEV
     {
         const char* tr = getenv("B200_GEMM_TRACE_PTR");   // developer timeline buffer (device pointer)
         p.trace = (tr && *tr) ? reinterpret_cast<long long*>(strtoull(tr, nullptr, 0)) : nullptr;
     }
-    p.dbg = env_int("B200_GEMM_DBG", 0);
 #endif
     p.cluster_reduce = (rs || env_int("B200_GEMM_CLUSTER", 1)) ? 1 : 0;   // split-K merge through DSMEM (cluster <= 8) vs global semaphores
 
@@ -902,7 +900,7 @@ int b200_silu_and_mul(const void* gate_up, void* y, int is_bf16, int rows, int i
     const size_t total = (size_t)rows * inter / 2;
     const int threads = 256;
     const size_t blocks = (total + threads - 1) / threads;
-    const unsigned g = (unsigned)(blocks < 4 * 148 * 8 ? blocks : 4 * 148 * 8);
+    const unsigned g = (unsigned)(blocks < 4 * num_sms() * 8 ? blocks : 4 * num_sms() * 8);
     const bool pdl = g_pdl.load() != 0;
     if (is_bf16)
         CUDA_CHECK(launch_ex(silu_and_mul_kernel<__nv_bfloat16>, dim3(g), dim3(threads), 0, (cudaStream_t)stream, pdl,

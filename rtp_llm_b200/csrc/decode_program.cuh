@@ -1,34 +1,32 @@
-// Persistent "decode program" kernel for sm_100a: the GEMMs and glue ops that sit between two attention calls of a decode
+// Persistent "decode program" kernel for sm_90a: the GEMMs and glue ops that sit between two attention calls of a decode
 // step run as ONE launch of 2 CTAs per SM; ops are separated by a grid-wide barrier (one atomic per CTA) instead of a
 // kernel boundary, and the weight stream never stops at an op boundary.
 //
-// Why (profiles/r01_kernel_bench.txt, VERDICT r1 weak #4-#6): a stand-alone weight-only GEMM pays ~7 us of fixed cost
-// (launch gap, barrier init + TMEM alloc, pipeline fill, epilogue, tail) around a 1.5-12 us main loop, and the glue kernels
-// pay ~4 us each for ~0 bytes.  Here
-//   * barrier init / TMEM alloc happen once per launch, not once per op;
+// Why: a stand-alone weight-only GEMM pays a fixed cost of several microseconds (launch gap, barrier init, pipeline fill,
+// epilogue, tail) around a main loop of comparable length, and the glue kernels pay a launch each for ~0 bytes.  Here
+//   * barrier init happens once per launch, not once per op;
 //   * every weight-only GEMM is split stream-K: the (n-tile, k-block) work list is cut into equal runs, one per CTA, so all
 //     2*SMs CTAs stream the same number of weight bytes whatever the tile count is; a tile that spans CTAs is finished by
 //     its lowest contributor from the others' fp32 partials in L2 (fixed summation order -> deterministic);
-//   * the four warp roles run as four independent loops over the op list.  The weight producer depends on nothing but its
+//   * the three warp roles run as three independent loops over the op list.  The weight producer depends on nothing but its
 //     ring slots, so it streams the NEXT GEMM's weights while the other warps are still in this op's epilogue, in a glue
 //     op, or waiting at the grid barrier.
 // What the reference does instead: one kernel per op under a CUDA graph (rtp_llm/cpp/cuda_graph/cuda_graph_runner.cc);
 // the op-by-op C ABI stays (include/b200_decode_ops.h) -- a program is RECORDED from the same calls (b200_program_*),
 // exactly like a graph capture.
 //
-// Roles (352 threads): warps 0-7 dequant + epilogue + glue ops ("dq"), warp 8 weight TMA, warp 9 activation TMA,
-// warp 10 MMA issue.  GEMM data path as in wo_gemm.cuh (weights dequantised in registers into TMEM, tcgen05.mma
-// A-from-TMEM x B-from-smem, fp32 accumulators in TMEM).
+// Roles (320 threads): warps 0-7 = two warpgroups for dequant + MMA + epilogue + glue ops ("dq"), warp 8 weight TMA,
+// warp 9 activation TMA.  GEMM data path as in wo_gemm.cuh (weights dequantised in registers into wgmma A fragments,
+// wgmma A-from-registers x B-from-smem, fp32 accumulators in registers).
 #pragma once
 #include "aux_kernels.cuh"
 #include "wo_gemm.cuh"
 
 namespace b200 {
 
-constexpr int kSegThreads = 352;
+constexpr int kSegThreads = 320;
 constexpr int kSegDqWarps = 8;
 constexpr int kSegDqThreads = kSegDqWarps * 32;
-constexpr int kSegAStages = 3;
 constexpr int kSegNormMaxVec = 4;
 constexpr int kSegNormMaxHidden = kSegNormMaxVec * kSegDqThreads * 8;
 
@@ -135,7 +133,7 @@ __device__ __forceinline__ void tensormap_acquire(const CUtensorMap* m) {
 }
 
 // developer fine-grained timeline (CTA 0 only): ftrace[op][slot][block] = clock64; slots: 0 W issue, 1 X issue, 2 dq wfull seen
-// (warp 0), 3 dq aempty seen, 4 dq afull arrive, 5 MMA operands ready, 6 MMA issued, 7 epilogue begin/end
+// (warp 0), 5 MMA operands ready, 6 MMA complete, 7 epilogue begin/end
 constexpr int kFtSlots = 8, kFtBlocks = 48;
 #define B200_FT(ft, slot, it)                                                                                      \
     do {                                                                                                           \
@@ -149,8 +147,6 @@ struct SegCfg {
     static constexpr int W_BYTES = gemm_w_bytes(FMT);
     static constexpr int WS = gemm_w_stages_for(FMT, BPAD, 106 * 1024);
     static constexpr int SMEM = XS * X_BYTES + WS * W_BYTES + kGemmSmemMisc;
-    static constexpr int TMEM_COLS = 256;
-    static_assert(BPAD + kSegAStages * 64 <= TMEM_COLS, "TMEM budget");
     static_assert(WS >= 3, "weight ring too shallow");
 };
 
@@ -166,13 +162,7 @@ struct SegSmem {
     __device__ __forceinline__ uint32_t wempty(uint32_t s) const { return base + BAR + 8 * (C::WS + s); }
     __device__ __forceinline__ uint32_t xfull(uint32_t s) const { return base + BAR + 8 * (2 * C::WS + s); }
     __device__ __forceinline__ uint32_t xempty(uint32_t s) const { return base + BAR + 8 * (2 * C::WS + C::XS + s); }
-    static constexpr uint32_t ABAR = BAR + 8 * (2 * C::WS + 2 * C::XS);
-    __device__ __forceinline__ uint32_t afull(uint32_t a) const { return base + ABAR + 8 * a; }
-    __device__ __forceinline__ uint32_t aempty(uint32_t a) const { return base + ABAR + 8 * (kSegAStages + a); }
-    __device__ __forceinline__ uint32_t dfull() const { return base + ABAR + 8 * (2 * kSegAStages); }
-    __device__ __forceinline__ uint32_t dempty() const { return base + ABAR + 8 * (2 * kSegAStages + 1); }
-    static constexpr uint32_t MISC = ABAR + 8 * (2 * kSegAStages + 2);
-    __device__ __forceinline__ uint32_t tmem_slot() const { return base + MISC; }
+    static constexpr uint32_t MISC = BAR + 8 * (2 * C::WS + 2 * C::XS);
     __device__ __forceinline__ uint32_t s_flag() const { return base + MISC + 4; }
     __device__ __forceinline__ uint32_t s_red(uint32_t w) const { return base + MISC + 16 + 4 * w; }
     static_assert(MISC + 16 + 4 * kSegDqWarps <= C::SMEM - 1024, "barrier area overflow");
@@ -235,66 +225,20 @@ __device__ __forceinline__ void seg_x_producer(const ProgOp* op, const SegSmem<F
     cx += (uint32_t)(g1 - g0);
 }
 
-// ------------------------------------------------------------------------------------------------ role: MMA issuer
-template <int FMT, typename T, int BPAD>
-__device__ __forceinline__ void seg_mma(const ProgOp* op, const SegSmem<FMT, BPAD>& sm, uint32_t tmem_base, uint32_t& cb, uint32_t& cs, unsigned long long* ft) {
-    using C = SegCfg<FMT, BPAD>;
-    constexpr bool kBf16 = std::is_same<T, __nv_bfloat16>::value;
-    constexpr uint32_t IDESC = make_idesc_f16(kGemmTileN, BPAD, kBf16);
-    int g0, g1;
-    sk_range(op->g, blockIdx.x, g0, g1);
-    const int k_blocks = op->g.k_blocks;
-    const uint32_t tmem_d = tmem_base, tmem_a = tmem_base + BPAD;
-    int k = g0;
-    uint32_t i = cb;
-    while (k < g1) {
-        const int tile_end = (k / k_blocks + 1) * k_blocks;
-        const int e = tile_end < g1 ? tile_end : g1;
-        mbar_wait_a(sm.dempty(), (cs & 1) ^ 1);     // the previous segment's epilogue has drained the accumulator
-        tc_fence_after();
-        for (int kk = k; kk < e; ++kk, ++i) {
-            const uint32_t sx = i % C::XS, phx = (i / C::XS) & 1;
-            const uint32_t a = i % kSegAStages, pha = (i / kSegAStages) & 1;
-            mbar_wait_a(sm.xfull(sx), phx);
-            mbar_wait_a(sm.afull(a), pha);
-            tc_fence_after();
-            if (elect_one()) {
-                B200_FT(ft, 5, kk - g0);
-                const uint32_t xs = sm.xring(sx);
-#pragma unroll
-                for (int j = 0; j < kGemmBK / 16; ++j) {
-                    const uint64_t bdesc = make_smem_desc_sw128(xs + (j >> 2) * (BPAD * 128) + (j & 3) * 32);
-                    umma_ts_f16(tmem_d, tmem_a + a * 64 + j * 8, bdesc, IDESC, (kk > k || j > 0) ? 1u : 0u);
-                }
-                umma_commit_a(sm.xempty(sx));
-                umma_commit_a(sm.aempty(a));
-                if (kk == e - 1) umma_commit_a(sm.dfull());
-                B200_FT(ft, 6, kk - g0);
-            }
-            __syncwarp();
-        }
-        ++cs;
-        k = e;
-    }
-    cb = i;
-}
-
-// ------------------------------------------------------------------------------------------------ role: dequant + epilogue
+// ------------------------------------------------------------------------------------------------ role: dequant + MMA + epilogue
 template <typename T>
 __device__ __forceinline__ float silu_mul_f(float g, float u) { return __fdividef(g, 1.f + __expf(-g)) * u; }   // fast divide: <= 2 ulp in fp32, far below the fp16 / bf16 rounding of the result
 
 template <int FMT, typename T, int BPAD>
-__device__ __forceinline__ void seg_dq(const ProgOp* op, const SegSmem<FMT, BPAD>& sm, uint32_t tmem_base, uint32_t& cb, uint32_t& cs, unsigned long long* ft) {
+__device__ __forceinline__ void seg_dq(const ProgOp* op, const SegSmem<FMT, BPAD>& sm, uint32_t& cb, uint32_t& cs, unsigned long long* ft) {
     using C = SegCfg<FMT, BPAD>;
     const SkGemmParams g = op->g;      // by value: the fields live in registers, not behind a global load per use
     int g0, g1;
     sk_range(g, blockIdx.x, g0, g1);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int quarter = warp & 3, grp = warp >> 2;
-    const int row = quarter * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(quarter * 32) << 16;
-    const uint32_t tmem_d = tmem_base, tmem_a = tmem_base + BPAD;
-    constexpr int SLICES = BPAD / 16;
+    const int t4 = lane & 3;
+    // this thread's accumulators (ptx.cuh, wgmma): rows[h] of the tile x batch columns 8i + 2*t4 + c, value acc[4i + 2h + c]
+    const int rows[2] = {16 * warp + (lane >> 2), 16 * warp + (lane >> 2) + 8};
     T* yp = reinterpret_cast<T*>(g.y);
 
     int k = g0;
@@ -303,71 +247,31 @@ __device__ __forceinline__ void seg_dq(const ProgOp* op, const SegSmem<FMT, BPAD
         const int tile = k / g.k_blocks;
         const int tile_beg = tile * g.k_blocks, tile_end = tile_beg + g.k_blocks;
         const int e = tile_end < g1 ? tile_end : g1;
-        // ---- dequantise this CTA's k-blocks of the tile into TMEM (the two warp groups take alternate blocks)
+        // ---- this CTA's k-blocks of the tile: dequantise into wgmma A fragments, multiply with the activation block
+        float acc[BPAD / 2];
+#pragma unroll
+        for (int q = 0; q < BPAD / 2; ++q) acc[q] = 0.f;
         for (int kk = k; kk < e; ++kk, ++i) {
-            if ((int)(i & 1) != grp) continue;
             const uint32_t s = i % C::WS, ph = (i / C::WS) & 1;
-            const uint32_t a = i % kSegAStages, pha = (i / kSegAStages) & 1;
+            const uint32_t sx = i % C::XS, phx = (i / C::XS) & 1;
             mbar_wait_a(sm.wfull(s), ph);
             if ((threadIdx.x & 127) == 0) B200_FT(ft, 2, kk - g0);
-            const uint32_t wb = sm.wring(s);
-            typename Pair<T>::type s2, zs2;
-            if (FMT == kFmtInt4) {
-                s2 = Pair<T>::bcast((uint16_t)lds_u16(wb + 8192 + row * 2));
-                zs2 = Pair<T>::bcast((uint16_t)lds_u16(wb + 8192 + 256 + row * 2));
-            }
+            uint32_t a[8][4];
+            load_w_frag<FMT, T>(sm.wring(s), warp, lane, a, sm.wempty(s));
+            mbar_wait_a(sm.xfull(sx), phx);
+            if ((threadIdx.x & 127) == 0) B200_FT(ft, 5, kk - g0);
+            const uint32_t xs = sm.xring(sx);
+            fence_regs(acc);
+            wgmma_fence();
 #pragma unroll
-            for (int half = 0; half < 2; ++half) {
-                uint32_t regs[2][16];
-                if (FMT == kFmtInt4) {
-                    uint4 v[2];
-#pragma unroll
-                    for (int cc = 0; cc < 2; ++cc) v[cc] = lds_v4(wb + (half * 2 + cc) * 2048 + row * 16);
-                    if (half == 1) {   // every byte of the stage this warp needs is in registers: release it
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive_a(sm.wempty(s));
-                    }
-#pragma unroll
-                    for (int cc = 0; cc < 2; ++cc) {
-                        Dequant4<T>::word(v[cc].x, s2, zs2, &regs[cc][0]);
-                        Dequant4<T>::word(v[cc].y, s2, zs2, &regs[cc][4]);
-                        Dequant4<T>::word(v[cc].z, s2, zs2, &regs[cc][8]);
-                        Dequant4<T>::word(v[cc].w, s2, zs2, &regs[cc][12]);
-                    }
-                } else {
-                    uint4 v[2][2];
-#pragma unroll
-                    for (int cc = 0; cc < 2; ++cc)
-#pragma unroll
-                        for (int h = 0; h < 2; ++h) v[cc][h] = lds_v4(wb + ((half * 2 + cc) * 2 + h) * 2048 + row * 16);
-                    if (half == 1) {
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive_a(sm.wempty(s));
-                    }
-#pragma unroll
-                    for (int cc = 0; cc < 2; ++cc)
-#pragma unroll
-                        for (int h = 0; h < 2; ++h) {
-                            Dequant8<T>::word(v[cc][h].x, &regs[cc][h * 8 + 0]);
-                            Dequant8<T>::word(v[cc][h].y, &regs[cc][h * 8 + 2]);
-                            Dequant8<T>::word(v[cc][h].z, &regs[cc][h * 8 + 4]);
-                            Dequant8<T>::word(v[cc][h].w, &regs[cc][h * 8 + 6]);
-                        }
-                }
-                if (half == 0) {
-                    mbar_wait_a(sm.aempty(a), pha ^ 1);
-                    if ((threadIdx.x & 127) == 0) B200_FT(ft, 3, kk - g0);
-                    tc_fence_after();
-                }
-                const uint32_t dst = tmem_a + lane_addr + a * 64 + half * 32;
-                tmem_st_32x32b_x16(dst, regs[0]);
-                tmem_st_32x32b_x16(dst + 16, regs[1]);
-            }
-            tmem_wait_st();
-            tc_fence_before();
+            for (int j = 0; j < kGemmBK / 16; ++j)
+                wgmma_rs<BPAD, T>(acc, a[j], make_smem_desc_sw128(xs + (j >> 2) * (BPAD * 128) + (j & 3) * 32), 1u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(acc);
             __syncwarp();
-            if (lane == 0) mbar_arrive_a(sm.afull(a));
-            if ((threadIdx.x & 127) == 0) B200_FT(ft, 4, kk - g0);
+            if (lane == 0) mbar_arrive_a(sm.xempty(sx));
+            if ((threadIdx.x & 127) == 0) B200_FT(ft, 6, kk - g0);
         }
 
         // ---- epilogue of the segment [k, e) of `tile`
@@ -375,51 +279,44 @@ __device__ __forceinline__ void seg_dq(const ProgOp* op, const SegSmem<FMT, BPAD
         const int first = tile_beg / g.per_cta, last = (tile_end - 1) / g.per_cta;
         const int nact = last - first + 1, my_idx = (int)blockIdx.x - first;
         // per-feature scale / bias are indexed by the PACKED column (with silu_mul the caller interleaves them like the weight)
-        const int n = tile * kGemmTileN + row;
-        float cscale = 1.f, bias = 0.f;
-        if (n < g.N) {
-            if (FMT == kFmtInt8) cscale = to_f32<T>(reinterpret_cast<const T*>(g.col_scale)[n]);
-            if (g.bias) bias = to_f32<T>(reinterpret_cast<const T*>(g.bias)[n]);
-        }
-        auto final_store = [&](int sl, const float (&v)[16]) {
+        float cscale[2] = {1.f, 1.f}, bias[2] = {0.f, 0.f};
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-                const int b = sl * 16 + j;
-                const float val = fmaf(v[j], cscale, bias);
-                if (g.silu_mul) {
-                    const float other = __shfl_xor_sync(0xffffffffu, val, 1);
-                    const int f = tile * 64 + (row >> 1);
-                    if (!(lane & 1) && b < g.B && f < g.N / 2)
-                        yp[(size_t)b * (g.N / 2) + f] = from_f32<T>(silu_mul_f<T>(val, other));
-                } else if (n < g.N && b < g.B) {
-                    yp[(size_t)b * g.N + n] = from_f32<T>(val);
-                }
+        for (int h = 0; h < 2; ++h) {
+            const int n = tile * kGemmTileN + rows[h];
+            if (n < g.N) {
+                if (FMT == kFmtInt8) cscale[h] = to_f32<T>(reinterpret_cast<const T*>(g.col_scale)[n]);
+                if (g.bias) bias[h] = to_f32<T>(reinterpret_cast<const T*>(g.bias)[n]);
+            }
+        }
+        // rows 2r / 2r+1 (gate / up with silu_mul) sit in lanes L / L+4; every lane must take part (shuffle)
+        auto final_store = [&](int h, int b, float a_v) {
+            const float val = fmaf(a_v, cscale[h], bias[h]);
+            const int n = tile * kGemmTileN + rows[h];
+            if (g.silu_mul) {
+                const float other = __shfl_xor_sync(0xffffffffu, val, 4);
+                const int f = tile * 64 + (rows[h] >> 1);
+                if (!(lane & 4) && b < g.B && f < g.N / 2)
+                    yp[(size_t)b * (g.N / 2) + f] = from_f32<T>(silu_mul_f<T>(val, other));
+            } else if (n < g.N && b < g.B) {
+                yp[(size_t)b * g.N + n] = from_f32<T>(val);
             }
         };
         if (threadIdx.x == 0) B200_FT(ft, 7, 2 * (int)(cs & 7));
-        mbar_wait_a(sm.dfull(), cs & 1);
-        tc_fence_after();
-        if (threadIdx.x == 0) B200_FT(ft, 7, 2 * (int)(cs & 7) + 1);
+        // partial slot layout [bpad/4][128 rows][4]: a float2 of this thread = batch columns b, b+1 (b even) of one row
+        constexpr size_t SLOT4 = (size_t)(BPAD / 4) * kGemmTileN;
+        float4* part0 = reinterpret_cast<float4*>(g.ws) + (size_t)tile * g.max_contrib * SLOT4;
+        auto part2 = [&](int c, int h, int b) {
+            return reinterpret_cast<float2*>(reinterpret_cast<float*>(part0 + (size_t)c * SLOT4 + (size_t)(b >> 2) * kGemmTileN + rows[h]) + (b & 3));
+        };
         if (g.aligned && nact > 1) {
             // ---- uniform split-K (every CTA of this op owns exactly one segment): the S contributors of the tile publish
             // their fp32 partials to L2, wait for each other, and EACH reduces 1/S of the tile in fixed order 0..S-1
             // (deterministic) -- S float4 loads in flight per thread, one round trip, instead of one CTA loading S partials.
             constexpr int ITEMS = (BPAD / 4) * kGemmTileN;       // (4 batch columns) x (feature row) units of the tile
-            constexpr size_t SLOT4 = (size_t)ITEMS;
-            float4* part0 = reinterpret_cast<float4*>(g.ws) + (size_t)tile * g.max_contrib * SLOT4;
-            for (int sl = grp; sl < SLICES; sl += 2) {
-                uint32_t r[16];
-                tmem_ld_32x32b_x16(tmem_d + lane_addr + sl * 16, r);
-                tmem_wait_ld();
 #pragma unroll
-                for (int q = 0; q < 4; ++q)
-                    __stcg(&part0[(size_t)my_idx * SLOT4 + (size_t)(sl * 4 + q) * kGemmTileN + row],
-                           make_float4(__uint_as_float(r[4 * q]), __uint_as_float(r[4 * q + 1]), __uint_as_float(r[4 * q + 2]),
-                                       __uint_as_float(r[4 * q + 3])));
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_a(sm.dempty());
+            for (int q = 0; q < BPAD / 8; ++q)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) __stcg(part2(my_idx, h, 8 * q + 2 * t4), make_float2(acc[4 * q + 2 * h], acc[4 * q + 2 * h + 1]));
             asm volatile("bar.sync 1, %0;" ::"n"(kSegDqThreads) : "memory");
             unsigned* arrivals = reinterpret_cast<unsigned*>(g.sem) + tile;
             if (threadIdx.x == 0) red_release_add(arrivals, 1u);
@@ -432,7 +329,7 @@ __device__ __forceinline__ void seg_dq(const ProgOp* op, const SegSmem<FMT, BPAD
                 const int item = base + lane;
                 const bool ok = item < it1;
                 const int q = item / kGemmTileN, rrow = item % kGemmTileN;
-                float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+                float4 sum = make_float4(0.f, 0.f, 0.f, 0.f);
                 if (ok) {
                     float4 t[8];
 #pragma unroll
@@ -440,17 +337,17 @@ __device__ __forceinline__ void seg_dq(const ProgOp* op, const SegSmem<FMT, BPAD
                         t[c] = c < nact ? __ldcg(&part0[(size_t)c * SLOT4 + (size_t)q * kGemmTileN + rrow]) : make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
                     for (int c = 0; c < 8; ++c) {
-                        acc.x += t[c].x;
-                        acc.y += t[c].y;
-                        acc.z += t[c].z;
-                        acc.w += t[c].w;
+                        sum.x += t[c].x;
+                        sum.y += t[c].y;
+                        sum.z += t[c].z;
+                        sum.w += t[c].w;
                     }
                     for (int c = 8; c < nact; ++c) {
                         const float4 u = __ldcg(&part0[(size_t)c * SLOT4 + (size_t)q * kGemmTileN + rrow]);
-                        acc.x += u.x;
-                        acc.y += u.y;
-                        acc.z += u.z;
-                        acc.w += u.w;
+                        sum.x += u.x;
+                        sum.y += u.y;
+                        sum.z += u.z;
+                        sum.w += u.w;
                     }
                 }
                 // feature `rrow` of the tile, batch columns 4q .. 4q+3
@@ -460,7 +357,7 @@ __device__ __forceinline__ void seg_dq(const ProgOp* op, const SegSmem<FMT, BPAD
                     if (FMT == kFmtInt8) cs2 = to_f32<T>(reinterpret_cast<const T*>(g.col_scale)[nn]);
                     if (g.bias) bi2 = to_f32<T>(reinterpret_cast<const T*>(g.bias)[nn]);
                 }
-                const float vals[4] = {fmaf(acc.x, cs2, bi2), fmaf(acc.y, cs2, bi2), fmaf(acc.z, cs2, bi2), fmaf(acc.w, cs2, bi2)};
+                const float vals[4] = {fmaf(sum.x, cs2, bi2), fmaf(sum.y, cs2, bi2), fmaf(sum.z, cs2, bi2), fmaf(sum.w, cs2, bi2)};
 #pragma unroll
                 for (int e4 = 0; e4 < 4; ++e4) {
                     const int b = q * 4 + e4;
@@ -488,47 +385,29 @@ __device__ __forceinline__ void seg_dq(const ProgOp* op, const SegSmem<FMT, BPAD
         // it finishes the tile last in time) keeps its partial in registers, waits until the other contributors have
         // published theirs, adds them in fixed order 1..nact-1 (deterministic) and stores the result. The others store
         // their fp32 partial to L2, signal once (fire-and-forget) and move on -- nobody but the reducer ever waits.
-        // partial slot layout [bpad/4][128 rows][4]: a thread moves float4 = 4 batch columns of its feature row
-        constexpr size_t SLOT4 = (size_t)(BPAD / 4) * kGemmTileN;
-        float4* part0 = reinterpret_cast<float4*>(g.ws) + (size_t)tile * g.max_contrib * SLOT4;
         if (nact > 1 && my_idx == 0) {
             // wait for the nact-1 published partials (lane 0 of every warp polls; no CTA barrier on this path)
             if (lane == 0) spin_until_ge(reinterpret_cast<const unsigned*>(g.sem) + tile, (unsigned)(nact - 1));
             __syncwarp();
         }
-        for (int sl = grp; sl < SLICES; sl += 2) {
-            uint32_t r[16];
-            tmem_ld_32x32b_x16(tmem_d + lane_addr + sl * 16, r);
-            tmem_wait_ld();
-            float v[16];
 #pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]);
-            if (nact == 1) {
-                final_store(sl, v);
-            } else if (my_idx == 0) {
-                for (int c = 1; c < nact; ++c) {
-                    float4 t[4];
+        for (int q = 0; q < BPAD / 8; ++q)
 #pragma unroll
-                    for (int q = 0; q < 4; ++q) t[q] = __ldcg(&part0[(size_t)c * SLOT4 + (size_t)(sl * 4 + q) * kGemmTileN + row]);
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        v[4 * q + 0] += t[q].x;
-                        v[4 * q + 1] += t[q].y;
-                        v[4 * q + 2] += t[q].z;
-                        v[4 * q + 3] += t[q].w;
-                    }
+            for (int h = 0; h < 2; ++h) {
+                const int b = 8 * q + 2 * t4;
+                float v0 = acc[4 * q + 2 * h], v1 = acc[4 * q + 2 * h + 1];
+                if (nact > 1 && my_idx != 0) {
+                    __stcg(part2(my_idx, h, b), make_float2(v0, v1));
+                    continue;
                 }
-                final_store(sl, v);
-            } else {
-#pragma unroll
-                for (int q = 0; q < 4; ++q)
-                    __stcg(&part0[(size_t)my_idx * SLOT4 + (size_t)(sl * 4 + q) * kGemmTileN + row],
-                           make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]));
+                for (int c = 1; c < nact; ++c) {
+                    const float2 u = __ldcg(part2(c, h, b));
+                    v0 += u.x;
+                    v1 += u.y;
+                }
+                final_store(h, b, v0);
+                final_store(h, b + 1, v1);
             }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_a(sm.dempty());     // accumulator drained: the MMA warp may start the next segment
         if (nact > 1) {
             // all dq threads' partial stores (or the reducer's polls) are done once they pass this barrier; thread 0's
             // gpu-scope fence is cumulative over what the barrier ordered before it
@@ -695,28 +574,15 @@ decode_segment_kernel(const __grid_constant__ ProgOp op0, const ProgOp* __restri
     if (threadIdx.x == 0) {
         for (int s = 0; s < C::WS; ++s) {
             mbar_init_a(sm.wfull(s), 1);
-            mbar_init_a(sm.wempty(s), 4);
+            mbar_init_a(sm.wempty(s), kSegDqWarps);   // both warpgroups read every weight stage
         }
         for (int s = 0; s < C::XS; ++s) {
             mbar_init_a(sm.xfull(s), 1);
-            mbar_init_a(sm.xempty(s), 1);
+            mbar_init_a(sm.xempty(s), kSegDqWarps);
         }
-        for (int a = 0; a < kSegAStages; ++a) {
-            mbar_init_a(sm.afull(a), 4);
-            mbar_init_a(sm.aempty(a), 1);
-        }
-        mbar_init_a(sm.dfull(), 1);
-        mbar_init_a(sm.dempty(), kSegDqWarps);
         fence_mbar_init();
     }
-    if (warp == kSegDqWarps + 2) {
-        tmem_alloc_a(sm.tmem_slot(), C::TMEM_COLS);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = lds_u32(sm.tmem_slot());
     if (use_pdl && threadIdx.x == 0) pdl_launch_dependents();
 
     if (warp == kSegDqWarps) {
@@ -734,13 +600,6 @@ decode_segment_kernel(const __grid_constant__ ProgOp op0, const ProgOp* __restri
             const ProgOp* op = ops ? &ops[i] : &op0;
             if (op->type == kOpGemm) seg_x_producer<QFMT, BPAD>(op, sm, cx, gbar, (unsigned)i * G, ops != nullptr, ftrace ? ftrace + (size_t)i * kFtSlots * kFtBlocks : nullptr);
         }
-    } else if (warp == kSegDqWarps + 2) {
-        // ---- MMA issuer
-        uint32_t cb = 0, cs = 0;
-        for (int i = 0; i < nops; ++i) {
-            const ProgOp* op = ops ? &ops[i] : &op0;
-            if (op->type == kOpGemm) seg_mma<QFMT, T, BPAD>(op, sm, tmem_base, cb, cs, ftrace ? ftrace + (size_t)i * kFtSlots * kFtBlocks : nullptr);
-        }
     } else {
         // ---- dequant / epilogue / glue warps: the role that owns the grid barrier
         if (use_pdl) pdl_wait();
@@ -753,7 +612,7 @@ decode_segment_kernel(const __grid_constant__ ProgOp op0, const ProgOp* __restri
                 trace[((size_t)i * G + blockIdx.x) * 2 + 0] = gt;
             }
             if (op->type == kOpGemm) {
-                seg_dq<QFMT, T, BPAD>(op, sm, tmem_base, cb, cs, ftrace ? ftrace + (size_t)i * kFtSlots * kFtBlocks : nullptr);
+                seg_dq<QFMT, T, BPAD>(op, sm, cb, cs, ftrace ? ftrace + (size_t)i * kFtSlots * kFtBlocks : nullptr);
             } else {
                 // glue ops read what the previous op wrote: wait for it (thread 0 polls, the named barrier publishes)
                 if (threadIdx.x == 0) grid_wait(gbar, (unsigned)i * G);
@@ -780,13 +639,8 @@ decode_segment_kernel(const __grid_constant__ ProgOp op0, const ProgOp* __restri
                 red_release_add(gbar, 1u);
             }
         }
-        tc_fence_before();
     }
     __syncthreads();
-    if (warp == kSegDqWarps + 2) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, C::TMEM_COLS);
-    }
     // last CTA out resets the counters for the next launch (every CTA has passed its last grid_wait by now: a wait for
     // op i needs i*G arrivals, the exit ticket is taken after this CTA's nops-th arrival)
     if (threadIdx.x == 0) {

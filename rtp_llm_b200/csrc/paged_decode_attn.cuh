@@ -1,11 +1,11 @@
-// Paged GQA decode attention for sm_100a.
+// Paged GQA decode attention for sm_90a.
 //
 // Replaces (same math, same cache layout, same page-list format):
-//   runXqa                      /root/reference/rtp_llm/models_py/bindings/cuda/ops/CudaXqa.h:65-84 (+CudaXqa.cc:124-221)
-//   XQA sm_90a kernel           /root/reference/3rdparty/xqa/mha_sm90.cu (cannot run on B200)
-//   FlashInferTRTLLMDecodeOp    /root/reference/rtp_llm/models_py/modules/factory/attention/cuda_impl/trtllm_gen.py:503-546
+//   runXqa                      rtp_llm/models_py/bindings/cuda/ops/CudaXqa.h:65-84 (+CudaXqa.cc:124-221)
+//   XQA sm_90a kernel           3rdparty/xqa/mha_sm90.cu
+//   FlashInferTRTLLMDecodeOp    rtp_llm/models_py/modules/factory/attention/cuda_impl/trtllm_gen.py:503-546
 //
-// Work decomposition (B200-first, not a port of XQA's warpgroup pipeline):
+// Work decomposition (not a port of XQA's warpgroup pipeline):
 //   grid = (nsplit, B*Hkv); one CTA owns (sequence b, kv head, a contiguous run of 64-token tiles).
 //   Warp 4 lane 0 = TMA producer: reads the K/V page ids of each tile from the page list and issues 4-D tensor-map
 //   loads (128-byte swizzle, one box per page and per 64-channel half) into a 3-stage shared-memory ring.

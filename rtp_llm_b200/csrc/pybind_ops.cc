@@ -333,7 +333,7 @@ void registerPyModuleOps(pybind11::module& m) {
 
 // standalone plugin form: module `b200_compute_ops` with the `rtp_llm_ops` submodule (cpp/pybind/ComputeInit.cc:18-27)
 PYBIND11_MODULE(b200_compute_ops, m) {
-    m.doc() = "B200-native decode ops behind rtp-llm's registerPyModuleOps seam";
-    auto ops = m.def_submodule("rtp_llm_ops", "rtp llm custom ops (B200 decode path)");
+    m.doc() = "Hopper-native decode ops behind rtp-llm's registerPyModuleOps seam";
+    auto ops = m.def_submodule("rtp_llm_ops", "rtp llm custom ops (Hopper decode path)");
     rtp_llm::registerPyModuleOps(ops);
 }

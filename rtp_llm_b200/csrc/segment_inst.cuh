@@ -28,12 +28,12 @@ int seg_one(const ProgOp* op0, const ProgOp* d_ops, int nops, unsigned* gbar, in
         CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kSegThreads, smem));
         CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
         if (occ < 1) return fail(B200_ECUDA, "decode_segment_kernel does not fit on an SM (smem %d)", smem);
-        // Every CTA must be co-resident (the ops synchronise grid-wide). Two CTAs per SM fit by construction (__launch_bounds__(352, 2),
-        // 2 x (SMEM + 1 KB) <= 227 KB, 2 x 256 TMEM columns); measured on B200: 296 CTAs run concurrently although the occupancy
-        // query answers 1 for this kernel. A wrong assumption here cannot hang the GPU: every spin-wait traps after a bound.
+        // Every CTA must be co-resident (the ops synchronise grid-wide): the grid is what the occupancy query reports, at most
+        // the two CTAs per SM the kernel is built for (__launch_bounds__(320, 2), 2 x (SMEM + 1 KB) <= 227 KB of the SM's 228 KB).
         static_assert(2 * (smem + 1024) <= 227 * 1024, "two CTAs per SM must fit");
-        max_grid[dev] = 2 * sms;
-        if (env_int("B200_SEG_GRID", 0) > 0) max_grid[dev] = env_int("B200_SEG_GRID", 0);   // developer override
+        max_grid[dev] = (occ < 2 ? occ : 2) * sms;
+        const int forced = env_int("B200_SEG_GRID", 0);   // developer override, never beyond the co-resident grid
+        if (forced > 0 && forced < max_grid[dev]) max_grid[dev] = forced;
         if (env_int("B200_DEBUG", 0)) fprintf(stderr, "[b200] decode_segment_kernel<bpad %d, fmt %d>: occupancy %d CTAs/SM, grid %d\n", BPAD, QFMT, occ, max_grid[dev]);
         configured[dev] = true;
     }

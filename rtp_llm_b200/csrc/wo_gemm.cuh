@@ -1,22 +1,22 @@
-// Weight-only (INT4 group-128 / INT8 per-column / INT8 group-128 / FP16) x FP16|BF16 GEMM for decode batches, sm_100a.
+// Weight-only (INT4 group-128 / INT8 per-column / INT8 group-128 / FP16) x FP16|BF16 GEMM for decode batches, sm_90a.
 //
-//   Y[b][n] = sum_k X[b][k] * W'[k][n] (+ bias[n]),   W' per /root/reference/rtp_llm/device/device_impl.py:183-222,242-300
+//   Y[b][n] = sum_k X[b][k] * W'[k][n] (+ bias[n]),   W' per rtp_llm/device/device_impl.py:183-222,242-300
 //   (SURVEY.md section 8 a8-a10).  Replaces the cutlass fpA_intB "mixed gemm" the reference loader still prepares weights
 //   for (device_impl.py:392-479) but whose kernel is absent from the snapshot; plugs in behind LinearBase.forward
-//   (/root/reference/rtp_llm/models_py/modules/factory/linear/linear_base.py:81).
+//   (rtp_llm/models_py/modules/factory/linear/linear_base.py:81).
 //
-// B200 design (swap-AB, weights stationary on the MMA M side):
+// Hopper design (swap-AB, weights stationary on the MMA M side):
 //   * one CTA = 128 output features x a run of 128-deep k-blocks (split-K across blockIdx.y);
 //   * two TMA warps: weights were re-laid out at load time into per-(n-tile,k-block) contiguous blobs (packed nibbles +
-//                the group's scales and zero*scale), so ONE cp.async.bulk stages a whole block (weight ring); the
-//                activation block [B x 128] comes through a 128B-swizzled tensor map, OOB rows zero-filled (activation ring);
-//   * dequant warps: dequantise IN REGISTERS (lop3 magic-number int->fp16, exact; hfma2 with the group scale / zero*scale)
-//                and store the fp16 operand straight INTO TENSOR MEMORY (tcgen05.st) -- the A operand of
-//   * MMA warp : one elected thread issues tcgen05.mma (M=128 features, N=batch pad, K=16) with A from TMEM and
-//                B (activations, K-major SW128) from shared memory, fp32 accumulators in TMEM;
-//   * epilogue : the dequant warps read the accumulators (tcgen05.ld); the split-K CTAs of a tile form a thread-block cluster
-//                and merge their fp32 partials through distributed shared memory in fixed order (deterministic); bias /
-//                per-column scale / optional fused SiLU(gate)*up applied; coalesced stores.
+//                the group's scales and zero*scale, in wgmma fragment order), so ONE cp.async.bulk stages a whole block
+//                (weight ring); the activation block [B x 128] comes through a 128B-swizzled tensor map, OOB rows
+//                zero-filled (activation ring);
+//   * two dequant + MMA warpgroups (64 features each): dequantise IN REGISTERS (lop3 magic-number int->fp16, exact; hfma2
+//                with the group scale / zero*scale) straight into the A fragments of wgmma (m64 x N=batch pad x k16,
+//                A from registers, B = activations K-major SW128 from shared memory), fp32 accumulators in registers;
+//   * epilogue : from the accumulator registers; the split-K CTAs of a tile form a thread-block cluster and merge their fp32
+//                partials through distributed shared memory in fixed order (deterministic); bias / per-column scale /
+//                optional fused SiLU(gate)*up applied.
 //   The FP16-weight variant feeds A from shared memory (TMA tensor map, SW128) with the same pipeline.
 #pragma once
 #include <type_traits>
@@ -39,10 +39,10 @@ __host__ __device__ constexpr int gemm_w_bytes(int fmt) {
 }
 // Shared-memory rings.  The weight ring (HBM stream) and the activation ring (L2 hits) are SEPARATE: a weight stage is
 // released as soon as the dequant warps hold its nibbles in registers, so its lifetime is one TMA latency, not the
-// whole dequant -> TMEM -> MMA chain, and the bytes in flight per SM (Little's law: ~44 GB/s * latency) stay high.
-// 8 dequant warps = two groups of four taking alternate k-blocks (see the dequant section of the kernel).
+// whole dequant -> MMA chain, and the bytes in flight per SM (Little's law: bandwidth per SM * latency) stay high.
+// 8 dequant warps = two warpgroups, each the MMA issuer of its 64 feature rows (see the dequant section of the kernel).
 __host__ __device__ constexpr int gemm_ndq_warps(int var) { (void)var; return 8; }
-__host__ __device__ constexpr int gemm_threads(int var) { return (gemm_ndq_warps(var) + 3) * 32; }
+__host__ __device__ constexpr int gemm_threads(int var) { return (gemm_ndq_warps(var) + 2) * 32; }
 __host__ __device__ constexpr int gemm_x_stage_bytes(int bpad) { return bpad * 256; }
 #ifndef B200_GEMM_XS
 #define B200_GEMM_XS 4
@@ -61,19 +61,6 @@ __host__ __device__ constexpr int gemm_min_ctas(int fmt, int bpad, int var) {
 __host__ __device__ constexpr int gemm_w_stages(int fmt, int bpad, int var) {
     return gemm_min_ctas(fmt, bpad, var) == 2 ? gemm_w_stages_for(fmt, bpad, 106 * 1024)
                                               : gemm_w_stages_for(fmt, bpad, 216 * 1024);
-}
-// Accumulator tiles the 8 k-steps of a block rotate over (the epilogue sums them). Measured (tools/gemm_trace.py): one
-// tile is enough -- back-to-back tcgen05.mma into the same accumulator pipeline fine; kept as a knob.
-__host__ __device__ constexpr int gemm_nacc(int bpad) { return bpad <= 64 ? 1 : 2; }
-__host__ __device__ constexpr int gemm_a_stages(int bpad, int var) {
-    (void)var;
-    return 3;
-}
-__host__ __device__ constexpr int gemm_tmem_cols(int fmt, int bpad, int var) {
-    int need = bpad * gemm_nacc(bpad) + (fmt == kFmtF16 ? 0 : gemm_a_stages(bpad, var) * 64);
-    int c = 32;
-    while (c < need) c *= 2;
-    return c;
 }
 __host__ __device__ constexpr int gemm_smem_bytes(int fmt, int bpad, int var) {
     return gemm_x_stages(bpad) * gemm_x_stage_bytes(bpad) + gemm_w_stages(fmt, bpad, var) * gemm_w_bytes(fmt) + kGemmSmemMisc;
@@ -104,7 +91,6 @@ struct GemmParams {
     int silu_mul;            // 1: tile rows 2r / 2r+1 are gate / up feature tile*64+r; y[b][tile*64+r] = silu(g)*u
     int cluster_reduce;      // 1: the nsplit CTAs of a tile form a cluster (1,nsplit,1) and merge through DSMEM
     long long* trace;        // developer timeline (tools/gemm_trace.py); null in production
-    int dbg;                 // developer experiments (env B200_GEMM_DBG): 1 no math, 2 no TMEM store, 4 no MMA; 0 in production
 };
 
 // The VAR == 1 kernels (gemm_cluster_rs.cu) take the descriptor of the reduce-scatter push after the common parameters; the
@@ -121,14 +107,15 @@ struct GemmParamsOf<1> {
     using type = GemmParamsRs;
 };
 
-// ---- int4 -> fp16/bf16 pairs.  Nibble p of a word holds u = q_s + 8; p<4 <-> k = 2p, p>=4 <-> k = 2(p-4)+1, so each
-// (w >> 4i) & 0x000f000f yields the (even k, odd k) pair of TMEM column i directly.
+// ---- int4 -> fp16/bf16 pairs.  Nibble p of a word holds u = q_s + 8; nibbles i and i+4 are the (even k, odd k) pair of
+// register i of a wgmma A fragment, so each (w >> 4i) & 0x000f000f yields that register directly. Registers 0 / 2 belong to
+// feature row A of the fragment, 1 / 3 to row B (= A + 8): each row has its own group scale and zero*scale.
 template <typename T>
 struct Dequant4;
 template <>
 struct Dequant4<__half> {
-    // out[i] = q_s * s + zs for columns i = 0..3 of one 32-bit word
-    static __device__ __forceinline__ void word(uint32_t w, __half2 s2, __half2 zs2, uint32_t* out) {
+    // out[i] = q_s * s + zs for registers i = 0..3 of one 32-bit word
+    static __device__ __forceinline__ void word(uint32_t w, __half2 sA, __half2 zA, __half2 sB, __half2 zB, uint32_t* out) {
         const uint32_t MAGIC = 0x64006400u;                 // 1024.0 | 1024.0
         const __half2 k1032 = __half2half2(__ushort_as_half(0x6408));   // 1032
         const __half2 k16th = __half2half2(__ushort_as_half(0x2C00));   // 1/16
@@ -143,10 +130,10 @@ struct Dequant4<__half> {
         __half2 h1 = __hfma2(*reinterpret_cast<__half2*>(&t1), k16th, k72);     // (1024+16u)/16 - 72 = u - 8, exact
         __half2 h2 = __hsub2(*reinterpret_cast<__half2*>(&t2), k1032);
         __half2 h3 = __hfma2(*reinterpret_cast<__half2*>(&t3), k16th, k72);
-        h0 = __hfma2(h0, s2, zs2);
-        h1 = __hfma2(h1, s2, zs2);
-        h2 = __hfma2(h2, s2, zs2);
-        h3 = __hfma2(h3, s2, zs2);
+        h0 = __hfma2(h0, sA, zA);
+        h1 = __hfma2(h1, sB, zB);
+        h2 = __hfma2(h2, sA, zA);
+        h3 = __hfma2(h3, sB, zB);
         out[0] = *reinterpret_cast<uint32_t*>(&h0);
         out[1] = *reinterpret_cast<uint32_t*>(&h1);
         out[2] = *reinterpret_cast<uint32_t*>(&h2);
@@ -155,7 +142,8 @@ struct Dequant4<__half> {
 };
 template <>
 struct Dequant4<__nv_bfloat16> {
-    static __device__ __forceinline__ void word(uint32_t w, __nv_bfloat162 s2, __nv_bfloat162 zs2, uint32_t* out) {
+    static __device__ __forceinline__ void word(uint32_t w, __nv_bfloat162 sA, __nv_bfloat162 zA, __nv_bfloat162 sB,
+                                                __nv_bfloat162 zB, uint32_t* out) {
         const uint32_t MAGIC = 0x43004300u;  // 128.0 | 128.0 (ulp 1)
         const __nv_bfloat162 k136 = __bfloat162bfloat162(__ushort_as_bfloat16(0x4308));  // 136
 #pragma unroll
@@ -163,7 +151,7 @@ struct Dequant4<__nv_bfloat16> {
             uint32_t t;
             asm("lop3.b32 %0, %1, 0x000f000f, %2, 0xea;" : "=r"(t) : "r"(w >> (4 * i)), "r"(MAGIC));
             __nv_bfloat162 h = __hsub2(*reinterpret_cast<__nv_bfloat162*>(&t), k136);  // u - 8, exact
-            h = __hfma2(h, s2, zs2);
+            h = (i & 1) ? __hfma2(h, sB, zB) : __hfma2(h, sA, zA);
             out[i] = *reinterpret_cast<uint32_t*>(&h);
         }
     }
@@ -214,12 +202,12 @@ __device__ __forceinline__ RsLane rs_lane(const GemmParamsRs& p, int n) {
                                         (size_t)(c - owner * Cs) * 32 + ((n & 7) >> 1) * 8;
     return l;
 }
-// v = this lane's value for (row b, column n); lanes 2i / 2i+1 hold adjacent columns: the even lane emits the pair.
-// Must be called by all 32 lanes of the warp with the same b.
+// v = this lane's value for (row b, column n); lanes L and L + delta hold adjacent columns n, n+1 of the same row b (delta a
+// power of two): the lane without the delta bit emits the pair. Must be called by all 32 lanes of the warp.
 template <typename T>
-__device__ __forceinline__ void rs_emit(const GemmParams& p, const RsLane& l, int b, int n, float v, int lane) {
-    const float hi = __shfl_down_sync(0xffffffffu, v, 1);
-    if (lane & 1) return;
+__device__ __forceinline__ void rs_emit(const GemmParams& p, const RsLane& l, int b, int n, float v, int lane, int delta) {
+    const float hi = __shfl_down_sync(0xffffffffu, v, delta);
+    if ((lane & delta) || b >= p.B) return;
     const uint32_t data = pack2<T>(v, hi);
     if (l.remote == nullptr) {
         *reinterpret_cast<uint32_t*>(reinterpret_cast<T*>(p.y) + (size_t)b * p.N + n) = data;
@@ -244,20 +232,75 @@ struct Pair<__nv_bfloat16> {
 };
 
 // developer timeline (only in -DB200_GEMM_DEV builds, see tools/gemm_trace.py): TRACE(slot, it) stores clock64() for CTA
-// (0,0); slots: 0 w-issue, 1 x-issue, 2 dq wfull, 3 dq math done, 4 dq aempty seen, 5 dq afull arrive (for it-1),
-// 6 mma operands ready, 7 mma issued
+// (0,0); slots: 0 w-issue, 1 x-issue, 2 dq wfull seen, 3 dq math done, 6 mma operands ready, 7 mma complete
 #ifdef B200_GEMM_DEV
 #define B200_TRACE(slot, it)                                                                     \
     do {                                                                                         \
         if (p.trace && blockIdx.x == 0 && blockIdx.y == 0 && (it) < 64) p.trace[(slot) * 64 + (it)] = clock64(); \
     } while (0)
-#define B200_DBG(bit) (p.dbg & (bit))
 #define B200_TRACING (p.trace != nullptr)
 #else
 #define B200_TRACE(slot, it) do { } while (0)
-#define B200_DBG(bit) 0
 #define B200_TRACING false
 #endif
+
+// The weight block of one (n-tile, k-block) as wgmma A fragments (ptx.cuh): dequant warp R = 0..7 (two warpgroups) owns
+// feature rows 16R..16R+15 of the 128-feature tile, a[j] is its fragment of k16-step j. The pack kernels below lay every
+// thread's bytes of a block out as consecutive 16-byte vectors (one conflict-free LDS.128 per warp and vector):
+//   INT4  : one word per k-step, vector (j / 4, R, lane); nibble i / i+4 = low / high element of a[j][i]
+//   8-bit : two words per k-step, vector (j / 2, R, lane); bytes 0-3 = a[j][0], a[j][1], bytes 4-7 = a[j][2], a[j][3]
+// Group scales / zero*scale stay per feature row after the payload. The stage is released (`empty`) as soon as the warp
+// holds its bytes in registers.
+template <int FMT, typename T>
+__device__ __forceinline__ void load_w_frag(uint32_t wb, int R, int lane, uint32_t (&a)[8][4], uint32_t empty_bar) {
+    const int rA = 16 * R + (lane >> 2), rB = rA + 8;
+    const uint32_t vec = wb + (uint32_t)(R * 32 + lane) * 16;
+    typename Pair<T>::type sA, zA, sB, zB;
+    if (FMT == kFmtInt4 || FMT == kFmtInt8G) {
+        constexpr int Q_BYTES = FMT == kFmtInt4 ? 8192 : 16384;
+        sA = Pair<T>::bcast((uint16_t)lds_u16(wb + Q_BYTES + rA * 2));
+        zA = Pair<T>::bcast((uint16_t)lds_u16(wb + Q_BYTES + 256 + rA * 2));
+        sB = Pair<T>::bcast((uint16_t)lds_u16(wb + Q_BYTES + rB * 2));
+        zB = Pair<T>::bcast((uint16_t)lds_u16(wb + Q_BYTES + 256 + rB * 2));
+    }
+    if (FMT == kFmtInt4) {
+        uint4 v[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) v[h] = lds_v4(vec + h * 4096);
+        __syncwarp();
+        if (lane == 0) mbar_arrive_a(empty_bar);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            Dequant4<T>::word(v[h].x, sA, zA, sB, zB, a[4 * h + 0]);
+            Dequant4<T>::word(v[h].y, sA, zA, sB, zB, a[4 * h + 1]);
+            Dequant4<T>::word(v[h].z, sA, zA, sB, zB, a[4 * h + 2]);
+            Dequant4<T>::word(v[h].w, sA, zA, sB, zB, a[4 * h + 3]);
+        }
+    } else {
+        uint4 v[4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) v[q] = lds_v4(vec + q * 4096);
+        __syncwarp();
+        if (lane == 0) mbar_arrive_a(empty_bar);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            Dequant8<T>::word(v[q].x, &a[2 * q][0]);
+            Dequant8<T>::word(v[q].y, &a[2 * q][2]);
+            Dequant8<T>::word(v[q].z, &a[2 * q + 1][0]);
+            Dequant8<T>::word(v[q].w, &a[2 * q + 1][2]);
+        }
+        if (FMT == kFmtInt8G) {   // group-wise 8-bit: W' = q_s * s + zero*scale, one rounding (as INT4)
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    typename Pair<T>::type h = *reinterpret_cast<typename Pair<T>::type*>(&a[j][i]);
+                    h = (i & 1) ? __hfma2(h, sB, zB) : __hfma2(h, sA, zA);
+                    a[j][i] = *reinterpret_cast<uint32_t*>(&h);
+                }
+        }
+    }
+}
 
 template <int FMT, typename T, int BPAD, int VAR>
 __global__ void __launch_bounds__(gemm_threads(VAR), gemm_min_ctas(FMT, BPAD, VAR))
@@ -267,14 +310,10 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
     constexpr int XS = gemm_x_stages(BPAD);                // activation ring depth
     constexpr int NDQ_WARPS = gemm_ndq_warps(VAR);
     constexpr int NDQ_THREADS = NDQ_WARPS * 32;
-    constexpr int W_WTMA = NDQ_WARPS, W_XTMA = NDQ_WARPS + 1, W_MMA = NDQ_WARPS + 2;
+    constexpr int W_WTMA = NDQ_WARPS, W_XTMA = NDQ_WARPS + 1;
     constexpr int X_BYTES = gemm_x_stage_bytes(BPAD);
     constexpr int W_BYTES = gemm_w_bytes(FMT);
-    constexpr int A_STAGES = gemm_a_stages(BPAD, VAR);
-    constexpr int TMEM_COLS = gemm_tmem_cols(FMT, BPAD, VAR);
-    constexpr int NACC = gemm_nacc(BPAD);
-    constexpr bool kBf16 = std::is_same<T, __nv_bfloat16>::value;
-    constexpr uint32_t IDESC = make_idesc_f16(kGemmTileN, BPAD, kBf16);
+    constexpr int NACC = BPAD / 2;                         // fp32 accumulators per thread (m64 x BPAD per warpgroup)
     static_assert(WS >= 3, "weight ring too shallow");
 
     // 1024-byte alignment is required by the 128B-swizzled tiles. The array is DECLARED aligned (the kernel has no static
@@ -288,15 +327,7 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
     uint64_t* wempty = wfull + WS;
     uint64_t* xfull = wempty + WS;
     uint64_t* xempty = xfull + XS;
-    uint64_t* afull = xempty + XS;                         // TMEM A buffer written
-#ifdef B200_GEMM_HALF_PUBLISH   // experiment (measured: no gain): publish the two 64-k halves of a TMEM buffer separately
-    uint64_t* aempty = afull + 2 * A_STAGES;               // afull[a] = first 64 k of buffer a, afull[A_STAGES + a] = second 64 k
-#else
-    uint64_t* aempty = afull + A_STAGES;                   // TMEM A buffer consumed by the MMA
-#endif
-    uint64_t* dfull = aempty + A_STAGES;                   // accumulator complete
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(dfull + 1);
-    int* s_flag = reinterpret_cast<int*>(tmem_slot + 1);
+    int* s_flag = reinterpret_cast<int*>(xempty + XS);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tile = blockIdx.x, split = blockIdx.y;
@@ -304,20 +335,6 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
         unsigned long long gt;
         asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
         atomicMin(reinterpret_cast<unsigned long long*>(&p.trace[8 * 64 + 14]), gt);   // earliest CTA start (ns)
-        {
-            const int cta = blockIdx.y * gridDim.x + blockIdx.x;
-            if (cta < 1024) {
-                uint32_t smid;
-                asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-                p.trace[8 * 64 + 16 + cta * 3 + 0] = smid;
-                p.trace[8 * 64 + 16 + cta * 3 + 1] = (long long)gt;
-            }
-        }
-        if ((blockIdx.x == 0 || blockIdx.x == gridDim.x - 1) && blockIdx.y == 0) {
-            const int o = blockIdx.x == 0 ? 0 : 4;
-            p.trace[8 * 64 + o + 0] = clock64();
-            p.trace[8 * 64 + o + 2] = (long long)gt;
-        }
     }
     const int kb0 = split * p.kb_per_split;
     const int kb1 = min(kb0 + p.kb_per_split, p.k_blocks);
@@ -326,37 +343,21 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
     if (threadIdx.x == 0) {
         for (int s = 0; s < WS; ++s) {
             mbar_init(&wfull[s], 1);
-            mbar_init(&wempty[s], FMT == kFmtF16 ? 1 : 4);
+            mbar_init(&wempty[s], NDQ_WARPS);   // every dequant warp reads (or multiplies from) every weight stage
         }
         for (int s = 0; s < XS; ++s) {
             mbar_init(&xfull[s], 1);
-            mbar_init(&xempty[s], 1);
+            mbar_init(&xempty[s], NDQ_WARPS);
         }
-        for (int a = 0; a < A_STAGES; ++a) {
-            mbar_init(&afull[a], 4);
-#ifdef B200_GEMM_HALF_PUBLISH
-            mbar_init(&afull[A_STAGES + a], 4);
-#endif
-            mbar_init(&aempty[a], 1);
-        }
-        mbar_init(dfull, 1);
         fence_mbar_init();
     }
-    if (warp == W_MMA) {
-        tmem_alloc(tmem_slot, TMEM_COLS);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t tmem_d = tmem_base;                // NACC accumulator tiles of BPAD fp32 columns, lane = output feature
-    const uint32_t tmem_a = tmem_base + NACC * BPAD;  // then A_STAGES buffers of 64 columns: the fp16 A operand
 
     if (warp == W_WTMA) {
         // ------------------------------------------------------------------ weight producer (HBM stream)
         // Weights never depend on the previous kernel: under programmatic dependent launch this warp starts
         // streaming at once; only the activation producer waits for the upstream grid.
+        if (p.use_pdl && lane == 0) pdl_launch_dependents();
         if (elect_one()) {
             if (FMT == kFmtF16) tma_prefetch_desc(&w_map);
             const uint8_t* wsrc = p.w_blob + ((size_t)tile * p.k_blocks + kb0) * (size_t)W_BYTES;
@@ -401,288 +402,148 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
                 }
             }
         }
-    } else if (warp == W_MMA) {
-        // ------------------------------------------------------------------ MMA issuer (one elected thread)
-        // Warp-uniform control flow + elect.sync: ptxas then knows a single thread issues the tcgen05 instructions and
-        // moves their operands to uniform registers directly (with `if (lane == 0)` it emits an ELECT/R2UR/branch
-        // "waterfall" loop around EVERY UTCHMMA, ~100 cycles each -- measured with tools/gemm_trace.py).
-        if (p.use_pdl && lane == 0) pdl_launch_dependents();
-        int sw = 0, sx = 0, a = 0;
-        uint32_t phw = 0, phx = 0, aph = 0;
-        for (int it = 0; it < nkb; ++it) {
-            mbar_wait(&xfull[sx], phx);
-            if (FMT == kFmtF16) mbar_wait(&wfull[sw], phw);
-            else mbar_wait(&afull[a], aph);
-            int sx_n = sx + 1, sw_n = sw + 1, a_n = a + 1;
-            uint32_t phx_n = phx, phw_n = phw, aph_n = aph;
-            if (sx_n == XS) { sx_n = 0; phx_n ^= 1; }
-            if (sw_n == WS) { sw_n = 0; phw_n ^= 1; }
-            if (a_n == A_STAGES) { a_n = 0; aph_n ^= 1; }
-            tc_fence_after();
-            if (elect_one()) {
-                B200_TRACE(6, it);
-                const uint32_t xs = smem_u32(xring + sx * X_BYTES);
-                const uint32_t wsm = smem_u32(wring + sw * W_BYTES);
-#pragma unroll
-                for (int j = 0; j < kGemmBK / 16; ++j) {
-                    if (B200_DBG(4)) break;
-#ifdef B200_GEMM_HALF_PUBLISH
-                    if (FMT != kFmtF16 && j == 4) {        // the second 64 k of the block are published separately
-                        mbar_wait(&afull[A_STAGES + a], aph);
-                        tc_fence_after();
-                    }
-#endif
-                    const uint64_t bdesc = make_smem_desc_sw128(xs + (j >> 2) * (BPAD * 128) + (j & 3) * 32);
-                    const uint32_t acc = (it > 0 || j >= NACC) ? 1u : 0u;
-                    const uint32_t dcol = tmem_d + (j % NACC) * BPAD;
-                    if (FMT == kFmtF16) {
-                        const uint64_t adesc = make_smem_desc_sw128(wsm + (j >> 2) * 16384 + (j & 3) * 32);
-                        umma_ss_f16(dcol, adesc, bdesc, IDESC, acc);
-                    } else {
-                        umma_ts_f16(dcol, tmem_a + a * 64 + j * 8, bdesc, IDESC, acc);
-                    }
-                }
-                umma_commit(&xempty[sx]);                       // activation stage consumed
-                if (FMT == kFmtF16) umma_commit(&wempty[sw]);   // f16 weights are read by the MMA itself
-                else umma_commit(&aempty[a]);                   // TMEM A buffer reusable
-                if (it == nkb - 1) umma_commit(dfull);          // accumulator final
-                B200_TRACE(7, it);
-            }
-            __syncwarp();
-            sx = sx_n; phx = phx_n;
-            sw = sw_n; phw = phw_n;
-            a = a_n; aph = aph_n;
-        }
     } else {
-        // ------------------------------------------------------------------ dequant warps (TMEM A producers)
-        // Two groups of four warps take ALTERNATE k-blocks (two blocks in flight per CTA); inside a group warp q owns TMEM
-        // lane quarter q, i.e. 32 feature rows x the whole 128-deep block, processed as two 64-k halves. One barrier round
-        // (weights landed / TMEM buffer free / buffer published) therefore covers 4096 weights per warp: the round's
-        // latency (~100 cycles per mbarrier operation even when the phase is already complete) is what bounds this loop.
-        const int quarter = warp & 3;     // TMEM lane quarter this warp may touch (hardware rule: warp id % 4)
-        const int grp = warp >> 2;        // dequant group 0/1
-        const int row = quarter * 32 + lane;
-        const uint32_t lane_addr = (uint32_t)(quarter * 32) << 16;
-        if (FMT != kFmtF16) {
-            constexpr int G = 2;
-            int s = grp % WS, a = grp % A_STAGES;
-            uint32_t ph = 0, aph = 0;
-            for (int it = grp; it < nkb; it += G) {
-                mbar_wait(&wfull[s], ph);
-                if (threadIdx.x == 0) B200_TRACE(2, it);
-                const uint32_t wb = smem_u32(wring) + s * W_BYTES;   // 32-bit shared address of this stage
-                typename Pair<T>::type s2, zs2;
-                if (FMT == kFmtInt4 || FMT == kFmtInt8G) {
-                    constexpr int Q_BYTES = FMT == kFmtInt4 ? 8192 : 16384;
-                    s2 = Pair<T>::bcast((uint16_t)lds_u16(wb + Q_BYTES + row * 2));
-                    zs2 = Pair<T>::bcast((uint16_t)lds_u16(wb + Q_BYTES + 256 + row * 2));
-                }
+        // ------------------------------------------------------------------ dequant + MMA warpgroups
+        // Warpgroup g (warps 4g..4g+3) owns feature rows 64g..64g+63 of the tile: each warp dequantises its 16 rows of every
+        // k-block into wgmma A fragments in registers and the warpgroup multiplies them with the activation block from
+        // shared memory (wgmma, A from registers, B K-major SW128), fp32 accumulators in registers. The FP16-weight variant
+        // multiplies straight from the TMA-loaded weight tile (A from shared memory).
+        const int R = warp;
+        const int t4 = lane & 3;
+        float acc[NACC];
 #pragma unroll
-                for (int half = 0; half < 2; ++half) {
-                    uint32_t regs[2][16];
-                    if (FMT == kFmtInt4) {
-                        uint4 v[2];
+        for (int q = 0; q < NACC; ++q) acc[q] = 0.f;
+        int sw = 0, sx = 0;
+        uint32_t phw = 0, phx = 0;
+        for (int it = 0; it < nkb; ++it) {
+            mbar_wait(&wfull[sw], phw);
+            if (threadIdx.x == 0) B200_TRACE(2, it);
+            uint32_t a[8][4];
+            if (FMT != kFmtF16) load_w_frag<FMT, T>(smem_u32(wring + sw * W_BYTES), R, lane, a, smem_u32(&wempty[sw]));
+            if (threadIdx.x == 0) B200_TRACE(3, it);
+            mbar_wait(&xfull[sx], phx);
+            if (threadIdx.x == 0) B200_TRACE(6, it);
+            const uint32_t xs = smem_u32(xring + sx * X_BYTES);
+            const uint32_t wsm = smem_u32(wring + sw * W_BYTES) + (uint32_t)(warp >> 2) * 8192;   // rows 64g.. of the tile
+            fence_regs(acc);
+            wgmma_fence();
 #pragma unroll
-                        for (int cc = 0; cc < 2; ++cc) v[cc] = lds_v4(wb + (half * 2 + cc) * 2048 + row * 16);
-                        if (half == 1) {   // every byte of the stage this warp needs is in registers: release it
-                            __syncwarp();
-                            if (lane == 0) mbar_arrive(&wempty[s]);
-                        }
-#pragma unroll
-                        for (int cc = 0; cc < 2; ++cc) {
-                            if (B200_DBG(1)) {
-#pragma unroll
-                                for (int q = 0; q < 16; ++q) regs[cc][q] = (q & 1) ? v[cc].x ^ v[cc].w : v[cc].y ^ v[cc].z;
-                                continue;
-                            }
-                            Dequant4<T>::word(v[cc].x, s2, zs2, &regs[cc][0]);
-                            Dequant4<T>::word(v[cc].y, s2, zs2, &regs[cc][4]);
-                            Dequant4<T>::word(v[cc].z, s2, zs2, &regs[cc][8]);
-                            Dequant4<T>::word(v[cc].w, s2, zs2, &regs[cc][12]);
-                        }
-                    } else {
-                        uint4 v[2][2];
-#pragma unroll
-                        for (int cc = 0; cc < 2; ++cc)
-#pragma unroll
-                            for (int h = 0; h < 2; ++h) v[cc][h] = lds_v4(wb + ((half * 2 + cc) * 2 + h) * 2048 + row * 16);
-                        if (half == 1) {
-                            __syncwarp();
-                            if (lane == 0) mbar_arrive(&wempty[s]);
-                        }
-#pragma unroll
-                        for (int cc = 0; cc < 2; ++cc)
-#pragma unroll
-                            for (int h = 0; h < 2; ++h) {
-                                Dequant8<T>::word(v[cc][h].x, &regs[cc][h * 8 + 0]);
-                                Dequant8<T>::word(v[cc][h].y, &regs[cc][h * 8 + 2]);
-                                Dequant8<T>::word(v[cc][h].z, &regs[cc][h * 8 + 4]);
-                                Dequant8<T>::word(v[cc][h].w, &regs[cc][h * 8 + 6]);
-                            }
-                        if (FMT == kFmtInt8G) {   // group-wise 8-bit: W' = q_s * s + zero*scale, one rounding (as INT4)
-#pragma unroll
-                            for (int cc = 0; cc < 2; ++cc)
-#pragma unroll
-                                for (int q = 0; q < 16; ++q) {
-                                    typename Pair<T>::type h = *reinterpret_cast<typename Pair<T>::type*>(&regs[cc][q]);
-                                    h = __hfma2(h, s2, zs2);
-                                    regs[cc][q] = *reinterpret_cast<uint32_t*>(&h);
-                                }
-                        }
-                    }
-                    if (half == 0) {
-                        if (threadIdx.x == 0) B200_TRACE(3, it);
-                        mbar_wait(&aempty[a], aph ^ 1);
-                        if (threadIdx.x == 0) B200_TRACE(4, it);
-                        tc_fence_after();
-                    }
-                    const uint32_t dst = tmem_a + lane_addr + a * 64 + half * 32;
-                    if (B200_DBG(2)) {
-                        if (regs[0][0] == 0x12345678u && regs[1][15] == 0x9abcdef0u) s_flag[1] = 1;  // keep the math alive
-                    } else {
-                        tmem_st_32x32b_x16(dst, regs[0]);
-                        tmem_st_32x32b_x16(dst + 16, regs[1]);
-                    }
-#ifdef B200_GEMM_HALF_PUBLISH
-                    // publish each 64-k half on its own barrier: the MMA starts on half 0 while half 1 is being dequantised
-                    tmem_wait_st();
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&afull[half * A_STAGES + a]);
-#endif
-                }
-#ifndef B200_GEMM_HALF_PUBLISH
-                // publish the block at once (measured: deferring the publish behind the next block's math is slower --
-                // the dequant -> MMA -> release chain, not the TMEM store latency, bounds the loop)
-                tmem_wait_st();
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&afull[a]);
-#endif
-                if (threadIdx.x == 0) B200_TRACE(5, it);
-                s += G;
-                if (s >= WS) {
-                    s -= WS;
-                    ph ^= 1;
-                }
-                a += G;
-                if (a >= A_STAGES) {
-                    a -= A_STAGES;
-                    aph ^= 1;
-                }
+            for (int j = 0; j < kGemmBK / 16; ++j) {
+                const uint64_t bdesc = make_smem_desc_sw128(xs + (j >> 2) * (BPAD * 128) + (j & 3) * 32);
+                if constexpr (FMT == kFmtF16) wgmma_ss<BPAD, T>(acc, make_smem_desc_sw128(wsm + (j >> 2) * 16384 + (j & 3) * 32), bdesc, 1u);
+                else wgmma_rs<BPAD, T>(acc, a[j], bdesc, 1u);
             }
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(acc);
+            if (threadIdx.x == 0) B200_TRACE(7, it);
+            __syncwarp();
+            if (lane == 0) {
+                mbar_arrive(&xempty[sx]);                       // activation stage consumed
+                if (FMT == kFmtF16) mbar_arrive(&wempty[sw]);   // f16 weights are read by the MMA itself
+            }
+            if (++sx == XS) { sx = 0; phx ^= 1; }
+            if (++sw == WS) { sw = 0; phw ^= 1; }
         }
+        // every dequant warp is past its last read of both rings: the epilogues below may reuse them as staging
+        asm volatile("bar.sync 1, %0;" ::"n"(NDQ_THREADS) : "memory");
 
         // ------------------------------------------------------------------ epilogue
-#define B200_TRACE_E(i)                                                                                          \
-    do {                                                                                                         \
-        if (B200_TRACING && threadIdx.x == 0 && blockIdx.x == 0 && blockIdx.y == 0) p.trace[8 * 64 + 8 + (i)] = clock64(); \
-    } while (0)
-        B200_TRACE_E(0);
-        mbar_wait(dfull, 0);
-        tc_fence_after();
-        B200_TRACE_E(1);
-        // warps with the same lane quarter share the batch columns in slices of 16
-        constexpr int SLICES = BPAD / 16;                   // 16-column slices of the accumulator
-        constexpr int KCS = NDQ_WARPS / 4;                  // warps per lane quarter
-        const int kce = warp >> 2;                          // this warp's index among them
-        const int n = tile * kGemmTileN + row;
-        const bool n_ok = n < p.N;
+        // this thread's accumulators: rows[h] (h = 0, 1) x batch columns 8i + 2*t4 + c, value acc[4i + 2h + c]
+        const int rows[2] = {16 * R + (lane >> 2), 16 * R + (lane >> 2) + 8};
         const int n_tiles = gridDim.x;
         T* yp = reinterpret_cast<T*>(p.y);
-        float cscale = 1.f, bias = 0.f;
-        if (n_ok) {
-            if (FMT == kFmtInt8) cscale = to_f32<T>(reinterpret_cast<const T*>(p.col_scale)[n]);
-            if (p.bias) bias = to_f32<T>(reinterpret_cast<const T*>(p.bias)[n]);
+        float cscale[2] = {1.f, 1.f}, bias[2] = {0.f, 0.f};
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int n = tile * kGemmTileN + rows[h];
+            if (n < p.N) {
+                if (FMT == kFmtInt8) cscale[h] = to_f32<T>(reinterpret_cast<const T*>(p.col_scale)[n]);
+                if (p.bias) bias[h] = to_f32<T>(reinterpret_cast<const T*>(p.bias)[n]);
+            }
         }
         float* fin = reinterpret_cast<float*>(wring);       // [bpad][128] fp32 staging for the fused SiLU*mul (weight ring is idle)
-        // 16 batch columns of this thread's feature row, summed over the NACC accumulator tiles
-        auto load_acc = [&](int sl, float (&v)[16]) {
-            uint32_t r[NACC][16];
-#pragma unroll
-            for (int q = 0; q < NACC; ++q) tmem_ld_32x32b_x16(tmem_d + lane_addr + q * BPAD + sl * 16, r[q]);
-            tmem_wait_ld();
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-                float a = __uint_as_float(r[0][j]);
-#pragma unroll
-                for (int q = 1; q < NACC; ++q) a += __uint_as_float(r[q][j]);
-                v[j] = a;
-            }
-        };
         if (p.nsplit == 1) {
-            RsLane rsl{};
-            if constexpr (VAR == 1) rsl = rs_lane(p, n);
-            for (int sl = kce; sl < SLICES; sl += KCS) {
-                float v[16];
-                load_acc(sl, v);
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const int b = sl * 16 + j;
-                    if (p.silu_mul) fin[b * kGemmTileN + row] = fmaf(v[j], cscale, bias);
-                    else if constexpr (VAR == 1) {
-                        if (b < p.B) rs_emit<T>(p, rsl, b, n, fmaf(v[j], cscale, bias), lane);    // N % 128 == 0 in this mode
-                    } else if (n_ok && b < p.B) yp[(size_t)b * p.N + n] = from_f32<T>(fmaf(v[j], cscale, bias));
-                }
+            RsLane rsl[2] = {};
+            if constexpr (VAR == 1) {
+                rsl[0] = rs_lane(p, tile * kGemmTileN + rows[0]);
+                rsl[1] = rs_lane(p, tile * kGemmTileN + rows[1]);
             }
+#pragma unroll
+            for (int i = 0; i < BPAD / 8; ++i)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int c = 0; c < 2; ++c) {
+                        const int b = 8 * i + 2 * t4 + c, n = tile * kGemmTileN + rows[h];
+                        const float v = fmaf(acc[4 * i + 2 * h + c], cscale[h], bias[h]);
+                        if (p.silu_mul) fin[b * kGemmTileN + rows[h]] = v;
+                        else if constexpr (VAR == 1) rs_emit<T>(p, rsl[h], b, n, v, lane, 4);   // N % 128 == 0 in this mode
+                        else if (n < p.N && b < p.B) yp[(size_t)b * p.N + n] = from_f32<T>(v);
+                    }
         } else if (p.cluster_reduce) {
             // split-K merge through distributed shared memory: park the fp32 partial tile [bpad][128] in this CTA's smem
-            // (the activation ring is idle once the accumulator is final); the merge itself follows the cluster barrier below.
+            // (the activation ring is idle now); the merge itself follows the cluster barrier below.
             float* red = reinterpret_cast<float*>(xring);
-            for (int sl = kce; sl < SLICES; sl += KCS) {
-                float v[16];
-                load_acc(sl, v);
 #pragma unroll
-                for (int j = 0; j < 16; ++j) red[(sl * 16 + j) * kGemmTileN + row] = v[j];
-            }
+            for (int i = 0; i < BPAD / 8; ++i)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int c = 0; c < 2; ++c) red[(8 * i + 2 * t4 + c) * kGemmTileN + rows[h]] = acc[4 * i + 2 * h + c];
         } else {
             // write the fp32 partial tile [bpad][128] (coalesced along n), then the last CTA of this n-tile reduces
             float* wsp = p.ws + ((size_t)split * n_tiles + tile) * (size_t)(BPAD * kGemmTileN);
-            for (int sl = kce; sl < SLICES; sl += KCS) {
-                float v[16];
-                load_acc(sl, v);
 #pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const int b = sl * 16 + j;
-                    if (b < p.B) __stcg(&wsp[(size_t)b * kGemmTileN + row], v[j]);
-                }
-            }
-            B200_TRACE_E(2);
+            for (int i = 0; i < BPAD / 8; ++i)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int c = 0; c < 2; ++c) {
+                        const int b = 8 * i + 2 * t4 + c;
+                        if (b < p.B) __stcg(&wsp[(size_t)b * kGemmTileN + rows[h]], acc[4 * i + 2 * h + c]);
+                    }
             __threadfence();
             asm volatile("bar.sync 1, %0;" ::"n"(NDQ_THREADS) : "memory");
-            B200_TRACE_E(3);
             if (threadIdx.x == 0) {
                 const int prev = atomicAdd(&p.sem[tile], 1);
                 *s_flag = (prev == p.nsplit - 1);
             }
             asm volatile("bar.sync 1, %0;" ::"n"(NDQ_THREADS) : "memory");
-            B200_TRACE_E(4);
             if (*s_flag) {
                 __threadfence();
+                // the reducer: thread = feature row (warp % 4) * 32 + lane, the two warps of a row share its 16-column slices
+                constexpr int SLICES = BPAD / 16, KCS = NDQ_WARPS / 4;
+                const int row = (warp & 3) * 32 + lane, kce = warp >> 2;
+                const int n = tile * kGemmTileN + row;
+                const bool n_ok = n < p.N;
+                float cs1 = 1.f, bi1 = 0.f;
+                if (n_ok) {
+                    if (FMT == kFmtInt8) cs1 = to_f32<T>(reinterpret_cast<const T*>(p.col_scale)[n]);
+                    if (p.bias) bi1 = to_f32<T>(reinterpret_cast<const T*>(p.bias)[n]);
+                }
                 for (int sl = kce; sl < SLICES; sl += KCS) {
                     // all loads of a slice are issued before the first use (the partials sit in L2)
-                    float acc[16];
+                    float s16[16];
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) acc[j] = 0.f;
+                    for (int j = 0; j < 16; ++j) s16[j] = 0.f;
                     for (int sp = 0; sp < p.nsplit; ++sp) {
                         const float* src = p.ws + ((size_t)sp * n_tiles + tile) * (size_t)(BPAD * kGemmTileN) + row;
 #pragma unroll
                         for (int j = 0; j < 16; ++j) {
                             const int b = sl * 16 + j;
-                            if (b < p.B) acc[j] += __ldcg(src + (size_t)b * kGemmTileN);
+                            if (b < p.B) s16[j] += __ldcg(src + (size_t)b * kGemmTileN);
                         }
                     }
 #pragma unroll
                     for (int j = 0; j < 16; ++j) {
                         const int b = sl * 16 + j;
-                        if (n_ok && b < p.B) yp[(size_t)b * p.N + n] = from_f32<T>(fmaf(acc[j], cscale, bias));
+                        if (n_ok && b < p.B) yp[(size_t)b * p.N + n] = from_f32<T>(fmaf(s16[j], cs1, bi1));
                     }
                 }
                 if (threadIdx.x == 0) p.sem[tile] = 0;
             }
         }
-        B200_TRACE_E(5);
-        tc_fence_before();
     }
 
     if (p.nsplit > 1 && p.cluster_reduce) {
@@ -714,7 +575,7 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
 #pragma unroll
                 for (int sp = 0; sp < 8; ++sp) acc += part[sp];
                 if (p.silu_mul) reinterpret_cast<float*>(wring)[b * kGemmTileN + row] = fmaf(acc, cscale, bias);
-                else if constexpr (VAR == 1) rs_emit<T>(p, rsl, b, n, fmaf(acc, cscale, bias), lane);
+                else if constexpr (VAR == 1) rs_emit<T>(p, rsl, b, n, fmaf(acc, cscale, bias), lane, 1);
                 else if (n_ok) yp[(size_t)b * p.N + n] = from_f32<T>(fmaf(acc, cscale, bias));
             }
         }
@@ -744,24 +605,23 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
         unsigned long long gt;
         asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
         atomicMax(reinterpret_cast<unsigned long long*>(&p.trace[8 * 64 + 15]), gt);   // latest CTA end (ns)
-        {
-            const int cta = blockIdx.y * gridDim.x + blockIdx.x;
-            if (cta < 1024) p.trace[8 * 64 + 16 + cta * 3 + 2] = (long long)gt;
-        }
-        if ((blockIdx.x == 0 || blockIdx.x == gridDim.x - 1) && blockIdx.y == 0) {
-            const int o = blockIdx.x == 0 ? 0 : 4;
-            p.trace[8 * 64 + o + 1] = clock64();
-            p.trace[8 * 64 + o + 3] = (long long)gt;
-        }
-    }
-    if (warp == W_MMA) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, TMEM_COLS);
     }
 }
 
 // ---- load-time re-layout kernels (replace device_impl.py:392-479 preprocess_weights_for_mixed_gemm): reference
-// (un-permuted) tensors -> per-(n-tile, k-block) blobs consumed above.
+// (un-permuted) tensors -> per-(n-tile, k-block) blobs consumed above (fragment order: see load_w_frag).
+// Element of register i of the A fragment of k-step j held by (warp R, lane): row 16R + lane/4 + 8*(i & 1),
+// k = 16j + 2*(lane % 4) + 8*(i >> 1) (+1 for the high half).
+__host__ __device__ __forceinline__ int frag_row(int R, int lane, int i) { return 16 * R + (lane >> 2) + 8 * (i & 1); }
+__host__ __device__ __forceinline__ int frag_k(int j, int lane, int i, int hi) { return 16 * j + 2 * (lane & 3) + 8 * (i >> 1) + hi; }
+// 8-bit payload byte -> (row, k within the block): vector (j / 2, R, lane) of 16 bytes, 8 bytes per k-step
+__host__ __device__ __forceinline__ void frag8_pos(int byte_in_block, int& r, int& kl) {
+    const int vec = byte_in_block / 16, bv = byte_in_block % 16;
+    const int q = vec / 256, R = (vec / 32) % 8, lane = vec % 32;
+    const int j = 2 * q + (bv >> 3), i = ((bv >> 2) & 1) * 2 + ((bv >> 1) & 1);
+    r = frag_row(R, lane, i);
+    kl = frag_k(j, lane, i, bv & 1);
+}
 // int4: q_packed [K][N/2] (byte = hi nibble col 2j+1, lo nibble col 2j, two's complement q_s), scales/zs [K/128][N] (16-bit).
 static __global__ void pack_w4_kernel(const uint8_t* __restrict__ q_packed, const uint16_t* __restrict__ scales,
                                const uint16_t* __restrict__ zs, int K, int N, uint8_t* __restrict__ blob) {
@@ -775,19 +635,18 @@ static __global__ void pack_w4_kernel(const uint8_t* __restrict__ q_packed, cons
         const int kb = (int)(blk % k_blocks), tile = (int)(blk / k_blocks);
         uint32_t out = 0;
         if (word_in_block < 2048) {
-            const int c = word_in_block / 512, r = (word_in_block % 512) / 4, j = word_in_block % 4;
-            const int n = tile * kGemmTileN + r;
-            if (n < N) {
+            // vector (j / 4, R, lane), word j % 4 of it = k-step j
+            const int vec = word_in_block / 4, R = (vec / 32) % 8, lane = vec % 32, j = (vec / 256) * 4 + word_in_block % 4;
 #pragma unroll
-                for (int pos = 0; pos < 8; ++pos) {
-                    const int kl = c * 32 + j * 8 + (pos < 4 ? 2 * pos : 2 * (pos - 4) + 1);
+            for (int pos = 0; pos < 8; ++pos) {
+                const int n = tile * kGemmTileN + frag_row(R, lane, pos & 3), kl = frag_k(j, lane, pos & 3, pos >> 2);
+                uint32_t u = 8;  // q_s = 0 for padded features
+                if (n < N) {
                     const uint8_t byte = q_packed[(size_t)(kb * kGemmBK + kl) * (N / 2) + n / 2];
                     const uint32_t nib = (n & 1) ? (byte >> 4) : (byte & 0xF);
-                    const uint32_t u = (nib + 8) & 0xF;  // two's complement q_s -> q_s + 8
-                    out |= u << (4 * pos);
+                    u = (nib + 8) & 0xF;  // two's complement q_s -> q_s + 8
                 }
-            } else {
-                out = 0x88888888u;  // q_s = 0 for padded features
+                out |= u << (4 * pos);
             }
         } else {
             const int w = word_in_block - 2048;          // 0..127: 64 words of scales then 64 words of zs
@@ -811,8 +670,9 @@ static __global__ void pack_w8_kernel(const int8_t* __restrict__ q, int K, int N
         const int byte_in_block = (int)(idx % kW8BlockBytes);
         const size_t blk = idx / kW8BlockBytes;
         const int kb = (int)(blk % k_blocks), tile = (int)(blk / k_blocks);
-        const int c = byte_in_block / 2048, r = (byte_in_block % 2048) / 16, i = byte_in_block % 16;
-        const int n = tile * kGemmTileN + r, k = kb * kGemmBK + c * 16 + i;
+        int r, kl;
+        frag8_pos(byte_in_block, r, kl);
+        const int n = tile * kGemmTileN + r, k = kb * kGemmBK + kl;
         blob[idx] = (n < N) ? (uint8_t)((int)q[(size_t)k * N + n] + 128) : (uint8_t)128;
     }
 }
@@ -828,8 +688,9 @@ static __global__ void pack_w8g_kernel(const int8_t* __restrict__ q, const uint1
         const size_t blk = idx / kW8GBlockBytes;
         const int kb = (int)(blk % k_blocks), tile = (int)(blk / k_blocks);
         if (byte_in_block < 16384) {
-            const int c = byte_in_block / 2048, r = (byte_in_block % 2048) / 16, i = byte_in_block % 16;
-            const int n = tile * kGemmTileN + r, k = kb * kGemmBK + c * 16 + i;
+            int r, kl;
+            frag8_pos(byte_in_block, r, kl);
+            const int n = tile * kGemmTileN + r, k = kb * kGemmBK + kl;
             blob[idx] = (n < N) ? (uint8_t)((int)q[(size_t)k * N + n] + 128) : (uint8_t)128;
         } else {
             const int w = byte_in_block - 16384;         // 256 bytes of scales then 256 bytes of zs

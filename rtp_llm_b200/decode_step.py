@@ -1,4 +1,4 @@
-"""One decode step of a dense Llama/Qwen-style stack on the B200 hot path (synthetic weights, synthetic page tables).
+"""One decode step of a dense Llama/Qwen-style stack on the H100 hot path (synthetic weights, synthetic page tables).
 
 This is the measurement harness of SURVEY.md section 8(d): per layer
     add_rmsnorm -> qkv GEMM -> rope + KV append -> paged decode attention -> o GEMM -> [TP all-reduce]
@@ -88,8 +88,8 @@ class DecodeStep:
         self.fuse_gemm_rs = (bool(fuse_gemm_rs) and fuse_ar_norm and tp_size > 1 and hasattr(comm, "gemm_rs")
                              and comm.gemm_rs_supported(batch, cfg.hidden))
         # RoPE + K/V append inside the attention kernel (b200_paged_decode_attn_rope): bit-identical, one launch less per layer,
-        # but measured 0.4 % SLOWER at the headline config (same box A/B, profiles/r02_fuse_rope_ab.txt): under PDL the stand-alone
-        # rope kernel hides behind its neighbours while the fused prologue sits on the attention kernel's critical path.
+        # but under PDL the stand-alone rope kernel hides behind its neighbours while the fused prologue sits on the attention
+        # kernel's critical path.
         # Default off; B200_FUSE_ROPE=1 or fuse_rope=True turns it on.
         if fuse_rope is None:
             fuse_rope = os.environ.get("B200_FUSE_ROPE", "0") == "1"

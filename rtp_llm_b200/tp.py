@@ -1,7 +1,7 @@
 """Tensor-parallel collectives of the decode path: SUM all-reduce of [B, hidden] after each row-parallel GEMM
 (reference: distributed/collective_torch.py:694-722, call sites hybrid/causal_attention.py:91-92, dense_mlp.py:104-105)
 and the all-gather of vocab-split logits (cpp/models/PyWrappedModel.cc:915-936).  One process per GPU,
-torch.distributed (NCCL over NVLink 5 / NVSwitch) as plumbing; both calls are CUDA-graph capturable."""
+torch.distributed (NCCL over NVLink 4 / NVSwitch) as plumbing; both calls are CUDA-graph capturable."""
 from __future__ import annotations
 
 import torch

@@ -10,7 +10,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run by the driver on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an NVIDIA H100 (sm_90)")
 
 
 @pytest.fixture(scope="session")

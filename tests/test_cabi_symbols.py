@@ -64,8 +64,8 @@ def test_argument_errors_of_the_round2_entry_points():
     assert lib.b200_peer_gather_norm(p, p, p, p, 0, 32, 4100, 1e-5, regs, 1 << 19, 0, 2, None) == -1 and b"hidden" in lib.b200_last_error()
 
 
-def test_sass_uses_the_blackwell_paths():
-    """The built library must contain tcgen05 MMA, TMEM ld/st and TMA instructions (SASS mnemonics of B200_PROFILING.md)."""
+def test_sass_uses_the_hopper_paths():
+    """The built library must contain warpgroup MMA (wgmma) and TMA instructions: tensor-map loads and bulk copies."""
     import shutil
     import subprocess
     cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
@@ -73,12 +73,12 @@ def test_sass_uses_the_blackwell_paths():
         import pytest
         pytest.skip("cuobjdump not available")
     sass = subprocess.run([cuobjdump, "-sass", build.build()], capture_output=True, text=True).stdout
-    for mnem in ("UTCHMMA", "STTM", "LDTM", "UTMALDG", "UBLKCP"):
+    for mnem in ("HGMMA", "WARPGROUP.ARRIVE", "UTMALDG", "UBLKCP"):
         assert mnem in sass, mnem
 
 
 def test_launch_shape_heuristics_on_the_baseline_shapes():
-    """Host-only: the split choices that the B200 measurements (profiles/) showed to be best."""
+    """Host-only: the split choices of the launch-shape heuristics on the baseline shapes (132 SMs when no device is visible)."""
     import ctypes
     lib = _lib.load()
 
@@ -91,9 +91,10 @@ def test_launch_shape_heuristics_on_the_baseline_shapes():
         ns, kb = ctypes.c_int(), ctypes.c_int()
         assert lib.b200_plan_gemm_split(K, N, ctypes.byref(ns), ctypes.byref(kb)) == 0
         return ns.value, kb.value
-    assert attn(32 * 8, 2048) == (1, 32)          # Llama-3-8B B32 ctx2048: one CTA per (sequence, kv head), 94 % of HBM peak
+    assert attn(32 * 8, 2048) == (1, 32)          # Llama-3-8B B32 ctx2048: one CTA per (sequence, kv head)
     assert attn(32 * 4, 2048) == (1, 32)          # TP2 per-rank shape
-    assert attn(32 * 1, 2048) == (4, 8)           # TP8 per-rank shape
+    assert attn(32 * 1, 2048) == (2, 16)          # TP8 per-rank shape: 32 units, the sequence split in two (the H100 cost
+                                                  # model's choice; not measured against other splits on an H100)
     ns, c = attn(8, 4096)                          # batch 1: split the sequence to fill the GPU
     assert ns > 1 and ns * c >= 64
     assert gemm(4096, 28672) == (1, 32)           # w13: 224 tiles, no split

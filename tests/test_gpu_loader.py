@@ -1,4 +1,4 @@
-"""Checkpoint -> kernel layout -> GEMM on a B200 (loader.py + device.py + linear.py): the GEMM through the loaded weights must
+"""Checkpoint -> kernel layout -> GEMM on an H100 (loader.py + device.py + linear.py): the GEMM through the loaded weights must
 equal X . W for the dense weight the checkpoint means; kernels survive the copies the reference loader makes."""
 import numpy as np
 import pytest

@@ -1,4 +1,4 @@
-"""GPU parity tests (run by the driver with -m gpu on a B200). Everything goes through the C ABI
+"""GPU parity tests (run with -m gpu on an H100). Everything goes through the C ABI
 (rtp_llm_b200.ops -> libb200_decode.so) and is compared with the CPU oracle on the same seeded inputs, with the golden
 fixtures the reference's code produced -- at BASELINE.json's full sizes too (the OpenMP oracle finishes those in well under
 a second per case); a deliberately naive GPU kernel (test-only library) is kept as a second opinion."""

@@ -1,5 +1,5 @@
 """b200_rope_append_ex (the full decode rope contract) against oracle_rope_append_ex, which is pinned to the reference's torch
-RoPE / RopeCache tables (tests/test_oracle_golden.py), through the C ABI on a B200."""
+RoPE / RopeCache tables (tests/test_oracle_golden.py), through the C ABI on an H100."""
 import numpy as np
 import pytest
 import torch

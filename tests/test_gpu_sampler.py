@@ -1,5 +1,5 @@
 """b200_sample (csrc/sampling.cuh) against the sampling oracle, which is pinned to the reference's CudaSamplerTest vectors
-(tests/test_sampler_oracle.py), through the C ABI on a B200."""
+(tests/test_sampler_oracle.py), through the C ABI on an H100."""
 import numpy as np
 import pytest
 import torch

@@ -85,9 +85,9 @@ def test_attn_op_support_gate():
     class I:
         is_prefill = True
     assert attention.B200DecodeAttnOp(C()).support(I()) is False          # decode only
-    C.size_per_head = 64
+    C.size_per_head = 96
     I.is_prefill = False
-    assert attention.B200DecodeAttnOp(C()).support(I()) is False          # head_dim 128 only
+    assert attention.B200DecodeAttnOp(C()).support(I()) is False          # head_dim 64 / 128 / 256 only
 
 
 def test_bench_reference_arm_runs_on_cpu_and_prints_the_contract_line():

@@ -260,7 +260,7 @@ def test_rope_ex_position_override_bias_logn_and_partial_dim():
 @pytest.mark.parametrize("tag", ["f16_512", "f16_4096", "bf16_512", "bf16_4096"])
 def test_norm_ops_match_the_reference_cuda_kernels(golden_dir, tag):
     """oracle_add_rmsnorm against OUTPUTS OF THE KERNELS THE REFERENCE BINDS (flashinfer rmsnorm / fused_add_rmsnorm,
-    RegisterBaseBindings.hpp:45-60), captured on a B200 by tools/make_gpu_golden.py: the stored residual must be bit-exact,
+    RegisterBaseBindings.hpp:45-60), captured with flashinfer 0.6.11.post2 on a B200 by tools/make_gpu_golden.py and re-captured bit-identically on an H100: the stored residual must be bit-exact,
     the normalised output may differ by one rounding step of the output type (sum-of-squares order)."""
     g = np.load(os.path.join(golden_dir, "flashinfer_glue_ops.npz"))
     is_bf16 = tag.startswith("bf16")

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Developer tool: per-k-block timeline (clock64) of CTA (0,0) of the weight-only GEMM."""
+"""Developer tool: per-k-block timeline (clock64) of CTA (0,0) of the weight-only GEMM (needs a B200_DEV=1 build)."""
 import os, sys
 import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -31,35 +31,11 @@ torch.cuda.synchronize()
 print("event-timed launch:", st.elapsed_time(en) * 1e3, "us")
 os.environ.pop("B200_GEMM_TRACE_PTR")
 ex = trace.cpu()[8 * 64:]
-res = trace.cpu()[8 * 64 + 16:].view(1024, 3)
 t = trace.cpu()[: 8 * 64].view(8, 64)
 t0 = int(t[0, 0])
-names = ["w_issue", "x_issue", "dq_wfull", "dq_math", "dq_aempty", "dq_afullarr", "mma_ready", "mma_issued"]
-print("it  " + " ".join(f"{n:>11s}" for n in names))
+# slots written by the kernel (wo_gemm.cuh, B200_TRACE): 4 and 5 are unused
+slots = {0: "w_issue", 1: "x_issue", 2: "dq_wfull", 3: "dq_math", 6: "mma_ready", 7: "mma_done"}
+print("it  " + " ".join(f"{n:>11s}" for n in slots.values()))
 for it in range(min(32, K // 128)):
-    print(f"{it:2d}  " + " ".join(f"{int(t[r, it]) - t0 if int(t[r, it]) else -1:11d}" for r in range(8)))
-
-for nm, o in (("first CTA", 0), ("last CTA", 4)):
-    cyc, ns = int(ex[o + 1] - ex[o + 0]), int(ex[o + 3] - ex[o + 2])
-    print(f"{nm}: {cyc} cycles in {ns} ns -> {cyc / max(ns, 1):.3f} GHz; start offset vs first CTA {int(ex[o + 2] - ex[2])} ns; entry->first W issue {t0 - int(ex[0])} cyc")
-e = [int(v) - int(ex[0]) for v in ex[8:14]]
-print("epilogue (cycles since kernel entry): enter", e[0], "dfull", e[1], "partials stored", e[2], "fence+bar", e[3], "atomic+bar", e[4], "done", e[5], "| kernel end", int(ex[1]) - int(ex[0]))
-
+    print(f"{it:2d}  " + " ".join(f"{int(t[r, it]) - t0 if int(t[r, it]) else -1:11d}" for r in slots))
 print("all CTAs: earliest start -> latest end:", int(ex[15]) - int(ex[14]), "ns")
-
-import collections
-t_min = int(ex[14])
-per_sm = collections.defaultdict(list)
-for c in range(1024):
-    if int(res[c, 1]) == 0:
-        continue
-    per_sm[int(res[c, 0])].append((int(res[c, 1]) - t_min, int(res[c, 2]) - t_min, c))
-overlap = 0
-for sm, lst in per_sm.items():
-    lst.sort()
-    for i in range(1, len(lst)):
-        if lst[i][0] < lst[i - 1][1]:
-            overlap += 1
-print("SMs used", len(per_sm), "CTAs", sum(len(v) for v in per_sm.values()), "pairs overlapping in time on one SM", overlap)
-for sm in sorted(per_sm)[:6]:
-    print("sm", sm, per_sm[sm])

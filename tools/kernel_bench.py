@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Per-kernel timing at the BASELINE shapes (developer tool, run under gpurun). CUDA events on the launching stream,
-warm-up, inputs rotated through > L2-size working sets so nothing is served from the 126 MB L2."""
+"""Per-kernel timing at the BASELINE shapes (developer tool, runs on the GPU). CUDA events on the launching stream,
+warm-up, inputs rotated through > L2-size working sets so nothing is served from the H100's 50 MB L2."""
 import json
 import math
 import os
@@ -14,7 +14,7 @@ from rtp_llm_b200 import ops  # noqa: E402
 from rtp_llm_b200._lib import B200_FMT_F16, B200_FMT_INT4, B200_FMT_INT8  # noqa: E402
 
 dev = torch.device("cuda:0")
-PEAK = 6572.5
+PEAK = 3350.0          # H100 SXM data-sheet HBM3 bandwidth (GB/s); a measured peak replaces it when present
 try:
     PEAK = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]
 except Exception:  # noqa: BLE001

@@ -69,20 +69,20 @@ def main():
 
 
 def fine(ft, names, ops_to_show):
-    slots = ["w_issue", "x_issue", "dq_wfull", "dq_aempty", "dq_afull", "mma_ready", "mma_issued"]
+    # slots written by decode_program.cuh (B200_FT): 3 and 4 are unused; slot 7 holds the epilogue stamps
+    slots = {0: "w_issue", 1: "x_issue", 2: "dq_wfull", 5: "mma_ready", 6: "mma_done"}
     for i in ops_to_show:
         f = ft[i]
         base = f[f > 0].min() if (f > 0).any() else 0
-        print(f"--- fine timeline of CTA 0, op {i} ({names[i]}): cycles since the op's first stamp; dq columns = warp group 0 (even blocks) / 1 (odd)")
-        print(" blk " + " ".join(f"{s:>10}" for s in slots))
+        print(f"--- fine timeline of CTA 0, op {i} ({names[i]}): cycles since the op's first stamp; dq columns = warpgroup 0")
+        print(" blk " + " ".join(f"{s:>10}" for s in slots.values()))
         for b in range(48):
-            if not (f[:7, b] > 0).any():
+            if not any(f[sl, b] > 0 for sl in slots):
                 continue
-            print(f"{b:4d} " + " ".join(f"{(f[sl, b] - base) if f[sl, b] > 0 else -1:10.0f}" for sl in range(7)))
+            print(f"{b:4d} " + " ".join(f"{(f[sl, b] - base) if f[sl, b] > 0 else -1:10.0f}" for sl in slots))
         ep = f[7]
-        print(" epilogues (segment: wait_begin, dfull_seen, done): " + ", ".join(
-            f"[{ep[2*c]-base:.0f}, {ep[2*c+1]-base:.0f}, {ep[16+c]-base:.0f}]" for c in range(8) if ep[2*c] > 0))
-
+        print(" epilogues (segment: begin, done): " + ", ".join(
+            f"[{ep[2*c]-base:.0f}, {ep[16+c]-base:.0f}]" for c in range(8) if ep[2*c] > 0))
 
 if __name__ == "__main__":
     main()
