@@ -13,10 +13,6 @@ LIB = os.path.join(HERE, "libb200_decode.so")
 SOURCES = ["c_api.cu", "gemm_cluster.cu", "gemm_cluster_rs.cu", "segment_f16.cu", "segment_bf16.cu"]
 NVCC_FLAGS = ["-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3",
               "-Xcompiler", "-fPIC", "-DB200_BUILD"]
-if os.environ.get("B200_DEV"):           # developer build: clock64 timeline + ablation switches in the cluster GEMM (tools/gemm_trace.py)
-    NVCC_FLAGS.append("-DB200_GEMM_DEV")  # goes to its own library (lib_dev.so, loaded through B200_LIB_PATH), never the product one
-    OBJDIR = os.path.join(HERE, "build_dev")
-    LIB = os.path.join(HERE, "lib_dev.so")
 TESTREF_SRC = os.path.join(ROOT, "tests", "native", "test_ref.cu")
 TESTREF_LIB = os.path.join(ROOT, "tests", "native", "libb200_testref.so")
 

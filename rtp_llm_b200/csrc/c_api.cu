@@ -53,6 +53,9 @@ int launched(const char* what) {
     return B200_OK;
 }
 
+// The library reads three environment variables, all test hooks that force one parameter of a launch plan the plan could
+// also pick itself, so that tests reach every cluster size and the two-shot all-reduce deterministically:
+// B200_ATTN_TILES_PER_SPLIT (attention split), B200_GEMM_SPLITK (cluster GEMM split-K) and B200_AR_TWOSHOT (all-reduce).
 int env_int(const char* name, int dflt) {
     const char* v = getenv(name);
     return (v && *v) ? atoi(v) : dflt;
@@ -70,19 +73,19 @@ int num_sms() {
     return sms[dev];
 }
 
-int seg_dispatch_f16(int bpad, int qfmt, const ProgOp* op0, const ProgOp* d_ops, int nops, unsigned* gbar, int grid, bool pdl,
+int seg_dispatch_f16(int bpad, int qfmt, const ProgOp* d_ops, int nops, unsigned* gbar, int grid, bool pdl,
                      unsigned long long* trace, cudaStream_t st, int* grid_out);
-int seg_dispatch_bf16(int bpad, int qfmt, const ProgOp* op0, const ProgOp* d_ops, int nops, unsigned* gbar, int grid, bool pdl,
+int seg_dispatch_bf16(int bpad, int qfmt, const ProgOp* d_ops, int nops, unsigned* gbar, int grid, bool pdl,
                       unsigned long long* trace, cudaStream_t st, int* grid_out);
 
 int segment_grid(bool bf16, int bpad, int qfmt, int* grid_out) {
-    return bf16 ? seg_dispatch_bf16(bpad, qfmt, nullptr, nullptr, 0, nullptr, 0, false, nullptr, nullptr, grid_out)
-                : seg_dispatch_f16(bpad, qfmt, nullptr, nullptr, 0, nullptr, 0, false, nullptr, nullptr, grid_out);
+    return bf16 ? seg_dispatch_bf16(bpad, qfmt, nullptr, 0, nullptr, 0, false, nullptr, nullptr, grid_out)
+                : seg_dispatch_f16(bpad, qfmt, nullptr, 0, nullptr, 0, false, nullptr, nullptr, grid_out);
 }
-int launch_segment(bool bf16, int bpad, int qfmt, const ProgOp* op0, const ProgOp* d_ops, int nops, unsigned* gbar, int grid,
-                   bool pdl, unsigned long long* trace, cudaStream_t st) {
-    return bf16 ? seg_dispatch_bf16(bpad, qfmt, op0, d_ops, nops, gbar, grid, pdl, trace, st, nullptr)
-                : seg_dispatch_f16(bpad, qfmt, op0, d_ops, nops, gbar, grid, pdl, trace, st, nullptr);
+int launch_segment(bool bf16, int bpad, int qfmt, const ProgOp* d_ops, int nops, unsigned* gbar, int grid, bool pdl,
+                   unsigned long long* trace, cudaStream_t st) {
+    return bf16 ? seg_dispatch_bf16(bpad, qfmt, d_ops, nops, gbar, grid, pdl, trace, st, nullptr)
+                : seg_dispatch_f16(bpad, qfmt, d_ops, nops, gbar, grid, pdl, trace, st, nullptr);
 }
 
 }  // namespace b200_host
@@ -151,7 +154,6 @@ void attn_split(int units, int max_tiles, int* nsplit, int* tiles_per_split, int
     // fixed time, streams its 32 KB tiles at min(60 GB/s -- what its 96 KB ring sustains --, HBM / resident CTAs), CTAs
     // beyond 2*SMs are back-filled (fractional waves), a split adds ~3 us of merge.
     const double slots = 2.0 * sms, hbm = 3.0e12, r_cta = 60e9, fixed = 3e-6, merge = 3e-6, tile_bytes = 32768.0 * head_dim / 128.0;
-    const bool cluster_ok = env_int("B200_ATTN_CLUSTER", 1) != 0;
     for (int c = 1; c <= max_tiles; ++c) {
         const int ns = (max_tiles + c - 1) / c;
         if (ns > kAttnMaxSplit) continue;
@@ -161,7 +163,7 @@ void attn_split(int units, int max_tiles, int* nsplit, int* tiles_per_split, int
         const double rate = std::min(r_cta, hbm / resident);
         // merging the splits: <= 8 splits form a cluster and merge through DSMEM (~1.5 us); more go through the L2 workspace and
         // a last-arriver loop whose cost grows with the split count (measured 26 us for 16 splits x 8 tiles, r02)
-        const double merge_cost = ns == 1 ? 0.0 : (ns <= 8 && cluster_ok ? 1.5e-6 : merge + 0.55e-6 * ns);
+        const double merge_cost = ns == 1 ? 0.0 : (ns <= 8 ? 1.5e-6 : merge + 0.55e-6 * ns);
         const double cost = waves * (fixed + c * tile_bytes / rate) + merge_cost;
         if (cost < best * (1.0 - 1e-6) || (std::fabs(cost - best) <= best * 1e-6 && c > best_c)) {
             best = cost;
@@ -181,18 +183,19 @@ void attn_split(int units, int max_tiles, int* nsplit, int* tiles_per_split, int
 
 // ---- GEMM launch shape
 int gemm_bpad(int B) { return B <= 16 ? 16 : (B <= 32 ? 32 : (B <= 64 ? 64 : 128)); }
-// one-kernel-per-GEMM path (gemm_cluster.cu): split-K so that one wave of 2*SMs CTAs is filled
-void gemm_split(int n_tiles, int k_blocks, int max_split, int* nsplit, int* kb_per_split) {
+// one-kernel-per-GEMM path (gemm_cluster.cu): split-K so that one wave of 2*SMs CTAs is filled. The nsplit CTAs of a tile
+// form one thread-block cluster (at most 8, the portable cluster size) and must be co-scheduled inside one GPC.
+constexpr int kGemmMaxSplit = 8;
+void gemm_split(int n_tiles, int k_blocks, int* nsplit, int* kb_per_split) {
     const int forced = env_int("B200_GEMM_SPLITK", 0);
     const long slots = 2L * num_sms();
     int best_s = 1;
     double best = 1e30;
-    const int smax = k_blocks < max_split ? k_blocks : max_split;
-    const bool cluster = max_split <= 8;   // cluster mode: the nsplit CTAs of a tile must be co-scheduled inside one GPC
+    const int smax = k_blocks < kGemmMaxSplit ? k_blocks : kGemmMaxSplit;
     for (int s = 1; s <= smax; ++s) {
         if (s > 1 && n_tiles >= slots) break;   // already more than a wave of tiles: splitting only adds merge traffic
-        if (cluster && s > 1 && (s & (s - 1))) continue;                       // powers of two pack GPCs without strays
-        if (cluster && s > 1 && n_tiles > 8 * (32 / s)) continue;              // >= 16 SMs (32 slots) per GPC, 8 GPCs
+        if (s > 1 && (s & (s - 1))) continue;                       // powers of two pack GPCs without strays
+        if (s > 1 && n_tiles > 8 * (32 / s)) continue;              // >= 16 SMs (32 slots) per GPC, 8 GPCs
         const int kbp = (k_blocks + s - 1) / s;
         const int se = (k_blocks + kbp - 1) / kbp;
         if (se != s) continue;
@@ -209,73 +212,28 @@ void gemm_split(int n_tiles, int k_blocks, int max_split, int* nsplit, int* kb_p
     *kb_per_split = kbp;
     *nsplit = (k_blocks + kbp - 1) / kbp;
 }
-constexpr size_t kGemmSemBytes = 16384;      // [n_tiles] tile semaphores ... [last 64 bytes] grid-barrier words of a stand-alone call
+constexpr size_t kGemmSemBytes = 16384;      // persistent kernel's split-K counters: [0, 2048) tile arrivals, [2048, 4096) departures
 
-// stream-K plan of the persistent kernel: the n_tiles*k_blocks work list is cut into runs of `per` k-blocks, one per CTA
-struct SkPlan {
-    int per, used, max_contrib, aligned;
-};
-int sk_max_contrib(int n_tiles, int k_blocks, int per) {
-    int mc = 1;
-    for (int t = 0; t < n_tiles; ++t) {
-        const long a = (long)t * k_blocks, b = a + k_blocks - 1;
-        const int c = (int)(b / per - a / per) + 1;
-        if (c > mc) mc = c;
-    }
-    return mc;
-}
-// Default plan = UNIFORM split-K: the run length is the smallest divisor of k_blocks that still gives every CTA at most one
-// run (or whole tiles when there are more tiles than CTAs), so every CTA owns exactly one segment and the S = k_blocks / per
-// contributors of a tile (S a power of two) merge their partials together. B200_SK_STREAMK=1 selects ragged stream-K runs
-// (equal k-block counts per CTA, tiles finished by their lowest contributor) for experiments.
-SkPlan sk_plan(int n_tiles, int k_blocks, int grid, int bpad, size_t ws_partial_bytes) {
+// Split-K plan of the persistent kernel: the n_tiles*k_blocks work list is cut into runs of `per` k-blocks, one per CTA.
+// The run length is the smallest divisor of k_blocks that still gives every CTA at most one run (or whole tiles when there
+// are more tiles than CTAs), so every CTA owns exactly one segment and the S = k_blocks / per contributors of a tile
+// (S a power of two, at most 16, their partials within ws_partial_bytes) merge their partials together.
+int sk_plan(int n_tiles, int k_blocks, int grid, int bpad, size_t ws_partial_bytes) {
     const long total = (long)n_tiles * k_blocks;
     const size_t slot = (size_t)bpad * kGemmTileN * sizeof(float);
-    int want = (int)((total + grid - 1) / grid);
-    SkPlan p{};
-    if (!env_int("B200_SK_STREAMK", 0)) {
-        int per = 0;
-        if (want >= k_blocks) {
-            per = (want + k_blocks - 1) / k_blocks * k_blocks;          // whole tiles, possibly several per CTA
-        } else {
-            for (int d = want; d <= k_blocks; ++d) {
-                const int S = k_blocks / d;
-                if (k_blocks % d == 0 && (S & (S - 1)) == 0 && S <= 16 && (size_t)n_tiles * S * slot <= ws_partial_bytes) {
-                    per = d;
-                    break;
-                }
-            }
-            if (!per) per = k_blocks;
-        }
-        p.per = per;
-        p.used = (int)((total + per - 1) / per);
-        p.max_contrib = per >= k_blocks ? 1 : k_blocks / per;
-        p.aligned = 1;
-        return p;
+    const int want = (int)((total + grid - 1) / grid);
+    if (want >= k_blocks) return (want + k_blocks - 1) / k_blocks * k_blocks;   // whole tiles, possibly several per CTA
+    for (int d = want; d <= k_blocks; ++d) {
+        const int S = k_blocks / d;
+        if (k_blocks % d == 0 && (S & (S - 1)) == 0 && S <= 16 && (size_t)n_tiles * S * slot <= ws_partial_bytes) return d;
     }
-    int per = want;
-    const int min_run = env_int("B200_SK_MIN_RUN", 2);
-    if (per < min_run) per = min_run < k_blocks ? min_run : k_blocks;
-    int mc = sk_max_contrib(n_tiles, k_blocks, per);
-    if (mc > 1 && (size_t)n_tiles * mc * slot > ws_partial_bytes) {
-        per = (per + k_blocks - 1) / k_blocks * k_blocks;   // no room for partials: whole tiles per CTA (always valid)
-        mc = 1;
-    }
-    p.per = per;
-    p.used = (int)((total + per - 1) / per);
-    p.max_contrib = mc;
-    p.aligned = 0;
-    return p;
+    return k_blocks;
 }
+// partial slots the plan needs at this grid and batch pad; a call with a smaller grid or batch pad picks a run at least as
+// long, so it needs no more and gets the same plan from a workspace of this size
 size_t sk_ws_bytes(int n_tiles, int k_blocks, int grid, int bpad) {
-    SkPlan p = sk_plan(n_tiles, k_blocks, grid, bpad, (size_t)-1);
-    size_t need = p.max_contrib > 1 ? (size_t)n_tiles * p.max_contrib * bpad * kGemmTileN * sizeof(float) : 0;
-    // the ragged stream-K plan (developer switch) never needs more than 3 + k_blocks / per slots per tile: cover it too
-    const long total = (long)n_tiles * k_blocks;
-    int per = (int)((total + grid - 1) / grid);
-    if (per < 2) per = 2;
-    const size_t ragged = (size_t)n_tiles * (size_t)(sk_max_contrib(n_tiles, k_blocks, per < k_blocks ? per : k_blocks)) * bpad * kGemmTileN * sizeof(float);
-    return need > ragged ? need : ragged;
+    const int per = sk_plan(n_tiles, k_blocks, grid, bpad, (size_t)-1);
+    return per < k_blocks ? (size_t)n_tiles * (k_blocks / per) * bpad * kGemmTileN * sizeof(float) : 0;
 }
 
 }  // namespace
@@ -299,7 +257,6 @@ struct b200_program {
     unsigned* d_bar = nullptr;
     unsigned long long* trace = nullptr;
     bool finalized = false;
-    bool fuse = true;
 };
 
 namespace {
@@ -338,9 +295,6 @@ int rec_call(std::function<int(void*)> fn) {
     g_rec->items.push_back(std::move(it));
     return B200_OK;
 }
-// developer switch B200_PROGRAM_FUSE_MASK: bit (1 << op type) must be set for an op type to be fused (default: all)
-bool recording_fused(int op_type) { return g_rec && g_rec->fuse && ((env_int("B200_PROGRAM_FUSE_MASK", -1) >> op_type) & 1); }
-
 }  // namespace
 
 extern "C" {
@@ -373,7 +327,7 @@ int b200_plan_attn_split(int units, int max_seq_len, int* nsplit, int* tiles_per
 
 int b200_plan_gemm_split(int K, int N, int* nsplit, int* k_blocks_per_split) {
     ARG_CHECK(K > 0 && K % kGemmBK == 0 && N > 0 && nsplit && k_blocks_per_split, "plan_gemm_split: bad argument");
-    gemm_split((N + kGemmTileN - 1) / kGemmTileN, K / kGemmBK, env_int("B200_GEMM_CLUSTER", 1) ? 8 : 16, nsplit, k_blocks_per_split);
+    gemm_split((N + kGemmTileN - 1) / kGemmTileN, K / kGemmBK, nsplit, k_blocks_per_split);
     return B200_OK;
 }
 
@@ -382,7 +336,7 @@ int b200_convert_block_table(int32_t* page_list, const int32_t* block_ids, int b
     ARG_CHECK(page_list && block_ids, "convert_block_table: null pointer");
     ARG_CHECK(batch >= 0 && max_blocks >= 0, "convert_block_table: negative size");
     if (batch == 0 || max_blocks == 0) return B200_OK;
-    if (recording_fused(kOpBlockTable)) {
+    if (g_rec) {
         ProgOp op{};
         op.type = kOpBlockTable;
         op.t.page_list = page_list;
@@ -391,7 +345,6 @@ int b200_convert_block_table(int32_t* page_list, const int32_t* block_ids, int b
         op.t.max_blocks = max_blocks;
         return rec_segment_op(op, -1, -1, -1);
     }
-    if (g_rec) return rec_call([=](void* st) { return b200_convert_block_table(page_list, block_ids, batch, max_blocks, st); });
     const int total = batch * max_blocks;
     const int threads = 256, blocks = (total + threads - 1) / threads;
     convert_block_table_kernel<<<blocks < 1024 ? blocks : 1024, threads, 0, (cudaStream_t)stream>>>(page_list, block_ids,
@@ -520,7 +473,7 @@ static int attn_impl(const void* q, const void* qkv, float rope_base, int q_len,
     const size_t sem_b = round_up(batch * kv_head_num * sizeof(int), 256);
     const size_t ml_b = round_up(batch * head_num * q_len * (size_t)p.nsplit * 2 * sizeof(float), 256);
     const size_t o_b = batch * head_num * q_len * (size_t)p.nsplit * head_dim * sizeof(float);
-    if (p.nsplit > 8 || (p.nsplit > 1 && !env_int("B200_ATTN_CLUSTER", 1))) {
+    if (p.nsplit > 8) {
         ARG_CHECK(workspace && workspace_bytes >= sem_b + ml_b + o_b,
                   "paged_decode_attn: workspace too small (%zu < %zu)", workspace_bytes, sem_b + ml_b + o_b);
         p.sem = reinterpret_cast<int*>(workspace);
@@ -538,7 +491,7 @@ static int attn_impl(const void* q, const void* qkv, float rope_base, int q_len,
         if (rc) return rc;
     }
     const dim3 grid(p.nsplit, (unsigned)(batch * kv_head_num), 1);
-    p.cluster_merge = (p.nsplit >= 2 && p.nsplit <= 8 && env_int("B200_ATTN_CLUSTER", 1)) ? 1 : 0;
+    p.cluster_merge = (p.nsplit >= 2 && p.nsplit <= 8) ? 1 : 0;   // 2..8 splits merge in a cluster, more through the workspace
     static bool configured_dev[16][6] = {};
     int dev = 0;
     cudaGetDevice(&dev);
@@ -642,13 +595,9 @@ int b200_pack_w8g(const int8_t* q, const void* scales, const void* zeros_x_scale
 size_t b200_wo_gemm_workspace_bytes(int max_batch, int N, int K) {
     if (max_batch <= 0 || N <= 0 || K <= 0 || K % kGemmBK) return 0;
     const int n_tiles = (N + kGemmTileN - 1) / kGemmTileN;
-    int ns, kbp;
-    gemm_split(n_tiles, K / kGemmBK, 16, &ns, &kbp);
-    // sized for the largest split either GEMM path may pick for any batch <= max_batch
-    const int bpad = gemm_bpad(max_batch);
-    const size_t part = ns > 1 ? (size_t)ns * n_tiles * bpad * kGemmTileN * sizeof(float) : 0;
-    const size_t sk = sk_ws_bytes(n_tiles, K / kGemmBK, 2 * num_sms(), bpad);
-    return kGemmSemBytes + (part > sk ? part : sk);
+    // the cluster kernel merges split-K in distributed shared memory; only the persistent kernel's partials need room, sized
+    // for its largest grid (2 CTAs per SM) and any batch <= max_batch
+    return kGemmSemBytes + sk_ws_bytes(n_tiles, K / kGemmBK, 2 * num_sms(), gemm_bpad(max_batch));
 }
 
 namespace {
@@ -699,7 +648,7 @@ int wo_gemm_impl(int fmt, int is_bf16, const void* x, int B, int K, int N, const
     ARG_CHECK(fmt != B200_FMT_INT8 || col_scale, "wo_gemm: INT8 needs col_scale");
     ARG_CHECK((((uintptr_t)x | (uintptr_t)w | (uintptr_t)y) & 15) == 0, "wo_gemm: x / w / y must be 16-byte aligned");
     const int n_tiles = (N + kGemmTileN - 1) / kGemmTileN;
-    ARG_CHECK(n_tiles <= 2032, "wo_gemm: N=%d too large", N);   // arrivals [0, 2048) + departures [2048, 4080) + 64 bytes of barrier words
+    ARG_CHECK(n_tiles <= 2032, "wo_gemm: N=%d too large", N);   // persistent kernel: arrivals [0, 2048), departures [2048, 2048 + n_tiles)
     const int bpad = gemm_bpad(B);
     const bool silu_mul = (flags & B200_GEMM_SILU_MUL) != 0;
     ARG_CHECK(!silu_mul || N % 128 == 0, "wo_gemm: SILU_MUL needs N %% 128 == 0 (gate/up interleaved per 128-feature tile)");
@@ -714,18 +663,15 @@ int wo_gemm_impl(int fmt, int is_bf16, const void* x, int B, int K, int N, const
         if (rc) return rc;
     }
 
-    // ---- weight-only INT8 / INT4 at decode batches: inside a decode program the GEMM is an op of the persistent kernel
-    // (uniform split-K merged through L2). A stand-alone call uses the cluster kernel below (split-K merged through DSMEM):
-    // the cluster kernel has no grid-wide barrier, so it is the default outside a program;
-    // B200_GEMM_PERSISTENT=1 routes stand-alone calls through the persistent kernel too (experiments / tests).
+    // ---- weight-only INT8 / INT4 at decode batches inside a decode program: an op of the persistent kernel (uniform split-K
+    // merged through L2). Every other GEMM, and every call outside a program, uses the cluster kernel below (split-K merged
+    // through DSMEM), which needs no grid-wide barrier.
     const bool seg_capable = (fmt == B200_FMT_INT8 || fmt == B200_FMT_INT4) && bpad <= 64;   // INT8G / FP16: cluster kernel only
-    const bool streamk = seg_capable && !rs && (recording_fused(kOpGemm) || env_int("B200_GEMM_PERSISTENT", 0));
-    if (streamk) {
+    if (g_rec && seg_capable && !rs) {
         ARG_CHECK(workspace && workspace_bytes >= kGemmSemBytes, "wo_gemm: workspace of at least %zu bytes required", kGemmSemBytes);
         int grid = 0;
         int rc = segment_grid(is_bf16 != 0, bpad, fmt, &grid);
         if (rc) return rc;
-        const SkPlan plan = sk_plan(n_tiles, K / kGemmBK, grid, bpad, workspace_bytes - kGemmSemBytes);
         ProgOp op{};
         op.xmap = xmap;
         op.type = kOpGemm;
@@ -741,20 +687,11 @@ int wo_gemm_impl(int fmt, int is_bf16, const void* x, int B, int K, int N, const
         g.k_blocks = K / kGemmBK;
         g.n_tiles = n_tiles;
         g.total_kb = n_tiles * g.k_blocks;
-        g.per_cta = plan.per;
-        g.max_contrib = plan.max_contrib;
-        g.aligned = plan.aligned;
+        g.per_cta = sk_plan(n_tiles, g.k_blocks, grid, bpad, workspace_bytes - kGemmSemBytes);
         g.sem = reinterpret_cast<int*>(workspace);
         g.ws = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + kGemmSemBytes);
         g.silu_mul = silu_mul ? 1 : 0;
-        if (recording_fused(kOpGemm)) return rec_segment_op(op, is_bf16 ? 1 : 0, bpad, fmt);
-        if (g_rec)
-            return rec_call([=](void* st) {
-                return b200_wo_gemm(fmt, is_bf16, x, B, K, N, w, col_scale, bias, y, workspace, workspace_bytes, flags, st);
-            });
-        unsigned* gbar = reinterpret_cast<unsigned*>(reinterpret_cast<uint8_t*>(workspace) + kGemmSemBytes - 64);
-        return launch_segment(is_bf16 != 0, bpad, fmt, &op, nullptr, 1, gbar, plan.used < grid ? plan.used : grid, use_pdl,
-                              nullptr, (cudaStream_t)stream);
+        return rec_segment_op(op, is_bf16 ? 1 : 0, bpad, fmt);
     }
     if (g_rec) {
         if (rs) {
@@ -768,7 +705,7 @@ int wo_gemm_impl(int fmt, int is_bf16, const void* x, int B, int K, int N, const
         });
     }
 
-    // ---- FP16 weights / batches above 64: one kernel per GEMM, cluster split-K (gemm_cluster.cu)
+    // ---- one kernel per GEMM, cluster split-K (gemm_cluster.cu)
     GemmParams p{};
     p.w_blob = reinterpret_cast<const uint8_t*>(w);
     p.col_scale = col_scale;
@@ -780,34 +717,7 @@ int wo_gemm_impl(int fmt, int is_bf16, const void* x, int B, int K, int N, const
     p.k_blocks = K / kGemmBK;
     p.use_pdl = use_pdl ? 1 : 0;
     p.silu_mul = silu_mul ? 1 : 0;
-#ifdef B200_GEMM_DEV
-    {
-        const char* tr = getenv("B200_GEMM_TRACE_PTR");   // developer timeline buffer (device pointer)
-        p.trace = (tr && *tr) ? reinterpret_cast<long long*>(strtoull(tr, nullptr, 0)) : nullptr;
-    }
-#endif
-    p.cluster_reduce = (rs || env_int("B200_GEMM_CLUSTER", 1)) ? 1 : 0;   // split-K merge through DSMEM (cluster <= 8) vs global semaphores
-
-    gemm_split(n_tiles, p.k_blocks, p.cluster_reduce ? 8 : 16, &p.nsplit, &p.kb_per_split);
-    if (p.silu_mul && !p.cluster_reduce) {
-        p.nsplit = 1;   // the fused activation is implemented for the direct and the cluster-merge epilogues
-        p.kb_per_split = p.k_blocks;
-    }
-    if (p.nsplit > 1 && !p.cluster_reduce) {
-        const size_t tile_bytes = (size_t)n_tiles * bpad * kGemmTileN * sizeof(float);
-        if (!workspace || workspace_bytes < kGemmSemBytes + tile_bytes * 2) {
-            p.nsplit = 1;  // no room for partials: fall back to one CTA per n-tile (still correct, just less parallel)
-            p.kb_per_split = p.k_blocks;
-        } else {
-            const size_t fit = (workspace_bytes - kGemmSemBytes) / tile_bytes;
-            if ((size_t)p.nsplit > fit) {
-                p.kb_per_split = (p.k_blocks + (int)fit - 1) / (int)fit;
-                p.nsplit = (p.k_blocks + p.kb_per_split - 1) / p.kb_per_split;
-            }
-            p.sem = reinterpret_cast<int*>(workspace);
-            p.ws = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + kGemmSemBytes);
-        }
-    }
+    gemm_split(n_tiles, p.k_blocks, &p.nsplit, &p.kb_per_split);
     CUtensorMap wmap;
     if (fmt == B200_FMT_F16) {
         const cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)N};
@@ -842,7 +752,7 @@ int b200_add_rmsnorm(const void* x, void* residual, const void* gamma, void* y, 
     if (rows == 0) return B200_OK;
     ARG_CHECK(x && gamma && y, "add_rmsnorm: null pointer");
     ARG_CHECK(hidden > 0 && hidden % 8 == 0 && hidden <= 12288, "add_rmsnorm: hidden=%d must be a multiple of 8, <= 12288", hidden);
-    if (recording_fused(kOpNorm) && hidden <= kSegNormMaxHidden) {
+    if (g_rec && hidden <= kSegNormMaxHidden) {
         ProgOp op{};
         op.type = kOpNorm;
         op.n.x = x;
@@ -919,7 +829,7 @@ int b200_rope_append(const void* qkv, void* q_out, void* kv_pool, const int32_t*
     ARG_CHECK(head_dim > 0 && head_dim % 2 == 0 && head_dim <= 512, "rope_append: head_dim %d unsupported", head_dim);
     ARG_CHECK(rope_base > 1.f, "rope_append: rope_base must be > 1");
     const float l2b = std::log2(rope_base);
-    if (recording_fused(kOpRope)) {
+    if (g_rec) {
         ProgOp op{};
         op.type = kOpRope;
         op.r.qkv = qkv;
@@ -936,11 +846,6 @@ int b200_rope_append(const void* qkv, void* q_out, void* kv_pool, const int32_t*
         op.r.log2_base = l2b;
         return rec_segment_op(op, is_bf16 ? 1 : 0, -1, -1);
     }
-    if (g_rec)
-        return rec_call([=](void* st) {
-            return b200_rope_append(qkv, q_out, kv_pool, page_list, sequence_lengths, is_bf16, batch, head_num, kv_head_num,
-                                    head_dim, max_blocks_per_seq, page_size, rope_base, st);
-        });
     const dim3 grid(batch, head_num + 2 * kv_head_num);
     const bool pdl = g_pdl.load() != 0;
     if (is_bf16)
@@ -995,7 +900,7 @@ int b200_embedding(const int32_t* ids, const void* table, void* out, int is_bf16
     if (rows == 0) return B200_OK;
     ARG_CHECK(ids && table && out, "embedding: null pointer");
     ARG_CHECK(hidden > 0 && hidden % 8 == 0, "embedding: hidden=%d must be a multiple of 8", hidden);
-    if (recording_fused(kOpEmbed)) {
+    if (g_rec) {
         ProgOp op{};
         op.type = kOpEmbed;
         op.e.ids = ids;
@@ -1005,7 +910,6 @@ int b200_embedding(const int32_t* ids, const void* table, void* out, int is_bf16
         op.e.hidden = hidden;
         return rec_segment_op(op, -1, -1, -1);
     }
-    if (g_rec) return rec_call([=](void* st) { return b200_embedding(ids, table, out, is_bf16, rows, hidden, st); });
     embedding_kernel<__half><<<rows, 128, 0, (cudaStream_t)stream>>>(ids, (const __half*)table, (__half*)out, hidden);
     return launched("embedding_kernel");
 }
@@ -1132,7 +1036,6 @@ int b200_peer_allreduce(const void* in, void* out, size_t bytes, int is_bf16, vo
     p.n16 = (int)(bytes / 16);
     int ctas = (p.n16 + 2 * kArThreads - 1) / (2 * kArThreads);   // ~2 chunks (32 B of payload) per thread
     if (ctas < 1) ctas = 1;
-    ctas = env_int("B200_AR_CTAS", ctas);
     if (ctas > kArMaxCtas) ctas = kArMaxCtas;
     const bool pdl = g_pdl.load() != 0;
     // W >= 3: reduce-scatter + all-gather (2 hops, (W-1)/W of the volume twice); W == 2: one hop. Env override for tests.
@@ -1140,8 +1043,6 @@ int b200_peer_allreduce(const void* in, void* out, size_t bytes, int is_bf16, vo
     if (two_shot) {
         int c2 = (p.n16 / world + kArThreads - 1) / kArThreads;
         if (c2 < 1) c2 = 1;
-        if (c2 > kArMaxCtas) c2 = kArMaxCtas;
-        c2 = env_int("B200_AR_CTAS", c2);
         if (c2 > kArMaxCtas) c2 = kArMaxCtas;
         if (is_bf16)
             CUDA_CHECK(launch_ex(peer_allreduce_twoshot_kernel<__nv_bfloat16>, dim3(c2), dim3(kArThreads), 0, (cudaStream_t)stream, pdl, p));
@@ -1235,7 +1136,6 @@ int b200_peer_argmax(const void* logits, int is_bf16, int rows, int vocab_local,
 int b200_program_create(b200_program** out) {
     ARG_CHECK(out, "program_create: null pointer");
     *out = new b200_program();
-    (*out)->fuse = env_int("B200_PROGRAM_FUSE", 1) != 0;
     return B200_OK;
 }
 
@@ -1286,8 +1186,7 @@ int b200_program_launch(b200_program* p, void* stream) {
             unsigned long long* tr = p->trace ? p->trace + (size_t)it.first * grid * 2 : nullptr;
             // fine timeline (CTA 0): after the coarse region, [op][kFtSlots][kFtBlocks]
             g_ftrace_next = p->trace ? p->trace + p->ops.size() * (size_t)grid * 2 + (size_t)it.first * kFtSlots * kFtBlocks : nullptr;
-            rc = launch_segment(bf16, bpad, qfmt, nullptr, p->d_ops + it.first, it.count, p->d_bar + i * 64, grid, pdl, tr,
-                                (cudaStream_t)stream);
+            rc = launch_segment(bf16, bpad, qfmt, p->d_ops + it.first, it.count, p->d_bar + i * 64, grid, pdl, tr, (cudaStream_t)stream);
             g_ftrace_next = nullptr;
         } else {
             rc = it.fn(stream);

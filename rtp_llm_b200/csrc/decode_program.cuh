@@ -5,9 +5,11 @@
 // Why: a stand-alone weight-only GEMM pays a fixed cost of several microseconds (launch gap, barrier init, pipeline fill,
 // epilogue, tail) around a main loop of comparable length, and the glue kernels pay a launch each for ~0 bytes.  Here
 //   * barrier init happens once per launch, not once per op;
-//   * every weight-only GEMM is split stream-K: the (n-tile, k-block) work list is cut into equal runs, one per CTA, so all
-//     2*SMs CTAs stream the same number of weight bytes whatever the tile count is; a tile that spans CTAs is finished by
-//     its lowest contributor from the others' fp32 partials in L2 (fixed summation order -> deterministic);
+//   * every weight-only GEMM is split uniformly along k: the (n-tile, k-block) work list is cut into equal runs, one per
+//     CTA, whose length divides k_blocks (or is a whole number of tiles when there are more tiles than CTAs), so the CTAs
+//     stream about the same number of weight bytes whatever the tile count is. A tile is then either one CTA's alone, or
+//     split among S CTAs (S a power of two) that each own one whole segment of it: they publish their fp32 partials to L2
+//     and each reduces 1/S of the tile in fixed order (deterministic);
 //   * the three warp roles run as three independent loops over the op list.  The weight producer depends on nothing but its
 //     ring slots, so it streams the NEXT GEMM's weights while the other warps are still in this op's epilogue, in a glue
 //     op, or waiting at the grid barrier.
@@ -40,11 +42,8 @@ struct SkGemmParams {
     int B, N, K;
     int k_blocks, n_tiles;
     int total_kb;            // n_tiles * k_blocks
-    int per_cta;             // k-blocks per CTA (stream-K run length)
-    int max_contrib;         // upper bound of CTAs contributing to one tile (sizes the partial slots)
-    int aligned;             // 1: per_cta divides k_blocks -> every CTA owns exactly one segment and the S = k_blocks / per_cta
-                             //    contributors of a tile merge their partials TOGETHER (each reduces 1/S of the tile)
-    float* ws;               // [n_tiles][max_contrib][bpad/4][128][4] fp32 partials
+    int per_cta;             // k-blocks per CTA (run length): divides k_blocks, or is a multiple of it
+    float* ws;               // [n_tiles][S = k_blocks / per_cta][bpad/4][128][4] fp32 partials (per_cta < k_blocks)
     int* sem;                // [n_tiles] arrivals, [2048 + n_tiles] departures; zero on entry / exit
     int silu_mul;            // 1: tile rows 2i / 2i+1 hold gate / up feature tile*64+i; y[b][tile*64+i] = silu(g)*u
 };
@@ -168,7 +167,7 @@ struct SegSmem {
     static_assert(MISC + 16 + 4 * kSegDqWarps <= C::SMEM - 1024, "barrier area overflow");
 };
 
-// stream-K run of this CTA for a GEMM op: global k-block range [g0, g1)
+// run of this CTA for a GEMM op: global k-block range [g0, g1)
 __device__ __forceinline__ void sk_range(const SkGemmParams& g, int cta, int& g0, int& g1) {
     const long long a = (long long)cta * g.per_cta;
     g0 = a < g.total_kb ? (int)a : g.total_kb;
@@ -200,13 +199,13 @@ __device__ __forceinline__ void seg_w_producer(const ProgOp* op, const SegSmem<F
 // ------------------------------------------------------------------------------------------------ role: activation producer
 template <int FMT, int BPAD>
 __device__ __forceinline__ void seg_x_producer(const ProgOp* op, const SegSmem<FMT, BPAD>& sm, uint32_t& cx, const unsigned* gbar,
-                                               unsigned target, bool from_gmem, unsigned long long* ft) {
+                                               unsigned target, unsigned long long* ft) {
     using C = SegCfg<FMT, BPAD>;
     int g0, g1;
     sk_range(op->g, blockIdx.x, g0, g1);
     const int k_blocks = op->g.k_blocks;
     if (g1 > g0 && elect_one()) {
-        if (from_gmem) tensormap_acquire(&op->xmap);
+        tensormap_acquire(&op->xmap);
         grid_wait(gbar, target);          // the activations come from the previous op
         fence_proxy_async_all();          // ... written with generic stores, read here through the async proxy
         uint32_t i = cx;
@@ -275,7 +274,7 @@ __device__ __forceinline__ void seg_dq(const ProgOp* op, const SegSmem<FMT, BPAD
         }
 
         // ---- epilogue of the segment [k, e) of `tile`
-        // contributors of this tile = the CTAs whose stream-K run intersects [tile_beg, tile_end)
+        // contributors of this tile = the CTAs whose run intersects [tile_beg, tile_end)
         const int first = tile_beg / g.per_cta, last = (tile_end - 1) / g.per_cta;
         const int nact = last - first + 1, my_idx = (int)blockIdx.x - first;
         // per-feature scale / bias are indexed by the PACKED column (with silu_mul the caller interleaves them like the weight)
@@ -304,12 +303,12 @@ __device__ __forceinline__ void seg_dq(const ProgOp* op, const SegSmem<FMT, BPAD
         if (threadIdx.x == 0) B200_FT(ft, 7, 2 * (int)(cs & 7));
         // partial slot layout [bpad/4][128 rows][4]: a float2 of this thread = batch columns b, b+1 (b even) of one row
         constexpr size_t SLOT4 = (size_t)(BPAD / 4) * kGemmTileN;
-        float4* part0 = reinterpret_cast<float4*>(g.ws) + (size_t)tile * g.max_contrib * SLOT4;
+        float4* part0 = reinterpret_cast<float4*>(g.ws) + (size_t)tile * nact * SLOT4;
         auto part2 = [&](int c, int h, int b) {
             return reinterpret_cast<float2*>(reinterpret_cast<float*>(part0 + (size_t)c * SLOT4 + (size_t)(b >> 2) * kGemmTileN + rows[h]) + (b & 3));
         };
-        if (g.aligned && nact > 1) {
-            // ---- uniform split-K (every CTA of this op owns exactly one segment): the S contributors of the tile publish
+        if (nact > 1) {
+            // ---- split tile (every CTA of this op owns exactly one segment): the S contributors of the tile publish
             // their fp32 partials to L2, wait for each other, and EACH reduces 1/S of the tile in fixed order 0..S-1
             // (deterministic) -- S float4 loads in flight per thread, one round trip, instead of one CTA loading S partials.
             constexpr int ITEMS = (BPAD / 4) * kGemmTileN;       // (4 batch columns) x (feature row) units of the tile
@@ -381,46 +380,15 @@ __device__ __forceinline__ void seg_dq(const ProgOp* op, const SegSmem<FMT, BPAD
                 }
             }
         } else {
-        // Stream-K fix-up with a DESIGNATED reducer: contributor 0 (the lowest CTA; the tile is the LAST segment of its run, so
-        // it finishes the tile last in time) keeps its partial in registers, waits until the other contributors have
-        // published theirs, adds them in fixed order 1..nact-1 (deterministic) and stores the result. The others store
-        // their fp32 partial to L2, signal once (fire-and-forget) and move on -- nobody but the reducer ever waits.
-        if (nact > 1 && my_idx == 0) {
-            // wait for the nact-1 published partials (lane 0 of every warp polls; no CTA barrier on this path)
-            if (lane == 0) spin_until_ge(reinterpret_cast<const unsigned*>(g.sem) + tile, (unsigned)(nact - 1));
-            __syncwarp();
-        }
+            // ---- the tile is this CTA's alone: store straight from the accumulators
 #pragma unroll
-        for (int q = 0; q < BPAD / 8; ++q)
+            for (int q = 0; q < BPAD / 8; ++q)
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int b = 8 * q + 2 * t4;
-                float v0 = acc[4 * q + 2 * h], v1 = acc[4 * q + 2 * h + 1];
-                if (nact > 1 && my_idx != 0) {
-                    __stcg(part2(my_idx, h, b), make_float2(v0, v1));
-                    continue;
+                for (int h = 0; h < 2; ++h) {
+                    const int b = 8 * q + 2 * t4;
+                    final_store(h, b, acc[4 * q + 2 * h]);
+                    final_store(h, b + 1, acc[4 * q + 2 * h + 1]);
                 }
-                for (int c = 1; c < nact; ++c) {
-                    const float2 u = __ldcg(part2(c, h, b));
-                    v0 += u.x;
-                    v1 += u.y;
-                }
-                final_store(h, b, v0);
-                final_store(h, b + 1, v1);
-            }
-        if (nact > 1) {
-            // all dq threads' partial stores (or the reducer's polls) are done once they pass this barrier; thread 0's
-            // gpu-scope fence is cumulative over what the barrier ordered before it
-            asm volatile("bar.sync 1, %0;" ::"n"(kSegDqThreads) : "memory");
-            if (threadIdx.x == 0) {
-                if (my_idx == 0) {
-                    g.sem[tile] = 0;                    // self-reset: every contribution has been consumed
-                } else {
-                    __threadfence();
-                    atomicAdd(&g.sem[tile], 1);         // result unused -> RED, no round trip on the critical path
-                }
-            }
-        }
         }
         if (threadIdx.x == 0) B200_FT(ft, 7, 16 + (int)(cs & 7));
         ++cs;
@@ -561,8 +529,8 @@ __device__ __forceinline__ void seg_block_table(const BlockTableParams& p, int c
 // trace (developer, may be null): [op][cta][2] globaltimer at op entry / op exit of the dq role.
 template <typename T, int BPAD, int QFMT>
 __global__ void __launch_bounds__(kSegThreads, 2)
-decode_segment_kernel(const __grid_constant__ ProgOp op0, const ProgOp* __restrict__ ops, int nops, unsigned* gbar, int use_pdl,
-                      unsigned long long* trace, unsigned long long* ftrace) {
+decode_segment_kernel(const ProgOp* __restrict__ ops, int nops, unsigned* gbar, int use_pdl, unsigned long long* trace,
+                      unsigned long long* ftrace) {
     using C = SegCfg<QFMT, BPAD>;
     extern __shared__ __align__(1024) uint8_t smem[];
     if (threadIdx.x == 0 && (smem_u32(smem) & 1023u)) __trap();
@@ -589,7 +557,7 @@ decode_segment_kernel(const __grid_constant__ ProgOp op0, const ProgOp* __restri
         // ---- weight producer: depends on nothing but ring slots -> runs ahead of every other role, across op boundaries
         uint32_t cw = 0;
         for (int i = 0; i < nops; ++i) {
-            const ProgOp* op = ops ? &ops[i] : &op0;
+            const ProgOp* op = &ops[i];
             if (op->type == kOpGemm) seg_w_producer<QFMT, BPAD>(op, sm, cw, ftrace ? ftrace + (size_t)i * kFtSlots * kFtBlocks : nullptr);
         }
     } else if (warp == kSegDqWarps + 1) {
@@ -597,15 +565,15 @@ decode_segment_kernel(const __grid_constant__ ProgOp op0, const ProgOp* __restri
         if (use_pdl) pdl_wait();
         uint32_t cx = 0;
         for (int i = 0; i < nops; ++i) {
-            const ProgOp* op = ops ? &ops[i] : &op0;
-            if (op->type == kOpGemm) seg_x_producer<QFMT, BPAD>(op, sm, cx, gbar, (unsigned)i * G, ops != nullptr, ftrace ? ftrace + (size_t)i * kFtSlots * kFtBlocks : nullptr);
+            const ProgOp* op = &ops[i];
+            if (op->type == kOpGemm) seg_x_producer<QFMT, BPAD>(op, sm, cx, gbar, (unsigned)i * G, ftrace ? ftrace + (size_t)i * kFtSlots * kFtBlocks : nullptr);
         }
     } else {
         // ---- dequant / epilogue / glue warps: the role that owns the grid barrier
         if (use_pdl) pdl_wait();
         uint32_t cb = 0, cs = 0;
         for (int i = 0; i < nops; ++i) {
-            const ProgOp* op = ops ? &ops[i] : &op0;
+            const ProgOp* op = &ops[i];
             if (trace && threadIdx.x == 0) {
                 unsigned long long gt;
                 asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));

@@ -16,7 +16,7 @@ using ParamsT = typename GemmParamsOf<B200_GEMM_VAR>::type;
 template <int FMT, typename T, int BPAD>
 int launch_one(const CUtensorMap& xmap, const CUtensorMap& wmap, const ParamsT& p, int n_tiles, cudaStream_t st) {
     auto kern = wo_gemm_kernel<FMT, T, BPAD, B200_GEMM_VAR>;
-    constexpr int smem = gemm_smem_bytes(FMT, BPAD, B200_GEMM_VAR);
+    constexpr int smem = gemm_smem_bytes(FMT, BPAD);
     static bool configured[16] = {};
     int dev = 0;
     cudaGetDevice(&dev);
@@ -27,7 +27,7 @@ int launch_one(const CUtensorMap& xmap, const CUtensorMap& wmap, const ParamsT& 
     }
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(n_tiles, p.nsplit, 1);
-    cfg.blockDim = dim3(gemm_threads(B200_GEMM_VAR), 1, 1);
+    cfg.blockDim = dim3(gemm_threads(), 1, 1);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = st;
     cudaLaunchAttribute attr[2];
@@ -37,7 +37,7 @@ int launch_one(const CUtensorMap& xmap, const CUtensorMap& wmap, const ParamsT& 
         attr[na].val.programmaticStreamSerializationAllowed = 1;
         ++na;
     }
-    if (p.nsplit > 1 && p.cluster_reduce) {
+    if (p.nsplit > 1) {
         attr[na].id = cudaLaunchAttributeClusterDimension;
         attr[na].val.clusterDim.x = 1;
         attr[na].val.clusterDim.y = (unsigned)p.nsplit;

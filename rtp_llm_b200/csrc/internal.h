@@ -41,10 +41,10 @@ int launch_cluster_gemm(int fmt, bool bf16, int bpad, const CUtensorMap& xmap, c
 int launch_cluster_gemm_rs(int fmt, bool bf16, int bpad, const CUtensorMap& xmap, const CUtensorMap& wmap,
                            const b200::GemmParamsRs& p, int n_tiles, cudaStream_t st);
 
-// segment_*.cu: the persistent stream-K kernel (csrc/decode_program.cuh). qfmt: B200_FMT_INT8 / B200_FMT_INT4.
+// segment_*.cu: the persistent decode-program kernel (csrc/decode_program.cuh). qfmt: B200_FMT_INT8 / B200_FMT_INT4.
 // grid == 0 asks for the co-resident grid size only (written to *grid_out).
 int segment_grid(bool bf16, int bpad, int qfmt, int* grid_out);
-int launch_segment(bool bf16, int bpad, int qfmt, const b200::ProgOp* op0, const b200::ProgOp* d_ops, int nops,
-                   unsigned* gbar, int grid, bool pdl, unsigned long long* trace, cudaStream_t st);
+int launch_segment(bool bf16, int bpad, int qfmt, const b200::ProgOp* d_ops, int nops, unsigned* gbar, int grid, bool pdl,
+                   unsigned long long* trace, cudaStream_t st);
 
 }  // namespace b200_host

@@ -9,8 +9,8 @@ using namespace b200_host;
 namespace {
 
 template <typename T, int BPAD, int QFMT>
-int seg_one(const ProgOp* op0, const ProgOp* d_ops, int nops, unsigned* gbar, int grid, bool pdl, unsigned long long* trace,
-            cudaStream_t st, int* grid_out) {
+int seg_one(const ProgOp* d_ops, int nops, unsigned* gbar, int grid, bool pdl, unsigned long long* trace, cudaStream_t st,
+            int* grid_out) {
     unsigned long long* ftrace = g_ftrace_next;   // developer fine timeline of the next launch (b200_program_set_trace)
     auto kern = decode_segment_kernel<T, BPAD, QFMT>;
     constexpr int smem = SegCfg<QFMT, BPAD>::SMEM;
@@ -32,9 +32,6 @@ int seg_one(const ProgOp* op0, const ProgOp* d_ops, int nops, unsigned* gbar, in
         // the two CTAs per SM the kernel is built for (__launch_bounds__(320, 2), 2 x (SMEM + 1 KB) <= 227 KB of the SM's 228 KB).
         static_assert(2 * (smem + 1024) <= 227 * 1024, "two CTAs per SM must fit");
         max_grid[dev] = (occ < 2 ? occ : 2) * sms;
-        const int forced = env_int("B200_SEG_GRID", 0);   // developer override, never beyond the co-resident grid
-        if (forced > 0 && forced < max_grid[dev]) max_grid[dev] = forced;
-        if (env_int("B200_DEBUG", 0)) fprintf(stderr, "[b200] decode_segment_kernel<bpad %d, fmt %d>: occupancy %d CTAs/SM, grid %d\n", BPAD, QFMT, occ, max_grid[dev]);
         configured[dev] = true;
     }
     if (grid_out) *grid_out = max_grid[dev];
@@ -50,27 +47,26 @@ int seg_one(const ProgOp* op0, const ProgOp* d_ops, int nops, unsigned* gbar, in
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = pdl ? 1 : 0;
-    static const ProgOp dummy{};
-    CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, op0 ? *op0 : dummy, d_ops, nops, gbar, pdl ? 1 : 0, trace, ftrace));
+    CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, d_ops, nops, gbar, pdl ? 1 : 0, trace, ftrace));
     return launched("decode_segment_kernel");
 }
 
 template <typename T, int QFMT>
-int seg_by_bpad(int bpad, const ProgOp* op0, const ProgOp* d_ops, int nops, unsigned* gbar, int grid, bool pdl,
+int seg_by_bpad(int bpad, const ProgOp* d_ops, int nops, unsigned* gbar, int grid, bool pdl,
                 unsigned long long* trace, cudaStream_t st, int* grid_out) {
     switch (bpad) {
-        case 16: return seg_one<T, 16, QFMT>(op0, d_ops, nops, gbar, grid, pdl, trace, st, grid_out);
-        case 32: return seg_one<T, 32, QFMT>(op0, d_ops, nops, gbar, grid, pdl, trace, st, grid_out);
-        case 64: return seg_one<T, 64, QFMT>(op0, d_ops, nops, gbar, grid, pdl, trace, st, grid_out);
+        case 16: return seg_one<T, 16, QFMT>(d_ops, nops, gbar, grid, pdl, trace, st, grid_out);
+        case 32: return seg_one<T, 32, QFMT>(d_ops, nops, gbar, grid, pdl, trace, st, grid_out);
+        case 64: return seg_one<T, 64, QFMT>(d_ops, nops, gbar, grid, pdl, trace, st, grid_out);
         default: return fail(B200_EINVAL, "segment kernel: batch pad %d unsupported (16/32/64)", bpad);
     }
 }
 
 template <typename T>
-int seg_dispatch(int bpad, int qfmt, const ProgOp* op0, const ProgOp* d_ops, int nops, unsigned* gbar, int grid, bool pdl,
+int seg_dispatch(int bpad, int qfmt, const ProgOp* d_ops, int nops, unsigned* gbar, int grid, bool pdl,
                  unsigned long long* trace, cudaStream_t st, int* grid_out) {
-    if (qfmt == B200_FMT_INT8) return seg_by_bpad<T, kFmtInt8>(bpad, op0, d_ops, nops, gbar, grid, pdl, trace, st, grid_out);
-    if (qfmt == B200_FMT_INT4) return seg_by_bpad<T, kFmtInt4>(bpad, op0, d_ops, nops, gbar, grid, pdl, trace, st, grid_out);
+    if (qfmt == B200_FMT_INT8) return seg_by_bpad<T, kFmtInt8>(bpad, d_ops, nops, gbar, grid, pdl, trace, st, grid_out);
+    if (qfmt == B200_FMT_INT4) return seg_by_bpad<T, kFmtInt4>(bpad, d_ops, nops, gbar, grid, pdl, trace, st, grid_out);
     return fail(B200_EINVAL, "segment kernel: weight format %d unsupported (INT8 / INT4)", qfmt);
 }
 

@@ -41,29 +41,25 @@ __host__ __device__ constexpr int gemm_w_bytes(int fmt) {
 // released as soon as the dequant warps hold its nibbles in registers, so its lifetime is one TMA latency, not the
 // whole dequant -> MMA chain, and the bytes in flight per SM (Little's law: bandwidth per SM * latency) stay high.
 // 8 dequant warps = two warpgroups, each the MMA issuer of its 64 feature rows (see the dequant section of the kernel).
-__host__ __device__ constexpr int gemm_ndq_warps(int var) { (void)var; return 8; }
-__host__ __device__ constexpr int gemm_threads(int var) { return (gemm_ndq_warps(var) + 2) * 32; }
+__host__ __device__ constexpr int gemm_ndq_warps() { return 8; }
+__host__ __device__ constexpr int gemm_threads() { return (gemm_ndq_warps() + 2) * 32; }
 __host__ __device__ constexpr int gemm_x_stage_bytes(int bpad) { return bpad * 256; }
-#ifndef B200_GEMM_XS
-#define B200_GEMM_XS 4
-#endif
-__host__ __device__ constexpr int gemm_x_stages(int bpad) { return bpad <= 32 ? B200_GEMM_XS : 3; }
+__host__ __device__ constexpr int gemm_x_stages(int bpad) { return bpad <= 32 ? 4 : 3; }
 constexpr int kGemmSmemMisc = 1024 /*align*/ + 1024 /*barriers*/;
 __host__ __device__ constexpr int gemm_w_stages_for(int fmt, int bpad, int budget) {
     int n = (budget - kGemmSmemMisc - gemm_x_stages(bpad) * gemm_x_stage_bytes(bpad)) / gemm_w_bytes(fmt);
     return n > 12 ? 12 : n;
 }
 // two CTAs per SM when at least 4 weight stages fit in half an SM's shared memory
-__host__ __device__ constexpr int gemm_min_ctas(int fmt, int bpad, int var) {
-    (void)var;
+__host__ __device__ constexpr int gemm_min_ctas(int fmt, int bpad) {
     return gemm_w_stages_for(fmt, bpad, 106 * 1024) >= 4 ? 2 : 1;
 }
-__host__ __device__ constexpr int gemm_w_stages(int fmt, int bpad, int var) {
-    return gemm_min_ctas(fmt, bpad, var) == 2 ? gemm_w_stages_for(fmt, bpad, 106 * 1024)
-                                              : gemm_w_stages_for(fmt, bpad, 216 * 1024);
+__host__ __device__ constexpr int gemm_w_stages(int fmt, int bpad) {
+    return gemm_min_ctas(fmt, bpad) == 2 ? gemm_w_stages_for(fmt, bpad, 106 * 1024)
+                                         : gemm_w_stages_for(fmt, bpad, 216 * 1024);
 }
-__host__ __device__ constexpr int gemm_smem_bytes(int fmt, int bpad, int var) {
-    return gemm_x_stages(bpad) * gemm_x_stage_bytes(bpad) + gemm_w_stages(fmt, bpad, var) * gemm_w_bytes(fmt) + kGemmSmemMisc;
+__host__ __device__ constexpr int gemm_smem_bytes(int fmt, int bpad) {
+    return gemm_x_stages(bpad) * gemm_x_stage_bytes(bpad) + gemm_w_stages(fmt, bpad) * gemm_w_bytes(fmt) + kGemmSmemMisc;
 }
 
 // Row-parallel GEMM under tensor parallelism (b200_wo_gemm_rs): the epilogue pushes every output element that another rank
@@ -84,13 +80,9 @@ struct GemmParams {
     void* y;                 // [B][N] (T)
     int B, N, K;
     int k_blocks;            // K / 128
-    int kb_per_split, nsplit;
-    float* ws;               // [nsplit][n_tiles][bpad][128] fp32 split-K partials
-    int* sem;                // [n_tiles], zero on entry / exit
+    int kb_per_split, nsplit;   // nsplit > 1: the nsplit CTAs of a tile form a cluster (1,nsplit,1) and merge through DSMEM
     int use_pdl;
     int silu_mul;            // 1: tile rows 2r / 2r+1 are gate / up feature tile*64+r; y[b][tile*64+r] = silu(g)*u
-    int cluster_reduce;      // 1: the nsplit CTAs of a tile form a cluster (1,nsplit,1) and merge through DSMEM
-    long long* trace;        // developer timeline (tools/gemm_trace.py); null in production
 };
 
 // The VAR == 1 kernels (gemm_cluster_rs.cu) take the descriptor of the reduce-scatter push after the common parameters; the
@@ -231,19 +223,6 @@ struct Pair<__nv_bfloat16> {
     }
 };
 
-// developer timeline (only in -DB200_GEMM_DEV builds, see tools/gemm_trace.py): TRACE(slot, it) stores clock64() for CTA
-// (0,0); slots: 0 w-issue, 1 x-issue, 2 dq wfull seen, 3 dq math done, 6 mma operands ready, 7 mma complete
-#ifdef B200_GEMM_DEV
-#define B200_TRACE(slot, it)                                                                     \
-    do {                                                                                         \
-        if (p.trace && blockIdx.x == 0 && blockIdx.y == 0 && (it) < 64) p.trace[(slot) * 64 + (it)] = clock64(); \
-    } while (0)
-#define B200_TRACING (p.trace != nullptr)
-#else
-#define B200_TRACE(slot, it) do { } while (0)
-#define B200_TRACING false
-#endif
-
 // The weight block of one (n-tile, k-block) as wgmma A fragments (ptx.cuh): dequant warp R = 0..7 (two warpgroups) owns
 // feature rows 16R..16R+15 of the 128-feature tile, a[j] is its fragment of k16-step j. The pack kernels below lay every
 // thread's bytes of a block out as consecutive 16-byte vectors (one conflict-free LDS.128 per warp and vector):
@@ -303,12 +282,12 @@ __device__ __forceinline__ void load_w_frag(uint32_t wb, int R, int lane, uint32
 }
 
 template <int FMT, typename T, int BPAD, int VAR>
-__global__ void __launch_bounds__(gemm_threads(VAR), gemm_min_ctas(FMT, BPAD, VAR))
+__global__ void __launch_bounds__(gemm_threads(), gemm_min_ctas(FMT, BPAD))
 wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant__ CUtensorMap w_map,
                const typename GemmParamsOf<VAR>::type p) {
-    constexpr int WS = gemm_w_stages(FMT, BPAD, VAR);      // weight ring depth
+    constexpr int WS = gemm_w_stages(FMT, BPAD);           // weight ring depth
     constexpr int XS = gemm_x_stages(BPAD);                // activation ring depth
-    constexpr int NDQ_WARPS = gemm_ndq_warps(VAR);
+    constexpr int NDQ_WARPS = gemm_ndq_warps();
     constexpr int NDQ_THREADS = NDQ_WARPS * 32;
     constexpr int W_WTMA = NDQ_WARPS, W_XTMA = NDQ_WARPS + 1;
     constexpr int X_BYTES = gemm_x_stage_bytes(BPAD);
@@ -327,15 +306,9 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
     uint64_t* wempty = wfull + WS;
     uint64_t* xfull = wempty + WS;
     uint64_t* xempty = xfull + XS;
-    int* s_flag = reinterpret_cast<int*>(xempty + XS);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tile = blockIdx.x, split = blockIdx.y;
-    if (B200_TRACING && threadIdx.x == 0) {
-        unsigned long long gt;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
-        atomicMin(reinterpret_cast<unsigned long long*>(&p.trace[8 * 64 + 14]), gt);   // earliest CTA start (ns)
-    }
     const int kb0 = split * p.kb_per_split;
     const int kb1 = min(kb0 + p.kb_per_split, p.k_blocks);
     const int nkb = kb1 - kb0;  // >= 1 by construction of the grid
@@ -366,7 +339,6 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
             for (int it = 0; it < nkb; ++it) {
                 uint8_t* stage = wring + s * W_BYTES;
                 mbar_wait(&wempty[s], ph ^ 1);
-                B200_TRACE(0, it);
                 mbar_arrive_expect_tx(&wfull[s], W_BYTES);
                 if (FMT == kFmtF16) {
                     const int k0 = (kb0 + it) * kGemmBK;
@@ -392,7 +364,6 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
                 uint8_t* stage = xring + s * X_BYTES;
                 const int k0 = (kb0 + it) * kGemmBK;
                 mbar_wait(&xempty[s], ph ^ 1);
-                B200_TRACE(1, it);
                 mbar_arrive_expect_tx(&xfull[s], X_BYTES);
                 tma_load_2d(stage, &x_map, k0, 0, &xfull[s]);
                 tma_load_2d(stage + BPAD * 128, &x_map, k0 + 64, 0, &xfull[s]);
@@ -417,12 +388,9 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
         uint32_t phw = 0, phx = 0;
         for (int it = 0; it < nkb; ++it) {
             mbar_wait(&wfull[sw], phw);
-            if (threadIdx.x == 0) B200_TRACE(2, it);
             uint32_t a[8][4];
             if (FMT != kFmtF16) load_w_frag<FMT, T>(smem_u32(wring + sw * W_BYTES), R, lane, a, smem_u32(&wempty[sw]));
-            if (threadIdx.x == 0) B200_TRACE(3, it);
             mbar_wait(&xfull[sx], phx);
-            if (threadIdx.x == 0) B200_TRACE(6, it);
             const uint32_t xs = smem_u32(xring + sx * X_BYTES);
             const uint32_t wsm = smem_u32(wring + sw * W_BYTES) + (uint32_t)(warp >> 2) * 8192;   // rows 64g.. of the tile
             fence_regs(acc);
@@ -436,7 +404,6 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
             wgmma_commit();
             wgmma_wait<0>();
             fence_regs(acc);
-            if (threadIdx.x == 0) B200_TRACE(7, it);
             __syncwarp();
             if (lane == 0) {
                 mbar_arrive(&xempty[sx]);                       // activation stage consumed
@@ -451,7 +418,6 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
         // ------------------------------------------------------------------ epilogue
         // this thread's accumulators: rows[h] (h = 0, 1) x batch columns 8i + 2*t4 + c, value acc[4i + 2h + c]
         const int rows[2] = {16 * R + (lane >> 2), 16 * R + (lane >> 2) + 8};
-        const int n_tiles = gridDim.x;
         T* yp = reinterpret_cast<T*>(p.y);
         float cscale[2] = {1.f, 1.f}, bias[2] = {0.f, 0.f};
 #pragma unroll
@@ -481,7 +447,7 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
                         else if constexpr (VAR == 1) rs_emit<T>(p, rsl[h], b, n, v, lane, 4);   // N % 128 == 0 in this mode
                         else if (n < p.N && b < p.B) yp[(size_t)b * p.N + n] = from_f32<T>(v);
                     }
-        } else if (p.cluster_reduce) {
+        } else {
             // split-K merge through distributed shared memory: park the fp32 partial tile [bpad][128] in this CTA's smem
             // (the activation ring is idle now); the merge itself follows the cluster barrier below.
             float* red = reinterpret_cast<float*>(xring);
@@ -491,62 +457,10 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
                 for (int h = 0; h < 2; ++h)
 #pragma unroll
                     for (int c = 0; c < 2; ++c) red[(8 * i + 2 * t4 + c) * kGemmTileN + rows[h]] = acc[4 * i + 2 * h + c];
-        } else {
-            // write the fp32 partial tile [bpad][128] (coalesced along n), then the last CTA of this n-tile reduces
-            float* wsp = p.ws + ((size_t)split * n_tiles + tile) * (size_t)(BPAD * kGemmTileN);
-#pragma unroll
-            for (int i = 0; i < BPAD / 8; ++i)
-#pragma unroll
-                for (int h = 0; h < 2; ++h)
-#pragma unroll
-                    for (int c = 0; c < 2; ++c) {
-                        const int b = 8 * i + 2 * t4 + c;
-                        if (b < p.B) __stcg(&wsp[(size_t)b * kGemmTileN + rows[h]], acc[4 * i + 2 * h + c]);
-                    }
-            __threadfence();
-            asm volatile("bar.sync 1, %0;" ::"n"(NDQ_THREADS) : "memory");
-            if (threadIdx.x == 0) {
-                const int prev = atomicAdd(&p.sem[tile], 1);
-                *s_flag = (prev == p.nsplit - 1);
-            }
-            asm volatile("bar.sync 1, %0;" ::"n"(NDQ_THREADS) : "memory");
-            if (*s_flag) {
-                __threadfence();
-                // the reducer: thread = feature row (warp % 4) * 32 + lane, the two warps of a row share its 16-column slices
-                constexpr int SLICES = BPAD / 16, KCS = NDQ_WARPS / 4;
-                const int row = (warp & 3) * 32 + lane, kce = warp >> 2;
-                const int n = tile * kGemmTileN + row;
-                const bool n_ok = n < p.N;
-                float cs1 = 1.f, bi1 = 0.f;
-                if (n_ok) {
-                    if (FMT == kFmtInt8) cs1 = to_f32<T>(reinterpret_cast<const T*>(p.col_scale)[n]);
-                    if (p.bias) bi1 = to_f32<T>(reinterpret_cast<const T*>(p.bias)[n]);
-                }
-                for (int sl = kce; sl < SLICES; sl += KCS) {
-                    // all loads of a slice are issued before the first use (the partials sit in L2)
-                    float s16[16];
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) s16[j] = 0.f;
-                    for (int sp = 0; sp < p.nsplit; ++sp) {
-                        const float* src = p.ws + ((size_t)sp * n_tiles + tile) * (size_t)(BPAD * kGemmTileN) + row;
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) {
-                            const int b = sl * 16 + j;
-                            if (b < p.B) s16[j] += __ldcg(src + (size_t)b * kGemmTileN);
-                        }
-                    }
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const int b = sl * 16 + j;
-                        if (n_ok && b < p.B) yp[(size_t)b * p.N + n] = from_f32<T>(fmaf(s16[j], cs1, bi1));
-                    }
-                }
-                if (threadIdx.x == 0) p.sem[tile] = 0;
-            }
         }
     }
 
-    if (p.nsplit > 1 && p.cluster_reduce) {
+    if (p.nsplit > 1) {
         // every thread of every CTA of the cluster (1, nsplit, 1) passes both barriers
         cluster_sync_all();
         if (warp < NDQ_WARPS) {
@@ -588,7 +502,7 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
             const float* fin = reinterpret_cast<const float*>(wring);
             T* yp = reinterpret_cast<T*>(p.y);
             const int n_out = p.N / 2;
-            const int S = (p.nsplit > 1 && p.cluster_reduce) ? p.nsplit : 1;
+            const int S = p.nsplit;
             const int rank = S > 1 ? (int)cluster_ctarank() : 0;
             for (int idx = threadIdx.x; idx < BPAD * 64; idx += NDQ_THREADS) {
                 const int b = idx >> 6, r = idx & 63;
@@ -601,11 +515,6 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
         }
     }
     __syncthreads();
-    if (B200_TRACING && threadIdx.x == 0) {
-        unsigned long long gt;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
-        atomicMax(reinterpret_cast<unsigned long long*>(&p.trace[8 * 64 + 15]), gt);   // latest CTA end (ns)
-    }
 }
 
 // ---- load-time re-layout kernels (replace device_impl.py:392-479 preprocess_weights_for_mixed_gemm): reference

@@ -153,7 +153,22 @@ def make_w8g(K, N, seed=1, simple=False):
     return q, s, zs
 
 
-def gemm_case(name, fmt, B, K, N, dtype=torch.float16, simple=False, onehot=False, env=None, bias=False, big=False):
+def run_gemm(name, x, w, ws, program, **kw):
+    """One wo_gemm call; program=True records it into a decode program and launches that, so it runs in the persistent
+    kernel (it must become the program's one fused op)."""
+    if not program:
+        return ops.wo_gemm(x, w, ws, **kw)
+    prog = ops.Program()
+    with prog.record():
+        y = ops.wo_gemm(x, w, ws, **kw)
+    report(name + " [recorded as one persistent-kernel op]", prog.num_ops == 1, f"num_ops={prog.num_ops}")
+    prog.launch()
+    torch.cuda.synchronize()
+    return y
+
+
+def gemm_case(name, fmt, B, K, N, dtype=torch.float16, simple=False, onehot=False, env=None, bias=False, big=False,
+              program=False):
     def fn():
         old = {}
         for k, v in (env or {}).items():
@@ -196,7 +211,7 @@ def gemm_case(name, fmt, B, K, N, dtype=torch.float16, simple=False, onehot=Fals
                 w = ops.pack_f16(wd)
                 ref = refk.ref_dequant_gemm(x, fmt, wd, None, None, 128, bias_t)
             ws = ops.gemm_workspace(max(B, 1), [(K, N)], dev)
-            y = ops.wo_gemm(x, w, ws, bias=bias_t)
+            y = run_gemm(name, x, w, ws, program, bias=bias_t)
             torch.cuda.synchronize()
             tol = 2e-2 if fmt == B200_FMT_INT4 else 1e-2
             if dtype == torch.bfloat16:
@@ -230,7 +245,7 @@ def gemm_case(name, fmt, B, K, N, dtype=torch.float16, simple=False, onehot=Fals
     guard(name, fn)
 
 
-def gemm_silu_case(name, fmt, B, K, inter, dtype=torch.float16, env=None):
+def gemm_silu_case(name, fmt, B, K, inter, dtype=torch.float16, env=None, program=False):
     """w13 GEMM with the fused SiLU*mul epilogue vs oracle (GEMM on the un-permuted weight, then silu_and_mul)."""
     def fn():
         old = {}
@@ -265,7 +280,7 @@ def gemm_silu_case(name, fmt, B, K, inter, dtype=torch.float16, env=None):
                 gu = orc.dequant_gemm(bits(x), "f16", bits(wd))
             exp = orc.from_bits(orc.silu_and_mul(gu), False)
             ws = ops.gemm_workspace(B, [(K, N)], dev)
-            y = ops.wo_gemm(x, w, ws, silu_mul=True)
+            y = run_gemm(name, x, w, ws, program, silu_mul=True)
             torch.cuda.synchronize()
             ok, info = diff_info(y, exp, 2e-2, 2e-2)
             report(name + " [fused silu*mul vs oracle]", ok and tuple(y.shape) == (B, inter), info)
@@ -362,8 +377,6 @@ if __name__ == "__main__":
             gemm_case(f"gemm {nm} B16 K256 N256", fmt, 16, 256, 256)
             gemm_case(f"gemm {nm} B5 K512 N384 bias", fmt, 5, 512, 384, bias=True)
             gemm_case(f"gemm {nm} B32 K1024 N256 splitk4", fmt, 32, 1024, 256, env={"B200_GEMM_SPLITK": 4})
-            gemm_case(f"gemm {nm} B19 K1024 N256 splitk8 semaphore", fmt, 19, 1024, 256,
-                      env={"B200_GEMM_SPLITK": 8, "B200_GEMM_CLUSTER": 0})
             gemm_case(f"gemm {nm} B19 K1024 N384 splitk3 bias cluster", fmt, 19, 1024, 384, env={"B200_GEMM_SPLITK": 3}, bias=True)
             gemm_case(f"gemm {nm} B33 K512 N200 (ragged N, bpad64)", fmt, 33, 512, 200)
             gemm_case(f"gemm {nm} B100 K512 N256 (bpad128)", fmt, 100, 512, 256)

@@ -64,7 +64,6 @@ ATTN_CASES = [
     ("cluster merge 8 splits g16", 2, 16, 1, 64, [500, 1], torch.float16, {"B200_ATTN_TILES_PER_SPLIT": 1}),
     ("cluster merge 2 splits bf16 p16", 4, 8, 2, 16, [10, 20, 65, 128], torch.bfloat16, {"B200_ATTN_TILES_PER_SPLIT": 1}),
     ("cluster merge 3 splits mha p32", 3, 4, 4, 32, [64, 65, 190], torch.float16, {"B200_ATTN_TILES_PER_SPLIT": 1}),
-    ("workspace merge (cluster off)", 3, 8, 2, 64, [63, 64, 700], torch.float16, {"B200_ATTN_TILES_PER_SPLIT": 2, "B200_ATTN_CLUSTER": 0}),
 ]
 
 
@@ -230,31 +229,23 @@ PERSISTENT = [
     ("whole tiles bf16", B200_FMT_INT4, 8, 256, 256, dict(dtype=torch.bfloat16)),
     ("ragged N bpad64", B200_FMT_INT4, 33, 512, 200, {}),
     ("Llama w2 B32", B200_FMT_INT4, 32, 14336, 4096, dict(big=True)),
-    ("ragged stream-K Llama w13 B32", B200_FMT_INT4, 32, 4096, 28672, dict(big=True, env_extra={"B200_SK_STREAMK": 1})),
-    ("ragged stream-K small", B200_FMT_INT8, 16, 1024, 640, dict(env_extra={"B200_SK_STREAMK": 1})),
 ]
 
 
 @pytest.mark.parametrize("case", PERSISTENT, ids=[c[0] for c in PERSISTENT])
 def test_gemm_persistent_kernel_standalone(case):
-    """The persistent kernel of the decode programs (csrc/decode_program.cuh) run as a one-op program: uniform split-K
-    merged by all contributors, whole tiles, and the ragged stream-K plan with a designated reducer."""
+    """The persistent kernel of the decode programs (csrc/decode_program.cuh) run as a one-op program: split tiles merged
+    by all their contributors, and whole tiles stored directly. The probe checks that the GEMM was recorded as an op of the
+    persistent kernel, not replayed through the cluster kernel."""
     name, fmt, B, K, N, kw = case
-    kw = dict(kw)
-    env = {"B200_GEMM_PERSISTENT": 1}
-    env.update(kw.pop("env_extra", {}))
-    _run(probe.gemm_case, name, fmt, B, K, N, env=env, **kw)
-    _run(probe.gemm_silu_case, name + " silu", fmt, 7, 512, 192, env=env)
+    _run(probe.gemm_case, name, fmt, B, K, N, program=True, **kw)
+    _run(probe.gemm_silu_case, name + " silu", fmt, 7, 512, 192, program=True)
 
 
 @pytest.mark.parametrize("fmt", [B200_FMT_F16, B200_FMT_INT8, B200_FMT_INT4, B200_FMT_INT8G], ids=["f16", "int8", "int4", "int8g"])
 def test_gemm_fused_silu_mul_vs_oracle(fmt):
     _run(probe.gemm_silu_case, "silu direct", fmt, 7, 256, 192)
     _run(probe.gemm_silu_case, "silu cluster split", fmt, 32, 1024, 128, env={"B200_GEMM_SPLITK": 4})
-
-
-def test_gemm_semaphore_split_path_still_correct():
-    _run(probe.gemm_case, "semaphore split", B200_FMT_INT4, 19, 1024, 256, env={"B200_GEMM_SPLITK": 8, "B200_GEMM_CLUSTER": 0})
 
 
 def test_gemm_is_linear_in_x():
