@@ -144,7 +144,7 @@ struct SegCfg {
     static constexpr int XS = gemm_x_stages(BPAD);
     static constexpr int X_BYTES = gemm_x_stage_bytes(BPAD);
     static constexpr int W_BYTES = gemm_w_bytes(FMT);
-    static constexpr int WS = gemm_w_stages_for(FMT, BPAD, 106 * 1024);
+    static constexpr int WS = gemm_w_stages_for(FMT, BPAD, 106 * 1024, XS);
     static constexpr int SMEM = XS * X_BYTES + WS * W_BYTES + kGemmSmemMisc;
     static_assert(WS >= 3, "weight ring too shallow");
 };

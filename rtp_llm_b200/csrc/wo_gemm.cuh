@@ -46,20 +46,25 @@ __host__ __device__ constexpr int gemm_threads() { return (gemm_ndq_warps() + 2)
 __host__ __device__ constexpr int gemm_x_stage_bytes(int bpad) { return bpad * 256; }
 __host__ __device__ constexpr int gemm_x_stages(int bpad) { return bpad <= 32 ? 4 : 3; }
 constexpr int kGemmSmemMisc = 1024 /*align*/ + 1024 /*barriers*/;
-__host__ __device__ constexpr int gemm_w_stages_for(int fmt, int bpad, int budget) {
-    int n = (budget - kGemmSmemMisc - gemm_x_stages(bpad) * gemm_x_stage_bytes(bpad)) / gemm_w_bytes(fmt);
+__host__ __device__ constexpr int gemm_w_stages_for(int fmt, int bpad, int budget, int xs) {
+    int n = (budget - kGemmSmemMisc - xs * gemm_x_stage_bytes(bpad)) / gemm_w_bytes(fmt);
     return n > 12 ? 12 : n;
+}
+// Activation ring of wo_gemm_kernel. Its pipelined main loop holds an activation stage until both halves of the block have
+// retired, so it takes 6 stages wherever two CTAs per SM still keep 6 weight stages (INT4 at batch pad <= 32); the other
+// formats keep gemm_x_stages rather than drop to one CTA per SM.
+__host__ __device__ constexpr int gemm_cluster_x_stages(int fmt, int bpad) {
+    return bpad <= 32 && gemm_w_stages_for(fmt, bpad, 106 * 1024, 6) >= 6 ? 6 : gemm_x_stages(bpad);
 }
 // two CTAs per SM when at least 4 weight stages fit in half an SM's shared memory
 __host__ __device__ constexpr int gemm_min_ctas(int fmt, int bpad) {
-    return gemm_w_stages_for(fmt, bpad, 106 * 1024) >= 4 ? 2 : 1;
+    return gemm_w_stages_for(fmt, bpad, 106 * 1024, gemm_cluster_x_stages(fmt, bpad)) >= 4 ? 2 : 1;
 }
 __host__ __device__ constexpr int gemm_w_stages(int fmt, int bpad) {
-    return gemm_min_ctas(fmt, bpad) == 2 ? gemm_w_stages_for(fmt, bpad, 106 * 1024)
-                                         : gemm_w_stages_for(fmt, bpad, 216 * 1024);
+    return gemm_w_stages_for(fmt, bpad, gemm_min_ctas(fmt, bpad) == 2 ? 106 * 1024 : 216 * 1024, gemm_cluster_x_stages(fmt, bpad));
 }
 __host__ __device__ constexpr int gemm_smem_bytes(int fmt, int bpad) {
-    return gemm_x_stages(bpad) * gemm_x_stage_bytes(bpad) + gemm_w_stages(fmt, bpad) * gemm_w_bytes(fmt) + kGemmSmemMisc;
+    return gemm_cluster_x_stages(fmt, bpad) * gemm_x_stage_bytes(bpad) + gemm_w_stages(fmt, bpad) * gemm_w_bytes(fmt) + kGemmSmemMisc;
 }
 
 // Row-parallel GEMM under tensor parallelism (b200_wo_gemm_rs): the epilogue pushes every output element that another rank
@@ -230,39 +235,49 @@ struct Pair<__nv_bfloat16> {
 //   8-bit : two words per k-step, vector (j / 2, R, lane); bytes 0-3 = a[j][0], a[j][1], bytes 4-7 = a[j][2], a[j][3]
 // Group scales / zero*scale stay per feature row after the payload. The stage is released (`empty`) as soon as the warp
 // holds its bytes in registers.
-template <int FMT, typename T>
-__device__ __forceinline__ void load_w_frag(uint32_t wb, int R, int lane, uint32_t (&a)[8][4], uint32_t empty_bar) {
+//
+// A block is dequantised in two halves of 4 k-steps (16 A registers each) so that the GEMM main loop can pipeline them:
+// half h is payload vector h (INT4) or vectors 2h, 2h+1 (8-bit).
+template <int FMT>
+constexpr int kWVecsPerHalf = FMT == kFmtInt4 ? 1 : 2;
+
+// Group scale / zero*scale of this thread's feature rows A and B (INT4 and INT8G; unused otherwise). Kept as raw 16-bit
+// values and broadcast at the use, where the broadcast folds into the hfma2 operand (.H0_H0) instead of costing a PRMT.
+struct WScales {
+    uint16_t sA, zA, sB, zB;
+};
+
+// This thread's scales and payload vectors of the block at shared address wb: v[h] is half h.
+template <int FMT>
+__device__ __forceinline__ void load_w_block(uint32_t wb, int R, int lane, WScales& s, uint4 (&v)[2][kWVecsPerHalf<FMT>]) {
     const int rA = 16 * R + (lane >> 2), rB = rA + 8;
     const uint32_t vec = wb + (uint32_t)(R * 32 + lane) * 16;
-    typename Pair<T>::type sA, zA, sB, zB;
     if (FMT == kFmtInt4 || FMT == kFmtInt8G) {
         constexpr int Q_BYTES = FMT == kFmtInt4 ? 8192 : 16384;
-        sA = Pair<T>::bcast((uint16_t)lds_u16(wb + Q_BYTES + rA * 2));
-        zA = Pair<T>::bcast((uint16_t)lds_u16(wb + Q_BYTES + 256 + rA * 2));
-        sB = Pair<T>::bcast((uint16_t)lds_u16(wb + Q_BYTES + rB * 2));
-        zB = Pair<T>::bcast((uint16_t)lds_u16(wb + Q_BYTES + 256 + rB * 2));
+        s.sA = (uint16_t)lds_u16(wb + Q_BYTES + rA * 2);
+        s.zA = (uint16_t)lds_u16(wb + Q_BYTES + 256 + rA * 2);
+        s.sB = (uint16_t)lds_u16(wb + Q_BYTES + rB * 2);
+        s.zB = (uint16_t)lds_u16(wb + Q_BYTES + 256 + rB * 2);
     }
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int q = 0; q < kWVecsPerHalf<FMT>; ++q) v[h][q] = lds_v4(vec + (h * kWVecsPerHalf<FMT> + q) * 4096);
+}
+
+// One half block (k-steps 4h..4h+3) -> a[0..3].
+template <int FMT, typename T>
+__device__ __forceinline__ void dequant_half(const uint4 (&v)[kWVecsPerHalf<FMT>], const WScales& s, uint32_t (*a)[4]) {
+    using P = Pair<T>;
+    const typename P::type sA = P::bcast(s.sA), zA = P::bcast(s.zA), sB = P::bcast(s.sB), zB = P::bcast(s.zB);
     if (FMT == kFmtInt4) {
-        uint4 v[2];
-#pragma unroll
-        for (int h = 0; h < 2; ++h) v[h] = lds_v4(vec + h * 4096);
-        __syncwarp();
-        if (lane == 0) mbar_arrive_a(empty_bar);
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            Dequant4<T>::word(v[h].x, sA, zA, sB, zB, a[4 * h + 0]);
-            Dequant4<T>::word(v[h].y, sA, zA, sB, zB, a[4 * h + 1]);
-            Dequant4<T>::word(v[h].z, sA, zA, sB, zB, a[4 * h + 2]);
-            Dequant4<T>::word(v[h].w, sA, zA, sB, zB, a[4 * h + 3]);
-        }
+        Dequant4<T>::word(v[0].x, sA, zA, sB, zB, a[0]);
+        Dequant4<T>::word(v[0].y, sA, zA, sB, zB, a[1]);
+        Dequant4<T>::word(v[0].z, sA, zA, sB, zB, a[2]);
+        Dequant4<T>::word(v[0].w, sA, zA, sB, zB, a[3]);
     } else {
-        uint4 v[4];
 #pragma unroll
-        for (int q = 0; q < 4; ++q) v[q] = lds_v4(vec + q * 4096);
-        __syncwarp();
-        if (lane == 0) mbar_arrive_a(empty_bar);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
+        for (int q = 0; q < 2; ++q) {
             Dequant8<T>::word(v[q].x, &a[2 * q][0]);
             Dequant8<T>::word(v[q].y, &a[2 * q][2]);
             Dequant8<T>::word(v[q].z, &a[2 * q + 1][0]);
@@ -270,7 +285,7 @@ __device__ __forceinline__ void load_w_frag(uint32_t wb, int R, int lane, uint32
         }
         if (FMT == kFmtInt8G) {   // group-wise 8-bit: W' = q_s * s + zero*scale, one rounding (as INT4)
 #pragma unroll
-            for (int j = 0; j < 8; ++j)
+            for (int j = 0; j < 4; ++j)
 #pragma unroll
                 for (int i = 0; i < 4; ++i) {
                     typename Pair<T>::type h = *reinterpret_cast<typename Pair<T>::type*>(&a[j][i]);
@@ -281,12 +296,32 @@ __device__ __forceinline__ void load_w_frag(uint32_t wb, int R, int lane, uint32
     }
 }
 
+// The whole block at once (the persistent kernel's serial loop).
+template <int FMT, typename T>
+__device__ __forceinline__ void load_w_frag(uint32_t wb, int R, int lane, uint32_t (&a)[8][4], uint32_t empty_bar) {
+    WScales s;
+    uint4 v[2][kWVecsPerHalf<FMT>];
+    load_w_block<FMT>(wb, R, lane, s, v);
+    __syncwarp();
+    if (lane == 0) mbar_arrive_a(empty_bar);
+    dequant_half<FMT, T>(v[0], s, &a[0]);
+    dequant_half<FMT, T>(v[1], s, &a[4]);
+}
+
+// Descriptor of k-step j of a K-major SW128 operand whose two 64-element boxes lie BOX_BYTES apart, as an offset to the
+// descriptor of k-step 0 (start address in 16-byte units: 32 bytes per k-step inside a box). A stage lies below 256 KB of
+// shared memory, so the sum never carries out of the 14-bit start field.
+template <int BOX_BYTES>
+__device__ __forceinline__ uint64_t sw128_kstep(uint64_t desc0, int j) {
+    return desc0 + (uint64_t)((j >> 2) * (BOX_BYTES >> 4) + (j & 3) * 2);
+}
+
 template <int FMT, typename T, int BPAD, int VAR>
 __global__ void __launch_bounds__(gemm_threads(), gemm_min_ctas(FMT, BPAD))
 wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant__ CUtensorMap w_map,
                const typename GemmParamsOf<VAR>::type p) {
     constexpr int WS = gemm_w_stages(FMT, BPAD);           // weight ring depth
-    constexpr int XS = gemm_x_stages(BPAD);                // activation ring depth
+    constexpr int XS = gemm_cluster_x_stages(FMT, BPAD);   // activation ring depth
     constexpr int NDQ_WARPS = gemm_ndq_warps();
     constexpr int NDQ_THREADS = NDQ_WARPS * 32;
     constexpr int W_WTMA = NDQ_WARPS, W_XTMA = NDQ_WARPS + 1;
@@ -384,33 +419,85 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
         float acc[NACC];
 #pragma unroll
         for (int q = 0; q < NACC; ++q) acc[q] = 0.f;
-        int sw = 0, sx = 0;
+        int sw = 0, sx = 0, px = 0, pw = 0;   // current / previous stage of each ring
         uint32_t phw = 0, phx = 0;
-        for (int it = 0; it < nkb; ++it) {
-            mbar_wait(&wfull[sw], phw);
-            uint32_t a[8][4];
-            if (FMT != kFmtF16) load_w_frag<FMT, T>(smem_u32(wring + sw * W_BYTES), R, lane, a, smem_u32(&wempty[sw]));
-            mbar_wait(&xfull[sx], phx);
-            const uint32_t xs = smem_u32(xring + sx * X_BYTES);
-            const uint32_t wsm = smem_u32(wring + sw * W_BYTES) + (uint32_t)(warp >> 2) * 8192;   // rows 64g.. of the tile
-            fence_regs(acc);
-            wgmma_fence();
-#pragma unroll
-            for (int j = 0; j < kGemmBK / 16; ++j) {
-                const uint64_t bdesc = make_smem_desc_sw128(xs + (j >> 2) * (BPAD * 128) + (j & 3) * 32);
-                if constexpr (FMT == kFmtF16) wgmma_ss<BPAD, T>(acc, make_smem_desc_sw128(wsm + (j >> 2) * 16384 + (j & 3) * 32), bdesc, 1u);
-                else wgmma_rs<BPAD, T>(acc, a[j], bdesc, 1u);
-            }
-            wgmma_commit();
-            wgmma_wait<0>();
-            fence_regs(acc);
+        fence_regs(acc);
+        if constexpr (FMT != kFmtF16) {
+            // Software pipeline over half blocks (4 k-steps) with two A buffers: after the MMAs of one half are committed,
+            // wgmma_wait<1> retires the group before them, which frees the other buffer, and the warp dequantises the next
+            // half into it while the tensor cores work. The weight stage is still released right after its LDS (the second
+            // half's raw words wait in registers); activation stage i once both halves of block i have retired. The MMAs
+            // into acc keep the serial order, so the sums are the same bits.
+            constexpr int NV = kWVecsPerHalf<FMT>;
+            uint32_t a0[4][4], a1[4][4];
+            uint4 v[2][NV];
+            WScales sc;
+            mbar_wait(&wfull[0], 0);
+            load_w_block<FMT>(smem_u32(wring), R, lane, sc, v);
             __syncwarp();
-            if (lane == 0) {
-                mbar_arrive(&xempty[sx]);                       // activation stage consumed
-                if (FMT == kFmtF16) mbar_arrive(&wempty[sw]);   // f16 weights are read by the MMA itself
+            if (lane == 0) mbar_arrive(&wempty[0]);
+            dequant_half<FMT, T>(v[0], sc, a0);
+            sw = 1;
+            mbar_wait(&xfull[0], 0);
+            for (int it = 0; it < nkb; ++it) {
+                const uint64_t bdesc = make_smem_desc_sw128(smem_u32(xring + sx * X_BYTES));
+                wgmma_fence();
+#pragma unroll
+                for (int j = 0; j < 4; ++j) wgmma_rs<BPAD, T>(acc, a0[j], sw128_kstep<BPAD * 128>(bdesc, j), 1u);
+                wgmma_commit();
+                wgmma_wait<1>();   // block it-1 has retired: a1 and its activation stage are free
+                __syncwarp();
+                if (it > 0 && lane == 0) mbar_arrive(&xempty[px]);
+                dequant_half<FMT, T>(v[1], sc, a1);
+                wgmma_fence();
+#pragma unroll
+                for (int j = 0; j < 4; ++j) wgmma_rs<BPAD, T>(acc, a1[j], sw128_kstep<BPAD * 128>(bdesc, 4 + j), 1u);
+                wgmma_commit();
+                wgmma_wait<1>();   // the first half of block it has retired: a0 is free
+                px = sx;
+                if (++sx == XS) { sx = 0; phx ^= 1; }
+                if (it + 1 < nkb) {
+                    if (sw == WS) { sw = 0; phw ^= 1; }
+                    mbar_wait(&wfull[sw], phw);
+                    load_w_block<FMT>(smem_u32(wring + sw * W_BYTES), R, lane, sc, v);
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&wempty[sw]);
+                    ++sw;
+                    dequant_half<FMT, T>(v[0], sc, a0);
+                    mbar_wait(&xfull[sx], phx);
+                }
             }
-            if (++sx == XS) { sx = 0; phx ^= 1; }
-            if (++sw == WS) { sw = 0; phw ^= 1; }
+        } else {
+            // FP16 weights feed the MMA from shared memory. One commit group stays in flight, so the waits for block it+1
+            // overlap the MMAs of block it; both stages of a block are released once its group has retired.
+            for (int it = 0; it < nkb; ++it) {
+                mbar_wait(&wfull[sw], phw);
+                mbar_wait(&xfull[sx], phx);
+                const uint64_t adesc = make_smem_desc_sw128(smem_u32(wring + sw * W_BYTES) + (uint32_t)(warp >> 2) * 8192);   // rows 64g..
+                const uint64_t bdesc = make_smem_desc_sw128(smem_u32(xring + sx * X_BYTES));
+                wgmma_fence();
+#pragma unroll
+                for (int j = 0; j < kGemmBK / 16; ++j)
+                    wgmma_ss<BPAD, T>(acc, sw128_kstep<16384>(adesc, j), sw128_kstep<BPAD * 128>(bdesc, j), 1u);
+                wgmma_commit();
+                wgmma_wait<1>();   // block it-1 has retired
+                __syncwarp();
+                if (it > 0 && lane == 0) {
+                    mbar_arrive(&xempty[px]);
+                    mbar_arrive(&wempty[pw]);
+                }
+                px = sx;
+                pw = sw;
+                if (++sx == XS) { sx = 0; phx ^= 1; }
+                if (++sw == WS) { sw = 0; phw ^= 1; }
+            }
+        }
+        wgmma_wait<0>();
+        fence_regs(acc);
+        __syncwarp();
+        if (lane == 0) {   // the last block's stages
+            mbar_arrive(&xempty[px]);
+            if (FMT == kFmtF16) mbar_arrive(&wempty[pw]);
         }
         // every dequant warp is past its last read of both rings: the epilogues below may reuse them as staging
         asm volatile("bar.sync 1, %0;" ::"n"(NDQ_THREADS) : "memory");
