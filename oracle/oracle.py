@@ -131,23 +131,61 @@ def paged_decode_attn(q_bits, kv_pool_bits, page_list, sequence_lengths, head_nu
     return out
 
 
-def paged_decode_attn_np(q, kv_pool, block_ids, sequence_lengths, tokens_per_block) -> np.ndarray:
-    """Tiny pure-numpy restatement (float64, no P rounding) for cross-checks. q [B,Hq,D] float, kv_pool [P,2,Hkv,T,D]."""
-    B, Hq, D = q.shape
+def paged_decode_attn_np(q, kv_pool, block_ids, sequence_lengths, tokens_per_block, q_scale=1.0, with_abs=False):
+    """Float64 restatement with no P rounding: the reference the attention error budget is measured from.
+
+    q [B,Hq,D], or [B,q_len,Hq,D] for several query tokens per sequence (query j sees positions 0 .. seq[b] + j);
+    kv_pool [P,2,Hkv,T,D] float; block_ids [B,M]. Returns out [B, Hq*D] (or [B, q_len, Hq*D]); with_abs=True returns
+    (out, E), where E = sum_t p_t |v_t| / sum_t p_t, of the same shape, is the size of the terms the output averages
+    (see attn_error_budget)."""
+    multi = q.ndim == 4
+    q4 = q if multi else q[:, None]
+    B, QL, Hq, D = q4.shape
     Hkv = kv_pool.shape[2]
     g = Hq // Hkv
-    out = np.zeros((B, Hq, D), np.float64)
+    T = tokens_per_block
+    out = np.zeros((B, QL, Hq, D), np.float64)
+    E = np.zeros_like(out)
     for b in range(B):
-        L = int(sequence_lengths[b]) + 1
-        npages = (L + tokens_per_block - 1) // tokens_per_block
-        pages = [int(block_ids[b][j]) for j in range(npages)]
-        k = np.concatenate([kv_pool[p, 0] for p in pages], axis=1)[:, :L]  # [Hkv, L, D]
-        v = np.concatenate([kv_pool[p, 1] for p in pages], axis=1)[:, :L]
-        for h in range(Hq):
-            s = (k[h // g].astype(np.float64) @ q[b, h].astype(np.float64)) / np.sqrt(D)
-            p = np.exp(s - s.max())
-            out[b, h] = (p[:, None] * v[h // g].astype(np.float64)).sum(0) / p.sum()
-    return out.reshape(B, Hq * D)
+        L = int(sequence_lengths[b]) + QL
+        pages = np.asarray(block_ids[b][: (L + T - 1) // T], np.int64)
+        kv = np.asarray(kv_pool[pages], np.float64)                               # [pages, 2, Hkv, T, D]
+        k = kv[:, 0].transpose(1, 0, 2, 3).reshape(Hkv, -1, D)[:, :L]            # [Hkv, L, D]
+        v = kv[:, 1].transpose(1, 0, 2, 3).reshape(Hkv, -1, D)[:, :L]
+        qh = np.asarray(q4[b], np.float64).reshape(QL, Hkv, g, D).transpose(1, 0, 2, 3).reshape(Hkv, QL * g, D)
+        s = (qh @ k.transpose(0, 2, 1)) * (q_scale / np.sqrt(D))                  # [Hkv, QL*g, L]
+        seen = np.arange(L)[None, :] <= (L - QL + np.arange(QL))[:, None]         # [QL, L]
+        s = np.where(np.repeat(seen, g, axis=0)[None], s, -np.inf)
+        p = np.exp(s - s.max(-1, keepdims=True))
+        den = p.sum(-1, keepdims=True)
+        o, e = (p @ v) / den, (p @ np.abs(v)) / den                               # [Hkv, QL*g, D]
+        out[b] = o.reshape(Hkv, QL, g, D).transpose(1, 0, 2, 3).reshape(QL, Hq, D)
+        E[b] = e.reshape(Hkv, QL, g, D).transpose(1, 0, 2, 3).reshape(QL, Hq, D)
+    shape = (B, QL, Hq * D) if multi else (B, Hq * D)
+    return (out.reshape(shape), E.reshape(shape)) if with_abs else out.reshape(shape)
+
+
+def ulp(x: np.ndarray, is_bf16: bool) -> np.ndarray:
+    """Spacing of fp16 / bf16 numbers at |x| (subnormal spacing below the smallest normal)."""
+    mant, emin = (7, -126) if is_bf16 else (10, -14)
+    e = np.floor(np.log2(np.maximum(np.abs(np.asarray(x, np.float64)), 2.0 ** emin)))
+    return 2.0 ** (e - mant)
+
+
+def attn_error_budget(ref: np.ndarray, E: np.ndarray, is_bf16: bool) -> np.ndarray:
+    """Per-element bound on |got - ref| for a correct paged decode attention kernel in T = fp16 / bf16, against the float64
+    reference (ref, E) of paged_decode_attn_np:  ulp_T(ref) + u_T * (E + |ref|),  u = 2^-11 (fp16) or 2^-8 (bf16).
+
+    Why: the kernel computes O = sum_t P_t v_t / l with l = sum_t p_t kept in fp32, and P_t = p_t rounded once to T as
+    the A operand of the PV product. Rounding to nearest moves each p_t by at most u * p_t (p_t in T's normal range, which
+    holds for every p_t that matters at the scores these tests draw), so the numerator moves by
+    at most u * sum_t p_t |v_t| and O by at most u * E. The fp32 work (scores, exp2, the row sum, the split merges) adds
+    errors of order 2^-24 per operation, far below u; u * |ref| covers it. The one final rounding of O to T costs half
+    an ulp_T(ref), and ulp_T(ref) leaves room for the fp32 terms near zero. The bound does not depend on the sequence
+    length, so a dropped token, tile or split, whose effect on the output shrinks like 1/L, still exceeds it where a
+    fixed rtol/atol of 1e-2 stops seeing it. The C oracle, which rounds P as the kernel does, stays near 0.12 of it."""
+    u = 2.0 ** -8 if is_bf16 else 2.0 ** -11
+    return ulp(ref, is_bf16) + u * (np.asarray(E, np.float64) + np.abs(ref))
 
 
 # ----------------------------------------------------------------------------------------------

@@ -48,7 +48,71 @@ def guard(name, fn):
     torch.cuda.synchronize()
 
 
+# Every kernel output goes through out= into a view of a larger buffer, between sentinel bands, so a store that runs past
+# the output (a ragged last tile, the padding rows of a batch pad, a query row past the group) shows up. The sentinel is a
+# NaN in fp16 and in bf16, and the view starts out filled with it too: an element the kernel never writes fails the value
+# check.
+GUARD_BYTES = 4096
+SENTINEL = 0x7FC1
+
+
+def guarded_empty(shape, dtype):
+    """(buffer, view): the view is `shape` of `dtype`, 16-byte aligned, with GUARD_BYTES of sentinel on each side."""
+    pad = GUARD_BYTES // 2
+    buf = torch.full((2 * pad + math.prod(shape),), SENTINEL, dtype=torch.int16, device=dev)
+    return buf, buf[pad:buf.numel() - pad].view(dtype).view(shape)
+
+
+def report_bands(name, buf):
+    pad = GUARD_BYTES // 2
+    bad = int((buf[:pad] != SENTINEL).sum().item() + (buf[buf.numel() - pad:] != SENTINEL).sum().item())
+    report(name + " [guard bands untouched]", bad == 0, f"{bad} sentinel elements overwritten" if bad else "")
+
+
 # ---------------------------------------------------------------------------------------------- attention
+def budget_info(got, ref, E, is_bf16):
+    """Check against the float64 reference with oracle.attn_error_budget; the info line carries the worst err/budget."""
+    got = got.float().cpu().numpy().reshape(ref.shape).astype(np.float64)
+    ratio = np.abs(got - ref) / orc.attn_error_budget(ref, E, is_bf16)
+    ratio[np.isnan(ratio)] = np.inf
+    bad = ratio > 1.0
+    info = f"worst err/budget={ratio.max():.3f} bad={int(bad.sum())}/{ratio.size}"
+    if bad.any():
+        idx = np.flatnonzero(bad)[:6]
+        info += " first_bad=" + ", ".join(f"{i}:{got.flat[i]:.5g}/{ref.flat[i]:.5g}" for i in idx)
+    return not bad.any(), info
+
+
+def within_ulp(got, exp, is_bf16):
+    """got (the kernel's T output) within one ulp of T of the float64 value exp."""
+    got = got.float().cpu().numpy().reshape(exp.shape).astype(np.float64)
+    err = np.abs(got - exp)
+    bad = ~(err <= orc.ulp(exp, is_bf16))
+    info = f"max_abs_err={np.nanmax(err):.4g} bad={int(bad.sum())}/{exp.size}"
+    if bad.any():
+        idx = np.flatnonzero(bad)[:6]
+        info += " first_bad=" + ", ".join(f"{i}:{got.flat[i]:.5g}/{exp.flat[i]:.5g}" for i in idx)
+    return not bad.any(), info
+
+
+class env_set:
+    """Set the library's test-hook environment variables for the duration of a block."""
+    def __init__(self, env):
+        self.env, self.old = env or {}, {}
+
+    def __enter__(self):
+        for k, v in self.env.items():
+            self.old[k] = os.environ.get(k)
+            os.environ[k] = str(v)
+
+    def __exit__(self, *exc):
+        for k, v in self.old.items():
+            if v is None:
+                os.environ.pop(k, None)
+            else:
+                os.environ[k] = v
+
+
 def make_attn_case(B, Hq, Hkv, T, lens, dtype, seed=0, shuffle=True, D=128):
     g = torch.Generator().manual_seed(seed)
     M = max(math.ceil(L / T) for L in lens)
@@ -65,31 +129,43 @@ def make_attn_case(B, Hq, Hkv, T, lens, dtype, seed=0, shuffle=True, D=128):
     return q, pool, block_ids, seq
 
 
-def run_attn(q, pool, block_ids, seq, max_len=None):
-    qd, poold, bd, sd = q.to(dev), pool.to(dev), block_ids.to(dev), seq.to(dev)
-    pl = ops.convert_block_table(bd)
-    B, Hq = q.shape[0], q.shape[1]
+def pad_block_table(block_ids, T, max_len):
+    """A max_seq_len looser than the sequences needs a page table that covers it: extra columns point at page 0."""
+    M = max(block_ids.shape[1], -(-max_len // T))
+    out = torch.zeros(block_ids.shape[0], M, dtype=torch.int32)
+    out[:, : block_ids.shape[1]] = block_ids
+    return out
+
+
+def run_attn(q, pool, block_ids, seq, max_len=None, q_scale=1.0):
+    """The kernel (output through out= between guard bands) and the naive GPU kernel on the same inputs."""
     max_len = max_len or int(seq.max().item()) + 1
+    qd, poold, sd = q.to(dev), pool.to(dev), seq.to(dev)
+    pl = ops.convert_block_table(pad_block_table(block_ids, pool.shape[3], max_len).to(dev))
+    B, Hq = q.shape[0], q.shape[1]
     ws = ops.attn_workspace(B, Hq, pool.shape[2], max_len, dev)
-    out = ops.paged_decode_attn(qd, poold, pl, sd, max_len, ws)
-    ref = refk.ref_paged_decode_attn(qd, poold, pl, sd)
+    buf, out = guarded_empty((B, Hq * pool.shape[4]), q.dtype)
+    ops.paged_decode_attn(qd, poold, pl, sd, max_len, ws, out=out, q_scale=q_scale)
+    ref = refk.ref_paged_decode_attn(qd, poold, pl, sd, q_scale)
     torch.cuda.synchronize()
-    return out, ref, ws
+    return out, ref, ws, buf
 
 
-def attn_vs_oracle(name, B, Hq, Hkv, T, lens, dtype=torch.float16, env=None, D=128):
+def attn_vs_oracle(name, B, Hq, Hkv, T, lens, dtype=torch.float16, env=None, D=128, q_scale=1.0, max_len=None):
+    """Checked against the float64 reference within the error budget; the C oracle (P rounded as the kernel does) and the
+    naive GPU kernel are second opinions at the reference's rtol = atol = 1e-2 (bf16: 2e-2)."""
     def fn():
-        old = {}
-        for k, v in (env or {}).items():
-            old[k] = os.environ.get(k)
-            os.environ[k] = str(v)
-        try:
+        with env_set(env):
             q, pool, block_ids, seq = make_attn_case(B, Hq, Hkv, T, lens, dtype, D=D)
-            out, ref, ws = run_attn(q, pool, block_ids, seq)
+            out, ref, ws, buf = run_attn(q, pool, block_ids, seq, max_len, q_scale)
             is_bf16 = dtype == torch.bfloat16
+            f64, E = orc.paged_decode_attn_np(q.float().numpy(), pool.float().numpy(), block_ids.numpy(), seq.numpy(), T, q_scale,
+                                              with_abs=True)
+            ok, info = budget_info(out, f64, E, is_bf16)
+            report(name + " [kernel vs float64, error budget]", ok, info)
             bits = lambda t: t.view(torch.int16).numpy().view(np.uint16)
             exp = orc.from_bits(orc.paged_decode_attn(bits(q), bits(pool), orc.convert_block_table(block_ids.numpy()),
-                                                      seq.numpy(), Hq, Hkv, D, T, is_bf16=is_bf16), is_bf16)
+                                                      seq.numpy(), Hq, Hkv, D, T, is_bf16=is_bf16, q_scale=q_scale), is_bf16)
             tol = 2e-2 if is_bf16 else 1e-2
             ok1, i1 = diff_info(ref, exp, tol, tol)
             report(name + " [ref-kernel vs oracle]", ok1, i1)
@@ -97,24 +173,23 @@ def attn_vs_oracle(name, B, Hq, Hkv, T, lens, dtype=torch.float16, env=None, D=1
             report(name + " [kernel vs oracle]", ok2, i2)
             sem_clean = int(ws[: B * Hkv * 4].view(torch.int32).abs().sum().item()) == 0
             report(name + " [semaphores reset]", sem_clean)
-        finally:
-            for k, v in old.items():
-                if v is None:
-                    os.environ.pop(k, None)
-                else:
-                    os.environ[k] = v
+            report_bands(name, buf)
     guard(name, fn)
 
 
 def attn_vs_ref_big(name, B, Hq, Hkv, T, S, dtype=torch.float16, ragged=False):
-    """BASELINE-size shapes: the CPU oracle is the checker (it finishes these in well under a second per case with
-    OpenMP); the naive GPU kernel is kept as a second opinion."""
+    """BASELINE-size shapes: checked against the float64 reference within the error budget; the C oracle (well under a
+    second per case with OpenMP) and the naive GPU kernel are second opinions at 1e-2."""
     def fn():
         rng = np.random.default_rng(4)
         lens = [int(x) for x in (rng.integers(S // 2, S + 1, B) if ragged else [S] * B)]
         q, pool, block_ids, seq = make_attn_case(B, Hq, Hkv, T, lens, dtype, seed=42)
-        out, ref, _ = run_attn(q, pool, block_ids, seq, max_len=S)
+        out, ref, _, buf = run_attn(q, pool, block_ids, seq, max_len=S)
         is_bf16 = dtype == torch.bfloat16
+        f64, E = orc.paged_decode_attn_np(q.float().numpy(), pool.float().numpy(), block_ids.numpy(), seq.numpy(), T,
+                                          with_abs=True)
+        ok, info = budget_info(out, f64, E, is_bf16)
+        report(name + " [kernel vs float64, error budget]", ok, info)
         bits = lambda t: t.view(torch.int16).numpy().view(np.uint16)
         exp = orc.from_bits(orc.paged_decode_attn(bits(q), bits(pool), orc.convert_block_table(block_ids.numpy()),
                                                   seq.numpy(), Hq, Hkv, 128, T, is_bf16=is_bf16), is_bf16)
@@ -122,6 +197,112 @@ def attn_vs_ref_big(name, B, Hq, Hkv, T, S, dtype=torch.float16, ragged=False):
         report(name + " [kernel vs oracle]", ok, info)
         ok, info = diff_info(out, ref.float().cpu().numpy(), 1e-2, 1e-2)
         report(name + " [kernel vs ref-kernel]", ok, info)
+        report_bands(name, buf)
+    guard(name, fn)
+
+
+def attn_position_probes(name, B, Hq, Hkv, T, lens, dtype=torch.float16, env=None, D=128, q_len=1, max_len=None):
+    """Exact probes of which cache positions each query reads; they fail on any indexing error at any length.
+
+    lens = tokens cached before the q_len new ones, so query j of sequence b sees positions 0 .. lens[b] + j. V holds small
+    integers that differ by batch row, kv head, position and channel; cache slots past a sequence hold NaN.
+    * Uniform scores: q = 0, so every p is 1 and every sum is exact in fp32. Each output is the mean of V over the positions
+      the query sees, to within one ulp of T: a dropped or repeated token, a wrong page, kv head or batch row shows.
+    * Dominant key: query head r of query j has q = 64 on channel c = j*group + r, and one key it sees has 64 there: a
+      score at least 256 above every other visible key at head_dim <= 256, so every other p underflows to 0 even in fp32
+      and the output is that key's V row exactly.
+      The key sits at seq + j for several query tokens; for one, at position 0, the new token, the page and tile
+      boundaries and the first token of a forced split, varied across heads. A key with twice that score sits at
+      seq + j + 1, which query j must not see (for the last query it lies past the sequence, in the page's spare slots)."""
+    def fn():
+        with env_set(env):
+            is_bf16 = dtype == torch.bfloat16
+            g = Hq // Hkv
+            assert q_len * g <= D
+            total = [L + q_len for L in lens]
+            npg = [-(-L // T) for L in total]
+            npages = sum(npg) + 1
+            rng = np.random.default_rng(len(name))
+            perm = iter((rng.permutation(npages - 1) + 1).tolist())
+            block_ids = torch.zeros(B, max(npg), dtype=torch.int32)
+            for b in range(B):
+                for j in range(npg[b]):
+                    block_ids[b, j] = next(perm)
+            K = np.full((npages, Hkv, T, D), np.nan, np.float32)
+            V = np.full((npages, Hkv, T, D), np.nan, np.float32)
+            vals, where = [], []
+            for b in range(B):
+                t = np.arange(npg[b] * T)                              # every slot of the sequence's pages
+                pg, off = block_ids[b, t // T].numpy(), t % T
+                h, c = np.arange(Hkv)[None, :, None], np.arange(D)[None, None, :]
+                v = ((7 * t[:, None, None] + 13 * c + 31 * h + 57 * b) % 17 - 8).astype(np.float32)
+                v[:, :, 0] = (t[:, None] + 29 * np.arange(Hkv)[None] + 53 * b) % 251 - 125
+                k = rng.integers(-2, 3, v.shape).astype(np.float32)
+                k[:, :, : q_len * g] = 0
+                V[pg, :, off], K[pg, :, off] = v, k
+                if total[b] < len(t):                                  # the first spare slot holds the last query's trap key
+                    V[pg[total[b]], :, off[total[b]]], K[pg[total[b]], :, off[total[b]]] = v[total[b]], 0.0
+                vals.append(v)
+                where.append((pg, off))
+            split = 64 * int((env or {}).get("B200_ATTN_TILES_PER_SPLIT", 0))
+            target = np.zeros((B, q_len, Hkv, g), np.int64)
+            for b in range(B):
+                pg, off = where[b]
+                last = lens[b]                                         # the new token of query 0
+                for j in range(q_len):
+                    for kh in range(Hkv):
+                        for r in range(g):
+                            c = j * g + r
+                            if q_len == 1:
+                                choice = [x for x in (0, last, T - 1, T, 63, 64, split) if 0 < x <= last or x == 0]
+                                pos = choice[(b * Hkv * g + kh * g + r) % len(choice)]
+                            else:
+                                pos = last + j
+                            target[b, j, kh, r] = pos
+                            K[pg[pos], kh, off[pos], c] = 64.0
+                            if last + j + 1 < len(pg):                   # seq + j + 1: invisible to query j
+                                K[pg[last + j + 1], kh, off[last + j + 1], c] = 128.0
+            pool = torch.from_numpy(np.stack([K, V], axis=1)).to(dtype)
+            seq = torch.tensor(lens, dtype=torch.int32)
+            ml = max_len or max(total)
+            pl = ops.convert_block_table(pad_block_table(block_ids, T, ml).to(dev))
+            ws = ops.attn_workspace(B * q_len, Hq, Hkv, ml, dev)
+
+            def run(q):
+                buf, out = guarded_empty((B, q_len, Hq * D), dtype)
+                if q_len == 1:
+                    ops.paged_decode_attn(q[:, 0].contiguous().to(dev), pool.to(dev), pl, seq.to(dev), ml, ws,
+                                          out=out.view(B, Hq * D))
+                else:
+                    ops.paged_decode_attn_multi(q.to(dev), pool.to(dev), pl, seq.to(dev), ml, ws, out=out)
+                torch.cuda.synchronize()
+                return out.view(B, q_len, Hq, D), buf
+
+            # uniform scores
+            out, buf = run(torch.zeros(B, q_len, Hq, D, dtype=dtype))
+            exp = np.zeros((B, q_len, Hq, D))
+            for b in range(B):
+                for j in range(q_len):
+                    exp[b, j] = np.repeat(vals[b][: lens[b] + j + 1].astype(np.float64).mean(0), g, axis=0)
+            ok, info = within_ulp(out, exp, is_bf16)
+            report(name + " [uniform scores: mean of the visible positions]", ok, info)
+            report_bands(name + " uniform", buf)
+
+            # dominant key
+            q = np.zeros((B, q_len, Hq, D), np.float32)
+            for j in range(q_len):
+                for h in range(Hq):
+                    q[:, j, h, j * g + h % g] = 64.0
+            out, buf = run(torch.from_numpy(q).to(dtype))
+            for b in range(B):
+                for j in range(q_len):
+                    for h in range(Hq):
+                        exp[b, j, h] = vals[b][target[b, j, h // g, h % g], h // g]
+            ok, info = within_ulp(out, exp, is_bf16)
+            report(name + " [dominant key: its V row exactly]", ok, info)
+            report_bands(name + " dominant", buf)
+            sem_clean = int(ws[: B * Hkv * 4].view(torch.int32).abs().sum().item()) == 0
+            report(name + " [semaphores reset]", sem_clean)
     guard(name, fn)
 
 
@@ -168,13 +349,10 @@ def run_gemm(name, x, w, ws, program, **kw):
 
 
 def gemm_case(name, fmt, B, K, N, dtype=torch.float16, simple=False, onehot=False, env=None, bias=False, big=False,
-              program=False):
+              program=False, ws_batch=None):
+    """ws_batch: size the workspace for this batch instead of B (a smaller one makes the persistent kernel take longer runs)."""
     def fn():
-        old = {}
-        for k, v in (env or {}).items():
-            old[k] = os.environ.get(k)
-            os.environ[k] = str(v)
-        try:
+        with env_set(env):
             rng = np.random.default_rng(2)
             if onehot:
                 xf = np.zeros((B, K), np.float32)
@@ -210,8 +388,9 @@ def gemm_case(name, fmt, B, K, N, dtype=torch.float16, simple=False, onehot=Fals
                 wd = torch.from_numpy(wf).to(dtype).to(dev)
                 w = ops.pack_f16(wd)
                 ref = refk.ref_dequant_gemm(x, fmt, wd, None, None, 128, bias_t)
-            ws = ops.gemm_workspace(max(B, 1), [(K, N)], dev)
-            y = run_gemm(name, x, w, ws, program, bias=bias_t)
+            ws = ops.gemm_workspace(ws_batch or B, [(K, N)], dev)
+            buf, y = guarded_empty((B, N), dtype)
+            run_gemm(name, x, w, ws, program, bias=bias_t, out=y)
             torch.cuda.synchronize()
             tol = 2e-2 if fmt == B200_FMT_INT4 else 1e-2
             if dtype == torch.bfloat16:
@@ -236,23 +415,14 @@ def gemm_case(name, fmt, B, K, N, dtype=torch.float16, simple=False, onehot=Fals
                 report(name + " [kernel vs oracle]", ok2, i2)
             sem_clean = int(ws[:16384].view(torch.int32).abs().sum().item()) == 0
             report(name + " [semaphores reset]", sem_clean)
-        finally:
-            for k, v in old.items():
-                if v is None:
-                    os.environ.pop(k, None)
-                else:
-                    os.environ[k] = v
+            report_bands(name, buf)
     guard(name, fn)
 
 
 def gemm_silu_case(name, fmt, B, K, inter, dtype=torch.float16, env=None, program=False):
     """w13 GEMM with the fused SiLU*mul epilogue vs oracle (GEMM on the un-permuted weight, then silu_and_mul)."""
     def fn():
-        old = {}
-        for k, v in (env or {}).items():
-            old[k] = os.environ.get(k)
-            os.environ[k] = str(v)
-        try:
+        with env_set(env):
             rng = np.random.default_rng(9)
             N = 2 * inter
             x = torch.from_numpy(rng.standard_normal((B, K)).astype(np.float32)).to(dtype).to(dev)
@@ -280,16 +450,12 @@ def gemm_silu_case(name, fmt, B, K, inter, dtype=torch.float16, env=None, progra
                 gu = orc.dequant_gemm(bits(x), "f16", bits(wd))
             exp = orc.from_bits(orc.silu_and_mul(gu), False)
             ws = ops.gemm_workspace(B, [(K, N)], dev)
-            y = run_gemm(name, x, w, ws, program, silu_mul=True)
+            buf, y = guarded_empty((B, inter), dtype)
+            run_gemm(name, x, w, ws, program, silu_mul=True, out=y)
             torch.cuda.synchronize()
             ok, info = diff_info(y, exp, 2e-2, 2e-2)
-            report(name + " [fused silu*mul vs oracle]", ok and tuple(y.shape) == (B, inter), info)
-        finally:
-            for k, v in old.items():
-                if v is None:
-                    os.environ.pop(k, None)
-                else:
-                    os.environ[k] = v
+            report(name + " [fused silu*mul vs oracle]", ok, info)
+            report_bands(name, buf)
     guard(name, fn)
 
 

@@ -64,13 +64,20 @@ ATTN_CASES = [
     ("cluster merge 8 splits g16", 2, 16, 1, 64, [500, 1], torch.float16, {"B200_ATTN_TILES_PER_SPLIT": 1}),
     ("cluster merge 2 splits bf16 p16", 4, 8, 2, 16, [10, 20, 65, 128], torch.bfloat16, {"B200_ATTN_TILES_PER_SPLIT": 1}),
     ("cluster merge 3 splits mha p32", 3, 4, 4, 32, [64, 65, 190], torch.float16, {"B200_ATTN_TILES_PER_SPLIT": 1}),
+    # attention.py passes q_scale = 1 / q_scaling
+    ("q_scale 0.5", 4, 8, 2, 64, [65, 128, 200, 513], torch.float16, None, dict(q_scale=0.5)),
+    ("q_scale 1/1.3 bf16 cluster merge", 3, 8, 2, 64, [63, 64, 700], torch.bfloat16, {"B200_ATTN_TILES_PER_SPLIT": 2},
+     dict(q_scale=1 / 1.3)),
+    # callers pass a loose bound on the lengths, and the split plan follows the bound, not the lengths
+    ("max_seq_len 4096", 3, 8, 2, 64, [100, 700, 1500], torch.float16, None, dict(max_len=4096)),
+    ("max_seq_len 8192 lengths 1..70", 70, 8, 2, 64, list(range(1, 71)), torch.bfloat16, None, dict(max_len=8192)),
 ]
 
 
 @pytest.mark.parametrize("case", ATTN_CASES, ids=[c[0] for c in ATTN_CASES])
 def test_attention_vs_oracle(case):
-    name, B, Hq, Hkv, T, lens, dtype, env = case
-    _run(probe.attn_vs_oracle, name, B, Hq, Hkv, T, lens, dtype, env)
+    name, B, Hq, Hkv, T, lens, dtype, env, *kw = case
+    _run(probe.attn_vs_oracle, name, B, Hq, Hkv, T, lens, dtype, env, **(kw[0] if kw else {}))
 
 
 HEAD_DIMS = [
@@ -104,13 +111,10 @@ MULTI_Q = [
 @pytest.mark.parametrize("case", MULTI_Q, ids=[c[0] for c in MULTI_Q])
 def test_attention_with_several_query_tokens_vs_oracle(case):
     """q_len speculative tokens per sequence (XQA max_q_len / trtllm-gen q_len_per_req): query j must equal a plain decode
-    attention over the first sequence_lengths + j + 1 positions (the oracle, one call per j)."""
+    attention over the first sequence_lengths + j + 1 positions. Checked against the float64 reference within the error
+    budget, with the C oracle (one call per j) as a second opinion at 1e-2 (bf16: 2e-2)."""
     name, B, q_len, Hq, Hkv, T, lens, dtype, env = case          # lens = tokens cached BEFORE the q_len new ones
-    old = {}
-    for k, v in (env or {}).items():
-        old[k] = os.environ.get(k)
-        os.environ[k] = str(v)
-    try:
+    with probe.env_set(env):
         dev = torch.device("cuda")
         is_bf16 = dtype == torch.bfloat16
         total = [L + q_len for L in lens]
@@ -121,8 +125,17 @@ def test_attention_with_several_query_tokens_vs_oracle(case):
         pl = ops.convert_block_table(block_ids.to(dev))
         max_len = max(total)
         ws = ops.attn_workspace(B * q_len, Hq, Hkv, max_len, dev)
-        out = ops.paged_decode_attn_multi(q.to(dev), pool.to(dev), pl, seq.to(dev), max_len, ws)
+        buf, out = probe.guarded_empty((B, q_len, Hq * 128), dtype)
+        ops.paged_decode_attn_multi(q.to(dev), pool.to(dev), pl, seq.to(dev), max_len, ws, out=out)
         torch.cuda.synchronize()
+        probe.RESULTS.clear()
+        f64, E = orc.paged_decode_attn_np(q.float().numpy(), pool.float().numpy(), block_ids.numpy(), seq.numpy(), T,
+                                          with_abs=True)
+        ok, info = probe.budget_info(out, f64, E, is_bf16)
+        probe.report(name + " [kernel vs float64, error budget]", ok, info)
+        probe.report_bands(name, buf)
+        bad = [n for n, ok in probe.RESULTS if not ok]
+        assert not bad, bad
         bits = lambda t: t.contiguous().view(torch.int16).numpy().view(np.uint16)
         pl_np = orc.convert_block_table(block_ids.numpy())
         tol = 2e-2 if is_bf16 else 1e-2
@@ -130,20 +143,44 @@ def test_attention_with_several_query_tokens_vs_oracle(case):
             exp = orc.from_bits(orc.paged_decode_attn(bits(q[:, j]), bits(pool), pl_np, (seq + j).numpy(), Hq, Hkv, 128, T,
                                                       is_bf16=is_bf16), is_bf16)
             np.testing.assert_allclose(out[:, j].float().cpu().numpy(), exp, rtol=tol, atol=tol, err_msg=f"query token {j}")
-    finally:
-        for k, v in old.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
 
 
-@pytest.mark.parametrize("cfg", [("Llama-3-8B B32 S2048", 32, 32, 8, 64, 2048, False),
-                                 ("Llama-3-8B B32 S2048 ragged", 32, 32, 8, 64, 2048, True),
-                                 ("Qwen2-72B TP8 B16 S8192", 16, 8, 1, 64, 8192, False)], ids=lambda c: c[0])
+@pytest.mark.parametrize("cfg", [("Llama-3-8B B32 S2048", 32, 32, 8, 64, 2048, False, torch.float16),
+                                 ("Llama-3-8B B32 S2048 ragged", 32, 32, 8, 64, 2048, True, torch.float16),
+                                 ("Llama-3-8B B32 S2048 bf16", 32, 32, 8, 64, 2048, False, torch.bfloat16),
+                                 ("Qwen2-72B TP8 B16 S8192", 16, 8, 1, 64, 8192, False, torch.float16),
+                                 ("Qwen2-72B TP8 B16 S8192 bf16", 16, 8, 1, 64, 8192, False, torch.bfloat16)],
+                         ids=lambda c: c[0])
 def test_attention_full_size_vs_oracle(cfg):
-    name, B, Hq, Hkv, T, S, ragged = cfg
-    _run(probe.attn_vs_ref_big, name, B, Hq, Hkv, T, S, torch.float16, ragged)
+    name, B, Hq, Hkv, T, S, ragged, dtype = cfg
+    _run(probe.attn_vs_ref_big, name, B, Hq, Hkv, T, S, dtype, ragged)
+
+
+POSITION_PROBES = [
+    # name, head_dim, B, q_len, Hq, Hkv, page, lens (cached before the new tokens), dtype, env, max_seq_len
+    ("p16 g4", 128, 4, 1, 8, 2, 16, [0, 15, 16, 130], torch.float16, None, None),
+    ("p32 mha d64 bf16", 64, 3, 1, 4, 4, 32, [31, 32, 200], torch.bfloat16, None, None),
+    ("p64 g8 d256", 256, 3, 1, 16, 2, 64, [63, 64, 513], torch.float16, None, None),
+    ("p128 g16 bf16", 128, 3, 1, 16, 1, 128, [127, 128, 300], torch.bfloat16, None, None),
+    ("cluster merge 8 splits g4", 128, 2, 1, 8, 2, 64, [500, 65], torch.float16, {"B200_ATTN_TILES_PER_SPLIT": 1}, None),
+    ("cluster merge 4 splits d64 p16 bf16", 64, 3, 1, 8, 2, 16, [130, 400, 7], torch.bfloat16,
+     {"B200_ATTN_TILES_PER_SPLIT": 2}, None),
+    ("workspace merge g8 p32 bf16", 128, 2, 1, 16, 2, 32, [900, 70], torch.bfloat16, {"B200_ATTN_TILES_PER_SPLIT": 1}, None),
+    ("workspace merge d256 g4 p16", 256, 2, 1, 4, 1, 16, [600, 3], torch.float16, {"B200_ATTN_TILES_PER_SPLIT": 1}, None),
+    ("max_seq_len 8192 lengths 1..70", 128, 70, 1, 8, 2, 64, list(range(0, 70)), torch.float16, None, 8192),
+    ("q_len 4 g4 p64", 128, 3, 4, 8, 2, 64, [10, 60, 300], torch.float16, None, None),
+    ("q_len 2 g8 p16 bf16 workspace merge", 128, 2, 2, 16, 2, 16, [900, 17], torch.bfloat16,
+     {"B200_ATTN_TILES_PER_SPLIT": 1}, None),
+    ("q_len 16 mha p32 cluster merge", 128, 2, 16, 2, 2, 32, [60, 300], torch.float16, {"B200_ATTN_TILES_PER_SPLIT": 2}, None),
+]
+
+
+@pytest.mark.parametrize("case", POSITION_PROBES, ids=[c[0] for c in POSITION_PROBES])
+def test_attention_reads_exactly_the_visible_positions(case):
+    """Exact probes (uniform scores, dominant key): an output off by one token, page, kv head or batch row fails at any
+    sequence length, where a tolerance check would lose it in the average."""
+    name, D, B, q_len, Hq, Hkv, T, lens, dtype, env, max_len = case
+    _run(probe.attn_position_probes, name, B, Hq, Hkv, T, lens, dtype, env, D=D, q_len=q_len, max_len=max_len)
 
 
 ROPE_FUSED = [
@@ -199,6 +236,23 @@ GEMM_SMALL = [
     ("ragged N bpad64", 33, 512, 200, {}),
     ("bpad128", 100, 512, 256, {}),
     ("bf16", 8, 256, 256, dict(dtype=torch.bfloat16)),
+    # uneven cluster split-K (runs 3, 3, 2), and 8 splits forced on 3 k-blocks (clamped to 3 single-block runs)
+    ("splitk3 bias", 19, 1024, 384, dict(env={"B200_GEMM_SPLITK": 3}, bias=True)),
+    ("splitk8 clamped K384", 32, 384, 256, dict(env={"B200_GEMM_SPLITK": 8})),
+    # one split over 25 k-blocks: an odd run that wraps every stage ring more than twice, at every batch pad
+    ("ring wrap B1", 1, 3200, 256, dict(env={"B200_GEMM_SPLITK": 1})),
+    ("ring wrap B17", 17, 3200, 256, dict(env={"B200_GEMM_SPLITK": 1})),
+    ("ring wrap B64", 64, 3200, 256, dict(env={"B200_GEMM_SPLITK": 1})),
+    ("ring wrap B128", 128, 3200, 256, dict(env={"B200_GEMM_SPLITK": 1})),
+    ("ring wrap B17 bf16", 17, 3200, 256, dict(env={"B200_GEMM_SPLITK": 1}, dtype=torch.bfloat16)),
+    # batch pad edges (16 | 17, 64 | 65), single-request decode, the largest batch, and a last tile of 8 features
+    ("B1", 1, 512, 256, {}),
+    ("B16", 16, 512, 256, {}),
+    ("B17", 17, 512, 256, {}),
+    ("B64", 64, 512, 256, {}),
+    ("B65", 65, 512, 256, {}),
+    ("B128", 128, 512, 256, {}),
+    ("N136", 17, 512, 136, {}),
 ]
 
 
@@ -226,9 +280,13 @@ def test_gemm_full_size_vs_oracle(cfg):
 PERSISTENT = [
     ("uniform split", B200_FMT_INT4, 32, 1024, 256, {}),
     ("uniform split bias int8", B200_FMT_INT8, 19, 1024, 384, dict(bias=True)),
-    ("whole tiles bf16", B200_FMT_INT4, 8, 256, 256, dict(dtype=torch.bfloat16)),
+    ("2-way split bf16", B200_FMT_INT4, 8, 256, 256, dict(dtype=torch.bfloat16)),
     ("ragged N bpad64", B200_FMT_INT4, 33, 512, 200, {}),
     ("Llama w2 B32", B200_FMT_INT4, 32, 14336, 4096, dict(big=True)),
+    ("16 contributors", B200_FMT_INT4, 32, 2048, 128, {}),
+    ("whole tiles", B200_FMT_INT4, 8, 128, 256, {}),
+    ("several tiles per CTA int8", B200_FMT_INT8, 8, 256, 76800, {}),
+    ("workspace for B16 forces longer runs", B200_FMT_INT4, 40, 1024, 256, dict(ws_batch=16)),
 ]
 
 
@@ -236,7 +294,12 @@ PERSISTENT = [
 def test_gemm_persistent_kernel_standalone(case):
     """The persistent kernel of the decode programs (csrc/decode_program.cuh) run as a one-op program: split tiles merged
     by all their contributors, and whole tiles stored directly. The probe checks that the GEMM was recorded as an op of the
-    persistent kernel, not replayed through the cluster kernel."""
+    persistent kernel, not replayed through the cluster kernel.
+
+    The last four shapes reach the branches of the run-length plan (sk_plan in c_api.cu) for any grid of 16 to 2 x 132
+    CTAs: one tile of 16 k-blocks is split 16 ways (the merge loop over contributors 8..15); one k-block per tile gives
+    whole tiles; 600 tiles of 2 k-blocks give each CTA several whole tiles, and at 264 CTAs leave 64 of them idle; a
+    workspace sized for batch 16 cannot hold the 8 partials of batch pad 64, so the plan falls back to 2 runs of 4."""
     name, fmt, B, K, N, kw = case
     _run(probe.gemm_case, name, fmt, B, K, N, program=True, **kw)
     _run(probe.gemm_silu_case, name + " silu", fmt, 7, 512, 192, program=True)
