@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <array>
 #include <atomic>
 #include <cmath>
 #include <cstdarg>
@@ -73,44 +74,11 @@ int num_sms() {
     return sms[dev];
 }
 
-int seg_dispatch_f16(int bpad, int qfmt, const ProgOp* d_ops, int nops, unsigned* gbar, int grid, bool pdl,
-                     unsigned long long* trace, cudaStream_t st, int* grid_out);
-int seg_dispatch_bf16(int bpad, int qfmt, const ProgOp* d_ops, int nops, unsigned* gbar, int grid, bool pdl,
-                      unsigned long long* trace, cudaStream_t st, int* grid_out);
-
-int segment_grid(bool bf16, int bpad, int qfmt, int* grid_out) {
-    return bf16 ? seg_dispatch_bf16(bpad, qfmt, nullptr, 0, nullptr, 0, false, nullptr, nullptr, grid_out)
-                : seg_dispatch_f16(bpad, qfmt, nullptr, 0, nullptr, 0, false, nullptr, nullptr, grid_out);
-}
-int launch_segment(bool bf16, int bpad, int qfmt, const ProgOp* d_ops, int nops, unsigned* gbar, int grid, bool pdl,
-                   unsigned long long* trace, cudaStream_t st) {
-    return bf16 ? seg_dispatch_bf16(bpad, qfmt, d_ops, nops, gbar, grid, pdl, trace, st, nullptr)
-                : seg_dispatch_f16(bpad, qfmt, d_ops, nops, gbar, grid, pdl, trace, st, nullptr);
-}
-
 }  // namespace b200_host
 
 namespace {
 
 std::atomic<int> g_pdl{0};
-
-// Launch through cudaLaunchKernelEx so a kernel can carry the programmatic-dependent-launch attribute: it may then be
-// scheduled while its predecessor drains (every kernel of the decode chain executes griddepcontrol.wait before it
-// touches dependent data, so this only overlaps launch latency, prologues and -- for the GEMM -- the weight prefetch).
-template <typename... KArgs, typename... Args>
-cudaError_t launch_ex(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl, Args... args) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = grid;
-    cfg.blockDim = block;
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
-}
 
 // ---- cuTensorMapEncodeTiled through the runtime (no link-time dependency on libcuda)
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -181,6 +149,17 @@ void attn_split(int units, int max_tiles, int* nsplit, int* tiles_per_split, int
     *tiles_per_split = best_c;
 }
 
+// Workspace of a launch whose splits merge through L2 (more than 8 splits): [sem][ml][o], one counter per (sequence, kv head),
+// then a running max / sum and a partial output per (query row, split).
+struct AttnWorkspace {
+    size_t sem, ml, o;
+};
+AttnWorkspace attn_workspace(size_t batch, size_t head_num, size_t kv_head_num, size_t q_len, size_t nsplit, size_t head_dim) {
+    const size_t slots = batch * head_num * q_len * nsplit;
+    return {round_up(batch * kv_head_num * sizeof(int), 256), round_up(slots * 2 * sizeof(float), 256),
+            slots * head_dim * sizeof(float)};
+}
+
 // ---- GEMM launch shape
 int gemm_bpad(int B) { return B <= 16 ? 16 : (B <= 32 ? 32 : (B <= 64 ? 64 : 128)); }
 // one-kernel-per-GEMM path (gemm_cluster.cu): split-K so that one wave of 2*SMs CTAs is filled. The nsplit CTAs of a tile
@@ -234,6 +213,46 @@ int sk_plan(int n_tiles, int k_blocks, int grid, int bpad, size_t ws_partial_byt
 size_t sk_ws_bytes(int n_tiles, int k_blocks, int grid, int bpad) {
     const int per = sk_plan(n_tiles, k_blocks, grid, bpad, (size_t)-1);
     return per < k_blocks ? (size_t)n_tiles * (k_blocks / per) * bpad * kGemmTileN * sizeof(float) : 0;
+}
+
+// ---- peer regions
+// A rank's peer-visible region: [2 parities][2 areas (one-shot / reduce-scatter, all-gather)][W sources][LL slot = 2 x message],
+// then the per-CTA epochs at 2 * parity.
+struct PeerStrides {
+    size_t src, area, parity;
+};
+PeerStrides peer_strides(size_t max_message_bytes) {
+    const size_t src = 2 * round_up(max_message_bytes, 256);   // LL doubles the bytes
+    return {src, (size_t)kArMaxWorld * src, 2 * (size_t)kArMaxWorld * src};
+}
+
+bool valid_peer_group(int rank, int world) { return world >= 2 && world <= kArMaxWorld && rank >= 0 && rank < world; }
+
+// The region pointers, epoch and strides of a peer kernel's parameters (PeerArParams and the GEMM's RsPush share the names).
+template <typename P>
+int set_peers(P& p, const char* who, void* const* regions, size_t max_message_bytes, int rank, int world) {
+    const PeerStrides s = peer_strides(max_message_bytes);
+    for (int r = 0; r < world; ++r) {
+        ARG_CHECK(regions[r], "%s: region %d is null", who, r);
+        p.region[r] = reinterpret_cast<uint8_t*>(regions[r]);
+    }
+    p.epoch = reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(regions[rank]) + 2 * s.parity);
+    p.src_stride = s.src;
+    p.parity_stride = s.parity;
+    p.rank = rank;
+    p.world = world;
+    return B200_OK;
+}
+int fill_ar_params(PeerArParams& p, void* const* regions, size_t max_message_bytes, int rank, int world) {
+    p.area_stride = peer_strides(max_message_bytes).area;
+    return set_peers(p, "peer collective", regions, max_message_bytes, rank, world);
+}
+
+// A recorded peer call keeps its own copy of the region list: the caller's array need not outlive the recording.
+std::array<void*, kArMaxWorld> copy_regions(void* const* regions, int world) {
+    std::array<void*, kArMaxWorld> c{};
+    std::copy(regions, regions + world, c.begin());
+    return c;
 }
 
 }  // namespace
@@ -381,44 +400,9 @@ int b200_paged_attn_plan(const int32_t* input_lengths, const int32_t* sequence_l
 size_t b200_paged_decode_attn_workspace_bytes(size_t batch, size_t head_num, size_t kv_head_num, size_t max_seq_len) {
     size_t tiles = (max_seq_len + kAttnTile - 1) / kAttnTile;
     size_t ns = tiles < (size_t)kAttnMaxSplit ? (tiles ? tiles : 1) : (size_t)kAttnMaxSplit;
-    size_t sem = round_up(batch * kv_head_num * sizeof(int), 256);
-    size_t ml = round_up(batch * head_num * ns * 2 * sizeof(float), 256);
-    size_t o = batch * head_num * ns * 256 * sizeof(float);      // sized for the largest head_dim (256)
-    return sem + ml + o;
-}
-
-static int attn_impl(const void* q, const void* qkv, float rope_base, int q_len, int is_bf16, void* out, size_t head_num, size_t kv_head_num,
-                     size_t head_dim, size_t batch, size_t max_blocks_per_seq, size_t max_seq_len, size_t page_size, const void* kv_pool,
-                     const int32_t* page_list, const uint32_t* sequence_lengths, float q_scale, void* workspace, size_t workspace_bytes,
-                     void* stream);
-
-int b200_paged_decode_attn(const void* q, int is_bf16, void* out, size_t head_num, size_t kv_head_num, size_t head_dim,
-                           size_t batch, size_t max_blocks_per_seq, size_t max_seq_len, size_t page_size,
-                           const void* kv_pool, const int32_t* page_list, const uint32_t* sequence_lengths,
-                           float q_scale, void* workspace, size_t workspace_bytes, void* stream) {
-    ARG_CHECK(q || batch == 0, "paged_decode_attn: null pointer");
-    return attn_impl(q, nullptr, 0.f, 1, is_bf16, out, head_num, kv_head_num, head_dim, batch, max_blocks_per_seq, max_seq_len, page_size,
-                     kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, stream);
-}
-
-int b200_paged_decode_attn_multi(const void* q, int is_bf16, void* out, size_t head_num, size_t kv_head_num, size_t head_dim,
-                                 size_t batch, size_t q_len, size_t max_blocks_per_seq, size_t max_seq_len, size_t page_size,
-                                 const void* kv_pool, const int32_t* page_list, const uint32_t* sequence_lengths, float q_scale,
-                                 void* workspace, size_t workspace_bytes, void* stream) {
-    ARG_CHECK(q || batch == 0, "paged_decode_attn_multi: null pointer");
-    ARG_CHECK(q_len >= 1 && q_len <= 16, "paged_decode_attn_multi: q_len %zu unsupported", q_len);
-    return attn_impl(q, nullptr, 0.f, (int)q_len, is_bf16, out, head_num, kv_head_num, head_dim, batch, max_blocks_per_seq, max_seq_len,
-                     page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, stream);
-}
-
-int b200_paged_decode_attn_rope(const void* qkv, int is_bf16, void* out, size_t head_num, size_t kv_head_num, size_t head_dim,
-                                size_t batch, size_t max_blocks_per_seq, size_t max_seq_len, size_t page_size, void* kv_pool,
-                                const int32_t* page_list, const uint32_t* sequence_lengths, float q_scale, float rope_base,
-                                void* workspace, size_t workspace_bytes, void* stream) {
-    ARG_CHECK(qkv || batch == 0, "paged_decode_attn_rope: null pointer");
-    ARG_CHECK(rope_base > 1.f, "paged_decode_attn_rope: rope_base must be > 1");
-    return attn_impl(nullptr, qkv, rope_base, 1, is_bf16, out, head_num, kv_head_num, head_dim, batch, max_blocks_per_seq, max_seq_len,
-                     page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, stream);
+    // sized for one query row per sequence and the largest head_dim (256)
+    const AttnWorkspace w = attn_workspace(batch, head_num, kv_head_num, 1, ns, 256);
+    return w.sem + w.ml + w.o;
 }
 
 static int attn_impl(const void* q, const void* qkv, float rope_base, int q_len, int is_bf16, void* out, size_t head_num, size_t kv_head_num,
@@ -469,16 +453,13 @@ static int attn_impl(const void* q, const void* qkv, float rope_base, int q_len,
     const int max_tiles = (int)((max_seq_len + kAttnTile - 1) / kAttnTile);
     attn_split((int)(batch * kv_head_num), max_tiles, &p.nsplit, &p.tiles_per_split, (int)head_dim);
 
-    // workspace carve-up: [sem][ml][o]
-    const size_t sem_b = round_up(batch * kv_head_num * sizeof(int), 256);
-    const size_t ml_b = round_up(batch * head_num * q_len * (size_t)p.nsplit * 2 * sizeof(float), 256);
-    const size_t o_b = batch * head_num * q_len * (size_t)p.nsplit * head_dim * sizeof(float);
     if (p.nsplit > 8) {
-        ARG_CHECK(workspace && workspace_bytes >= sem_b + ml_b + o_b,
-                  "paged_decode_attn: workspace too small (%zu < %zu)", workspace_bytes, sem_b + ml_b + o_b);
+        const AttnWorkspace w = attn_workspace(batch, head_num, kv_head_num, q_len, p.nsplit, head_dim);
+        ARG_CHECK(workspace && workspace_bytes >= w.sem + w.ml + w.o,
+                  "paged_decode_attn: workspace too small (%zu < %zu)", workspace_bytes, w.sem + w.ml + w.o);
         p.sem = reinterpret_cast<int*>(workspace);
-        p.ws_ml = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + sem_b);
-        p.ws_o = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + sem_b + ml_b);
+        p.ws_ml = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + w.sem);
+        p.ws_o = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + w.sem + w.ml);
     }
 
     CUtensorMap map;
@@ -492,51 +473,49 @@ static int attn_impl(const void* q, const void* qkv, float rope_base, int q_len,
     }
     const dim3 grid(p.nsplit, (unsigned)(batch * kv_head_num), 1);
     p.cluster_merge = (p.nsplit >= 2 && p.nsplit <= 8) ? 1 : 0;   // 2..8 splits merge in a cluster, more through the workspace
-    static bool configured_dev[16][6] = {};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    ARG_CHECK(dev >= 0 && dev < 16, "device ordinal %d out of range", dev);
-    auto launch = [&](auto kern, bool& configured, int smem_bytes) -> cudaError_t {
-        if (!configured) {
-            cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
-            if (e != cudaSuccess) return e;
-            configured = true;
-        }
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = grid;
-        cfg.blockDim = dim3(kAttnThreads);
-        cfg.dynamicSmemBytes = smem_bytes;
-        cfg.stream = (cudaStream_t)stream;
-        cudaLaunchAttribute attr[2];
-        int na = 0;
-        if (g_pdl.load() != 0) {
-            attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-            attr[na].val.programmaticStreamSerializationAllowed = 1;
-            ++na;
-        }
-        if (p.cluster_merge) {
-            attr[na].id = cudaLaunchAttributeClusterDimension;
-            attr[na].val.clusterDim.x = (unsigned)p.nsplit;
-            attr[na].val.clusterDim.y = 1;
-            attr[na].val.clusterDim.z = 1;
-            ++na;
-        }
-        cfg.attrs = attr;
-        cfg.numAttrs = na;
-        return cudaLaunchKernelEx(&cfg, kern, map, p);
+    const dim3 cluster(p.cluster_merge ? p.nsplit : 1);
+    auto launch = [&](auto t, auto hd) {
+        constexpr auto kern = paged_decode_attn_kernel<decltype(t), decltype(hd)::value>;
+        const int smem = attn_smem_bytes(decltype(hd)::value);
+        int rc = configure_once<kern>(smem);
+        if (rc) return rc;
+        CUDA_CHECK(launch_ex(kern, {grid, dim3(kAttnThreads), (size_t)smem, (cudaStream_t)stream, g_pdl.load() != 0, cluster}, map, p));
+        return launched("paged_decode_attn_kernel");
     };
-    const int di = head_dim == 64 ? 0 : (head_dim == 128 ? 1 : 2);
-    bool& configured = configured_dev[dev][di * 2 + (is_bf16 ? 1 : 0)];
-    if (is_bf16) {
-        if (di == 0) CUDA_CHECK(launch(paged_decode_attn_kernel<__nv_bfloat16, 64>, configured, attn_smem_bytes(64)));
-        else if (di == 1) CUDA_CHECK(launch(paged_decode_attn_kernel<__nv_bfloat16, 128>, configured, attn_smem_bytes(128)));
-        else CUDA_CHECK(launch(paged_decode_attn_kernel<__nv_bfloat16, 256>, configured, attn_smem_bytes(256)));
-    } else {
-        if (di == 0) CUDA_CHECK(launch(paged_decode_attn_kernel<__half, 64>, configured, attn_smem_bytes(64)));
-        else if (di == 1) CUDA_CHECK(launch(paged_decode_attn_kernel<__half, 128>, configured, attn_smem_bytes(128)));
-        else CUDA_CHECK(launch(paged_decode_attn_kernel<__half, 256>, configured, attn_smem_bytes(256)));
-    }
-    return launched("paged_decode_attn_kernel");
+    return by_dtype(is_bf16, [&](auto t) {
+        if (head_dim == 64) return launch(t, std::integral_constant<int, 64>());
+        if (head_dim == 128) return launch(t, std::integral_constant<int, 128>());
+        return launch(t, std::integral_constant<int, 256>());
+    });
+}
+
+int b200_paged_decode_attn(const void* q, int is_bf16, void* out, size_t head_num, size_t kv_head_num, size_t head_dim,
+                           size_t batch, size_t max_blocks_per_seq, size_t max_seq_len, size_t page_size,
+                           const void* kv_pool, const int32_t* page_list, const uint32_t* sequence_lengths,
+                           float q_scale, void* workspace, size_t workspace_bytes, void* stream) {
+    ARG_CHECK(q || batch == 0, "paged_decode_attn: null pointer");
+    return attn_impl(q, nullptr, 0.f, 1, is_bf16, out, head_num, kv_head_num, head_dim, batch, max_blocks_per_seq, max_seq_len, page_size,
+                     kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, stream);
+}
+
+int b200_paged_decode_attn_multi(const void* q, int is_bf16, void* out, size_t head_num, size_t kv_head_num, size_t head_dim,
+                                 size_t batch, size_t q_len, size_t max_blocks_per_seq, size_t max_seq_len, size_t page_size,
+                                 const void* kv_pool, const int32_t* page_list, const uint32_t* sequence_lengths, float q_scale,
+                                 void* workspace, size_t workspace_bytes, void* stream) {
+    ARG_CHECK(q || batch == 0, "paged_decode_attn_multi: null pointer");
+    ARG_CHECK(q_len >= 1 && q_len <= 16, "paged_decode_attn_multi: q_len %zu unsupported", q_len);
+    return attn_impl(q, nullptr, 0.f, (int)q_len, is_bf16, out, head_num, kv_head_num, head_dim, batch, max_blocks_per_seq, max_seq_len,
+                     page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, stream);
+}
+
+int b200_paged_decode_attn_rope(const void* qkv, int is_bf16, void* out, size_t head_num, size_t kv_head_num, size_t head_dim,
+                                size_t batch, size_t max_blocks_per_seq, size_t max_seq_len, size_t page_size, void* kv_pool,
+                                const int32_t* page_list, const uint32_t* sequence_lengths, float q_scale, float rope_base,
+                                void* workspace, size_t workspace_bytes, void* stream) {
+    ARG_CHECK(qkv || batch == 0, "paged_decode_attn_rope: null pointer");
+    ARG_CHECK(rope_base > 1.f, "paged_decode_attn_rope: rope_base must be > 1");
+    return attn_impl(nullptr, qkv, rope_base, 1, is_bf16, out, head_num, kv_head_num, head_dim, batch, max_blocks_per_seq, max_seq_len,
+                     page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ GEMM
@@ -600,44 +579,10 @@ size_t b200_wo_gemm_workspace_bytes(int max_batch, int N, int K) {
     return kGemmSemBytes + sk_ws_bytes(n_tiles, K / kGemmBK, 2 * num_sms(), gemm_bpad(max_batch));
 }
 
-namespace {
-struct RsDesc {
-    void* regions[kArMaxWorld];
-    size_t max_message_bytes;
-    int rank, world;
-};
-int wo_gemm_impl(int fmt, int is_bf16, const void* x, int B, int K, int N, const void* w, const void* col_scale,
-                 const void* bias, void* y, void* workspace, size_t workspace_bytes, int flags, const RsDesc* rs, void* stream);
-int fill_ar_params(PeerArParams& p, void* const* regions, size_t max_message_bytes, int rank, int world);
-}  // namespace
-
-int b200_wo_gemm(int fmt, int is_bf16, const void* x, int B, int K, int N, const void* w, const void* col_scale,
-                 const void* bias, void* y, void* workspace, size_t workspace_bytes, int flags, void* stream) {
-    return wo_gemm_impl(fmt, is_bf16, x, B, K, N, w, col_scale, bias, y, workspace, workspace_bytes, flags, nullptr, stream);
-}
-
-int b200_wo_gemm_rs(int fmt, int is_bf16, const void* x, int B, int K, int N, const void* w, const void* col_scale,
-                    const void* bias, void* y, void* workspace, size_t workspace_bytes, int flags, void* const* regions,
-                    size_t max_message_bytes, int rank, int world, void* stream) {
-    ARG_CHECK(regions, "wo_gemm_rs: null regions");
-    ARG_CHECK(world >= 2 && world <= kArMaxWorld && rank >= 0 && rank < world, "wo_gemm_rs: bad rank/world %d/%d", rank, world);
-    ARG_CHECK(N % 128 == 0 && N % (8 * world) == 0 && N <= 8192, "wo_gemm_rs: N=%d must be a multiple of 128 and of 8*world, <= 8192", N);
-    ARG_CHECK((size_t)B * N * 2 <= max_message_bytes, "wo_gemm_rs: message of %zu bytes exceeds the region", (size_t)B * N * 2);
-    ARG_CHECK(!(flags & B200_GEMM_SILU_MUL), "wo_gemm_rs: SILU_MUL cannot be combined with the reduce-scatter push");
-    RsDesc d{};
-    for (int r = 0; r < world; ++r) {
-        ARG_CHECK(regions[r], "wo_gemm_rs: region %d is null", r);
-        d.regions[r] = regions[r];
-    }
-    d.max_message_bytes = max_message_bytes;
-    d.rank = rank;
-    d.world = world;
-    return wo_gemm_impl(fmt, is_bf16, x, B, K, N, w, col_scale, bias, y, workspace, workspace_bytes, flags, &d, stream);
-}
-
-namespace {
-int wo_gemm_impl(int fmt, int is_bf16, const void* x, int B, int K, int N, const void* w, const void* col_scale,
-                 const void* bias, void* y, void* workspace, size_t workspace_bytes, int flags, const RsDesc* rs, void* stream) {
+// rs: the reduce-scatter push of b200_wo_gemm_rs, or null
+static int wo_gemm_impl(int fmt, int is_bf16, const void* x, int B, int K, int N, const void* w, const void* col_scale,
+                        const void* bias, void* y, void* workspace, size_t workspace_bytes, int flags, const RsPush* rs,
+                        void* stream) {
     if (B == 0) return B200_OK;
     ARG_CHECK(fmt == B200_FMT_F16 || fmt == B200_FMT_INT8 || fmt == B200_FMT_INT4 || fmt == B200_FMT_INT8G,
               "wo_gemm: unknown weight format %d", fmt);
@@ -670,7 +615,7 @@ int wo_gemm_impl(int fmt, int is_bf16, const void* x, int B, int K, int N, const
     if (g_rec && seg_capable && !rs) {
         ARG_CHECK(workspace && workspace_bytes >= kGemmSemBytes, "wo_gemm: workspace of at least %zu bytes required", kGemmSemBytes);
         int grid = 0;
-        int rc = segment_grid(is_bf16 != 0, bpad, fmt, &grid);
+        int rc = by_dtype(is_bf16, [&](auto t) { return segment_grid<decltype(t)>(bpad, fmt, &grid); });
         if (rc) return rc;
         ProgOp op{};
         op.xmap = xmap;
@@ -694,14 +639,11 @@ int wo_gemm_impl(int fmt, int is_bf16, const void* x, int B, int K, int N, const
         return rec_segment_op(op, is_bf16 ? 1 : 0, bpad, fmt);
     }
     if (g_rec) {
-        if (rs) {
-            const RsDesc d = *rs;
-            return rec_call([=](void* st) {
-                return wo_gemm_impl(fmt, is_bf16, x, B, K, N, w, col_scale, bias, y, workspace, workspace_bytes, flags, &d, st);
-            });
-        }
+        const bool has_rs = rs != nullptr;
+        const RsPush d = has_rs ? *rs : RsPush{};
         return rec_call([=](void* st) {
-            return b200_wo_gemm(fmt, is_bf16, x, B, K, N, w, col_scale, bias, y, workspace, workspace_bytes, flags, st);
+            return wo_gemm_impl(fmt, is_bf16, x, B, K, N, w, col_scale, bias, y, workspace, workspace_bytes, flags,
+                                has_rs ? &d : nullptr, st);
         });
     }
 
@@ -731,20 +673,30 @@ int wo_gemm_impl(int fmt, int is_bf16, const void* x, int B, int K, int N, const
     if (rs) {
         GemmParamsRs prs{};
         static_cast<GemmParams&>(prs) = p;
-        PeerArParams ap{};
-        int rc = fill_ar_params(ap, rs->regions, rs->max_message_bytes, rs->rank, rs->world);
-        if (rc) return rc;
-        for (int r = 0; r < rs->world; ++r) prs.rs.region[r] = ap.region[r];
-        prs.rs.epoch = ap.epoch;
-        prs.rs.src_stride = ap.src_stride;
-        prs.rs.parity_stride = ap.parity_stride;
-        prs.rs.rank = rs->rank;
-        prs.rs.world = rs->world;
+        prs.rs = *rs;
         return launch_cluster_gemm_rs(fmt, is_bf16 != 0, bpad, xmap, wmap, prs, n_tiles, (cudaStream_t)stream);
     }
     return launch_cluster_gemm(fmt, is_bf16 != 0, bpad, xmap, wmap, p, n_tiles, (cudaStream_t)stream);
 }
-}  // namespace
+
+int b200_wo_gemm(int fmt, int is_bf16, const void* x, int B, int K, int N, const void* w, const void* col_scale,
+                 const void* bias, void* y, void* workspace, size_t workspace_bytes, int flags, void* stream) {
+    return wo_gemm_impl(fmt, is_bf16, x, B, K, N, w, col_scale, bias, y, workspace, workspace_bytes, flags, nullptr, stream);
+}
+
+int b200_wo_gemm_rs(int fmt, int is_bf16, const void* x, int B, int K, int N, const void* w, const void* col_scale,
+                    const void* bias, void* y, void* workspace, size_t workspace_bytes, int flags, void* const* regions,
+                    size_t max_message_bytes, int rank, int world, void* stream) {
+    ARG_CHECK(regions, "wo_gemm_rs: null regions");
+    ARG_CHECK(valid_peer_group(rank, world), "wo_gemm_rs: bad rank/world %d/%d", rank, world);
+    ARG_CHECK(N % 128 == 0 && N % (8 * world) == 0 && N <= 8192, "wo_gemm_rs: N=%d must be a multiple of 128 and of 8*world, <= 8192", N);
+    ARG_CHECK((size_t)B * N * 2 <= max_message_bytes, "wo_gemm_rs: message of %zu bytes exceeds the region", (size_t)B * N * 2);
+    ARG_CHECK(!(flags & B200_GEMM_SILU_MUL), "wo_gemm_rs: SILU_MUL cannot be combined with the reduce-scatter push");
+    RsPush rs{};
+    int rc = set_peers(rs, "wo_gemm_rs", regions, max_message_bytes, rank, world);
+    if (rc) return rc;
+    return wo_gemm_impl(fmt, is_bf16, x, B, K, N, w, col_scale, bias, y, workspace, workspace_bytes, flags, &rs, stream);
+}
 
 // ------------------------------------------------------------------------------------------------ glue ops
 int b200_add_rmsnorm(const void* x, void* residual, const void* gamma, void* y, int is_bf16, int rows, int hidden,
@@ -768,14 +720,12 @@ int b200_add_rmsnorm(const void* x, void* residual, const void* gamma, void* y, 
     const int threads = hidden / 8 >= 512 ? 512 : (hidden / 8 >= 256 ? 256 : 128);
     const size_t smem = (size_t)hidden * sizeof(float);
     const bool pdl = g_pdl.load() != 0;
-    if (is_bf16)
-        CUDA_CHECK(launch_ex(add_rmsnorm_kernel<__nv_bfloat16>, dim3(rows), dim3(threads), smem, (cudaStream_t)stream, pdl,
-                             (const __nv_bfloat16*)x, (__nv_bfloat16*)residual, (const __nv_bfloat16*)gamma,
-                             (__nv_bfloat16*)y, hidden, eps));
-    else
-        CUDA_CHECK(launch_ex(add_rmsnorm_kernel<__half>, dim3(rows), dim3(threads), smem, (cudaStream_t)stream, pdl,
-                             (const __half*)x, (__half*)residual, (const __half*)gamma, (__half*)y, hidden, eps));
-    return launched("add_rmsnorm_kernel");
+    return by_dtype(is_bf16, [&](auto t) {
+        using T = decltype(t);
+        CUDA_CHECK(launch_ex(add_rmsnorm_kernel<T>, {dim3(rows), dim3(threads), smem, (cudaStream_t)stream, pdl}, (const T*)x,
+                             (T*)residual, (const T*)gamma, (T*)y, hidden, eps));
+        return launched("add_rmsnorm_kernel");
+    });
 }
 
 int b200_qk_rmsnorm(void* qkv, const void* q_gamma, const void* k_gamma, const void* q_bias, const void* k_bias, int is_bf16,
@@ -792,14 +742,12 @@ int b200_qk_rmsnorm(void* qkv, const void* q_gamma, const void* k_gamma, const v
     const int units = rows * (head_num + kv_head_num), wpb = 8;
     const dim3 grid((units + wpb - 1) / wpb);
     const bool pdl = g_pdl.load() != 0;
-    if (is_bf16)
-        CUDA_CHECK(launch_ex(qk_rmsnorm_kernel<__nv_bfloat16>, grid, dim3(wpb * 32), 0, (cudaStream_t)stream, pdl, (__nv_bfloat16*)qkv,
-                             (const __nv_bfloat16*)q_gamma, (const __nv_bfloat16*)k_gamma, (const __nv_bfloat16*)q_bias,
-                             (const __nv_bfloat16*)k_bias, rows, head_num, kv_head_num, head_dim, eps));
-    else
-        CUDA_CHECK(launch_ex(qk_rmsnorm_kernel<__half>, grid, dim3(wpb * 32), 0, (cudaStream_t)stream, pdl, (__half*)qkv, (const __half*)q_gamma,
-                             (const __half*)k_gamma, (const __half*)q_bias, (const __half*)k_bias, rows, head_num, kv_head_num, head_dim, eps));
-    return launched("qk_rmsnorm_kernel");
+    return by_dtype(is_bf16, [&](auto t) {
+        using T = decltype(t);
+        CUDA_CHECK(launch_ex(qk_rmsnorm_kernel<T>, {grid, dim3(wpb * 32), 0, (cudaStream_t)stream, pdl}, (T*)qkv, (const T*)q_gamma,
+                             (const T*)k_gamma, (const T*)q_bias, (const T*)k_bias, rows, head_num, kv_head_num, head_dim, eps));
+        return launched("qk_rmsnorm_kernel");
+    });
 }
 
 int b200_silu_and_mul(const void* gate_up, void* y, int is_bf16, int rows, int inter, void* stream) {
@@ -812,13 +760,12 @@ int b200_silu_and_mul(const void* gate_up, void* y, int is_bf16, int rows, int i
     const size_t blocks = (total + threads - 1) / threads;
     const unsigned g = (unsigned)(blocks < 4 * num_sms() * 8 ? blocks : 4 * num_sms() * 8);
     const bool pdl = g_pdl.load() != 0;
-    if (is_bf16)
-        CUDA_CHECK(launch_ex(silu_and_mul_kernel<__nv_bfloat16>, dim3(g), dim3(threads), 0, (cudaStream_t)stream, pdl,
-                             (const __nv_bfloat16*)gate_up, (__nv_bfloat16*)y, rows, inter));
-    else
-        CUDA_CHECK(launch_ex(silu_and_mul_kernel<__half>, dim3(g), dim3(threads), 0, (cudaStream_t)stream, pdl,
-                             (const __half*)gate_up, (__half*)y, rows, inter));
-    return launched("silu_and_mul_kernel");
+    return by_dtype(is_bf16, [&](auto t) {
+        using T = decltype(t);
+        CUDA_CHECK(launch_ex(silu_and_mul_kernel<T>, {dim3(g), dim3(threads), 0, (cudaStream_t)stream, pdl}, (const T*)gate_up, (T*)y,
+                             rows, inter));
+        return launched("silu_and_mul_kernel");
+    });
 }
 
 int b200_rope_append(const void* qkv, void* q_out, void* kv_pool, const int32_t* page_list,
@@ -848,15 +795,13 @@ int b200_rope_append(const void* qkv, void* q_out, void* kv_pool, const int32_t*
     }
     const dim3 grid(batch, head_num + 2 * kv_head_num);
     const bool pdl = g_pdl.load() != 0;
-    if (is_bf16)
-        CUDA_CHECK(launch_ex(rope_append_kernel<__nv_bfloat16>, grid, dim3(head_dim / 2), 0, (cudaStream_t)stream, pdl,
-                             (const __nv_bfloat16*)qkv, (__nv_bfloat16*)q_out, (__nv_bfloat16*)kv_pool, page_list,
-                             sequence_lengths, head_num, kv_head_num, head_dim, (int)max_blocks_per_seq, page_size, l2b));
-    else
-        CUDA_CHECK(launch_ex(rope_append_kernel<__half>, grid, dim3(head_dim / 2), 0, (cudaStream_t)stream, pdl,
-                             (const __half*)qkv, (__half*)q_out, (__half*)kv_pool, page_list, sequence_lengths, head_num,
-                             kv_head_num, head_dim, (int)max_blocks_per_seq, page_size, l2b));
-    return launched("rope_append_kernel");
+    return by_dtype(is_bf16, [&](auto t) {
+        using T = decltype(t);
+        CUDA_CHECK(launch_ex(rope_append_kernel<T>, {grid, dim3(head_dim / 2), 0, (cudaStream_t)stream, pdl}, (const T*)qkv,
+                             (T*)q_out, (T*)kv_pool, page_list, sequence_lengths, head_num, kv_head_num, head_dim,
+                             (int)max_blocks_per_seq, page_size, l2b));
+        return launched("rope_append_kernel");
+    });
 }
 
 int b200_rope_append_ex(const void* qkv, const void* qkv_bias, void* q_out, void* kv_pool, const int32_t* page_list,
@@ -882,17 +827,13 @@ int b200_rope_append_ex(const void* qkv, const void* qkv_bias, void* q_out, void
     const dim3 grid(batch, head_num + 2 * kv_head_num);
     const bool pdl = g_pdl.load() != 0;
     const float2* cache = reinterpret_cast<const float2*>(cos_sin_cache);
-    if (is_bf16)
-        CUDA_CHECK(launch_ex(rope_append_ex_kernel<__nv_bfloat16>, grid, dim3(head_dim / 2), 0, (cudaStream_t)stream, pdl,
-                             (const __nv_bfloat16*)qkv, (const __nv_bfloat16*)qkv_bias, (__nv_bfloat16*)q_out, (__nv_bfloat16*)kv_pool,
-                             page_list, sequence_lengths, position_ids, cache, cache_positions, rc, use_logn_attn, head_num,
-                             kv_head_num, head_dim, max_blocks_per_seq, page_size));
-    else
-        CUDA_CHECK(launch_ex(rope_append_ex_kernel<__half>, grid, dim3(head_dim / 2), 0, (cudaStream_t)stream, pdl, (const __half*)qkv,
-                             (const __half*)qkv_bias, (__half*)q_out, (__half*)kv_pool, page_list, sequence_lengths, position_ids,
-                             cache, cache_positions, rc, use_logn_attn, head_num, kv_head_num, head_dim, max_blocks_per_seq,
-                             page_size));
-    return launched("rope_append_ex_kernel");
+    return by_dtype(is_bf16, [&](auto t) {
+        using T = decltype(t);
+        CUDA_CHECK(launch_ex(rope_append_ex_kernel<T>, {grid, dim3(head_dim / 2), 0, (cudaStream_t)stream, pdl}, (const T*)qkv,
+                             (const T*)qkv_bias, (T*)q_out, (T*)kv_pool, page_list, sequence_lengths, position_ids, cache,
+                             cache_positions, rc, use_logn_attn, head_num, kv_head_num, head_dim, max_blocks_per_seq, page_size));
+        return launched("rope_append_ex_kernel");
+    });
 }
 
 int b200_embedding(const int32_t* ids, const void* table, void* out, int is_bf16, int rows, int hidden, void* stream) {
@@ -920,13 +861,12 @@ int b200_argmax(const void* logits, int dtype, int rows, int vocab, int32_t* out
     ARG_CHECK(vocab > 0, "argmax: vocab must be positive");
     ARG_CHECK(dtype >= 0 && dtype <= 2, "argmax: dtype %d unknown (0 fp16, 1 bf16, 2 fp32)", dtype);
     if (g_rec) return rec_call([=](void* st) { return b200_argmax(logits, dtype, rows, vocab, out, st); });
-    if (dtype == 0)
-        argmax_kernel<__half><<<rows, 1024, 0, (cudaStream_t)stream>>>((const __half*)logits, vocab, out);
-    else if (dtype == 1)
-        argmax_kernel<__nv_bfloat16><<<rows, 1024, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)logits, vocab, out);
-    else
-        argmax_kernel<float><<<rows, 1024, 0, (cudaStream_t)stream>>>((const float*)logits, vocab, out);
-    return launched("argmax_kernel");
+    auto launch = [&](auto t) {
+        using T = decltype(t);
+        argmax_kernel<T><<<rows, 1024, 0, (cudaStream_t)stream>>>((const T*)logits, vocab, out);
+        return launched("argmax_kernel");
+    };
+    return dtype == 2 ? launch(0.f) : by_dtype(dtype == 1, launch);
 }
 
 int b200_sample(float* logits, int rows, int vocab, const int32_t* history, const int32_t* hist_len, int hist_stride,
@@ -962,14 +902,13 @@ int b200_sample(float* logits, int rows, int vocab, const int32_t* history, cons
     p.rows = rows;
     p.vocab = vocab;
     p.hist_stride = hist_stride;
-    CUDA_CHECK(launch_ex(sample_kernel, dim3(rows), dim3(kSampleThreads), 0, (cudaStream_t)stream, g_pdl.load() != 0, p));
+    CUDA_CHECK(launch_ex(sample_kernel, {dim3(rows), dim3(kSampleThreads), 0, (cudaStream_t)stream, g_pdl.load() != 0}, p));
     return launched("sample_kernel");
 }
 
 // ------------------------------------------------------------------------------------------------ peer all-reduce
 size_t b200_peer_ar_region_bytes(size_t max_message_bytes) {
-    // [2 parities][2 areas (one-shot / reduce-scatter, all-gather)][W sources][LL slot = 2 x message] + per-CTA epochs
-    return 2 * 2 * (size_t)kArMaxWorld * 2 * round_up(max_message_bytes, 256) + kArMaxCtas * sizeof(uint32_t) + 256;
+    return 2 * peer_strides(max_message_bytes).parity + kArMaxCtas * sizeof(uint32_t) + 256;
 }
 
 int b200_peer_alloc(size_t bytes, void** ptr, void* ipc_handle_out /*64 bytes*/) {
@@ -996,34 +935,15 @@ int b200_peer_open(const void* ipc_handle /*64 bytes*/, void** ptr) {
     return B200_OK;
 }
 
-namespace {
-int fill_ar_params(PeerArParams& p, void* const* regions, size_t max_message_bytes, int rank, int world) {
-    const size_t src_stride = 2 * round_up(max_message_bytes, 256);          // LL doubles the bytes
-    const size_t area_stride = (size_t)kArMaxWorld * src_stride;
-    const size_t parity_stride = 2 * area_stride;
-    for (int r = 0; r < world; ++r) {
-        ARG_CHECK(regions[r], "peer collective: region %d is null", r);
-        p.region[r] = reinterpret_cast<uint8_t*>(regions[r]);
-    }
-    p.epoch = reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(regions[rank]) + 2 * parity_stride);
-    p.src_stride = src_stride;
-    p.area_stride = area_stride;
-    p.parity_stride = parity_stride;
-    p.rank = rank;
-    p.world = world;
-    return B200_OK;
-}
-}  // namespace
-
 int b200_peer_allreduce(const void* in, void* out, size_t bytes, int is_bf16, void* const* regions, size_t max_message_bytes,
                         int call_parity, int rank, int world, void* stream) {
     (void)call_parity;   // since r02 the slot parity comes from the device-side call counter (graph replays of any length are safe)
     ARG_CHECK(in && out && regions, "peer_allreduce: null pointer");
-    ARG_CHECK(world >= 2 && world <= kArMaxWorld && rank >= 0 && rank < world, "peer_allreduce: bad rank/world %d/%d", rank, world);
+    ARG_CHECK(valid_peer_group(rank, world), "peer_allreduce: bad rank/world %d/%d", rank, world);
     ARG_CHECK(bytes > 0 && bytes % 16 == 0 && bytes <= max_message_bytes, "peer_allreduce: message of %zu bytes unsupported", bytes);
     ARG_CHECK((((uintptr_t)in | (uintptr_t)out) & 15) == 0, "peer_allreduce: in/out must be 16-byte aligned");
     if (g_rec) {
-        std::vector<void*> regs(regions, regions + world);
+        const auto regs = copy_regions(regions, world);
         return rec_call([=](void* st) {
             return b200_peer_allreduce(in, out, bytes, is_bf16, regs.data(), max_message_bytes, 0, rank, world, st);
         });
@@ -1040,46 +960,31 @@ int b200_peer_allreduce(const void* in, void* out, size_t bytes, int is_bf16, vo
     const bool pdl = g_pdl.load() != 0;
     // W >= 3: reduce-scatter + all-gather (2 hops, (W-1)/W of the volume twice); W == 2: one hop. Env override for tests.
     const int two_shot = env_int("B200_AR_TWOSHOT", world >= 3 ? 1 : 0) && (p.n16 % world == 0);
-    if (two_shot) {
-        int c2 = (p.n16 / world + kArThreads - 1) / kArThreads;
-        if (c2 < 1) c2 = 1;
-        if (c2 > kArMaxCtas) c2 = kArMaxCtas;
-        if (is_bf16)
-            CUDA_CHECK(launch_ex(peer_allreduce_twoshot_kernel<__nv_bfloat16>, dim3(c2), dim3(kArThreads), 0, (cudaStream_t)stream, pdl, p));
-        else
-            CUDA_CHECK(launch_ex(peer_allreduce_twoshot_kernel<__half>, dim3(c2), dim3(kArThreads), 0, (cudaStream_t)stream, pdl, p));
-        return launched("peer_allreduce_twoshot_kernel");
-    }
-    if (is_bf16)
-        CUDA_CHECK(launch_ex(peer_allreduce_kernel<__nv_bfloat16>, dim3(ctas), dim3(kArThreads), 0, (cudaStream_t)stream, pdl, p));
-    else
-        CUDA_CHECK(launch_ex(peer_allreduce_kernel<__half>, dim3(ctas), dim3(kArThreads), 0, (cudaStream_t)stream, pdl, p));
-    return launched("peer_allreduce_kernel");
+    return by_dtype(is_bf16, [&](auto t) {
+        using T = decltype(t);
+        if (two_shot) {
+            int c2 = (p.n16 / world + kArThreads - 1) / kArThreads;
+            if (c2 < 1) c2 = 1;
+            if (c2 > kArMaxCtas) c2 = kArMaxCtas;
+            CUDA_CHECK(launch_ex(peer_allreduce_twoshot_kernel<T>, {dim3(c2), dim3(kArThreads), 0, (cudaStream_t)stream, pdl}, p));
+            return launched("peer_allreduce_twoshot_kernel");
+        }
+        CUDA_CHECK(launch_ex(peer_allreduce_kernel<T>, {dim3(ctas), dim3(kArThreads), 0, (cudaStream_t)stream, pdl}, p));
+        return launched("peer_allreduce_kernel");
+    });
 }
 
-namespace {
-int allreduce_norm_impl(const void* in, void* residual, const void* gamma, void* y, int is_bf16, int rows, int hidden,
-                        float eps, void* const* regions, size_t max_message_bytes, int rank, int world, int pushed, void* stream);
-}
-int b200_peer_allreduce_norm(const void* in, void* residual, const void* gamma, void* y, int is_bf16, int rows, int hidden,
-                             float eps, void* const* regions, size_t max_message_bytes, int rank, int world, void* stream) {
-    return allreduce_norm_impl(in, residual, gamma, y, is_bf16, rows, hidden, eps, regions, max_message_bytes, rank, world, 0, stream);
-}
-int b200_peer_gather_norm(const void* in, void* residual, const void* gamma, void* y, int is_bf16, int rows, int hidden,
-                          float eps, void* const* regions, size_t max_message_bytes, int rank, int world, void* stream) {
-    return allreduce_norm_impl(in, residual, gamma, y, is_bf16, rows, hidden, eps, regions, max_message_bytes, rank, world, 1, stream);
-}
-namespace {
-int allreduce_norm_impl(const void* in, void* residual, const void* gamma, void* y, int is_bf16, int rows, int hidden,
-                        float eps, void* const* regions, size_t max_message_bytes, int rank, int world, int pushed, void* stream) {
+static int allreduce_norm_impl(const void* in, void* residual, const void* gamma, void* y, int is_bf16, int rows, int hidden,
+                               float eps, void* const* regions, size_t max_message_bytes, int rank, int world, int pushed,
+                               void* stream) {
     ARG_CHECK(in && residual && gamma && y && regions, "peer_allreduce_norm: null pointer");
-    ARG_CHECK(world >= 2 && world <= kArMaxWorld && rank >= 0 && rank < world, "peer_allreduce_norm: bad rank/world %d/%d", rank, world);
+    ARG_CHECK(valid_peer_group(rank, world), "peer_allreduce_norm: bad rank/world %d/%d", rank, world);
     ARG_CHECK(rows > 0 && rows <= 65535, "peer_allreduce_norm: rows %d unsupported", rows);
     ARG_CHECK(hidden > 0 && hidden % (8 * world) == 0 && hidden <= 8192, "peer_allreduce_norm: hidden %d must be a multiple of 8*world and <= 8192", hidden);
     ARG_CHECK((size_t)rows * hidden * 2 <= max_message_bytes, "peer_allreduce_norm: message of %zu bytes exceeds the region", (size_t)rows * hidden * 2);
     ARG_CHECK((((uintptr_t)in | (uintptr_t)residual | (uintptr_t)gamma | (uintptr_t)y) & 15) == 0, "peer_allreduce_norm: pointers must be 16-byte aligned");
     if (g_rec) {
-        std::vector<void*> regs(regions, regions + world);
+        const auto regs = copy_regions(regions, world);
         return rec_call([=](void* st) {
             return allreduce_norm_impl(in, residual, gamma, y, is_bf16, rows, hidden, eps, regs.data(), max_message_bytes, rank, world, pushed, st);
         });
@@ -1097,21 +1002,28 @@ int allreduce_norm_impl(const void* in, void* residual, const void* gamma, void*
     p.pushed = pushed;
     const size_t smem = (size_t)hidden * sizeof(float) + (size_t)(hidden / 8 / world) * 16;
     const bool pdl = g_pdl.load() != 0;
-    if (is_bf16)
-        CUDA_CHECK(launch_ex(peer_allreduce_norm_kernel<__nv_bfloat16>, dim3(rows), dim3(kArThreads), smem, (cudaStream_t)stream, pdl, p));
-    else
-        CUDA_CHECK(launch_ex(peer_allreduce_norm_kernel<__half>, dim3(rows), dim3(kArThreads), smem, (cudaStream_t)stream, pdl, p));
-    return launched("peer_allreduce_norm_kernel");
+    return by_dtype(is_bf16, [&](auto t) {
+        CUDA_CHECK(launch_ex(peer_allreduce_norm_kernel<decltype(t)>, {dim3(rows), dim3(kArThreads), smem, (cudaStream_t)stream, pdl}, p));
+        return launched("peer_allreduce_norm_kernel");
+    });
 }
-}  // namespace
+
+int b200_peer_allreduce_norm(const void* in, void* residual, const void* gamma, void* y, int is_bf16, int rows, int hidden,
+                             float eps, void* const* regions, size_t max_message_bytes, int rank, int world, void* stream) {
+    return allreduce_norm_impl(in, residual, gamma, y, is_bf16, rows, hidden, eps, regions, max_message_bytes, rank, world, 0, stream);
+}
+int b200_peer_gather_norm(const void* in, void* residual, const void* gamma, void* y, int is_bf16, int rows, int hidden,
+                          float eps, void* const* regions, size_t max_message_bytes, int rank, int world, void* stream) {
+    return allreduce_norm_impl(in, residual, gamma, y, is_bf16, rows, hidden, eps, regions, max_message_bytes, rank, world, 1, stream);
+}
 
 int b200_peer_argmax(const void* logits, int is_bf16, int rows, int vocab_local, int vocab_total, int32_t* out,
                      void* const* regions, size_t max_message_bytes, int rank, int world, void* stream) {
     ARG_CHECK(logits && out && regions, "peer_argmax: null pointer");
-    ARG_CHECK(world >= 2 && world <= kArMaxWorld && rank >= 0 && rank < world, "peer_argmax: bad rank/world %d/%d", rank, world);
+    ARG_CHECK(valid_peer_group(rank, world), "peer_argmax: bad rank/world %d/%d", rank, world);
     ARG_CHECK(rows > 0 && (size_t)rows * 16 <= max_message_bytes && vocab_local > 0 && vocab_total > 0, "peer_argmax: bad shape");
     if (g_rec) {
-        std::vector<void*> regs(regions, regions + world);
+        const auto regs = copy_regions(regions, world);
         return rec_call([=](void* st) {
             return b200_peer_argmax(logits, is_bf16, rows, vocab_local, vocab_total, out, regs.data(), max_message_bytes, rank, world, st);
         });
@@ -1125,11 +1037,10 @@ int b200_peer_argmax(const void* logits, int is_bf16, int rows, int vocab_local,
     p.vocab_local = vocab_local;
     p.vocab_total = vocab_total;
     const bool pdl = g_pdl.load() != 0;
-    if (is_bf16)
-        CUDA_CHECK(launch_ex(peer_argmax_kernel<__nv_bfloat16>, dim3(rows), dim3(kArThreads), 0, (cudaStream_t)stream, pdl, p));
-    else
-        CUDA_CHECK(launch_ex(peer_argmax_kernel<__half>, dim3(rows), dim3(kArThreads), 0, (cudaStream_t)stream, pdl, p));
-    return launched("peer_argmax_kernel");
+    return by_dtype(is_bf16, [&](auto t) {
+        CUDA_CHECK(launch_ex(peer_argmax_kernel<decltype(t)>, {dim3(rows), dim3(kArThreads), 0, (cudaStream_t)stream, pdl}, p));
+        return launched("peer_argmax_kernel");
+    });
 }
 
 // ------------------------------------------------------------------------------------------------ decode programs
@@ -1181,12 +1092,15 @@ int b200_program_launch(b200_program* p, void* stream) {
             const bool bf16 = it.bf16 > 0;
             const int bpad = it.bpad > 0 ? it.bpad : 32, qfmt = it.qfmt > 0 ? it.qfmt : B200_FMT_INT4;
             int grid = 0;
-            rc = segment_grid(bf16, bpad, qfmt, &grid);
+            rc = by_dtype(bf16, [&](auto t) { return segment_grid<decltype(t)>(bpad, qfmt, &grid); });
             if (rc) return rc;
             unsigned long long* tr = p->trace ? p->trace + (size_t)it.first * grid * 2 : nullptr;
             // fine timeline (CTA 0): after the coarse region, [op][kFtSlots][kFtBlocks]
             g_ftrace_next = p->trace ? p->trace + p->ops.size() * (size_t)grid * 2 + (size_t)it.first * kFtSlots * kFtBlocks : nullptr;
-            rc = launch_segment(bf16, bpad, qfmt, p->d_ops + it.first, it.count, p->d_bar + i * 64, grid, pdl, tr, (cudaStream_t)stream);
+            rc = by_dtype(bf16, [&](auto t) {
+                return launch_segment<decltype(t)>(bpad, qfmt, p->d_ops + it.first, it.count, p->d_bar + i * 64, grid, pdl, tr,
+                                                   (cudaStream_t)stream);
+            });
             g_ftrace_next = nullptr;
         } else {
             rc = it.fn(stream);

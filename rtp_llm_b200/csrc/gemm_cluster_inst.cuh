@@ -15,38 +15,13 @@ using ParamsT = typename GemmParamsOf<B200_GEMM_VAR>::type;
 
 template <int FMT, typename T, int BPAD>
 int launch_one(const CUtensorMap& xmap, const CUtensorMap& wmap, const ParamsT& p, int n_tiles, cudaStream_t st) {
-    auto kern = wo_gemm_kernel<FMT, T, BPAD, B200_GEMM_VAR>;
+    constexpr auto kern = wo_gemm_kernel<FMT, T, BPAD, B200_GEMM_VAR>;
     constexpr int smem = gemm_smem_bytes(FMT, BPAD);
-    static bool configured[16] = {};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 16) return fail(B200_EINVAL, "device ordinal %d out of range", dev);
-    if (!configured[dev]) {
-        CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        configured[dev] = true;
-    }
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(n_tiles, p.nsplit, 1);
-    cfg.blockDim = dim3(gemm_threads(), 1, 1);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[2];
-    int na = 0;
-    if (p.use_pdl) {
-        attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[na].val.programmaticStreamSerializationAllowed = 1;
-        ++na;
-    }
-    if (p.nsplit > 1) {
-        attr[na].id = cudaLaunchAttributeClusterDimension;
-        attr[na].val.clusterDim.x = 1;
-        attr[na].val.clusterDim.y = (unsigned)p.nsplit;
-        attr[na].val.clusterDim.z = 1;
-        ++na;
-    }
-    cfg.attrs = attr;
-    cfg.numAttrs = na;
-    CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, xmap, wmap, p));
+    int rc = configure_once<kern>(smem);
+    if (rc) return rc;
+    // nsplit > 1: the nsplit CTAs of a tile form one cluster along y
+    const dim3 grid(n_tiles, p.nsplit), cluster(1, p.nsplit);
+    CUDA_CHECK(launch_ex(kern, {grid, dim3(gemm_threads()), smem, st, p.use_pdl != 0, cluster}, xmap, wmap, p));
     return launched("wo_gemm_kernel");
 }
 

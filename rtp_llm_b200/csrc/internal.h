@@ -1,6 +1,8 @@
 // Shared between the translation units of libb200_decode.so (host side only; nothing here is part of the C ABI).
 #pragma once
 #include <cuda.h>
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
 #include <cstdarg>
@@ -34,6 +36,66 @@ extern thread_local unsigned long long* g_ftrace_next;   // developer: fine time
         if (_e != cudaSuccess) return b200_host::fail(B200_ECUDA, "%s failed: %s", #expr, cudaGetErrorString(_e)); \
     } while (0)
 
+// Calls f with a value of the activation type (__nv_bfloat16 when bf16, else __half), so a launch is written once for both.
+template <typename F>
+auto by_dtype(bool bf16, F&& f) {
+    return bf16 ? f(__nv_bfloat16()) : f(__half());
+}
+
+// Sets a kernel's dynamic shared-memory limit, and a carve-out preference other than the default, once per device. Static,
+// like launch_ex, so that their instantiations stay out of the library's exported symbols.
+template <auto Kernel>
+static int configure_once(int smem, int carveout = cudaSharedmemCarveoutDefault) {
+    static bool configured[16] = {};
+    int dev = 0;
+    cudaGetDevice(&dev);
+    ARG_CHECK(dev >= 0 && dev < 16, "device ordinal %d out of range", dev);
+    if (!configured[dev]) {
+        CUDA_CHECK(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        if (carveout != cudaSharedmemCarveoutDefault)
+            CUDA_CHECK(cudaFuncSetAttribute(Kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carveout));
+        configured[dev] = true;
+    }
+    return B200_OK;
+}
+
+struct LaunchCfg {
+    dim3 grid, block;
+    size_t smem;
+    cudaStream_t stream;
+    bool pdl;
+    dim3 cluster = dim3(1, 1, 1);   // thread-block cluster shape; 1 x 1 x 1 launches without clusters
+};
+
+// Launch through cudaLaunchKernelEx so a kernel can carry the programmatic-dependent-launch attribute: it may then be
+// scheduled while its predecessor drains (every kernel of the decode chain executes griddepcontrol.wait before it
+// touches dependent data, so this only overlaps launch latency, prologues and -- for the GEMM -- the weight prefetch).
+template <typename... KArgs, typename... Args>
+static cudaError_t launch_ex(void (*kern)(KArgs...), const LaunchCfg& c, Args... args) {
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = c.grid;
+    cfg.blockDim = c.block;
+    cfg.dynamicSmemBytes = c.smem;
+    cfg.stream = c.stream;
+    cudaLaunchAttribute attr[2];
+    int na = 0;
+    if (c.pdl) {
+        attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr[na].val.programmaticStreamSerializationAllowed = 1;
+        ++na;
+    }
+    if (c.cluster.x * c.cluster.y * c.cluster.z > 1) {
+        attr[na].id = cudaLaunchAttributeClusterDimension;
+        attr[na].val.clusterDim.x = c.cluster.x;
+        attr[na].val.clusterDim.y = c.cluster.y;
+        attr[na].val.clusterDim.z = c.cluster.z;
+        ++na;
+    }
+    cfg.attrs = attr;
+    cfg.numAttrs = na;
+    return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
+}
+
 // gemm_cluster.cu: the one-kernel-per-GEMM path (cluster split-K merge); FP16 weights and batches > 64 use it
 int launch_cluster_gemm(int fmt, bool bf16, int bpad, const CUtensorMap& xmap, const CUtensorMap& wmap,
                         const b200::GemmParams& p, int n_tiles, cudaStream_t st);
@@ -41,10 +103,13 @@ int launch_cluster_gemm(int fmt, bool bf16, int bpad, const CUtensorMap& xmap, c
 int launch_cluster_gemm_rs(int fmt, bool bf16, int bpad, const CUtensorMap& xmap, const CUtensorMap& wmap,
                            const b200::GemmParamsRs& p, int n_tiles, cudaStream_t st);
 
-// segment_*.cu: the persistent decode-program kernel (csrc/decode_program.cuh). qfmt: B200_FMT_INT8 / B200_FMT_INT4.
-// grid == 0 asks for the co-resident grid size only (written to *grid_out).
-int segment_grid(bool bf16, int bpad, int qfmt, int* grid_out);
-int launch_segment(bool bf16, int bpad, int qfmt, const b200::ProgOp* d_ops, int nops, unsigned* gbar, int grid, bool pdl,
+// segment_f16.cu / segment_bf16.cu (T = __half / __nv_bfloat16): the persistent decode-program kernel
+// (csrc/decode_program.cuh). qfmt: B200_FMT_INT8 / B200_FMT_INT4. segment_grid gives the co-resident grid, the grid every
+// launch of that kernel uses.
+template <typename T>
+int segment_grid(int bpad, int qfmt, int* grid);
+template <typename T>
+int launch_segment(int bpad, int qfmt, const b200::ProgOp* d_ops, int nops, unsigned* gbar, int grid, bool pdl,
                    unsigned long long* trace, cudaStream_t st);
 
 }  // namespace b200_host

@@ -34,8 +34,10 @@ __device__ __forceinline__ float lds_f32(uint32_t saddr) {
 }
 
 // ---------------------------------------------------------------- mbarrier
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+// On raw 32-bit shared addresses (a persistent kernel keeps ONE base register and constant offsets instead of a dozen 64-bit
+// generic pointers); the pointer forms below wrap them.
+__device__ __forceinline__ void mbar_init_a(uint32_t bar, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
 }
 __device__ __forceinline__ void fence_mbar_init() {
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -45,48 +47,6 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
 }
 __device__ __forceinline__ void fence_proxy_async_global() {
     asm volatile("fence.proxy.async.global;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n\t}" ::"r"(smem_u32(bar)),
-                 "r"(bytes)
-                 : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    return ok != 0;
-}
-// non-blocking probe (no hardware suspend): lets a loop ask early and consume the answer after other work
-__device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    while (!mbar_try_wait(bar, parity)) {
-    }
-}
-
-
-// ---- the same primitives on raw 32-bit shared addresses (a persistent kernel keeps ONE base register and constant
-// offsets instead of a dozen 64-bit generic pointers)
-__device__ __forceinline__ void mbar_init_a(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
 }
 __device__ __forceinline__ void mbar_arrive_a(uint32_t bar) {
     asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(bar) : "memory");
@@ -114,18 +74,31 @@ __device__ __forceinline__ void mbar_wait_a(uint32_t bar, uint32_t parity) {
         if (++spins > (1u << 22)) __trap();
     }
 }
-__device__ __forceinline__ void tma_load_2d_a(uint32_t smem_dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
+
+__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) { mbar_init_a(smem_u32(bar), count); }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) { mbar_arrive_a(smem_u32(bar)); }
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
+    mbar_arrive_expect_tx_a(smem_u32(bar), bytes);
+}
+__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) { return mbar_try_wait_a(smem_u32(bar), parity); }
+// non-blocking probe (no hardware suspend): lets a loop ask early and consume the answer after other work
+__device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
+    uint32_t ok;
     asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-        ::"r"(smem_dst),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(bar)
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}"
+        : "=r"(ok)
+        : "r"(smem_u32(bar)), "r"(parity)
         : "memory");
+    return ok != 0;
 }
-__device__ __forceinline__ void tma_bulk_load_a(uint32_t smem_dst, const void* gsrc, uint32_t bytes, uint32_t bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_dst),
-                 "l"(gsrc), "r"(bytes), "r"(bar)
-                 : "memory");
+// no liveness guard here: the GEMM and attention hot loops wait through this form
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+    while (!mbar_try_wait(bar, parity)) {
+    }
 }
+
 __device__ __forceinline__ void sts_u32(uint32_t saddr, uint32_t v) {
     asm volatile("st.shared.u32 [%0], %1;" ::"r"(saddr), "r"(v) : "memory");
 }
@@ -145,19 +118,24 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
         "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(smem_u32(bar))
         : "memory");
 }
-__device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
+__device__ __forceinline__ void tma_load_2d_a(uint32_t smem_dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
     asm volatile(
         "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-        ::"r"(smem_u32(smem_dst)),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(smem_u32(bar))
+        ::"r"(smem_dst),
+        "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(bar)
         : "memory");
 }
+__device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
+    tma_load_2d_a(smem_u32(smem_dst), map, c0, c1, smem_u32(bar));
+}
 // 1-D bulk copy (global -> shared), bytes multiple of 16, both addresses 16B aligned.
-__device__ __forceinline__ void tma_bulk_load(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                     smem_u32(smem_dst)),
-                 "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
+__device__ __forceinline__ void tma_bulk_load_a(uint32_t smem_dst, const void* gsrc, uint32_t bytes, uint32_t bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_dst),
+                 "l"(gsrc), "r"(bytes), "r"(bar)
                  : "memory");
+}
+__device__ __forceinline__ void tma_bulk_load(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
+    tma_bulk_load_a(smem_u32(smem_dst), gsrc, bytes, smem_u32(bar));
 }
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
