@@ -28,6 +28,8 @@ extern "C" {
 #define B200_FMT_INT8 1  /* per-column symmetric INT8 (device_impl.py:183-222), packed by b200_pack_w8 */
 #define B200_FMT_INT4 2  /* GPTQ/AWQ group-128 INT4 (device_impl.py:242-300), packed by b200_pack_w4 */
 #define B200_FMT_INT8G 3 /* GPTQ/AWQ group-128 INT8 (device_impl.py:256-258 is_int8 branch: q_s = q_u - 128), packed by b200_pack_w8g */
+#define B200_FMT_INT4_G64 4 /* GPTQ/AWQ group-64 INT4, packed by b200_pack_w4 with group 64 */
+#define B200_FMT_INT4_G32 5 /* GPTQ/AWQ group-32 INT4, packed by b200_pack_w4 with group 32 */
 
 /* flags of b200_wo_gemm */
 #define B200_GEMM_PDL 1  /* launch with programmatic dependent launch (weights prefetched before the upstream grid ends) */
@@ -120,7 +122,10 @@ int b200_paged_decode_attn_rope(const void* qkv, int is_bf16, void* out, size_t 
  * instead of the FT sm80 interleave, weights become per-(128 features x 128 k) blobs that one TMA bulk copy stages.
  * Inputs are the loader's UN-permuted tensors (device pointers):
  *   b200_pack_w4: q_packed uint8 [K][N/2] (low nibble = even column, two's complement q_s = q_u - 8, device_impl.py:204-209),
- *                 scales, zeros_x_scales [K/128][N] 16-bit in the ACTIVATION type (fp16 or bf16)
+ *                 scales, zeros_x_scales [K/group][N] 16-bit in the ACTIVATION type (fp16 or bf16); group 128, 64 or 32
+ *                 selects the blob format B200_FMT_INT4 / _INT4_G64 / _INT4_G32. Blob per block: 8192 bytes of nibbles, then
+ *                 group 128: 128 scales and 128 zeros_x_scales; group 64 / 32: per group in k order, 128 {scale, zeros_x_scale}
+ *                 pairs (9216 / 10240 bytes per block)
  *   b200_pack_w8: q int8 [K][N] (device_impl.py:183-202); the per-column scale stays a separate [N] tensor
  *   b200_pack_w8g: q int8 [K][N] (8-bit group-wise checkpoints, q_s = q_u - 128, device_impl.py:256-274) + scales,
  *                 zeros_x_scales [K/128][N] as for b200_pack_w4; dequant W' = q_s * s + zeros_x_scales (device_impl.py:284-291)
@@ -139,7 +144,7 @@ size_t b200_wo_gemm_workspace_bytes(int max_batch, int N, int K);
 /* Y[B][N] = X[B][K] . W' (+ bias).  The compute behind LinearBase.forward
  * (rtp_llm/models_py/modules/factory/linear/linear_base.py:81; call sites modules/hybrid/causal_attention.py:83,90,
  * dense_mlp.py:99,103; lm_head cpp/models/PyWrappedModel.cc:1041-1046) for weight-only INT4/INT8 and FP16 weights.
- *   w         B200_FMT_INT4/INT8/INT8G: blob from b200_pack_w4/8/8g; B200_FMT_F16: W [N][K] (K contiguous)
+ *   w         B200_FMT_INT4/INT4_G64/INT4_G32/INT8/INT8G: blob from b200_pack_w4/8/8g; B200_FMT_F16: W [N][K] (K contiguous)
  *   col_scale INT8 only: [N] per-column scale in the activation type
  *   bias      optional [N]
  * B <= 128, K % 128 == 0, x / y / w 16-byte aligned. */
@@ -242,7 +247,7 @@ int b200_peer_allreduce_norm(const void* in, void* residual, const void* gamma, 
  * registers; the columns this rank owns are stored to y. MUST be followed on the same stream by b200_peer_gather_norm over
  * the same y / regions with no other collective of this communicator in between (both derive the exchange epoch from the
  * communicator's device-side call counter). Bits are those of b200_wo_gemm + b200_peer_allreduce_norm.
- * N % 128 == 0, N % (8*world) == 0, N <= 8192, B*N*2 <= max_message_bytes, no SILU_MUL. */
+ * N % 128 == 0, N % (8*world) == 0, N <= 8192, B*N*2 <= max_message_bytes, no SILU_MUL, not B200_FMT_INT4_G64 / _G32. */
 int b200_wo_gemm_rs(int fmt, int is_bf16, const void* x, int B, int K, int N, const void* w, const void* col_scale,
                     const void* bias, void* y, void* workspace, size_t workspace_bytes, int flags, void* const* regions,
                     size_t max_message_bytes, int rank, int world, void* stream);

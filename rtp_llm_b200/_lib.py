@@ -7,6 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("B200_LIB_PATH") or os.path.join(HERE, "libb200_decode.so")   # override: developer A/B builds
 
 B200_FMT_F16, B200_FMT_INT8, B200_FMT_INT4, B200_FMT_INT8G = 0, 1, 2, 3
+B200_FMT_INT4_G64, B200_FMT_INT4_G32 = 4, 5
 B200_GEMM_PDL = 1
 B200_GEMM_SILU_MUL = 2
 

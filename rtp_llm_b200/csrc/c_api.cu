@@ -522,7 +522,7 @@ int b200_paged_decode_attn_rope(const void* qkv, int is_bf16, void* out, size_t 
 size_t b200_wo_gemm_packed_bytes(int fmt, int K, int N) {
     if (K <= 0 || N <= 0 || K % kGemmBK) return 0;
     const size_t n_tiles = (N + kGemmTileN - 1) / kGemmTileN, kb = K / kGemmBK;
-    if (fmt == B200_FMT_INT4) return n_tiles * kb * kW4BlockBytes;
+    if (fmt == B200_FMT_INT4 || fmt == B200_FMT_INT4_G64 || fmt == B200_FMT_INT4_G32) return n_tiles * kb * gemm_w_bytes(fmt);
     if (fmt == B200_FMT_INT8) return n_tiles * kb * kW8BlockBytes;
     if (fmt == B200_FMT_INT8G) return n_tiles * kb * kW8GBlockBytes;
     if (fmt != B200_FMT_F16) return 0;
@@ -532,14 +532,15 @@ size_t b200_wo_gemm_packed_bytes(int fmt, int K, int N) {
 int b200_pack_w4(const uint8_t* q_packed, const void* scales, const void* zeros_x_scales, int K, int N, int group,
                  void* blob, void* stream) {
     ARG_CHECK(q_packed && scales && zeros_x_scales && blob, "pack_w4: null pointer");
-    ARG_CHECK(group == kGemmBK, "pack_w4: group size %d unsupported (128 only)", group);
+    ARG_CHECK(group == 128 || group == 64 || group == 32, "pack_w4: group size %d unsupported (128, 64 or 32)", group);
     ARG_CHECK(K > 0 && K % kGemmBK == 0, "pack_w4: K=%d must be a positive multiple of 128", K);
     ARG_CHECK(N > 0 && N % 2 == 0, "pack_w4: N=%d must be positive and even", N);
-    const size_t words = b200_wo_gemm_packed_bytes(B200_FMT_INT4, K, N) / 4;
+    const int fmt = group == 128 ? B200_FMT_INT4 : (group == 64 ? B200_FMT_INT4_G64 : B200_FMT_INT4_G32);
+    const size_t words = b200_wo_gemm_packed_bytes(fmt, K, N) / 4;
     const int threads = 256;
     const size_t blocks = (words + threads - 1) / threads;
     pack_w4_kernel<<<(unsigned)(blocks < 65535 ? blocks : 65535), threads, 0, (cudaStream_t)stream>>>(
-        q_packed, reinterpret_cast<const uint16_t*>(scales), reinterpret_cast<const uint16_t*>(zeros_x_scales), K, N,
+        q_packed, reinterpret_cast<const uint16_t*>(scales), reinterpret_cast<const uint16_t*>(zeros_x_scales), K, N, group,
         reinterpret_cast<uint8_t*>(blob));
     return launched("pack_w4_kernel");
 }
@@ -584,7 +585,8 @@ static int wo_gemm_impl(int fmt, int is_bf16, const void* x, int B, int K, int N
                         const void* bias, void* y, void* workspace, size_t workspace_bytes, int flags, const RsPush* rs,
                         void* stream) {
     if (B == 0) return B200_OK;
-    ARG_CHECK(fmt == B200_FMT_F16 || fmt == B200_FMT_INT8 || fmt == B200_FMT_INT4 || fmt == B200_FMT_INT8G,
+    ARG_CHECK(fmt == B200_FMT_F16 || fmt == B200_FMT_INT8 || fmt == B200_FMT_INT4 || fmt == B200_FMT_INT8G || fmt == B200_FMT_INT4_G64 ||
+                  fmt == B200_FMT_INT4_G32,
               "wo_gemm: unknown weight format %d", fmt);
     ARG_CHECK(x && w && y, "wo_gemm: null pointer");
     ARG_CHECK(B > 0 && B <= 128, "wo_gemm: batch %d unsupported (1..128 per call)", B);
@@ -611,7 +613,7 @@ static int wo_gemm_impl(int fmt, int is_bf16, const void* x, int B, int K, int N
     // ---- weight-only INT8 / INT4 at decode batches inside a decode program: an op of the persistent kernel (uniform split-K
     // merged through L2). Every other GEMM, and every call outside a program, uses the cluster kernel below (split-K merged
     // through DSMEM), which needs no grid-wide barrier.
-    const bool seg_capable = (fmt == B200_FMT_INT8 || fmt == B200_FMT_INT4) && bpad <= 64;   // INT8G / FP16: cluster kernel only
+    const bool seg_capable = (fmt == B200_FMT_INT8 || fmt == B200_FMT_INT4) && bpad <= 64;   // INT8G / INT4 g64, g32 / FP16: cluster kernel only
     if (g_rec && seg_capable && !rs) {
         ARG_CHECK(workspace && workspace_bytes >= kGemmSemBytes, "wo_gemm: workspace of at least %zu bytes required", kGemmSemBytes);
         int grid = 0;
@@ -688,6 +690,7 @@ int b200_wo_gemm_rs(int fmt, int is_bf16, const void* x, int B, int K, int N, co
                     const void* bias, void* y, void* workspace, size_t workspace_bytes, int flags, void* const* regions,
                     size_t max_message_bytes, int rank, int world, void* stream) {
     ARG_CHECK(regions, "wo_gemm_rs: null regions");
+    ARG_CHECK(fmt != B200_FMT_INT4_G64 && fmt != B200_FMT_INT4_G32, "wo_gemm_rs: INT4 group-64 / group-32 weights (format %d) unsupported", fmt);
     ARG_CHECK(valid_peer_group(rank, world), "wo_gemm_rs: bad rank/world %d/%d", rank, world);
     ARG_CHECK(N % 128 == 0 && N % (8 * world) == 0 && N <= 8192, "wo_gemm_rs: N=%d must be a multiple of 128 and of 8*world, <= 8192", N);
     ARG_CHECK((size_t)B * N * 2 <= max_message_bytes, "wo_gemm_rs: message of %zu bytes exceeds the region", (size_t)B * N * 2);

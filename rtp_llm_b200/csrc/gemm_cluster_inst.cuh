@@ -40,6 +40,10 @@ int by_fmt(int fmt, int bpad, const CUtensorMap& xmap, const CUtensorMap& wmap, 
         case B200_FMT_F16: return by_bpad<kFmtF16, T>(bpad, xmap, wmap, p, n_tiles, st);
         case B200_FMT_INT8: return by_bpad<kFmtInt8, T>(bpad, xmap, wmap, p, n_tiles, st);
         case B200_FMT_INT8G: return by_bpad<kFmtInt8G, T>(bpad, xmap, wmap, p, n_tiles, st);
+#if B200_GEMM_VAR == 0   // INT4 g64 / g32: plain output only (b200_wo_gemm_rs rejects them)
+        case B200_FMT_INT4_G64: return by_bpad<kFmtInt4G64, T>(bpad, xmap, wmap, p, n_tiles, st);
+        case B200_FMT_INT4_G32: return by_bpad<kFmtInt4G32, T>(bpad, xmap, wmap, p, n_tiles, st);
+#endif
         default: return by_bpad<kFmtInt4, T>(bpad, xmap, wmap, p, n_tiles, st);
     }
 }

@@ -1,4 +1,4 @@
-// Weight-only (INT4 group-128 / INT8 per-column / INT8 group-128 / FP16) x FP16|BF16 GEMM for decode batches, sm_90a.
+// Weight-only (INT4 group-128 / -64 / -32 / INT8 per-column / INT8 group-128 / FP16) x FP16|BF16 GEMM for decode batches, sm_90a.
 //
 //   Y[b][n] = sum_k X[b][k] * W'[k][n] (+ bias[n]),   W' per rtp_llm/device/device_impl.py:183-222,242-300
 //   (SURVEY.md section 8 a8-a10).  Replaces the cutlass fpA_intB "mixed gemm" the reference loader still prepares weights
@@ -25,17 +25,26 @@
 
 namespace b200 {
 
-enum : int { kFmtF16 = 0, kFmtInt8 = 1, kFmtInt4 = 2, kFmtInt8G = 3 };   // Int8G: 8-bit GPTQ/AWQ, group 128 (device_impl.py:256-258)
+// Int8G: 8-bit GPTQ/AWQ, group 128 (device_impl.py:256-258); Int4G64 / Int4G32: INT4 with quantisation groups of 64 / 32 k
+enum : int { kFmtF16 = 0, kFmtInt8 = 1, kFmtInt4 = 2, kFmtInt8G = 3, kFmtInt4G64 = 4, kFmtInt4G32 = 5 };
 
-constexpr int kGemmBK = 128;       // k elements per pipeline stage (= one INT4 quantisation group)
+constexpr int kGemmBK = 128;       // k elements per pipeline stage (= one group-128 quantisation group)
 constexpr int kGemmTileN = 128;    // output features per CTA (MMA M)
 constexpr int kW4BlockBytes = 8192 + 256 + 256;
 constexpr int kW8BlockBytes = 16384;
 constexpr int kW8GBlockBytes = 16384 + 256 + 256;   // + the group's scales and zero*scale, like the INT4 blob
 constexpr int kW16BlockBytes = 32768;
 
+__host__ __device__ constexpr bool is_int4(int fmt) { return fmt == kFmtInt4 || fmt == kFmtInt4G64 || fmt == kFmtInt4G32; }
+// quantisation group (k elements) of a weight format; 128 for the formats without groups
+__host__ __device__ constexpr int fmt_group(int fmt) { return fmt == kFmtInt4G64 ? 64 : (fmt == kFmtInt4G32 ? 32 : kGemmBK); }
+// INT4 blob of group g: the 8192-byte nibble payload, then per group in k order 128 rows of {scale, zero*scale} (512 bytes;
+// group 128 keeps its 256 bytes of scales followed by 256 bytes of zero*scale)
+__host__ __device__ constexpr int w4_block_bytes(int group) { return 8192 + (kGemmBK / group) * 512; }
+
 __host__ __device__ constexpr int gemm_w_bytes(int fmt) {
-    return fmt == kFmtInt4 ? kW4BlockBytes : (fmt == kFmtInt8 ? kW8BlockBytes : (fmt == kFmtInt8G ? kW8GBlockBytes : kW16BlockBytes));
+    return is_int4(fmt) ? w4_block_bytes(fmt_group(fmt))
+                        : (fmt == kFmtInt8 ? kW8BlockBytes : (fmt == kFmtInt8G ? kW8GBlockBytes : kW16BlockBytes));
 }
 // Shared-memory rings.  The weight ring (HBM stream) and the activation ring (L2 hits) are SEPARATE: a weight stage is
 // released as soon as the dequant warps hold its nibbles in registers, so its lifetime is one TMA latency, not the
@@ -51,8 +60,8 @@ __host__ __device__ constexpr int gemm_w_stages_for(int fmt, int bpad, int budge
     return n > 12 ? 12 : n;
 }
 // Activation ring of wo_gemm_kernel. Its pipelined main loop holds an activation stage until both halves of the block have
-// retired, so it takes 6 stages wherever two CTAs per SM still keep 6 weight stages (INT4 at batch pad <= 32); the other
-// formats keep gemm_x_stages rather than drop to one CTA per SM.
+// retired, so it takes 6 stages wherever two CTAs per SM still keep 6 weight stages (INT4 g128 / g64 at batch pad <= 32,
+// g32 at batch pad 16); the other cases keep gemm_x_stages rather than drop to one CTA per SM.
 __host__ __device__ constexpr int gemm_cluster_x_stages(int fmt, int bpad) {
     return bpad <= 32 && gemm_w_stages_for(fmt, bpad, 106 * 1024, 6) >= 6 ? 6 : gemm_x_stages(bpad);
 }
@@ -239,20 +248,34 @@ struct Pair<__nv_bfloat16> {
 // A block is dequantised in two halves of 4 k-steps (16 A registers each) so that the GEMM main loop can pipeline them:
 // half h is payload vector h (INT4) or vectors 2h, 2h+1 (8-bit).
 template <int FMT>
-constexpr int kWVecsPerHalf = FMT == kFmtInt4 ? 1 : 2;
+constexpr int kWVecsPerHalf = is_int4(FMT) ? 1 : 2;
 
 // Group scale / zero*scale of this thread's feature rows A and B (INT4 and INT8G; unused otherwise). Kept as raw 16-bit
 // values and broadcast at the use, where the broadcast folds into the hfma2 operand (.H0_H0) instead of costing a PRMT.
 struct WScales {
     uint16_t sA, zA, sB, zB;
 };
+// INT4 g64 / g32: the same per group of the block, each row's {scale, zero*scale} pair in one register (one LDS.32, and the
+// hfma2 operands take its halves as .H0_H0 / .H1_H1), so four groups cost the registers of two 16-bit pairs.
+template <int NG>
+struct WScalesG {
+    uint32_t A[NG], B[NG];
+};
+template <int FMT>
+using WScalesOf = std::conditional_t<is_int4(FMT) && fmt_group(FMT) < kGemmBK, WScalesG<kGemmBK / fmt_group(FMT)>, WScales>;
 
 // This thread's scales and payload vectors of the block at shared address wb: v[h] is half h.
 template <int FMT>
-__device__ __forceinline__ void load_w_block(uint32_t wb, int R, int lane, WScales& s, uint4 (&v)[2][kWVecsPerHalf<FMT>]) {
+__device__ __forceinline__ void load_w_block(uint32_t wb, int R, int lane, WScalesOf<FMT>& s, uint4 (&v)[2][kWVecsPerHalf<FMT>]) {
     const int rA = 16 * R + (lane >> 2), rB = rA + 8;
     const uint32_t vec = wb + (uint32_t)(R * 32 + lane) * 16;
-    if (FMT == kFmtInt4 || FMT == kFmtInt8G) {
+    if constexpr (FMT == kFmtInt4G64 || FMT == kFmtInt4G32) {
+#pragma unroll
+        for (int g = 0; g < kGemmBK / fmt_group(FMT); ++g) {
+            s.A[g] = lds_u32(wb + 8192 + g * 512 + rA * 4);
+            s.B[g] = lds_u32(wb + 8192 + g * 512 + rB * 4);
+        }
+    } else if (FMT == kFmtInt4 || FMT == kFmtInt8G) {
         constexpr int Q_BYTES = FMT == kFmtInt4 ? 8192 : 16384;
         s.sA = (uint16_t)lds_u16(wb + Q_BYTES + rA * 2);
         s.zA = (uint16_t)lds_u16(wb + Q_BYTES + 256 + rA * 2);
@@ -265,33 +288,45 @@ __device__ __forceinline__ void load_w_block(uint32_t wb, int R, int lane, WScal
         for (int q = 0; q < kWVecsPerHalf<FMT>; ++q) v[h][q] = lds_v4(vec + (h * kWVecsPerHalf<FMT> + q) * 4096);
 }
 
-// One half block (k-steps 4h..4h+3) -> a[0..3].
-template <int FMT, typename T>
-__device__ __forceinline__ void dequant_half(const uint4 (&v)[kWVecsPerHalf<FMT>], const WScales& s, uint32_t (*a)[4]) {
+// One half block (k-steps 4H..4H+3) -> a[0..3].
+template <int FMT, typename T, int H>
+__device__ __forceinline__ void dequant_half(const uint4 (&v)[kWVecsPerHalf<FMT>], const WScalesOf<FMT>& s, uint32_t (*a)[4]) {
     using P = Pair<T>;
-    const typename P::type sA = P::bcast(s.sA), zA = P::bcast(s.zA), sB = P::bcast(s.sB), zB = P::bcast(s.zB);
-    if (FMT == kFmtInt4) {
-        Dequant4<T>::word(v[0].x, sA, zA, sB, zB, a[0]);
-        Dequant4<T>::word(v[0].y, sA, zA, sB, zB, a[1]);
-        Dequant4<T>::word(v[0].z, sA, zA, sB, zB, a[2]);
-        Dequant4<T>::word(v[0].w, sA, zA, sB, zB, a[3]);
-    } else {
+    if constexpr (FMT == kFmtInt4G64 || FMT == kFmtInt4G32) {
+        // word w of the half is k-step 4H + w, which lies in group (4H + w) * 16 / g: g64 takes group H for the whole half,
+        // g32 group 2H for words 0-1 and 2H + 1 for words 2-3
+        const uint32_t w[4] = {v[0].x, v[0].y, v[0].z, v[0].w};
 #pragma unroll
-        for (int q = 0; q < 2; ++q) {
-            Dequant8<T>::word(v[q].x, &a[2 * q][0]);
-            Dequant8<T>::word(v[q].y, &a[2 * q][2]);
-            Dequant8<T>::word(v[q].z, &a[2 * q + 1][0]);
-            Dequant8<T>::word(v[q].w, &a[2 * q + 1][2]);
+        for (int i = 0; i < 4; ++i) {
+            const int g = (4 * H + i) * 16 / fmt_group(FMT);
+            Dequant4<T>::word(w[i], P::bcast((uint16_t)s.A[g]), P::bcast((uint16_t)(s.A[g] >> 16)), P::bcast((uint16_t)s.B[g]),
+                              P::bcast((uint16_t)(s.B[g] >> 16)), a[i]);
         }
-        if (FMT == kFmtInt8G) {   // group-wise 8-bit: W' = q_s * s + zero*scale, one rounding (as INT4)
+    } else {
+        const typename P::type sA = P::bcast(s.sA), zA = P::bcast(s.zA), sB = P::bcast(s.sB), zB = P::bcast(s.zB);
+        if (FMT == kFmtInt4) {
+            Dequant4<T>::word(v[0].x, sA, zA, sB, zB, a[0]);
+            Dequant4<T>::word(v[0].y, sA, zA, sB, zB, a[1]);
+            Dequant4<T>::word(v[0].z, sA, zA, sB, zB, a[2]);
+            Dequant4<T>::word(v[0].w, sA, zA, sB, zB, a[3]);
+        } else {
 #pragma unroll
-            for (int j = 0; j < 4; ++j)
+            for (int q = 0; q < 2; ++q) {
+                Dequant8<T>::word(v[q].x, &a[2 * q][0]);
+                Dequant8<T>::word(v[q].y, &a[2 * q][2]);
+                Dequant8<T>::word(v[q].z, &a[2 * q + 1][0]);
+                Dequant8<T>::word(v[q].w, &a[2 * q + 1][2]);
+            }
+            if (FMT == kFmtInt8G) {   // group-wise 8-bit: W' = q_s * s + zero*scale, one rounding (as INT4)
 #pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    typename Pair<T>::type h = *reinterpret_cast<typename Pair<T>::type*>(&a[j][i]);
-                    h = (i & 1) ? __hfma2(h, sB, zB) : __hfma2(h, sA, zA);
-                    a[j][i] = *reinterpret_cast<uint32_t*>(&h);
-                }
+                for (int j = 0; j < 4; ++j)
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        typename Pair<T>::type h = *reinterpret_cast<typename Pair<T>::type*>(&a[j][i]);
+                        h = (i & 1) ? __hfma2(h, sB, zB) : __hfma2(h, sA, zA);
+                        a[j][i] = *reinterpret_cast<uint32_t*>(&h);
+                    }
+            }
         }
     }
 }
@@ -299,13 +334,13 @@ __device__ __forceinline__ void dequant_half(const uint4 (&v)[kWVecsPerHalf<FMT>
 // The whole block at once (the persistent kernel's serial loop).
 template <int FMT, typename T>
 __device__ __forceinline__ void load_w_frag(uint32_t wb, int R, int lane, uint32_t (&a)[8][4], uint32_t empty_bar) {
-    WScales s;
+    WScalesOf<FMT> s;
     uint4 v[2][kWVecsPerHalf<FMT>];
     load_w_block<FMT>(wb, R, lane, s, v);
     __syncwarp();
     if (lane == 0) mbar_arrive_a(empty_bar);
-    dequant_half<FMT, T>(v[0], s, &a[0]);
-    dequant_half<FMT, T>(v[1], s, &a[4]);
+    dequant_half<FMT, T, 0>(v[0], s, &a[0]);
+    dequant_half<FMT, T, 1>(v[1], s, &a[4]);
 }
 
 // Descriptor of k-step j of a K-major SW128 operand whose two 64-element boxes lie BOX_BYTES apart, as an offset to the
@@ -431,12 +466,12 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
             constexpr int NV = kWVecsPerHalf<FMT>;
             uint32_t a0[4][4], a1[4][4];
             uint4 v[2][NV];
-            WScales sc;
+            WScalesOf<FMT> sc;
             mbar_wait(&wfull[0], 0);
             load_w_block<FMT>(smem_u32(wring), R, lane, sc, v);
             __syncwarp();
             if (lane == 0) mbar_arrive(&wempty[0]);
-            dequant_half<FMT, T>(v[0], sc, a0);
+            dequant_half<FMT, T, 0>(v[0], sc, a0);
             sw = 1;
             mbar_wait(&xfull[0], 0);
             for (int it = 0; it < nkb; ++it) {
@@ -448,7 +483,7 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
                 wgmma_wait<1>();   // block it-1 has retired: a1 and its activation stage are free
                 __syncwarp();
                 if (it > 0 && lane == 0) mbar_arrive(&xempty[px]);
-                dequant_half<FMT, T>(v[1], sc, a1);
+                dequant_half<FMT, T, 1>(v[1], sc, a1);
                 wgmma_fence();
 #pragma unroll
                 for (int j = 0; j < 4; ++j) wgmma_rs<BPAD, T>(acc, a1[j], sw128_kstep<BPAD * 128>(bdesc, 4 + j), 1u);
@@ -463,7 +498,7 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
                     __syncwarp();
                     if (lane == 0) mbar_arrive(&wempty[sw]);
                     ++sw;
-                    dequant_half<FMT, T>(v[0], sc, a0);
+                    dequant_half<FMT, T, 0>(v[0], sc, a0);
                     mbar_wait(&xfull[sx], phx);
                 }
             }
@@ -618,16 +653,18 @@ __host__ __device__ __forceinline__ void frag8_pos(int byte_in_block, int& r, in
     r = frag_row(R, lane, i);
     kl = frag_k(j, lane, i, bv & 1);
 }
-// int4: q_packed [K][N/2] (byte = hi nibble col 2j+1, lo nibble col 2j, two's complement q_s), scales/zs [K/128][N] (16-bit).
+// int4: q_packed [K][N/2] (byte = hi nibble col 2j+1, lo nibble col 2j, two's complement q_s), scales/zs [K/group][N] (16-bit),
+// group 128, 64 or 32.
 static __global__ void pack_w4_kernel(const uint8_t* __restrict__ q_packed, const uint16_t* __restrict__ scales,
-                               const uint16_t* __restrict__ zs, int K, int N, uint8_t* __restrict__ blob) {
+                               const uint16_t* __restrict__ zs, int K, int N, int group, uint8_t* __restrict__ blob) {
     const int k_blocks = K / kGemmBK;
     const int n_tiles = (N + kGemmTileN - 1) / kGemmTileN;
-    const size_t total_words = (size_t)n_tiles * k_blocks * (kW4BlockBytes / 4);
+    const int block_words = w4_block_bytes(group) / 4, gpb = kGemmBK / group;   // groups per k-block
+    const size_t total_words = (size_t)n_tiles * k_blocks * block_words;
     for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total_words;
          idx += (size_t)gridDim.x * blockDim.x) {
-        const int word_in_block = (int)(idx % (kW4BlockBytes / 4));
-        const size_t blk = idx / (kW4BlockBytes / 4);
+        const int word_in_block = (int)(idx % block_words);
+        const size_t blk = idx / block_words;
         const int kb = (int)(blk % k_blocks), tile = (int)(blk / k_blocks);
         uint32_t out = 0;
         if (word_in_block < 2048) {
@@ -644,6 +681,10 @@ static __global__ void pack_w4_kernel(const uint8_t* __restrict__ q_packed, cons
                 }
                 out |= u << (4 * pos);
             }
+        } else if (gpb > 1) {
+            const int g = (word_in_block - 2048) / 128, r = (word_in_block - 2048) % 128, n = tile * kGemmTileN + r;
+            const size_t row = (size_t)(kb * gpb + g) * N + n;    // group g of the block: word r = {scale, zero*scale} of row r
+            if (n < N) out = scales[row] | ((uint32_t)zs[row] << 16);
         } else {
             const int w = word_in_block - 2048;          // 0..127: 64 words of scales then 64 words of zs
             const uint16_t* src = (w < 64) ? scales : zs;

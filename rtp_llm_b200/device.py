@@ -93,9 +93,20 @@ class B200Impl:
         if quant_mode == torch.int8 and zeros_x_scales is None:
             raise ValueError("INT8 per-column weights are packed by apply_int8 (the scale rides along)")
         assert scales is not None and zeros_x_scales is not None, "the b200 group-wise blobs carry scales and zero*scale"
+        # the reference's hook takes no group argument: the group is what the scales' row count implies
+        K, N = tensor.shape[0], tensor.shape[1] * (1 if quant_mode == torch.int8 else 2)
+        rows = scales.numel() // N
+        group = K // rows if rows and K % rows == 0 else 0
+        scales, zeros_x_scales = scales.reshape(rows, N), zeros_x_scales.reshape(rows, N)
         if quant_mode == torch.int8:        # 8-bit group-wise
+            if group != 128:
+                raise ValueError(f"8-bit group-wise weights: group size {group or f'K/{rows}'} unsupported (128 only; K={K}, "
+                                 f"{rows} scale rows)")
             return ops.pack_w8g(tensor.to(self.device).contiguous(), scales.to(self.act_dtype).to(self.device).contiguous(),
                                 zeros_x_scales.to(self.act_dtype).to(self.device).contiguous()).data
+        if group not in (32, 64) and (group < 128 or group % 128):
+            raise ValueError(f"INT4 group-wise weights: group size {group or f'K/{rows}'} unsupported (32, 64 or a multiple of "
+                             f"128, per-channel included; K={K}, {rows} scale rows)")
         packed = ops.pack_w4(tensor.to(self.device).contiguous(), scales.to(self.act_dtype).to(self.device).contiguous(),
-                             zeros_x_scales.to(self.act_dtype).to(self.device).contiguous())
+                             zeros_x_scales.to(self.act_dtype).to(self.device).contiguous(), group)
         return packed.data

@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference's Linear seam: a LinearBase strategy for weight-only INT4 (GPTQ/AWQ g128) / INT8 /
+"""Host-side mirror of the reference's Linear seam: a LinearBase strategy for weight-only INT4 (GPTQ/AWQ g128 / g64 / g32) / INT8 /
 FP16 weights (/root/reference/rtp_llm/models_py/modules/factory/linear/linear_base.py:16-102; registration
 factory.py:43-51; the CUDA strategies that exist today, impl/cuda/__init__.py:15-28, do not cover weight-only INT4/INT8 --
 an int8-typed weight with scales raises "No suitable Linear strategy", factory.py:113-120).

@@ -28,7 +28,7 @@ QW, QZ, QS = ".qweight", ".qzeros", ".scales"
 class QuantConfig:
     method: str              # "gptq" | "awq" | "int8" (per-column weight-only, quantised at load time) | "none"
     bits: int = 4
-    group_size: int = 128
+    group_size: int = 128    # 4-bit: 32, 64, 128 (or a larger multiple of 128), -1 = per channel; 8-bit: 128
 
     @property
     def gptq(self) -> bool:
@@ -98,8 +98,10 @@ class B200Loader:
         qw, qz, qs = torch.cat(qws, dim=1), torch.cat(qzs, dim=1), torch.cat(qss, dim=1)
         if pad_in:                                                    # w2: the inter size is its INPUT axis
             qw = pad_dim(qw, pad_in // pad_div if q.gptq else pad_in, 0)
-            qz = pad_dim(qz, max(pad_in // q.group_size, 1), 0)
-            qs = pad_dim(qs, max(pad_in // q.group_size, 1), 0)
+            # per channel (group_size -1): the one row of zeros / scales covers the padded rows too
+            rows = max(pad_in // q.group_size, 1) if q.group_size > 0 else 0
+            qz = pad_dim(qz, rows, 0)
+            qs = pad_dim(qs, rows, 0)
         return self.impl.unpack_groupwise(qw, qz, qs.to(torch.float16), q.gptq, q.awq, q.bits)
 
     def _groupwise(self, prefixes, pad_in: int = 0, pad_out: int = 0, gate_up_inter: int = 0) -> ops.PackedWeight:

@@ -7,7 +7,8 @@ from typing import Optional
 import torch
 
 from . import _lib
-from ._lib import B200_FMT_F16, B200_FMT_INT4, B200_FMT_INT8, B200_FMT_INT8G, B200Error, check
+from ._lib import (B200_FMT_F16, B200_FMT_INT4, B200_FMT_INT4_G32, B200_FMT_INT4_G64, B200_FMT_INT8, B200_FMT_INT8G, B200Error,
+                   check)
 
 
 def _stream() -> int:
@@ -163,18 +164,41 @@ class PackedWeight:
         return PackedWeight(fmt, K, N, data if data.is_contiguous() else data.contiguous(), col_scale)
 
 
+_W4_FORMATS = {128: B200_FMT_INT4, 64: B200_FMT_INT4_G64, 32: B200_FMT_INT4_G32}
+
+
+def w4_format(K: int, group: int, scales: torch.Tensor, zeros_x_scales: torch.Tensor):
+    """(blob format, kernel group, scales, zeros_x_scales) for INT4 weights of quantisation group `group` over K rows.
+
+    128, 64 and 32 have their own blob formats (B200_FMT_INT4, _INT4_G64, _INT4_G32). A larger multiple of 128, per-channel
+    (group = K, or -1) included, becomes group 128 with each scale / zero*scale row repeated: every weight keeps its own s and
+    zero*s, so the dequantised weights are the same bits. Any other group is left for the library to reject."""
+    if group == -1:
+        group = K
+    if group != 128 and (group <= 0 or scales.shape[0] * group != K or zeros_x_scales.shape[0] != scales.shape[0]):
+        raise B200Error(f"pack_w4: group {group} does not match K={K} and scales / zeros_x_scales of {scales.shape[0]} / "
+                        f"{zeros_x_scales.shape[0]} rows")
+    if group > 128 and group % 128 == 0:
+        r = group // 128
+        return (B200_FMT_INT4, 128, scales.repeat_interleave(r, dim=0).contiguous(),
+                zeros_x_scales.repeat_interleave(r, dim=0).contiguous())
+    return _W4_FORMATS.get(group, B200_FMT_INT4), group, scales, zeros_x_scales
+
+
 def pack_w4(q_packed: torch.Tensor, scales: torch.Tensor, zeros_x_scales: torch.Tensor, group: int = 128) -> PackedWeight:
-    """q_packed uint8/int8 [K,N/2], scales / zeros_x_scales [K/g,N] in the activation dtype (CUDA)."""
+    """q_packed uint8/int8 [K,N/2], scales / zeros_x_scales [K/g,N] in the activation dtype (CUDA). The group picks the blob
+    format (w4_format); the trailer records the group as given (per-channel: K)."""
     _cuda_contig(q_packed, scales, zeros_x_scales)
     K, N = q_packed.shape[0], q_packed.shape[1] * 2
-    n = _lib.load().b200_wo_gemm_packed_bytes(B200_FMT_INT4, K, N)
+    fmt, kernel_group, scales, zeros_x_scales = w4_format(K, group, scales, zeros_x_scales)
+    n = _lib.load().b200_wo_gemm_packed_bytes(fmt, K, N)
     if n == 0:
         raise B200Error(f"pack_w4: unsupported shape K={K} N={N}")
     blob = torch.empty(int(n) + _TRAILER_BYTES, dtype=torch.uint8, device=q_packed.device)
-    check(_lib.load().b200_pack_w4(_p(q_packed), _p(scales), _p(zeros_x_scales), K, N, group, _p(blob), _stream()),
+    check(_lib.load().b200_pack_w4(_p(q_packed), _p(scales), _p(zeros_x_scales), K, N, kernel_group, _p(blob), _stream()),
           "b200_pack_w4")
-    PackedWeight._write_trailer(blob, B200_FMT_INT4, K, N, group)
-    return PackedWeight(B200_FMT_INT4, K, N, blob)
+    PackedWeight._write_trailer(blob, fmt, K, N, K if group == -1 else group)
+    return PackedWeight(fmt, K, N, blob)
 
 
 def pack_w8(q: torch.Tensor, col_scale: torch.Tensor) -> PackedWeight:

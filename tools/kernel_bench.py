@@ -70,18 +70,19 @@ def bench_attn(B, Hq, Hkv, S, T=64, nrot=3, env=None):
     return us
 
 
-def bench_gemm(fmt, B, K, N, env=None, pdl=False):
+def bench_gemm(fmt, B, K, N, env=None, pdl=False, group=128):
+    """group: quantisation group of INT4 weights (128, 64, 32); bytes count the scale and zero*scale of every group."""
     for k, v in (env or {}).items():
         os.environ[k] = str(v)
-    nm = {B200_FMT_F16: "f16", B200_FMT_INT8: "int8", B200_FMT_INT4: "int4"}[fmt]
-    wbytes = {B200_FMT_F16: 2 * K * N, B200_FMT_INT8: K * N + 2 * N, B200_FMT_INT4: K * N / 2 + K * N / 128 * 4}[fmt]
+    nm = {B200_FMT_F16: "f16", B200_FMT_INT8: "int8", B200_FMT_INT4: f"int4 g{group}"}[fmt]
+    wbytes = {B200_FMT_F16: 2 * K * N, B200_FMT_INT8: K * N + 2 * N, B200_FMT_INT4: K * N / 2 + K * N / group * 4}[fmt]
     nrot = max(2, int(300e6 // wbytes) + 1)
     ws_ = []
     for r in range(nrot):
         if fmt == B200_FMT_INT4:
             qp = torch.randint(0, 256, (K, N // 2), device=dev, dtype=torch.uint8)
-            s = (torch.randn(K // 128, N, device=dev).abs() * 0.01 + 1e-3).half()
-            w = ops.pack_w4(qp, s, s)
+            s = (torch.randn(K // group, N, device=dev).abs() * 0.01 + 1e-3).half()
+            w = ops.pack_w4(qp, s, s, group)
         elif fmt == B200_FMT_INT8:
             w = ops.pack_w8(torch.randint(-128, 128, (K, N), device=dev, dtype=torch.int8), torch.ones(N, device=dev).half())
         else:
@@ -108,7 +109,10 @@ if __name__ == "__main__":
     if which[0] == "one_attn":     # one_attn B Hq Hkv S
         bench_attn(int(which[1]), int(which[2]), int(which[3]), int(which[4]))
         sys.exit(0)
-    print(torch.cuda.get_device_name(0), "peak", PEAK)
+    import subprocess
+    power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                           capture_output=True, text=True).stdout.strip()
+    print(torch.cuda.get_device_name(0), "power limit, max SM clock:", power or "unknown", "peak", PEAK)
     if "attn" in which:
         bench_attn(32, 32, 8, 2048)
         for c in (2, 4, 8, 16, 32):
@@ -125,6 +129,13 @@ if __name__ == "__main__":
         bench_gemm(B200_FMT_INT4, 32, 4096, 28672, pdl=True)
         bench_gemm(B200_FMT_INT4, 1, 4096, 28672)
         bench_gemm(B200_FMT_INT4, 64, 4096, 28672)
+        for group in (64, 32):                        # GPTQ / AWQ checkpoints with finer groups, same Llama-3-8B shapes
+            bench_gemm(B200_FMT_INT4, 32, 4096, 6144, group=group)
+            bench_gemm(B200_FMT_INT4, 32, 4096, 4096, group=group)
+            bench_gemm(B200_FMT_INT4, 32, 4096, 28672, group=group)
+            bench_gemm(B200_FMT_INT4, 32, 14336, 4096, group=group)
+            bench_gemm(B200_FMT_INT4, 1, 4096, 28672, group=group)
+            bench_gemm(B200_FMT_INT4, 64, 4096, 28672, group=group)
         bench_gemm(B200_FMT_INT8, 32, 4096, 28672)
         bench_gemm(B200_FMT_F16, 32, 4096, 28672)
         bench_gemm(B200_FMT_F16, 32, 4096, 128256)
