@@ -55,6 +55,9 @@ uint64_t b200_launch_count(void);
  * (workspaces) and for tests of the heuristics. */
 int b200_plan_attn_split(int units, int max_seq_len, int* nsplit, int* tiles_per_split);
 int b200_plan_gemm_split(int K, int N, int* nsplit, int* k_blocks_per_split);
+/* Diagnostic: thread-block clusters of cluster_size (1..8) CTAs of the weight-only GEMM kernel (INT4 group 128, FP16, batch
+ * pad 32) that the current device holds co-resident (cudaOccupancyMaxActiveClusters). */
+int b200_wo_gemm_max_active_clusters(int cluster_size, int* num_clusters);
 
 /* ------------------------------------------------------------------------------------------------ indexing */
 
@@ -138,7 +141,8 @@ int b200_pack_w8g(const int8_t* q, const void* scales, const void* zeros_x_scale
                   void* stream);
 
 /* Scratch for split-K / stream-K partials + semaphores (+ the grid-barrier words of a stand-alone call); zero-fill once
- * after allocation. Always required for INT8 / INT4 weights (at least 16 KiB). */
+ * after allocation (the kernels leave the semaphores at zero). Required for INT8 / INT4 weights, and for any weight format
+ * whose split-K plan splits K (at least 24 KiB); b200_wo_gemm rejects a smaller one. */
 size_t b200_wo_gemm_workspace_bytes(int max_batch, int N, int K);
 
 /* Y[B][N] = X[B][K] . W' (+ bias).  The compute behind LinearBase.forward

@@ -19,6 +19,7 @@ SIGNATURES = {
     "b200_set_pdl": (c_int, [c_int]),
     "b200_plan_attn_split": (c_int, [c_int, c_int, c_void_p, c_void_p]),
     "b200_plan_gemm_split": (c_int, [c_int, c_int, c_void_p, c_void_p]),
+    "b200_wo_gemm_max_active_clusters": (c_int, [c_int, c_void_p]),
     "b200_convert_block_table": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "b200_paged_attn_plan": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_void_p] * 5 + [c_void_p]),
     "b200_paged_decode_attn_workspace_bytes": (c_size_t, [c_size_t] * 4),

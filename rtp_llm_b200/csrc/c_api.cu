@@ -163,7 +163,9 @@ AttnWorkspace attn_workspace(size_t batch, size_t head_num, size_t kv_head_num, 
 // ---- GEMM launch shape
 int gemm_bpad(int B) { return B <= 16 ? 16 : (B <= 32 ? 32 : (B <= 64 ? 64 : 128)); }
 // one-kernel-per-GEMM path (gemm_cluster.cu): split-K so that one wave of 2*SMs CTAs is filled. The nsplit CTAs of a tile
-// form one thread-block cluster (at most 8, the portable cluster size) and must be co-scheduled inside one GPC.
+// merge their partials through L2 (at most 8 slots; the reduce-scatter GEMM merges them in a thread-block cluster, and 8 is
+// the portable cluster size). The GPC rule below stays from the cluster merge, which needs a cluster's CTAs in one GPC: it
+// keeps the plan of the two merges the same, so the reduce-scatter GEMM and the plain one give the same bits.
 constexpr int kGemmMaxSplit = 8;
 void gemm_split(int n_tiles, int k_blocks, int* nsplit, int* kb_per_split) {
     const int forced = env_int("B200_GEMM_SPLITK", 0);
@@ -191,7 +193,18 @@ void gemm_split(int n_tiles, int k_blocks, int* nsplit, int* kb_per_split) {
     *kb_per_split = kbp;
     *nsplit = (k_blocks + kbp - 1) / kbp;
 }
-constexpr size_t kGemmSemBytes = 16384;      // persistent kernel's split-K counters: [0, 2048) tile arrivals, [2048, 4096) departures
+// Counters at the head of the GEMM workspace, partials after them. [0, 16384): the persistent kernel's split-K counters (int
+// [0, 2048) tile arrivals, [2048, 4096) departures); [16384, 24576): the plain kernel's tile arrivals (l2_merge). Apart, because
+// a decode program runs plain GEMMs (INT8G, INT4 g64 / g32) next to persistent-kernel ops on the same workspace.
+constexpr size_t kGemmTileSemOffset = 16384;
+constexpr size_t kGemmSemBytes = kGemmTileSemOffset + 2048 * sizeof(unsigned);
+
+// partial slots of the plain kernel's split-K plan at this batch pad: [n_tiles][nsplit][bpad * 128] fp32, none unsplit
+size_t gemm_partial_bytes(int n_tiles, int k_blocks, int bpad) {
+    int nsplit, kbp;
+    gemm_split(n_tiles, k_blocks, &nsplit, &kbp);
+    return nsplit > 1 ? (size_t)n_tiles * nsplit * bpad * kGemmTileN * sizeof(float) : 0;
+}
 
 // Split-K plan of the persistent kernel: the n_tiles*k_blocks work list is cut into runs of `per` k-blocks, one per CTA.
 // The run length is the smallest divisor of k_blocks that still gives every CTA at most one run (or whole tiles when there
@@ -575,9 +588,11 @@ int b200_pack_w8g(const int8_t* q, const void* scales, const void* zeros_x_scale
 size_t b200_wo_gemm_workspace_bytes(int max_batch, int N, int K) {
     if (max_batch <= 0 || N <= 0 || K <= 0 || K % kGemmBK) return 0;
     const int n_tiles = (N + kGemmTileN - 1) / kGemmTileN;
-    // the cluster kernel merges split-K in distributed shared memory; only the persistent kernel's partials need room, sized
-    // for its largest grid (2 CTAs per SM) and any batch <= max_batch
-    return kGemmSemBytes + sk_ws_bytes(n_tiles, K / kGemmBK, 2 * num_sms(), gemm_bpad(max_batch));
+    // partials of the plain kernel's split-K plan (any batch <= max_batch has a batch pad no larger) and of the persistent
+    // kernel's, sized for its largest grid (2 CTAs per SM); the two never run at once, so they share the room
+    const size_t plain = gemm_partial_bytes(n_tiles, K / kGemmBK, gemm_bpad(max_batch));
+    const size_t persistent = sk_ws_bytes(n_tiles, K / kGemmBK, 2 * num_sms(), gemm_bpad(max_batch));
+    return kGemmSemBytes + (plain > persistent ? plain : persistent);
 }
 
 // rs: the reduce-scatter push of b200_wo_gemm_rs, or null
@@ -611,8 +626,8 @@ static int wo_gemm_impl(int fmt, int is_bf16, const void* x, int B, int K, int N
     }
 
     // ---- weight-only INT8 / INT4 at decode batches inside a decode program: an op of the persistent kernel (uniform split-K
-    // merged through L2). Every other GEMM, and every call outside a program, uses the cluster kernel below (split-K merged
-    // through DSMEM), which needs no grid-wide barrier.
+    // merged through L2). Every other GEMM, and every call outside a program, uses the one-kernel-per-GEMM path below, which
+    // needs no grid-wide barrier.
     const bool seg_capable = (fmt == B200_FMT_INT8 || fmt == B200_FMT_INT4) && bpad <= 64;   // INT8G / INT4 g64, g32 / FP16: cluster kernel only
     if (g_rec && seg_capable && !rs) {
         ARG_CHECK(workspace && workspace_bytes >= kGemmSemBytes, "wo_gemm: workspace of at least %zu bytes required", kGemmSemBytes);
@@ -649,7 +664,7 @@ static int wo_gemm_impl(int fmt, int is_bf16, const void* x, int B, int K, int N
         });
     }
 
-    // ---- one kernel per GEMM, cluster split-K (gemm_cluster.cu)
+    // ---- one kernel per GEMM, split-K merged by the last split CTA of a tile (gemm_cluster.cu)
     GemmParams p{};
     p.w_blob = reinterpret_cast<const uint8_t*>(w);
     p.col_scale = col_scale;
@@ -662,6 +677,14 @@ static int wo_gemm_impl(int fmt, int is_bf16, const void* x, int B, int K, int N
     p.use_pdl = use_pdl ? 1 : 0;
     p.silu_mul = silu_mul ? 1 : 0;
     gemm_split(n_tiles, p.k_blocks, &p.nsplit, &p.kb_per_split);
+    if (p.nsplit > 1 && !rs) {   // split-K partials merge through the workspace (l2_merge)
+        const size_t need = kGemmSemBytes + gemm_partial_bytes(n_tiles, p.k_blocks, bpad);
+        ARG_CHECK(workspace && workspace_bytes >= need,
+                  "wo_gemm: workspace of %zu bytes too small for %d split-K partials of %d x %d (%zu bytes needed; size it "
+                  "with b200_wo_gemm_workspace_bytes)", workspace ? workspace_bytes : (size_t)0, p.nsplit, B, N, need);
+        p.tile_sem = reinterpret_cast<unsigned*>(reinterpret_cast<uint8_t*>(workspace) + kGemmTileSemOffset);
+        p.ws = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + kGemmSemBytes);
+    }
     CUtensorMap wmap;
     if (fmt == B200_FMT_F16) {
         const cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)N};

@@ -1,5 +1,6 @@
-// One-kernel-per-GEMM path (wo_gemm.cuh: cluster split-K merge through DSMEM), instantiated twice: gemm_cluster.cu (VAR 0,
-// plain output) and gemm_cluster_rs.cu (VAR 1, the epilogue pushes the TP reduce-scatter words, b200_wo_gemm_rs) -- two
+// One-kernel-per-GEMM path (wo_gemm.cuh), instantiated twice: gemm_cluster.cu (VAR 0, plain output, split-K merged through
+// L2) and gemm_cluster_rs.cu (VAR 1, the epilogue pushes the TP reduce-scatter words, b200_wo_gemm_rs; split-K merged
+// through DSMEM in a thread-block cluster) -- two
 // translation units so that the extra epilogue code cannot cost the plain kernels a register, and both compile in parallel.
 // The including file defines B200_GEMM_VAR and B200_GEMM_LAUNCH_NAME.
 #pragma once
@@ -19,8 +20,8 @@ int launch_one(const CUtensorMap& xmap, const CUtensorMap& wmap, const ParamsT& 
     constexpr int smem = gemm_smem_bytes(FMT, BPAD);
     int rc = configure_once<kern>(smem);
     if (rc) return rc;
-    // nsplit > 1: the nsplit CTAs of a tile form one cluster along y
-    const dim3 grid(n_tiles, p.nsplit), cluster(1, p.nsplit);
+    // VAR 1, nsplit > 1: the nsplit CTAs of a tile form one cluster along y; the plain kernels launch single CTAs
+    const dim3 grid(n_tiles, p.nsplit), cluster(1, B200_GEMM_VAR == 1 ? p.nsplit : 1);
     CUDA_CHECK(launch_ex(kern, {grid, dim3(gemm_threads()), smem, st, p.use_pdl != 0, cluster}, xmap, wmap, p));
     return launched("wo_gemm_kernel");
 }

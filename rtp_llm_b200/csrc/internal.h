@@ -96,10 +96,11 @@ static cudaError_t launch_ex(void (*kern)(KArgs...), const LaunchCfg& c, Args...
     return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }
 
-// gemm_cluster.cu: the one-kernel-per-GEMM path (cluster split-K merge); FP16 weights and batches > 64 use it
+// gemm_cluster.cu: the one-kernel-per-GEMM path (split-K merged through L2); FP16 weights and batches > 64 use it
 int launch_cluster_gemm(int fmt, bool bf16, int bpad, const CUtensorMap& xmap, const CUtensorMap& wmap,
                         const b200::GemmParams& p, int n_tiles, cudaStream_t st);
-// gemm_cluster_rs.cu: the same kernels with the TP reduce-scatter push in the epilogue (p.rs filled in)
+// gemm_cluster_rs.cu: the same kernels with the TP reduce-scatter push in the epilogue (p.rs filled in), split-K merged in a
+// thread-block cluster
 int launch_cluster_gemm_rs(int fmt, bool bf16, int bpad, const CUtensorMap& xmap, const CUtensorMap& wmap,
                            const b200::GemmParamsRs& p, int n_tiles, cudaStream_t st);
 

@@ -14,9 +14,10 @@
 //   * two dequant + MMA warpgroups (64 features each): dequantise IN REGISTERS (lop3 magic-number int->fp16, exact; hfma2
 //                with the group scale / zero*scale) straight into the A fragments of wgmma (m64 x N=batch pad x k16,
 //                A from registers, B = activations K-major SW128 from shared memory), fp32 accumulators in registers;
-//   * epilogue : from the accumulator registers; the split-K CTAs of a tile form a thread-block cluster and merge their fp32
-//                partials through distributed shared memory in fixed order (deterministic); bias / per-column scale /
-//                optional fused SiLU(gate)*up applied.
+//   * epilogue : from the accumulator registers; the split-K CTAs of a tile park their fp32 partials in an L2 workspace and
+//                the last one to arrive sums them in fixed split order (deterministic) and writes the tile (l2_merge); bias /
+//                per-column scale / optional fused SiLU(gate)*up applied. The reduce-scatter instances (VAR 1) merge the
+//                same partials in the same order through distributed shared memory instead, in a thread-block cluster.
 //   The FP16-weight variant feeds A from shared memory (TMA tensor map, SW128) with the same pipeline.
 #pragma once
 #include <type_traits>
@@ -94,9 +95,11 @@ struct GemmParams {
     void* y;                 // [B][N] (T)
     int B, N, K;
     int k_blocks;            // K / 128
-    int kb_per_split, nsplit;   // nsplit > 1: the nsplit CTAs of a tile form a cluster (1,nsplit,1) and merge through DSMEM
+    int kb_per_split, nsplit;   // nsplit > 1: the nsplit CTAs of a tile merge their partials (VAR 0: l2_merge; VAR 1: a cluster)
     int use_pdl;
     int silu_mul;            // 1: tile rows 2r / 2r+1 are gate / up feature tile*64+r; y[b][tile*64+r] = silu(g)*u
+    float* ws;               // VAR 0, nsplit > 1: partial slots [n_tiles][nsplit][bpad * 128] fp32
+    unsigned* tile_sem;      // VAR 0, nsplit > 1: arrival counter per tile, zero on entry and on exit
 };
 
 // The VAR == 1 kernels (gemm_cluster_rs.cu) take the descriptor of the reduce-scatter push after the common parameters; the
@@ -351,6 +354,57 @@ __device__ __forceinline__ uint64_t sw128_kstep(uint64_t desc0, int j) {
     return desc0 + (uint64_t)((j >> 2) * (BOX_BYTES >> 4) + (j & 3) * 2);
 }
 
+// Split-K merge of the plain GEMM (VAR 0) through L2, run by the dequant threads of every split CTA of a tile. Each stores its
+// fp32 partial to workspace slot (tile, split) in accumulator order, as float4 [NACC / 4][thread] (the stores and loads of a
+// warp are coalesced) and counts itself in the tile's arrival counter. The last CTA to arrive sums the nsplit slots in split order
+// 0..nsplit-1 into acc (fixed order: deterministic, and the order of the cluster merge, so both give the same bits), resets
+// the counter for the next launch and returns true; it then writes the whole tile. flag: one word of shared memory.
+// Single CTAs, unlike a cluster, need no free slots in one GPC at once, so split CTAs start as any SM frees up.
+template <int NACC, int NDQ_THREADS>
+__device__ __forceinline__ bool l2_merge(const GemmParams& p, float (&acc)[NACC], int tile, int split, uint32_t* flag) {
+    // under PDL the previous kernel, possibly a GEMM on the same workspace, has finished with it only past this wait
+    if (p.use_pdl) pdl_wait();
+    constexpr int SLOT4 = NACC / 4 * NDQ_THREADS;         // float4 per slot: [NACC / 4][thread]
+    float4* part = reinterpret_cast<float4*>(p.ws) + (size_t)tile * p.nsplit * SLOT4 + threadIdx.x;
+#pragma unroll
+    for (int j = 0; j < NACC / 4; ++j)
+        __stcg(part + split * SLOT4 + j * NDQ_THREADS, make_float4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]));
+    asm volatile("bar.sync 1, %0;" ::"n"(NDQ_THREADS) : "memory");
+    if (threadIdx.x == 0) {
+        unsigned* arrivals = p.tile_sem + tile;
+        unsigned prev;
+        asm volatile("atom.acq_rel.gpu.global.add.u32 %0, [%1], 1;" : "=r"(prev) : "l"(arrivals) : "memory");
+        const bool last = prev == (unsigned)(p.nsplit - 1);
+        if (last) *arrivals = 0;   // every split has arrived: no one else touches the counter in this launch
+        *flag = last;
+    }
+    asm volatile("bar.sync 1, %0;" ::"n"(NDQ_THREADS) : "memory");
+    if (!*flag) return false;
+    // the loads of all splits of a float4 go out together, so the merge waits about NACC / 4 L2 round trips, not nsplit
+    const int S = p.nsplit;
+#pragma unroll
+    for (int j = 0; j < NACC / 4; ++j) {
+        float4 v[8];
+#pragma unroll
+        for (int sp = 0; sp < 8; ++sp)
+            if (sp < S) v[sp] = __ldcg(part + sp * SLOT4 + j * NDQ_THREADS);
+        float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+        for (int sp = 0; sp < 8; ++sp)
+            if (sp < S) {
+                a.x += v[sp].x;
+                a.y += v[sp].y;
+                a.z += v[sp].z;
+                a.w += v[sp].w;
+            }
+        acc[4 * j] = a.x;
+        acc[4 * j + 1] = a.y;
+        acc[4 * j + 2] = a.z;
+        acc[4 * j + 3] = a.w;
+    }
+    return true;
+}
+
 template <int FMT, typename T, int BPAD, int VAR>
 __global__ void __launch_bounds__(gemm_threads(), gemm_min_ctas(FMT, BPAD))
 wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant__ CUtensorMap w_map,
@@ -538,20 +592,34 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
         asm volatile("bar.sync 1, %0;" ::"n"(NDQ_THREADS) : "memory");
 
         // ------------------------------------------------------------------ epilogue
+        bool own = true;   // this CTA writes the tile
+        if constexpr (VAR == 0) {
+            if (p.nsplit > 1) own = l2_merge<NACC, NDQ_THREADS>(p, acc, tile, split, reinterpret_cast<uint32_t*>(xempty + XS));
+        }
         // this thread's accumulators: rows[h] (h = 0, 1) x batch columns 8i + 2*t4 + c, value acc[4i + 2h + c]
         const int rows[2] = {16 * R + (lane >> 2), 16 * R + (lane >> 2) + 8};
         T* yp = reinterpret_cast<T*>(p.y);
-        float cscale[2] = {1.f, 1.f}, bias[2] = {0.f, 0.f};
+        if (VAR == 1 && p.nsplit > 1) {
+            // split-K merge through distributed shared memory: park the fp32 partial tile [bpad][128] in this CTA's smem
+            // (the activation ring is idle now); the merge itself follows the cluster barrier below.
+            float* red = reinterpret_cast<float*>(xring);
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int n = tile * kGemmTileN + rows[h];
-            if (n < p.N) {
-                if (FMT == kFmtInt8) cscale[h] = to_f32<T>(reinterpret_cast<const T*>(p.col_scale)[n]);
-                if (p.bias) bias[h] = to_f32<T>(reinterpret_cast<const T*>(p.bias)[n]);
+            for (int i = 0; i < BPAD / 8; ++i)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int c = 0; c < 2; ++c) red[(8 * i + 2 * t4 + c) * kGemmTileN + rows[h]] = acc[4 * i + 2 * h + c];
+        } else if (own) {
+            float cscale[2] = {1.f, 1.f}, bias[2] = {0.f, 0.f};
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int n = tile * kGemmTileN + rows[h];
+                if (n < p.N) {
+                    if (FMT == kFmtInt8) cscale[h] = to_f32<T>(reinterpret_cast<const T*>(p.col_scale)[n]);
+                    if (p.bias) bias[h] = to_f32<T>(reinterpret_cast<const T*>(p.bias)[n]);
+                }
             }
-        }
-        float* fin = reinterpret_cast<float*>(wring);       // [bpad][128] fp32 staging for the fused SiLU*mul (weight ring is idle)
-        if (p.nsplit == 1) {
+            float* fin = reinterpret_cast<float*>(wring);       // [bpad][128] fp32 staging for the fused SiLU*mul (weight ring is idle)
             RsLane rsl[2] = {};
             if constexpr (VAR == 1) {
                 rsl[0] = rs_lane(p, tile * kGemmTileN + rows[0]);
@@ -569,71 +637,52 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
                         else if constexpr (VAR == 1) rs_emit<T>(p, rsl[h], b, n, v, lane, 4);   // N % 128 == 0 in this mode
                         else if (n < p.N && b < p.B) yp[(size_t)b * p.N + n] = from_f32<T>(v);
                     }
-        } else {
-            // split-K merge through distributed shared memory: park the fp32 partial tile [bpad][128] in this CTA's smem
-            // (the activation ring is idle now); the merge itself follows the cluster barrier below.
-            float* red = reinterpret_cast<float*>(xring);
-#pragma unroll
-            for (int i = 0; i < BPAD / 8; ++i)
-#pragma unroll
-                for (int h = 0; h < 2; ++h)
-#pragma unroll
-                    for (int c = 0; c < 2; ++c) red[(8 * i + 2 * t4 + c) * kGemmTileN + rows[h]] = acc[4 * i + 2 * h + c];
+            if (p.silu_mul) {
+                // fused SiLU(gate) * up (replaces rtp_llm_ops.silu_and_mul after the w13 GEMM, modules/hybrid/dense_mlp.py:95-106)
+                asm volatile("bar.sync 1, %0;" ::"n"(NDQ_THREADS) : "memory");
+                const int n_out = p.N / 2;
+                for (int idx = threadIdx.x; idx < BPAD * 64; idx += NDQ_THREADS) {
+                    const int b = idx >> 6, r = idx & 63;
+                    const int j = tile * 64 + r;
+                    if (b >= p.B || j >= n_out) continue;
+                    const float g = fin[b * kGemmTileN + 2 * r], u = fin[b * kGemmTileN + 2 * r + 1];   // rows 2r / 2r+1 = gate / up pair
+                    yp[(size_t)b * n_out + j] = from_f32<T>(__fdividef(g, 1.f + __expf(-g)) * u);   // fast divide: <= 2 ulp in fp32, below the rounding of the result
+                }
+            }
         }
     }
 
-    if (p.nsplit > 1) {
-        // every thread of every CTA of the cluster (1, nsplit, 1) passes both barriers
-        cluster_sync_all();
-        if (warp < NDQ_WARPS) {
-            const int S = p.nsplit;
-            const int rank = (int)cluster_ctarank();          // == blockIdx.y
-            const int row = threadIdx.x & (kGemmTileN - 1);
-            const int lane_grp = threadIdx.x >> 7;             // NDQ_THREADS / 128 column lanes
-            const int n = tile * kGemmTileN + row;
-            const bool n_ok = n < p.N;
-            float cscale = 1.f, bias = 0.f;
-            if (n_ok) {
-                if (FMT == kFmtInt8) cscale = to_f32<T>(reinterpret_cast<const T*>(p.col_scale)[n]);
-                if (p.bias) bias = to_f32<T>(reinterpret_cast<const T*>(p.bias)[n]);
-            }
-            const float* red = reinterpret_cast<const float*>(xring);
-            T* yp = reinterpret_cast<T*>(p.y);
-            RsLane rsl{};
-            if constexpr (VAR == 1) rsl = rs_lane(p, n);
-            // CTA `rank` owns batch columns rank, rank+S, ...; fixed summation order sp = 0..S-1 (deterministic)
-            for (int b = rank + lane_grp * S; b < p.B; b += S * (NDQ_THREADS / kGemmTileN)) {
-                const uint32_t laddr = smem_u32(red + b * kGemmTileN + row);
-                float part[8];
+    if constexpr (VAR == 1) {
+        if (p.nsplit > 1) {
+            // every thread of every CTA of the cluster (1, nsplit, 1) passes both barriers (the reduce-scatter GEMM never
+            // fuses SiLU*mul)
+            cluster_sync_all();
+            if (warp < NDQ_WARPS) {
+                const int S = p.nsplit;
+                const int rank = (int)cluster_ctarank();          // == blockIdx.y
+                const int row = threadIdx.x & (kGemmTileN - 1);
+                const int lane_grp = threadIdx.x >> 7;             // NDQ_THREADS / 128 column lanes
+                const int n = tile * kGemmTileN + row;
+                float cscale = 1.f, bias = 0.f;
+                if (n < p.N) {
+                    if (FMT == kFmtInt8) cscale = to_f32<T>(reinterpret_cast<const T*>(p.col_scale)[n]);
+                    if (p.bias) bias = to_f32<T>(reinterpret_cast<const T*>(p.bias)[n]);
+                }
+                const float* red = reinterpret_cast<const float*>(xring);
+                const RsLane rsl = rs_lane(p, n);
+                // CTA `rank` owns batch columns rank, rank+S, ...; fixed summation order sp = 0..S-1 (deterministic)
+                for (int b = rank + lane_grp * S; b < p.B; b += S * (NDQ_THREADS / kGemmTileN)) {
+                    const uint32_t laddr = smem_u32(red + b * kGemmTileN + row);
+                    float part[8];
 #pragma unroll
-                for (int sp = 0; sp < 8; ++sp) part[sp] = sp < S ? dsmem_ld_f32(dsmem_addr(laddr, sp)) : 0.f;
-                float acc = 0.f;
+                    for (int sp = 0; sp < 8; ++sp) part[sp] = sp < S ? dsmem_ld_f32(dsmem_addr(laddr, sp)) : 0.f;
+                    float acc = 0.f;
 #pragma unroll
-                for (int sp = 0; sp < 8; ++sp) acc += part[sp];
-                if (p.silu_mul) reinterpret_cast<float*>(wring)[b * kGemmTileN + row] = fmaf(acc, cscale, bias);
-                else if constexpr (VAR == 1) rs_emit<T>(p, rsl, b, n, fmaf(acc, cscale, bias), lane, 1);
-                else if (n_ok) yp[(size_t)b * p.N + n] = from_f32<T>(fmaf(acc, cscale, bias));
+                    for (int sp = 0; sp < 8; ++sp) acc += part[sp];
+                    rs_emit<T>(p, rsl, b, n, fmaf(acc, cscale, bias), lane, 1);
+                }
             }
-        }
-        cluster_sync_all();   // peers may still be reading this CTA's partial
-    }
-    if (p.silu_mul) {
-        // fused SiLU(gate) * up (replaces rtp_llm_ops.silu_and_mul after the w13 GEMM, modules/hybrid/dense_mlp.py:95-106)
-        __syncthreads();
-        if (warp < NDQ_WARPS) {
-            const float* fin = reinterpret_cast<const float*>(wring);
-            T* yp = reinterpret_cast<T*>(p.y);
-            const int n_out = p.N / 2;
-            const int S = p.nsplit;
-            const int rank = S > 1 ? (int)cluster_ctarank() : 0;
-            for (int idx = threadIdx.x; idx < BPAD * 64; idx += NDQ_THREADS) {
-                const int b = idx >> 6, r = idx & 63;
-                if (b >= p.B || (b % S) != rank) continue;      // with a cluster merge each CTA owns the columns b % S == rank
-                const int j = tile * 64 + r;
-                if (j >= n_out) continue;
-                const float g = fin[b * kGemmTileN + 2 * r], u = fin[b * kGemmTileN + 2 * r + 1];   // rows 2r / 2r+1 = gate / up pair
-                yp[(size_t)b * n_out + j] = from_f32<T>(__fdividef(g, 1.f + __expf(-g)) * u);   // fast divide: <= 2 ulp in fp32, below the rounding of the result
-            }
+            cluster_sync_all();   // peers may still be reading this CTA's partial
         }
     }
     __syncthreads();

@@ -113,6 +113,20 @@ if __name__ == "__main__":
     power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
                            capture_output=True, text=True).stdout.strip()
     print(torch.cuda.get_device_name(0), "power limit, max SM clock:", power or "unknown", "peak", PEAK)
+    if "clusters" in which:
+        # co-resident clusters of the INT4 g128 batch-pad-32 GEMM kernel: a split-K cluster of S CTAs needs S slots in ONE GPC
+        import ctypes
+        from rtp_llm_b200 import _lib
+        for size in (1, 2, 4, 8):
+            n = ctypes.c_int(0)
+            _lib.check(_lib.load().b200_wo_gemm_max_active_clusters(size, ctypes.byref(n)), "wo_gemm_max_active_clusters")
+            print(f"clusters of {size}: {n.value} co-resident ({n.value * size} CTAs, {torch.cuda.get_device_properties(0).multi_processor_count} SMs)",
+                  flush=True)
+    if "splits" in which:
+        # o and w2 of Llama-3-8B at B32 with every split-K the plan may pick
+        for K, N in ((4096, 4096), (14336, 4096)):
+            for s in (1, 2, 4, 8):
+                bench_gemm(B200_FMT_INT4, 32, K, N, env={"B200_GEMM_SPLITK": s})
     if "attn" in which:
         bench_attn(32, 32, 8, 2048)
         for c in (2, 4, 8, 16, 32):
