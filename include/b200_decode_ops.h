@@ -168,6 +168,11 @@ int b200_qk_rmsnorm(void* qkv, const void* q_gamma, const void* k_gamma, const v
                     int rows, int head_num, int kv_head_num, int head_dim, float eps, void* stream);
 /* silu_and_mul: y[r][c] = silu(gate_up[r][c]) * gate_up[r][inter + c]. */
 int b200_silu_and_mul(const void* gate_up, void* y, int is_bf16, int rows, int inter, void* stream);
+/* Column gather y[r][j] = x[r][perm[j]] over x, y [rows][K] fp16 / bf16 (a bit copy): the input of a GEMM whose weight is a GPTQ
+ * act-order (desc_act) weight with its rows sorted by g_idx. perm int32 [K] is a permutation of 0..K-1 (not checked here: it
+ * is checked once when the weight is packed). x != y; K % 8 == 0, K <= 65536; x, perm, y 16-byte aligned. Inside a decode
+ * program it is its own launch. */
+int b200_permute_cols(const void* x, const int32_t* perm, void* y, int is_bf16, int rows, int K, void* stream);
 /* FusedRopeKVCacheDecodeOp.forward (rtp_llm/ops/fused_rope_kvcache_op.py:202-246), RopeStyle::Base, NeoX pairing:
  * rotates q and k of qkv [B][(Hq+2Hkv)*D] at position sequence_lengths[b], writes q to q_out [B][Hq*D] and K,V of the
  * new token into the paged cache. */

@@ -41,6 +41,7 @@ SIGNATURES = {
     "b200_add_rmsnorm": (c_int, [c_void_p] * 4 + [c_int, c_int, c_int, c_float, c_void_p]),
     "b200_qk_rmsnorm": (c_int, [c_void_p] * 5 + [c_int] * 5 + [c_float, c_void_p]),
     "b200_silu_and_mul": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "b200_permute_cols": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "b200_rope_append": (c_int, [c_void_p] * 5 + [c_int] * 7 + [c_float, c_void_p]),
     "b200_rope_append_ex": (c_int, [c_void_p] * 8 + [c_int, c_void_p] + [c_int] * 8 + [c_void_p]),
     "b200_embedding": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),

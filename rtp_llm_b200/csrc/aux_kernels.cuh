@@ -374,6 +374,38 @@ __global__ void rope_append_ex_kernel(const T* __restrict__ qkv, const T* __rest
     }
 }
 
+// Column gather y[r][j] = x[r][perm[j]] (the activation side of a GPTQ act-order weight whose rows were sorted by g_idx).
+// A bit copy of 16-bit values, so one kernel serves fp16 and bf16. One CTA per row: the row is staged in shared memory
+// through 16-byte loads, then each thread gathers 8 columns and writes them as one 16-byte vector. K % 8 == 0, x / y / perm
+// 16-byte aligned, perm a permutation of 0..K-1 (checked on the host when the weight is packed). perm is constant after load,
+// so the first indices are read before the PDL wait; nothing is written before it.
+static __global__ void permute_cols_kernel(const uint16_t* __restrict__ x, const int32_t* __restrict__ perm,
+                                           uint16_t* __restrict__ y, int K) {
+    pdl_launch_dependents();
+    extern __shared__ uint4 s_row4[];
+    const uint16_t* s_row = reinterpret_cast<const uint16_t*>(s_row4);
+    const int K8 = K / 8;
+    const int4* pv = reinterpret_cast<const int4*>(perm);
+    int4 p0 = make_int4(0, 0, 0, 0), p1 = p0;
+    if ((int)threadIdx.x < K8) {
+        p0 = pv[2 * threadIdx.x];
+        p1 = pv[2 * threadIdx.x + 1];
+    }
+    pdl_wait();
+    const uint4* xv = reinterpret_cast<const uint4*>(x + (size_t)blockIdx.x * K);
+    for (int i = threadIdx.x; i < K8; i += blockDim.x) s_row4[i] = xv[i];
+    __syncthreads();
+    uint4* yv = reinterpret_cast<uint4*>(y + (size_t)blockIdx.x * K);
+    for (int j = threadIdx.x; j < K8; j += blockDim.x) {
+        if (j != (int)threadIdx.x) {
+            p0 = pv[2 * j];
+            p1 = pv[2 * j + 1];
+        }
+        yv[j] = make_uint4(s_row[p0.x] | ((uint32_t)s_row[p0.y] << 16), s_row[p0.z] | ((uint32_t)s_row[p0.w] << 16),
+                           s_row[p1.x] | ((uint32_t)s_row[p1.y] << 16), s_row[p1.z] | ((uint32_t)s_row[p1.w] << 16));
+    }
+}
+
 // token embedding gather: out[b][:] = table[ids[b]][:]
 template <typename T>
 __global__ void embedding_kernel(const int32_t* __restrict__ ids, const T* __restrict__ table, T* __restrict__ out,

@@ -794,6 +794,26 @@ int b200_silu_and_mul(const void* gate_up, void* y, int is_bf16, int rows, int i
     });
 }
 
+// the staged row is K 16-bit values in shared memory: 128 KB at the limit
+static constexpr int kPermuteMaxK = 65536;
+
+int b200_permute_cols(const void* x, const int32_t* perm, void* y, int is_bf16, int rows, int K, void* stream) {
+    (void)is_bf16;   // a bit copy of 16-bit values: the same kernel serves both dtypes
+    if (rows == 0) return B200_OK;
+    ARG_CHECK(x && perm && y, "permute_cols: null pointer");
+    ARG_CHECK(x != y, "permute_cols: x and y must not be the same buffer (the gather cannot run in place)");
+    ARG_CHECK(rows > 0, "permute_cols: rows=%d must be positive", rows);
+    ARG_CHECK(K > 0 && K % 8 == 0 && K <= kPermuteMaxK, "permute_cols: K=%d must be a positive multiple of 8, <= %d", K, kPermuteMaxK);
+    ARG_CHECK((((uintptr_t)x | (uintptr_t)y | (uintptr_t)perm) & 15) == 0, "permute_cols: x / perm / y must be 16-byte aligned");
+    if (g_rec) return rec_call([=](void* st) { return b200_permute_cols(x, perm, y, is_bf16, rows, K, st); });
+    const int rc = configure_once<permute_cols_kernel>(kPermuteMaxK * 2);
+    if (rc) return rc;
+    const int threads = K / 8 >= 512 ? 512 : (K / 8 >= 256 ? 256 : 128);
+    CUDA_CHECK(launch_ex(permute_cols_kernel, {dim3(rows), dim3(threads), (size_t)K * 2, (cudaStream_t)stream, g_pdl.load() != 0},
+                         (const uint16_t*)x, perm, (uint16_t*)y, K));
+    return launched("permute_cols_kernel");
+}
+
 int b200_rope_append(const void* qkv, void* q_out, void* kv_pool, const int32_t* page_list,
                      const int32_t* sequence_lengths, int is_bf16, int batch, int head_num, int kv_head_num,
                      int head_dim, int max_blocks_per_seq, int page_size, float rope_base, void* stream) {

@@ -60,13 +60,21 @@ def weight_bytes(cfg: ModelConfig, K: int, N: int) -> float:
 
 class DecodeStep:
     """Synthetic decode step. tp_size > 1 shards exactly as the reference's TP split (utils/model_weight.py:1489-1580):
-    qkv / w13 column-parallel, o / w2 row-parallel + all-reduce, lm_head vocab-parallel + all-gather."""
+    qkv / w13 column-parallel, o / w2 row-parallel + all-reduce, lm_head vocab-parallel + all-gather.
+
+    act_order=True (TP 1, quant int4 / int8g): every quantised weight is a GPTQ act-order weight with its rows sorted by g_idx,
+    from seeded random row orders. qkv, o and w13 carry theirs in the blob, and x is gathered (b200_permute_cols) into a static
+    buffer before each of them; w2's order is folded into w13's output columns, as B200Loader.layer does. A row-parallel o
+    shard would mix groups of every rank, so TP > 1 is rejected."""
 
     def __init__(self, cfg: ModelConfig, batch: int, ctx: int, device: torch.device, tp_rank: int = 0, tp_size: int = 1,
                  dtype=torch.float16, seed: int = 0, keep_reference: bool = False, ragged: bool = False,
                  pdl: bool = False, comm=None, fuse_silu: bool = True, fuse_ar_norm: bool = True, fuse_rope: Optional[bool] = None,
-                 fuse_gemm_rs: Optional[bool] = None):
+                 fuse_gemm_rs: Optional[bool] = None, act_order: bool = False):
         assert cfg.head_num % tp_size == 0 and cfg.inter % tp_size == 0
+        if act_order and (tp_size != 1 or cfg.quant not in ("int4", "int8g")):
+            raise ValueError(f"act_order needs tp_size 1 and quant int4 / int8g (got tp_size {tp_size}, quant {cfg.quant})")
+        self.act_order = act_order
         self.cfg, self.B, self.ctx, self.dev, self.dtype = cfg, batch, ctx, device, dtype
         self.tp_rank, self.tp_size, self.comm, self.pdl = tp_rank, tp_size, comm, pdl
         self.Hq = cfg.head_num // tp_size
@@ -97,22 +105,22 @@ class DecodeStep:
         g = torch.Generator(device="cpu").manual_seed(seed * 1000 + 17)
         H = cfg.hidden
 
-        def pack_ref(refw, gate_up_inter: int = 0):
+        def pack_ref(refw, gate_up_inter: int = 0, perm=None, col_perm=None):
             """Reference-layout tuple -> kernel layout. gate_up_inter > 0: a [K, 2I] gate|up weight whose columns are
-            first interleaved per 64 outputs so the GEMM epilogue can apply SiLU(gate)*up (ops.interleave_gate_up)."""
+            first interleaved per 64 outputs so the GEMM epilogue can apply SiLU(gate)*up (ops.interleave_gate_up).
+            perm: act-order row order carried by the blob; col_perm: w2's row order folded into a gate|up weight's columns."""
             fmt, w, s, zs = refw
             gi = gate_up_inter
-            if fmt == "int4":
+            if fmt in ("int4", "int8g"):
                 w, s, zs = w.to(device), s.to(device), zs.to(device)
+                if col_perm is not None:
+                    order = torch.cat([col_perm, col_perm + s.shape[1] // 2])
+                    w = ops.permute_columns(w, order, packed_int4=fmt == "int4")
+                    s, zs = ops.permute_columns(s, order), ops.permute_columns(zs, order)
                 if gi:
-                    w, s, zs = (ops.interleave_gate_up(w, gi, packed_int4=True), ops.interleave_gate_up(s, gi),
+                    w, s, zs = (ops.interleave_gate_up(w, gi, packed_int4=fmt == "int4"), ops.interleave_gate_up(s, gi),
                                 ops.interleave_gate_up(zs, gi))
-                return ops.pack_w4(w, s, zs)
-            if fmt == "int8g":
-                w, s, zs = w.to(device), s.to(device), zs.to(device)
-                if gi:
-                    w, s, zs = ops.interleave_gate_up(w, gi), ops.interleave_gate_up(s, gi), ops.interleave_gate_up(zs, gi)
-                return ops.pack_w8g(w, s, zs)
+                return (ops.pack_w4 if fmt == "int4" else ops.pack_w8g)(w, s, zs, perm=perm)
             if fmt == "int8":
                 w, s = w.to(device), s.to(device)
                 if gi:
@@ -123,7 +131,8 @@ class DecodeStep:
                 w = ops.interleave_gate_up(w, gi)
             return ops.pack_f16(w)
 
-        def make_weight(K: int, N: int, gen_seed: int, quant: Optional[str] = None, gate_up_inter: int = 0):
+        def make_weight(K: int, N: int, gen_seed: int, quant: Optional[str] = None, gate_up_inter: int = 0, perm=None,
+                        col_perm=None):
             quant = quant or cfg.quant
             gg = torch.Generator(device=device).manual_seed(gen_seed)
             if quant == "int4":
@@ -145,7 +154,7 @@ class DecodeStep:
             else:
                 wkn = (torch.randn(K, N, generator=gg, device=device) * 0.02).to(dtype)
                 refw = ("f16", wkn, None, None)
-            w = pack_ref(refw, gate_up_inter)
+            w = pack_ref(refw, gate_up_inter, perm, col_perm)
             return w, (tuple(t.cpu() if torch.is_tensor(t) else t for t in refw) if keep_reference else None)
 
         self.layers: List[dict] = []
@@ -168,9 +177,16 @@ class DecodeStep:
                 L["w13"] = pack_ref(r2, self.inter if self.fuse_silu else 0)
                 L["full"] = dict(qkv=f0, o=f1, w13=f2, w2=f3)
             else:
-                L["qkv"], r0 = make_weight(H, qkv_n, base + 1)
-                L["o"], r1 = make_weight(self.Hq * self.D, H, base + 2)
-                L["w13"], r2 = make_weight(H, 2 * self.inter, base + 3, gate_up_inter=self.inter if self.fuse_silu else 0)
+                P = {}
+                if act_order:
+                    ga = torch.Generator().manual_seed(base + 9)
+                    P = dict(qkv=torch.randperm(H, generator=ga), o=torch.randperm(self.Hq * self.D, generator=ga),
+                             w13=torch.randperm(H, generator=ga), w2=torch.randperm(self.inter, generator=ga))
+                    L["perm"] = P
+                L["qkv"], r0 = make_weight(H, qkv_n, base + 1, perm=P.get("qkv"))
+                L["o"], r1 = make_weight(self.Hq * self.D, H, base + 2, perm=P.get("o"))
+                L["w13"], r2 = make_weight(H, 2 * self.inter, base + 3, gate_up_inter=self.inter if self.fuse_silu else 0,
+                                           perm=P.get("w13"), col_perm=P.get("w2"))
                 L["w2"], r3 = make_weight(self.inter, H, base + 4)
             L["ln1"] = (1.0 + 0.1 * torch.randn(H, generator=g)).to(dtype).to(device)
             L["ln2"] = (1.0 + 0.1 * torch.randn(H, generator=g)).to(dtype).to(device)
@@ -231,6 +247,8 @@ class DecodeStep:
         self.logits = buf(batch, self.vocab)
         self.logits_all = buf(tp_size, batch, self.vocab) if tp_size > 1 else None
         self.next_ids = buf(batch, dt=torch.int32)
+        self.x_perm = buf(batch, H) if act_order else None                    # x[:, perm] before qkv / w13
+        self.attn_perm = buf(batch, self.Hq * self.D) if act_order else None  # attn[:, perm] before o
         shapes = [(H, qkv_n), (self.Hq * self.D, H), (H, 2 * self.inter), (self.inter, H), (H, self.vocab)]
         self.gemm_ws = ops.gemm_workspace(batch, shapes, device)
         self.attn_ws = ops.attn_workspace(batch, self.Hq, self.Hkv, ctx, device)
@@ -267,7 +285,7 @@ class DecodeStep:
         if self.fuse_gemm_rs and hasattr(self.comm, "gemm_rs"):    # (bench.py swaps the communicator for its NCCL parity arm)
             self.comm.gemm_rs(x, w, self.gemm_ws, self.proj, pdl=self.pdl)
         else:
-            ops.wo_gemm(x, w, self.gemm_ws, out=self.proj, pdl=self.pdl)
+            ops.wo_gemm(x, w, self.gemm_ws, out=self.proj, pdl=self.pdl, x_perm=self.attn_perm)
 
     def _ar_norm(self, t, gamma):
         """[TP all-reduce of the row-parallel GEMM output t] + residual add + RMSNorm -> self.x. With the peer communicator the
@@ -295,7 +313,7 @@ class DecodeStep:
                 first = False
             else:
                 self._ar_norm(self.proj, L["ln1"])          # all-reduce of the previous layer's w2 output rides along
-            ops.wo_gemm(self.x, L["qkv"], self.gemm_ws, out=self.qkv, pdl=self.pdl)
+            ops.wo_gemm(self.x, L["qkv"], self.gemm_ws, out=self.qkv, pdl=self.pdl, x_perm=self.x_perm)
             if self.fuse_rope:    # RoPE + K/V append inside the attention kernel (one launch instead of two)
                 ops.paged_decode_attn_rope(self.qkv, L["kv"], self.page_list, self.seq_lens, self.Hq, self.ctx, cfg.rope_base,
                                            self.attn_ws, out=self.attn)
@@ -305,9 +323,9 @@ class DecodeStep:
             self._row_gemm(self.attn, L["o"])
             self._ar_norm(self.proj, L["ln2"])
             if self.fuse_silu:     # SiLU(gate)*up in the GEMM epilogue (gate/up columns interleaved at load time)
-                ops.wo_gemm(self.x, L["w13"], self.gemm_ws, out=self.act, pdl=self.pdl, silu_mul=True)
+                ops.wo_gemm(self.x, L["w13"], self.gemm_ws, out=self.act, pdl=self.pdl, silu_mul=True, x_perm=self.x_perm)
             else:
-                ops.wo_gemm(self.x, L["w13"], self.gemm_ws, out=self.gu, pdl=self.pdl)
+                ops.wo_gemm(self.x, L["w13"], self.gemm_ws, out=self.gu, pdl=self.pdl, x_perm=self.x_perm)
                 ops.silu_and_mul(self.gu, out=self.act)
             self._row_gemm(self.act, L["w2"])
         self._ar_norm(self.proj, self.final_ln)

@@ -34,6 +34,35 @@ def pack_int8_tensor_to_packed_int4(t: torch.Tensor) -> torch.Tensor:
     return (u[:, 1::2] * 16 + u[:, ::2]).contiguous()
 
 
+def act_order_perm(g_idx, group: int, K: int):
+    """Row order of a GPTQ act-order (desc_act) weight: `perm` int64 [K] with sorted row j = checkpoint row perm[j] (a stable
+    argsort of g_idx), so that group r becomes rows [r*group, (r+1)*group) and the usual blob formats serve the weight; the
+    GEMM then consumes x[:, perm]. None when g_idx is absent or trivial (g_idx[k] == k // group: static groups, no act-order,
+    per channel), so those weights take the unpermuted path bit for bit. group -1 means per channel (group = K).
+
+    AutoGPTQ stores g_idx in the checkpoint's row order, g_idx[k] = (rank of k in the act-order) // group, so every group has
+    exactly `group` rows; anything else is not a checkpoint this layout can serve and raises ValueError."""
+    if g_idx is None:
+        return None
+    if group == -1:
+        group = K
+    g = torch.as_tensor(g_idx).detach().to("cpu", torch.int64).reshape(-1)
+    if group <= 0 or K % group:
+        raise ValueError(f"g_idx: group size {group} does not divide K={K}")
+    if g.numel() != K:
+        raise ValueError(f"g_idx has {g.numel()} entries, expected K={K}")
+    groups = K // group
+    if g.numel() and (int(g.min()) < 0 or int(g.max()) >= groups):
+        raise ValueError(f"g_idx values must lie in [0, {groups}) (K={K}, group {group}), got [{int(g.min())}, {int(g.max())}]")
+    counts = torch.bincount(g, minlength=groups)
+    if not bool((counts == group).all()):
+        r = int(torch.nonzero(counts != group)[0])
+        raise ValueError(f"g_idx: group {r} has {int(counts[r])} rows, every group must have exactly {group}")
+    if torch.equal(g, torch.arange(K) // group):
+        return None
+    return torch.sort(g, stable=True).indices
+
+
 class B200Impl:
     """Drop-in for CudaImpl's weight hooks. The returned `kernel` tensors are self-describing blobs (ops.PackedWeight: a
     trailer inside the tensor names format / K / N), so they survive the loader's `.contiguous().to(device)`, clones and
@@ -81,15 +110,23 @@ class B200Impl:
         return q_out, zeros_x_scales, scales
 
     def preprocess_groupwise_weight_params(self, qweight_int32, qzeros_int32, scales_fp16, device: str, gptq: bool,
-                                           awq: bool, weight_bits: int):
+                                           awq: bool, weight_bits: int, g_idx=None):
+        """g_idx: a GPTQ checkpoint's `.g_idx` (act-order). The rows are sorted by it and the blob carries the order
+        (act_order_perm); None or a trivial g_idx gives the plain blob."""
         q_packed, zs, scales = self.unpack_groupwise(qweight_int32, qzeros_int32, scales_fp16, gptq, awq, weight_bits)
+        perm = None
+        if g_idx is not None:
+            K, rows = q_packed.shape[0], scales.reshape(scales.shape[0], -1).shape[0]
+            perm = act_order_perm(g_idx, K // rows if rows and K % rows == 0 else 0, K)
+            if perm is not None:
+                q_packed = q_packed[perm.to(q_packed.device)]
         kernel = self.preprocess_weights_for_mixed_gemm(q_packed, torch.int8 if weight_bits == 8 else torch.quint4x2, scales=scales,
-                                                        zeros_x_scales=zs)
+                                                        zeros_x_scales=zs, perm=perm)
         return kernel, zs.to(self.device), scales.to(self.device)
 
     # -- replaces device_impl.py:392-479
     def preprocess_weights_for_mixed_gemm(self, tensor: torch.Tensor, quant_mode, arch: str = "", scales=None,
-                                          zeros_x_scales=None):
+                                          zeros_x_scales=None, perm=None):
         if quant_mode == torch.int8 and zeros_x_scales is None:
             raise ValueError("INT8 per-column weights are packed by apply_int8 (the scale rides along)")
         assert scales is not None and zeros_x_scales is not None, "the b200 group-wise blobs carry scales and zero*scale"
@@ -103,10 +140,10 @@ class B200Impl:
                 raise ValueError(f"8-bit group-wise weights: group size {group or f'K/{rows}'} unsupported (128 only; K={K}, "
                                  f"{rows} scale rows)")
             return ops.pack_w8g(tensor.to(self.device).contiguous(), scales.to(self.act_dtype).to(self.device).contiguous(),
-                                zeros_x_scales.to(self.act_dtype).to(self.device).contiguous()).data
+                                zeros_x_scales.to(self.act_dtype).to(self.device).contiguous(), perm=perm).data
         if group not in (32, 64) and (group < 128 or group % 128):
             raise ValueError(f"INT4 group-wise weights: group size {group or f'K/{rows}'} unsupported (32, 64 or a multiple of "
                              f"128, per-channel included; K={K}, {rows} scale rows)")
         packed = ops.pack_w4(tensor.to(self.device).contiguous(), scales.to(self.act_dtype).to(self.device).contiguous(),
-                             zeros_x_scales.to(self.act_dtype).to(self.device).contiguous(), group)
+                             zeros_x_scales.to(self.act_dtype).to(self.device).contiguous(), group, perm=perm)
         return packed.data

@@ -73,6 +73,10 @@ class B200WeightOnlyLinear(LinearBase):
         if self.packed.fmt == B200_FMT_INT8 and self.packed.col_scale is None:
             self.packed.col_scale = weight_scales
         self._ws = _workspace(self.packed.data.device, self.MAX_BATCH, self.packed.K, self.packed.N)
+        # act-order weights: x[:, perm] is gathered here before the GEMM; 16-bit activations of either dtype (viewed at call
+        # time), sized once like the workspace so that captured graphs keep pointing at it
+        self._x_perm = (torch.empty(self.MAX_BATCH * self.packed.K * 2, dtype=torch.uint8, device=self.packed.data.device)
+                        if self.packed.perm is not None else None)
 
     def forward(self, input: torch.Tensor) -> torch.Tensor:
         lead = input.shape[:-1]
@@ -82,8 +86,9 @@ class B200WeightOnlyLinear(LinearBase):
         if self.packed.col_scale is not None and self.packed.col_scale.dtype != x.dtype:
             self.packed.col_scale = self.packed.col_scale.to(x.dtype).contiguous()   # the loader keeps INT8 scales in fp32 (device_impl.py:190)
         ws = self._ws
+        xp = None if self._x_perm is None else self._x_perm.view(x.dtype).view(self.MAX_BATCH, self.packed.K)
         outs = []
         for i in range(0, x.shape[0], self.MAX_BATCH):   # decode batches are <= 128; larger inputs go in slabs
-            outs.append(ops.wo_gemm(x[i:i + self.MAX_BATCH], self.packed, ws, bias=self.bias))
+            outs.append(ops.wo_gemm(x[i:i + self.MAX_BATCH], self.packed, ws, bias=self.bias, x_perm=xp))
         y = outs[0] if len(outs) == 1 else torch.cat(outs, 0)
         return y.reshape(*lead, self.packed.N)

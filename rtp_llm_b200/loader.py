@@ -7,6 +7,8 @@ per-column INT8 path, read from safetensors and pushed through the device hooks 
   * padding        the FFN inter size is padded to `align_size`: w2 along its INPUT rows (GPTQ qweight rows are packed 8:1 ->
                    align_size / 8; AWQ: align_size), zeros / scales by align_size / group_size rows; w1 / w3 along their
                    OUTPUT columns (group_wise_quant_weight.py:123-176, utils/model_weight.py:74-110 `pad`)
+  * act-order      GPTQ `desc_act` checkpoints carry `<prefix>.g_idx`: rows are sorted by it (device.act_order_perm) and the
+                   blob carries the order, except for w2, whose order is folded into w13's output columns (B200Loader.layer)
   * post-process   load_config.exported_device.preprocess_groupwise_weight_params(qweight, qzeros, scales, device, gptq, awq,
                    bits) (group_wise_quant_weight.py:392-425) -> here B200Impl (device.py); per-column INT8:
                    exported_device.apply_int8(kernel, device) (weight_only_quant_weight.py:94-105)
@@ -19,9 +21,9 @@ from typing import Dict, Optional
 import torch
 
 from . import ops
-from .device import B200Impl
+from .device import B200Impl, act_order_perm
 
-QW, QZ, QS = ".qweight", ".qzeros", ".scales"
+QW, QZ, QS, GI = ".qweight", ".qzeros", ".scales", ".g_idx"
 
 
 @dataclasses.dataclass
@@ -104,14 +106,51 @@ class B200Loader:
             qs = pad_dim(qs, rows, 0)
         return self.impl.unpack_groupwise(qw, qz, qs.to(torch.float16), q.gptq, q.awq, q.bits)
 
-    def _groupwise(self, prefixes, pad_in: int = 0, pad_out: int = 0, gate_up_inter: int = 0) -> ops.PackedWeight:
+    def act_order(self, prefixes) -> Optional[torch.Tensor]:
+        """The row order (act_order_perm) the merged weights `prefixes` share, or None (no act-order: AWQ, no `.g_idx`, or a
+        trivial one). Merged parts see the same input, so AutoGPTQ gives them the same g_idx; different ones cannot be served by
+        one sorted weight and raise ValueError."""
+        if not self.q.gptq:
+            return None
+        perms = []
+        for p in prefixes:
+            K = self.r.get(p + QW).shape[0] * 32 // self.q.bits      # GPTQ qweight: [K * bits / 32, N]
+            perms.append(act_order_perm(self.r.get(p + GI), self.q.group_size, K) if p + GI in self.r else None)
+        for p, perm in zip(prefixes[1:], perms[1:]):
+            same = (perm is None and perms[0] is None) or (perm is not None and perms[0] is not None and torch.equal(perm, perms[0]))
+            if not same:
+                raise ValueError(f"act-order: {prefixes[0]} and {p} are merged into one weight but have different g_idx")
+        return perms[0]
+
+    def sorted_tensors(self, prefixes, pad_in: int = 0, pad_out: int = 0, col_perm: Optional[torch.Tensor] = None):
+        """groupwise_tensors with act-order applied on the host: (q, zeros_x_scales, scales, perm). Rows sorted by g_idx (sorted
+        row j = checkpoint row perm[j]; perm None without act-order). col_perm: w2's order, applied to each half of a gate|up
+        weight's output columns (the fold, see layer())."""
         q_packed, zs, scales = self.groupwise_tensors(prefixes, pad_in, pad_out)
+        perm = self.act_order(prefixes)
+        if perm is not None:
+            # w2 padding: the padded rows are groups of their own and keep their place after the sorted rows
+            perm = torch.cat([perm, torch.arange(perm.numel(), q_packed.shape[0])])
+            q_packed = q_packed[perm]
+        if col_perm is not None:
+            half = scales.shape[1] // 2
+            cp = torch.cat([col_perm, torch.arange(col_perm.numel(), half)])             # the padded inter columns stay put
+            order = torch.cat([cp, cp + half])
+            q_packed = ops.permute_columns(q_packed, order, packed_int4=self.q.bits == 4)
+            zs, scales = ops.permute_columns(zs, order), ops.permute_columns(scales, order)
+        return q_packed, zs, scales, perm
+
+    def _groupwise(self, prefixes, pad_in: int = 0, pad_out: int = 0, gate_up_inter: int = 0,
+                   col_perm: Optional[torch.Tensor] = None, keep_perm: bool = True) -> ops.PackedWeight:
+        """keep_perm=False: the weight's own row order is folded into another weight (w2 into w13), so the blob omits it."""
+        q_packed, zs, scales, perm = self.sorted_tensors(prefixes, pad_in, pad_out, col_perm)
         q_packed, zs, scales = q_packed.to(self.device), zs.to(self.act_dtype).to(self.device), scales.to(self.act_dtype).to(self.device)
         if gate_up_inter:
             q_packed = ops.interleave_gate_up(q_packed, gate_up_inter, packed_int4=self.q.bits == 4)
             zs, scales = ops.interleave_gate_up(zs, gate_up_inter), ops.interleave_gate_up(scales, gate_up_inter)
         pack = ops.pack_w4 if self.q.bits == 4 else ops.pack_w8g     # 8-bit: q_s int8 [K, N], one byte per weight
-        return pack(q_packed.contiguous(), scales.contiguous(), zs.contiguous(), self.q.group_size)
+        return pack(q_packed.contiguous(), scales.contiguous(), zs.contiguous(), self.q.group_size,
+                    perm=perm if keep_perm else None)
 
     # ---- per-column INT8 (quantised at load time from FP16/BF16 weights) and plain FP16
     def _dense(self, prefixes, pad_in: int = 0, pad_out: int = 0, gate_up_inter: int = 0) -> ops.PackedWeight:
@@ -136,12 +175,22 @@ class B200Loader:
         return self._groupwise(prefixes, **kw) if self.q.method in ("gptq", "awq") else self._dense(prefixes, **kw)
 
     def layer(self, names: Dict[str, str], inter: Optional[int] = None) -> Dict[str, ops.PackedWeight]:
-        """qkv / o / w13 / w2 of one decoder layer. `inter` = the checkpoint's FFN inter size (needed for padding + fusion)."""
+        """qkv / o / w13 / w2 of one decoder layer. `inter` = the checkpoint's FFN inter size (needed for padding + fusion).
+
+        Act-order: qkv, o and w13 carry their row order (the GEMM gathers x). w2's order P2 is folded into w13 instead: column i
+        of w2's input is SiLU(gate_i) * up_i, so w13 with its gate and up columns permuted by P2 emits act[:, P2] directly and
+        the sorted w2 needs no gather."""
         out = {"qkv": self._load([names["q"], names["k"], names["v"]]), "o": self._load([names["o"]])}
         pad = self.align
         inter_p = inter if inter is None or not pad else (inter + pad - 1) // pad * pad
         fuse = self.fuse_silu and inter_p is not None and inter_p % 64 == 0
-        out["w13"] = self._load([names["gate"], names["up"]], pad_out=pad, gate_up_inter=inter_p if fuse else 0)
-        out["w2"] = self._load([names["down"]], pad_in=pad)
+        w13_kw = dict(pad_out=pad, gate_up_inter=inter_p if fuse else 0)
+        if self.q.method in ("gptq", "awq"):
+            p2 = self.act_order([names["down"]])
+            out["w13"] = self._groupwise([names["gate"], names["up"]], col_perm=p2, **w13_kw)
+            out["w2"] = self._groupwise([names["down"]], pad_in=pad, keep_perm=False)
+        else:
+            out["w13"] = self._dense([names["gate"], names["up"]], **w13_kw)
+            out["w2"] = self._dense([names["down"]], pad_in=pad)
         out["w13_fused_silu"] = fuse
         return out

@@ -131,7 +131,8 @@ def paged_decode_attn_rope(qkv: torch.Tensor, kv_cache_base: torch.Tensor, page_
 
 # ------------------------------------------------------------------------------------------------ weight-only GEMM
 _TRAILER_BYTES = 256
-_TRAILER_MAGIC = 0x42323030574F4731        # "B200WOG1"
+_TRAILER_MAGIC = 0x42323030574F4731        # "B200WOG1": [blob | trailer]
+_TRAILER_MAGIC_PERM = 0x42323030574F4732   # "B200WOG2": [blob | perm int32 [K] | trailer]
 
 
 class PackedWeight:
@@ -140,14 +141,19 @@ class PackedWeight:
     Quantised blobs are SELF-DESCRIBING: the uint8 tensor is [blob bytes | 256-byte trailer] with a magic number, the format and
     (K, N, group). The reference loader hands kernels around as plain tensors and copies them freely
     (device_impl.py:296-298 `.contiguous().to(device)`, state-dict round trips): a Python attribute on the tensor would be
-    lost there, the trailer travels with the bytes. PackedWeight.from_tensor() rebuilds the description from any copy."""
+    lost there, the trailer travels with the bytes. PackedWeight.from_tensor() rebuilds the description from any copy.
 
-    def __init__(self, fmt: int, K: int, N: int, data: torch.Tensor, col_scale: Optional[torch.Tensor] = None):
-        self.fmt, self.K, self.N, self.data, self.col_scale = fmt, K, N, data, col_scale
+    A GPTQ act-order weight (rows sorted by g_idx, see device.act_order_perm) also carries its row order: the tensor is then
+    [blob | perm int32 [K] | trailer] under its own magic, and `perm` is an int32 view into it. Sorted row j is the
+    checkpoint's row perm[j], so the GEMM must consume x[:, perm] (wo_gemm gathers it)."""
+
+    def __init__(self, fmt: int, K: int, N: int, data: torch.Tensor, col_scale: Optional[torch.Tensor] = None,
+                 perm: Optional[torch.Tensor] = None):
+        self.fmt, self.K, self.N, self.data, self.col_scale, self.perm = fmt, K, N, data, col_scale, perm
 
     @staticmethod
-    def _write_trailer(data: torch.Tensor, fmt: int, K: int, N: int, group: int) -> None:
-        t = torch.tensor([_TRAILER_MAGIC, fmt, K, N, group], dtype=torch.int64)
+    def _write_trailer(data: torch.Tensor, fmt: int, K: int, N: int, group: int, magic: int = _TRAILER_MAGIC) -> None:
+        t = torch.tensor([magic, fmt, K, N, group], dtype=torch.int64)
         data[-_TRAILER_BYTES:-_TRAILER_BYTES + 40] = t.view(torch.uint8).to(data.device)
 
     @staticmethod
@@ -155,13 +161,38 @@ class PackedWeight:
         if data.dtype != torch.uint8 or data.dim() != 1 or data.numel() <= _TRAILER_BYTES:
             raise B200Error("not a b200 weight blob (expected a 1-D uint8 tensor with a trailer)")
         t = data[-_TRAILER_BYTES:-_TRAILER_BYTES + 40].cpu().view(torch.int64).tolist()
-        if t[0] != _TRAILER_MAGIC:
+        if t[0] not in (_TRAILER_MAGIC, _TRAILER_MAGIC_PERM):
             raise B200Error("not a b200 weight blob (bad magic): quantised weights must be loaded through B200Impl")
         fmt, K, N = int(t[1]), int(t[2]), int(t[3])
         n = int(_lib.load().b200_wo_gemm_packed_bytes(fmt, K, N))
-        if n + _TRAILER_BYTES != data.numel():
-            raise B200Error(f"b200 weight blob has {data.numel()} bytes, expected {n + _TRAILER_BYTES} for K={K} N={N}")
-        return PackedWeight(fmt, K, N, data if data.is_contiguous() else data.contiguous(), col_scale)
+        perm_bytes = 4 * K if t[0] == _TRAILER_MAGIC_PERM else 0
+        if n + perm_bytes + _TRAILER_BYTES != data.numel():
+            raise B200Error(f"b200 weight blob has {data.numel()} bytes, expected {n + perm_bytes + _TRAILER_BYTES} for K={K} N={N}")
+        data = data if data.is_contiguous() else data.contiguous()
+        perm = data[n:n + perm_bytes].view(torch.int32) if perm_bytes else None
+        return PackedWeight(fmt, K, N, data, col_scale, perm)
+
+
+def _blob(n: int, K: int, perm: Optional[torch.Tensor], device) -> torch.Tensor:
+    """[n blob bytes (for the pack kernel to fill) | (perm) | zeroed trailer] tensor, so that equal weights give equal bytes;
+    with a perm, its int32 bytes are written in place after a host check that it is a permutation of 0..K-1 (the gather
+    kernel indexes shared memory with it unchecked)."""
+    extra = 0 if perm is None else 4 * K
+    blob = torch.empty(n + extra + _TRAILER_BYTES, dtype=torch.uint8, device=device)
+    blob[-_TRAILER_BYTES:].zero_()
+    if perm is None:
+        return blob
+    p = perm.detach().to("cpu", torch.int64).reshape(-1)
+    if p.numel() != K or not torch.equal(torch.sort(p).values, torch.arange(K)):
+        raise B200Error(f"perm must be a permutation of 0..{K - 1} (got {p.numel()} entries)")
+    blob[n:n + 4 * K] = p.to(torch.int32).view(torch.uint8).to(device)
+    return blob
+
+
+def _packed(fmt: int, K: int, N: int, blob: torch.Tensor, group: int, n: int, has_perm: bool,
+            col_scale: Optional[torch.Tensor] = None) -> PackedWeight:
+    PackedWeight._write_trailer(blob, fmt, K, N, group, _TRAILER_MAGIC_PERM if has_perm else _TRAILER_MAGIC)
+    return PackedWeight(fmt, K, N, blob, col_scale, blob[n:n + 4 * K].view(torch.int32) if has_perm else None)
 
 
 _W4_FORMATS = {128: B200_FMT_INT4, 64: B200_FMT_INT4_G64, 32: B200_FMT_INT4_G32}
@@ -185,20 +216,21 @@ def w4_format(K: int, group: int, scales: torch.Tensor, zeros_x_scales: torch.Te
     return _W4_FORMATS.get(group, B200_FMT_INT4), group, scales, zeros_x_scales
 
 
-def pack_w4(q_packed: torch.Tensor, scales: torch.Tensor, zeros_x_scales: torch.Tensor, group: int = 128) -> PackedWeight:
+def pack_w4(q_packed: torch.Tensor, scales: torch.Tensor, zeros_x_scales: torch.Tensor, group: int = 128,
+            perm: Optional[torch.Tensor] = None) -> PackedWeight:
     """q_packed uint8/int8 [K,N/2], scales / zeros_x_scales [K/g,N] in the activation dtype (CUDA). The group picks the blob
-    format (w4_format); the trailer records the group as given (per-channel: K)."""
+    format (w4_format); the trailer records the group as given (per-channel: K). perm: the row order of an act-order weight
+    whose rows were sorted by g_idx (PackedWeight), stored in the blob."""
     _cuda_contig(q_packed, scales, zeros_x_scales)
     K, N = q_packed.shape[0], q_packed.shape[1] * 2
     fmt, kernel_group, scales, zeros_x_scales = w4_format(K, group, scales, zeros_x_scales)
     n = _lib.load().b200_wo_gemm_packed_bytes(fmt, K, N)
     if n == 0:
         raise B200Error(f"pack_w4: unsupported shape K={K} N={N}")
-    blob = torch.empty(int(n) + _TRAILER_BYTES, dtype=torch.uint8, device=q_packed.device)
+    blob = _blob(int(n), K, perm, q_packed.device)
     check(_lib.load().b200_pack_w4(_p(q_packed), _p(scales), _p(zeros_x_scales), K, N, kernel_group, _p(blob), _stream()),
           "b200_pack_w4")
-    PackedWeight._write_trailer(blob, fmt, K, N, K if group == -1 else group)
-    return PackedWeight(fmt, K, N, blob)
+    return _packed(fmt, K, N, blob, K if group == -1 else group, int(n), perm is not None)
 
 
 def pack_w8(q: torch.Tensor, col_scale: torch.Tensor) -> PackedWeight:
@@ -207,23 +239,24 @@ def pack_w8(q: torch.Tensor, col_scale: torch.Tensor) -> PackedWeight:
     n = _lib.load().b200_wo_gemm_packed_bytes(B200_FMT_INT8, K, N)
     if n == 0:
         raise B200Error(f"pack_w8: unsupported shape K={K} N={N}")
-    blob = torch.empty(int(n) + _TRAILER_BYTES, dtype=torch.uint8, device=q.device)
+    blob = _blob(int(n), K, None, q.device)
     check(_lib.load().b200_pack_w8(_p(q), K, N, _p(blob), _stream()), "b200_pack_w8")
     PackedWeight._write_trailer(blob, B200_FMT_INT8, K, N, 0)
     return PackedWeight(B200_FMT_INT8, K, N, blob, col_scale)
 
 
-def pack_w8g(q: torch.Tensor, scales: torch.Tensor, zeros_x_scales: torch.Tensor, group: int = 128) -> PackedWeight:
-    """8-bit group-wise (GPTQ/AWQ W8): q int8 [K,N] (q_s = q_u - 128), scales / zeros_x_scales [K/g,N] in the activation dtype."""
+def pack_w8g(q: torch.Tensor, scales: torch.Tensor, zeros_x_scales: torch.Tensor, group: int = 128,
+             perm: Optional[torch.Tensor] = None) -> PackedWeight:
+    """8-bit group-wise (GPTQ/AWQ W8): q int8 [K,N] (q_s = q_u - 128), scales / zeros_x_scales [K/g,N] in the activation dtype.
+    perm: as for pack_w4."""
     _cuda_contig(q, scales, zeros_x_scales)
     K, N = q.shape
     n = _lib.load().b200_wo_gemm_packed_bytes(B200_FMT_INT8G, K, N)
     if n == 0:
         raise B200Error(f"pack_w8g: unsupported shape K={K} N={N}")
-    blob = torch.empty(int(n) + _TRAILER_BYTES, dtype=torch.uint8, device=q.device)
+    blob = _blob(int(n), K, perm, q.device)
     check(_lib.load().b200_pack_w8g(_p(q), _p(scales), _p(zeros_x_scales), K, N, group, _p(blob), _stream()), "b200_pack_w8g")
-    PackedWeight._write_trailer(blob, B200_FMT_INT8G, K, N, group)
-    return PackedWeight(B200_FMT_INT8G, K, N, blob)
+    return _packed(B200_FMT_INT8G, K, N, blob, group, int(n), perm is not None)
 
 
 def pack_f16(w_kn: torch.Tensor) -> PackedWeight:
@@ -247,23 +280,51 @@ def gate_up_order(inter: int, device=None) -> torch.Tensor:
     return torch.stack([j, j + inter], dim=1).reshape(-1)
 
 
-def interleave_gate_up(w: torch.Tensor, inter: int, packed_int4: bool = False) -> torch.Tensor:
-    """Apply gate_up_order to the column axis of a reference-layout tensor ([K, 2I], or uint8 [K, I] packed int4 -- low
-    nibble = even column --, or scales [G, 2I] / [2I])."""
-    order = gate_up_order(inter, w.device)
+def permute_columns(w: torch.Tensor, order: torch.Tensor, packed_int4: bool = False) -> torch.Tensor:
+    """Column j of the result = column order[j] of w ([K, N], or uint8 [K, N/2] packed int4 -- low nibble = even column --, or
+    scales [G, N] / [N])."""
+    order = order.to(w.device)
     if packed_int4:
-        full = torch.stack([w & 0xF, w >> 4], dim=-1).reshape(w.shape[0], -1)       # one nibble per column [K, 2I]
+        full = torch.stack([w & 0xF, w >> 4], dim=-1).reshape(w.shape[0], -1)       # one nibble per column [K, N]
         full = full.index_select(-1, order)
         return (full[:, 0::2] | (full[:, 1::2] << 4)).contiguous()
     return w.index_select(-1, order).contiguous()
 
 
+def interleave_gate_up(w: torch.Tensor, inter: int, packed_int4: bool = False) -> torch.Tensor:
+    """Apply gate_up_order to the column axis of a reference-layout tensor (see permute_columns for the layouts)."""
+    return permute_columns(w, gate_up_order(inter, w.device), packed_int4)
+
+
+def permute_cols(x: torch.Tensor, perm: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out[r][j] = x[r][perm[j]] (x [rows, K] fp16 / bf16, perm int32 [K] on the device): a bit copy."""
+    _cuda_contig(x, perm, out)
+    rows, K = x.shape
+    if perm.dtype != torch.int32 or perm.numel() != K:
+        raise B200Error(f"permute_cols: perm must be int32 [{K}]")
+    if out is None:
+        out = torch.empty_like(x)
+    if out.shape != x.shape or out.dtype != x.dtype:
+        raise B200Error(f"permute_cols: out {tuple(out.shape)} {out.dtype} does not match x {tuple(x.shape)} {x.dtype}")
+    check(_lib.load().b200_permute_cols(_p(x), _p(perm), _p(out), _is_bf16(x), rows, K, _stream()), "b200_permute_cols")
+    return out
+
+
 def wo_gemm(x: torch.Tensor, w: PackedWeight, workspace: torch.Tensor, bias: Optional[torch.Tensor] = None,
-            out: Optional[torch.Tensor] = None, pdl: bool = False, silu_mul: bool = False) -> torch.Tensor:
+            out: Optional[torch.Tensor] = None, pdl: bool = False, silu_mul: bool = False,
+            x_perm: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """y = x . W (+ bias). An act-order weight (w.perm set) needs x_perm, a scratch [>= B, K] of x's dtype: x[:, w.perm] is
+    gathered into it (b200_permute_cols) and the GEMM reads that."""
     _cuda_contig(x, w.data, workspace, bias, out)
     B, K = x.shape
     if K != w.K:
         raise B200Error(f"wo_gemm: x has K={K}, weight has K={w.K}")
+    if w.perm is not None:
+        if x_perm is None:
+            raise B200Error("wo_gemm: the weight is act-order (rows sorted by g_idx): pass x_perm, a [>= B, K] scratch for x[:, perm]")
+        if x_perm.dim() != 2 or x_perm.shape[0] < B or x_perm.shape[1] != K or x_perm.dtype != x.dtype:
+            raise B200Error(f"wo_gemm: x_perm must be [>= {B}, {K}] {x.dtype}, got {tuple(x_perm.shape)} {x_perm.dtype}")
+        x = permute_cols(x, w.perm, out=x_perm[:B])
     if out is None:
         out = torch.empty((B, w.N // 2 if silu_mul else w.N), dtype=x.dtype, device=x.device)
     check(_lib.load().b200_wo_gemm(w.fmt, _is_bf16(x), _p(x), B, K, w.N, _p(w.data), _p(w.col_scale), _p(bias), _p(out),

@@ -70,8 +70,20 @@ def bench_attn(B, Hq, Hkv, S, T=64, nrot=3, env=None):
     return us
 
 
-def bench_gemm(fmt, B, K, N, env=None, pdl=False, group=128):
-    """group: quantisation group of INT4 weights (128, 64, 32); bytes count the scale and zero*scale of every group."""
+def bench_permute(B, K, nrot=4):
+    """b200_permute_cols on [B, K] fp16; bytes = the row read and written, plus the perm."""
+    xs = [torch.randn(B, K, device=dev).half() for _ in range(nrot)]
+    perm = torch.randperm(K, device=dev).to(torch.int32)
+    y = torch.empty(B, K, device=dev).half()
+    us = timeit(lambda i: ops.permute_cols(xs[i], perm, out=y), nrot)
+    byt = 2 * 2 * B * K + 4 * K
+    print(f"permute_cols B{B} K{K}: {us:8.2f} us  {byt / us / 1e3:7.0f} GB/s", flush=True)
+    return us
+
+
+def bench_gemm(fmt, B, K, N, env=None, pdl=False, group=128, act_order=False):
+    """group: quantisation group of INT4 weights (128, 64, 32); bytes count the scale and zero*scale of every group.
+    act_order: the weight carries a row order (GPTQ act-order), so each call is the x gather plus the GEMM."""
     for k, v in (env or {}).items():
         os.environ[k] = str(v)
     nm = {B200_FMT_F16: "f16", B200_FMT_INT8: "int8", B200_FMT_INT4: f"int4 g{group}"}[fmt]
@@ -82,7 +94,7 @@ def bench_gemm(fmt, B, K, N, env=None, pdl=False, group=128):
         if fmt == B200_FMT_INT4:
             qp = torch.randint(0, 256, (K, N // 2), device=dev, dtype=torch.uint8)
             s = (torch.randn(K // group, N, device=dev).abs() * 0.01 + 1e-3).half()
-            w = ops.pack_w4(qp, s, s, group)
+            w = ops.pack_w4(qp, s, s, group, perm=torch.randperm(K) if act_order else None)
         elif fmt == B200_FMT_INT8:
             w = ops.pack_w8(torch.randint(-128, 128, (K, N), device=dev, dtype=torch.int8), torch.ones(N, device=dev).half())
         else:
@@ -91,11 +103,12 @@ def bench_gemm(fmt, B, K, N, env=None, pdl=False, group=128):
     x = torch.randn(B, K, device=dev).half()
     y = torch.empty(B, N, device=dev).half()
     wk = ops.gemm_workspace(B, [(K, N)], dev)
-    us = timeit(lambda i: ops.wo_gemm(x, ws_[i], wk, out=y, pdl=pdl), nrot)
+    xp = torch.empty(B, K, device=dev).half() if act_order else None
+    us = timeit(lambda i: ops.wo_gemm(x, ws_[i], wk, out=y, pdl=pdl, x_perm=xp), nrot)
     byt = wbytes + 2 * B * (K + N)
     for k in (env or {}):
         os.environ.pop(k, None)
-    print(f"gemm {nm} B{B} K{K} N{N} {env or ''}{' pdl' if pdl else ''}: {us:8.1f} us  {byt / us / 1e3:7.0f} GB/s  frac={byt / us / 1e3 / PEAK:.3f}",
+    print(f"gemm {nm} B{B} K{K} N{N} {env or ''}{' pdl' if pdl else ''}{' act-order (gather + GEMM)' if act_order else ''}: {us:8.1f} us  {byt / us / 1e3:7.0f} GB/s  frac={byt / us / 1e3 / PEAK:.3f}",
           flush=True)
     return us
 
@@ -127,6 +140,13 @@ if __name__ == "__main__":
         for K, N in ((4096, 4096), (14336, 4096)):
             for s in (1, 2, 4, 8):
                 bench_gemm(B200_FMT_INT4, 32, K, N, env={"B200_GEMM_SPLITK": s})
+    if "permute" in which:
+        # GPTQ act-order: the x gather alone, then the Llama-3-8B INT4 GEMMs it precedes (qkv, o, w13) with and without it
+        for K in (4096, 8192, 14336):
+            bench_permute(32, K)
+        for K, N in ((4096, 6144), (4096, 4096), (4096, 28672)):
+            bench_gemm(B200_FMT_INT4, 32, K, N)
+            bench_gemm(B200_FMT_INT4, 32, K, N, act_order=True)
     if "attn" in which:
         bench_attn(32, 32, 8, 2048)
         for c in (2, 4, 8, 16, 32):
