@@ -215,8 +215,10 @@ int b200_argmax(const void* logits, int dtype, int rows, int vocab, int32_t* out
  * tokens of `history` (hist_len[r] valid ids of [rows][hist_stride]), softmax (the probabilities REPLACE the logits, as in the
  * reference), top-k (keep p >= the k-th largest; top_k <= 0 = no limit; top_k == 1 = argmax, lowest index on ties), top-p
  * within what is left (smallest set of largest p reaching top_p; |top_p| < 1e-7 or >= 1 = no limit), renormalise, and one
- * inverse-CDF draw in index order with the caller's uniform[r] in [0, 1).  Same distribution as the reference's flashinfer
- * rejection sampler, different random stream: the caller owns the randomness, so the op is deterministic and graph-replayable.
+ * inverse-CDF draw in index order with the caller's uniform[r] in [0, 1), which always returns a kept token with p > 0
+ * (token -1 and token_prob 0 only for a row without positive finite mass, i.e. NaN logits).  Same distribution as the
+ * reference's flashinfer rejection sampler, different random stream: the caller owns the randomness, so the op is
+ * deterministic and graph-replayable.
  * process[r] == 0 (do_sample false) skips temperature / penalties for that row. count_ws: [rows][vocab] int32, zero on entry
  * and on exit (only read with penalties). Optional outputs: token_prob_out[r] (renormalised probability of the drawn token,
  * for cum_log_probs += log p), probs_out [rows][vocab] (output_all_probs after renormalisation). logits fp32, contiguous. */

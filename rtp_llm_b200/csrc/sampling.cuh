@@ -15,6 +15,11 @@
 // (its own accuracy test compares distributions, CudaSamplerTest.cc:143-147), the random stream is not: here the caller
 // owns the randomness (one float per row), which makes the op deterministic and replayable in a CUDA graph.
 // One CTA per row; thresholds are found by bisection on the float bit pattern (no sort, no vocabulary-sized scratch).
+// The draw: each thread sums a contiguous chunk of ceil(V/1024) kept probabilities, a block scan of the chunk sums gives each
+// chunk's start, and the target u * total (clamped below total) goes to the last thread with mass whose start is <= target:
+// exactly one owner, so every draw returns a kept token with p > 0. It walks its chunk and, when rounding leaves the target
+// beyond the chunk's own sum, takes the chunk's last kept token with p > 0. Token -1 (token_prob 0) only when the row has no
+// positive finite mass, i.e. NaN logits. Under PDL the kernel waits for its predecessor before it reads anything.
 #pragma once
 #include "ptx.cuh"
 
@@ -67,8 +72,9 @@ __device__ __forceinline__ float block_reduce_max(float v, float* s_red) {
 __global__ void __launch_bounds__(kSampleThreads) sample_kernel(const SampleParams p) {
     __shared__ float s_red[kSampleThreads / 32];
     __shared__ float s_scan[kSampleThreads];
-    __shared__ int s_pick;
+    __shared__ int s_pick, s_owner;
     const int row = blockIdx.x, tid = threadIdx.x, V = p.vocab;
+    pdl_wait();                        // under PDL the logits and the per-row inputs come from the kernels before this one
     float* lg = p.logits + (size_t)row * V;
     const bool process = !p.process || p.process[row];
 
@@ -172,6 +178,7 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(const SamplePara
     float mine = 0.f;
     for (int i = i0; i < i1; ++i) mine += lg[i] >= thr ? lg[i] : 0.f;
     s_scan[tid] = mine;
+    if (tid == 0) s_owner = s_pick = -1;
     __syncthreads();
     for (int off = 1; off < kSampleThreads; off <<= 1) {   // Hillis-Steele inclusive scan
         const float add = tid >= off ? s_scan[tid - off] : 0.f;
@@ -180,18 +187,22 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(const SamplePara
         __syncthreads();
     }
     const float total = s_scan[kSampleThreads - 1];
-    const float target = k == 1 ? 0.f : p.uniform[row] * total;   // top_k == 1: the lowest index among the maxima (argmax semantics)
-    if (tid == 0) s_pick = 0;
+    // top_k == 1: the lowest index among the maxima (argmax semantics). u * total can round up to total: clamp below it.
+    const float target = k == 1 ? 0.f : fminf(p.uniform[row] * total, __uint_as_float(__float_as_uint(total) - 1u));
+    const float start = tid ? s_scan[tid - 1] : 0.f;
+    // Every prefix sum is rounded in its own tree order, so the chunk intervals [start, s_scan[tid]) can overlap or leave gaps.
+    // The owner is the LAST thread with positive mass whose start is <= target: exactly one thread. It exists whenever the
+    // kept mass is positive, because the first thread with mass starts at an exact 0 (only zeros precede it) and target >= 0.
+    const int warp_owner = __reduce_max_sync(0xffffffffu, mine > 0.f && start <= target ? tid : -1);
+    if ((tid & 31) == 0 && warp_owner >= 0) atomicMax(&s_owner, warp_owner);
     __syncthreads();
-    // exactly one thread owns the target: the first whose inclusive chunk sum exceeds it
-    const float before = s_scan[tid] - mine;
-    if (mine > 0.f && before <= target && target < s_scan[tid]) {
-        float c = before;
+    if (tid == s_owner) {
+        float c = start;
         int pick = -1;
         for (int i = i0; i < i1; ++i) {
-            if (lg[i] >= thr) {
+            if (lg[i] >= thr && lg[i] > 0.f) {
                 c += lg[i];
-                pick = i;                  // the chunk's last kept token is the fallback when rounding undershoots
+                pick = i;                  // the chunk's last kept token with p > 0 is the fallback when rounding undershoots
                 if (c > target) break;
             }
         }
