@@ -92,7 +92,7 @@ size_t b200_paged_decode_attn_workspace_bytes(size_t batch, size_t head_num, siz
  *                reference); attention covers positions 0..sequence_lengths[b] inclusive
  *   max_seq_len  host upper bound of sequence_lengths[b]+1 (sizes the sequence split; as XQAAttnOp.cc:149)
  *   softmax scale = q_scale * head_dim^-1/2.
- * Supported: head_dim 64 / 128 / 256, head_num/kv_head_num in 1..16, page_size in {16,32,64,128}. */
+ * Supported: head_dim 64 / 128 / 256, head_num/kv_head_num in 1..64, page_size in {16,32,64,128}. */
 int b200_paged_decode_attn(const void* q, int is_bf16, void* out, size_t head_num, size_t kv_head_num, size_t head_dim,
                            size_t batch, size_t max_blocks_per_seq, size_t max_seq_len, size_t page_size,
                            const void* kv_pool, const int32_t* page_list, const uint32_t* sequence_lengths,
@@ -101,7 +101,7 @@ int b200_paged_decode_attn(const void* q, int is_bf16, void* out, size_t head_nu
 /* q_len > 1 query tokens per sequence (verification of speculative tokens: runXqa's max_q_len, CudaXqa.h:59-84; trtllm-gen's
  * q_len_per_req, trtllm_gen.py:544): q [batch][q_len][head_num][head_dim], out [batch][q_len][head_num*head_dim]; the K/V of all
  * q_len new tokens are already in the cache; sequence_lengths[b] = tokens cached BEFORE them, query j attends to positions
- * 0 .. sequence_lengths[b] + j. (head_num / kv_head_num) * q_len <= 16; max_seq_len bounds sequence_lengths[b] + q_len; size the
+ * 0 .. sequence_lengths[b] + j. (head_num / kv_head_num) * q_len <= 64; max_seq_len bounds sequence_lengths[b] + q_len; size the
  * workspace with b200_paged_decode_attn_workspace_bytes(batch * q_len, ...). q_len == 1 is b200_paged_decode_attn. */
 int b200_paged_decode_attn_multi(const void* q, int is_bf16, void* out, size_t head_num, size_t kv_head_num, size_t head_dim,
                                  size_t batch, size_t q_len, size_t max_blocks_per_seq, size_t max_seq_len, size_t page_size,
@@ -113,7 +113,7 @@ int b200_paged_decode_attn_multi(const void* q, int is_bf16, void* out, size_t h
  * bindings/cuda/XQAAttnOp.cc:119-156) by one launch. `qkv` is the qkv GEMM output [batch][(head_num + 2 kv_head_num) * head_dim],
  * un-rotated; q is rotated on load, the CTA that owns the tile of position sequence_lengths[b] rotates k and appends k, v to
  * `kv_pool` before streaming it. RopeStyle::Base, NeoX pairing, same arithmetic as b200_rope_append: cache contents and attention
- * output are bit-identical to the two-call sequence. */
+ * output are bit-identical to the two-call sequence. head_num / kv_head_num <= 16 (one token per sequence). */
 int b200_paged_decode_attn_rope(const void* qkv, int is_bf16, void* out, size_t head_num, size_t kv_head_num, size_t head_dim,
                                 size_t batch, size_t max_blocks_per_seq, size_t max_seq_len, size_t page_size, void* kv_pool,
                                 const int32_t* page_list, const uint32_t* sequence_lengths, float q_scale, float rope_base,
@@ -179,6 +179,13 @@ int b200_permute_cols(const void* x, const int32_t* perm, void* y, int is_bf16, 
 int b200_rope_append(const void* qkv, void* q_out, void* kv_pool, const int32_t* page_list,
                      const int32_t* sequence_lengths, int is_bf16, int batch, int head_num, int kv_head_num,
                      int head_dim, int max_blocks_per_seq, int page_size, float rope_base, void* stream);
+/* b200_rope_append for q_len new tokens per sequence (verification of speculative tokens): row x of qkv [batch*q_len][...]
+ * is token j = x % q_len of sequence b = x / q_len, rotated and appended at position (and cache slot) sequence_lengths[b] + j;
+ * q_out [batch*q_len][Hq*D] is the q [batch][q_len][Hq][D] of b200_paged_decode_attn_multi. q_len == 1 is b200_rope_append.
+ * Inside a decode program it is its own launch. */
+int b200_rope_append_multi(const void* qkv, void* q_out, void* kv_pool, const int32_t* page_list,
+                           const int32_t* sequence_lengths, int is_bf16, int batch, int head_num, int kv_head_num,
+                           int head_dim, int max_blocks_per_seq, int page_size, float rope_base, int q_len, void* stream);
 /* The full decode contract of FusedRopeKVCacheDecodeOp.forward (rtp_llm/ops/fused_rope_kvcache_op.py:202-246; device code
  * rtp_llm/models_py/bindings/common/kernels/rotary_position_embedding.h:322-442,889-1062). b200_rope_config mirrors the
  * fields of RopeConfig (rtp_llm/cpp/model_utils/RopeConfig.h:21-42) the decode path reads.
@@ -226,6 +233,22 @@ int b200_sample(float* logits, int rows, int vocab, const int32_t* history, cons
                 int32_t* count_ws, const float* temperature, const float* repetition, const float* presence,
                 const float* frequency, const int32_t* top_k, const float* top_p, const float* uniform, const uint8_t* process,
                 int32_t* token_out, float* token_prob_out, float* probs_out, void* stream);
+
+/* Verification of num_draft = n speculative tokens per sequence (the chain form of the reference's speculative-sampling kernel,
+ * rtp_llm/models_py/bindings/cuda/kernels/speculative_sampling/sampling.cu), after a step over the batch*(n+1) rows
+ * [last accepted token, draft 0 .. draft n-1] of each sequence.
+ *   draft_tokens [batch][n]; out_tokens [batch][n+1]: the accepted drafts, one correction or bonus token, then -1;
+ *   accepted [batch] in 0..n (the sequence advances by accepted + 1).
+ * Greedy (target_probs == NULL): target_ids [batch][n+1] (b200_argmax of the rows); accepted = the first i with
+ *   draft[i] != target_ids[i] (n if none), the emitted token is target_ids[accepted].
+ * Sampling: target_probs [batch][n+1][vocab] fp32 (probs_out of b200_sample over the rows), draft_probs [batch][n][vocab] or
+ *   NULL (deterministic drafts, one-hot), uniform [batch][n+1] in [0, 1). Draft i = d is accepted iff uniform[i] * p(d) < q(d)
+ *   in fp32 (p = draft_probs[i][d], or 1); at the first rejection the token is drawn from max(0, q - p) (from q when that has
+ *   no mass), after n acceptances from target row n, both with uniform[n] by inverse CDF in index order as b200_sample draws
+ *   (always a token with positive mass; -1 only for a row without any). Same distribution as the reference, caller-owned
+ *   randomness. One CTA per sequence. */
+int b200_spec_verify(const float* target_probs, const int32_t* target_ids, const float* draft_probs, const int32_t* draft_tokens,
+                     const float* uniform, int batch, int num_draft, int vocab, int32_t* out_tokens, int32_t* accepted, void* stream);
 
 /* ------------------------------------------------------------------------------------------------ TP all-reduce over NVLink peer memory */
 

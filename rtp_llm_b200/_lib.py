@@ -43,10 +43,12 @@ SIGNATURES = {
     "b200_silu_and_mul": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "b200_permute_cols": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "b200_rope_append": (c_int, [c_void_p] * 5 + [c_int] * 7 + [c_float, c_void_p]),
+    "b200_rope_append_multi": (c_int, [c_void_p] * 5 + [c_int] * 7 + [c_float, c_int, c_void_p]),
     "b200_rope_append_ex": (c_int, [c_void_p] * 8 + [c_int, c_void_p] + [c_int] * 8 + [c_void_p]),
     "b200_embedding": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "b200_argmax": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "b200_sample": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int] + [c_void_p] * 13),
+    "b200_spec_verify": (c_int, [c_void_p] * 5 + [c_int] * 3 + [c_void_p] * 3),
     "b200_peer_ar_region_bytes": (c_size_t, [c_size_t]),
     "b200_peer_alloc": (c_int, [c_size_t, c_void_p, c_void_p]),
     "b200_peer_open": (c_int, [c_void_p, c_void_p]),

@@ -10,7 +10,8 @@
 Inside the reference tree the impl is appended to DECODE_MHA_IMPS (attention/__init__.py:91-100); see INTEGRATION.md.
 Config / input objects are duck-typed: any object with the reference's attribute names works (AttentionConfigs:
 head_num, kv_head_num, size_per_head, kernel_tokens_per_block|tokens_per_block, max_seq_len, need_rope_kv_cache,
-rope_config.base, q_scaling; PyAttentionInputs: sequence_lengths, kv_cache_kernel_block_id_device, is_prefill).
+rope_config.base, q_scaling; PyAttentionInputs: sequence_lengths, kv_cache_kernel_block_id_device, is_prefill, and
+input_lengths for a verification step of speculative tokens, which runs q_len = max(input_lengths) tokens per sequence).
 """
 from __future__ import annotations
 
@@ -48,6 +49,19 @@ class B200AttnParams:
     batch_size: int
     max_seq_len: int
     workspace: torch.Tensor
+    q_len: int = 1                         # query tokens per sequence (> 1: verification of speculative tokens)
+
+
+_MAX_ROWS = 64       # query rows (group x q_len) per (sequence, kv head) of b200_paged_decode_attn(_multi)
+
+
+def _q_len(attn_inputs) -> int:
+    """Tokens per sequence of a decode step: max(input_lengths) when the inputs carry them (speculative verification,
+    uniform across the batch), else 1."""
+    lens = getattr(attn_inputs, "input_lengths", None)
+    if lens is None or (torch.is_tensor(lens) and lens.numel() == 0):
+        return 1
+    return max(int(lens.max().item()) if torch.is_tensor(lens) else int(max(lens)), 1)
 
 
 class B200DecodeAttnOp:
@@ -59,8 +73,8 @@ class B200DecodeAttnOp:
         if getattr(attn_inputs, "is_prefill", False):
             return False
         group = c.head_num // max(c.kv_head_num, 1)
-        ok = (c.size_per_head in (64, 128, 256) and c.head_num % max(c.kv_head_num, 1) == 0 and 1 <= group <= 16
-              and _tokens_per_block(c) in (16, 32, 64, 128))
+        ok = (c.size_per_head in (64, 128, 256) and c.head_num % max(c.kv_head_num, 1) == 0
+              and 1 <= group * _q_len(attn_inputs) <= _MAX_ROWS and _tokens_per_block(c) in (16, 32, 64, 128))
         kv_dtype = str(getattr(c, "kv_cache_dtype", "BASE"))
         return ok and "FP8" not in kv_dtype.upper() and torch.cuda.is_available() and \
             torch.cuda.get_device_capability() == (9, 0)
@@ -76,9 +90,10 @@ class B200DecodeAttnOp:
         max_seq_len = int(getattr(self.cfg, "max_seq_len", 0)) or int(block_ids.shape[1]) * _tokens_per_block(self.cfg)
         # sequence_lengths may equal max_seq_len (tokens already cached): the kernel covers positions 0..sequence_lengths
         # inclusive, so the bound is max_seq_len + 1 exactly as XQAAttnOp.cc:147-149 passes it, capped by the page table
-        max_seq_len = min(max_seq_len + 1, int(block_ids.shape[1]) * _tokens_per_block(self.cfg))
-        ws = ops.attn_workspace(B, self.cfg.head_num, self.cfg.kv_head_num, max_seq_len, block_ids.device)
-        return B200AttnParams(page_list, attn_inputs.sequence_lengths, B, max_seq_len, ws)
+        q_len = _q_len(attn_inputs)
+        max_seq_len = min(max_seq_len + q_len, int(block_ids.shape[1]) * _tokens_per_block(self.cfg))
+        ws = ops.attn_workspace(B * q_len, self.cfg.head_num, self.cfg.kv_head_num, max_seq_len, block_ids.device)
+        return B200AttnParams(page_list, attn_inputs.sequence_lengths, B, max_seq_len, ws, q_len)
 
     def update(self, params: B200AttnParams, attn_inputs) -> None:
         if params is None:
@@ -103,6 +118,12 @@ class B200DecodeAttnOp:
         if not seq.is_cuda and not seq.is_pinned():
             raise B200Error("sequence_lengths must be device-accessible (CUDA or pinned host memory)")
         q_scale = 1.0 / float(getattr(self.cfg, "q_scaling", 1.0) or 1.0)
+        if params.q_len > 1:      # q [B*q_len, Hq*D] token-major -> [B, q_len, Hq, D]; out [B*q_len, Hq*D]
+            D = base.shape[-1]
+            q4 = q.reshape(params.batch_size, params.q_len, -1, D)
+            out = ops.paged_decode_attn_multi(q4, base, params.kv_cache_offset, seq, params.max_seq_len, params.workspace,
+                                              q_scale=q_scale)
+            return out.reshape(params.batch_size * params.q_len, -1)
         return ops.paged_decode_attn(q, base, params.kv_cache_offset, seq, params.max_seq_len, params.workspace,
                                      q_scale=q_scale)
 
@@ -116,11 +137,11 @@ class B200RopeKVCacheDecodeOp:
     def prepare(self, attn_inputs):
         return attn_inputs
 
-    def forward(self, qkv: torch.Tensor, kv_cache, page_list: torch.Tensor, sequence_lengths: torch.Tensor):
+    def forward(self, qkv: torch.Tensor, kv_cache, page_list: torch.Tensor, sequence_lengths: torch.Tensor, q_len: int = 1):
         base = kv_cache.kv_cache_base if hasattr(kv_cache, "kv_cache_base") else kv_cache
         rope = getattr(self.cfg, "rope_config", None)
         rope_base = float(getattr(rope, "base", 10000.0)) if rope is not None else 10000.0
-        return ops.rope_append(qkv, base, page_list, sequence_lengths, self.cfg.head_num, rope_base)
+        return ops.rope_append(qkv, base, page_list, sequence_lengths, self.cfg.head_num, rope_base, q_len=q_len)
 
 
 class B200DecodeImpl(FMHAImplBase):
@@ -140,9 +161,13 @@ class B200DecodeImpl(FMHAImplBase):
         return B200DecodeAttnOp(attn_configs).support(attn_inputs)
 
     def forward(self, qkv: torch.Tensor, kv_cache, layer_idx: int = 0) -> torch.Tensor:
+        """qkv [B*q_len, (Hq+2Hkv)*D], token-major (row b*q_len + j = token j of sequence b); q_len = 1 is plain decode."""
+        q_len = self.fmha_params.q_len
+        if q_len > 1 and qkv.shape[0] != self.fmha_params.batch_size * q_len:
+            raise B200Error(f"qkv has {qkv.shape[0]} rows, expected batch {self.fmha_params.batch_size} x q_len {q_len}")
         if self.need_rope_kv_cache:
             q = self.rope_kvcache_impl.forward(qkv, kv_cache, self.fmha_params.kv_cache_offset,
-                                               self.fmha_params.sequence_lengths)
+                                               self.fmha_params.sequence_lengths, q_len)
         else:
             q = qkv
         return self.fmha_impl.forward(q, kv_cache, self.fmha_params)

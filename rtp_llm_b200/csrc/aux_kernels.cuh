@@ -219,22 +219,25 @@ __global__ void silu_and_mul_kernel(const T* __restrict__ gate_up, T* __restrict
 
 // Decode RoPE (NeoX pairing, RopeStyle::Base, angle = pos * base^(-2i/dim)) + K,V append into the paged cache.
 // Contract: SURVEY.md appendix C; call site /root/reference/rtp_llm/ops/fused_rope_kvcache_op.py:202-246.
-// grid (B, Hq + 2*Hkv), D/2 threads.
-template <typename T>
+// q_len new tokens per sequence (speculative-token verification): row x of qkv [B*q_len] is token j = x % q_len of sequence
+// b = x / q_len, rotated and appended at position seq_lens[b] + j; q_out [B*q_len][Hq*D].
+// grid (B*q_len, Hq + 2*Hkv), D/2 threads. MULTI = false is the one-token instance (q_len == 1, no division by q_len).
+template <typename T, bool MULTI = false>
 __global__ void rope_append_kernel(const T* __restrict__ qkv, T* __restrict__ q_out, T* __restrict__ kv_pool,
                                    const int32_t* __restrict__ page_list, const int32_t* __restrict__ seq_lens,
                                    int head_num, int kv_head_num, int head_dim, int max_blocks, int tokens_per_block,
-                                   float log2_base) {
+                                   float log2_base, int q_len) {
     pdl_launch_dependents();
     pdl_wait();
-    const int b = blockIdx.x, h = blockIdx.y, i = threadIdx.x, half = head_dim / 2;
-    const int pos = seq_lens[b];
-    const T* src = qkv + ((size_t)b * (head_num + 2 * kv_head_num) + h) * head_dim;
+    const int x = blockIdx.x, h = blockIdx.y, i = threadIdx.x, half = head_dim / 2;
+    const int b = MULTI ? x / q_len : x;
+    const int pos = seq_lens[b] + (MULTI ? x % q_len : 0);
+    const T* src = qkv + ((size_t)x * (head_num + 2 * kv_head_num) + h) * head_dim;
     const size_t page_elems = (size_t)kv_head_num * tokens_per_block * head_dim;
     T* dst;
     bool rotate = true;
     if (h < head_num) {
-        dst = q_out + ((size_t)b * head_num + h) * head_dim;
+        dst = q_out + ((size_t)x * head_num + h) * head_dim;
     } else {
         const bool is_v = h >= head_num + kv_head_num;
         const int kvh = is_v ? h - head_num - kv_head_num : h - head_num;

@@ -429,8 +429,11 @@ static int attn_impl(const void* q, const void* qkv, float rope_base, int q_len,
     ARG_CHECK(kv_head_num > 0 && head_num % kv_head_num == 0, "paged_decode_attn: head_num %zu not a multiple of kv_head_num %zu",
               head_num, kv_head_num);
     const int group = (int)(head_num / kv_head_num);
-    ARG_CHECK(group >= 1 && group <= 16, "paged_decode_attn: group size %d unsupported (1..16)", group);
-    ARG_CHECK(group * q_len <= 16, "paged_decode_attn: group %d x q_len %d exceeds the 16 rows of one MMA tile", group, q_len);
+    // the fused rope loads q into one 16-row tile; the plain q load takes up to four
+    ARG_CHECK(!qkv || group <= 16, "paged_decode_attn_rope: group size %d unsupported (1..16)", group);
+    ARG_CHECK(group >= 1 && group <= kAttnMaxRows, "paged_decode_attn: group size %d unsupported (1..%d)", group, kAttnMaxRows);
+    ARG_CHECK(group * q_len <= kAttnMaxRows, "paged_decode_attn: group %d x q_len %d exceeds the limit of %d query rows per (sequence, kv head)",
+              group, q_len, kAttnMaxRows);
     ARG_CHECK(page_size == 16 || page_size == 32 || page_size == 64 || page_size == 128,
               "paged_decode_attn: page_size %zu unsupported (16/32/64/128)", page_size);
     ARG_CHECK(max_seq_len >= 1, "paged_decode_attn: max_seq_len must be >= 1");
@@ -487,18 +490,25 @@ static int attn_impl(const void* q, const void* qkv, float rope_base, int q_len,
     const dim3 grid(p.nsplit, (unsigned)(batch * kv_head_num), 1);
     p.cluster_merge = (p.nsplit >= 2 && p.nsplit <= 8) ? 1 : 0;   // 2..8 splits merge in a cluster, more through the workspace
     const dim3 cluster(p.cluster_merge ? p.nsplit : 1);
-    auto launch = [&](auto t, auto hd) {
-        constexpr auto kern = paged_decode_attn_kernel<decltype(t), decltype(hd)::value>;
+    auto launch = [&](auto t, auto hd, auto rt) {
+        constexpr auto kern = paged_decode_attn_kernel<decltype(t), decltype(hd)::value, decltype(rt)::value>;
         const int smem = attn_smem_bytes(decltype(hd)::value);
         int rc = configure_once<kern>(smem);
         if (rc) return rc;
         CUDA_CHECK(launch_ex(kern, {grid, dim3(kAttnThreads), (size_t)smem, (cudaStream_t)stream, g_pdl.load() != 0, cluster}, map, p));
         return launched("paged_decode_attn_kernel");
     };
+    // query rows in 16-row tiles: 1, 2 or 4 per (sequence, kv head)
+    const int rows = group * q_len;
+    auto by_rows = [&](auto t, auto hd) {
+        if (rows <= 16) return launch(t, hd, std::integral_constant<int, 1>());
+        if (rows <= 32) return launch(t, hd, std::integral_constant<int, 2>());
+        return launch(t, hd, std::integral_constant<int, 4>());
+    };
     return by_dtype(is_bf16, [&](auto t) {
-        if (head_dim == 64) return launch(t, std::integral_constant<int, 64>());
-        if (head_dim == 128) return launch(t, std::integral_constant<int, 128>());
-        return launch(t, std::integral_constant<int, 256>());
+        if (head_dim == 64) return by_rows(t, std::integral_constant<int, 64>());
+        if (head_dim == 128) return by_rows(t, std::integral_constant<int, 128>());
+        return by_rows(t, std::integral_constant<int, 256>());
     });
 }
 
@@ -516,7 +526,7 @@ int b200_paged_decode_attn_multi(const void* q, int is_bf16, void* out, size_t h
                                  const void* kv_pool, const int32_t* page_list, const uint32_t* sequence_lengths, float q_scale,
                                  void* workspace, size_t workspace_bytes, void* stream) {
     ARG_CHECK(q || batch == 0, "paged_decode_attn_multi: null pointer");
-    ARG_CHECK(q_len >= 1 && q_len <= 16, "paged_decode_attn_multi: q_len %zu unsupported", q_len);
+    ARG_CHECK(q_len >= 1 && q_len <= (size_t)kAttnMaxRows, "paged_decode_attn_multi: q_len %zu unsupported (1..%d)", q_len, kAttnMaxRows);
     return attn_impl(q, nullptr, 0.f, (int)q_len, is_bf16, out, head_num, kv_head_num, head_dim, batch, max_blocks_per_seq, max_seq_len,
                      page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, stream);
 }
@@ -814,14 +824,20 @@ int b200_permute_cols(const void* x, const int32_t* perm, void* y, int is_bf16, 
     return launched("permute_cols_kernel");
 }
 
-int b200_rope_append(const void* qkv, void* q_out, void* kv_pool, const int32_t* page_list,
-                     const int32_t* sequence_lengths, int is_bf16, int batch, int head_num, int kv_head_num,
-                     int head_dim, int max_blocks_per_seq, int page_size, float rope_base, void* stream) {
+static int rope_append_impl(const void* qkv, void* q_out, void* kv_pool, const int32_t* page_list, const int32_t* sequence_lengths,
+                            int is_bf16, int batch, int q_len, int head_num, int kv_head_num, int head_dim, int max_blocks_per_seq,
+                            int page_size, float rope_base, void* stream) {
     if (batch == 0) return B200_OK;
     ARG_CHECK(qkv && q_out && kv_pool && page_list && sequence_lengths, "rope_append: null pointer");
     ARG_CHECK(head_dim > 0 && head_dim % 2 == 0 && head_dim <= 512, "rope_append: head_dim %d unsupported", head_dim);
     ARG_CHECK(rope_base > 1.f, "rope_append: rope_base must be > 1");
+    ARG_CHECK(batch > 0 && q_len >= 1 && (long)batch * q_len <= 0x7fffffffL, "rope_append: bad shape batch %d x q_len %d", batch, q_len);
     const float l2b = std::log2(rope_base);
+    if (g_rec && q_len > 1)   // its own launch: the persistent kernel's rope op appends one token per sequence
+        return rec_call([=](void* st) {
+            return rope_append_impl(qkv, q_out, kv_pool, page_list, sequence_lengths, is_bf16, batch, q_len, head_num, kv_head_num,
+                                    head_dim, max_blocks_per_seq, page_size, rope_base, st);
+        });
     if (g_rec) {
         ProgOp op{};
         op.type = kOpRope;
@@ -839,15 +855,31 @@ int b200_rope_append(const void* qkv, void* q_out, void* kv_pool, const int32_t*
         op.r.log2_base = l2b;
         return rec_segment_op(op, is_bf16 ? 1 : 0, -1, -1);
     }
-    const dim3 grid(batch, head_num + 2 * kv_head_num);
+    const dim3 grid(batch * q_len, head_num + 2 * kv_head_num);
     const bool pdl = g_pdl.load() != 0;
     return by_dtype(is_bf16, [&](auto t) {
         using T = decltype(t);
-        CUDA_CHECK(launch_ex(rope_append_kernel<T>, {grid, dim3(head_dim / 2), 0, (cudaStream_t)stream, pdl}, (const T*)qkv,
+        CUDA_CHECK(launch_ex(q_len > 1 ? rope_append_kernel<T, true> : rope_append_kernel<T, false>,
+                             {grid, dim3(head_dim / 2), 0, (cudaStream_t)stream, pdl}, (const T*)qkv,
                              (T*)q_out, (T*)kv_pool, page_list, sequence_lengths, head_num, kv_head_num, head_dim,
-                             (int)max_blocks_per_seq, page_size, l2b));
+                             (int)max_blocks_per_seq, page_size, l2b, q_len));
         return launched("rope_append_kernel");
     });
+}
+
+int b200_rope_append(const void* qkv, void* q_out, void* kv_pool, const int32_t* page_list,
+                     const int32_t* sequence_lengths, int is_bf16, int batch, int head_num, int kv_head_num,
+                     int head_dim, int max_blocks_per_seq, int page_size, float rope_base, void* stream) {
+    return rope_append_impl(qkv, q_out, kv_pool, page_list, sequence_lengths, is_bf16, batch, 1, head_num, kv_head_num, head_dim,
+                            max_blocks_per_seq, page_size, rope_base, stream);
+}
+
+int b200_rope_append_multi(const void* qkv, void* q_out, void* kv_pool, const int32_t* page_list,
+                           const int32_t* sequence_lengths, int is_bf16, int batch, int head_num, int kv_head_num,
+                           int head_dim, int max_blocks_per_seq, int page_size, float rope_base, int q_len, void* stream) {
+    ARG_CHECK(q_len >= 1, "rope_append_multi: q_len %d must be >= 1", q_len);
+    return rope_append_impl(qkv, q_out, kv_pool, page_list, sequence_lengths, is_bf16, batch, q_len, head_num, kv_head_num, head_dim,
+                            max_blocks_per_seq, page_size, rope_base, stream);
 }
 
 int b200_rope_append_ex(const void* qkv, const void* qkv_bias, void* q_out, void* kv_pool, const int32_t* page_list,
@@ -950,6 +982,35 @@ int b200_sample(float* logits, int rows, int vocab, const int32_t* history, cons
     p.hist_stride = hist_stride;
     CUDA_CHECK(launch_ex(sample_kernel, {dim3(rows), dim3(kSampleThreads), 0, (cudaStream_t)stream, g_pdl.load() != 0}, p));
     return launched("sample_kernel");
+}
+
+int b200_spec_verify(const float* target_probs, const int32_t* target_ids, const float* draft_probs, const int32_t* draft_tokens,
+                     const float* uniform, int batch, int num_draft, int vocab, int32_t* out_tokens, int32_t* accepted, void* stream) {
+    ARG_CHECK(batch >= 0 && batch <= 65535, "spec_verify: batch %d unsupported (0..65535)", batch);
+    ARG_CHECK(num_draft >= 0, "spec_verify: num_draft %d must be >= 0", num_draft);
+    ARG_CHECK(vocab > 0, "spec_verify: vocab must be positive");
+    if (batch == 0) return B200_OK;
+    ARG_CHECK(out_tokens && accepted && (draft_tokens || num_draft == 0), "spec_verify: null pointer");
+    ARG_CHECK(target_probs || target_ids, "spec_verify: need target_probs (sampling) or target_ids (greedy)");
+    ARG_CHECK(!target_probs || uniform, "spec_verify: sampling mode needs uniform");
+    ARG_CHECK(!draft_probs || target_probs, "spec_verify: draft_probs need target_probs");
+    if (g_rec)
+        return rec_call([=](void* st) {
+            return b200_spec_verify(target_probs, target_ids, draft_probs, draft_tokens, uniform, batch, num_draft, vocab, out_tokens,
+                                    accepted, st);
+        });
+    SpecVerifyParams p{};
+    p.target_probs = target_probs;
+    p.target_ids = target_ids;
+    p.draft_probs = draft_probs;
+    p.draft_tokens = draft_tokens;
+    p.uniform = uniform;
+    p.out_tokens = out_tokens;
+    p.accepted = accepted;
+    p.num_draft = num_draft;
+    p.vocab = vocab;
+    CUDA_CHECK(launch_ex(spec_verify_kernel, {dim3(batch), dim3(kSampleThreads), 0, (cudaStream_t)stream, g_pdl.load() != 0}, p));
+    return launched("spec_verify_kernel");
 }
 
 // ------------------------------------------------------------------------------------------------ peer all-reduce

@@ -13,6 +13,9 @@
 //   (ldmatrix + mma.sync m16n8k16; the whole GQA group is packed into the MMA M dimension so every K/V byte is read
 //   from HBM exactly once), online softmax with quad-level shuffles, private running (m, l, O) per warp, merged
 //   through shared memory at the end.  Sequence splits are merged by the last-arriving CTA (semaphore), XQA-style.
+//   Query rows (group x q_len, up to 64) span RT = 1 / 2 / 4 row tiles of 16: consumer warp w owns row tile w % RT and,
+//   within each 64-token stage, the 16-token slices w / RT + k * (4 / RT) one after another, so K/V are still read from
+//   HBM once per (sequence, kv head) and a warp's registers are those of one row tile. RT == 1 is the single-tile kernel.
 //   The kernel is HBM-bound: per CTA 96 KB of K/V in flight, two CTAs per SM.
 #pragma once
 #include "ptx.cuh"
@@ -23,6 +26,7 @@ constexpr int kAttnTile = 64;          // tokens per pipeline stage
 constexpr int kAttnStages = 3;
 constexpr int kAttnD = 128;            // head dim
 constexpr int kAttnConsumerWarps = 4;
+constexpr int kAttnMaxRows = 64;       // query rows (group x q_len) per (sequence, kv head): four 16-row MMA tiles
 constexpr int kAttnThreads = (kAttnConsumerWarps + 1) * 32;
 // per head dim D (64 / 128 / 256): a stage holds the D/64 64-channel halves of K, then those of V, 8 KB each (64 tokens x 128 B)
 __host__ __device__ constexpr int attn_stage_bytes(int D) { return 2 * (D / 64) * kAttnTile * 128; }
@@ -39,7 +43,8 @@ struct AttnParams {
     int B, Hq, Hkv, group, M;
     int q_len;                // query tokens per sequence (1 = plain decode; > 1 = verification of speculative tokens, XQA's
                               // max_q_len / trtllm-gen's q_len_per_req): q [B][q_len][Hq][D], query j attends to positions
-                              // 0 .. seq_lens[b] + j, its GQA rows sit at MMA rows j * group + g (group * q_len <= 16)
+                              // 0 .. seq_lens[b] + j, its GQA rows sit at MMA rows j * group + g (group * q_len <= 64,
+                              // row tile (j * group + g) / 16)
     int T, log2T;             // tokens per page
     int box_h, boxes_per_tile;
     int nsplit, tiles_per_split;
@@ -58,13 +63,19 @@ struct AttnParams {
                               //    their partial (m, l, O) through distributed shared memory; no workspace, no semaphore
 };
 
-template <typename T, int D = kAttnD>
+// RT: 16-row tiles of query rows (rows = group * q_len rounded up to 16 / 32 / 64)
+template <typename T, int D = kAttnD, int RT = 1>
 __global__ void __launch_bounds__(kAttnThreads, D <= 128 ? 2 : 1)
 paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const AttnParams p) {
     constexpr int NH = D / 64;                       // 64-channel halves per K / V row
     constexpr int STAGE = attn_stage_bytes(D);
     constexpr int OROW = D + 8;                      // floats; +8 banks per row -> conflict-free float2 stores
+    constexpr int NW = kAttnConsumerWarps / RT;      // warps per row tile (each takes RT of a stage's 4 slices)
     static_assert(D == 64 || D == 128 || D == 256, "head_dim 64 / 128 / 256");
+    static_assert(RT == 1 || RT == 2 || RT == 4, "1, 2 or 4 row tiles");
+    // the merge staging (per-warp o / m / l, then the cluster partial [rows][D] + (m, l)) reuses the K/V ring
+    static_assert((kAttnConsumerWarps * 16 * (OROW + 2) + RT * 16 * (D + 2)) * 4 <= kAttnStages * STAGE,
+                  "merge staging exceeds the K/V ring");
     extern __shared__ uint8_t smem_raw[];
     // 1024-byte alignment for the 128B-swizzled boxes
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -141,7 +152,7 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const AttnP
         int first_end = t1;                               // tiles [t0, first_end) are issued before the append
         bool own = false;
         int pos = 0;
-        if (D == 128 && p.qkv != nullptr) {   // fused rope is built for head_dim 128 (the host rejects other sizes)
+        if (D == 128 && RT == 1 && p.qkv != nullptr) {   // fused rope: head_dim 128, one row tile (the host rejects others)
             pos = p.seq_lens[b];
             own = pos < len && (pos / kAttnTile) >= t0 && (pos / kAttnTile) < t1;      // this CTA streams the new token's tile
             if (own) first_end = min(min(t0 + kAttnStages, t1), pos / kAttnTile);
@@ -191,10 +202,12 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const AttnP
     // ---------------------------------------------------------------------- consumers
     const int qrow = lane >> 2;          // fragment row (and row + 8)
     const int qcol = (lane & 3) * 2;     // fragment column pair
+    const int rt = warp % RT;            // this warp's row tile: MMA rows rt * 16 + qrow (and + 8)
+    const int row0 = rt * 16 + qrow, row1 = row0 + 8;
     // Q fragments for the whole head dim: 8 k-steps x 4 regs. Rows >= group are zero.
     uint32_t qf[D / 16][4];
     bool q_loaded = false;
-    if constexpr (D == 128) {
+    if constexpr (D == 128 && RT == 1) {
       if (p.qkv) {
         q_loaded = true;
         // un-rotated q straight from the qkv GEMM output; the NeoX partner of column c < 64 is column c + 64 = the same
@@ -239,10 +252,10 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const AttnP
     }
     if (!q_loaded) {
         // MMA row R = j * group + g  <->  query token j, head kvh * group + g
-        const bool v0 = qrow < rows, v1 = (qrow + 8) < rows;
+        const bool v0 = row0 < rows, v1 = row1 < rows;
         const T* qall = reinterpret_cast<const T*>(p.q);
-        const T* q0 = qall + (((size_t)b * p.q_len + qrow / p.group) * p.Hq + (size_t)kvh * p.group + qrow % p.group) * D;
-        const T* q1 = qall + (((size_t)b * p.q_len + (qrow + 8) / p.group) * p.Hq + (size_t)kvh * p.group + (qrow + 8) % p.group) * D;
+        const T* q0 = qall + (((size_t)b * p.q_len + row0 / p.group) * p.Hq + (size_t)kvh * p.group + row0 % p.group) * D;
+        const T* q1 = qall + (((size_t)b * p.q_len + row1 / p.group) * p.Hq + (size_t)kvh * p.group + row1 % p.group) * D;
 #pragma unroll
         for (int kk = 0; kk < D / 16; ++kk) {
             const int c = kk * 16 + qcol;
@@ -259,13 +272,13 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const AttnP
     float m0 = -INFINITY, m1 = -INFINITY;  // running max (raw score units) for rows qrow / qrow+8
     float l0 = 0.f, l1 = 0.f;              // per-thread partial row sums (quad-reduced at the end)
     const float sl2 = p.scale_log2;
-    const int off0 = p.q_len - 1 - min(qrow / p.group, p.q_len - 1), off1 = p.q_len - 1 - min((qrow + 8) / p.group, p.q_len - 1);
+    const int off0 = p.q_len - 1 - min(row0 / p.group, p.q_len - 1), off1 = p.q_len - 1 - min(row1 / p.group, p.q_len - 1);
 
     // ldmatrix lane geometry
     const int mi = lane >> 3, mr = lane & 7;
-    const int k_tokrow = warp * 16 + (mi >> 1) * 8 + mr;  // K: matrices (tok0-7,c),(tok0-7,c+1),(tok8-15,c),(tok8-15,c+1)
+    const int k_tokrow0 = warp / RT * 16 + (mi >> 1) * 8 + mr;  // K: matrices (tok0-7,c),(tok0-7,c+1),(tok8-15,c),(tok8-15,c+1)
     const int k_chunk_add = mi & 1;
-    const int v_tokrow = warp * 16 + (mi & 1) * 8 + mr;   // V (trans): (tok0-7,c),(tok8-15,c),(tok0-7,c+1),(tok8-15,c+1)
+    const int v_tokrow0 = warp / RT * 16 + (mi & 1) * 8 + mr;   // V (trans): (tok0-7,c),(tok8-15,c),(tok0-7,c+1),(tok8-15,c+1)
     const int v_chunk_add = mi >> 1;
 
     for (int i = t0; i < t1; ++i) {
@@ -275,14 +288,19 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const AttnP
         uint8_t* stage = smem + s * STAGE;
         const uint32_t k_base = smem_u32(stage), v_base = k_base + NH * 8192;
 
-        const int tok0 = i * kAttnTile + warp * 16;
-        const int valid = len - tok0;  // tokens of this warp's slice that exist (may be <= 0)
+#pragma unroll
+      for (int ks = 0; ks < RT; ++ks) {
+        const int slice = warp / RT + ks * NW;           // 16-token slice of the stage
+        const int k_tokrow = k_tokrow0 + ks * NW * 16, v_tokrow = v_tokrow0 + ks * NW * 16;
+        const int tok0 = i * kAttnTile + slice * 16;
+        const int valid = len - tok0;  // tokens of this slice that exist (may be <= 0)
         if (valid < 16) {
             // Rows past the end of the sequence hold stale / never-written bytes: P is 0 there but 0 * NaN = NaN,
-            // so the V rows are zeroed before use (K garbage is masked on the scores below).
+            // so the V rows are zeroed before use (K garbage is masked on the scores below). With RT > 1 the warps of the
+            // other row tiles zero the same rows: they all store zeros, and each reads only after its own stores.
             const int first = valid < 0 ? 0 : valid;
             for (int r = first; r < 16; ++r) {
-                uint8_t* row = stage + NH * 8192 + (warp * 16 + r) * 128;
+                uint8_t* row = stage + NH * 8192 + (slice * 16 + r) * 128;
 #pragma unroll
                 for (int h = 0; h < NH; ++h) reinterpret_cast<uint32_t*>(row + h * 8192)[lane] = 0u;
             }
@@ -364,6 +382,7 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const AttnP
             mma_m16n8k16<T>(o[2 * n2], pf, vb[0], vb[1]);
             mma_m16n8k16<T>(o[2 * n2 + 1], pf, vb[2], vb[3]);
         }
+      }
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty_bar[s]);
     }
@@ -374,7 +393,7 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const AttnP
     l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
     l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
 
-    // ---------------------------------------------------------------------- merge the 4 warps through smem
+    // ---------------------------------------------------------------------- merge the NW warps of each row tile through smem
     asm volatile("bar.sync 1, 128;" ::: "memory");  // everyone is done reading the K/V ring
     float* o_s = reinterpret_cast<float*>(smem);                              // [4][16][OROW]
     float* m_s = o_s + kAttnConsumerWarps * 16 * OROW;                        // [4][16]
@@ -403,18 +422,20 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const AttnP
     auto out_row = [&](int r) {
         return reinterpret_cast<T*>(p.out) + (((size_t)b * p.q_len + r / p.group) * p.Hq + (size_t)kvh * p.group + r % p.group) * D;
     };
-    // per-CTA partial of the cluster merge: [16 rows][D] fp32 + (m, l) per row, behind the per-warp staging area
+    // per-CTA partial of the cluster merge: [rows][D] fp32 + (m, l) per row, behind the per-warp staging area
     float* part_o = l_s + kAttnConsumerWarps * 16;
-    float* part_ml = part_o + 16 * D;
+    float* part_ml = part_o + RT * 16 * D;
     for (int r = 0; r < rows; ++r) {
+        // row r is row rr of row tile r / 16, staged by the warps w = r / 16 + RT * j (j < NW)
+        const int wt = RT == 1 ? 0 : r >> 4, rr = RT == 1 ? r : r & 15;
         float m = -INFINITY;
 #pragma unroll
-        for (int w = 0; w < kAttnConsumerWarps; ++w) m = fmaxf(m, m_s[w * 16 + r]);
-        float f[kAttnConsumerWarps], l = 0.f;
+        for (int j = 0; j < NW; ++j) m = fmaxf(m, m_s[(wt + RT * j) * 16 + rr]);
+        float f[NW], l = 0.f;
 #pragma unroll
-        for (int w = 0; w < kAttnConsumerWarps; ++w) {
-            f[w] = (m == -INFINITY) ? 0.f : fast_exp2((m_s[w * 16 + r] - m) * sl2);  // -inf -> 0
-            l = fmaf(f[w], l_s[w * 16 + r], l);
+        for (int j = 0; j < NW; ++j) {
+            f[j] = (m == -INFINITY) ? 0.f : fast_exp2((m_s[(wt + RT * j) * 16 + rr] - m) * sl2);  // -inf -> 0
+            l = fmaf(f[j], l_s[(wt + RT * j) * 16 + rr], l);
         }
         if (d0 == 0) {
             if (p.cluster_merge) {
@@ -431,7 +452,7 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const AttnP
             if (d >= D) break;
             float acc = 0.f;
 #pragma unroll
-            for (int w = 0; w < kAttnConsumerWarps; ++w) acc = fmaf(f[w], o_s[((size_t)w * 16 + r) * OROW + d], acc);
+            for (int w = 0; w < NW; ++w) acc = fmaf(f[w], o_s[((size_t)(wt + RT * w) * 16 + rr) * OROW + d], acc);
             if (p.cluster_merge) part_o[r * D + d] = acc;
             else if (nact == 1) out_row(r)[d] = from_f32<T>(acc / l);
             else p.ws_o[(ws_base + r) * D + d] = acc;

@@ -69,6 +69,55 @@ __device__ __forceinline__ float block_reduce_max(float v, float* s_red) {
     return t;
 }
 
+// One inverse-CDF draw over the masses mass(i) >= 0 of i in [0, V) in index order (every thread of the CTA calls it): each
+// thread sums a contiguous chunk of ceil(V/1024) masses, a block scan of the chunk sums gives each chunk's start, and the
+// target u * total (clamped below total; 0 when `lowest` asks for the first index with mass) goes to the last thread with mass
+// whose start is <= target. Returns the token (-1 when no mass is positive) and the scanned total, identical in every thread.
+template <typename Mass>
+__device__ __forceinline__ int chunked_draw(const Mass& mass, int V, float u, bool lowest, float* s_scan, int* s_pick,
+                                            int* s_owner, float* total_out) {
+    const int tid = threadIdx.x;
+    const int per = (V + kSampleThreads - 1) / kSampleThreads;
+    const int i0 = tid * per, i1 = min(V, i0 + per);
+    float mine = 0.f;
+    for (int i = i0; i < i1; ++i) mine += mass(i);
+    s_scan[tid] = mine;
+    if (tid == 0) *s_owner = *s_pick = -1;
+    __syncthreads();
+    for (int off = 1; off < kSampleThreads; off <<= 1) {   // Hillis-Steele inclusive scan
+        const float add = tid >= off ? s_scan[tid - off] : 0.f;
+        __syncthreads();
+        s_scan[tid] += add;
+        __syncthreads();
+    }
+    const float total = s_scan[kSampleThreads - 1];
+    // u * total can round up to total: clamp below it.
+    const float target = lowest ? 0.f : fminf(u * total, __uint_as_float(__float_as_uint(total) - 1u));
+    const float start = tid ? s_scan[tid - 1] : 0.f;
+    // Every prefix sum is rounded in its own tree order, so the chunk intervals [start, s_scan[tid]) can overlap or leave gaps.
+    // The owner is the LAST thread with positive mass whose start is <= target: exactly one thread. It exists whenever the
+    // kept mass is positive, because the first thread with mass starts at an exact 0 (only zeros precede it) and target >= 0.
+    const int warp_owner = __reduce_max_sync(0xffffffffu, mine > 0.f && start <= target ? tid : -1);
+    if ((tid & 31) == 0 && warp_owner >= 0) atomicMax(s_owner, warp_owner);
+    __syncthreads();
+    if (tid == *s_owner) {
+        float c = start;
+        int pick = -1;
+        for (int i = i0; i < i1; ++i) {
+            const float m = mass(i);
+            if (m > 0.f) {
+                c += m;
+                pick = i;                  // the chunk's last token with mass is the fallback when rounding undershoots
+                if (c > target) break;
+            }
+        }
+        *s_pick = pick;
+    }
+    __syncthreads();
+    *total_out = total;
+    return *s_pick;
+}
+
 __global__ void __launch_bounds__(kSampleThreads) sample_kernel(const SampleParams p) {
     __shared__ float s_red[kSampleThreads / 32];
     __shared__ float s_scan[kSampleThreads];
@@ -173,43 +222,10 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(const SamplePara
     }
 
     // ---- draw: inverse CDF over the kept tokens in index order (contiguous chunk per thread, block scan of chunk sums)
-    const int per = (V + kSampleThreads - 1) / kSampleThreads;
-    const int i0 = tid * per, i1 = min(V, i0 + per);
-    float mine = 0.f;
-    for (int i = i0; i < i1; ++i) mine += lg[i] >= thr ? lg[i] : 0.f;
-    s_scan[tid] = mine;
-    if (tid == 0) s_owner = s_pick = -1;
-    __syncthreads();
-    for (int off = 1; off < kSampleThreads; off <<= 1) {   // Hillis-Steele inclusive scan
-        const float add = tid >= off ? s_scan[tid - off] : 0.f;
-        __syncthreads();
-        s_scan[tid] += add;
-        __syncthreads();
-    }
-    const float total = s_scan[kSampleThreads - 1];
-    // top_k == 1: the lowest index among the maxima (argmax semantics). u * total can round up to total: clamp below it.
-    const float target = k == 1 ? 0.f : fminf(p.uniform[row] * total, __uint_as_float(__float_as_uint(total) - 1u));
-    const float start = tid ? s_scan[tid - 1] : 0.f;
-    // Every prefix sum is rounded in its own tree order, so the chunk intervals [start, s_scan[tid]) can overlap or leave gaps.
-    // The owner is the LAST thread with positive mass whose start is <= target: exactly one thread. It exists whenever the
-    // kept mass is positive, because the first thread with mass starts at an exact 0 (only zeros precede it) and target >= 0.
-    const int warp_owner = __reduce_max_sync(0xffffffffu, mine > 0.f && start <= target ? tid : -1);
-    if ((tid & 31) == 0 && warp_owner >= 0) atomicMax(&s_owner, warp_owner);
-    __syncthreads();
-    if (tid == s_owner) {
-        float c = start;
-        int pick = -1;
-        for (int i = i0; i < i1; ++i) {
-            if (lg[i] >= thr && lg[i] > 0.f) {
-                c += lg[i];
-                pick = i;                  // the chunk's last kept token with p > 0 is the fallback when rounding undershoots
-                if (c > target) break;
-            }
-        }
-        s_pick = pick;
-    }
-    __syncthreads();
-    const int tok = s_pick;
+    // top_k == 1: the lowest index among the maxima (argmax semantics)
+    float total;
+    const int tok = chunked_draw([&](int i) { return lg[i] >= thr ? lg[i] : 0.f; }, V, p.uniform[row], k == 1, s_scan, &s_pick,
+                                 &s_owner, &total);
     const float inv_total = 1.f / total;
     if (tid == 0) {
         p.token_out[row] = tok;
@@ -218,6 +234,73 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(const SamplePara
     if (p.probs_out) {
         float* po = p.probs_out + (size_t)row * V;
         for (int i = tid; i < V; i += kSampleThreads) po[i] = lg[i] >= thr ? lg[i] * inv_total : 0.f;
+    }
+}
+
+// Verification of n = num_draft speculative tokens per sequence against the target model's rows of the same step
+// (the reference's speculative-sampling kernel, bindings/cuda/kernels/speculative_sampling/sampling.cu, chain form).
+// Greedy (target_probs == NULL): accept draft i while it equals target_ids[i]; emit target_ids[accepted].
+// Sampling: accept draft d_i iff uniform[i] * p(d_i) < q(d_i) (fp32; p = draft_probs, 1 for deterministic drafts), stop at the
+// first rejection and draw from the residual max(0, q - p) -- from q itself when the residual has no mass -- or, with every draft
+// accepted, the bonus token from the last row; both draws use uniform[n] and chunked_draw. One CTA of 1024 threads per sequence.
+struct SpecVerifyParams {
+    const float* target_probs;    // optional [B][n+1][V]
+    const int32_t* target_ids;    // [B][n+1] (greedy mode)
+    const float* draft_probs;     // optional [B][n][V]
+    const int32_t* draft_tokens;  // [B][n]
+    const float* uniform;         // [B][n+1] (sampling mode)
+    int32_t* out_tokens;          // [B][n+1]: accepted drafts, one correction / bonus token, then -1
+    int32_t* accepted;            // [B]
+    int num_draft, vocab;
+};
+
+__global__ void __launch_bounds__(kSampleThreads) spec_verify_kernel(const SpecVerifyParams p) {
+    __shared__ float s_scan[kSampleThreads];
+    __shared__ int s_pick, s_owner;
+    const int b = blockIdx.x, tid = threadIdx.x, n = p.num_draft, V = p.vocab;
+    pdl_wait();                        // under PDL the target rows come from the kernels before this one
+    const int32_t* draft = p.draft_tokens + (size_t)b * n;
+    int acc = 0, tok;
+    if (!p.target_probs) {
+        const int32_t* ids = p.target_ids + (size_t)b * (n + 1);
+        while (acc < n && draft[acc] == ids[acc]) ++acc;
+        tok = ids[acc];
+    } else {
+        const float* u = p.uniform + (size_t)b * (n + 1);
+        auto trow = [&](int i) { return p.target_probs + ((size_t)b * (n + 1) + i) * V; };
+        auto drow = [&](int i) { return p.draft_probs + ((size_t)b * n + i) * V; };
+        // every thread walks the same chain (the same loads, the same fp32 compares): a uniform decision
+        for (; acc < n; ++acc) {
+            const int d = draft[acc];
+            const bool in = d >= 0 && d < V;
+            const float q = in ? trow(acc)[d] : 0.f;
+            const float pd = p.draft_probs ? (in ? drow(acc)[d] : 0.f) : 1.f;
+            if (!(u[acc] * pd < q)) break;
+        }
+        float total;
+        if (acc < n) {
+            const float* t = trow(acc);
+            const int d = draft[acc];
+            if (p.draft_probs) {
+                const float* dp = drow(acc);
+                tok = chunked_draw([&](int x) { return fmaxf(0.f, t[x] - dp[x]); }, V, u[n], false, s_scan, &s_pick, &s_owner, &total);
+            } else {
+                tok = chunked_draw([&](int x) { return fmaxf(0.f, t[x] - (x == d ? 1.f : 0.f)); }, V, u[n], false, s_scan, &s_pick,
+                                   &s_owner, &total);
+            }
+            if (!(total > 0.f)) {          // the residual has no mass (q <= p everywhere): draw from q
+                __syncthreads();           // every thread has read the first draw's shared result
+                tok = chunked_draw([&](int x) { return t[x] > 0.f ? t[x] : 0.f; }, V, u[n], false, s_scan, &s_pick, &s_owner, &total);
+            }
+        } else {
+            const float* t = trow(n);
+            tok = chunked_draw([&](int x) { return t[x] > 0.f ? t[x] : 0.f; }, V, u[n], false, s_scan, &s_pick, &s_owner, &total);
+        }
+    }
+    if (tid == 0) {
+        int32_t* out = p.out_tokens + (size_t)b * (n + 1);
+        for (int i = 0; i <= n; ++i) out[i] = i < acc ? draft[i] : (i == acc ? tok : -1);
+        p.accepted[b] = acc;
     }
 }
 

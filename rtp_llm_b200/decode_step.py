@@ -65,13 +65,25 @@ class DecodeStep:
     act_order=True (TP 1, quant int4 / int8g): every quantised weight is a GPTQ act-order weight with its rows sorted by g_idx,
     from seeded random row orders. qkv, o and w13 carry theirs in the blob, and x is gathered (b200_permute_cols) into a static
     buffer before each of them; w2's order is folded into w13's output columns, as B200Loader.layer does. A row-parallel o
-    shard would mix groups of every rank, so TP > 1 is rejected."""
+    shard would mix groups of every rank, so TP > 1 is rejected.
+
+    q_len > 1 (TP 1, op by op or under a CUDA graph; not in a decode program): a verification step of speculative tokens. Each
+    sequence feeds q_len tokens, ids_h [B, q_len] = the last accepted token and q_len - 1 drafts, at positions seq_lens_h[b] + j.
+    Every op runs on the B * q_len rows (rope_append / paged_decode_attn_multi for the attention), argmax picks each row's
+    token, and spec_verify (greedy) checks the drafts against them: out_tokens [B, q_len], accepted [B]."""
 
     def __init__(self, cfg: ModelConfig, batch: int, ctx: int, device: torch.device, tp_rank: int = 0, tp_size: int = 1,
                  dtype=torch.float16, seed: int = 0, keep_reference: bool = False, ragged: bool = False,
                  pdl: bool = False, comm=None, fuse_silu: bool = True, fuse_ar_norm: bool = True, fuse_rope: Optional[bool] = None,
-                 fuse_gemm_rs: Optional[bool] = None, act_order: bool = False):
+                 fuse_gemm_rs: Optional[bool] = None, act_order: bool = False, q_len: int = 1):
         assert cfg.head_num % tp_size == 0 and cfg.inter % tp_size == 0
+        if q_len < 1:
+            raise ValueError(f"q_len must be >= 1 (got {q_len})")
+        if q_len > 1 and (batch * q_len > 128 or tp_size != 1):
+            raise ValueError(f"a verification step (q_len {q_len}) needs batch * q_len <= 128 (the GEMM row limit) and tp_size 1 "
+                             f"(got batch {batch}, tp_size {tp_size})")
+        self.q_len = q_len
+        R = batch * q_len                               # token rows of the step
         if act_order and (tp_size != 1 or cfg.quant not in ("int4", "int8g")):
             raise ValueError(f"act_order needs tp_size 1 and quant int4 / int8g (got tp_size {tp_size}, quant {cfg.quant})")
         self.act_order = act_order
@@ -101,7 +113,7 @@ class DecodeStep:
         # Default off; B200_FUSE_ROPE=1 or fuse_rope=True turns it on.
         if fuse_rope is None:
             fuse_rope = os.environ.get("B200_FUSE_ROPE", "0") == "1"
-        self.fuse_rope = bool(fuse_rope) and cfg.head_dim == 128
+        self.fuse_rope = bool(fuse_rope) and cfg.head_dim == 128 and q_len == 1    # the fused rope appends one token
         g = torch.Generator(device="cpu").manual_seed(seed * 1000 + 17)
         H = cfg.hidden
 
@@ -225,33 +237,41 @@ class DecodeStep:
             lens = torch.randint(ctx // 2, ctx + 1, (batch,), generator=gl)
         else:
             lens = torch.full((batch,), ctx)
-        self.seq_lens_h = (lens - 1).to(torch.int32).pin_memory()       # tokens already cached (SURVEY a3)
-        self.ids_h = torch.randint(0, cfg.vocab, (batch,), generator=gp).to(torch.int32).pin_memory()
+        self.seq_lens_h = (lens - q_len).to(torch.int32).pin_memory()   # tokens already cached (SURVEY a3)
+        self.ids_h = torch.randint(0, cfg.vocab, (batch,) if q_len == 1 else (batch, q_len), generator=gp).to(torch.int32).pin_memory()
         self.next_h = torch.zeros(batch, dtype=torch.int32).pin_memory()
+        if q_len > 1:
+            self.drafts_h = torch.zeros(batch, q_len - 1, dtype=torch.int32).pin_memory()
+            self.out_tokens_h = torch.zeros(batch, q_len, dtype=torch.int32).pin_memory()
+            self.accepted_h = torch.zeros(batch, dtype=torch.int32).pin_memory()
 
         # ---- static device buffers (graph-capturable: nothing is allocated inside step())
         def buf(*shape, dt=dtype):
             return torch.empty(*shape, dtype=dt, device=device)
-        self.ids = buf(batch, dt=torch.int32)
+        self.ids = buf(R, dt=torch.int32)
         self.seq_lens = buf(batch, dt=torch.int32)
         self.block_ids = buf(batch, self.M, dt=torch.int32)
         self.page_list = buf(batch, 1, 2, self.M, dt=torch.int32)
-        self.resid = buf(batch, H)
-        self.x = buf(batch, H)
-        self.qkv = buf(batch, qkv_n)
-        self.q = buf(batch, self.Hq * self.D)
-        self.attn = buf(batch, self.Hq * self.D)
-        self.proj = buf(batch, H)
-        self.gu = buf(batch, 2 * self.inter)
-        self.act = buf(batch, self.inter)
-        self.logits = buf(batch, self.vocab)
+        self.resid = buf(R, H)
+        self.x = buf(R, H)
+        self.qkv = buf(R, qkv_n)
+        self.q = buf(R, self.Hq * self.D)
+        self.attn = buf(R, self.Hq * self.D)
+        self.proj = buf(R, H)
+        self.gu = buf(R, 2 * self.inter)
+        self.act = buf(R, self.inter)
+        self.logits = buf(R, self.vocab)
         self.logits_all = buf(tp_size, batch, self.vocab) if tp_size > 1 else None
-        self.next_ids = buf(batch, dt=torch.int32)
-        self.x_perm = buf(batch, H) if act_order else None                    # x[:, perm] before qkv / w13
-        self.attn_perm = buf(batch, self.Hq * self.D) if act_order else None  # attn[:, perm] before o
+        self.next_ids = buf(R, dt=torch.int32)                                # each row's greedy token
+        if q_len > 1:
+            self.drafts = buf(batch, q_len - 1, dt=torch.int32)
+            self.out_tokens = buf(batch, q_len, dt=torch.int32)
+            self.accepted = buf(batch, dt=torch.int32)
+        self.x_perm = buf(R, H) if act_order else None                        # x[:, perm] before qkv / w13
+        self.attn_perm = buf(R, self.Hq * self.D) if act_order else None      # attn[:, perm] before o
         shapes = [(H, qkv_n), (self.Hq * self.D, H), (H, 2 * self.inter), (self.inter, H), (H, self.vocab)]
-        self.gemm_ws = ops.gemm_workspace(batch, shapes, device)
-        self.attn_ws = ops.attn_workspace(batch, self.Hq, self.Hkv, ctx, device)
+        self.gemm_ws = ops.gemm_workspace(R, shapes, device)
+        self.attn_ws = ops.attn_workspace(R, self.Hq, self.Hkv, ctx, device)
         ops.set_pdl(pdl)
         self.graph: Optional[torch.cuda.CUDAGraph] = None
         self.prog = None
@@ -261,17 +281,27 @@ class DecodeStep:
     # ------------------------------------------------------------------ host <-> device
     def upload_inputs(self):
         """H2D of one step's inputs from pinned host memory (token ids, lengths, block table)."""
-        self.ids.copy_(self.ids_h, non_blocking=True)
+        self.ids.copy_(self.ids_h.view(-1), non_blocking=True)
         self.seq_lens.copy_(self.seq_lens_h, non_blocking=True)
         self.block_ids.copy_(self.block_ids_h, non_blocking=True)
+        if self.q_len > 1:
+            self.drafts_h.copy_(self.ids_h[:, 1:])
+            self.drafts.copy_(self.drafts_h, non_blocking=True)
 
     def download_outputs(self):
+        if self.q_len > 1:
+            self.out_tokens_h.copy_(self.out_tokens, non_blocking=True)
+            self.accepted_h.copy_(self.accepted, non_blocking=True)
+            return
         self.next_h.copy_(self.next_ids, non_blocking=True)
 
     def h2d_bytes(self) -> int:
-        return self.ids_h.numel() * 4 + self.seq_lens_h.numel() * 4 + self.block_ids_h.numel() * 4
+        drafts = self.drafts_h.numel() * 4 if self.q_len > 1 else 0
+        return self.ids_h.numel() * 4 + self.seq_lens_h.numel() * 4 + self.block_ids_h.numel() * 4 + drafts
 
     def d2h_bytes(self) -> int:
+        if self.q_len > 1:
+            return self.out_tokens_h.numel() * 4 + self.accepted_h.numel() * 4
         return self.next_h.numel() * 4
 
     # ------------------------------------------------------------------ the step
@@ -317,6 +347,11 @@ class DecodeStep:
             if self.fuse_rope:    # RoPE + K/V append inside the attention kernel (one launch instead of two)
                 ops.paged_decode_attn_rope(self.qkv, L["kv"], self.page_list, self.seq_lens, self.Hq, self.ctx, cfg.rope_base,
                                            self.attn_ws, out=self.attn)
+            elif self.q_len > 1:  # K/V of all q_len tokens appended, then each query token attends up to its own position
+                ops.rope_append(self.qkv, L["kv"], self.page_list, self.seq_lens, self.Hq, cfg.rope_base, q_out=self.q,
+                                q_len=self.q_len)
+                ops.paged_decode_attn_multi(self.q.view(self.B, self.q_len, self.Hq, self.D), L["kv"], self.page_list, self.seq_lens,
+                                            self.ctx, self.attn_ws, out=self.attn.view(self.B, self.q_len, self.Hq * self.D))
             else:
                 ops.rope_append(self.qkv, L["kv"], self.page_list, self.seq_lens, self.Hq, cfg.rope_base, q_out=self.q)
                 ops.paged_decode_attn(self.q, L["kv"], self.page_list, self.seq_lens, self.ctx, self.attn_ws, out=self.attn)
@@ -332,6 +367,9 @@ class DecodeStep:
         ops.wo_gemm(self.x, self.lm_head, self.gemm_ws, out=self.logits, pdl=self.pdl)
         if self.tp_size == 1:
             ops.argmax(self.logits, out=self.next_ids)
+            if self.q_len > 1:
+                ops.spec_verify(self.drafts, target_ids=self.next_ids.view(self.B, self.q_len), out_tokens=self.out_tokens,
+                                accepted=self.accepted)
         elif hasattr(self.comm, "argmax"):
             self.comm.argmax(self.logits, cfg.vocab, self.next_ids)     # vocab-parallel greedy sampling, own kernel
 
@@ -352,6 +390,8 @@ class DecodeStep:
         persistent-kernel launch. Requires every call in step_core to go through the C ABI (own peer all-reduce, not NCCL)."""
         from . import tp as tpmod
         assert self.tp_size == 1 or isinstance(self.comm, tpmod.PeerComm), "a program cannot record NCCL calls"
+        if self.q_len > 1:
+            raise ValueError("a verification step (q_len > 1) runs op by op or under a CUDA graph, not as a decode program")
         self.prog = ops.Program()
         with self.prog.record():
             self.step_core()
@@ -392,7 +432,7 @@ class DecodeStep:
         qkv_n = (self.Hq + 2 * self.Hkv) * self.D
         w = (weight_bytes(cfg, H, qkv_n) + weight_bytes(cfg, self.Hq * self.D, H) + weight_bytes(cfg, H, 2 * self.inter)
              + weight_bytes(cfg, self.inter, H)) * cfg.layers
-        lens = (self.seq_lens_h.to(torch.int64) + 1).sum().item()
+        lens = (self.seq_lens_h.to(torch.int64) + self.q_len).sum().item()
         kv = 2.0 * lens * self.Hkv * self.D * 2 * cfg.layers
         lm = 2.0 * H * self.vocab
         return dict(weights=w, kv=kv, lm_head=lm, total=w + kv + lm)

@@ -363,15 +363,25 @@ def silu_and_mul(gate_up, out=None):
     return out
 
 
-def rope_append(qkv, kv_cache_base, page_list, sequence_lengths, head_num, rope_base, q_out=None):
+def rope_append(qkv, kv_cache_base, page_list, sequence_lengths, head_num, rope_base, q_out=None, q_len: int = 1):
+    """qkv [B*q_len, (Hq+2Hkv)*D]: q_len new tokens per sequence (row b*q_len + j = token j of sequence b, rotated and
+    appended at sequence_lengths[b] + j). Returns q [B*q_len, Hq*D]."""
     _cuda_contig(qkv, kv_cache_base, page_list, sequence_lengths, q_out)
     P, two, Hkv, T, D = kv_cache_base.shape
-    B = qkv.shape[0]
+    rows = qkv.shape[0]
+    if q_len < 1 or rows % q_len:
+        raise B200Error(f"rope_append: {rows} qkv rows are not a multiple of q_len {q_len}")
     if q_out is None:
-        q_out = torch.empty((B, head_num * D), dtype=qkv.dtype, device=qkv.device)
-    check(_lib.load().b200_rope_append(_p(qkv), _p(q_out), _p(kv_cache_base), _p(page_list), _p(sequence_lengths),
-                                       _is_bf16(qkv), B, head_num, Hkv, D, page_list.shape[-1], T, rope_base, _stream()),
-          "b200_rope_append")
+        q_out = torch.empty((rows, head_num * D), dtype=qkv.dtype, device=qkv.device)
+    lib = _lib.load()
+    if q_len == 1:
+        check(lib.b200_rope_append(_p(qkv), _p(q_out), _p(kv_cache_base), _p(page_list), _p(sequence_lengths),
+                                   _is_bf16(qkv), rows, head_num, Hkv, D, page_list.shape[-1], T, rope_base, _stream()),
+              "b200_rope_append")
+    else:
+        check(lib.b200_rope_append_multi(_p(qkv), _p(q_out), _p(kv_cache_base), _p(page_list), _p(sequence_lengths),
+                                         _is_bf16(qkv), rows // q_len, head_num, Hkv, D, page_list.shape[-1], T, rope_base, q_len,
+                                         _stream()), "b200_rope_append_multi")
     return q_out
 
 
@@ -431,6 +441,42 @@ def sample(logits: torch.Tensor, top_k: torch.Tensor, top_p: torch.Tensor, unifo
                                   _p(count_ws), _p(temperature), _p(repetition), _p(presence), _p(frequency), _p(top_k), _p(top_p),
                                   _p(uniform), _p(process), _p(tok), _p(tprob), _p(probs), _stream()), "b200_sample")
     return tok, tprob, probs
+
+
+def spec_verify(draft_tokens: torch.Tensor, *, target_probs: Optional[torch.Tensor] = None,
+                target_ids: Optional[torch.Tensor] = None, draft_probs: Optional[torch.Tensor] = None,
+                uniform: Optional[torch.Tensor] = None, out_tokens: Optional[torch.Tensor] = None,
+                accepted: Optional[torch.Tensor] = None):
+    """Verify n = draft_tokens.shape[1] speculative tokens per sequence (b200_spec_verify). Greedy: target_ids int32 [B, n+1]
+    (argmax of the step's rows). Sampling: target_probs fp32 [B, n+1, V], optional draft_probs fp32 [B, n, V] (None =
+    deterministic drafts), uniform fp32 [B, n+1]. Returns (out_tokens int32 [B, n+1]: accepted drafts, then one correction or
+    bonus token, then -1; accepted int32 [B])."""
+    _cuda_contig(draft_tokens, target_probs, target_ids, draft_probs, uniform, out_tokens, accepted)
+    B, n = draft_tokens.shape
+    if target_probs is None and target_ids is None:
+        raise B200Error("spec_verify: pass target_probs (sampling) or target_ids (greedy)")
+    if target_probs is not None:
+        if target_probs.dtype != torch.float32 or target_probs.dim() != 3 or tuple(target_probs.shape[:2]) != (B, n + 1):
+            raise B200Error(f"spec_verify: target_probs must be fp32 [{B}, {n + 1}, V]")
+        V = target_probs.shape[2]
+        if uniform is None or uniform.dtype != torch.float32 or uniform.numel() != B * (n + 1):
+            raise B200Error(f"spec_verify: sampling mode needs uniform fp32 [{B}, {n + 1}]")
+        if draft_probs is not None and (draft_probs.dtype != torch.float32 or tuple(draft_probs.shape) != (B, n, V)):
+            raise B200Error(f"spec_verify: draft_probs must be fp32 [{B}, {n}, {V}]")
+    else:
+        if target_ids.dtype != torch.int32 or tuple(target_ids.shape) != (B, n + 1):
+            raise B200Error(f"spec_verify: target_ids must be int32 [{B}, {n + 1}]")
+        V = 1                                   # the vocabulary is not read in greedy mode
+    if draft_tokens.dtype != torch.int32:
+        raise B200Error("spec_verify: draft_tokens must be int32")
+    dev = draft_tokens.device
+    if out_tokens is None:
+        out_tokens = torch.empty((B, n + 1), dtype=torch.int32, device=dev)
+    if accepted is None:
+        accepted = torch.empty(B, dtype=torch.int32, device=dev)
+    check(_lib.load().b200_spec_verify(_p(target_probs), _p(target_ids), _p(draft_probs), _p(draft_tokens), _p(uniform), B, n, V,
+                                       _p(out_tokens), _p(accepted), _stream()), "b200_spec_verify")
+    return out_tokens, accepted
 
 
 # ------------------------------------------------------------------------------------------------ decode programs

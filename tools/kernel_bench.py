@@ -70,6 +70,25 @@ def bench_attn(B, Hq, Hkv, S, T=64, nrot=3, env=None):
     return us
 
 
+def bench_attn_multi(B, Hq, Hkv, S, q_len, T=64, nrot=3):
+    """b200_paged_decode_attn_multi with q_len query tokens per sequence (group * q_len query rows per kv head); the K/V bytes
+    are those of plain decode, 2*B*S*Hkv*D*2 with S the cached length the last query sees."""
+    M = math.ceil(S / T)
+    P = B * M + 1
+    pools = [torch.randn(P, 2, Hkv, T, 128, device=dev).half() for _ in range(nrot)]
+    q = torch.randn(B, q_len, Hq, 128, device=dev).half()
+    bid = (torch.randperm(P - 1, device=dev).to(torch.int32) + 1).reshape(B, M)
+    pl = ops.convert_block_table(bid)
+    seq = torch.full((B,), S - q_len, dtype=torch.int32, device=dev)
+    ws = ops.attn_workspace(B * q_len, Hq, Hkv, S, dev)
+    out = torch.empty(B, q_len, Hq * 128, device=dev).half()
+    us = timeit(lambda i: ops.paged_decode_attn_multi(q, pools[i], pl, seq, S, ws, out=out), nrot)
+    byt = 2 * B * S * Hkv * 128 * 2
+    print(f"attn-multi B{B} Hq{Hq} Hkv{Hkv} S{S} q_len {q_len} (rows {Hq // Hkv * q_len}): {us:8.1f} us  {byt / us / 1e3:7.0f} GB/s  "
+          f"frac={byt / us / 1e3 / PEAK:.3f}", flush=True)
+    return us
+
+
 def bench_permute(B, K, nrot=4):
     """b200_permute_cols on [B, K] fp16; bytes = the row read and written, plus the perm."""
     xs = [torch.randn(B, K, device=dev).half() for _ in range(nrot)]
@@ -154,6 +173,10 @@ if __name__ == "__main__":
         bench_attn(1, 32, 8, 4096)
         bench_attn(64, 32, 8, 4096)
         bench_attn(16, 8, 1, 8192)
+    if "attn-multi" in which:
+        # speculative-token verification at group 8 (Qwen2-72B / Llama-3-70B): 8, 16, 32, 64 query rows per kv head
+        t = {n: bench_attn_multi(32, 64, 8, 2048, n) for n in (1, 2, 4, 8)}
+        print("attn-multi time relative to q_len 2 (16 rows): " + ", ".join(f"q_len {n}: {t[n] / t[2]:.2f}x" for n in t), flush=True)
     if "gemm" in which:
         for B in (32,):
             bench_gemm(B200_FMT_INT4, B, 4096, 6144)
