@@ -211,6 +211,17 @@ int b200_rope_append_ex(const void* qkv, const void* qkv_bias, void* q_out, void
                         const int32_t* sequence_lengths, const int32_t* position_ids, const float* cos_sin_cache,
                         int cache_positions, const b200_rope_config* cfg, int use_logn_attn, int is_bf16, int batch, int head_num,
                         int kv_head_num, int head_dim, int max_blocks_per_seq, int page_size, void* stream);
+/* b200_rope_append_ex for q_len new tokens per sequence (verification of speculative tokens), with the same per-row rules:
+ * row x of qkv [batch*q_len][...] is token j = x % q_len of sequence b = x / q_len; its K/V go to slot sequence_lengths[b] + j,
+ * and it is rotated at position_ids[x] (position_ids [batch*q_len]) when that entry is > 0, else at that slot. Dynamic-NTK
+ * seq_len, the logn factor and the cos_sin_cache bound are taken per row from that position, so token j has the bits of a
+ * one-token b200_rope_append_ex at sequence_lengths + j. q_out [batch*q_len][Hq*D] is the q [batch][q_len][Hq][D] of
+ * b200_paged_decode_attn_multi. q_len == 1 is b200_rope_append_ex. Inside a decode program it is its own launch. */
+int b200_rope_append_ex_multi(const void* qkv, const void* qkv_bias, void* q_out, void* kv_pool, const int32_t* page_list,
+                              const int32_t* sequence_lengths, const int32_t* position_ids, const float* cos_sin_cache,
+                              int cache_positions, const b200_rope_config* cfg, int use_logn_attn, int is_bf16, int batch,
+                              int head_num, int kv_head_num, int head_dim, int max_blocks_per_seq, int page_size, int q_len,
+                              void* stream);
 /* embedding gather out[b] = table[ids[b]] (rtp_ops.embedding). */
 int b200_embedding(const int32_t* ids, const void* table, void* out, int is_bf16, int rows, int hidden, void* stream);
 /* greedy sampling: out[r] = argmax(logits[r]) (lowest index on ties; CudaSampleOp.cc:330,453). dtype: 0 fp16, 1 bf16, 2 fp32 */

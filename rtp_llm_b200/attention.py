@@ -10,8 +10,10 @@
 Inside the reference tree the impl is appended to DECODE_MHA_IMPS (attention/__init__.py:91-100); see INTEGRATION.md.
 Config / input objects are duck-typed: any object with the reference's attribute names works (AttentionConfigs:
 head_num, kv_head_num, size_per_head, kernel_tokens_per_block|tokens_per_block, max_seq_len, need_rope_kv_cache,
-rope_config.base, q_scaling; PyAttentionInputs: sequence_lengths, kv_cache_kernel_block_id_device, is_prefill, and
-input_lengths for a verification step of speculative tokens, which runs q_len = max(input_lengths) tokens per sequence).
+rope_config (style, dim, base, scale, factor1, factor2, max_pos, extrapolation_factor, mscale, is_neox_style; see rope.py),
+use_logn_attn, q_scaling; PyAttentionInputs: sequence_lengths, kv_cache_kernel_block_id_device, is_prefill, combo_position_ids
+when the rotation positions are not the cache slots, and input_lengths for a verification step of speculative tokens, which
+runs q_len = max(input_lengths) tokens per sequence).
 """
 from __future__ import annotations
 
@@ -20,7 +22,7 @@ from typing import Optional
 
 import torch
 
-from . import ops
+from . import ops, rope
 from ._lib import B200Error
 
 try:  # inside the reference tree the real base class is used; standalone, a structural stand-in
@@ -128,20 +130,36 @@ class B200DecodeAttnOp:
                                      q_scale=q_scale)
 
 
+def _position_ids(attn_inputs) -> Optional[torch.Tensor]:
+    """combo_position_ids of the inputs when present and non-empty: one rotation position per qkv row (entries <= 0 keep the
+    cache slot)."""
+    pid = getattr(attn_inputs, "combo_position_ids", None)
+    return pid if torch.is_tensor(pid) and pid.numel() > 0 else None
+
+
 class B200RopeKVCacheDecodeOp:
-    """== FusedRopeKVCacheDecodeOp (rtp_llm/ops/fused_rope_kvcache_op.py:176-272), RopeStyle::Base / NeoX pairing."""
+    """== FusedRopeKVCacheDecodeOp (rtp_llm/ops/fused_rope_kvcache_op.py:176-272): the rope config's style, rotary dim,
+    scaling, Yarn / Llama3 factors, logn attention (attn_configs.use_logn_attn) and position ids, NeoX pairing; see rope.py
+    for which kernel serves which config."""
 
     def __init__(self, attn_configs):
         self.cfg = attn_configs
+        self.spec = rope.spec_of(getattr(attn_configs, "rope_config", None), int(attn_configs.size_per_head))
+        self.use_logn_attn = bool(getattr(attn_configs, "use_logn_attn", False))
+
+    def supported(self) -> bool:
+        return rope.supported(self.spec, int(self.cfg.size_per_head))
 
     def prepare(self, attn_inputs):
         return attn_inputs
 
-    def forward(self, qkv: torch.Tensor, kv_cache, page_list: torch.Tensor, sequence_lengths: torch.Tensor, q_len: int = 1):
+    def forward(self, qkv: torch.Tensor, kv_cache, page_list: torch.Tensor, sequence_lengths: torch.Tensor, q_len: int = 1,
+                position_ids: Optional[torch.Tensor] = None):
         base = kv_cache.kv_cache_base if hasattr(kv_cache, "kv_cache_base") else kv_cache
-        rope = getattr(self.cfg, "rope_config", None)
-        rope_base = float(getattr(rope, "base", 10000.0)) if rope is not None else 10000.0
-        return ops.rope_append(qkv, base, page_list, sequence_lengths, self.cfg.head_num, rope_base, q_len=q_len)
+        if position_ids is not None and (position_ids.device != qkv.device or position_ids.dtype != torch.int32):
+            position_ids = position_ids.to(device=qkv.device, dtype=torch.int32)
+        return rope.rope_append(self.spec, qkv, base, page_list, sequence_lengths, self.cfg.head_num, q_len=q_len,
+                                use_logn_attn=self.use_logn_attn, position_ids=position_ids)
 
 
 class B200DecodeImpl(FMHAImplBase):
@@ -155,9 +173,15 @@ class B200DecodeImpl(FMHAImplBase):
         self.attn_inputs = attn_inputs
         self.fmha_params = self.fmha_impl.prepare(attn_inputs)
         self._captured_seq_lens = attn_inputs.sequence_lengths
+        if self.need_rope_kv_cache:     # the cos/sin table is uploaded here, never inside a graph capture
+            rope.table(self.rope_kvcache_impl.spec, attn_inputs.kv_cache_kernel_block_id_device.device)
 
     @staticmethod
     def support(attn_configs, attn_inputs) -> bool:
+        """The attention shape is served, and so is the rope config when this impl applies it (an unserved rope style,
+        non-NeoX pairing or an odd / oversized rotary dim falls through to another impl)."""
+        if bool(getattr(attn_configs, "need_rope_kv_cache", True)) and not B200RopeKVCacheDecodeOp(attn_configs).supported():
+            return False
         return B200DecodeAttnOp(attn_configs).support(attn_inputs)
 
     def forward(self, qkv: torch.Tensor, kv_cache, layer_idx: int = 0) -> torch.Tensor:
@@ -167,13 +191,16 @@ class B200DecodeImpl(FMHAImplBase):
             raise B200Error(f"qkv has {qkv.shape[0]} rows, expected batch {self.fmha_params.batch_size} x q_len {q_len}")
         if self.need_rope_kv_cache:
             q = self.rope_kvcache_impl.forward(qkv, kv_cache, self.fmha_params.kv_cache_offset,
-                                               self.fmha_params.sequence_lengths, q_len)
+                                               self.fmha_params.sequence_lengths, q_len, _position_ids(self.attn_inputs))
         else:
             q = qkv
         return self.fmha_impl.forward(q, kv_cache, self.fmha_params)
 
     def prepare_cuda_graph(self, attn_inputs) -> None:
-        """Refresh per-step metadata IN PLACE (attention/common.py:88-138): page list and sequence lengths."""
+        """Refresh per-step metadata IN PLACE (attention/common.py:88-138): page list, sequence lengths and position ids."""
         self.fmha_impl.update_kv_cache_offset(self.fmha_params.kv_cache_offset, attn_inputs.kv_cache_kernel_block_id_device)
         if attn_inputs.sequence_lengths is not self._captured_seq_lens:
             self._captured_seq_lens.copy_(attn_inputs.sequence_lengths, non_blocking=True)
+        pid, captured = _position_ids(attn_inputs), _position_ids(self.attn_inputs)
+        if pid is not None and captured is not None and pid is not captured:
+            captured.copy_(pid, non_blocking=True)

@@ -322,7 +322,12 @@ __device__ __forceinline__ float2 rope_coef(const RopeCfg& c, int zid, int pos) 
     return make_float2(sc * cs, sc * sn);
 }
 
-template <typename T>
+// q_len new tokens per sequence (MULTI, verification of speculative tokens): grid (B, Hq + 2*Hkv, q_len); row
+// x = b * q_len + j of qkv / q_out / position_ids is token j = blockIdx.z of sequence b, appended at slot seq_lens[b] + j and
+// rotated at position_ids[x] (when > 0) or that slot. q_len rides in gridDim.z so both instances share one parameter block.
+// Everything after the row / slot / position choice is the one-token arithmetic: token j gives the bits of a one-token call at
+// seq_lens + j.
+template <typename T, bool MULTI = false>
 __global__ void rope_append_ex_kernel(const T* __restrict__ qkv, const T* __restrict__ bias, T* __restrict__ q_out,
                                       T* __restrict__ kv_pool, const int32_t* __restrict__ page_list,
                                       const int32_t* __restrict__ seq_lens, const int32_t* __restrict__ position_ids,
@@ -331,15 +336,16 @@ __global__ void rope_append_ex_kernel(const T* __restrict__ qkv, const T* __rest
     pdl_launch_dependents();
     pdl_wait();
     const int b = blockIdx.x, h = blockIdx.y, i = threadIdx.x, half = head_dim / 2, rhalf = cfg.dim / 2;
-    const int slot = seq_lens[b];                                  // where K/V of the new token go (tokens already cached)
-    const int pos = (position_ids && position_ids[b] > 0) ? position_ids[b] : slot;
-    const T* src = qkv + ((size_t)b * (head_num + 2 * kv_head_num) + h) * head_dim;
+    const int x = MULTI ? b * (int)gridDim.z + (int)blockIdx.z : b;
+    const int slot = seq_lens[b] + (MULTI ? (int)blockIdx.z : 0);  // where K/V of the new token go (tokens already cached)
+    const int pos = (position_ids && position_ids[x] > 0) ? position_ids[x] : slot;
+    const T* src = qkv + ((size_t)x * (head_num + 2 * kv_head_num) + h) * head_dim;
     const T* bsrc = bias ? bias + (size_t)h * head_dim : nullptr;
     const size_t page_elems = (size_t)kv_head_num * tokens_per_block * head_dim;
     T* dst;
     bool rotate = cfg.style != 0, is_q = h < head_num;
     if (is_q) {
-        dst = q_out + ((size_t)b * head_num + h) * head_dim;
+        dst = q_out + ((size_t)x * head_num + h) * head_dim;
     } else {
         const bool is_v = h >= head_num + kv_head_num;
         const int kvh = is_v ? h - head_num - kv_head_num : h - head_num;

@@ -882,10 +882,11 @@ int b200_rope_append_multi(const void* qkv, void* q_out, void* kv_pool, const in
                             max_blocks_per_seq, page_size, rope_base, stream);
 }
 
-int b200_rope_append_ex(const void* qkv, const void* qkv_bias, void* q_out, void* kv_pool, const int32_t* page_list,
-                        const int32_t* sequence_lengths, const int32_t* position_ids, const float* cos_sin_cache,
-                        int cache_positions, const b200_rope_config* cfg, int use_logn_attn, int is_bf16, int batch, int head_num,
-                        int kv_head_num, int head_dim, int max_blocks_per_seq, int page_size, void* stream) {
+static int rope_append_ex_impl(const void* qkv, const void* qkv_bias, void* q_out, void* kv_pool, const int32_t* page_list,
+                               const int32_t* sequence_lengths, const int32_t* position_ids, const float* cos_sin_cache,
+                               int cache_positions, const b200_rope_config* cfg, int use_logn_attn, int is_bf16, int batch,
+                               int q_len, int head_num, int kv_head_num, int head_dim, int max_blocks_per_seq, int page_size,
+                               void* stream) {
     if (batch == 0) return B200_OK;
     ARG_CHECK(qkv && q_out && kv_pool && page_list && sequence_lengths && cfg, "rope_append_ex: null pointer");
     ARG_CHECK(head_dim > 0 && head_dim % 2 == 0 && head_dim <= 512, "rope_append_ex: head_dim %d unsupported", head_dim);
@@ -894,24 +895,46 @@ int b200_rope_append_ex(const void* qkv, const void* qkv_bias, void* q_out, void
     ARG_CHECK(cfg->style == 0 || cfg->base > 1.f, "rope_append_ex: rope base must be > 1");
     ARG_CHECK(!cos_sin_cache || cache_positions > 0, "rope_append_ex: a cos/sin cache needs its number of positions");
     ARG_CHECK(!use_logn_attn || cfg->max_pos > 1, "rope_append_ex: logn attention needs max_pos > 1");
+    ARG_CHECK(batch > 0 && q_len >= 1 && q_len <= 65535, "rope_append_ex: bad shape batch %d x q_len %d", batch, q_len);
     const b200_rope_config cc = *cfg;
     if (g_rec)
         return rec_call([=](void* st) {
-            return b200_rope_append_ex(qkv, qkv_bias, q_out, kv_pool, page_list, sequence_lengths, position_ids, cos_sin_cache,
-                                       cache_positions, &cc, use_logn_attn, is_bf16, batch, head_num, kv_head_num, head_dim,
+            return rope_append_ex_impl(qkv, qkv_bias, q_out, kv_pool, page_list, sequence_lengths, position_ids, cos_sin_cache,
+                                       cache_positions, &cc, use_logn_attn, is_bf16, batch, q_len, head_num, kv_head_num, head_dim,
                                        max_blocks_per_seq, page_size, st);
         });
     RopeCfg rc{cc.style, cc.dim, cc.base, cc.scale, cc.factor1, cc.factor2, cc.max_pos, cc.extrapolation_factor, cc.mscale};
-    const dim3 grid(batch, head_num + 2 * kv_head_num);
+    const dim3 grid(batch, head_num + 2 * kv_head_num, q_len);
     const bool pdl = g_pdl.load() != 0;
     const float2* cache = reinterpret_cast<const float2*>(cos_sin_cache);
     return by_dtype(is_bf16, [&](auto t) {
         using T = decltype(t);
-        CUDA_CHECK(launch_ex(rope_append_ex_kernel<T>, {grid, dim3(head_dim / 2), 0, (cudaStream_t)stream, pdl}, (const T*)qkv,
+        CUDA_CHECK(launch_ex(q_len > 1 ? rope_append_ex_kernel<T, true> : rope_append_ex_kernel<T, false>,
+                             {grid, dim3(head_dim / 2), 0, (cudaStream_t)stream, pdl}, (const T*)qkv,
                              (const T*)qkv_bias, (T*)q_out, (T*)kv_pool, page_list, sequence_lengths, position_ids, cache,
                              cache_positions, rc, use_logn_attn, head_num, kv_head_num, head_dim, max_blocks_per_seq, page_size));
         return launched("rope_append_ex_kernel");
     });
+}
+
+int b200_rope_append_ex(const void* qkv, const void* qkv_bias, void* q_out, void* kv_pool, const int32_t* page_list,
+                        const int32_t* sequence_lengths, const int32_t* position_ids, const float* cos_sin_cache,
+                        int cache_positions, const b200_rope_config* cfg, int use_logn_attn, int is_bf16, int batch, int head_num,
+                        int kv_head_num, int head_dim, int max_blocks_per_seq, int page_size, void* stream) {
+    return rope_append_ex_impl(qkv, qkv_bias, q_out, kv_pool, page_list, sequence_lengths, position_ids, cos_sin_cache,
+                               cache_positions, cfg, use_logn_attn, is_bf16, batch, 1, head_num, kv_head_num, head_dim,
+                               max_blocks_per_seq, page_size, stream);
+}
+
+int b200_rope_append_ex_multi(const void* qkv, const void* qkv_bias, void* q_out, void* kv_pool, const int32_t* page_list,
+                              const int32_t* sequence_lengths, const int32_t* position_ids, const float* cos_sin_cache,
+                              int cache_positions, const b200_rope_config* cfg, int use_logn_attn, int is_bf16, int batch,
+                              int head_num, int kv_head_num, int head_dim, int max_blocks_per_seq, int page_size, int q_len,
+                              void* stream) {
+    ARG_CHECK(q_len >= 1, "rope_append_ex_multi: q_len %d must be >= 1", q_len);
+    return rope_append_ex_impl(qkv, qkv_bias, q_out, kv_pool, page_list, sequence_lengths, position_ids, cos_sin_cache,
+                               cache_positions, cfg, use_logn_attn, is_bf16, batch, q_len, head_num, kv_head_num, head_dim,
+                               max_blocks_per_seq, page_size, stream);
 }
 
 int b200_embedding(const int32_t* ids, const void* table, void* out, int is_bf16, int rows, int hidden, void* stream) {

@@ -14,6 +14,10 @@
 #include <cuda_runtime.h>
 #include <torch/extension.h>
 
+#include <algorithm>
+#include <cmath>
+#include <map>
+#include <mutex>
 #include <optional>
 #include <stdexcept>
 #include <string>
@@ -35,8 +39,19 @@ static void check_rc(int rc, const char* what) {
 static void* cur_stream() { return at::cuda::getCurrentCUDAStream(at::cuda::current_device()).stream(); }
 
 // ---- standalone mirrors of the reference types (member names as in the reference)
+// The RopeConfig fields the decode rope reads (cpp/model_utils/RopeConfig.h:21-42). The defaults are plain Base at base 10000
+// over the whole head (dim 0 = size_per_head), which is what this seam computed before it read anything but `base`.
 struct RopeConfig {
+    int style = 1;   // RopeStyle: 0 No, 1 Base, 2 Glm2, 3 DynamicNTK, 4 QwenDynamicNTK, 5 Yarn, 6 Llama3, 7 Mrope
+    int dim = 0;
     double base = 10000.0;
+    double scale = 1.0;
+    double factor1 = 0.0;
+    double factor2 = 0.0;
+    int max_pos = 0;
+    double extrapolation_factor = 1.0;
+    double mscale = 1.0;
+    bool is_neox_style = true;
 };
 struct AttentionConfigs {
     size_t head_num = 0;
@@ -47,6 +62,7 @@ struct AttentionConfigs {
     size_t kernel_tokens_per_block = 0;
     float q_scaling = 1.0f;
     bool need_rope_kv_cache = true;
+    bool use_logn_attn = false;
     bool kv_cache_fp8 = false;   // KvCacheDataType::FP8 in the reference
     size_t max_seq_len = 32768;
 };
@@ -54,6 +70,8 @@ struct PyAttentionInputs {
     bool is_prefill = false;
     torch::Tensor sequence_lengths;                 // [B] int32, tokens already cached; CUDA or pinned host
     torch::Tensor kv_cache_kernel_block_id_device;  // [B, M] int32
+    torch::Tensor input_lengths;                    // [B]: a verification step runs q_len = max(input_lengths) tokens per sequence
+    torch::Tensor combo_position_ids;               // [B * q_len] int32 rotation positions (entries <= 0 keep the cache slot)
 };
 struct LayerKVCache {
     torch::Tensor kv_cache_base;  // [P, 2, Hkv, T, D]
@@ -68,14 +86,91 @@ using ParamsBasePtr = std::shared_ptr<ParamsBase>;
 struct B200AttnParams: public ParamsBase {
     size_t batch_size = 0;
     size_t max_seq_len = 0;
+    size_t q_len = 1;                // query tokens per sequence (> 1: verification of speculative tokens)
     torch::Tensor kv_cache_offset;   // [B, 1, 2, M] int32
     torch::Tensor sequence_lengths;  // shares storage with the engine's tensor so graph replay can refresh it in place
+    torch::Tensor position_ids;      // the inputs' combo_position_ids (undefined when absent)
     torch::Tensor workspace;
 };
 using B200AttnParamsPtr = std::shared_ptr<B200AttnParams>;
 
 static size_t page_size_of(const AttentionConfigs& c) {
     return c.kernel_tokens_per_block ? c.kernel_tokens_per_block : c.tokens_per_block;
+}
+
+// == attention._q_len: max(input_lengths) when the inputs carry them, else 1
+static size_t q_len_of(const PyAttentionInputs& in) {
+    if (!in.input_lengths.defined() || in.input_lengths.numel() == 0) return 1;
+    return (size_t)std::max<int64_t>(in.input_lengths.max().item<int64_t>(), 1);
+}
+
+static torch::Tensor position_ids_of(const PyAttentionInputs& in) {
+    return in.combo_position_ids.defined() && in.combo_position_ids.numel() > 0 ? in.combo_position_ids : torch::Tensor();
+}
+
+// ---- the rope config, decided as rtp_llm_b200/rope.py decides it (the two seams serve the same configs with the same bits)
+static int rotary_dim(const AttentionConfigs& c) { return c.rope_config.dim ? c.rope_config.dim : (int)c.size_per_head; }
+
+static bool rope_supported(const AttentionConfigs& c) {
+    const RopeConfig& r = c.rope_config;
+    const int s = r.style, dim = rotary_dim(c);
+    const bool served = s == 0 || s == 1 || s == 3 || s == 4 || s == 5 || s == 6;   // not Glm2 (2), Mrope (7) or unknown styles
+    return served && r.is_neox_style && dim % 2 == 0 && dim > 0 && dim <= (int)c.size_per_head && (s == 0 || r.base > 1.0);
+}
+
+// Base over the whole head at scale 1 without logn or position ids: b200_rope_append(_multi), the bits of a base-only config
+static bool rope_is_plain_base(const AttentionConfigs& c, bool has_position_ids) {
+    const RopeConfig& r = c.rope_config;
+    return r.style == 1 && r.scale == 1.0 && rotary_dim(c) == (int)c.size_per_head && r.is_neox_style && !c.use_logn_attn &&
+           !has_position_ids;
+}
+
+// rope.build_table: the fp32 [int(max_pos * scale)][dim] interleaved (cos, sin) table of RopeCache.cc:16-85 for Base and Yarn,
+// with the same ATen calls as the Python builder (so the same bits); undefined for other styles or an empty range.
+static torch::Tensor build_rope_table(const RopeConfig& r, int dim) {
+    const int64_t positions = (int64_t)(r.max_pos * r.scale);
+    if ((r.style != 1 && r.style != 5) || positions <= 0) return torch::Tensor();
+    const auto f32 = torch::kFloat;
+    const torch::Tensor exps = torch::arange(0, dim, 2).to(f32) / dim;
+    torch::Tensor freqs, cos, sin;
+    if (r.style == 1) {
+        const torch::Tensor inv_freq = torch::reciprocal(torch::pow(torch::scalar_tensor(r.base, f32), exps)) * 1.0;
+        torch::Tensor t = torch::arange(positions).to(f32);
+        t.div_(r.scale);
+        freqs = torch::outer(t, inv_freq);
+        cos = freqs.cos();
+        sin = freqs.sin();
+    } else {
+        const torch::Tensor pos_freqs = torch::pow(torch::scalar_tensor(r.base, f32), exps);
+        const torch::Tensor inv_e = torch::reciprocal(pos_freqs) * 1.0, inv_i = torch::reciprocal(pos_freqs * r.scale) * 1.0;
+        auto corr = [&](double nrot) { return (double)dim * std::log(r.max_pos / (nrot * 2.0 * M_PI)) / (2.0 * std::log(r.base)); };
+        const double low = (double)std::max(0, (int)std::floor(corr(r.factor1)));
+        double high = (double)std::min(dim - 1, (int)std::ceil(corr(r.factor2)));
+        if (std::abs(low - high) < 1e-6) high += 0.001;
+        const torch::Tensor ramp = torch::clamp((torch::arange(dim / 2).to(f32) - low) / (high - low), 0, 1);
+        const torch::Tensor mask = torch::rsub(ramp, 1.0) * r.extrapolation_factor;
+        const torch::Tensor inv_freq = inv_i * torch::rsub(mask, 1.0) + inv_e * mask;
+        freqs = torch::outer(torch::arange(positions).to(f32), inv_freq);
+        cos = freqs.cos() * r.mscale;
+        sin = freqs.sin() * r.mscale;
+    }
+    return torch::stack({cos, sin}, -1).reshape({positions, -1}).contiguous();
+}
+
+// rope.table: built and uploaded once per (config, device)
+static torch::Tensor rope_table(const RopeConfig& r, int dim, const torch::Device& device) {
+    static std::mutex mu;
+    static std::map<std::string, torch::Tensor> tables;
+    char key[256];
+    snprintf(key, sizeof(key), "%d %d %a %a %a %a %d %a %a %s", r.style, dim, r.base, r.scale, r.factor1, r.factor2, r.max_pos,
+             r.extrapolation_factor, r.mscale, device.str().c_str());
+    std::lock_guard<std::mutex> lock(mu);
+    auto it = tables.find(key);
+    if (it == tables.end()) {
+        torch::Tensor t = build_rope_table(r, dim);
+        it = tables.emplace(key, t.defined() ? t.to(device) : t).first;
+    }
+    return it->second;
 }
 
 static void update_offset_tensor(const torch::Tensor& kv_cache_offset, const torch::Tensor& block_ids) {
@@ -95,11 +190,16 @@ class B200AttnOp {
 public:
     explicit B200AttnOp(const AttentionConfigs& attn_configs): attn_configs_(attn_configs) {}
 
+    // group * q_len <= 64 query rows per (sequence, kv head); when this seam applies the rope, the rope config must be served
+    // (attention.B200DecodeImpl.support applies the same rule), so an engine falls through to another op instead
     bool support(PyAttentionInputs attn_inputs) {
         const auto& c = attn_configs_;
         if (attn_inputs.is_prefill || c.kv_cache_fp8 || c.kv_head_num == 0 || c.head_num % c.kv_head_num) return false;
+        if (c.need_rope_kv_cache && !rope_supported(c)) return false;
         const size_t group = c.head_num / c.kv_head_num, T = page_size_of(c);
-        if ((c.size_per_head != 64 && c.size_per_head != 128 && c.size_per_head != 256) || group < 1 || group > 16) return false;
+        if ((c.size_per_head != 64 && c.size_per_head != 128 && c.size_per_head != 256) || group < 1 ||
+            group * q_len_of(attn_inputs) > 64)
+            return false;
         if (!(T == 16 || T == 32 || T == 64 || T == 128)) return false;
         return b200_device_check(at::cuda::current_device()) == 0;
     }
@@ -113,12 +213,17 @@ public:
         params->kv_cache_offset = torch::empty({batch, 1, 2, block_ids.size(1)}, block_ids.options());
         update_offset_tensor(params->kv_cache_offset, block_ids);
         params->batch_size = (size_t)batch;
-        const size_t cap = (size_t)block_ids.size(1) * page_size_of(attn_configs_);
-        params->max_seq_len = attn_configs_.max_seq_len + 1 < cap ? attn_configs_.max_seq_len + 1 : cap;   // XQAAttnOp.cc:147-149 passes max_seq_len + 1
+        params->q_len = q_len_of(attn_inputs);
+        // XQAAttnOp.cc:147-149 passes max_seq_len + 1; with q_len tokens per sequence the bound is max_seq_len + q_len
+        const size_t cap = (size_t)block_ids.size(1) * page_size_of(attn_configs_), want = attn_configs_.max_seq_len + params->q_len;
+        params->max_seq_len = want < cap ? want : cap;
         params->sequence_lengths = attn_inputs.sequence_lengths;
-        const size_t ws = b200_paged_decode_attn_workspace_bytes(params->batch_size, attn_configs_.head_num,
+        params->position_ids = position_ids_of(attn_inputs);
+        const size_t ws = b200_paged_decode_attn_workspace_bytes(params->batch_size * params->q_len, attn_configs_.head_num,
                                                                  attn_configs_.kv_head_num, params->max_seq_len);
         params->workspace = torch::zeros({(int64_t)(ws ? ws : 256)}, torch::TensorOptions().dtype(torch::kUInt8).device(block_ids.device()));
+        if (attn_configs_.need_rope_kv_cache)   // the cos/sin table is uploaded here, never inside a graph capture
+            rope_table(attn_configs_.rope_config, rotary_dim(attn_configs_), block_ids.device());
         return params;
     }
 
@@ -127,6 +232,7 @@ public:
         update_offset_tensor(params->kv_cache_offset, attn_inputs.kv_cache_kernel_block_id_device);
         params->batch_size = (size_t)attn_inputs.kv_cache_kernel_block_id_device.size(0);
         params->sequence_lengths = attn_inputs.sequence_lengths;
+        params->position_ids = position_ids_of(attn_inputs);
     }
 
     void updateKvCacheOffset(const torch::Tensor& kv_cache_offset, const torch::Tensor& kv_cache_block_id_device) {
@@ -137,15 +243,26 @@ public:
         B200_CHECK(kv_cache.has_value(), "decode should have kv cache.");
         B200_CHECK(params != nullptr, "B200AttnOp::forward received null params");
         const auto& c = attn_configs_;
-        const int64_t batch = input.size(0);
-        torch::Tensor out = torch::empty({batch, (int64_t)(c.head_num * c.size_per_head)}, input.options());
+        const int64_t rows = input.size(0);
+        torch::Tensor out = torch::empty({rows, (int64_t)(c.head_num * c.size_per_head)}, input.options());
         const auto& pool = kv_cache->kv_cache_base;
-        check_rc(b200_paged_decode_attn(input.data_ptr(), input.scalar_type() == torch::kBFloat16, out.data_ptr(), c.head_num,
-                                        c.kv_head_num, c.size_per_head, params->batch_size,
-                                        (size_t)params->kv_cache_offset.size(3), params->max_seq_len, page_size_of(c), pool.data_ptr(),
-                                        params->kv_cache_offset.data_ptr<int>(),
-                                        reinterpret_cast<const uint32_t*>(params->sequence_lengths.data_ptr()), 1.0f / c.q_scaling,
-                                        params->workspace.data_ptr(), (size_t)params->workspace.numel(), cur_stream()),
+        const int is_bf16 = input.scalar_type() == torch::kBFloat16;
+        const auto* seq = reinterpret_cast<const uint32_t*>(params->sequence_lengths.data_ptr());
+        if (params->q_len > 1) {   // input [B*q_len, Hq*D] token-major == q [B][q_len][Hq][D]; out [B*q_len, Hq*D]
+            B200_CHECK(rows == (int64_t)(params->batch_size * params->q_len), "B200AttnOp: input rows must be batch x q_len");
+            check_rc(b200_paged_decode_attn_multi(input.data_ptr(), is_bf16, out.data_ptr(), c.head_num, c.kv_head_num, c.size_per_head,
+                                                  params->batch_size, params->q_len, (size_t)params->kv_cache_offset.size(3),
+                                                  params->max_seq_len, page_size_of(c), pool.data_ptr(),
+                                                  params->kv_cache_offset.data_ptr<int>(), seq, 1.0f / c.q_scaling,
+                                                  params->workspace.data_ptr(), (size_t)params->workspace.numel(), cur_stream()),
+                     "b200_paged_decode_attn_multi");
+            return out;
+        }
+        check_rc(b200_paged_decode_attn(input.data_ptr(), is_bf16, out.data_ptr(), c.head_num, c.kv_head_num, c.size_per_head,
+                                        params->batch_size, (size_t)params->kv_cache_offset.size(3), params->max_seq_len,
+                                        page_size_of(c), pool.data_ptr(), params->kv_cache_offset.data_ptr<int>(), seq,
+                                        1.0f / c.q_scaling, params->workspace.data_ptr(), (size_t)params->workspace.numel(),
+                                        cur_stream()),
                  "b200_paged_decode_attn");
         return out;
     }
@@ -154,16 +271,55 @@ private:
     AttentionConfigs attn_configs_;
 };
 
-// rope + append: FusedRopeKVCacheDecodeOp.forward (rtp_llm/ops/fused_rope_kvcache_op.py:202-246)
+// rope + append: FusedRopeKVCacheDecodeOp.forward (rtp_llm/ops/fused_rope_kvcache_op.py:202-246). qkv [B*q_len, (Hq+2Hkv)*D]
+// token-major, q_len from the params; returns q [B*q_len, Hq*D]. A plain Base config without logn or position ids runs
+// b200_rope_append(_multi); every other served config runs b200_rope_append_ex(_multi), with the cos/sin table for Base and Yarn.
 static torch::Tensor b200_rope_kvcache_decode(const torch::Tensor& qkv, const LayerKVCache& kv_cache, const B200AttnParamsPtr& params,
                                               const AttentionConfigs& c) {
+    B200_CHECK(params != nullptr, "b200_rope_kvcache_decode received null params");
+    B200_CHECK(rope_supported(c), "b200_rope_kvcache_decode: rope config not served (style / pairing / rotary dim)");
     const auto& pool = kv_cache.kv_cache_base;
+    const int q_len = (int)params->q_len, rows = (int)qkv.size(0), is_bf16 = qkv.scalar_type() == torch::kBFloat16;
+    B200_CHECK(q_len >= 1 && rows % q_len == 0, "b200_rope_kvcache_decode: qkv rows must be a multiple of q_len");
     torch::Tensor q = torch::empty({qkv.size(0), (int64_t)(c.head_num * c.size_per_head)}, qkv.options());
-    check_rc(b200_rope_append(qkv.data_ptr(), q.data_ptr(), pool.data_ptr(), params->kv_cache_offset.data_ptr<int>(),
-                              params->sequence_lengths.data_ptr<int>(), qkv.scalar_type() == torch::kBFloat16, (int)qkv.size(0),
-                              (int)c.head_num, (int)c.kv_head_num, (int)c.size_per_head, (int)params->kv_cache_offset.size(3),
-                              (int)page_size_of(c), (float)c.rope_config.base, cur_stream()),
-             "b200_rope_append");
+    const int32_t* seq = params->sequence_lengths.data_ptr<int>();
+    const int M = (int)params->kv_cache_offset.size(3), T = (int)page_size_of(c);
+    torch::Tensor pid = params->position_ids;
+    if (rope_is_plain_base(c, pid.defined())) {
+        if (q_len == 1)
+            check_rc(b200_rope_append(qkv.data_ptr(), q.data_ptr(), pool.data_ptr(), params->kv_cache_offset.data_ptr<int>(), seq,
+                                      is_bf16, rows, (int)c.head_num, (int)c.kv_head_num, (int)c.size_per_head, M, T,
+                                      (float)c.rope_config.base, cur_stream()),
+                     "b200_rope_append");
+        else
+            check_rc(b200_rope_append_multi(qkv.data_ptr(), q.data_ptr(), pool.data_ptr(), params->kv_cache_offset.data_ptr<int>(), seq,
+                                            is_bf16, rows / q_len, (int)c.head_num, (int)c.kv_head_num, (int)c.size_per_head, M, T,
+                                            (float)c.rope_config.base, q_len, cur_stream()),
+                     "b200_rope_append_multi");
+        return q;
+    }
+    if (pid.defined()) {
+        B200_CHECK(pid.numel() == rows, "b200_rope_kvcache_decode: combo_position_ids needs one entry per qkv row");
+        pid = pid.to(qkv.device(), torch::kInt32).contiguous();
+    }
+    const RopeConfig& r = c.rope_config;
+    const b200_rope_config cfg{r.style, rotary_dim(c), (float)r.base, (float)r.scale, (float)r.factor1, (float)r.factor2, r.max_pos,
+                               (float)r.extrapolation_factor, (float)r.mscale};
+    const torch::Tensor table = rope_table(r, cfg.dim, qkv.device());
+    const float* cache = table.defined() ? table.data_ptr<float>() : nullptr;
+    const int cache_positions = table.defined() ? (int)table.size(0) : 0;
+    const int32_t* pids = pid.defined() ? pid.data_ptr<int>() : nullptr;
+    if (q_len == 1)
+        check_rc(b200_rope_append_ex(qkv.data_ptr(), nullptr, q.data_ptr(), pool.data_ptr(), params->kv_cache_offset.data_ptr<int>(),
+                                     seq, pids, cache, cache_positions, &cfg, c.use_logn_attn, is_bf16, rows, (int)c.head_num,
+                                     (int)c.kv_head_num, (int)c.size_per_head, M, T, cur_stream()),
+                 "b200_rope_append_ex");
+    else
+        check_rc(b200_rope_append_ex_multi(qkv.data_ptr(), nullptr, q.data_ptr(), pool.data_ptr(),
+                                           params->kv_cache_offset.data_ptr<int>(), seq, pids, cache, cache_positions, &cfg,
+                                           c.use_logn_attn, is_bf16, rows / q_len, (int)c.head_num, (int)c.kv_head_num,
+                                           (int)c.size_per_head, M, T, q_len, cur_stream()),
+                 "b200_rope_append_ex_multi");
     return q;
 }
 
@@ -284,7 +440,18 @@ void registerPyModuleOps(pybind11::module& m) {
           py::arg("layernorm_eps"), py::arg("q_group_num"), py::arg("k_group_num"), py::arg("m"), py::arg("n"), py::arg("norm_size"));
     m.def("embedding", &embedding, "Embedding lookup kernel", py::arg("output"), py::arg("input"), py::arg("weight"),
           py::arg("position_ids") = py::none(), py::arg("token_type_ids") = py::none(), py::arg("text_tokens_mask") = py::none());
-    py::class_<RopeConfig>(m, "RopeConfig").def(py::init<>()).def_readwrite("base", &RopeConfig::base);
+    py::class_<RopeConfig>(m, "RopeConfig")
+        .def(py::init<>())
+        .def_readwrite("style", &RopeConfig::style)
+        .def_readwrite("dim", &RopeConfig::dim)
+        .def_readwrite("base", &RopeConfig::base)
+        .def_readwrite("scale", &RopeConfig::scale)
+        .def_readwrite("factor1", &RopeConfig::factor1)
+        .def_readwrite("factor2", &RopeConfig::factor2)
+        .def_readwrite("max_pos", &RopeConfig::max_pos)
+        .def_readwrite("extrapolation_factor", &RopeConfig::extrapolation_factor)
+        .def_readwrite("mscale", &RopeConfig::mscale)
+        .def_readwrite("is_neox_style", &RopeConfig::is_neox_style);
     py::class_<AttentionConfigs>(m, "AttentionConfigs")
         .def(py::init<>())
         .def_readwrite("head_num", &AttentionConfigs::head_num)
@@ -295,13 +462,16 @@ void registerPyModuleOps(pybind11::module& m) {
         .def_readwrite("kernel_tokens_per_block", &AttentionConfigs::kernel_tokens_per_block)
         .def_readwrite("q_scaling", &AttentionConfigs::q_scaling)
         .def_readwrite("need_rope_kv_cache", &AttentionConfigs::need_rope_kv_cache)
+        .def_readwrite("use_logn_attn", &AttentionConfigs::use_logn_attn)
         .def_readwrite("kv_cache_fp8", &AttentionConfigs::kv_cache_fp8)
         .def_readwrite("max_seq_len", &AttentionConfigs::max_seq_len);
     py::class_<PyAttentionInputs>(m, "PyAttentionInputs")
         .def(py::init<>())
         .def_readwrite("is_prefill", &PyAttentionInputs::is_prefill)
         .def_readwrite("sequence_lengths", &PyAttentionInputs::sequence_lengths)
-        .def_readwrite("kv_cache_kernel_block_id_device", &PyAttentionInputs::kv_cache_kernel_block_id_device);
+        .def_readwrite("kv_cache_kernel_block_id_device", &PyAttentionInputs::kv_cache_kernel_block_id_device)
+        .def_readwrite("input_lengths", &PyAttentionInputs::input_lengths)
+        .def_readwrite("combo_position_ids", &PyAttentionInputs::combo_position_ids);
     py::class_<LayerKVCache>(m, "LayerKVCache")
         .def(py::init<>())
         .def_readwrite("kv_cache_base", &LayerKVCache::kv_cache_base)
@@ -310,7 +480,8 @@ void registerPyModuleOps(pybind11::module& m) {
     py::class_<B200AttnParams, B200AttnParamsPtr, ParamsBase>(m, "B200AttnParams")
         .def(py::init<>())
         .def("__cpp_ptr__", [](B200AttnParams& self) { return reinterpret_cast<uintptr_t>(&self); }, "Get C++ object pointer address")
-        .def_readwrite("kv_cache_offset", &B200AttnParams::kv_cache_offset);
+        .def_readwrite("kv_cache_offset", &B200AttnParams::kv_cache_offset)
+        .def_readonly("q_len", &B200AttnParams::q_len);
     // same .def list as registerXQAAttnOp (XQAAttnOp.cc:158-176)
     py::class_<B200AttnOp>(m, "B200AttnOp")
         .def(py::init<const AttentionConfigs&>(), py::arg("attn_configs"))

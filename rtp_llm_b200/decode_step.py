@@ -17,8 +17,9 @@ from typing import Dict, List, Optional
 
 import torch
 
-from . import ops
+from . import ops, rope
 from ._lib import B200_FMT_F16, B200_FMT_INT4, B200_FMT_INT8, B200_FMT_INT8G
+from .rope import LLAMA3, RopeSpec
 
 
 @dataclasses.dataclass
@@ -35,9 +36,15 @@ class ModelConfig:
     eps: float = 1e-5
     quant: str = "int4"          # "f16" | "int8" (per column) | "int4" (group 128) | "int8g" (8-bit group 128)
     tokens_per_block: int = 64   # KVCacheConfig.seq_size_per_block default (ConfigModules.h:174)
+    # None: plain Base rotation at rope_base (b200_rope_append). A rope config runs b200_rope_append_ex(_multi) with it, and
+    # the cos/sin table for Base and Yarn (rope.py); rope_base is then unused.
+    rope: Optional[RopeSpec] = None
 
 
 LLAMA3_8B = ModelConfig("Llama-3-8B", 4096, 32, 32, 8, 128, 14336, 128256)
+# Llama-3.1 / 3.2 / 3.3: Llama3 frequency scaling (factor 8, low / high frequency factor 1 / 4, original max positions 8192)
+LLAMA31_8B = ModelConfig("Llama-3.1-8B", 4096, 32, 32, 8, 128, 14336, 128256,
+                         rope=RopeSpec(style=LLAMA3, dim=128, base=500000.0, scale=8.0, factor1=1.0, factor2=4.0, max_pos=8192))
 QWEN2_72B = ModelConfig("Qwen2-72B", 8192, 80, 64, 8, 128, 29696, 152064, rope_base=1000000.0, eps=1e-6)  # GPTQ-padded inter
 TINY = ModelConfig("tiny", 512, 2, 4, 2, 128, 512, 1024, tokens_per_block=16)
 
@@ -113,7 +120,10 @@ class DecodeStep:
         # Default off; B200_FUSE_ROPE=1 or fuse_rope=True turns it on.
         if fuse_rope is None:
             fuse_rope = os.environ.get("B200_FUSE_ROPE", "0") == "1"
-        self.fuse_rope = bool(fuse_rope) and cfg.head_dim == 128 and q_len == 1    # the fused rope appends one token
+        # the fused rope appends one token with plain Base rotation
+        self.fuse_rope = bool(fuse_rope) and cfg.head_dim == 128 and q_len == 1 and cfg.rope is None
+        if cfg.rope is not None:
+            self.rope_cfg, self.rope_table = rope.c_config(cfg.rope), rope.table(cfg.rope, device)
         g = torch.Generator(device="cpu").manual_seed(seed * 1000 + 17)
         H = cfg.hidden
 
@@ -330,6 +340,14 @@ class DecodeStep:
             self.comm.all_reduce(t)
         ops.add_rmsnorm(t, self.resid, gamma, self.cfg.eps, out=self.x)
 
+    def _rope_append(self, L):
+        if self.cfg.rope is None:
+            ops.rope_append(self.qkv, L["kv"], self.page_list, self.seq_lens, self.Hq, self.cfg.rope_base, q_out=self.q,
+                            q_len=self.q_len)
+        else:
+            ops.rope_append_ex(self.qkv, L["kv"], self.page_list, self.seq_lens, self.Hq, self.rope_cfg, q_out=self.q,
+                               cos_sin_cache=self.rope_table, q_len=self.q_len)
+
     def step_core(self):
         """Everything up to the sampled token (TP1 / peer communicator) or the local logits (NCCL): C-ABI calls only, so it
         can be recorded into a decode program."""
@@ -348,12 +366,11 @@ class DecodeStep:
                 ops.paged_decode_attn_rope(self.qkv, L["kv"], self.page_list, self.seq_lens, self.Hq, self.ctx, cfg.rope_base,
                                            self.attn_ws, out=self.attn)
             elif self.q_len > 1:  # K/V of all q_len tokens appended, then each query token attends up to its own position
-                ops.rope_append(self.qkv, L["kv"], self.page_list, self.seq_lens, self.Hq, cfg.rope_base, q_out=self.q,
-                                q_len=self.q_len)
+                self._rope_append(L)
                 ops.paged_decode_attn_multi(self.q.view(self.B, self.q_len, self.Hq, self.D), L["kv"], self.page_list, self.seq_lens,
                                             self.ctx, self.attn_ws, out=self.attn.view(self.B, self.q_len, self.Hq * self.D))
             else:
-                ops.rope_append(self.qkv, L["kv"], self.page_list, self.seq_lens, self.Hq, cfg.rope_base, q_out=self.q)
+                self._rope_append(L)
                 ops.paged_decode_attn(self.q, L["kv"], self.page_list, self.seq_lens, self.ctx, self.attn_ws, out=self.attn)
             self._row_gemm(self.attn, L["o"])
             self._ar_norm(self.proj, L["ln2"])

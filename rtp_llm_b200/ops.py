@@ -386,19 +386,30 @@ def rope_append(qkv, kv_cache_base, page_list, sequence_lengths, head_num, rope_
 
 
 def rope_append_ex(qkv, kv_cache_base, page_list, sequence_lengths, head_num, rope_cfg: "_lib.RopeConfig", q_out=None, bias=None,
-                   position_ids=None, cos_sin_cache=None, use_logn_attn=False):
+                   position_ids=None, cos_sin_cache=None, use_logn_attn=False, q_len: int = 1):
     """FusedRopeKVCacheDecodeOp.forward with the whole rope contract (styles, position_ids override, bias, cos/sin cache,
-    logn): see b200_rope_append_ex in include/b200_decode_ops.h. cos_sin_cache: fp32 [positions, dim] interleaved (cos, sin)."""
+    logn): see b200_rope_append_ex in include/b200_decode_ops.h. cos_sin_cache: fp32 [positions, dim] interleaved (cos, sin).
+    q_len > 1: qkv [B*q_len, ...] holds q_len new tokens per sequence (row b*q_len + j = token j of sequence b, appended at
+    sequence_lengths[b] + j) and position_ids, when given, has one entry per row. Returns q [B*q_len, Hq*D]."""
     import ctypes
     _cuda_contig(qkv, kv_cache_base, page_list, sequence_lengths, q_out, bias, position_ids, cos_sin_cache)
     P, two, Hkv, T, D = kv_cache_base.shape
-    B = qkv.shape[0]
+    rows = qkv.shape[0]
+    if q_len < 1 or rows % q_len:
+        raise B200Error(f"rope_append_ex: {rows} qkv rows are not a multiple of q_len {q_len}")
+    if position_ids is not None and position_ids.numel() != rows:
+        raise B200Error(f"rope_append_ex: {position_ids.numel()} position ids for {rows} qkv rows")
     if q_out is None:
-        q_out = torch.empty((B, head_num * D), dtype=qkv.dtype, device=qkv.device)
-    check(_lib.load().b200_rope_append_ex(_p(qkv), _p(bias), _p(q_out), _p(kv_cache_base), _p(page_list), _p(sequence_lengths),
-                                          _p(position_ids), _p(cos_sin_cache), cos_sin_cache.shape[0] if cos_sin_cache is not None else 0,
-                                          ctypes.cast(ctypes.pointer(rope_cfg), ctypes.c_void_p), 1 if use_logn_attn else 0,
-                                          _is_bf16(qkv), B, head_num, Hkv, D, page_list.shape[-1], T, _stream()), "b200_rope_append_ex")
+        q_out = torch.empty((rows, head_num * D), dtype=qkv.dtype, device=qkv.device)
+    lib = _lib.load()
+    args = (_p(qkv), _p(bias), _p(q_out), _p(kv_cache_base), _p(page_list), _p(sequence_lengths), _p(position_ids),
+            _p(cos_sin_cache), cos_sin_cache.shape[0] if cos_sin_cache is not None else 0,
+            ctypes.cast(ctypes.pointer(rope_cfg), ctypes.c_void_p), 1 if use_logn_attn else 0, _is_bf16(qkv), rows // q_len, head_num,
+            Hkv, D, page_list.shape[-1], T)
+    if q_len == 1:
+        check(lib.b200_rope_append_ex(*args, _stream()), "b200_rope_append_ex")
+    else:
+        check(lib.b200_rope_append_ex_multi(*args, q_len, _stream()), "b200_rope_append_ex_multi")
     return q_out
 
 

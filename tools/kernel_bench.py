@@ -89,6 +89,34 @@ def bench_attn_multi(B, Hq, Hkv, S, q_len, T=64, nrot=3):
     return us
 
 
+def bench_rope(kind, B, Hq, Hkv, q_len, S=2048, T=64, D=128, nrot=4):
+    """RoPE + K/V append of q_len tokens per sequence at cached length S - q_len: b200_rope_append(_multi) ("base") against
+    b200_rope_append_ex(_multi) with the Llama3 in-kernel formula ("llama3") or the Yarn cos/sin table ("yarn table").
+    Bytes = qkv read + q written + K/V written (+ the table rows read)."""
+    from rtp_llm_b200 import rope
+    M = math.ceil(S / T)
+    P = B * M + 1
+    pools = [torch.zeros(P, 2, Hkv, T, D, device=dev).half() for _ in range(nrot)]
+    qkv = torch.randn(B * q_len, (Hq + 2 * Hkv) * D, device=dev).half()
+    q = torch.empty(B * q_len, Hq * D, device=dev).half()
+    pl = ops.convert_block_table((torch.randperm(P - 1, device=dev).to(torch.int32) + 1).reshape(B, M))
+    seq = torch.full((B,), S - q_len, dtype=torch.int32, device=dev)
+    spec = {"llama3": rope.RopeSpec(style=rope.LLAMA3, dim=D, base=500000.0, scale=8.0, factor1=1.0, factor2=4.0, max_pos=8192),
+            "yarn table": rope.RopeSpec(style=rope.YARN, dim=D, base=1000000.0, scale=4.0, factor1=1.0, factor2=32.0, max_pos=32768,
+                                        mscale=1.14)}.get(kind)
+    if spec is None:
+        fn = lambda i: ops.rope_append(qkv, pools[i], pl, seq, Hq, 500000.0, q_out=q, q_len=q_len)
+        tbytes = 0
+    else:
+        rc, table = rope.c_config(spec), rope.table(spec, dev)
+        fn = lambda i: ops.rope_append_ex(qkv, pools[i], pl, seq, Hq, rc, q_out=q, cos_sin_cache=table, q_len=q_len)
+        tbytes = B * q_len * D * 4 if table is not None else 0
+    us = timeit(fn, nrot)
+    byt = B * q_len * ((Hq + 2 * Hkv) * D * 2 + (Hq + 2 * Hkv) * D * 2) + tbytes
+    print(f"rope {kind:10s} B{B} Hq{Hq} Hkv{Hkv} D{D} q_len {q_len}: {us:7.2f} us  {byt / us / 1e3:7.0f} GB/s", flush=True)
+    return us
+
+
 def bench_permute(B, K, nrot=4):
     """b200_permute_cols on [B, K] fp16; bytes = the row read and written, plus the perm."""
     xs = [torch.randn(B, K, device=dev).half() for _ in range(nrot)]
@@ -177,6 +205,11 @@ if __name__ == "__main__":
         # speculative-token verification at group 8 (Qwen2-72B / Llama-3-70B): 8, 16, 32, 64 query rows per kv head
         t = {n: bench_attn_multi(32, 64, 8, 2048, n) for n in (1, 2, 4, 8)}
         print("attn-multi time relative to q_len 2 (16 rows): " + ", ".join(f"q_len {n}: {t[n] / t[2]:.2f}x" for n in t), flush=True)
+    if "rope" in which:
+        # Llama-3 shape (Hq 32, Hkv 8, D 128) at B 32: the Base-only kernel against the full-contract kernel, 1 and 4 tokens
+        for n in (1, 4):
+            t = {k: bench_rope(k, 32, 32, 8, n) for k in ("base", "llama3", "yarn table")}
+            print(f"rope q_len {n} relative to base: " + ", ".join(f"{k}: {t[k] / t['base']:.2f}x" for k in t), flush=True)
     if "gemm" in which:
         for B in (32,):
             bench_gemm(B200_FMT_INT4, B, 4096, 6144)

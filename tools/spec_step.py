@@ -1,5 +1,6 @@
 #!/usr/bin/env python
-"""Cost of a speculative-token verification step (developer tool, runs on the GPU): Llama-3-8B INT4 at ctx 2048, one
+"""Cost of a speculative-token verification step (developer tool, runs on the GPU): Llama-3-8B INT4 at ctx 2048 (or
+Llama-3.1-8B with its Llama3 rope scaling, --model llama31), one
 DecodeStep per (batch, q_len) with batch * q_len <= 128, CUDA graph + PDL. The q_len variants of a batch are replayed in
 alternation, `--runs` times each, and each run times `--iters` graph replays with CUDA events. Prints ms per step and the break-even
 number of accepted drafts per step, t(q_len) / t(1) - 1: a verification step of q_len tokens pays off when it accepts more
@@ -15,11 +16,14 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from rtp_llm_b200 import ops  # noqa: E402
-from rtp_llm_b200.decode_step import LLAMA3_8B, DecodeStep  # noqa: E402
+from rtp_llm_b200.decode_step import LLAMA3_8B, LLAMA31_8B, DecodeStep  # noqa: E402
+
+MODELS = {"llama3": LLAMA3_8B, "llama31": LLAMA31_8B}
 
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--model", choices=sorted(MODELS), default="llama3")
     ap.add_argument("--batches", default="8,16,32")
     ap.add_argument("--q-lens", default="1,2,4")
     ap.add_argument("--ctx", type=int, default=2048)
@@ -38,7 +42,7 @@ def main():
     for B in sorted({c[0] for c in cfgs}):             # one batch at a time: its q_len variants are held together
         steps = {}
         for c in [c for c in cfgs if c[0] == B]:
-            m = DecodeStep(LLAMA3_8B, B, a.ctx, dev, pdl=True, q_len=c[1])
+            m = DecodeStep(MODELS[a.model], B, a.ctx, dev, pdl=True, q_len=c[1])
             m.capture()
             steps[c] = m
         for _ in range(a.runs):
@@ -54,7 +58,7 @@ def main():
         del steps, m
         torch.cuda.empty_cache()
     ops.set_pdl(False)
-    res = {"device": torch.cuda.get_device_name(0), "nvidia_smi_name_power_limit": power, "ctx": a.ctx, "runs": a.runs, "rows": []}
+    res = {"device": torch.cuda.get_device_name(0), "nvidia_smi_name_power_limit": power, "model": MODELS[a.model].name, "ctx": a.ctx, "runs": a.runs, "rows": []}
     for B, n in cfgs:
         t = sorted(times[(B, n)])
         med = t[len(t) // 2]
