@@ -36,8 +36,9 @@ class ModelConfig:
     eps: float = 1e-5
     quant: str = "int4"          # "f16" | "int8" (per column) | "int4" (group 128) | "int8g" (8-bit group 128)
     tokens_per_block: int = 64   # KVCacheConfig.seq_size_per_block default (ConfigModules.h:174)
-    # None: plain Base rotation at rope_base (b200_rope_append). A rope config runs b200_rope_append_ex(_multi) with it, and
-    # the cos/sin table for Base and Yarn (rope.py); rope_base is then unused.
+    # None: plain Base rotation at rope_base. A rope config replaces rope_base; the step appends through rope.rope_append,
+    # which runs b200_rope_append(_multi) for a plain Base config and b200_rope_append_ex(_multi) for every other one, with
+    # the cos/sin table for Base and Yarn (rope.py).
     rope: Optional[RopeSpec] = None
 
 
@@ -120,10 +121,9 @@ class DecodeStep:
         # Default off; B200_FUSE_ROPE=1 or fuse_rope=True turns it on.
         if fuse_rope is None:
             fuse_rope = os.environ.get("B200_FUSE_ROPE", "0") == "1"
+        self.rope_spec = RopeSpec(dim=self.D, base=cfg.rope_base) if cfg.rope is None else rope.spec_of(cfg.rope, self.D)
         # the fused rope appends one token with plain Base rotation
-        self.fuse_rope = bool(fuse_rope) and cfg.head_dim == 128 and q_len == 1 and cfg.rope is None
-        if cfg.rope is not None:
-            self.rope_cfg, self.rope_table = rope.c_config(cfg.rope), rope.table(cfg.rope, device)
+        self.fuse_rope = bool(fuse_rope) and cfg.head_dim == 128 and q_len == 1 and rope.is_plain_base(self.rope_spec, self.D)
         g = torch.Generator(device="cpu").manual_seed(seed * 1000 + 17)
         H = cfg.hidden
 
@@ -282,6 +282,7 @@ class DecodeStep:
         shapes = [(H, qkv_n), (self.Hq * self.D, H), (H, 2 * self.inter), (self.inter, H), (H, self.vocab)]
         self.gemm_ws = ops.gemm_workspace(R, shapes, device)
         self.attn_ws = ops.attn_workspace(R, self.Hq, self.Hkv, ctx, device)
+        rope.table(self.rope_spec, self.qkv.device)    # the cos/sin table is uploaded here, never inside a graph capture
         ops.set_pdl(pdl)
         self.graph: Optional[torch.cuda.CUDAGraph] = None
         self.prog = None
@@ -340,14 +341,6 @@ class DecodeStep:
             self.comm.all_reduce(t)
         ops.add_rmsnorm(t, self.resid, gamma, self.cfg.eps, out=self.x)
 
-    def _rope_append(self, L):
-        if self.cfg.rope is None:
-            ops.rope_append(self.qkv, L["kv"], self.page_list, self.seq_lens, self.Hq, self.cfg.rope_base, q_out=self.q,
-                            q_len=self.q_len)
-        else:
-            ops.rope_append_ex(self.qkv, L["kv"], self.page_list, self.seq_lens, self.Hq, self.rope_cfg, q_out=self.q,
-                               cos_sin_cache=self.rope_table, q_len=self.q_len)
-
     def step_core(self):
         """Everything up to the sampled token (TP1 / peer communicator) or the local logits (NCCL): C-ABI calls only, so it
         can be recorded into a decode program."""
@@ -363,14 +356,15 @@ class DecodeStep:
                 self._ar_norm(self.proj, L["ln1"])          # all-reduce of the previous layer's w2 output rides along
             ops.wo_gemm(self.x, L["qkv"], self.gemm_ws, out=self.qkv, pdl=self.pdl, x_perm=self.x_perm)
             if self.fuse_rope:    # RoPE + K/V append inside the attention kernel (one launch instead of two)
-                ops.paged_decode_attn_rope(self.qkv, L["kv"], self.page_list, self.seq_lens, self.Hq, self.ctx, cfg.rope_base,
-                                           self.attn_ws, out=self.attn)
+                ops.paged_decode_attn_rope(self.qkv, L["kv"], self.page_list, self.seq_lens, self.Hq, self.ctx,
+                                           self.rope_spec.base, self.attn_ws, out=self.attn)
             elif self.q_len > 1:  # K/V of all q_len tokens appended, then each query token attends up to its own position
-                self._rope_append(L)
+                rope.rope_append(self.rope_spec, self.qkv, L["kv"], self.page_list, self.seq_lens, self.Hq, q_out=self.q,
+                                 q_len=self.q_len)
                 ops.paged_decode_attn_multi(self.q.view(self.B, self.q_len, self.Hq, self.D), L["kv"], self.page_list, self.seq_lens,
                                             self.ctx, self.attn_ws, out=self.attn.view(self.B, self.q_len, self.Hq * self.D))
             else:
-                self._rope_append(L)
+                rope.rope_append(self.rope_spec, self.qkv, L["kv"], self.page_list, self.seq_lens, self.Hq, q_out=self.q)
                 ops.paged_decode_attn(self.q, L["kv"], self.page_list, self.seq_lens, self.ctx, self.attn_ws, out=self.attn)
             self._row_gemm(self.attn, L["o"])
             self._ar_norm(self.proj, L["ln2"])

@@ -1,72 +1,107 @@
-"""Whole-decode-step parity: the GPU step (rtp_llm_b200.decode_step.DecodeStep on the TINY config) against the CPU oracle
-composed op by op on the same weights / page tables / inputs. Used by tests (-m gpu) and __graft_entry__.smoke()."""
+"""Whole-decode-step parity: the GPU step (rtp_llm_b200.decode_step.DecodeStep) against the CPU oracle composed op by op on
+the same weights / page tables / inputs, in every mode of the step. Used by tests (-m gpu) and __graft_entry__.smoke()."""
 import dataclasses
 
 import numpy as np
 import torch
 
 from oracle import oracle as orc
+from rtp_llm_b200 import ops, rope
 from rtp_llm_b200.decode_step import TINY, DecodeStep
+from tests.spec_oracle import spec_verify_np
+
+# Llama-3.1 rope on the tiny config. Llama3 keeps a rotary dim's angle below wavelength max_pos / factor2, divides it by scale
+# above max_pos / factor1 and blends in between. max_pos 16 puts about three quarters of the dims at the tiny contexts'
+# positions (20..70) in the blended or divided band, so the step's logit tolerance separates Llama3 from Base rotation; at
+# Llama-3.1's own max_pos these short contexts would rotate almost as Base does.
+TINY31 = dataclasses.replace(TINY, quant="int4", rope=rope.RopeSpec(style=rope.LLAMA3, dim=128, base=500000.0, scale=8.0,
+                                                                    factor1=1.0, factor2=4.0, max_pos=16))
 
 
-def _bits(t: torch.Tensor) -> np.ndarray:
+def bits(t: torch.Tensor) -> np.ndarray:
     return t.detach().cpu().contiguous().view(torch.int16).numpy().view(np.uint16)
 
 
-def _gemm(x_bits, ref, is_bf16=False):
+def gemm(x_bits, ref, is_bf16=False):
     fmt, w, s, zs = ref
     if fmt == "int4":
-        return orc.dequant_gemm(x_bits, "int4", w.numpy(), scales=_bits(s), zeros_x_scales=_bits(zs), group=128, is_bf16=is_bf16)
+        return orc.dequant_gemm(x_bits, "int4", w.numpy(), scales=bits(s), zeros_x_scales=bits(zs), group=128, is_bf16=is_bf16)
     if fmt == "int8g":
-        return orc.dequant_gemm(x_bits, "int8g", w.numpy(), scales=_bits(s), zeros_x_scales=_bits(zs), group=128, is_bf16=is_bf16)
+        return orc.dequant_gemm(x_bits, "int8g", w.numpy(), scales=bits(s), zeros_x_scales=bits(zs), group=128, is_bf16=is_bf16)
     if fmt == "int8":
-        return orc.dequant_gemm(x_bits, "int8", w.numpy(), scales=_bits(s), is_bf16=is_bf16)
-    return orc.dequant_gemm(x_bits, "f16", _bits(w), is_bf16=is_bf16)
+        return orc.dequant_gemm(x_bits, "int8", w.numpy(), scales=bits(s), is_bf16=is_bf16)
+    return orc.dequant_gemm(x_bits, "f16", bits(w), is_bf16=is_bf16)
 
 
 def oracle_step(model: DecodeStep, kv_before):
-    cfg = model.cfg
-    ids = model.ids_h.numpy()
+    """The logits of one step of `model` (a DecodeStep, or any object with the attributes read here), op by op on the CPU.
+    - q_len tokens per sequence: every token's K/V is appended at seq + j before any query attends; query j attends up to
+      seq + j.
+    - the step's rope spec, under the seams' rule: the b200_rope_append oracle for a plain Base spec, else the full rope
+      contract with the spec's fields and its cos/sin table.
+    - act-order (a layer with "perm"): x[:, perm] before qkv / w13, attn[:, perm] before o, and the SiLU*mul output in w2's
+      row order before w2 (what the folded w13 emits). L["ref"] holds the sorted qkv / o / w2 and the checkpoint-order w13."""
+    cfg, B, n, Hq, Hkv, D, T = model.cfg, model.B, model.q_len, model.Hq, model.Hkv, model.D, model.cfg.tokens_per_block
+    spec = model.rope_spec
     seq = model.seq_lens_h.numpy()
     pl = orc.convert_block_table(model.block_ids_h.numpy())
-    resid = _bits(model.embed)[ids]
+    if rope.is_plain_base(spec, D):
+        def append(qkv, pool, s):
+            return orc.rope_append(qkv, pool, pl, s, Hq, Hkv, D, T, spec.base)
+    else:
+        fields = {f: getattr(spec, f) for f, _ in orc.RopeConfig._fields_}
+        table = rope.build_table(spec)
+        cache = None if table is None else table.numpy()
+
+        def append(qkv, pool, s):
+            return orc.rope_append_ex(qkv, pool, pl, s, Hq, Hkv, D, T, fields, cos_sin_cache=cache)
+    resid = bits(model.embed)[model.ids_h.numpy().reshape(-1)]
     proj = None
     for li, L in enumerate(model.layers):
+        P = {k: v.numpy() for k, v in L.get("perm", {}).items()}
+        gathered = lambda t, k: t[:, P[k]] if P else t  # noqa: E731
         if li == 0:
-            x, _ = orc.add_rmsnorm(resid, None, _bits(L["ln1"]), cfg.eps)
+            x, _ = orc.add_rmsnorm(resid, None, bits(L["ln1"]), cfg.eps)
         else:
-            x, resid = orc.add_rmsnorm(proj, resid, _bits(L["ln1"]), cfg.eps)
-        qkv = _gemm(x, L["ref"]["qkv"])
-        q, pool = orc.rope_append(qkv, kv_before[li], pl, seq, model.Hq, model.Hkv, model.D, cfg.tokens_per_block, cfg.rope_base)
-        a = orc.paged_decode_attn(q.reshape(model.B, model.Hq, model.D), pool, pl, seq, model.Hq, model.Hkv, model.D,
-                                  cfg.tokens_per_block)
-        proj = _gemm(a, L["ref"]["o"])
-        x, resid = orc.add_rmsnorm(proj, resid, _bits(L["ln2"]), cfg.eps)
-        gu = _gemm(x, L["ref"]["w13"])
-        act = orc.silu_and_mul(gu)
-        proj = _gemm(act, L["ref"]["w2"])
-    x, resid = orc.add_rmsnorm(proj, resid, _bits(model.final_ln), cfg.eps)
-    logits = _gemm(x, model.lm_head_ref)
-    return orc.from_bits(logits, False)
+            x, resid = orc.add_rmsnorm(proj, resid, bits(L["ln1"]), cfg.eps)
+        qkv = gemm(gathered(x, "qkv"), L["ref"]["qkv"]).reshape(B, n, -1)
+        pool, qs = kv_before[li], []
+        for j in range(n):
+            qj, pool = append(np.ascontiguousarray(qkv[:, j]), pool, seq + j)
+            qs.append(qj)
+        a = np.stack([orc.paged_decode_attn(qs[j].reshape(B, Hq, D), pool, pl, seq + j, Hq, Hkv, D, T) for j in range(n)],
+                     axis=1).reshape(B * n, -1)
+        proj = gemm(gathered(a, "o"), L["ref"]["o"])
+        x, resid = orc.add_rmsnorm(proj, resid, bits(L["ln2"]), cfg.eps)
+        act = orc.silu_and_mul(gemm(gathered(x, "w13"), L["ref"]["w13"]))
+        proj = gemm(gathered(act, "w2"), L["ref"]["w2"])
+    x, resid = orc.add_rmsnorm(proj, resid, bits(model.final_ln), cfg.eps)
+    return orc.from_bits(gemm(x, model.lm_head_ref), False)
 
 
-def check_tiny_step(dev, quant="int4", batch=3, ctx=40, graph=False, pdl=False, program=False, fuse_rope=False) -> float:
-    cfg = dataclasses.replace(TINY, quant=quant)
-    model = DecodeStep(cfg, batch, ctx, dev, keep_reference=True, ragged=True, seed=1, pdl=pdl, fuse_rope=fuse_rope)
-    kv_before = [_bits(L["kv"]) for L in model.layers]
-    if program:
-        model.build_program()
-        assert model.prog.num_ops > 0, "nothing was fused into the persistent kernel"
-    if graph:
-        for L, kb in zip(model.layers, kv_before):   # capture() runs the step (appends K/V): the append is idempotent
-            pass
-        model.capture()
-        model.replay()
-    else:
-        model.run()
-    torch.cuda.synchronize(dev)
-    if pdl:
-        from rtp_llm_b200 import ops
+def check_step(cfg=TINY, quant=None, batch=3, ctx=40, mode="eager", q_len=1, act_order=False, fuse_rope=False, seed=1,
+               dev=torch.device("cuda:0")) -> float:
+    """Builds DecodeStep(cfg with `quant`, ragged lengths, reference weights kept), runs one step and checks it against
+    oracle_step. mode: "eager" (op by op), or any of "graph" (captured and replayed), "pdl" and "program" (recorded into a
+    decode program) together. Asserts finite logits within 3e-2 * rms + 3e-2 of the oracle, greedy tokens equal to the
+    oracle's argmax wherever its top-2 margin exceeds twice that error, and for q_len > 1 the verifier's out_tokens /
+    accepted on the step's own greedy rows. Returns the max |logit error|."""
+    if quant is not None:
+        cfg = dataclasses.replace(cfg, quant=quant)
+    model = DecodeStep(cfg, batch, ctx, dev, keep_reference=True, ragged=True, seed=seed, pdl="pdl" in mode, fuse_rope=fuse_rope,
+                       act_order=act_order, q_len=q_len)
+    try:                                    # DecodeStep(pdl=True) switched PDL on library-wide
+        kv_before = [bits(L["kv"]) for L in model.layers]
+        if "program" in mode:
+            model.build_program()
+            assert model.prog.num_ops > 0, "nothing was fused into the persistent kernel"
+        if "graph" in mode:                 # capture() runs the step (appends K/V) before recording it: the append is idempotent
+            model.capture()
+            model.replay()
+        else:
+            model.run()
+        torch.cuda.synchronize(dev)
+    finally:
         ops.set_pdl(False)
     got = model.logits.float().cpu().numpy()
     exp = oracle_step(model, kv_before)
@@ -74,11 +109,13 @@ def check_tiny_step(dev, quant="int4", batch=3, ctx=40, graph=False, pdl=False, 
     err = float(np.abs(got - exp).max())
     assert np.isfinite(got).all()
     assert err <= 3e-2 * scale + 3e-2, f"logits differ: max err {err} vs rms {scale}"
-    # greedy token: must equal the oracle's argmax wherever the oracle's top-2 margin exceeds the error bound
     nxt = model.next_ids.cpu().numpy()
     oa = orc.argmax(exp)
     srt = np.sort(exp, axis=-1)
-    margin = srt[:, -1] - srt[:, -2]
-    sure = margin > 2 * err + 1e-6
+    sure = srt[:, -1] - srt[:, -2] > 2 * err + 1e-6
     assert (nxt[sure] == oa[sure]).all(), (nxt, oa)
+    if q_len > 1:
+        eo, ea = spec_verify_np(model.ids_h[:, 1:].numpy(), target_ids=nxt.reshape(model.B, q_len))
+        np.testing.assert_array_equal(model.accepted.cpu().numpy(), ea)
+        np.testing.assert_array_equal(model.out_tokens.cpu().numpy(), eo)
     return err

@@ -1,6 +1,6 @@
 """GPTQ act-order (desc_act) weights on an H100: the column gather b200_permute_cols (eager, CUDA graph + PDL, decode program),
 the GEMM of a weight that carries its row order, the loader on act-order checkpoints (qkv, o, fused SiLU w13 and the w2 order
-folded into w13), blob copies, and DecodeStep(act_order=True) against a perm-aware oracle."""
+folded into w13), blob copies, and DecodeStep(act_order=True) against the step oracle, also with q_len > 1 and Llama-3.1 rope."""
 import dataclasses
 import io
 
@@ -10,7 +10,6 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
-from oracle import oracle as orc  # noqa: E402
 from rtp_llm_b200 import ops  # noqa: E402
 from rtp_llm_b200._lib import B200Error  # noqa: E402
 from rtp_llm_b200.decode_step import TINY, DecodeStep  # noqa: E402
@@ -18,7 +17,7 @@ from rtp_llm_b200.device import B200Impl  # noqa: E402
 from rtp_llm_b200.linear import B200WeightOnlyLinear  # noqa: E402
 from rtp_llm_b200.loader import B200Loader, CheckpointReader, QuantConfig  # noqa: E402
 from tests import act_order_ckpt  # noqa: E402
-from tests.step_oracle import _bits, _gemm  # noqa: E402
+from tests.step_oracle import TINY31, check_step  # noqa: E402
 
 dev = torch.device("cuda")
 DT = [torch.float16, torch.bfloat16]
@@ -223,56 +222,20 @@ def test_layer_through_the_loader(tmp_path, bits, group):
 
 
 # ---------------------------------------------------------------------------------------------- the whole step
-def _oracle_step_act_order(model, kv_before):
-    """tests/step_oracle.oracle_step with the gathers: x[:, perm] before qkv / w13, attn[:, perm] before o, and the SiLU*mul
-    output in w2's row order before w2 (what the folded w13 emits). The weights in L["ref"] are the sorted ones (qkv, o, w2)
-    and the checkpoint-order gate|up (w13)."""
-    cfg = model.cfg
-    ids, seq = model.ids_h.numpy(), model.seq_lens_h.numpy()
-    pl = orc.convert_block_table(model.block_ids_h.numpy())
-    resid = _bits(model.embed)[ids]
-    proj = None
-    for li, L in enumerate(model.layers):
-        P = {k: v.numpy() for k, v in L["perm"].items()}
-        if li == 0:
-            x, _ = orc.add_rmsnorm(resid, None, _bits(L["ln1"]), cfg.eps)
-        else:
-            x, resid = orc.add_rmsnorm(proj, resid, _bits(L["ln1"]), cfg.eps)
-        qkv = _gemm(x[:, P["qkv"]], L["ref"]["qkv"])
-        q, pool = orc.rope_append(qkv, kv_before[li], pl, seq, model.Hq, model.Hkv, model.D, cfg.tokens_per_block, cfg.rope_base)
-        a = orc.paged_decode_attn(q.reshape(model.B, model.Hq, model.D), pool, pl, seq, model.Hq, model.Hkv, model.D,
-                                  cfg.tokens_per_block)
-        proj = _gemm(a.reshape(model.B, -1)[:, P["o"]], L["ref"]["o"])
-        x, resid = orc.add_rmsnorm(proj, resid, _bits(L["ln2"]), cfg.eps)
-        act = orc.silu_and_mul(_gemm(x[:, P["w13"]], L["ref"]["w13"]))
-        proj = _gemm(act[:, P["w2"]], L["ref"]["w2"])
-    x, resid = orc.add_rmsnorm(proj, resid, _bits(model.final_ln), cfg.eps)
-    return orc.from_bits(_gemm(x, model.lm_head_ref), False)
-
-
 @pytest.mark.parametrize("mode", ["eager", "graph", "graph+pdl", "program", "program+graph+pdl"])
 @pytest.mark.parametrize("quant", ["int4", "int8g"])
 def test_decode_step_with_act_order_matches_the_oracle(quant, mode):
-    cfg = dataclasses.replace(TINY, quant=quant)
-    pdl = "pdl" in mode
-    model = DecodeStep(cfg, 5, 70, dev, keep_reference=True, ragged=True, seed=2, pdl=pdl, act_order=True)
-    kv_before = [_bits(L["kv"]) for L in model.layers]
-    try:
-        if "program" in mode:
-            model.build_program()
-        if "graph" in mode:
-            model.capture()
-            model.replay()
-        else:
-            model.run()
-        torch.cuda.synchronize()
-    finally:
-        ops.set_pdl(False)
-    got = model.logits.float().cpu().numpy()
-    exp = _oracle_step_act_order(model, kv_before)
-    scale = float(np.sqrt((exp ** 2).mean()))
-    err = float(np.abs(got - exp).max())
-    assert np.isfinite(got).all() and err <= 3e-2 * scale + 3e-2, f"logits differ: max err {err} vs rms {scale}"
+    check_step(quant=quant, batch=5, ctx=70, mode=mode, act_order=True, seed=2, dev=dev)
+
+
+# act-order with the other step modes: a verification step (q_len 2) and the Llama-3.1 rope
+COMBOS = [(TINY, 2, "eager"), (TINY, 2, "graph+pdl"), (TINY31, 1, "eager")]
+
+
+@pytest.mark.parametrize("case", COMBOS, ids=["int4 q_len 2 eager", "int4 q_len 2 graph+pdl", "llama31 eager"])
+def test_act_order_step_with_verification_or_llama31_rope_matches_the_oracle(case):
+    cfg, q_len, mode = case
+    check_step(cfg, quant="int4", batch=5, ctx=70, mode=mode, q_len=q_len, act_order=True, seed=2, dev=dev)
 
 
 def test_act_order_adds_three_gathers_per_layer_and_nothing_when_off():

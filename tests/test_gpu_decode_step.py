@@ -3,32 +3,32 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
-from tests.step_oracle import check_tiny_step  # noqa: E402
+from tests.step_oracle import check_step  # noqa: E402
 
 
 @pytest.mark.parametrize("quant", ["int4", "int8", "int8g", "f16"])
 def test_tiny_decode_step_matches_oracle(quant):
-    check_tiny_step(torch.device("cuda:0"), quant=quant, batch=3, ctx=40)
+    check_step(quant=quant, batch=3, ctx=40)
 
 
 def test_tiny_decode_step_under_cuda_graph():
-    check_tiny_step(torch.device("cuda:0"), quant="int4", batch=5, ctx=70, graph=True)
+    check_step(quant="int4", batch=5, ctx=70, mode="graph")
 
 
 def test_tiny_decode_step_with_programmatic_dependent_launch():
-    check_tiny_step(torch.device("cuda:0"), quant="int4", batch=5, ctx=70, graph=True, pdl=True)
-    check_tiny_step(torch.device("cuda:0"), quant="int8", batch=3, ctx=40, graph=False, pdl=True)
+    check_step(quant="int4", batch=5, ctx=70, mode="graph+pdl")
+    check_step(quant="int8", batch=3, ctx=40, mode="pdl")
 
 
 @pytest.mark.parametrize("quant", ["int4", "int8", "f16"])
 def test_tiny_decode_step_as_program(quant):
     """The same step recorded into a decode program (GEMMs / norms / rope fused into the persistent kernel)."""
-    check_tiny_step(torch.device("cuda:0"), quant=quant, batch=3, ctx=40, program=True)
+    check_step(quant=quant, batch=3, ctx=40, mode="program")
 
 
 def test_tiny_decode_step_as_program_under_cuda_graph_with_pdl():
-    check_tiny_step(torch.device("cuda:0"), quant="int4", batch=5, ctx=70, graph=True, pdl=True, program=True)
-    check_tiny_step(torch.device("cuda:0"), quant="int8", batch=17, ctx=70, graph=True, program=True)
+    check_step(quant="int4", batch=5, ctx=70, mode="program+graph+pdl")
+    check_step(quant="int8", batch=17, ctx=70, mode="program+graph")
 
 
 def test_program_replays_are_identical_and_match_op_by_op():
@@ -56,5 +56,5 @@ def test_program_replays_are_identical_and_match_op_by_op():
 
 
 def test_tiny_decode_step_with_rope_fused_into_attention():
-    check_tiny_step(torch.device("cuda:0"), quant="int4", batch=5, ctx=70, graph=True, pdl=True, fuse_rope=True)
-    check_tiny_step(torch.device("cuda:0"), quant="int8", batch=3, ctx=40, program=True, fuse_rope=True)
+    check_step(quant="int4", batch=5, ctx=70, mode="graph+pdl", fuse_rope=True)
+    check_step(quant="int8", batch=3, ctx=40, mode="program", fuse_rope=True)

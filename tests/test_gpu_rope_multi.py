@@ -1,8 +1,8 @@
 """GPU tests (H100) of the full rope contract for several tokens per sequence and through the attention seams:
 b200_rope_append_ex_multi against successive one-token calls, B200DecodeImpl and the pybind B200AttnOp against the op-by-op
-oracle for each rope style at q_len 1 and 3, and a DecodeStep verification step under a Llama-3.1 rope config."""
+oracle for each rope style at q_len 1 and 3, and a DecodeStep under a Llama-3.1 rope config (verification steps and decode
+programs included) against the step oracle."""
 import ctypes
-import dataclasses
 import importlib.util
 import math
 from types import SimpleNamespace
@@ -14,11 +14,9 @@ import torch
 pytestmark = pytest.mark.gpu
 
 from oracle import oracle as orc  # noqa: E402
-from rtp_llm_b200 import _lib, attention, build, ops, rope  # noqa: E402
+from rtp_llm_b200 import _lib, attention, build, ops  # noqa: E402
 from rtp_llm_b200._lib import RopeConfig  # noqa: E402
-from rtp_llm_b200.decode_step import TINY, DecodeStep  # noqa: E402
-from tests.spec_oracle import spec_verify_np  # noqa: E402
-from tests.step_oracle import _bits, _gemm  # noqa: E402
+from tests.step_oracle import TINY31, check_step  # noqa: E402
 from tests.test_gpu_rope import CASES  # noqa: E402
 
 DEV = torch.device("cuda")
@@ -256,97 +254,11 @@ def test_pybind_seam_serves_group_32_and_refuses_unserved_rope():
 
 
 # ------------------------------------------------------------------------------------------------------------ step
-TINY31 = dataclasses.replace(TINY, quant="int4", rope=rope.RopeSpec(style=rope.LLAMA3, dim=128, base=500000.0, scale=8.0,
-                                                                    factor1=1.0, factor2=4.0, max_pos=64))
-
-
-def _oracle_step_multi(model: DecodeStep, kv_before):
-    """The op-by-op oracle of a (verification) step with the model's rope config: the one-token rope contract and attention
-    applied per token j at seq + j."""
-    cfg, B, n = model.cfg, model.B, model.q_len
-    rc = {f: getattr(cfg.rope, f) for f in ("style", "dim", "base", "scale", "factor1", "factor2", "max_pos", "extrapolation_factor",
-                                            "mscale")}
-    seq = model.seq_lens_h.numpy().astype(np.int32)
-    pl = orc.convert_block_table(model.block_ids_h.numpy())
-    resid = _bits(model.embed)[model.ids_h.numpy().reshape(-1)]
-    proj = None
-    for li, L in enumerate(model.layers):
-        if li == 0:
-            x, _ = orc.add_rmsnorm(resid, None, _bits(L["ln1"]), cfg.eps)
-        else:
-            x, resid = orc.add_rmsnorm(proj, resid, _bits(L["ln1"]), cfg.eps)
-        qkv = _gemm(x, L["ref"]["qkv"]).reshape(B, n, -1)
-        pool, qs = kv_before[li], []
-        for j in range(n):
-            qj, pool = orc.rope_append_ex(np.ascontiguousarray(qkv[:, j]), pool, pl, seq + j, model.Hq, model.Hkv, model.D,
-                                          cfg.tokens_per_block, rc)
-            qs.append(qj)
-        a = np.stack([orc.paged_decode_attn(qs[j].reshape(B, model.Hq, model.D), pool, pl, seq + j, model.Hq, model.Hkv, model.D,
-                                            cfg.tokens_per_block) for j in range(n)], axis=1).reshape(B * n, -1)
-        proj = _gemm(a, L["ref"]["o"])
-        x, resid = orc.add_rmsnorm(proj, resid, _bits(L["ln2"]), cfg.eps)
-        act = orc.silu_and_mul(_gemm(x, L["ref"]["w13"]))
-        proj = _gemm(act, L["ref"]["w2"])
-    x, resid = orc.add_rmsnorm(proj, resid, _bits(model.final_ln), cfg.eps)
-    return orc.from_bits(_gemm(x, model.lm_head_ref), False)
-
-
-STEP = [(1, "eager"), (2, "eager"), (4, "eager"), (4, "graph pdl"), (1, "graph pdl")]
+# program: rope_append_ex is recorded as its own launch between the persistent-kernel segments
+STEP = [(1, "eager"), (2, "eager"), (4, "eager"), (4, "graph pdl"), (1, "graph pdl"), (1, "program"), (1, "program graph pdl")]
 
 
 @pytest.mark.parametrize("case", STEP, ids=[f"q_len {n} {m}" for n, m in STEP])
 def test_llama31_step_vs_oracle(case):
-    """max_pos 64 on a 40-token context with ragged lengths: positions on both sides of the Llama3 frequency split."""
     q_len, mode = case
-    model = DecodeStep(TINY31, 3, 40, DEV, keep_reference=True, ragged=True, seed=1, pdl="pdl" in mode, q_len=q_len)
-    try:
-        kv_before = [_bits(L["kv"]) for L in model.layers]
-        if "graph" in mode:
-            model.capture()
-            model.replay()
-        else:
-            model.run()
-        torch.cuda.synchronize()
-    finally:
-        ops.set_pdl(False)
-    got = model.logits.float().cpu().numpy()
-    exp = _oracle_step_multi(model, kv_before)
-    scale = float(np.sqrt((exp ** 2).mean()))
-    err = float(np.abs(got - exp).max())
-    assert np.isfinite(got).all()
-    assert err <= 3e-2 * scale + 3e-2, f"logits differ: max err {err} vs rms {scale}"
-
-
-@pytest.mark.parametrize("k", [1, 3])
-def test_llama31_verification_step_accepts_the_tokens_plain_steps_produce(k):
-    plain = DecodeStep(TINY31, 4, 40, DEV, ragged=True, seed=2)
-    spec = DecodeStep(TINY31, 4, 40, DEV, ragged=True, seed=2, q_len=k + 1)
-    plain.seq_lens_h.copy_(spec.seq_lens_h)
-    plain.ids_h.copy_(spec.ids_h[:, 0])
-    toks, logits = [plain.ids_h.clone()], []
-    for _ in range(k + 1):
-        plain.upload_inputs()
-        plain.run()
-        torch.cuda.synchronize()
-        logits.append(plain.logits.float().cpu().numpy())
-        toks.append(plain.next_ids.cpu())
-        plain.ids_h.copy_(plain.next_ids.cpu())
-        plain.seq_lens_h += 1
-    spec.ids_h.copy_(torch.stack(toks[:k + 1], dim=1))
-    spec.upload_inputs()
-    spec.run()
-    torch.cuda.synchronize()
-    got = spec.logits.float().cpu().numpy().reshape(spec.B, k + 1, -1)
-    exp = np.stack(logits, axis=1)
-    scale = float(np.sqrt((exp ** 2).mean()))
-    err = float(np.abs(got - exp).max())
-    assert err <= 3e-2 * scale + 3e-2, f"logits differ: max err {err} vs rms {scale}"
-    srt = np.sort(exp, axis=-1)
-    sure = ((srt[..., -1] - srt[..., -2]) > 2 * err + 1e-6).all(axis=1)
-    assert sure.any(), "no sequence with a clear margin at every step"
-    acc, out = spec.accepted.cpu().numpy(), spec.out_tokens.cpu().numpy()
-    assert (acc[sure] == k).all(), acc
-    np.testing.assert_array_equal(out[sure, k], toks[k + 1].numpy()[sure])
-    np.testing.assert_array_equal(out[sure, :k], torch.stack(toks[1:k + 1], dim=1).numpy()[sure])
-    eo, ea = spec_verify_np(spec.ids_h[:, 1:].numpy(), target_ids=spec.next_ids.view(spec.B, k + 1).cpu().numpy())
-    np.testing.assert_array_equal(acc, ea)
+    check_step(TINY31, batch=3, ctx=40, mode=mode, q_len=q_len, dev=DEV)

@@ -13,7 +13,7 @@ from rtp_llm_b200 import ops  # noqa: E402
 from rtp_llm_b200.decode_step import TINY, DecodeStep  # noqa: E402
 from tests import gpu_probe as probe  # noqa: E402
 from tests.spec_oracle import spec_verify_np  # noqa: E402
-from tests.step_oracle import _bits, _gemm  # noqa: E402
+from tests.step_oracle import TINY31, check_step  # noqa: E402
 
 DEV = torch.device("cuda")
 TILES = "B200_ATTN_TILES_PER_SPLIT"
@@ -192,35 +192,6 @@ def test_spec_verify_sampling_vs_oracle(n, with_draft_probs):
 
 
 # ---------------------------------------------------------------------------------------------------- decode step
-def _oracle_step_multi(model: DecodeStep, kv_before):
-    """oracle_step of step_oracle with q_len tokens per sequence: the per-call oracle rope append and attention, applied per
-    token j at seq + j (every token's K/V is appended before any query attends)."""
-    cfg, B, n = model.cfg, model.B, model.q_len
-    seq = model.seq_lens_h.numpy().astype(np.int32)
-    pl = orc.convert_block_table(model.block_ids_h.numpy())
-    resid = _bits(model.embed)[model.ids_h.numpy().reshape(-1)]
-    proj = None
-    for li, L in enumerate(model.layers):
-        if li == 0:
-            x, _ = orc.add_rmsnorm(resid, None, _bits(L["ln1"]), cfg.eps)
-        else:
-            x, resid = orc.add_rmsnorm(proj, resid, _bits(L["ln1"]), cfg.eps)
-        qkv = _gemm(x, L["ref"]["qkv"]).reshape(B, n, -1)
-        pool, qs = kv_before[li], []
-        for j in range(n):
-            qj, pool = orc.rope_append(np.ascontiguousarray(qkv[:, j]), pool, pl, seq + j, model.Hq, model.Hkv, model.D,
-                                       cfg.tokens_per_block, cfg.rope_base)
-            qs.append(qj)
-        a = np.stack([orc.paged_decode_attn(qs[j].reshape(B, model.Hq, model.D), pool, pl, seq + j, model.Hq, model.Hkv, model.D,
-                                            cfg.tokens_per_block) for j in range(n)], axis=1).reshape(B * n, -1)
-        proj = _gemm(a, L["ref"]["o"])
-        x, resid = orc.add_rmsnorm(proj, resid, _bits(L["ln2"]), cfg.eps)
-        act = orc.silu_and_mul(_gemm(x, L["ref"]["w13"]))
-        proj = _gemm(act, L["ref"]["w2"])
-    x, resid = orc.add_rmsnorm(proj, resid, _bits(model.final_ln), cfg.eps)
-    return orc.from_bits(_gemm(x, model.lm_head_ref), False)
-
-
 STEP = [(q, n, "eager") for q in ("int4", "int8", "int8g", "f16") for n in (2, 4)] + \
        [("int4", 4, "graph"), ("int4", 4, "pdl"), ("f16", 2, "graph pdl"), ("int8g", 4, "graph")]
 
@@ -228,28 +199,7 @@ STEP = [(q, n, "eager") for q in ("int4", "int8", "int8g", "f16") for n in (2, 4
 @pytest.mark.parametrize("case", STEP, ids=[f"{q} q_len {n} {m}" for q, n, m in STEP])
 def test_verification_step_vs_oracle(case):
     quant, q_len, mode = case
-    cfg = dataclasses.replace(TINY, quant=quant)
-    model = DecodeStep(cfg, 3, 40, DEV, keep_reference=True, ragged=True, seed=1, pdl="pdl" in mode, q_len=q_len)
-    try:
-        kv_before = [_bits(L["kv"]) for L in model.layers]
-        if "graph" in mode:
-            model.capture()
-            model.replay()
-        else:
-            model.run()
-        torch.cuda.synchronize()
-    finally:
-        ops.set_pdl(False)
-    got = model.logits.float().cpu().numpy()
-    exp = _oracle_step_multi(model, kv_before)
-    scale = float(np.sqrt((exp ** 2).mean()))
-    err = float(np.abs(got - exp).max())
-    assert np.isfinite(got).all()
-    assert err <= 3e-2 * scale + 3e-2, f"logits differ: max err {err} vs rms {scale}"
-    rows = model.next_ids.view(model.B, q_len).cpu().numpy()
-    eo, ea = spec_verify_np(model.ids_h[:, 1:].numpy(), target_ids=rows)
-    np.testing.assert_array_equal(model.accepted.cpu().numpy(), ea)
-    np.testing.assert_array_equal(model.out_tokens.cpu().numpy(), eo)
+    check_step(quant=quant, batch=3, ctx=40, mode=mode, q_len=q_len, dev=DEV)
 
 
 def test_verification_step_is_not_a_program():
@@ -259,11 +209,12 @@ def test_verification_step_is_not_a_program():
 
 
 @pytest.mark.parametrize("k", [1, 3])
-def test_verification_step_accepts_the_tokens_plain_steps_produce(k):
+@pytest.mark.parametrize("cfg", [dataclasses.replace(TINY, quant="int4"), TINY31], ids=["int4", "llama31"])
+def test_verification_step_accepts_the_tokens_plain_steps_produce(cfg, k):
     """k greedy single-token steps on one model, then one q_len = k + 1 step on an identical model with those tokens as drafts:
     row j's logits match plain step j, and wherever every plain step's top-2 margin is clear of the error, all k drafts are
-    accepted and the emitted token is plain step k's."""
-    cfg = dataclasses.replace(TINY, quant="int4")
+    accepted and the emitted token is plain step k's. Everywhere, the verifier's decisions are those of the reference on the
+    step's own greedy rows."""
     plain = DecodeStep(cfg, 4, 40, DEV, ragged=True, seed=2)
     spec = DecodeStep(cfg, 4, 40, DEV, ragged=True, seed=2, q_len=k + 1)
     plain.seq_lens_h.copy_(spec.seq_lens_h)
@@ -293,3 +244,5 @@ def test_verification_step_accepts_the_tokens_plain_steps_produce(k):
     assert (acc[sure] == k).all(), acc
     np.testing.assert_array_equal(out[sure, k], toks[k + 1].numpy()[sure])
     np.testing.assert_array_equal(out[sure, :k], torch.stack(toks[1:k + 1], dim=1).numpy()[sure])
+    eo, ea = spec_verify_np(spec.ids_h[:, 1:].numpy(), target_ids=spec.next_ids.view(spec.B, k + 1).cpu().numpy())
+    np.testing.assert_array_equal(acc, ea)

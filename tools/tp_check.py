@@ -62,13 +62,13 @@ def types_ns(model, cfg, kv_before, world):
     rank generated the full pool from a common seed and kept only ITS kv heads, so ranks hold different K/V)."""
     import types
     full = types.SimpleNamespace()
-    full.cfg, full.B, full.D = cfg, model.B, model.D
+    full.cfg, full.B, full.D, full.q_len, full.rope_spec = cfg, model.B, model.D, model.q_len, model.rope_spec
     full.Hq, full.Hkv = cfg.head_num, cfg.kv_head_num
     full.ids_h, full.seq_lens_h, full.block_ids_h = model.ids_h, model.seq_lens_h, model.block_ids_h
     full.embed, full.final_ln = model.embed, model.final_ln
     full.lm_head_ref = model.lm_head_full
     full.layers = [dict(ln1=L["ln1"], ln2=L["ln2"], ref=L["full"]) for L in model.layers]
-    full.kv_before = [step_oracle._bits(L["kv_full"]) for L in model.layers]
+    full.kv_before = [step_oracle.bits(L["kv_full"]) for L in model.layers]
     return full
 
 
