@@ -261,6 +261,35 @@ int b200_sample(float* logits, int rows, int vocab, const int32_t* history, cons
 int b200_spec_verify(const float* target_probs, const int32_t* target_ids, const float* draft_probs, const int32_t* draft_tokens,
                      const float* uniform, int batch, int num_draft, int vocab, int32_t* out_tokens, int32_t* accepted, void* stream);
 
+/* One beam-search step over the lm_head logits of `batch` requests x W = beam_width beams. The semantics are restated from the
+ * Hugging Face / TensorRT-LLM beam-search convention; the reference's vendored kernels (3rdparty/trt_beam_search) are not in
+ * this tree, so parity with them is unpinned, as for the GEMM.
+ *   logits [batch*W][vocab] (row b*W + i = beam i of request b), dtype 0 fp16, 1 bf16, 2 fp32, read as they are (no cast);
+ *   cum_log_probs fp32 [batch][W]. W in 1..32, vocab >= 2W, ceil(vocab / 4096) * 2W <= 4096, vocab <= 2^26.
+ * Every candidate (i, v) scores cum[b][i] + (x - m_i) - log sum_v exp(x - m_i) in fp32 (x the logit, m_i the row max: a log-softmax
+ * per beam); candidates rank by score descending, equal scores by lower flat index i*vocab + v. -inf logits and rows with
+ * cum = -inf give -inf scores, which rank last, by index (first step: cum[b][1:] = -inf, so only beam 0 contributes).
+ * Outputs: the top 2W candidates in rank order, cand_token / cand_parent (beam index 0..W-1) / cand_score [batch][2W]; the next
+ * beams next_token / next_parent / next_cum [batch][W] = the first W ranked candidates whose token is not eos_id (-1: none). Each
+ * row adds at most one EOS candidate, so W of the 2W are never EOS; the EOS candidates among the first W ranks are the finished
+ * hypotheses (length penalty, early stopping and the finished-hypothesis set stay the caller's).
+ * workspace: b200_beam_search_step_workspace_bytes(batch, W, vocab) bytes, ZERO on first use; every call leaves it zero-ready
+ * (self-resetting arrival counters). One launch, deterministic, graph-capturable; under PDL it waits before reading logits / cum. */
+size_t b200_beam_search_step_workspace_bytes(int batch, int beam_width, int vocab);
+int b200_beam_search_step(const void* logits, int dtype, const float* cum_log_probs, int batch, int beam_width, int vocab, int eos_id,
+                          int32_t* cand_token, int32_t* cand_parent, float* cand_score, int32_t* next_token, int32_t* next_parent,
+                          float* next_cum, void* workspace, size_t workspace_bytes, void* stream);
+
+/* No-repeat-n-gram ban, in place, before b200_sample or b200_beam_search_step (Hugging Face no_repeat_ngram_size over the whole
+ * history the caller passes; restated, parity with the reference's banRepeatNgram kernel unpinned). history [rows][hist_stride]
+ * and hist_len [rows] as b200_sample takes them (hist_len is clamped to hist_stride). For row r with n = ngram_size[r] > 0 and
+ * L = hist_len[r]: for every start s in [0, L - n] with h[s .. s+n-2] == h[L-n+1 .. L-1], logits[r][h[s+n-1]] = -inf (n == 1 bans
+ * every token of the history); ids outside [0, vocab) are ignored; n <= 0 or L < n leaves the row alone. Every other logit keeps
+ * its bits. logits dtype 0 fp16, 1 bf16, 2 fp32. Temperature, the penalties and b200_sample leave -inf at -inf, so the order of
+ * this op and those does not matter. One CTA per row; under PDL it waits before reading anything. */
+int b200_ban_repeat_ngram(void* logits, int dtype, int rows, int vocab, const int32_t* history, const int32_t* hist_len, int hist_stride,
+                          const int32_t* ngram_size, void* stream);
+
 /* ------------------------------------------------------------------------------------------------ TP all-reduce over NVLink peer memory */
 
 /* One-shot SUM all-reduce of a small [rows][hidden] fp16/bf16 tensor, the exchange after each row-parallel GEMM

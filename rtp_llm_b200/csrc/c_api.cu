@@ -1036,6 +1036,119 @@ int b200_spec_verify(const float* target_probs, const int32_t* target_ids, const
     return launched("spec_verify_kernel");
 }
 
+namespace {
+// Byte offsets of the beam step's workspace arrays (BeamParams), each 256-byte aligned; total = 0 for an unsupported shape.
+struct BeamWorkspace {
+    size_t count, chunk_stat, chunk_val, chunk_idx, row_stat, row_val, row_idx, total;
+};
+BeamWorkspace beam_workspace(int batch, int beam_width, int vocab) {
+    BeamWorkspace w{};
+    if (batch < 0 || beam_width < 1 || beam_width > kBeamMaxWidth || vocab < 2 * beam_width || vocab > (1 << 26)) return w;
+    const size_t rows = (size_t)batch * beam_width, S = (vocab + kBeamChunk - 1) / kBeamChunk, K = 2 * beam_width;
+    if (S * K > (size_t)kBeamMaxItems) return w;
+    size_t o = 0;
+    auto take = [&](size_t bytes) {
+        const size_t at = o;
+        o = round_up(o + bytes, 256);
+        return at;
+    };
+    w.count = take((rows + batch) * 4);
+    w.chunk_stat = take(rows * S * 8);
+    w.chunk_val = take(rows * S * K * 4);
+    w.chunk_idx = take(rows * S * K * 4);
+    w.row_stat = take(rows * 8);
+    w.row_val = take(rows * K * 4);
+    w.row_idx = take(rows * K * 4);
+    w.total = o;
+    return w;
+}
+}  // namespace
+
+size_t b200_beam_search_step_workspace_bytes(int batch, int beam_width, int vocab) {
+    return beam_workspace(batch, beam_width, vocab).total;
+}
+
+int b200_beam_search_step(const void* logits, int dtype, const float* cum_log_probs, int batch, int beam_width, int vocab, int eos_id,
+                          int32_t* cand_token, int32_t* cand_parent, float* cand_score, int32_t* next_token, int32_t* next_parent,
+                          float* next_cum, void* workspace, size_t workspace_bytes, void* stream) {
+    ARG_CHECK(beam_width >= 1 && beam_width <= kBeamMaxWidth, "beam_search_step: beam_width %d unsupported (1..%d)", beam_width,
+              kBeamMaxWidth);
+    ARG_CHECK(vocab >= 2 * beam_width, "beam_search_step: vocab %d must be >= 2 * beam_width (%d)", vocab, 2 * beam_width);
+    ARG_CHECK(vocab <= (1 << 26), "beam_search_step: vocab %d exceeds %d", vocab, 1 << 26);
+    ARG_CHECK((size_t)(vocab + kBeamChunk - 1) / kBeamChunk * 2 * beam_width <= (size_t)kBeamMaxItems,
+              "beam_search_step: vocab %d x beam_width %d exceeds the row merge (ceil(vocab / %d) * 2 * beam_width <= %d)", vocab,
+              beam_width, kBeamChunk, kBeamMaxItems);
+    ARG_CHECK(dtype >= 0 && dtype <= 2, "beam_search_step: dtype %d unknown (0 fp16, 1 bf16, 2 fp32)", dtype);
+    ARG_CHECK(batch >= 0 && (long)batch * beam_width <= 65535, "beam_search_step: batch %d x beam_width %d exceeds 65535 rows", batch,
+              beam_width);
+    if (batch == 0) return B200_OK;
+    ARG_CHECK(logits && cum_log_probs && cand_token && cand_parent && cand_score && next_token && next_parent && next_cum,
+              "beam_search_step: null pointer");
+    const BeamWorkspace w = beam_workspace(batch, beam_width, vocab);
+    ARG_CHECK(workspace && workspace_bytes >= w.total,
+              "beam_search_step: workspace too small (%zu < %zu bytes, see b200_beam_search_step_workspace_bytes)",
+              workspace ? workspace_bytes : (size_t)0, w.total);
+    if (g_rec)
+        return rec_call([=](void* st) {
+            return b200_beam_search_step(logits, dtype, cum_log_probs, batch, beam_width, vocab, eos_id, cand_token, cand_parent,
+                                         cand_score, next_token, next_parent, next_cum, workspace, workspace_bytes, st);
+        });
+    char* ws = static_cast<char*>(workspace);
+    BeamParams p{};
+    p.logits = logits;
+    p.cum = cum_log_probs;
+    p.count = reinterpret_cast<uint32_t*>(ws + w.count);
+    p.chunk_stat = reinterpret_cast<float2*>(ws + w.chunk_stat);
+    p.chunk_val = reinterpret_cast<float*>(ws + w.chunk_val);
+    p.chunk_idx = reinterpret_cast<uint32_t*>(ws + w.chunk_idx);
+    p.row_stat = reinterpret_cast<float2*>(ws + w.row_stat);
+    p.row_val = reinterpret_cast<float*>(ws + w.row_val);
+    p.row_idx = reinterpret_cast<uint32_t*>(ws + w.row_idx);
+    p.cand_token = cand_token;
+    p.cand_parent = cand_parent;
+    p.cand_score = cand_score;
+    p.next_token = next_token;
+    p.next_parent = next_parent;
+    p.next_cum = next_cum;
+    p.W = beam_width;
+    p.V = vocab;
+    p.S = (vocab + kBeamChunk - 1) / kBeamChunk;
+    p.eos = eos_id;
+    const LaunchCfg cfg{dim3(p.S, batch * beam_width), dim3(kBeamThreads), 0, (cudaStream_t)stream, g_pdl.load() != 0};
+    auto launch = [&](auto t) {
+        CUDA_CHECK(launch_ex(beam_search_kernel<decltype(t)>, cfg, p));
+        return launched("beam_search_kernel");
+    };
+    return dtype == 2 ? launch(0.f) : by_dtype(dtype == 1, launch);
+}
+
+int b200_ban_repeat_ngram(void* logits, int dtype, int rows, int vocab, const int32_t* history, const int32_t* hist_len, int hist_stride,
+                          const int32_t* ngram_size, void* stream) {
+    ARG_CHECK(rows >= 0 && rows <= 65535, "ban_repeat_ngram: rows %d unsupported (0..65535)", rows);
+    ARG_CHECK(vocab > 0, "ban_repeat_ngram: vocab must be positive");
+    ARG_CHECK(dtype >= 0 && dtype <= 2, "ban_repeat_ngram: dtype %d unknown (0 fp16, 1 bf16, 2 fp32)", dtype);
+    ARG_CHECK(hist_stride > 0, "ban_repeat_ngram: hist_stride must be positive");
+    if (rows == 0) return B200_OK;
+    ARG_CHECK(logits && history && hist_len && ngram_size, "ban_repeat_ngram: null pointer");
+    if (g_rec)
+        return rec_call([=](void* st) {
+            return b200_ban_repeat_ngram(logits, dtype, rows, vocab, history, hist_len, hist_stride, ngram_size, st);
+        });
+    BanNgramParams p{};
+    p.logits = logits;
+    p.history = history;
+    p.hist_len = hist_len;
+    p.ngram_size = ngram_size;
+    p.vocab = vocab;
+    p.hist_stride = hist_stride;
+    const LaunchCfg cfg{dim3(rows), dim3(256), 0, (cudaStream_t)stream, g_pdl.load() != 0};
+    auto launch = [&](auto t) {
+        CUDA_CHECK(launch_ex(ban_repeat_ngram_kernel<decltype(t)>, cfg, p));
+        return launched("ban_repeat_ngram_kernel");
+    };
+    return dtype == 2 ? launch(0.f) : by_dtype(dtype == 1, launch);
+}
+
 // ------------------------------------------------------------------------------------------------ peer all-reduce
 size_t b200_peer_ar_region_bytes(size_t max_message_bytes) {
     return 2 * peer_strides(max_message_bytes).parity + kArMaxCtas * sizeof(uint32_t) + 256;

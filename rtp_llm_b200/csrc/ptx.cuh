@@ -221,6 +221,8 @@ template <>
 __device__ __forceinline__ __half from_f32<__half>(float v) { return __float2half_rn(v); }
 template <>
 __device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
+template <>
+__device__ __forceinline__ float from_f32<float>(float v) { return v; }
 
 // The rotation of one RoPE channel pair with the rounding sequence PINNED (explicit mul / fma intrinsics): every kernel that
 // rotates (rope_append, rope_append_ex, the persistent kernel's rope op, the attention kernel's fused rope) produces the same

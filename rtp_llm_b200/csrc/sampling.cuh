@@ -304,4 +304,282 @@ __global__ void __launch_bounds__(kSampleThreads) spec_verify_kernel(const SpecV
     }
 }
 
+// ------------------------------------------------------------------------------------------------ beam search
+// One beam-search step over the [B*W][V] lm_head logits (Hugging Face / TRT-LLM convention). Every candidate (i, v) of request b
+// scores cum[b][i] + (x - m_i) - log sum_v exp(x - m_i) in fp32 and candidates rank by score descending, then by lower flat index
+// i*V + v. Within a row the score is monotone in the logit, so each row's top 2W is taken on the raw logits and only W * 2W
+// survivors meet in the cross-beam ranking.
+// Grid (S = ceil(V / kBeamChunk), B*W), kBeamThreads threads, one launch in three levels joined by self-resetting arrival
+// counters in the caller's workspace (as the GEMM's l2_merge): every CTA takes the top 2W, the max and sum exp(x - max) of its
+// chunk; the last chunk CTA of a row to arrive merges the row's S partials; the last row of a request to arrive ranks the
+// request's W * 2W survivors and writes the outputs. Every merge reads the partials in a fixed order: deterministic.
+// Selection is by bisection on an order-preserving uint32 key of the fp32 value (no sort): the threshold key with at least 2W
+// items at or above it, then, among the items at the threshold, the lowest indices by a second bisection.
+constexpr int kBeamThreads = 256;
+constexpr int kBeamChunk = 4096;       // logits per CTA (staged in shared memory as keys)
+constexpr int kBeamMaxItems = 4096;    // items one selection holds: kBeamChunk, S * 2W (row merge) and W * 2W (request merge)
+constexpr int kBeamMaxWidth = 32;
+constexpr uint32_t kBeamPad = 0xFFFFFFFFu;   // index of a padding item (key 0, below every real key)
+
+struct BeamParams {
+    const void* logits;       // [B*W][V] fp16 / bf16 / fp32
+    const float* cum;         // [B][W]
+    uint32_t* count;          // [B*W + B] arrival counters, zero on entry and on exit
+    float2* chunk_stat;       // [B*W][S] (max, sum exp(x - max)) of each chunk
+    float* chunk_val;         // [B*W][S][2W] top 2W logits of each chunk (-inf for a row whose cum is -inf)
+    uint32_t* chunk_idx;      // [B*W][S][2W] their vocabulary ids (kBeamPad: padding)
+    float2* row_stat;         // [B*W] (max, sum exp(x - max)) of each row
+    float* row_val;           // [B*W][2W]
+    uint32_t* row_idx;        // [B*W][2W]
+    int32_t* cand_token;      // [B][2W]
+    int32_t* cand_parent;     // [B][2W]
+    float* cand_score;        // [B][2W]
+    int32_t* next_token;      // [B][W]
+    int32_t* next_parent;     // [B][W]
+    float* next_cum;          // [B][W]
+    int W, V, S, eos;
+};
+
+// fp32 -> uint32 with the same order (-0 is folded into +0 first, so equal values have equal keys), and back
+__device__ __forceinline__ uint32_t beam_key(float x) {
+    const uint32_t u = __float_as_uint(x + 0.f);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float beam_value(uint32_t k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k); }
+
+// Block-wide count of the items that satisfy pred, identical in every thread. One barrier per count: the per-warp sums go to
+// one of two halves of s_red [2][warps] by `par`, so a count writes the half whose readers (two counts back) have all passed
+// the previous count's barrier.
+template <typename Pred>
+__device__ __forceinline__ int beam_count(int n, const Pred& pred, int* s_red, int& par) {
+    int c = 0;
+    for (int j = threadIdx.x; j < n; j += kBeamThreads) c += pred(j) ? 1 : 0;
+    c = __reduce_add_sync(0xffffffffu, c);
+    int* red = s_red + par * (kBeamThreads / 32);
+    par ^= 1;
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = c;
+    __syncthreads();
+    int t = 0;
+#pragma unroll
+    for (int w = 0; w < kBeamThreads / 32; ++w) t += red[w];
+    return t;
+}
+
+// The K largest of the n >= K items (key[j], idx[j]) by key descending, then idx ascending (indices unique), into out_key /
+// out_idx [K] in rank order. Every thread of the CTA calls it, after a barrier that makes key / idx visible; it ends with one.
+// Cost: up to 32 block-wide counts to find the threshold key (fewer when a count hits K exactly), and when several items sit
+// at the threshold, two more counts and up to 32 for the index bisection among them.
+__device__ void beam_select(int n, int K, const uint32_t* key, const uint32_t* idx, uint32_t* sel_key, uint32_t* sel_idx,
+                            uint32_t* out_key, uint32_t* out_idx, int* s_red, int* s_n) {
+    int par = 0;
+    uint32_t lo = 0u, hi = 0xFFFFFFFFu;             // invariant: count(key >= lo) >= K
+    bool exact = false;                             // count(key >= lo) == K: the K items at or above lo are the answer
+    while (lo < hi) {
+        const uint32_t mid = lo + (uint32_t)(((uint64_t)hi - lo + 1u) >> 1);
+        const int c = beam_count(n, [&](int j) { return key[j] >= mid; }, s_red, par);
+        if (c >= K) lo = mid;
+        else hi = mid - 1u;
+        if (c == K) {
+            exact = true;
+            break;
+        }
+    }
+    const uint32_t T = lo;
+    uint32_t U = 0xFFFFFFFFu;                       // items at the threshold with idx <= U are taken
+    if (!exact && beam_count(n, [&](int j) { return key[j] >= T; }, s_red, par) > K) {
+        const int need = K - beam_count(n, [&](int j) { return key[j] > T; }, s_red, par);
+        uint32_t a = 0u, z = 0xFFFFFFFFu;           // the least u with count(key == T && idx <= u) >= need
+        while (a < z) {
+            const uint32_t mid = a + ((z - a) >> 1);
+            if (beam_count(n, [&](int j) { return key[j] == T && idx[j] <= mid; }, s_red, par) >= need) z = mid;
+            else a = mid + 1u;
+        }
+        U = a;
+    }
+    if (threadIdx.x == 0) *s_n = 0;
+    __syncthreads();
+    for (int j = threadIdx.x; j < n; j += kBeamThreads) {
+        const uint32_t k = key[j];
+        if (k > T || (k == T && idx[j] <= U)) {
+            const int s = atomicAdd(s_n, 1);        // slot order is arbitrary: the rank below fixes the output order
+            sel_key[s] = k;
+            sel_idx[s] = idx[j];
+        }
+    }
+    __syncthreads();
+    for (int s = threadIdx.x; s < K; s += kBeamThreads) {
+        const uint32_t k = sel_key[s], x = sel_idx[s];
+        int r = 0;
+        for (int t = 0; t < K; ++t) r += (sel_key[t] > k || (sel_key[t] == k && sel_idx[t] < x)) ? 1 : 0;
+        out_key[r] = k;
+        out_idx[r] = x;
+    }
+    __syncthreads();
+}
+
+// Counts this CTA in *counter (expected arrivals: `of`); true in the last one to arrive, which resets the counter. The CTA's
+// workspace stores (st.cg) are issued before the barrier; the last arriver reads the others' with ld.cg.
+__device__ __forceinline__ bool beam_arrive(uint32_t* counter, int of, int* s_flag) {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence();
+        unsigned prev;
+        asm volatile("atom.acq_rel.gpu.global.add.u32 %0, [%1], 1;" : "=r"(prev) : "l"(counter) : "memory");
+        const bool last = prev == (unsigned)(of - 1);
+        if (last) *counter = 0;        // every CTA has arrived: no one else touches the counter in this launch
+        *s_flag = last;
+    }
+    __syncthreads();
+    if (*s_flag) __threadfence();
+    return *s_flag;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kBeamThreads) beam_search_kernel(const BeamParams p) {
+    __shared__ uint32_t s_key[kBeamMaxItems], s_idx[kBeamMaxItems];
+    __shared__ uint32_t s_sel_key[2 * kBeamMaxWidth], s_sel_idx[2 * kBeamMaxWidth];
+    __shared__ uint32_t s_out_key[2 * kBeamMaxWidth], s_out_idx[2 * kBeamMaxWidth];
+    __shared__ int s_red[2 * (kBeamThreads / 32)], s_n, s_flag;
+    __shared__ float s_fred[kBeamThreads / 32];
+    const int tid = threadIdx.x, c = blockIdx.x, row = blockIdx.y, W = p.W, V = p.V, S = p.S, K = 2 * W;
+    const int b = row / W;
+    pdl_wait();                        // under PDL the logits and cum come from the kernels before this one
+    constexpr uint32_t kNegInf = 0x007FFFFFu;                  // beam_key(-inf)
+    auto dead = [&](int r) { return !(p.cum[r] > -INFINITY); };   // cum -inf (or NaN): every score of the row is -inf
+
+    // ---- level 1: this chunk's top 2W keys and its (max, sum exp)
+    {
+        const T* lg = reinterpret_cast<const T*>(p.logits) + (size_t)row * V;
+        const int v0 = c * kBeamChunk, n = min(kBeamChunk, V - v0);
+        const bool d = dead(row);
+        float m = -INFINITY;
+        for (int j = tid; j < n; j += kBeamThreads) {
+            float x = to_f32<T>(lg[v0 + j]);
+            if (x != x) x = -INFINITY;                         // NaN ranks with the masked logits
+            m = fmaxf(m, x);
+            s_key[j] = d ? kNegInf : beam_key(x);
+            s_idx[j] = v0 + j;
+        }
+        for (int j = n + tid; j < K; j += kBeamThreads) {       // a short last chunk: pad to 2W items
+            s_key[j] = 0u;
+            s_idx[j] = kBeamPad - j;
+        }
+#pragma unroll
+        for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+        if ((tid & 31) == 0) s_fred[tid >> 5] = m;
+        __syncthreads();
+        m = -INFINITY;
+#pragma unroll
+        for (int w = 0; w < kBeamThreads / 32; ++w) m = fmaxf(m, s_fred[w]);
+        // sum exp(x - m) from the staged keys (each thread reads its own): NaN counts as -inf here too, and a row with cum -inf,
+        // whose keys are all -inf, gets z = 0, which no score reads
+        float z = 0.f;
+        if (m > -INFINITY)
+            for (int j = tid; j < n; j += kBeamThreads) z += expf(beam_value(s_key[j]) - m);
+#pragma unroll
+        for (int o = 16; o; o >>= 1) z += __shfl_xor_sync(0xffffffffu, z, o);
+        __syncthreads();
+        if ((tid & 31) == 0) s_fred[tid >> 5] = z;
+        __syncthreads();
+        z = 0.f;
+#pragma unroll
+        for (int w = 0; w < kBeamThreads / 32; ++w) z += s_fred[w];
+        beam_select(max(n, K), K, s_key, s_idx, s_sel_key, s_sel_idx, s_out_key, s_out_idx, s_red, &s_n);
+        const size_t slot = (size_t)row * S + c;
+        for (int r = tid; r < K; r += kBeamThreads) {
+            __stcg(p.chunk_val + slot * K + r, beam_value(s_out_key[r]));
+            __stcg(p.chunk_idx + slot * K + r, s_out_idx[r]);
+        }
+        if (tid == 0) __stcg(p.chunk_stat + slot, make_float2(m, z));
+    }
+    if (!beam_arrive(p.count + row, S, &s_flag)) return;
+
+    // ---- level 2 (last chunk of the row): the row's top 2W of the S * 2W chunk survivors, and the row's (max, sum exp)
+    {
+        const int n = S * K;
+        for (int j = tid; j < n; j += kBeamThreads) {
+            const uint32_t x = __ldcg(p.chunk_idx + (size_t)row * n + j);
+            s_idx[j] = x;
+            s_key[j] = x >= (uint32_t)V ? 0u : beam_key(__ldcg(p.chunk_val + (size_t)row * n + j));
+        }
+        __syncthreads();
+        beam_select(n, K, s_key, s_idx, s_sel_key, s_sel_idx, s_out_key, s_out_idx, s_red, &s_n);
+        for (int r = tid; r < K; r += kBeamThreads) {
+            __stcg(p.row_val + (size_t)row * K + r, beam_value(s_out_key[r]));
+            __stcg(p.row_idx + (size_t)row * K + r, s_out_idx[r]);
+        }
+        if (tid == 0) {
+            float m = -INFINITY, z = 0.f;
+            for (int s = 0; s < S; ++s) m = fmaxf(m, __ldcg(p.chunk_stat + (size_t)row * S + s).x);
+            for (int s = 0; s < S; ++s) {
+                const float2 st = __ldcg(p.chunk_stat + (size_t)row * S + s);
+                if (st.x > -INFINITY) z += st.y * expf(st.x - m);
+            }
+            __stcg(p.row_stat + row, make_float2(m, z));
+        }
+    }
+    if (!beam_arrive(p.count + gridDim.y + b, W, &s_flag)) return;
+
+    // ---- level 3 (last row of the request): rank the W * 2W survivors by score, then by flat index i * V + v
+    const int n = W * K;
+    for (int j = tid; j < n; j += kBeamThreads) {
+        const int i = j / K, r = b * W + i;
+        const float x = __ldcg(p.row_val + (size_t)r * K + j % K);
+        const uint32_t v = __ldcg(p.row_idx + (size_t)r * K + j % K);
+        const float2 st = __ldcg(p.row_stat + r);
+        const float cum = p.cum[r];
+        const float score = (dead(r) || !(x > -INFINITY)) ? -INFINITY : cum + ((x - st.x) - logf(st.y));
+        s_key[j] = beam_key(score);
+        s_idx[j] = (uint32_t)i * (uint32_t)V + v;
+    }
+    __syncthreads();
+    beam_select(n, K, s_key, s_idx, s_sel_key, s_sel_idx, s_out_key, s_out_idx, s_red, &s_n);
+    for (int r = tid; r < K; r += kBeamThreads) {
+        const uint32_t x = s_out_idx[r];
+        p.cand_token[b * K + r] = (int32_t)(x % (uint32_t)V);
+        p.cand_parent[b * K + r] = (int32_t)(x / (uint32_t)V);
+        p.cand_score[b * K + r] = beam_value(s_out_key[r]);
+    }
+    if (tid == 0) {                    // the first W candidates that are not EOS (each row adds at most one EOS to the 2W)
+        int taken = 0;
+        for (int r = 0; r < K && taken < W; ++r) {
+            const uint32_t x = s_out_idx[r];
+            const int tok = (int)(x % (uint32_t)V);
+            if (tok == p.eos) continue;
+            p.next_token[b * W + taken] = tok;
+            p.next_parent[b * W + taken] = (int)(x / (uint32_t)V);
+            p.next_cum[b * W + taken] = beam_value(s_out_key[r]);
+            ++taken;
+        }
+    }
+}
+
+// No-repeat-n-gram ban (Hugging Face no_repeat_ngram_size over the whole history): for every start s in [0, L - n] whose
+// first n - 1 tokens equal the last n - 1 tokens of the history, logits[h[s + n - 1]] = -inf. One CTA per row; every thread
+// takes a share of the starts. Several threads may store -inf to the same logit: the same bits, so the result is deterministic.
+struct BanNgramParams {
+    void* logits;                 // [rows][vocab] fp16 / bf16 / fp32, edited in place
+    const int32_t* history;       // [rows][hist_stride]
+    const int32_t* hist_len;      // [rows]
+    const int32_t* ngram_size;    // [rows]; <= 0: off
+    int vocab, hist_stride;
+};
+
+template <typename T>
+__global__ void __launch_bounds__(256) ban_repeat_ngram_kernel(const BanNgramParams p) {
+    const int row = blockIdx.x;
+    pdl_wait();                        // under PDL the logits and the history come from the kernels before this one
+    const int n = p.ngram_size[row];
+    const int L = min(p.hist_len[row], p.hist_stride);
+    if (n <= 0 || L < n) return;
+    const int32_t* h = p.history + (size_t)row * p.hist_stride;
+    T* lg = reinterpret_cast<T*>(p.logits) + (size_t)row * p.vocab;
+    for (int s = threadIdx.x; s <= L - n; s += blockDim.x) {
+        bool match = true;
+        for (int k = 0; k < n - 1 && match; ++k) match = h[s + k] == h[L - n + 1 + k];
+        const int t = h[s + n - 1];
+        if (match && t >= 0 && t < p.vocab) lg[t] = from_f32<T>(-INFINITY);
+    }
+}
+
 }  // namespace b200

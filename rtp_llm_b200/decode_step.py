@@ -78,18 +78,44 @@ class DecodeStep:
     q_len > 1 (TP 1, op by op or under a CUDA graph; not in a decode program): a verification step of speculative tokens. Each
     sequence feeds q_len tokens, ids_h [B, q_len] = the last accepted token and q_len - 1 drafts, at positions seq_lens_h[b] + j.
     Every op runs on the B * q_len rows (rope_append / paged_decode_attn_multi for the attention), argmax picks each row's
-    token, and spec_verify (greedy) checks the drafts against them: out_tokens [B, q_len], accepted [B]."""
+    token, and spec_verify (greedy) checks the drafts against them: out_tokens [B, q_len], accepted [B].
+
+    beam_width W > 1 (TP 1, q_len 1, op by op or under a CUDA graph; not in a decode program): beam search over `batch` requests.
+    Each beam is a sequence of its own, so every op runs on B * W rows, row b * W + i = beam i of request b, with its own
+    page-table row. The prompt (ctx - max_new_tokens tokens already cached) shares its full pages among a request's W beams;
+    from the prompt's last, partial page onward every beam owns private pages. The step ends in ban_repeat_ngram (when
+    no_repeat_ngram > 0) and beam_search_step instead of argmax, then forks in place with static buffers: cum_log_probs takes
+    next_cum, the token history rows are gathered by next_parent and the new token appended, new beam j takes its parent's
+    page-table entries for the full pages, and the parent's partial last page is copied into j's own page (every source page
+    gathered into scratch first, then scattered, since a beam can be a parent and a child in the same step). Then the ids
+    become next_token and the lengths grow by one: the next call runs the next step. upload_inputs() restarts from the prompt;
+    a step past max_new_tokens since then raises ValueError (the page-table rows end there), in run() and in replay().
+    The device state: beam_cum [B, W], hist [B*W, ctx] / hist_len [B*W], beam_out (the beam_search_step outputs)."""
 
     def __init__(self, cfg: ModelConfig, batch: int, ctx: int, device: torch.device, tp_rank: int = 0, tp_size: int = 1,
                  dtype=torch.float16, seed: int = 0, keep_reference: bool = False, ragged: bool = False,
                  pdl: bool = False, comm=None, fuse_silu: bool = True, fuse_ar_norm: bool = True, fuse_rope: Optional[bool] = None,
-                 fuse_gemm_rs: Optional[bool] = None, act_order: bool = False, q_len: int = 1):
+                 fuse_gemm_rs: Optional[bool] = None, act_order: bool = False, q_len: int = 1, beam_width: int = 1,
+                 no_repeat_ngram: int = 0, max_new_tokens: int = 16):
         assert cfg.head_num % tp_size == 0 and cfg.inter % tp_size == 0
         if q_len < 1:
             raise ValueError(f"q_len must be >= 1 (got {q_len})")
         if q_len > 1 and (batch * q_len > 128 or tp_size != 1):
             raise ValueError(f"a verification step (q_len {q_len}) needs batch * q_len <= 128 (the GEMM row limit) and tp_size 1 "
                              f"(got batch {batch}, tp_size {tp_size})")
+        if not 1 <= beam_width <= 32:
+            raise ValueError(f"beam_width must be in 1..32 (got {beam_width})")
+        if beam_width > 1 and (batch * beam_width > 128 or tp_size != 1 or q_len != 1):
+            raise ValueError(f"beam search (beam_width {beam_width}) needs batch * beam_width <= 128 (the GEMM row limit), tp_size 1 "
+                             f"and q_len 1 (got batch {batch}, tp_size {tp_size}, q_len {q_len})")
+        if beam_width > 1 and not 1 <= max_new_tokens < ctx:
+            raise ValueError(f"max_new_tokens must be in 1..ctx-1 (got {max_new_tokens}, ctx {ctx})")
+        if no_repeat_ngram != 0 and beam_width == 1:
+            raise ValueError(f"no_repeat_ngram {no_repeat_ngram} needs beam search (beam_width > 1); the greedy step has no ban")
+        self.W, self.ngram, self.max_new_tokens = beam_width, no_repeat_ngram, max_new_tokens
+        self.beam_steps = 0                             # beam steps run since the prompt (upload_inputs)
+        self.requests = batch
+        batch = batch * beam_width                      # sequences (page-table rows) of the step
         self.q_len = q_len
         R = batch * q_len                               # token rows of the step
         if act_order and (tp_size != 1 or cfg.quant not in ("int4", "int8g")):
@@ -247,8 +273,21 @@ class DecodeStep:
             lens = torch.randint(ctx // 2, ctx + 1, (batch,), generator=gl)
         else:
             lens = torch.full((batch,), ctx)
+        if beam_width > 1:    # one prompt per request, room for max_new_tokens
+            lens = (lens.view(-1, beam_width)[:, :1].expand(-1, beam_width).reshape(-1) - max_new_tokens + 1).clamp(min=1)
         self.seq_lens_h = (lens - q_len).to(torch.int32).pin_memory()   # tokens already cached (SURVEY a3)
         self.ids_h = torch.randint(0, cfg.vocab, (batch,) if q_len == 1 else (batch, q_len), generator=gp).to(torch.int32).pin_memory()
+        if beam_width > 1:
+            self.own_pages = self.block_ids_h.clone()                 # every beam's private pages, by page-table index
+            full = self.seq_lens_h.view(-1, beam_width)[:, 0] // T    # the prompt's full pages, shared by the request's beams
+            blk = self.block_ids_h.view(-1, beam_width, self.M)
+            for b in range(blk.shape[0]):
+                f = int(full[b])
+                blk[b, 1:, :f] = blk[b, 0, :f]
+                if f < self.M:                                        # the prompt's partial page: the same tokens in every beam
+                    for L in self.layers:
+                        L["kv"][blk[b, 1:, f].long().to(device)] = L["kv"][int(blk[b, 0, f])].clone()
+            self.ids_h.copy_(self.ids_h.view(-1, beam_width)[:, :1].expand(-1, beam_width).reshape(-1))
         self.next_h = torch.zeros(batch, dtype=torch.int32).pin_memory()
         if q_len > 1:
             self.drafts_h = torch.zeros(batch, q_len - 1, dtype=torch.int32).pin_memory()
@@ -277,6 +316,31 @@ class DecodeStep:
             self.drafts = buf(batch, q_len - 1, dt=torch.int32)
             self.out_tokens = buf(batch, q_len, dt=torch.int32)
             self.accepted = buf(batch, dt=torch.int32)
+        if beam_width > 1:
+            W, B = beam_width, self.requests
+            self.beam_cum = buf(B, W, dt=torch.float32)
+            self.hist = buf(R, ctx, dt=torch.int32)
+            self.hist_len = buf(R, dt=torch.int32)
+            self.ngram_size = torch.full((R,), no_repeat_ngram, dtype=torch.int32, device=device)
+            self.beam_out = {k: buf(B, n, dt=dt) for k, n, dt in (
+                ("cand_token", 2 * W, torch.int32), ("cand_parent", 2 * W, torch.int32), ("cand_score", 2 * W, torch.float32),
+                ("next_token", W, torch.int32), ("next_parent", W, torch.int32), ("next_cum", W, torch.float32))}
+            self.beam_ws = ops.beam_search_workspace(B, W, self.vocab, device)
+            self.own_pages_i32 = self.own_pages.to(device)
+            self.own_pages_d = self.own_pages_i32.to(torch.int64)
+            self.row_base = torch.arange(R, device=device) // W * W                  # row of beam 0 of each row's request
+            self.row_m = torch.arange(R, device=device) * self.M
+            self.page_idx = torch.arange(self.M, device=device)
+            # fork scratch (static: the fork runs inside a CUDA graph)
+            self.parent_row, self.pos = buf(R, dt=torch.int64), buf(R, dt=torch.int64)
+            self.src_flat, self.dst_flat, self.pick_flat = (buf(R, dt=torch.int64) for _ in range(3))
+            self.src_page, self.dst_page = buf(R, dt=torch.int64), buf(R, dt=torch.int64)
+            self.partial = buf(R, dt=torch.bool)
+            self.full_mask = buf(R, self.M, dt=torch.bool)
+            self.blk_parent = buf(R, self.M, dt=torch.int32)
+            self.hist_parent = buf(R, ctx, dt=torch.int32)
+            self.len_parent = buf(R, dt=torch.int32)
+            self.page_scratch = buf(R, 2, self.Hkv, T, self.D)
         self.x_perm = buf(R, H) if act_order else None                        # x[:, perm] before qkv / w13
         self.attn_perm = buf(R, self.Hq * self.D) if act_order else None      # attn[:, perm] before o
         shapes = [(H, qkv_n), (self.Hq * self.D, H), (H, 2 * self.inter), (self.inter, H), (H, self.vocab)]
@@ -298,13 +362,26 @@ class DecodeStep:
         if self.q_len > 1:
             self.drafts_h.copy_(self.ids_h[:, 1:])
             self.drafts.copy_(self.drafts_h, non_blocking=True)
+        if self.W > 1:        # back to the prompt: beam 0 alone live (cum 0), the input token as the whole history
+            self.beam_cum.fill_(-math.inf)
+            self.beam_cum[:, 0] = 0.0
+            self.hist[:, 0].copy_(self.ids)
+            self.hist_len.fill_(1)
+            self.beam_steps = 0
+
+    def _count_beam_step(self):
+        if self.W > 1:
+            if self.beam_steps >= self.max_new_tokens:
+                raise ValueError(f"beam step {self.beam_steps + 1} since the prompt exceeds max_new_tokens {self.max_new_tokens}: "
+                                 "call upload_inputs() to restart from the prompt")
+            self.beam_steps += 1
 
     def download_outputs(self):
         if self.q_len > 1:
             self.out_tokens_h.copy_(self.out_tokens, non_blocking=True)
             self.accepted_h.copy_(self.accepted, non_blocking=True)
             return
-        self.next_h.copy_(self.next_ids, non_blocking=True)
+        self.next_h.copy_(self.beam_out["next_token"].view(-1) if self.W > 1 else self.next_ids, non_blocking=True)
 
     def h2d_bytes(self) -> int:
         drafts = self.drafts_h.numel() * 4 if self.q_len > 1 else 0
@@ -376,13 +453,57 @@ class DecodeStep:
             self._row_gemm(self.act, L["w2"])
         self._ar_norm(self.proj, self.final_ln)
         ops.wo_gemm(self.x, self.lm_head, self.gemm_ws, out=self.logits, pdl=self.pdl)
-        if self.tp_size == 1:
+        if self.W > 1:
+            if self.ngram > 0:
+                ops.ban_repeat_ngram(self.logits, self.hist, self.hist_len, self.ngram_size)
+            ops.beam_search_step(self.logits, self.beam_cum, self.W, workspace=self.beam_ws, out=self.beam_out)
+            self.fork()
+        elif self.tp_size == 1:
             ops.argmax(self.logits, out=self.next_ids)
             if self.q_len > 1:
                 ops.spec_verify(self.drafts, target_ids=self.next_ids.view(self.B, self.q_len), out_tokens=self.out_tokens,
                                 accepted=self.accepted)
         elif hasattr(self.comm, "argmax"):
             self.comm.argmax(self.logits, cfg.vocab, self.next_ids)     # vocab-parallel greedy sampling, own kernel
+
+    def fork(self):
+        """Beam mode, after beam_search_step: every row becomes the new beam of its slot (see the class docstring). Torch index
+        ops on static buffers only, so a CUDA graph replays it."""
+        o, T, M, cap = self.beam_out, self.cfg.tokens_per_block, self.M, self.hist.shape[1]
+        torch.add(self.row_base, o["next_parent"].view(-1), out=self.parent_row)
+        self.beam_cum.copy_(o["next_cum"])
+        # token history: the parent's row, then the new token
+        torch.index_select(self.hist, 0, self.parent_row, out=self.hist_parent)
+        torch.index_select(self.hist_len, 0, self.parent_row, out=self.len_parent)
+        self.hist.copy_(self.hist_parent)
+        self.pos.copy_(self.len_parent)
+        self.pos.clamp_(max=cap - 1)
+        self.hist.scatter_(1, self.pos.view(-1, 1), o["next_token"].view(-1, 1))
+        self.hist_len.copy_(self.pos)
+        self.hist_len.add_(1)
+        # page table: the parent's entries for the pages the step filled (q = (seq + 1) // T of them), the own pages after them
+        self.pos.copy_(self.seq_lens)
+        self.pos.add_(1)
+        self.pos.floor_divide_(T)
+        torch.lt(self.page_idx.view(1, -1), self.pos.view(-1, 1), out=self.full_mask)
+        torch.index_select(self.block_ids, 0, self.parent_row, out=self.blk_parent)
+        torch.where(self.full_mask, self.blk_parent, self.own_pages_i32, out=self.block_ids)
+        # the parent's partial page q into the own page q, two-phase (a parent may be another row's child); with no partial
+        # page (q == M) every row copies its own page onto itself
+        torch.lt(self.pos, M, out=self.partial)
+        self.pos.clamp_(max=M - 1)
+        torch.add(self.row_m, self.pos, out=self.dst_flat)
+        torch.mul(self.parent_row, M, out=self.src_flat)
+        self.src_flat.add_(self.pos)
+        torch.where(self.partial, self.src_flat, self.dst_flat, out=self.pick_flat)
+        own = self.own_pages_d.view(-1)
+        torch.index_select(own, 0, self.pick_flat, out=self.src_page)
+        torch.index_select(own, 0, self.dst_flat, out=self.dst_page)
+        for L in self.layers:
+            torch.index_select(L["kv"], 0, self.src_page, out=self.page_scratch)
+            L["kv"].index_copy_(0, self.dst_page, self.page_scratch)
+        self.ids.copy_(o["next_token"].view(-1))
+        self.seq_lens.add_(1)
 
     def step_tail(self):
         """TP > 1 with stock NCCL: gather the vocab-split logits and sample (torch plumbing, outside the program)."""
@@ -393,6 +514,7 @@ class DecodeStep:
 
     def step(self):
         """One decode step, op by op (one kernel per call)."""
+        self._count_beam_step()
         self.step_core()
         self.step_tail()
 
@@ -403,6 +525,9 @@ class DecodeStep:
         assert self.tp_size == 1 or isinstance(self.comm, tpmod.PeerComm), "a program cannot record NCCL calls"
         if self.q_len > 1:
             raise ValueError("a verification step (q_len > 1) runs op by op or under a CUDA graph, not as a decode program")
+        if self.W > 1:
+            raise ValueError("a beam-search step runs op by op or under a CUDA graph, not as a decode program (its fork is "
+                             "torch index ops, not C-ABI calls)")
         self.prog = ops.Program()
         with self.prog.record():
             self.step_core()
@@ -427,14 +552,19 @@ class DecodeStep:
         with torch.cuda.stream(s):
             for _ in range(2):
                 self.run()
+                if self.W > 1:              # a beam step advances its state: every warm-up starts from the prompt
+                    self.upload_inputs()
         torch.cuda.current_stream(self.dev).wait_stream(s)
         torch.cuda.synchronize(self.dev)
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
             self.run()
+        if self.W > 1:
+            self.upload_inputs()            # the recorded step has not run: the first replay is step 1
         torch.cuda.synchronize(self.dev)
 
     def replay(self):
+        self._count_beam_step()
         self.graph.replay()
 
     # ------------------------------------------------------------------ accounting (SURVEY 8d)

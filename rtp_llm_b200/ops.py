@@ -490,6 +490,76 @@ def spec_verify(draft_tokens: torch.Tensor, *, target_probs: Optional[torch.Tens
     return out_tokens, accepted
 
 
+_LOGIT_DTYPES = {torch.float16: 0, torch.bfloat16: 1, torch.float32: 2}
+
+
+def _logit_dtype(who: str, logits: torch.Tensor) -> int:
+    if logits.dtype not in _LOGIT_DTYPES:
+        raise B200Error(f"{who}: logits must be fp16, bf16 or fp32 (got {logits.dtype})")
+    return _LOGIT_DTYPES[logits.dtype]
+
+
+def beam_search_workspace(batch: int, beam_width: int, vocab: int, device) -> torch.Tensor:
+    """Zeroed workspace of b200_beam_search_step for up to `batch` requests (its counters reset themselves after every call)."""
+    n = int(_lib.load().b200_beam_search_step_workspace_bytes(batch, beam_width, vocab))
+    if n == 0:
+        raise B200Error(f"beam_search_step: unsupported shape batch {batch}, beam_width {beam_width}, vocab {vocab}")
+    return torch.zeros(n, dtype=torch.uint8, device=device)
+
+
+def beam_search_step(logits: torch.Tensor, cum_log_probs: torch.Tensor, beam_width: int, eos_id: int = -1,
+                     workspace: Optional[torch.Tensor] = None, out: Optional[dict] = None) -> dict:
+    """One beam-search step (b200_beam_search_step): logits [B*W, V] fp16 / bf16 / fp32 (row b*W + i = beam i of request b),
+    cum_log_probs fp32 [B, W]. Returns dict(cand_token, cand_parent, cand_score [B, 2W]: the top 2W candidates in rank order;
+    next_token, next_parent, next_cum [B, W]: the first W of them whose token is not eos_id). `out` may hold those six
+    tensors preallocated (graph capture); `workspace` comes from beam_search_workspace."""
+    W = beam_width
+    if not 1 <= W <= 32:
+        raise B200Error(f"beam_search_step: beam_width {W} unsupported (1..32)")
+    if logits.dim() != 2 or logits.shape[0] % W:
+        raise B200Error(f"beam_search_step: logits must be [B * {W}, V] (got {tuple(logits.shape)})")
+    dt = _logit_dtype("beam_search_step", logits)
+    rows, V = logits.shape
+    B = rows // W
+    if V < 2 * W:
+        raise B200Error(f"beam_search_step: vocab {V} must be >= 2 * beam_width ({2 * W})")
+    if cum_log_probs.dtype != torch.float32 or cum_log_probs.numel() != B * W:
+        raise B200Error(f"beam_search_step: cum_log_probs must be fp32 [{B}, {W}]")
+    dev = logits.device
+    shapes = dict(cand_token=(torch.int32, 2 * W), cand_parent=(torch.int32, 2 * W), cand_score=(torch.float32, 2 * W),
+                  next_token=(torch.int32, W), next_parent=(torch.int32, W), next_cum=(torch.float32, W))
+    out = dict(out or {})
+    for k, (dtype, n) in shapes.items():
+        if k not in out:
+            out[k] = torch.empty((B, n), dtype=dtype, device=dev)
+        elif out[k].dtype != dtype or out[k].numel() != B * n:
+            raise B200Error(f"beam_search_step: {k} must be {dtype} [{B}, {n}]")
+    if workspace is None:
+        workspace = beam_search_workspace(B, W, V, dev)
+    _cuda_contig(logits, cum_log_probs, workspace, *out.values())
+    check(_lib.load().b200_beam_search_step(_p(logits), dt, _p(cum_log_probs), B, W, V, eos_id, *(_p(out[k]) for k in shapes),
+                                            _p(workspace), workspace.numel(), _stream()), "b200_beam_search_step")
+    return out
+
+
+def ban_repeat_ngram(logits: torch.Tensor, history: torch.Tensor, hist_len: torch.Tensor, ngram_size: torch.Tensor) -> torch.Tensor:
+    """No-repeat-n-gram ban in place (b200_ban_repeat_ngram): logits [rows, V] fp16 / bf16 / fp32, history int32
+    [rows, stride], hist_len int32 [rows], ngram_size int32 [rows] (<= 0: off). Returns logits."""
+    dt = _logit_dtype("ban_repeat_ngram", logits)
+    if logits.dim() != 2:
+        raise B200Error(f"ban_repeat_ngram: logits must be [rows, V] (got {tuple(logits.shape)})")
+    rows, V = logits.shape
+    if history.dtype != torch.int32 or history.dim() != 2 or history.shape[0] != rows or history.shape[1] < 1:
+        raise B200Error(f"ban_repeat_ngram: history must be int32 [{rows}, stride >= 1]")
+    for name, t in (("hist_len", hist_len), ("ngram_size", ngram_size)):
+        if t.dtype != torch.int32 or t.numel() != rows:
+            raise B200Error(f"ban_repeat_ngram: {name} must be int32 [{rows}]")
+    _cuda_contig(logits, history, hist_len, ngram_size)
+    check(_lib.load().b200_ban_repeat_ngram(_p(logits), dt, rows, V, _p(history), _p(hist_len), history.shape[1], _p(ngram_size),
+                                            _stream()), "b200_ban_repeat_ngram")
+    return logits
+
+
 # ------------------------------------------------------------------------------------------------ decode programs
 class Program:
     """Recorded sequence of op calls (b200_program_*): `with prog.record(): <ops...>` then `prog.launch()` replays them

@@ -89,6 +89,28 @@ def bench_attn_multi(B, Hq, Hkv, S, q_len, T=64, nrot=3):
     return us
 
 
+def bench_beam(B, W, V=128256, ngram=0, hist=2048, nrot=8):
+    """b200_beam_search_step on fp16 logits [B*W, V] (rotated through nrot sets, > L2), preceded by b200_ban_repeat_ngram
+    over `hist` history tokens per row when ngram > 0."""
+    rows = B * W
+    g = torch.Generator(device=dev).manual_seed(1)
+    xs = [(torch.randn(rows, V, generator=g, device=dev) * 3).half() for _ in range(nrot)]
+    cum = -torch.rand(B, W, generator=g, device=dev)
+    ws = ops.beam_search_workspace(B, W, V, dev)
+    out = ops.beam_search_step(xs[0], cum, W, workspace=ws)
+    h = torch.randint(0, 64, (rows, hist), generator=g, device=dev, dtype=torch.int32)
+    hl = torch.full((rows,), hist, dtype=torch.int32, device=dev)
+    ng = torch.full((rows,), ngram, dtype=torch.int32, device=dev)
+
+    def fn(i):
+        if ngram > 0:
+            ops.ban_repeat_ngram(xs[i], h, hl, ng)
+        ops.beam_search_step(xs[i], cum, W, workspace=ws, out=out)
+    us = timeit(fn, nrot)
+    print(f"beam B{B} W{W} V{V}" + (f" + ban n{ngram} over {hist}" if ngram else "") + f": {us:8.1f} us", flush=True)
+    return us
+
+
 def bench_rope(kind, B, Hq, Hkv, q_len, S=2048, T=64, D=128, nrot=4):
     """RoPE + K/V append of q_len tokens per sequence at cached length S - q_len: b200_rope_append(_multi) ("base") against
     b200_rope_append_ex(_multi) with the Llama3 in-kernel formula ("llama3") or the Yarn cos/sin table ("yarn table").
@@ -205,6 +227,14 @@ if __name__ == "__main__":
         # speculative-token verification at group 8 (Qwen2-72B / Llama-3-70B): 8, 16, 32, 64 query rows per kv head
         t = {n: bench_attn_multi(32, 64, 8, 2048, n) for n in (1, 2, 4, 8)}
         print("attn-multi time relative to q_len 2 (16 rows): " + ", ".join(f"q_len {n}: {t[n] / t[2]:.2f}x" for n in t), flush=True)
+    if "beam" in which:
+        # beam search over Llama-3's vocabulary, with and without the 3-gram ban over 2048 history tokens, alternating
+        for B, W in ((8, 4), (32, 4), (4, 16)):
+            t = {n: [] for n in (0, 3)}
+            for _ in range(3):
+                for n in t:
+                    t[n].append(bench_beam(B, W, ngram=n))
+            print(f"beam B{B} W{W} V128256 median: step {sorted(t[0])[1]:.1f} us, ban n3 + step {sorted(t[3])[1]:.1f} us", flush=True)
     if "rope" in which:
         # Llama-3 shape (Hq 32, Hkv 8, D 128) at B 32: the Base-only kernel against the full-contract kernel, 1 and 4 tokens
         for n in (1, 4):
