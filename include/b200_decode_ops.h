@@ -280,6 +280,22 @@ int b200_beam_search_step(const void* logits, int dtype, const float* cum_log_pr
                           int32_t* cand_token, int32_t* cand_parent, float* cand_score, int32_t* next_token, int32_t* next_parent,
                           float* next_cum, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Per-token log-probabilities of the lm_head output (OpenAI-style logprobs / top_logprobs), without copying the probabilities
+ * to the host. logits [rows][vocab], dtype 0 fp16, 1 bf16, 2 fp32, read as they are. Each row's lp(i) = (x_i - m) - log sum_v
+ * exp(x_v - m) in fp32, m the row max: the log-softmax of the logits AS GIVEN, i.e. the raw model distribution before
+ * temperature, penalties and top-k / top-p (what b200_sample draws from is the filtered distribution; its token_prob_out is
+ * that one's renormalised probability). NaN logits count as -inf.
+ *   token_logprob [rows] = lp(tokens[r]) when tokens [rows] is given (NaN for an id outside [0, vocab));
+ *   top_ids int32 / top_logprobs fp32 [rows][top_n]: the top_n largest lp in descending order, equal values by lower id.
+ * top_n in 0..64 and <= vocab, with ceil(vocab / 4096) * top_n <= 4096 (at vocab 152064: top_n <= 64); vocab <= 2^26; rows <= 65535.
+ * A row without a finite logit gives NaN. Same grid and code as the first two levels of b200_beam_search_step: one CTA per
+ * 4096-logit chunk, the last one of a row to arrive merges the row's chunks in a fixed order. workspace:
+ * b200_token_logprobs_workspace_bytes(rows, vocab, top_n) bytes, ZERO on first use, left zero-ready by every call. One launch,
+ * deterministic, graph-capturable; under PDL it waits before reading anything. */
+size_t b200_token_logprobs_workspace_bytes(int rows, int vocab, int top_n);
+int b200_token_logprobs(const void* logits, int dtype, int rows, int vocab, int top_n, const int32_t* tokens, float* token_logprob,
+                        int32_t* top_ids, float* top_logprobs, void* workspace, size_t workspace_bytes, void* stream);
+
 /* No-repeat-n-gram ban, in place, before b200_sample or b200_beam_search_step (Hugging Face no_repeat_ngram_size over the whole
  * history the caller passes; restated, parity with the reference's banRepeatNgram kernel unpinned). history [rows][hist_stride]
  * and hist_len [rows] as b200_sample takes them (hist_len is clamped to hist_stride). For row r with n = ngram_size[r] > 0 and

@@ -1122,6 +1122,78 @@ int b200_beam_search_step(const void* logits, int dtype, const float* cum_log_pr
     return dtype == 2 ? launch(0.f) : by_dtype(dtype == 1, launch);
 }
 
+namespace {
+// Byte offsets of the log-prob kernel's workspace arrays (LogprobParams), each 256-byte aligned; total = 0 for an unsupported
+// shape.
+struct LogprobWorkspace {
+    size_t count, chunk_stat, chunk_val, chunk_idx, total;
+};
+LogprobWorkspace logprob_workspace(int rows, int vocab, int top_n) {
+    LogprobWorkspace w{};
+    const size_t S = vocab > 0 ? (vocab + kBeamChunk - 1) / kBeamChunk : 0;
+    if (rows < 0 || rows > 65535 || vocab < 1 || vocab > (1 << 26) || top_n < 0 || top_n > kLogprobMaxTopN || top_n > vocab ||
+        S * top_n > (size_t)kBeamMaxItems)
+        return w;
+    size_t o = 0;
+    auto take = [&](size_t bytes) {
+        const size_t at = o;
+        o = round_up(o + bytes, 256);
+        return at;
+    };
+    w.count = take((size_t)max(rows, 1) * 4);
+    w.chunk_stat = take((size_t)rows * S * 8);
+    w.chunk_val = take((size_t)rows * S * top_n * 4);
+    w.chunk_idx = take((size_t)rows * S * top_n * 4);
+    w.total = o;
+    return w;
+}
+}  // namespace
+
+size_t b200_token_logprobs_workspace_bytes(int rows, int vocab, int top_n) { return logprob_workspace(rows, vocab, top_n).total; }
+
+int b200_token_logprobs(const void* logits, int dtype, int rows, int vocab, int top_n, const int32_t* tokens, float* token_logprob,
+                        int32_t* top_ids, float* top_logprobs, void* workspace, size_t workspace_bytes, void* stream) {
+    ARG_CHECK(rows >= 0 && rows <= 65535, "token_logprobs: rows %d unsupported (0..65535)", rows);
+    ARG_CHECK(vocab > 0 && vocab <= (1 << 26), "token_logprobs: vocab %d unsupported (1..%d)", vocab, 1 << 26);
+    ARG_CHECK(top_n >= 0 && top_n <= kLogprobMaxTopN && top_n <= vocab, "token_logprobs: top_n %d unsupported (0..min(%d, vocab))",
+              top_n, kLogprobMaxTopN);
+    ARG_CHECK((size_t)(vocab + kBeamChunk - 1) / kBeamChunk * top_n <= (size_t)kBeamMaxItems,
+              "token_logprobs: vocab %d x top_n %d exceeds the row merge (ceil(vocab / %d) * top_n <= %d)", vocab, top_n, kBeamChunk,
+              kBeamMaxItems);
+    ARG_CHECK(dtype >= 0 && dtype <= 2, "token_logprobs: dtype %d unknown (0 fp16, 1 bf16, 2 fp32)", dtype);
+    if (rows == 0) return B200_OK;
+    ARG_CHECK(logits && (!tokens || token_logprob) && (top_n == 0 || (top_ids && top_logprobs)), "token_logprobs: null pointer");
+    const LogprobWorkspace w = logprob_workspace(rows, vocab, top_n);
+    ARG_CHECK(workspace && workspace_bytes >= w.total,
+              "token_logprobs: workspace too small (%zu < %zu bytes, see b200_token_logprobs_workspace_bytes)",
+              workspace ? workspace_bytes : (size_t)0, w.total);
+    if (g_rec)
+        return rec_call([=](void* st) {
+            return b200_token_logprobs(logits, dtype, rows, vocab, top_n, tokens, token_logprob, top_ids, top_logprobs, workspace,
+                                       workspace_bytes, st);
+        });
+    char* ws = static_cast<char*>(workspace);
+    LogprobParams p{};
+    p.logits = logits;
+    p.tokens = tokens;
+    p.token_logprob = token_logprob;
+    p.top_ids = top_ids;
+    p.top_logprobs = top_logprobs;
+    p.count = reinterpret_cast<uint32_t*>(ws + w.count);
+    p.chunk_stat = reinterpret_cast<float2*>(ws + w.chunk_stat);
+    p.chunk_val = reinterpret_cast<float*>(ws + w.chunk_val);
+    p.chunk_idx = reinterpret_cast<uint32_t*>(ws + w.chunk_idx);
+    p.V = vocab;
+    p.S = (vocab + kBeamChunk - 1) / kBeamChunk;
+    p.top_n = top_n;
+    const LaunchCfg cfg{dim3(p.S, rows), dim3(kBeamThreads), 0, (cudaStream_t)stream, g_pdl.load() != 0};
+    auto launch = [&](auto t) {
+        CUDA_CHECK(launch_ex(token_logprobs_kernel<decltype(t)>, cfg, p));
+        return launched("token_logprobs_kernel");
+    };
+    return dtype == 2 ? launch(0.f) : by_dtype(dtype == 1, launch);
+}
+
 int b200_ban_repeat_ngram(void* logits, int dtype, int rows, int vocab, const int32_t* history, const int32_t* hist_len, int hist_stride,
                           const int32_t* ngram_size, void* stream) {
     ARG_CHECK(rows >= 0 && rows <= 65535, "ban_repeat_ngram: rows %d unsupported (0..65535)", rows);

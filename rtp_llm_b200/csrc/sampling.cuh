@@ -434,91 +434,120 @@ __device__ __forceinline__ bool beam_arrive(uint32_t* counter, int of, int* s_fl
     return *s_flag;
 }
 
+// Shared memory of a chunk-and-merge top-K kernel (the beam step and the token log-probs): the staged items of one selection
+// and beam_select's scratch.
+struct TopkSmem {
+    uint32_t key[kBeamMaxItems], idx[kBeamMaxItems];
+    uint32_t sel_key[2 * kBeamMaxWidth], sel_idx[2 * kBeamMaxWidth];
+    uint32_t out_key[2 * kBeamMaxWidth], out_idx[2 * kBeamMaxWidth];
+    int red[2 * (kBeamThreads / 32)], n, flag;
+    float fred[kBeamThreads / 32];
+};
+
+// Level 1 of a chunk-and-merge top-K kernel, on the logits [v0, v0 + n) of one row: their max m and sum exp(x - m) to *stat,
+// and for K > 0 their top K keys (NaN ranks with -inf; every key -inf when `dead`; a short chunk padded to K items) to
+// val / idx [K] in rank order. Every store is st.cg, for the merge's ld.cg after the arrival counter.
+template <typename T>
+__device__ __forceinline__ void topk_chunk(const T* lg, int v0, int n, int K, bool dead, TopkSmem& sm, float2* stat, float* val,
+                                           uint32_t* idx) {
+    constexpr uint32_t kNegInf = 0x007FFFFFu;                  // beam_key(-inf)
+    const int tid = threadIdx.x;
+    float m = -INFINITY;
+    for (int j = tid; j < n; j += kBeamThreads) {
+        float x = to_f32<T>(lg[v0 + j]);
+        if (x != x) x = -INFINITY;                             // NaN ranks with the masked logits
+        m = fmaxf(m, x);
+        sm.key[j] = dead ? kNegInf : beam_key(x);
+        sm.idx[j] = v0 + j;
+    }
+    for (int j = n + tid; j < K; j += kBeamThreads) {           // a short last chunk: pad to K items
+        sm.key[j] = 0u;
+        sm.idx[j] = kBeamPad - j;
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((tid & 31) == 0) sm.fred[tid >> 5] = m;
+    __syncthreads();
+    m = -INFINITY;
+#pragma unroll
+    for (int w = 0; w < kBeamThreads / 32; ++w) m = fmaxf(m, sm.fred[w]);
+    // sum exp(x - m) from the staged keys (each thread reads its own): NaN counts as -inf here too, and a dead row, whose keys
+    // are all -inf, gets z = 0, which no score reads
+    float z = 0.f;
+    if (m > -INFINITY)
+        for (int j = tid; j < n; j += kBeamThreads) z += expf(beam_value(sm.key[j]) - m);
+#pragma unroll
+    for (int o = 16; o; o >>= 1) z += __shfl_xor_sync(0xffffffffu, z, o);
+    __syncthreads();
+    if ((tid & 31) == 0) sm.fred[tid >> 5] = z;
+    __syncthreads();
+    z = 0.f;
+#pragma unroll
+    for (int w = 0; w < kBeamThreads / 32; ++w) z += sm.fred[w];
+    if (K > 0) {
+        beam_select(max(n, K), K, sm.key, sm.idx, sm.sel_key, sm.sel_idx, sm.out_key, sm.out_idx, sm.red, &sm.n);
+        for (int r = tid; r < K; r += kBeamThreads) {
+            __stcg(val + r, beam_value(sm.out_key[r]));
+            __stcg(idx + r, sm.out_idx[r]);
+        }
+    }
+    if (tid == 0) __stcg(stat, make_float2(m, z));
+}
+
+// Level 2, in the last chunk CTA of a row to arrive: the row's top K of its S * K chunk survivors (val / idx [S][K]) into
+// sm.out_key / sm.out_idx in rank order (for K > 0), and the row's (max, sum exp) merged from its S chunk stats in chunk order,
+// returned in thread 0 only.
+__device__ __forceinline__ float2 topk_row_merge(int S, int K, int V, const float2* stat, const float* val, const uint32_t* idx,
+                                                 TopkSmem& sm) {
+    const int tid = threadIdx.x, n = S * K;
+    if (K > 0) {
+        for (int j = tid; j < n; j += kBeamThreads) {
+            const uint32_t x = __ldcg(idx + j);
+            sm.idx[j] = x;
+            sm.key[j] = x >= (uint32_t)V ? 0u : beam_key(__ldcg(val + j));
+        }
+        __syncthreads();
+        beam_select(n, K, sm.key, sm.idx, sm.sel_key, sm.sel_idx, sm.out_key, sm.out_idx, sm.red, &sm.n);
+    }
+    float m = -INFINITY, z = 0.f;
+    if (tid == 0) {
+        for (int s = 0; s < S; ++s) m = fmaxf(m, __ldcg(stat + s).x);
+        for (int s = 0; s < S; ++s) {
+            const float2 st = __ldcg(stat + s);
+            if (st.x > -INFINITY) z += st.y * expf(st.x - m);
+        }
+    }
+    return make_float2(m, z);
+}
+
 template <typename T>
 __global__ void __launch_bounds__(kBeamThreads) beam_search_kernel(const BeamParams p) {
-    __shared__ uint32_t s_key[kBeamMaxItems], s_idx[kBeamMaxItems];
-    __shared__ uint32_t s_sel_key[2 * kBeamMaxWidth], s_sel_idx[2 * kBeamMaxWidth];
-    __shared__ uint32_t s_out_key[2 * kBeamMaxWidth], s_out_idx[2 * kBeamMaxWidth];
-    __shared__ int s_red[2 * (kBeamThreads / 32)], s_n, s_flag;
-    __shared__ float s_fred[kBeamThreads / 32];
+    __shared__ TopkSmem sm;
     const int tid = threadIdx.x, c = blockIdx.x, row = blockIdx.y, W = p.W, V = p.V, S = p.S, K = 2 * W;
     const int b = row / W;
     pdl_wait();                        // under PDL the logits and cum come from the kernels before this one
-    constexpr uint32_t kNegInf = 0x007FFFFFu;                  // beam_key(-inf)
     auto dead = [&](int r) { return !(p.cum[r] > -INFINITY); };   // cum -inf (or NaN): every score of the row is -inf
 
     // ---- level 1: this chunk's top 2W keys and its (max, sum exp)
     {
-        const T* lg = reinterpret_cast<const T*>(p.logits) + (size_t)row * V;
-        const int v0 = c * kBeamChunk, n = min(kBeamChunk, V - v0);
-        const bool d = dead(row);
-        float m = -INFINITY;
-        for (int j = tid; j < n; j += kBeamThreads) {
-            float x = to_f32<T>(lg[v0 + j]);
-            if (x != x) x = -INFINITY;                         // NaN ranks with the masked logits
-            m = fmaxf(m, x);
-            s_key[j] = d ? kNegInf : beam_key(x);
-            s_idx[j] = v0 + j;
-        }
-        for (int j = n + tid; j < K; j += kBeamThreads) {       // a short last chunk: pad to 2W items
-            s_key[j] = 0u;
-            s_idx[j] = kBeamPad - j;
-        }
-#pragma unroll
-        for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-        if ((tid & 31) == 0) s_fred[tid >> 5] = m;
-        __syncthreads();
-        m = -INFINITY;
-#pragma unroll
-        for (int w = 0; w < kBeamThreads / 32; ++w) m = fmaxf(m, s_fred[w]);
-        // sum exp(x - m) from the staged keys (each thread reads its own): NaN counts as -inf here too, and a row with cum -inf,
-        // whose keys are all -inf, gets z = 0, which no score reads
-        float z = 0.f;
-        if (m > -INFINITY)
-            for (int j = tid; j < n; j += kBeamThreads) z += expf(beam_value(s_key[j]) - m);
-#pragma unroll
-        for (int o = 16; o; o >>= 1) z += __shfl_xor_sync(0xffffffffu, z, o);
-        __syncthreads();
-        if ((tid & 31) == 0) s_fred[tid >> 5] = z;
-        __syncthreads();
-        z = 0.f;
-#pragma unroll
-        for (int w = 0; w < kBeamThreads / 32; ++w) z += s_fred[w];
-        beam_select(max(n, K), K, s_key, s_idx, s_sel_key, s_sel_idx, s_out_key, s_out_idx, s_red, &s_n);
+        const int v0 = c * kBeamChunk;
         const size_t slot = (size_t)row * S + c;
-        for (int r = tid; r < K; r += kBeamThreads) {
-            __stcg(p.chunk_val + slot * K + r, beam_value(s_out_key[r]));
-            __stcg(p.chunk_idx + slot * K + r, s_out_idx[r]);
-        }
-        if (tid == 0) __stcg(p.chunk_stat + slot, make_float2(m, z));
+        topk_chunk(reinterpret_cast<const T*>(p.logits) + (size_t)row * V, v0, min(kBeamChunk, V - v0), K, dead(row), sm,
+                   p.chunk_stat + slot, p.chunk_val + slot * K, p.chunk_idx + slot * K);
     }
-    if (!beam_arrive(p.count + row, S, &s_flag)) return;
+    if (!beam_arrive(p.count + row, S, &sm.flag)) return;
 
     // ---- level 2 (last chunk of the row): the row's top 2W of the S * 2W chunk survivors, and the row's (max, sum exp)
     {
-        const int n = S * K;
-        for (int j = tid; j < n; j += kBeamThreads) {
-            const uint32_t x = __ldcg(p.chunk_idx + (size_t)row * n + j);
-            s_idx[j] = x;
-            s_key[j] = x >= (uint32_t)V ? 0u : beam_key(__ldcg(p.chunk_val + (size_t)row * n + j));
-        }
-        __syncthreads();
-        beam_select(n, K, s_key, s_idx, s_sel_key, s_sel_idx, s_out_key, s_out_idx, s_red, &s_n);
+        const float2 st = topk_row_merge(S, K, V, p.chunk_stat + (size_t)row * S, p.chunk_val + (size_t)row * S * K,
+                                         p.chunk_idx + (size_t)row * S * K, sm);
         for (int r = tid; r < K; r += kBeamThreads) {
-            __stcg(p.row_val + (size_t)row * K + r, beam_value(s_out_key[r]));
-            __stcg(p.row_idx + (size_t)row * K + r, s_out_idx[r]);
+            __stcg(p.row_val + (size_t)row * K + r, beam_value(sm.out_key[r]));
+            __stcg(p.row_idx + (size_t)row * K + r, sm.out_idx[r]);
         }
-        if (tid == 0) {
-            float m = -INFINITY, z = 0.f;
-            for (int s = 0; s < S; ++s) m = fmaxf(m, __ldcg(p.chunk_stat + (size_t)row * S + s).x);
-            for (int s = 0; s < S; ++s) {
-                const float2 st = __ldcg(p.chunk_stat + (size_t)row * S + s);
-                if (st.x > -INFINITY) z += st.y * expf(st.x - m);
-            }
-            __stcg(p.row_stat + row, make_float2(m, z));
-        }
+        if (tid == 0) __stcg(p.row_stat + row, st);
     }
-    if (!beam_arrive(p.count + gridDim.y + b, W, &s_flag)) return;
+    if (!beam_arrive(p.count + gridDim.y + b, W, &sm.flag)) return;
 
     // ---- level 3 (last row of the request): rank the W * 2W survivors by score, then by flat index i * V + v
     const int n = W * K;
@@ -529,28 +558,87 @@ __global__ void __launch_bounds__(kBeamThreads) beam_search_kernel(const BeamPar
         const float2 st = __ldcg(p.row_stat + r);
         const float cum = p.cum[r];
         const float score = (dead(r) || !(x > -INFINITY)) ? -INFINITY : cum + ((x - st.x) - logf(st.y));
-        s_key[j] = beam_key(score);
-        s_idx[j] = (uint32_t)i * (uint32_t)V + v;
+        sm.key[j] = beam_key(score);
+        sm.idx[j] = (uint32_t)i * (uint32_t)V + v;
     }
     __syncthreads();
-    beam_select(n, K, s_key, s_idx, s_sel_key, s_sel_idx, s_out_key, s_out_idx, s_red, &s_n);
+    beam_select(n, K, sm.key, sm.idx, sm.sel_key, sm.sel_idx, sm.out_key, sm.out_idx, sm.red, &sm.n);
     for (int r = tid; r < K; r += kBeamThreads) {
-        const uint32_t x = s_out_idx[r];
+        const uint32_t x = sm.out_idx[r];
         p.cand_token[b * K + r] = (int32_t)(x % (uint32_t)V);
         p.cand_parent[b * K + r] = (int32_t)(x / (uint32_t)V);
-        p.cand_score[b * K + r] = beam_value(s_out_key[r]);
+        p.cand_score[b * K + r] = beam_value(sm.out_key[r]);
     }
     if (tid == 0) {                    // the first W candidates that are not EOS (each row adds at most one EOS to the 2W)
         int taken = 0;
         for (int r = 0; r < K && taken < W; ++r) {
-            const uint32_t x = s_out_idx[r];
+            const uint32_t x = sm.out_idx[r];
             const int tok = (int)(x % (uint32_t)V);
             if (tok == p.eos) continue;
             p.next_token[b * W + taken] = tok;
             p.next_parent[b * W + taken] = (int)(x / (uint32_t)V);
-            p.next_cum[b * W + taken] = beam_value(s_out_key[r]);
+            p.next_cum[b * W + taken] = beam_value(sm.out_key[r]);
             ++taken;
         }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------ token log-probabilities
+// Per row of the [rows][V] lm_head logits, in fp32, lp(i) = (x_i - m) - log sum_v exp(x_v - m) with m the row max: the log-softmax
+// of the logits as given, i.e. the raw model distribution before temperature, penalties and top-k / top-p. Outputs the drawn
+// token's lp (token_logprob[r] = lp(tokens[r])) and the top_n largest lp of the row in descending order, equal values by lower
+// id. The grid and the code are the beam step's first two levels: (S = ceil(V / kBeamChunk), rows) CTAs each take their chunk's
+// (max, sum exp) and top top_n (topk_chunk), and the last CTA of a row to arrive at its self-resetting counter merges the row's
+// S partials in chunk order (topk_row_merge). NaN logits count as -inf; a token id outside [0, V) and a row without a finite
+// logit give NaN.
+struct LogprobParams {
+    const void* logits;       // [rows][V] fp16 / bf16 / fp32
+    const int32_t* tokens;    // optional [rows]
+    float* token_logprob;     // [rows] (with tokens)
+    int32_t* top_ids;         // [rows][top_n]
+    float* top_logprobs;      // [rows][top_n]
+    uint32_t* count;          // [rows] arrival counters, zero on entry and on exit
+    float2* chunk_stat;       // [rows][S]
+    float* chunk_val;         // [rows][S][top_n]
+    uint32_t* chunk_idx;      // [rows][S][top_n]
+    int V, S, top_n;
+};
+constexpr int kLogprobMaxTopN = 2 * kBeamMaxWidth;   // the selection's output slots (TopkSmem::out_key)
+
+template <typename T>
+__global__ void __launch_bounds__(kBeamThreads) token_logprobs_kernel(const LogprobParams p) {
+    __shared__ TopkSmem sm;
+    __shared__ float s_m, s_logz;
+    const int tid = threadIdx.x, c = blockIdx.x, row = blockIdx.y, V = p.V, S = p.S, K = p.top_n;
+    pdl_wait();                        // under PDL the logits and the tokens come from the kernels before this one
+    const T* lg = reinterpret_cast<const T*>(p.logits) + (size_t)row * V;
+    {
+        const int v0 = c * kBeamChunk;
+        const size_t slot = (size_t)row * S + c;
+        topk_chunk(lg, v0, min(kBeamChunk, V - v0), K, false, sm, p.chunk_stat + slot, p.chunk_val + slot * K,
+                   p.chunk_idx + slot * K);
+    }
+    if (!beam_arrive(p.count + row, S, &sm.flag)) return;
+
+    const float2 st = topk_row_merge(S, K, V, p.chunk_stat + (size_t)row * S, p.chunk_val + (size_t)row * S * K,
+                                     p.chunk_idx + (size_t)row * S * K, sm);
+    if (tid == 0) {
+        s_m = st.x;
+        s_logz = logf(st.y);
+        if (p.tokens) {
+            const int t = p.tokens[row];
+            float x = NAN;
+            if (t >= 0 && t < V) {
+                x = to_f32<T>(lg[t]);
+                if (x != x) x = -INFINITY;
+            }
+            p.token_logprob[row] = (x - st.x) - s_logz;
+        }
+    }
+    __syncthreads();
+    for (int r = tid; r < K; r += kBeamThreads) {
+        p.top_ids[(size_t)row * K + r] = (int32_t)sm.out_idx[r];
+        p.top_logprobs[(size_t)row * K + r] = (beam_value(sm.out_key[r]) - s_m) - s_logz;
     }
 }
 

@@ -13,7 +13,7 @@ from __future__ import annotations
 import dataclasses
 import math
 import os
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Sequence, Union
 
 import torch
 
@@ -48,6 +48,69 @@ LLAMA31_8B = ModelConfig("Llama-3.1-8B", 4096, 32, 32, 8, 128, 14336, 128256,
                          rope=RopeSpec(style=LLAMA3, dim=128, base=500000.0, scale=8.0, factor1=1.0, factor2=4.0, max_pos=8192))
 QWEN2_72B = ModelConfig("Qwen2-72B", 8192, 80, 64, 8, 128, 29696, 152064, rope_base=1000000.0, eps=1e-6)  # GPTQ-padded inter
 TINY = ModelConfig("tiny", 512, 2, 4, 2, 128, 512, 1024, tokens_per_block=16)
+
+
+@dataclasses.dataclass
+class SamplingParams:
+    """Per-request sampling parameters of DecodeStep's sampling mode: each field is one value for every request or a sequence of
+    one value per request, with b200_sample's meaning (top_k <= 0 and top_p >= 1: no limit; repetition 1, presence 0 and
+    frequency 0: off). seed fixes the step's uniforms (sampling_uniforms)."""
+    temperature: Union[float, Sequence[float]] = 1.0
+    top_k: Union[int, Sequence[int]] = 0
+    top_p: Union[float, Sequence[float]] = 1.0
+    repetition: Union[float, Sequence[float]] = 1.0
+    presence: Union[float, Sequence[float]] = 0.0
+    frequency: Union[float, Sequence[float]] = 0.0
+    seed: int = 0
+
+    def has_penalties(self) -> bool:
+        return any(any(float(v) != off for v in (x if isinstance(x, (list, tuple)) else [x]))
+                   for x, off in ((self.repetition, 1.0), (self.presence, 0.0), (self.frequency, 0.0)))
+
+
+_U32 = 0xFFFFFFFF
+
+
+def _mix32(x: torch.Tensor, tmp: torch.Tensor) -> None:
+    """A 32-bit integer hash, in place on int64 values in [0, 2^32): xor-shift / multiply rounds whose multipliers stay below
+    2^31, so no product leaves int64. tmp: scratch of x's shape."""
+    for shift, mul in ((16, 0x7FEB352D), (15, 0x2C1B3C6D), (16, 0)):
+        torch.bitwise_right_shift(x, shift, out=tmp)
+        x.bitwise_xor_(tmp)
+        if mul:
+            x.mul_(mul).bitwise_and_(_U32)
+
+
+class _Uniforms:
+    """n uniforms in [0, 1) per step, a pure function of (seed, step, i): u = (h(h(h(seed + 0x9E3779B9) ^ step) ^ i) >> 8) / 2^24
+    with h = _mix32 (all mod 2^32) and
+    `step` an int64 [1] tensor. Torch ops into static buffers only, so a CUDA graph replays them and each replay draws from the
+    step counter it finds on the device."""
+
+    def __init__(self, seed: int, n: int, device):
+        self.key = torch.tensor([(seed + 0x9E3779B9) & _U32], dtype=torch.int64, device=device)
+        self.k1, self.t1 = torch.empty_like(self.key), torch.empty_like(self.key)
+        _mix32(self.key, self.t1)
+        self.idx = torch.arange(n, dtype=torch.int64, device=device)
+        self.x, self.t = torch.empty_like(self.idx), torch.empty_like(self.idx)
+
+    def draw(self, step: torch.Tensor, out: torch.Tensor) -> None:
+        torch.bitwise_xor(self.key, step, out=self.k1)
+        _mix32(self.k1, self.t1)
+        torch.bitwise_xor(self.k1, self.idx, out=self.x)
+        _mix32(self.x, self.t)
+        self.x.bitwise_right_shift_(8)
+        out.copy_(self.x)
+        out.mul_(1.0 / (1 << 24))
+
+
+def sampling_uniforms(seed: int, step: int, n: int) -> torch.Tensor:
+    """The n uniforms (fp32, CPU) the sampling mode draws at `step` (0 = the first step since upload_inputs()): the first
+    B * q_len go to b200_sample's rows, at q_len > 1 the next B * q_len to b200_spec_verify."""
+    u = _Uniforms(seed, n, "cpu")
+    out = torch.empty(n, dtype=torch.float32)
+    u.draw(torch.tensor([step], dtype=torch.int64), out)
+    return out
 
 
 def _fmt(q: str) -> int:
@@ -90,13 +153,29 @@ class DecodeStep:
     gathered into scratch first, then scattered, since a beam can be a parent and a child in the same step). Then the ids
     become next_token and the lengths grow by one: the next call runs the next step. upload_inputs() restarts from the prompt;
     a step past max_new_tokens since then raises ValueError (the page-table rows end there), in run() and in replay().
-    The device state: beam_cum [B, W], hist [B*W, ctx] / hist_len [B*W], beam_out (the beam_search_step outputs)."""
+    The device state: beam_cum [B, W], hist [B*W, ctx] / hist_len [B*W], beam_out (the beam_search_step outputs).
+
+    sampling=SamplingParams (TP 1, beam_width 1, batch * q_len <= 128, op by op or under a CUDA graph; not in a decode program):
+    sampled decoding. The per-request parameters sit in static device buffers; after the lm_head the step copies the logits to a
+    static fp32 buffer (samp_logits: b200_sample works in place and leaves the probabilities there), runs ban_repeat_ngram when
+    no_repeat_ngram > 0, then b200_sample with the row's token history for the penalties. Its uniforms (one per row, `uniform`)
+    are drawn on the device inside the step from (seed, step since upload_inputs()), see sampling_uniforms, so every graph
+    replay draws new ones. With logprobs = n >= 0, b200_token_logprobs then scores the raw lm_head output: the drawn token's
+    log-prob and the top n (lp_out); with logprobs None it does not run.
+    At q_len 1 the step advances as the beam mode does: cum_log_probs += log(token_prob) (the reference's rule), the token
+    joins the history, ids become the drawn tokens and the lengths grow by one; upload_inputs() restarts from the prompt and a
+    step past max_new_tokens raises ValueError.
+    At q_len > 1 it verifies drafts by sampling: b200_sample runs over the B * q_len rows with probs_out into target_probs
+    [B, q_len, V], then spec_verify in sampling mode with deterministic drafts (draft_probs None) and its own uniforms [B, q_len].
+    Like the greedy verification step it does not advance. Penalties and the n-gram ban are rejected there: row j's history
+    would have to hold drafts 0..j-1."""
 
     def __init__(self, cfg: ModelConfig, batch: int, ctx: int, device: torch.device, tp_rank: int = 0, tp_size: int = 1,
                  dtype=torch.float16, seed: int = 0, keep_reference: bool = False, ragged: bool = False,
                  pdl: bool = False, comm=None, fuse_silu: bool = True, fuse_ar_norm: bool = True, fuse_rope: Optional[bool] = None,
                  fuse_gemm_rs: Optional[bool] = None, act_order: bool = False, q_len: int = 1, beam_width: int = 1,
-                 no_repeat_ngram: int = 0, max_new_tokens: int = 16):
+                 no_repeat_ngram: int = 0, max_new_tokens: int = 16, sampling: Optional[SamplingParams] = None,
+                 logprobs: Optional[int] = None):
         assert cfg.head_num % tp_size == 0 and cfg.inter % tp_size == 0
         if q_len < 1:
             raise ValueError(f"q_len must be >= 1 (got {q_len})")
@@ -108,12 +187,26 @@ class DecodeStep:
         if beam_width > 1 and (batch * beam_width > 128 or tp_size != 1 or q_len != 1):
             raise ValueError(f"beam search (beam_width {beam_width}) needs batch * beam_width <= 128 (the GEMM row limit), tp_size 1 "
                              f"and q_len 1 (got batch {batch}, tp_size {tp_size}, q_len {q_len})")
-        if beam_width > 1 and not 1 <= max_new_tokens < ctx:
+        if sampling is not None:
+            if tp_size != 1 or beam_width != 1 or batch * q_len > 128:
+                raise ValueError(f"sampling needs tp_size 1, beam_width 1 and batch * q_len <= 128 (the GEMM row limit) (got tp_size "
+                                 f"{tp_size}, beam_width {beam_width}, batch {batch}, q_len {q_len})")
+            if q_len > 1 and (sampling.has_penalties() or no_repeat_ngram != 0):
+                raise ValueError("sampled verification (q_len > 1) takes no penalties and no n-gram ban: row j's history would "
+                                 "have to hold drafts 0..j-1")
+            if logprobs is not None and not 0 <= logprobs <= ops.LOGPROB_MAX_TOP_N:
+                raise ValueError(f"logprobs must be in 0..{ops.LOGPROB_MAX_TOP_N} (got {logprobs})")
+        elif logprobs is not None:
+            raise ValueError("logprobs needs the sampling mode (sampling=SamplingParams(...))")
+        self.samp = sampling
+        self.logprobs = logprobs
+        self.sample_advances = sampling is not None and q_len == 1
+        if (beam_width > 1 or self.sample_advances) and not 1 <= max_new_tokens < ctx:
             raise ValueError(f"max_new_tokens must be in 1..ctx-1 (got {max_new_tokens}, ctx {ctx})")
-        if no_repeat_ngram != 0 and beam_width == 1:
+        if no_repeat_ngram != 0 and beam_width == 1 and sampling is None:
             raise ValueError(f"no_repeat_ngram {no_repeat_ngram} needs beam search (beam_width > 1); the greedy step has no ban")
         self.W, self.ngram, self.max_new_tokens = beam_width, no_repeat_ngram, max_new_tokens
-        self.beam_steps = 0                             # beam steps run since the prompt (upload_inputs)
+        self.beam_steps = 0                             # beam / sampled steps run since the prompt (upload_inputs)
         self.requests = batch
         batch = batch * beam_width                      # sequences (page-table rows) of the step
         self.q_len = q_len
@@ -275,6 +368,8 @@ class DecodeStep:
             lens = torch.full((batch,), ctx)
         if beam_width > 1:    # one prompt per request, room for max_new_tokens
             lens = (lens.view(-1, beam_width)[:, :1].expand(-1, beam_width).reshape(-1) - max_new_tokens + 1).clamp(min=1)
+        elif self.sample_advances:
+            lens = (lens - max_new_tokens + 1).clamp(min=1)
         self.seq_lens_h = (lens - q_len).to(torch.int32).pin_memory()   # tokens already cached (SURVEY a3)
         self.ids_h = torch.randint(0, cfg.vocab, (batch,) if q_len == 1 else (batch, q_len), generator=gp).to(torch.int32).pin_memory()
         if beam_width > 1:
@@ -341,6 +436,37 @@ class DecodeStep:
             self.hist_parent = buf(R, ctx, dt=torch.int32)
             self.len_parent = buf(R, dt=torch.int32)
             self.page_scratch = buf(R, 2, self.Hkv, T, self.D)
+        if sampling is not None:
+            def per_row(v, dt):
+                t = torch.tensor(v if isinstance(v, (list, tuple)) else [v] * batch, dtype=dt)
+                if t.numel() != batch:
+                    raise ValueError(f"sampling: {len(v)} values for {batch} requests")
+                return t.repeat_interleave(q_len).to(device)
+            sp = sampling
+            self.samp_params = dict(temperature=per_row(sp.temperature, torch.float32), top_k=per_row(sp.top_k, torch.int32),
+                                    top_p=per_row(sp.top_p, torch.float32))
+            if sp.has_penalties():
+                self.samp_params.update(repetition=per_row(sp.repetition, torch.float32), presence=per_row(sp.presence, torch.float32),
+                                        frequency=per_row(sp.frequency, torch.float32),
+                                        count_ws=torch.zeros(R, self.vocab, dtype=torch.int32, device=device))
+            self.samp_logits = buf(R, self.vocab, dt=torch.float32)
+            self.token_prob = buf(R, dt=torch.float32)
+            self.log_prob = buf(R, dt=torch.float32)
+            self.uniform = buf(R if q_len == 1 else 2 * R, dt=torch.float32)
+            self.draw_step = torch.zeros(1, dtype=torch.int64, device=device)
+            self.uniforms = _Uniforms(sp.seed, self.uniform.numel(), device)
+            if q_len == 1:
+                self.cum_log_probs = buf(R, dt=torch.float32)
+                self.hist = buf(R, ctx, dt=torch.int32)
+                self.hist_len = buf(R, dt=torch.int32)
+                self.ngram_size = torch.full((R,), no_repeat_ngram, dtype=torch.int32, device=device)
+                self.hist_pos = buf(R, dt=torch.int64)
+            else:
+                self.target_probs = buf(batch, q_len, self.vocab, dt=torch.float32)
+            if logprobs is not None:
+                self.lp_out = dict(token_logprob=buf(R, dt=torch.float32), top_ids=buf(R, logprobs, dt=torch.int32),
+                                   top_logprobs=buf(R, logprobs, dt=torch.float32))
+                self.lp_ws = ops.token_logprobs_workspace(R, self.vocab, logprobs, device)
         self.x_perm = buf(R, H) if act_order else None                        # x[:, perm] before qkv / w13
         self.attn_perm = buf(R, self.Hq * self.D) if act_order else None      # attn[:, perm] before o
         shapes = [(H, qkv_n), (self.Hq * self.D, H), (H, 2 * self.inter), (self.inter, H), (H, self.vocab)]
@@ -368,11 +494,20 @@ class DecodeStep:
             self.hist[:, 0].copy_(self.ids)
             self.hist_len.fill_(1)
             self.beam_steps = 0
+        if self.samp is not None:  # back to the prompt: step 0 of the uniforms; at q_len 1 the input token as the whole history
+            self.draw_step.zero_()
+            if self.q_len == 1:
+                self.cum_log_probs.zero_()
+                self.hist[:, 0].copy_(self.ids)
+                self.hist_len.fill_(1)
+                self.beam_steps = 0
+
+    sample_advances = False
 
     def _count_beam_step(self):
-        if self.W > 1:
+        if self.W > 1 or self.sample_advances:
             if self.beam_steps >= self.max_new_tokens:
-                raise ValueError(f"beam step {self.beam_steps + 1} since the prompt exceeds max_new_tokens {self.max_new_tokens}: "
+                raise ValueError(f"step {self.beam_steps + 1} since the prompt exceeds max_new_tokens {self.max_new_tokens}: "
                                  "call upload_inputs() to restart from the prompt")
             self.beam_steps += 1
 
@@ -458,6 +593,8 @@ class DecodeStep:
                 ops.ban_repeat_ngram(self.logits, self.hist, self.hist_len, self.ngram_size)
             ops.beam_search_step(self.logits, self.beam_cum, self.W, workspace=self.beam_ws, out=self.beam_out)
             self.fork()
+        elif self.samp is not None:
+            self.sample()
         elif self.tp_size == 1:
             ops.argmax(self.logits, out=self.next_ids)
             if self.q_len > 1:
@@ -505,6 +642,36 @@ class DecodeStep:
         self.ids.copy_(o["next_token"].view(-1))
         self.seq_lens.add_(1)
 
+    def sample(self):
+        """Sampling mode, after the lm_head (see the class docstring). b200 kernels and torch ops on static buffers only, so a CUDA
+        graph replays it."""
+        R, sp = self.B * self.q_len, self.samp_params
+        self.uniforms.draw(self.draw_step, self.uniform)
+        self.draw_step.add_(1)
+        self.samp_logits.copy_(self.logits)
+        adv = self.q_len == 1
+        if adv and self.ngram > 0:
+            ops.ban_repeat_ngram(self.samp_logits, self.hist, self.hist_len, self.ngram_size)
+        hist = dict(history=self.hist, hist_len=self.hist_len) if adv else {}
+        ops.sample(self.samp_logits, sp["top_k"], sp["top_p"], self.uniform[:R], temperature=sp["temperature"],
+                   repetition=sp.get("repetition"), presence=sp.get("presence"), frequency=sp.get("frequency"),
+                   count_ws=sp.get("count_ws"), out=dict(token=self.next_ids, token_prob=self.token_prob,
+                                                         **({} if adv else dict(probs=self.target_probs))), **hist)
+        if self.logprobs is not None:
+            ops.token_logprobs(self.logits, self.logprobs, tokens=self.next_ids, workspace=self.lp_ws, out=self.lp_out)
+        if not adv:
+            ops.spec_verify(self.drafts, target_probs=self.target_probs, uniform=self.uniform[R:], out_tokens=self.out_tokens,
+                            accepted=self.accepted)
+            return
+        torch.log(self.token_prob, out=self.log_prob)
+        self.cum_log_probs.add_(self.log_prob)
+        self.hist_pos.copy_(self.hist_len)
+        self.hist_pos.clamp_(max=self.hist.shape[1] - 1)
+        self.hist.scatter_(1, self.hist_pos.view(-1, 1), self.next_ids.view(-1, 1))
+        self.hist_len.add_(1)
+        self.ids.copy_(self.next_ids)
+        self.seq_lens.add_(1)
+
     def step_tail(self):
         """TP > 1 with stock NCCL: gather the vocab-split logits and sample (torch plumbing, outside the program)."""
         if self.tp_size > 1 and not hasattr(self.comm, "argmax"):
@@ -528,6 +695,9 @@ class DecodeStep:
         if self.W > 1:
             raise ValueError("a beam-search step runs op by op or under a CUDA graph, not as a decode program (its fork is "
                              "torch index ops, not C-ABI calls)")
+        if self.samp is not None:
+            raise ValueError("a sampling step runs op by op or under a CUDA graph, not as a decode program (its uniforms and "
+                             "state updates are torch ops, not C-ABI calls)")
         self.prog = ops.Program()
         with self.prog.record():
             self.step_core()
@@ -552,14 +722,14 @@ class DecodeStep:
         with torch.cuda.stream(s):
             for _ in range(2):
                 self.run()
-                if self.W > 1:              # a beam step advances its state: every warm-up starts from the prompt
+                if self.W > 1 or self.samp is not None:   # the state / the draw counter advance: every warm-up starts from the prompt
                     self.upload_inputs()
         torch.cuda.current_stream(self.dev).wait_stream(s)
         torch.cuda.synchronize(self.dev)
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
             self.run()
-        if self.W > 1:
+        if self.W > 1 or self.samp is not None:
             self.upload_inputs()            # the recorded step has not run: the first replay is step 1
         torch.cuda.synchronize(self.dev)
 

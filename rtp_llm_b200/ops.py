@@ -2,6 +2,7 @@
 libb200_decode.so. Every function launches on the current CUDA stream and is CUDA-graph capturable."""
 from __future__ import annotations
 
+import math
 from typing import Optional
 
 import torch
@@ -436,18 +437,25 @@ def sample(logits: torch.Tensor, top_k: torch.Tensor, top_p: torch.Tensor, unifo
            temperature: Optional[torch.Tensor] = None, history: Optional[torch.Tensor] = None,
            hist_len: Optional[torch.Tensor] = None, repetition: Optional[torch.Tensor] = None,
            presence: Optional[torch.Tensor] = None, frequency: Optional[torch.Tensor] = None,
-           process: Optional[torch.Tensor] = None, count_ws: Optional[torch.Tensor] = None, want_probs: bool = False):
+           process: Optional[torch.Tensor] = None, count_ws: Optional[torch.Tensor] = None, want_probs: bool = False,
+           out: Optional[dict] = None):
     """sampleGreedy's CUDA path (CudaSampleOp.cc:423-463) on fp32 logits [B, V], IN PLACE (logits become probabilities).
-    Returns (tokens int32 [B], token_prob fp32 [B], renormalised probs [B, V] or None)."""
-    _cuda_contig(logits, top_k, top_p, uniform, temperature, history, hist_len, repetition, presence, frequency, process, count_ws)
+    Returns (tokens int32 [B], token_prob fp32 [B], renormalised probs [B, V] or None). `out` may hold preallocated
+    token int32 [B], token_prob fp32 [B] and probs fp32 [B, V] (graph capture); a given probs implies want_probs."""
+    out = out or {}
+    B, V = logits.shape
+    for k, dtype, n in (("token", torch.int32, B), ("token_prob", torch.float32, B), ("probs", torch.float32, B * V)):
+        if k in out and (out[k].dtype != dtype or out[k].numel() != n):
+            raise B200Error(f"sample: out[{k!r}] must be {dtype} with {n} elements")
+    _cuda_contig(logits, top_k, top_p, uniform, temperature, history, hist_len, repetition, presence, frequency, process, count_ws,
+                 *out.values())
     if logits.dtype != torch.float32:
         raise B200Error("sample: logits must be fp32 (the reference sampler runs on fp32 logits)")
-    B, V = logits.shape
     if (repetition is not None or presence is not None or frequency is not None) and count_ws is None:
         count_ws = torch.zeros(B, V, dtype=torch.int32, device=logits.device)
-    tok = torch.empty(B, dtype=torch.int32, device=logits.device)
-    tprob = torch.empty(B, dtype=torch.float32, device=logits.device)
-    probs = torch.empty_like(logits) if want_probs else None
+    tok = out.get("token", torch.empty(B, dtype=torch.int32, device=logits.device))
+    tprob = out.get("token_prob", torch.empty(B, dtype=torch.float32, device=logits.device))
+    probs = out.get("probs", torch.empty_like(logits) if want_probs else None)
     check(_lib.load().b200_sample(_p(logits), B, V, _p(history), _p(hist_len), history.shape[1] if history is not None else 0,
                                   _p(count_ws), _p(temperature), _p(repetition), _p(presence), _p(frequency), _p(top_k), _p(top_p),
                                   _p(uniform), _p(process), _p(tok), _p(tprob), _p(probs), _stream()), "b200_sample")
@@ -539,6 +547,55 @@ def beam_search_step(logits: torch.Tensor, cum_log_probs: torch.Tensor, beam_wid
     _cuda_contig(logits, cum_log_probs, workspace, *out.values())
     check(_lib.load().b200_beam_search_step(_p(logits), dt, _p(cum_log_probs), B, W, V, eos_id, *(_p(out[k]) for k in shapes),
                                             _p(workspace), workspace.numel(), _stream()), "b200_beam_search_step")
+    return out
+
+
+LOGPROB_MAX_TOP_N = 64
+
+
+def token_logprobs_workspace(rows: int, vocab: int, top_n: int, device) -> torch.Tensor:
+    """Zeroed workspace of b200_token_logprobs (its counters reset themselves after every call)."""
+    n = int(_lib.load().b200_token_logprobs_workspace_bytes(rows, vocab, top_n))
+    if n == 0:
+        raise B200Error(f"token_logprobs: unsupported shape rows {rows}, vocab {vocab}, top_n {top_n}")
+    return torch.zeros(n, dtype=torch.uint8, device=device)
+
+
+def token_logprobs(logits: torch.Tensor, top_n: int = 0, tokens: Optional[torch.Tensor] = None,
+                   workspace: Optional[torch.Tensor] = None, out: Optional[dict] = None) -> dict:
+    """Log-probabilities of the raw lm_head output (b200_token_logprobs): logits [rows, V] fp16 / bf16 / fp32, log-softmax per row
+    in fp32 before any temperature, penalty or filter. Returns dict(token_logprob fp32 [rows] = lp of tokens int32 [rows], when
+    tokens is given; top_ids int32 / top_logprobs fp32 [rows, top_n]: the top_n largest, descending, equal values by lower id).
+    top_n in 0..64 (and <= V, ceil(V / 4096) * top_n <= 4096). `out` may hold the output tensors preallocated (graph capture);
+    `workspace` comes from token_logprobs_workspace."""
+    dt = _logit_dtype("token_logprobs", logits)
+    if logits.dim() != 2:
+        raise B200Error(f"token_logprobs: logits must be [rows, V] (got {tuple(logits.shape)})")
+    rows, V = logits.shape
+    if not 0 <= top_n <= min(LOGPROB_MAX_TOP_N, V) or (V + 4095) // 4096 * top_n > 4096:
+        raise B200Error(f"token_logprobs: top_n {top_n} unsupported (0..{LOGPROB_MAX_TOP_N}, <= vocab {V}, "
+                        f"ceil(vocab / 4096) * top_n <= 4096)")
+    if tokens is not None and (tokens.dtype != torch.int32 or tokens.numel() != rows):
+        raise B200Error(f"token_logprobs: tokens must be int32 [{rows}]")
+    dev = logits.device
+    shapes = dict(top_ids=(torch.int32, (rows, top_n)), top_logprobs=(torch.float32, (rows, top_n)))
+    if tokens is not None:
+        shapes["token_logprob"] = (torch.float32, (rows,))
+    out = dict(out or {})
+    for k, (dtype, shape) in shapes.items():
+        if k not in out:
+            out[k] = torch.empty(shape, dtype=dtype, device=dev)
+        elif out[k].dtype != dtype or out[k].numel() != math.prod(shape):
+            raise B200Error(f"token_logprobs: {k} must be {dtype} {list(shape)}")
+    need = int(_lib.load().b200_token_logprobs_workspace_bytes(rows, V, top_n))
+    if workspace is None:
+        workspace = token_logprobs_workspace(rows, V, top_n, dev)
+    elif workspace.dtype != torch.uint8 or workspace.numel() < need:
+        raise B200Error(f"token_logprobs: workspace must be uint8 of at least {need} bytes (token_logprobs_workspace)")
+    _cuda_contig(logits, tokens, workspace, *out.values())
+    check(_lib.load().b200_token_logprobs(_p(logits), dt, rows, V, top_n, _p(tokens), _p(out.get("token_logprob")),
+                                          _p(out["top_ids"]), _p(out["top_logprobs"]), _p(workspace), workspace.numel(), _stream()),
+          "b200_token_logprobs")
     return out
 
 

@@ -111,6 +111,40 @@ def bench_beam(B, W, V=128256, ngram=0, hist=2048, nrot=8):
     return us
 
 
+def bench_logprobs(B, top_n, V=128256, nrot=8):
+    """b200_token_logprobs on fp16 logits [B, V] (rotated through nrot sets, > L2): the drawn token's log-prob and the top_n."""
+    g = torch.Generator(device=dev).manual_seed(2)
+    xs = [(torch.randn(B, V, generator=g, device=dev) * 3).half() for _ in range(nrot)]
+    tok = torch.randint(0, V, (B,), generator=g, device=dev, dtype=torch.int32)
+    ws = ops.token_logprobs_workspace(B, V, top_n, dev)
+    out = ops.token_logprobs(xs[0], top_n, tokens=tok, workspace=ws)
+    us = timeit(lambda i: ops.token_logprobs(xs[i], top_n, tokens=tok, workspace=ws, out=out), nrot)
+    print(f"logprobs B{B} V{V} top_n {top_n}: {us:8.1f} us  {B * V * 2 / us / 1e3:7.0f} GB/s", flush=True)
+    return us
+
+
+def bench_sample(B, top_k, top_p, V=128256, nrot=4, copy_only=False):
+    """b200_sample on fp32 logits [B, V] at temperature 0.8 with every row's top_k / top_p. The op works in place, so each call
+    first copies fresh logits into its buffer (rotated through nrot sources); copy_only times that copy alone."""
+    g = torch.Generator(device=dev).manual_seed(3)
+    src = [torch.randn(B, V, generator=g, device=dev) * 3 for _ in range(nrot)]
+    x = torch.empty(B, V, device=dev)
+    k = torch.full((B,), top_k, dtype=torch.int32, device=dev)
+    p = torch.full((B,), top_p, device=dev)
+    t = torch.full((B,), 0.8, device=dev)
+    u = torch.rand(B, generator=g, device=dev)
+    out = dict(token=torch.empty(B, dtype=torch.int32, device=dev), token_prob=torch.empty(B, device=dev))
+
+    def fn(i):
+        x.copy_(src[i])
+        if not copy_only:
+            ops.sample(x, k, p, u, temperature=t, out=out)
+    us = timeit(fn, nrot)
+    what = "copy alone" if copy_only else f"copy + sample top_k {top_k} top_p {top_p}"
+    print(f"sample B{B} V{V} {what}: {us:8.1f} us", flush=True)
+    return us
+
+
 def bench_rope(kind, B, Hq, Hkv, q_len, S=2048, T=64, D=128, nrot=4):
     """RoPE + K/V append of q_len tokens per sequence at cached length S - q_len: b200_rope_append(_multi) ("base") against
     b200_rope_append_ex(_multi) with the Llama3 in-kernel formula ("llama3") or the Yarn cos/sin table ("yarn table").
@@ -235,6 +269,19 @@ if __name__ == "__main__":
                 for n in t:
                     t[n].append(bench_beam(B, W, ngram=n))
             print(f"beam B{B} W{W} V128256 median: step {sorted(t[0])[1]:.1f} us, ban n3 + step {sorted(t[3])[1]:.1f} us", flush=True)
+    if "logprobs" in which:
+        # the log-prob kernel over Llama-3's vocabulary at B 32: the drawn token's log-prob alone, and with the top 5 / 20
+        t = {n: sorted(bench_logprobs(32, n) for _ in range(3))[1] for n in (0, 5, 20)}
+        print("logprobs B32 V128256 median: " + ", ".join(f"top_n {n}: {v:.1f} us" for n, v in t.items()), flush=True)
+    if "sample" in which:
+        # b200_sample alone (one 1024-thread CTA per row, bisection passes over the vocabulary): top-k 50 and top-p 0.9 each
+        # and together, minus the logit copy the in-place op needs before every call
+        for B in (8, 32):
+            c = sorted(bench_sample(B, 0, 1.0, copy_only=True) for _ in range(3))[1]
+            for k, p in ((50, 1.0), (0, 0.9), (50, 0.9)):
+                m = sorted(bench_sample(B, k, p) for _ in range(3))[1]
+                print(f"sample B{B} V128256 top_k {k} top_p {p} median: {m - c:.1f} us (copy + sample {m:.1f}, copy {c:.1f})",
+                      flush=True)
     if "rope" in which:
         # Llama-3 shape (Hq 32, Hkv 8, D 128) at B 32: the Base-only kernel against the full-contract kernel, 1 and 4 tokens
         for n in (1, 4):
