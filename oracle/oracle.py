@@ -189,6 +189,155 @@ def attn_error_budget(ref: np.ndarray, E: np.ndarray, is_bf16: bool) -> np.ndarr
 
 
 # ----------------------------------------------------------------------------------------------
+# Weight-only GEMM: float64 reference, error budget and exact rounding
+# ----------------------------------------------------------------------------------------------
+def round_t(x, is_bf16: bool) -> np.ndarray:
+    """float64 -> the nearest fp16 / bf16 value, ties to even, rounded ONCE (returned as float64). Subnormals are kept,
+    values past the largest finite number by half an ulp or more become +-inf, NaN stays NaN. numpy's float64 -> float16
+    cast is the same single rounding; a float64 -> float32 -> bf16 chain rounds twice and can differ at ties."""
+    mant, emin, emax = (7, -126, 127) if is_bf16 else (10, -14, 15)
+    x = np.asarray(x, np.float64)
+    _, e = np.frexp(x)                                         # x = m * 2^e, 0.5 <= |m| < 1: floor(log2 |x|) = e - 1, exactly
+    q = np.ldexp(1.0, np.maximum(e - 1, emin) - mant)          # the spacing of T at |x|
+    r = np.round(x / q) * q                                    # x / q is exact (q a power of two); np.round ties to even
+    r = np.where(np.abs(r) > (2.0 - 2.0 ** -mant) * 2.0 ** emax, np.copysign(np.inf, x), r)
+    return np.where(np.isfinite(x), r, x)
+
+
+def f64_to_bits(x, is_bf16: bool) -> np.ndarray:
+    """float64 -> fp16 / bf16 bit patterns (uint16) with the one rounding of round_t."""
+    r = round_t(x, is_bf16)
+    if is_bf16:
+        return (r.astype(np.float32).view(np.uint32) >> 16).astype(np.uint16)   # r is a bf16 value: the float32 cast is exact
+    return r.astype(np.float16).view(np.uint16)
+
+
+def _vals(a, is_bf16: bool) -> np.ndarray:
+    """fp16 / bf16 values as float64, from uint16 bit patterns or from any float array that already holds T values."""
+    a = np.asarray(a)
+    return from_bits(a, is_bf16).astype(np.float64) if a.dtype == np.uint16 else a.astype(np.float64)
+
+
+def dequant_exact(fmt: str, weight, scales=None, zeros_x_scales=None, group: int = 128, is_bf16=False) -> np.ndarray:
+    """The weight W' [K,N] the GEMM's tensor cores multiply, in float64 (every value exactly a T value):
+      * int4 (group 128 / 64 / 32) and int8g: W' = round_T(q_s * s + zs), ONE rounding, as hfma2(q_s, s, zs) in the kernel
+        (Dequant4, dequant_half). q_s (<= 8 bits) * s (<= 11) is exact in float64, and so is the sum with zs at any exponent
+        gap below 2^30, so the only rounding is round_t's. The group of row k is k // group.
+      * int8 per-column: W' = q_s, exact; the column scale is the epilogue's (gemm_np's cscale).
+      * f16: W' = W.
+    weight: int4 uint8 [K,N/2] (low nibble = even column); int8 / int8g int8 [K,N]; f16 the values or their bits.
+    scales / zeros_x_scales [K/group, N]: the values (as float) or their uint16 bits. Unlike dequant_np, nothing passes through
+    float32 on the way."""
+    if fmt == "f16":
+        return _vals(weight, is_bf16)
+    if fmt == "int8":
+        return np.asarray(weight).astype(np.float64)
+    if fmt not in ("int4", "int8g"):
+        raise ValueError(fmt)
+    q = unpack_int4_signed(weight) if fmt == "int4" else np.asarray(weight)
+    s = np.repeat(_vals(scales, is_bf16), group, axis=0)
+    z = np.repeat(_vals(zeros_x_scales, is_bf16), group, axis=0)
+    return round_t(q.astype(np.float64) * s + z, is_bf16)
+
+
+def gemm_np(x, w_deq, cscale=None, bias=None) -> Tuple[np.ndarray, np.ndarray]:
+    """Float64 Y = (X . W') * cscale + bias and the size of its terms A = (|X| . |W'|) * |cscale| + |bias| (both [B,N]).
+    x [B,K], w_deq [K,N] (dequant_exact), cscale / bias [N] or None; all float values (T values in practice)."""
+    x = np.asarray(x, np.float64)
+    w = np.asarray(w_deq, np.float64)
+    ref, A = x @ w, np.abs(x) @ np.abs(w)
+    if cscale is not None:
+        c = np.asarray(cscale, np.float64)[None, :]
+        ref, A = ref * c, A * np.abs(c)
+    if bias is not None:
+        b = np.asarray(bias, np.float64)[None, :]
+        ref, A = ref + b, A + np.abs(b)
+    return ref, A
+
+
+def gemm_fp32_error(A: np.ndarray, K: int, nsplit: int = 1) -> np.ndarray:
+    """Bound on |v - ref| for the fp32 value v the GEMM's epilogue holds before its final rounding to T (see
+    gemm_error_budget): 2^-24 * (272 * kbp + nsplit) * A, kbp = the k-blocks of the longest split."""
+    kb = -(-int(K) // 128)
+    kbp = -(-kb // max(int(nsplit), 1))
+    return 2.0 ** -24 * (272 * kbp + nsplit) * np.asarray(A, np.float64)
+
+
+def gemm_error_budget(ref: np.ndarray, A: np.ndarray, K: int, nsplit: int, is_bf16: bool) -> np.ndarray:
+    """Per-element bound on |y - ref| for a correct weight-only GEMM in T = fp16 / bf16, against gemm_np's (ref, A):
+    ulp_T(ref) + c * A,  c = 2^-24 * (272 * kbp + nsplit),  kbp = ceil(ceil(K / 128) / nsplit).
+
+    Why: every product x_k * W'_k is exact in fp32 (two T significands, <= 22 bits). A split of kbp k-blocks accumulates them
+    in 8 * kbp tensor-core k16 steps, each adding 16 products to the fp32 accumulator. How the hardware rounds inside that
+    sum is not documented, so the bound assumes the worst of a 24-bit adder without guard bits: the 17 addends (the
+    accumulator and 16 products) are aligned to the largest exponent E and each of the 16 shifted ones is truncated to a
+    multiple of 2^(E-23), losing up to 2^(E-23) <= 2^-23 * max|addend| each; the sum is then normalised to 24 bits by
+    truncation, losing up to another 2^-23 of its magnitude. Every addend and every running sum is at most A (the sum of
+    |terms|), so one step loses at most 17 * 2^-23 * A = 34 * 2^-24 * A, and the chain of 8 * kbp steps 272 * kbp * 2^-24 * A.
+    The nsplit fp32 partials are merged in a fixed order with round-to-nearest adds (nsplit - 1 of them, 2^-24 * A each),
+    and the epilogue's fmaf(acc, cscale, bias) rounds once more (2^-24 * A). The one final rounding to T costs half an
+    ulp_T; ulp_T(ref) leaves room for the value crossing a binade. A call whose split is not known may pass nsplit = 1:
+    that bound is the loosest for any split <= 16. The one assumption is that the adder keeps at least fp32's 24 bits
+    at the largest addend's exponent; a narrower window is not an fp32 accumulation.
+
+    The bound grows with K because it is a worst case; a kernel rounding to nearest and summing random-signed terms stays
+    far below it. gemm_rounded_fractions is the sharper check for that regime. Measured on an H100 80GB HBM3 (700 W power
+    limit): see DESIGN section 4 for the worst err/budget per path and dtype; everywhere it is below 0.5 -- the final
+    rounding's half ulp, with the fp32 error far below c * A."""
+    return ulp(ref, is_bf16) + gemm_fp32_error(A, K, nsplit)
+
+
+def _ordinal(bits: np.ndarray) -> np.ndarray:
+    """fp16 / bf16 bit patterns -> integers in the order of their values, adjacent values one apart (+0 and -0 both 0)."""
+    b = np.asarray(bits, np.uint16).astype(np.int32)
+    mag = b & 0x7FFF
+    return np.where(b & 0x8000, -mag, mag)
+
+
+# Thresholds of gemm_rounded_fractions for random data (see its docstring for the measured values they leave room below).
+GEMM_MIN_ROUNDED = 0.9
+GEMM_MIN_WITHIN_ONE = 0.99
+
+
+def gemm_rounded_fractions(got, ref, is_bf16: bool) -> Tuple[float, float]:
+    """(fraction of outputs equal to round_T(ref), fraction at most one T step away from it). got: the kernel's output as
+    T values or uint16 bits; ref: gemm_np's float64 result.
+
+    An fp32 kernel's accumulation error is small next to ulp_T(y) for all but the outputs much smaller than their terms
+    (|y| << A), so it rounds almost every output correctly and hardly any by more than one step. A kernel that rounds its
+    split partials or W' twice adds an error of a good fraction of an ulp_T to most outputs, which the worst-case budget
+    still allows at large K, and drops well below both thresholds. At the Llama-3-8B w2 shape (B 32, K 14336, INT4,
+    tests/test_gemm_budget.py) a simulated round-to-nearest fp32 kernel gives 0.998 / 0.9998 (fp16, unsplit) and
+    0.9996 / 0.99998 (bf16); the two double-rounding mutants give 0.56-0.59 / 0.86-0.88. On an H100 80GB HBM3 (700 W
+    power limit), over the 289 random-data GEMM cases of the suite, the kernels gave at least 0.980 / 0.9974. Thresholds
+    GEMM_MIN_ROUNDED = 0.9 / GEMM_MIN_WITHIN_ONE = 0.99 leave room below that and stay above the mutants."""
+    g = np.asarray(got)
+    gb = g if g.dtype == np.uint16 else f64_to_bits(g.astype(np.float64), is_bf16)
+    rb = f64_to_bits(ref, is_bf16)
+    d = np.abs(_ordinal(gb) - _ordinal(rb))
+    bad = np.isnan(from_bits(gb, is_bf16))
+    return float(((d == 0) & ~bad).mean()), float(((d <= 1) & ~bad).mean())
+
+
+def silu_mul_np(g: np.ndarray, u: np.ndarray) -> np.ndarray:
+    """Float64 silu(g) * u."""
+    return g / (1.0 + np.exp(-g)) * u
+
+
+def silu_mul_budget(g, Ag, u, Au, K: int, nsplit: int, is_bf16: bool) -> np.ndarray:
+    """Bound on |y - silu(g) u| for the fused SiLU*mul epilogue, from the float64 gate / up (g, Ag), (u, Au) of gemm_np. The
+    kernel evaluates __fdividef(g, 1 + __expf(-g)) * u on its fp32 g, u (each within e = gemm_fp32_error of the reference)
+    and rounds once to T. |silu'| <= 1.1 everywhere, so the inputs' errors move the result by at most
+    1.1 e_g (|u| + e_u) + |silu(g)| e_u; __expf is within 2 + 1.16 |g| fp32 ulps and the divide within 2 ulps, the multiply
+    half an ulp, so the evaluation adds at most 2^-23 (6 + 2 |g|) |result|; the final rounding is within ulp_T."""
+    g, u = np.asarray(g, np.float64), np.asarray(u, np.float64)
+    eg, eu = gemm_fp32_error(Ag, K, nsplit), gemm_fp32_error(Au, K, nsplit)
+    ref = silu_mul_np(g, u)
+    sg = g / (1.0 + np.exp(-g))
+    return ulp(ref, is_bf16) + 1.1 * eg * (np.abs(u) + eu) + np.abs(sg) * eu + 2.0 ** -23 * (6 + 2 * np.abs(g)) * np.abs(ref)
+
+
+# ----------------------------------------------------------------------------------------------
 # Weight-only quantisation
 # ----------------------------------------------------------------------------------------------
 def unpack_groupwise_int4(qweight, qzeros, scales_f16, group: int, is_gptq: bool):

@@ -334,6 +334,59 @@ def make_w8g(K, N, seed=1, simple=False):
     return q, s, zs
 
 
+def _bits16(t):
+    return t.detach().cpu().contiguous().view(torch.int16).numpy().view(np.uint16)
+
+
+def _f64(t, is_bf16):
+    return None if t is None else orc.from_bits(_bits16(t), is_bf16).astype(np.float64)
+
+
+def gemm_nsplit(K, N, program):
+    """The split the budget may assume: the cluster kernel's plan (B200_GEMM_SPLITK included), 1 for the persistent kernel
+    (its run plan is not exposed; 1 gives the loosest bound)."""
+    if program:
+        return 1
+    import ctypes
+    from rtp_llm_b200 import _lib
+    ns, kbp = ctypes.c_int(), ctypes.c_int()
+    _lib.check(_lib.load().b200_plan_gemm_split(K, N, ctypes.byref(ns), ctypes.byref(kbp)), "b200_plan_gemm_split")
+    return ns.value
+
+
+def gemm_vs_f64(name, y, x, w_deq, nsplit, is_bf16, cscale=None, bias=None):
+    """The primary GEMM check: every output within oracle.gemm_error_budget of the float64 reference of W' = w_deq
+    (oracle.dequant_exact), and the correctly rounded fractions above their thresholds. x / cscale / bias: device tensors."""
+    ref, A = orc.gemm_np(_f64(x, is_bf16), w_deq, _f64(cscale, is_bf16), _f64(bias, is_bf16))
+    got = _bits16(y).reshape(ref.shape)
+    gv = orc.from_bits(got, is_bf16).astype(np.float64)
+    ratio = np.abs(gv - ref) / orc.gemm_error_budget(ref, A, w_deq.shape[0], nsplit, is_bf16)
+    ratio[np.isnan(ratio)] = np.inf
+    eq, one = orc.gemm_rounded_fractions(got, ref, is_bf16)
+    bad = ratio > 1.0
+    ok = not bad.any() and eq >= orc.GEMM_MIN_ROUNDED and one >= orc.GEMM_MIN_WITHIN_ONE
+    info = f"worst err/budget={ratio.max():.3f} rounded={eq:.5f} within_one={one:.6f} bad={int(bad.sum())}/{ratio.size}"
+    if bad.any():
+        idx = np.flatnonzero(bad)[:6]
+        info += " first_bad=" + ", ".join(f"{i}:{gv.flat[i]:.5g}/{ref.flat[i]:.5g}" for i in idx)
+    report(name + " [kernel vs float64, error budget]", ok, info)
+
+
+def silu_vs_f64(name, y, x, w_deq, nsplit, is_bf16, cscale=None):
+    """The fused SiLU*mul epilogue against silu(g) u of the float64 gate / up GEMMs (w_deq in the reference column order:
+    gate columns, then up), within oracle.silu_mul_budget."""
+    inter = w_deq.shape[1] // 2
+    xv, cs = _f64(x, is_bf16), _f64(cscale, is_bf16)
+    g, Ag = orc.gemm_np(xv, w_deq[:, :inter], None if cs is None else cs[:inter])
+    u, Au = orc.gemm_np(xv, w_deq[:, inter:], None if cs is None else cs[inter:])
+    ref = orc.silu_mul_np(g, u)
+    gv = orc.from_bits(_bits16(y).reshape(ref.shape), is_bf16).astype(np.float64)
+    ratio = np.abs(gv - ref) / orc.silu_mul_budget(g, Ag, u, Au, w_deq.shape[0], nsplit, is_bf16)
+    ratio[np.isnan(ratio)] = np.inf
+    report(name + " [fused silu*mul vs float64, error budget]", not (ratio > 1.0).any(),
+           f"worst err/budget={ratio.max():.3f} bad={int((ratio > 1.0).sum())}/{ratio.size}")
+
+
 def run_gemm(name, x, w, ws, program, **kw):
     """One wo_gemm call; program=True records it into a decode program and launches that, so it runs in the persistent
     kernel (it must become the program's one fused op)."""
@@ -392,6 +445,18 @@ def gemm_case(name, fmt, B, K, N, dtype=torch.float16, simple=False, onehot=Fals
             buf, y = guarded_empty((B, N), dtype)
             run_gemm(name, x, w, ws, program, bias=bias_t, out=y)
             torch.cuda.synchronize()
+            is_bf16 = dtype == torch.bfloat16
+            if fmt == B200_FMT_INT4:
+                w_deq = orc.dequant_exact("int4", qp, _bits16(sd), _bits16(zd), 128, is_bf16)
+            elif fmt == B200_FMT_INT8G:
+                w_deq = orc.dequant_exact("int8g", q8, _bits16(sd), _bits16(zd), 128, is_bf16)
+            elif fmt == B200_FMT_INT8:
+                w_deq = orc.dequant_exact("int8", q8)
+            else:
+                w_deq = orc.dequant_exact("f16", _bits16(wd), is_bf16=is_bf16)
+            gemm_vs_f64(name, y, x, w_deq, gemm_nsplit(K, N, program), is_bf16,
+                        cscale=sd if fmt == B200_FMT_INT8 else None, bias=bias_t)
+            # second opinions: the naive GPU kernel and the C oracle, at the reference's tolerance
             tol = 2e-2 if fmt == B200_FMT_INT4 else 1e-2
             if dtype == torch.bfloat16:
                 tol = 4e-2
@@ -420,7 +485,8 @@ def gemm_case(name, fmt, B, K, N, dtype=torch.float16, simple=False, onehot=Fals
 
 
 def gemm_silu_case(name, fmt, B, K, inter, dtype=torch.float16, env=None, program=False):
-    """w13 GEMM with the fused SiLU*mul epilogue vs oracle (GEMM on the un-permuted weight, then silu_and_mul)."""
+    """w13 GEMM with the fused SiLU*mul epilogue against silu(g) u of the float64 GEMM within oracle.silu_mul_budget, and
+    the C oracle (GEMM on the un-permuted weight, then silu_and_mul) as a second opinion."""
     def fn():
         with env_set(env):
             rng = np.random.default_rng(9)
@@ -453,6 +519,16 @@ def gemm_silu_case(name, fmt, B, K, inter, dtype=torch.float16, env=None, progra
             buf, y = guarded_empty((B, inter), dtype)
             run_gemm(name, x, w, ws, program, silu_mul=True, out=y)
             torch.cuda.synchronize()
+            is_bf16 = dtype == torch.bfloat16
+            if fmt == B200_FMT_INT4:
+                w_deq = orc.dequant_exact("int4", qp, bits(sd), bits(zd), 128, is_bf16)
+            elif fmt == B200_FMT_INT8G:
+                w_deq = orc.dequant_exact("int8g", q8, bits(sd), bits(zd), 128, is_bf16)
+            elif fmt == B200_FMT_INT8:
+                w_deq = orc.dequant_exact("int8", q8)
+            else:
+                w_deq = orc.dequant_exact("f16", bits(wd), is_bf16=is_bf16)
+            silu_vs_f64(name, y, x, w_deq, gemm_nsplit(K, N, program), is_bf16, cscale=sd if fmt == B200_FMT_INT8 else None)
             ok, info = diff_info(y, exp, 2e-2, 2e-2)
             report(name + " [fused silu*mul vs oracle]", ok, info)
             report_bands(name, buf)

@@ -106,6 +106,10 @@ def _gemm_vs_refs(group, B, K, N, dtype=torch.float16, bias=False, env=None):
         ref = refk.ref_dequant_gemm(x, B200_FMT_INT4, qd, sd, zd, group, bias_t)
         torch.cuda.synchronize()
     is_bf16 = dtype == torch.bfloat16
+    with probe.env_set(env):
+        nsplit = probe.gemm_nsplit(K, N, False)
+    probe.gemm_vs_f64(name, y, x, orc.dequant_exact("int4", qp, bits(sd), bits(zd), group, is_bf16), nsplit, is_bf16, bias=bias_t)
+    # second opinions: the naive GPU kernel and the C oracle, at the reference's tolerance
     tol = 4e-2 if is_bf16 else 2e-2
     probe.report(name + " [kernel vs ref-kernel]", *probe.diff_info(y, ref.float().cpu().numpy(), tol, tol))
     exp = orc.dequant_gemm(bits(x), "int4", qp, scales=bits(sd), zeros_x_scales=bits(zd), group=group,
@@ -208,6 +212,9 @@ def test_fused_silu_mul(group, env):
         torch.cuda.synchronize()
     gu = orc.dequant_gemm(bits(x), "int4", qp, scales=bits(sd), zeros_x_scales=bits(zd), group=group)
     probe.RESULTS.clear()
+    with probe.env_set(env):
+        nsplit = probe.gemm_nsplit(K, N, False)
+    probe.silu_vs_f64("silu", y, x, orc.dequant_exact("int4", qp, bits(sd), bits(zd), group), nsplit, False)
     probe.report("silu", *probe.diff_info(y, orc.from_bits(orc.silu_and_mul(gu), False), 2e-2, 2e-2))
     probe.report_bands("silu", buf)
     bad = [n for n, ok in probe.RESULTS if not ok]
