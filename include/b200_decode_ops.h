@@ -222,6 +222,21 @@ int b200_rope_append_ex_multi(const void* qkv, const void* qkv_bias, void* q_out
                               int cache_positions, const b200_rope_config* cfg, int use_logn_attn, int is_bf16, int batch,
                               int head_num, int kv_head_num, int head_dim, int max_blocks_per_seq, int page_size, int q_len,
                               void* stream);
+/* QK-RMSNorm (Qwen3's q_norm / k_norm) + RoPE + K/V append in one launch: b200_rope_append_multi / b200_rope_append_ex_multi
+ * after each q and k head of qkv is RMS-normalised with q_gamma / k_gamma [head_dim] and eps. q_out and the K/V pool get the
+ * bits of b200_qk_rmsnorm(copy of qkv, q_gamma, k_gamma, NULL, NULL, ..., eps) followed by the rope entry on that copy; v
+ * heads are copied as they are and qkv is only read. q_len >= 1 tokens per sequence (1: the one-token entries' rules).
+ * head_dim % 64 == 0 and <= 256; both gammas required; no qkv bias (it belongs to the qkv GEMM, before the norm). Inside a
+ * decode program each is its own launch (the persistent kernel's rope op does not normalise). */
+int b200_qk_norm_rope_append(const void* qkv, const void* q_gamma, const void* k_gamma, float eps, void* q_out, void* kv_pool,
+                             const int32_t* page_list, const int32_t* sequence_lengths, int is_bf16, int batch, int head_num,
+                             int kv_head_num, int head_dim, int max_blocks_per_seq, int page_size, float rope_base, int q_len,
+                             void* stream);
+int b200_qk_norm_rope_append_ex(const void* qkv, const void* q_gamma, const void* k_gamma, float eps, void* q_out, void* kv_pool,
+                                const int32_t* page_list, const int32_t* sequence_lengths, const int32_t* position_ids,
+                                const float* cos_sin_cache, int cache_positions, const b200_rope_config* cfg, int use_logn_attn,
+                                int is_bf16, int batch, int head_num, int kv_head_num, int head_dim, int max_blocks_per_seq,
+                                int page_size, int q_len, void* stream);
 /* embedding gather out[b] = table[ids[b]] (rtp_ops.embedding). */
 int b200_embedding(const int32_t* ids, const void* table, void* out, int is_bf16, int rows, int hidden, void* stream);
 /* greedy sampling: out[r] = argmax(logits[r]) (lowest index on ties; CudaSampleOp.cc:330,453). dtype: 0 fp16, 1 bf16, 2 fp32 */

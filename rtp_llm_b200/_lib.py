@@ -46,6 +46,9 @@ SIGNATURES = {
     "b200_rope_append_multi": (c_int, [c_void_p] * 5 + [c_int] * 7 + [c_float, c_int, c_void_p]),
     "b200_rope_append_ex": (c_int, [c_void_p] * 8 + [c_int, c_void_p] + [c_int] * 8 + [c_void_p]),
     "b200_rope_append_ex_multi": (c_int, [c_void_p] * 8 + [c_int, c_void_p] + [c_int] * 9 + [c_void_p]),
+    "b200_qk_norm_rope_append": (c_int, [c_void_p] * 3 + [c_float] + [c_void_p] * 4 + [c_int] * 7 + [c_float, c_int, c_void_p]),
+    "b200_qk_norm_rope_append_ex": (c_int, [c_void_p] * 3 + [c_float] + [c_void_p] * 6 + [c_int, c_void_p] + [c_int] * 9
+                                    + [c_void_p]),
     "b200_embedding": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "b200_argmax": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "b200_sample": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int] + [c_void_p] * 13),

@@ -217,19 +217,60 @@ __global__ void silu_and_mul_kernel(const T* __restrict__ gate_up, T* __restrict
     }
 }
 
+// ---- QK-RMSNorm inside the rope kernels (the QKN instances below; Qwen3's q_norm / k_norm before RoPE)
+// A rope CTA of D/2 threads holds one q or k head, thread i channels i and i + D/2. qk_rmsnorm_kernel's sum runs over a warp
+// whose lane l holds the pairs (2l + 64m, 2l + 1 + 64m), so the head is staged in shared memory and EVERY warp of the CTA forms
+// that sum in that order (xor butterfly: all lanes end with the same bits) -- one barrier, no second broadcast. Then each
+// channel is round_T(v * scale * gamma), the value b200_qk_rmsnorm would have left in qkv, and the rotation reads that.
+// D % 64 == 0 and D <= kQkNormMaxD (checked on the host).
+constexpr int kQkNormMaxD = 256;
+
+template <typename T>
+__device__ __forceinline__ float qk_norm_scale(const T* __restrict__ src, int head_dim, float eps) {
+    __shared__ uint32_t s_head[kQkNormMaxD / 2];
+    T* s = reinterpret_cast<T*>(s_head);
+    const int i = threadIdx.x, lane = threadIdx.x & 31, half = head_dim / 2;
+    s[i] = src[i];
+    s[i + half] = src[i + half];
+    __syncthreads();
+    float ss = 0.f;
+    for (int c = lane * 2; c < head_dim; c += 64) {
+        const float2 v = unpack2<T>(s_head[c / 2]);
+        ss = fmaf(v.x, v.x, fmaf(v.y, v.y, ss));
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+    return rsqrtf(ss / (float)head_dim + eps);
+}
+
+template <typename T>
+__device__ __forceinline__ float qk_norm_apply(T v, float scale, T g) {
+    return to_f32<T>(from_f32<T>(to_f32<T>(v) * scale * to_f32<T>(g)));
+}
+
 // Decode RoPE (NeoX pairing, RopeStyle::Base, angle = pos * base^(-2i/dim)) + K,V append into the paged cache.
 // Contract: SURVEY.md appendix C; call site /root/reference/rtp_llm/ops/fused_rope_kvcache_op.py:202-246.
 // q_len new tokens per sequence (speculative-token verification): row x of qkv [B*q_len] is token j = x % q_len of sequence
 // b = x / q_len, rotated and appended at position seq_lens[b] + j; q_out [B*q_len][Hq*D].
 // grid (B*q_len, Hq + 2*Hkv), D/2 threads. MULTI = false is the one-token instance (q_len == 1, no division by q_len).
-template <typename T, bool MULTI = false>
-__global__ void rope_append_kernel(const T* __restrict__ qkv, T* __restrict__ q_out, T* __restrict__ kv_pool,
-                                   const int32_t* __restrict__ page_list, const int32_t* __restrict__ seq_lens,
-                                   int head_num, int kv_head_num, int head_dim, int max_blocks, int tokens_per_block,
-                                   float log2_base, int q_len) {
+// QKN: q and k heads are RMS-normalised first (qk_norm_scale); the bits of b200_qk_rmsnorm followed by this kernel.
+template <typename T, bool MULTI, bool QKN>
+__device__ __forceinline__ void rope_append_body(const T* __restrict__ qkv, T* __restrict__ q_out, T* __restrict__ kv_pool,
+                                                 const int32_t* __restrict__ page_list, const int32_t* __restrict__ seq_lens,
+                                                 int head_num, int kv_head_num, int head_dim, int max_blocks, int tokens_per_block,
+                                                 float log2_base, int q_len, const T* __restrict__ q_gamma,
+                                                 const T* __restrict__ k_gamma, float eps) {
     pdl_launch_dependents();
-    pdl_wait();
     const int x = blockIdx.x, h = blockIdx.y, i = threadIdx.x, half = head_dim / 2;
+    T g0, g1;   // QKN: the gammas are weights, constant after load, so they are read before the PDL wait
+    if constexpr (QKN) {
+        if (h < head_num + kv_head_num) {
+            const T* gamma = h < head_num ? q_gamma : k_gamma;
+            g0 = gamma[i];
+            g1 = gamma[i + half];
+        }
+    }
+    pdl_wait();
     const int b = MULTI ? x / q_len : x;
     const int pos = seq_lens[b] + (MULTI ? x % q_len : 0);
     const T* src = qkv + ((size_t)x * (head_num + 2 * kv_head_num) + h) * head_dim;
@@ -245,11 +286,16 @@ __global__ void rope_append_kernel(const T* __restrict__ qkv, T* __restrict__ q_
         dst = kv_pool + (size_t)page * page_elems + ((size_t)kvh * tokens_per_block + pos % tokens_per_block) * head_dim;
         rotate = !is_v;
     }
-    const float x0 = to_f32<T>(src[i]), x1 = to_f32<T>(src[i + half]);
+    float x0 = to_f32<T>(src[i]), x1 = to_f32<T>(src[i + half]);
     if (rotate) {
         const float inv_freq = exp2f(-2.0f * (float)i / (float)head_dim * log2_base);
         float sn, cs;
         sincosf((float)pos * inv_freq, &sn, &cs);
+        if constexpr (QKN) {   // q or k head (uniform over the CTA: the barrier inside is safe), after the angle
+            const float scale = qk_norm_scale<T>(src, head_dim, eps);
+            x0 = qk_norm_apply<T>(src[i], scale, g0);
+            x1 = qk_norm_apply<T>(src[i + half], scale, g1);
+        }
         float r0, r1;
         rope_rotate(x0, x1, cs, sn, r0, r1);
         dst[i] = from_f32<T>(r0);
@@ -258,6 +304,26 @@ __global__ void rope_append_kernel(const T* __restrict__ qkv, T* __restrict__ q_
         dst[i] = src[i];
         dst[i + half] = src[i + half];
     }
+}
+
+template <typename T, bool MULTI = false>
+__global__ void rope_append_kernel(const T* __restrict__ qkv, T* __restrict__ q_out, T* __restrict__ kv_pool,
+                                   const int32_t* __restrict__ page_list, const int32_t* __restrict__ seq_lens,
+                                   int head_num, int kv_head_num, int head_dim, int max_blocks, int tokens_per_block,
+                                   float log2_base, int q_len) {
+    rope_append_body<T, MULTI, false>(qkv, q_out, kv_pool, page_list, seq_lens, head_num, kv_head_num, head_dim, max_blocks,
+                                      tokens_per_block, log2_base, q_len, nullptr, nullptr, 0.f);
+}
+
+// rope_append_kernel with QK-RMSNorm: q_gamma / k_gamma [head_dim], no bias.
+template <typename T, bool MULTI = false>
+__global__ void qk_norm_rope_append_kernel(const T* __restrict__ qkv, T* __restrict__ q_out, T* __restrict__ kv_pool,
+                                           const int32_t* __restrict__ page_list, const int32_t* __restrict__ seq_lens,
+                                           int head_num, int kv_head_num, int head_dim, int max_blocks, int tokens_per_block,
+                                           float log2_base, int q_len, const T* __restrict__ q_gamma,
+                                           const T* __restrict__ k_gamma, float eps) {
+    rope_append_body<T, MULTI, true>(qkv, q_out, kv_pool, page_list, seq_lens, head_num, kv_head_num, head_dim, max_blocks,
+                                     tokens_per_block, log2_base, q_len, q_gamma, k_gamma, eps);
 }
 
 
@@ -327,12 +393,15 @@ __device__ __forceinline__ float2 rope_coef(const RopeCfg& c, int zid, int pos) 
 // rotated at position_ids[x] (when > 0) or that slot. q_len rides in gridDim.z so both instances share one parameter block.
 // Everything after the row / slot / position choice is the one-token arithmetic: token j gives the bits of a one-token call at
 // seq_lens + j.
-template <typename T, bool MULTI = false>
-__global__ void rope_append_ex_kernel(const T* __restrict__ qkv, const T* __restrict__ bias, T* __restrict__ q_out,
-                                      T* __restrict__ kv_pool, const int32_t* __restrict__ page_list,
-                                      const int32_t* __restrict__ seq_lens, const int32_t* __restrict__ position_ids,
-                                      const float2* __restrict__ cos_sin_cache, int cache_positions, RopeCfg cfg, int use_logn,
-                                      int head_num, int kv_head_num, int head_dim, int max_blocks, int tokens_per_block) {
+// QKN: q and k heads are RMS-normalised first (qk_norm_scale; no bias); the bits of b200_qk_rmsnorm followed by this kernel.
+template <typename T, bool MULTI, bool QKN>
+__device__ __forceinline__ void rope_append_ex_body(const T* __restrict__ qkv, const T* __restrict__ bias, T* __restrict__ q_out,
+                                                    T* __restrict__ kv_pool, const int32_t* __restrict__ page_list,
+                                                    const int32_t* __restrict__ seq_lens, const int32_t* __restrict__ position_ids,
+                                                    const float2* __restrict__ cos_sin_cache, int cache_positions, const RopeCfg& cfg,
+                                                    int use_logn, int head_num, int kv_head_num, int head_dim, int max_blocks,
+                                                    int tokens_per_block, const T* __restrict__ q_gamma,
+                                                    const T* __restrict__ k_gamma, float eps) {
     pdl_launch_dependents();
     pdl_wait();
     const int b = blockIdx.x, h = blockIdx.y, i = threadIdx.x, half = head_dim / 2, rhalf = cfg.dim / 2;
@@ -354,7 +423,16 @@ __global__ void rope_append_ex_kernel(const T* __restrict__ qkv, const T* __rest
         rotate = rotate && !is_v;
     }
     // thread i owns the channel pair (i, i + dim/2) for i < dim/2, and the pass-through channels dim + i, dim + i + (head_dim-dim)/2 ...
+    float scale = 0.f;
+    const T* gamma = is_q ? q_gamma : k_gamma;
+    const bool norm = QKN && !(h >= head_num + kv_head_num);   // q or k head (uniform over the CTA: the barrier inside is safe)
+    if constexpr (QKN) {
+        if (norm) scale = qk_norm_scale<T>(src, head_dim, eps);
+    }
     auto load = [&](int c) {
+        if constexpr (QKN) {
+            if (norm) return qk_norm_apply<T>(src[c], scale, gamma[c]);
+        }
         float v = to_f32<T>(src[c]);
         if (bsrc) v = to_f32<T>(from_f32<T>(v + to_f32<T>(bsrc[c])));
         return v;
@@ -381,6 +459,31 @@ __global__ void rope_append_ex_kernel(const T* __restrict__ qkv, const T* __rest
         if (is_q && use_logn && pos > cfg.max_pos) v *= logf((float)(pos + 1)) / logf((float)cfg.max_pos);
         dst[c] = from_f32<T>(v);
     }
+}
+
+template <typename T, bool MULTI = false>
+__global__ void rope_append_ex_kernel(const T* __restrict__ qkv, const T* __restrict__ bias, T* __restrict__ q_out,
+                                      T* __restrict__ kv_pool, const int32_t* __restrict__ page_list,
+                                      const int32_t* __restrict__ seq_lens, const int32_t* __restrict__ position_ids,
+                                      const float2* __restrict__ cos_sin_cache, int cache_positions, RopeCfg cfg, int use_logn,
+                                      int head_num, int kv_head_num, int head_dim, int max_blocks, int tokens_per_block) {
+    rope_append_ex_body<T, MULTI, false>(qkv, bias, q_out, kv_pool, page_list, seq_lens, position_ids, cos_sin_cache,
+                                         cache_positions, cfg, use_logn, head_num, kv_head_num, head_dim, max_blocks,
+                                         tokens_per_block, nullptr, nullptr, 0.f);
+}
+
+// rope_append_ex_kernel with QK-RMSNorm: q_gamma / k_gamma [head_dim]; qkv carries no bias (it belongs to the qkv GEMM, before
+// the norm).
+template <typename T, bool MULTI = false>
+__global__ void qk_norm_rope_append_ex_kernel(const T* __restrict__ qkv, T* __restrict__ q_out, T* __restrict__ kv_pool,
+                                              const int32_t* __restrict__ page_list, const int32_t* __restrict__ seq_lens,
+                                              const int32_t* __restrict__ position_ids, const float2* __restrict__ cos_sin_cache,
+                                              int cache_positions, RopeCfg cfg, int use_logn, int head_num, int kv_head_num,
+                                              int head_dim, int max_blocks, int tokens_per_block, const T* __restrict__ q_gamma,
+                                              const T* __restrict__ k_gamma, float eps) {
+    rope_append_ex_body<T, MULTI, true>(qkv, nullptr, q_out, kv_pool, page_list, seq_lens, position_ids, cos_sin_cache,
+                                        cache_positions, cfg, use_logn, head_num, kv_head_num, head_dim, max_blocks,
+                                        tokens_per_block, q_gamma, k_gamma, eps);
 }
 
 // Column gather y[r][j] = x[r][perm[j]] (the activation side of a GPTQ act-order weight whose rows were sorted by g_idx).

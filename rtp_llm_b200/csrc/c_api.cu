@@ -824,19 +824,21 @@ int b200_permute_cols(const void* x, const int32_t* perm, void* y, int is_bf16, 
     return launched("permute_cols_kernel");
 }
 
+// q_gamma / k_gamma non-null: QK-RMSNorm first (qk_norm_rope_append_kernel), always its own launch inside a decode program.
 static int rope_append_impl(const void* qkv, void* q_out, void* kv_pool, const int32_t* page_list, const int32_t* sequence_lengths,
                             int is_bf16, int batch, int q_len, int head_num, int kv_head_num, int head_dim, int max_blocks_per_seq,
-                            int page_size, float rope_base, void* stream) {
+                            int page_size, float rope_base, const void* q_gamma, const void* k_gamma, float eps, void* stream) {
     if (batch == 0) return B200_OK;
     ARG_CHECK(qkv && q_out && kv_pool && page_list && sequence_lengths, "rope_append: null pointer");
     ARG_CHECK(head_dim > 0 && head_dim % 2 == 0 && head_dim <= 512, "rope_append: head_dim %d unsupported", head_dim);
     ARG_CHECK(rope_base > 1.f, "rope_append: rope_base must be > 1");
     ARG_CHECK(batch > 0 && q_len >= 1 && (long)batch * q_len <= 0x7fffffffL, "rope_append: bad shape batch %d x q_len %d", batch, q_len);
+    const bool qkn = q_gamma != nullptr;
     const float l2b = std::log2(rope_base);
-    if (g_rec && q_len > 1)   // its own launch: the persistent kernel's rope op appends one token per sequence
+    if (g_rec && (q_len > 1 || qkn))   // its own launch: the persistent kernel's rope op appends one token per sequence, unnormed
         return rec_call([=](void* st) {
             return rope_append_impl(qkv, q_out, kv_pool, page_list, sequence_lengths, is_bf16, batch, q_len, head_num, kv_head_num,
-                                    head_dim, max_blocks_per_seq, page_size, rope_base, st);
+                                    head_dim, max_blocks_per_seq, page_size, rope_base, q_gamma, k_gamma, eps, st);
         });
     if (g_rec) {
         ProgOp op{};
@@ -859,8 +861,14 @@ static int rope_append_impl(const void* qkv, void* q_out, void* kv_pool, const i
     const bool pdl = g_pdl.load() != 0;
     return by_dtype(is_bf16, [&](auto t) {
         using T = decltype(t);
-        CUDA_CHECK(launch_ex(q_len > 1 ? rope_append_kernel<T, true> : rope_append_kernel<T, false>,
-                             {grid, dim3(head_dim / 2), 0, (cudaStream_t)stream, pdl}, (const T*)qkv,
+        const LaunchCfg lc{grid, dim3(head_dim / 2), 0, (cudaStream_t)stream, pdl};
+        if (qkn) {
+            CUDA_CHECK(launch_ex(q_len > 1 ? qk_norm_rope_append_kernel<T, true> : qk_norm_rope_append_kernel<T, false>, lc,
+                                 (const T*)qkv, (T*)q_out, (T*)kv_pool, page_list, sequence_lengths, head_num, kv_head_num, head_dim,
+                                 (int)max_blocks_per_seq, page_size, l2b, q_len, (const T*)q_gamma, (const T*)k_gamma, eps));
+            return launched("qk_norm_rope_append_kernel");
+        }
+        CUDA_CHECK(launch_ex(q_len > 1 ? rope_append_kernel<T, true> : rope_append_kernel<T, false>, lc, (const T*)qkv,
                              (T*)q_out, (T*)kv_pool, page_list, sequence_lengths, head_num, kv_head_num, head_dim,
                              (int)max_blocks_per_seq, page_size, l2b, q_len));
         return launched("rope_append_kernel");
@@ -871,7 +879,7 @@ int b200_rope_append(const void* qkv, void* q_out, void* kv_pool, const int32_t*
                      const int32_t* sequence_lengths, int is_bf16, int batch, int head_num, int kv_head_num,
                      int head_dim, int max_blocks_per_seq, int page_size, float rope_base, void* stream) {
     return rope_append_impl(qkv, q_out, kv_pool, page_list, sequence_lengths, is_bf16, batch, 1, head_num, kv_head_num, head_dim,
-                            max_blocks_per_seq, page_size, rope_base, stream);
+                            max_blocks_per_seq, page_size, rope_base, nullptr, nullptr, 0.f, stream);
 }
 
 int b200_rope_append_multi(const void* qkv, void* q_out, void* kv_pool, const int32_t* page_list,
@@ -879,14 +887,26 @@ int b200_rope_append_multi(const void* qkv, void* q_out, void* kv_pool, const in
                            int head_dim, int max_blocks_per_seq, int page_size, float rope_base, int q_len, void* stream) {
     ARG_CHECK(q_len >= 1, "rope_append_multi: q_len %d must be >= 1", q_len);
     return rope_append_impl(qkv, q_out, kv_pool, page_list, sequence_lengths, is_bf16, batch, q_len, head_num, kv_head_num, head_dim,
-                            max_blocks_per_seq, page_size, rope_base, stream);
+                            max_blocks_per_seq, page_size, rope_base, nullptr, nullptr, 0.f, stream);
 }
 
+int b200_qk_norm_rope_append(const void* qkv, const void* q_gamma, const void* k_gamma, float eps, void* q_out, void* kv_pool,
+                             const int32_t* page_list, const int32_t* sequence_lengths, int is_bf16, int batch, int head_num,
+                             int kv_head_num, int head_dim, int max_blocks_per_seq, int page_size, float rope_base, int q_len,
+                             void* stream) {
+    ARG_CHECK(q_gamma && k_gamma, "qk_norm_rope_append: null gamma");
+    ARG_CHECK(head_dim % 64 == 0 && head_dim <= kQkNormMaxD, "qk_norm_rope_append: head_dim %d must be 64, 128 or 256", head_dim);
+    ARG_CHECK(q_len >= 1, "qk_norm_rope_append: q_len %d must be >= 1", q_len);
+    return rope_append_impl(qkv, q_out, kv_pool, page_list, sequence_lengths, is_bf16, batch, q_len, head_num, kv_head_num, head_dim,
+                            max_blocks_per_seq, page_size, rope_base, q_gamma, k_gamma, eps, stream);
+}
+
+// q_gamma / k_gamma non-null (qkv_bias null): QK-RMSNorm first (qk_norm_rope_append_ex_kernel).
 static int rope_append_ex_impl(const void* qkv, const void* qkv_bias, void* q_out, void* kv_pool, const int32_t* page_list,
                                const int32_t* sequence_lengths, const int32_t* position_ids, const float* cos_sin_cache,
                                int cache_positions, const b200_rope_config* cfg, int use_logn_attn, int is_bf16, int batch,
                                int q_len, int head_num, int kv_head_num, int head_dim, int max_blocks_per_seq, int page_size,
-                               void* stream) {
+                               const void* q_gamma, const void* k_gamma, float eps, void* stream) {
     if (batch == 0) return B200_OK;
     ARG_CHECK(qkv && q_out && kv_pool && page_list && sequence_lengths && cfg, "rope_append_ex: null pointer");
     ARG_CHECK(head_dim > 0 && head_dim % 2 == 0 && head_dim <= 512, "rope_append_ex: head_dim %d unsupported", head_dim);
@@ -901,7 +921,7 @@ static int rope_append_ex_impl(const void* qkv, const void* qkv_bias, void* q_ou
         return rec_call([=](void* st) {
             return rope_append_ex_impl(qkv, qkv_bias, q_out, kv_pool, page_list, sequence_lengths, position_ids, cos_sin_cache,
                                        cache_positions, &cc, use_logn_attn, is_bf16, batch, q_len, head_num, kv_head_num, head_dim,
-                                       max_blocks_per_seq, page_size, st);
+                                       max_blocks_per_seq, page_size, q_gamma, k_gamma, eps, st);
         });
     RopeCfg rc{cc.style, cc.dim, cc.base, cc.scale, cc.factor1, cc.factor2, cc.max_pos, cc.extrapolation_factor, cc.mscale};
     const dim3 grid(batch, head_num + 2 * kv_head_num, q_len);
@@ -909,8 +929,15 @@ static int rope_append_ex_impl(const void* qkv, const void* qkv_bias, void* q_ou
     const float2* cache = reinterpret_cast<const float2*>(cos_sin_cache);
     return by_dtype(is_bf16, [&](auto t) {
         using T = decltype(t);
-        CUDA_CHECK(launch_ex(q_len > 1 ? rope_append_ex_kernel<T, true> : rope_append_ex_kernel<T, false>,
-                             {grid, dim3(head_dim / 2), 0, (cudaStream_t)stream, pdl}, (const T*)qkv,
+        const LaunchCfg lc{grid, dim3(head_dim / 2), 0, (cudaStream_t)stream, pdl};
+        if (q_gamma) {
+            CUDA_CHECK(launch_ex(q_len > 1 ? qk_norm_rope_append_ex_kernel<T, true> : qk_norm_rope_append_ex_kernel<T, false>, lc,
+                                 (const T*)qkv, (T*)q_out, (T*)kv_pool, page_list, sequence_lengths, position_ids, cache,
+                                 cache_positions, rc, use_logn_attn, head_num, kv_head_num, head_dim, max_blocks_per_seq, page_size,
+                                 (const T*)q_gamma, (const T*)k_gamma, eps));
+            return launched("qk_norm_rope_append_ex_kernel");
+        }
+        CUDA_CHECK(launch_ex(q_len > 1 ? rope_append_ex_kernel<T, true> : rope_append_ex_kernel<T, false>, lc, (const T*)qkv,
                              (const T*)qkv_bias, (T*)q_out, (T*)kv_pool, page_list, sequence_lengths, position_ids, cache,
                              cache_positions, rc, use_logn_attn, head_num, kv_head_num, head_dim, max_blocks_per_seq, page_size));
         return launched("rope_append_ex_kernel");
@@ -923,7 +950,7 @@ int b200_rope_append_ex(const void* qkv, const void* qkv_bias, void* q_out, void
                         int kv_head_num, int head_dim, int max_blocks_per_seq, int page_size, void* stream) {
     return rope_append_ex_impl(qkv, qkv_bias, q_out, kv_pool, page_list, sequence_lengths, position_ids, cos_sin_cache,
                                cache_positions, cfg, use_logn_attn, is_bf16, batch, 1, head_num, kv_head_num, head_dim,
-                               max_blocks_per_seq, page_size, stream);
+                               max_blocks_per_seq, page_size, nullptr, nullptr, 0.f, stream);
 }
 
 int b200_rope_append_ex_multi(const void* qkv, const void* qkv_bias, void* q_out, void* kv_pool, const int32_t* page_list,
@@ -934,7 +961,20 @@ int b200_rope_append_ex_multi(const void* qkv, const void* qkv_bias, void* q_out
     ARG_CHECK(q_len >= 1, "rope_append_ex_multi: q_len %d must be >= 1", q_len);
     return rope_append_ex_impl(qkv, qkv_bias, q_out, kv_pool, page_list, sequence_lengths, position_ids, cos_sin_cache,
                                cache_positions, cfg, use_logn_attn, is_bf16, batch, q_len, head_num, kv_head_num, head_dim,
-                               max_blocks_per_seq, page_size, stream);
+                               max_blocks_per_seq, page_size, nullptr, nullptr, 0.f, stream);
+}
+
+int b200_qk_norm_rope_append_ex(const void* qkv, const void* q_gamma, const void* k_gamma, float eps, void* q_out, void* kv_pool,
+                                const int32_t* page_list, const int32_t* sequence_lengths, const int32_t* position_ids,
+                                const float* cos_sin_cache, int cache_positions, const b200_rope_config* cfg, int use_logn_attn,
+                                int is_bf16, int batch, int head_num, int kv_head_num, int head_dim, int max_blocks_per_seq,
+                                int page_size, int q_len, void* stream) {
+    ARG_CHECK(q_gamma && k_gamma, "qk_norm_rope_append_ex: null gamma");
+    ARG_CHECK(head_dim % 64 == 0 && head_dim <= kQkNormMaxD, "qk_norm_rope_append_ex: head_dim %d must be 64, 128 or 256", head_dim);
+    ARG_CHECK(q_len >= 1, "qk_norm_rope_append_ex: q_len %d must be >= 1", q_len);
+    return rope_append_ex_impl(qkv, nullptr, q_out, kv_pool, page_list, sequence_lengths, position_ids, cos_sin_cache,
+                               cache_positions, cfg, use_logn_attn, is_bf16, batch, q_len, head_num, kv_head_num, head_dim,
+                               max_blocks_per_seq, page_size, q_gamma, k_gamma, eps, stream);
 }
 
 int b200_embedding(const int32_t* ids, const void* table, void* out, int is_bf16, int rows, int hidden, void* stream) {

@@ -1,7 +1,7 @@
 """One decode step of a dense Llama/Qwen-style stack on the H100 hot path (synthetic weights, synthetic page tables).
 
 This is the measurement harness of SURVEY.md section 8(d): per layer
-    add_rmsnorm -> qkv GEMM -> rope + KV append -> paged decode attention -> o GEMM -> [TP all-reduce]
+    add_rmsnorm -> qkv GEMM -> [QK-norm +] rope + KV append -> paged decode attention -> o GEMM -> [TP all-reduce]
     -> add_rmsnorm -> w13 GEMM -> SiLU*mul -> w2 GEMM -> [TP all-reduce]
 then final norm -> lm_head (fp16 weights) -> greedy argmax, all on one stream under one CUDA graph.
 It mirrors the call order of the reference's Python model graph (model_desc/qwen3.py:57-138,
@@ -40,6 +40,9 @@ class ModelConfig:
     # which runs b200_rope_append(_multi) for a plain Base config and b200_rope_append_ex(_multi) for every other one, with
     # the cos/sin table for Base and Yarn (rope.py).
     rope: Optional[RopeSpec] = None
+    # Qwen3's QK-norm: every layer carries q_norm / k_norm gammas [head_dim], and each q and k head is RMS-normalised (eps) before
+    # the rotation, inside the rope launch (rope.rope_append(qk_norm=...) -> b200_qk_norm_rope_append(_ex)).
+    qk_norm: bool = False
 
 
 LLAMA3_8B = ModelConfig("Llama-3-8B", 4096, 32, 32, 8, 128, 14336, 128256)
@@ -48,6 +51,12 @@ LLAMA31_8B = ModelConfig("Llama-3.1-8B", 4096, 32, 32, 8, 128, 14336, 128256,
                          rope=RopeSpec(style=LLAMA3, dim=128, base=500000.0, scale=8.0, factor1=1.0, factor2=4.0, max_pos=8192))
 QWEN2_72B = ModelConfig("Qwen2-72B", 8192, 80, 64, 8, 128, 29696, 152064, rope_base=1000000.0, eps=1e-6)  # GPTQ-padded inter
 TINY = ModelConfig("tiny", 512, 2, 4, 2, 128, 512, 1024, tokens_per_block=16)
+QWEN3_8B = ModelConfig("Qwen3-8B", 4096, 36, 32, 8, 128, 12288, 151936, rope_base=1000000.0, eps=1e-6, qk_norm=True)
+# Hq * D = 8192 != hidden 5120: the o projection is not square
+QWEN3_32B = ModelConfig("Qwen3-32B", 5120, 64, 64, 8, 128, 25600, 151936, rope_base=1000000.0, eps=1e-6, qk_norm=True)
+# the tests' Qwen3: QK-norm, and Hq * D = 1024 != hidden 512 as in Qwen3-32B
+TINY_QWEN3 = ModelConfig("tiny-qwen3", 512, 2, 8, 2, 128, 512, 1024, rope_base=1000000.0, eps=1e-6, tokens_per_block=16,
+                         qk_norm=True)
 
 
 @dataclasses.dataclass
@@ -241,8 +250,9 @@ class DecodeStep:
         if fuse_rope is None:
             fuse_rope = os.environ.get("B200_FUSE_ROPE", "0") == "1"
         self.rope_spec = RopeSpec(dim=self.D, base=cfg.rope_base) if cfg.rope is None else rope.spec_of(cfg.rope, self.D)
-        # the fused rope appends one token with plain Base rotation
-        self.fuse_rope = bool(fuse_rope) and cfg.head_dim == 128 and q_len == 1 and rope.is_plain_base(self.rope_spec, self.D)
+        # the fused rope appends one token with plain Base rotation, and does not normalise q / k
+        self.fuse_rope = (bool(fuse_rope) and cfg.head_dim == 128 and q_len == 1 and rope.is_plain_base(self.rope_spec, self.D)
+                          and not cfg.qk_norm)
         g = torch.Generator(device="cpu").manual_seed(seed * 1000 + 17)
         H = cfg.hidden
 
@@ -336,6 +346,11 @@ class DecodeStep:
                 L["ref"] = dict(qkv=r0, o=r1, w13=r2, w2=r3)
             self.layers.append(L)
         self.final_ln = (1.0 + 0.1 * torch.randn(H, generator=g)).to(dtype).to(device)
+        if cfg.qk_norm:   # a generator of their own, so that no other weight moves; [D], replicated under TP
+            gn = torch.Generator(device="cpu").manual_seed(seed * 1000 + 29)
+            for L in self.layers:
+                L["q_norm"] = (1.0 + 0.1 * torch.randn(self.D, generator=gn)).to(dtype).to(device)
+                L["k_norm"] = (1.0 + 0.1 * torch.randn(self.D, generator=gn)).to(dtype).to(device)
         if shard_full:
             _, self.lm_head_full = make_weight(H, cfg.vocab, seed * 100003 + 999983, quant="f16")
             self.lm_head_ref = tpmod.shard_lm_head(self.lm_head_full, self.vocab, tp_rank)
@@ -553,6 +568,13 @@ class DecodeStep:
             self.comm.all_reduce(t)
         ops.add_rmsnorm(t, self.resid, gamma, self.cfg.eps, out=self.x)
 
+    def _rope_append(self, L):
+        """q of the step's rows into self.q, their K/V into layer L's cache: rope.rope_append, with L's QK-norm when the config
+        has one."""
+        qk_norm = (L["q_norm"], L["k_norm"], self.cfg.eps) if self.cfg.qk_norm else None
+        rope.rope_append(self.rope_spec, self.qkv, L["kv"], self.page_list, self.seq_lens, self.Hq, q_out=self.q, q_len=self.q_len,
+                         qk_norm=qk_norm)
+
     def step_core(self):
         """Everything up to the sampled token (TP1 / peer communicator) or the local logits (NCCL): C-ABI calls only, so it
         can be recorded into a decode program."""
@@ -571,12 +593,11 @@ class DecodeStep:
                 ops.paged_decode_attn_rope(self.qkv, L["kv"], self.page_list, self.seq_lens, self.Hq, self.ctx,
                                            self.rope_spec.base, self.attn_ws, out=self.attn)
             elif self.q_len > 1:  # K/V of all q_len tokens appended, then each query token attends up to its own position
-                rope.rope_append(self.rope_spec, self.qkv, L["kv"], self.page_list, self.seq_lens, self.Hq, q_out=self.q,
-                                 q_len=self.q_len)
+                self._rope_append(L)
                 ops.paged_decode_attn_multi(self.q.view(self.B, self.q_len, self.Hq, self.D), L["kv"], self.page_list, self.seq_lens,
                                             self.ctx, self.attn_ws, out=self.attn.view(self.B, self.q_len, self.Hq * self.D))
             else:
-                rope.rope_append(self.rope_spec, self.qkv, L["kv"], self.page_list, self.seq_lens, self.Hq, q_out=self.q)
+                self._rope_append(L)
                 ops.paged_decode_attn(self.q, L["kv"], self.page_list, self.seq_lens, self.ctx, self.attn_ws, out=self.attn)
             self._row_gemm(self.attn, L["o"])
             self._ar_norm(self.proj, L["ln2"])

@@ -2,7 +2,8 @@
 per-column INT8 path, read from safetensors and pushed through the device hooks exactly as the reference's loader does
 (SURVEY 8 f-4).  What is mirrored, file:line in /root/reference:
   * tensor names   `<prefix>.qweight / .qzeros / .scales`                    model_loader/group_wise_quant_weight.py:32-36
-  * which layers   qkv, o, w1 / w3 (merged into w13), w2                     group_wise_quant_weight.py:304-316
+  * which layers   qkv, o, w1 / w3 (merged into w13), w2                     group_wise_quant_weight.py:304-316;
+                   Qwen3's q_norm / k_norm gammas `<prefix>.weight`, unquantised, when the layer names them
   * merge rules    q|k|v and gate|up concatenated along the OUTPUT axis (GPTQ qweight [K/8, N]: dim 1; AWQ qweight [K, N/8]: dim 1)
   * padding        the FFN inter size is padded to `align_size`: w2 along its INPUT rows (GPTQ qweight rows are packed 8:1 ->
                    align_size / 8; AWQ: align_size), zeros / scales by align_size / group_size rows; w1 / w3 along their
@@ -174,13 +175,22 @@ class B200Loader:
     def _load(self, prefixes, **kw) -> ops.PackedWeight:
         return self._groupwise(prefixes, **kw) if self.q.method in ("gptq", "awq") else self._dense(prefixes, **kw)
 
+    def qk_norms(self, names: Dict[str, str]) -> Dict[str, torch.Tensor]:
+        """Qwen3's QK-norm gammas: `<names["q_norm"]>.weight` / `<names["k_norm"]>.weight` (HF: ...self_attn.q_norm.weight) as
+        contiguous act-dtype [head_dim] tensors on the loader's device, for the names given. A missing tensor raises the
+        reader's KeyError, which names it."""
+        return {k: self.r.get(names[k] + ".weight").to(self.act_dtype).to(self.device).contiguous()
+                for k in ("q_norm", "k_norm") if k in names}
+
     def layer(self, names: Dict[str, str], inter: Optional[int] = None) -> Dict[str, ops.PackedWeight]:
-        """qkv / o / w13 / w2 of one decoder layer. `inter` = the checkpoint's FFN inter size (needed for padding + fusion).
+        """qkv / o / w13 / w2 of one decoder layer, and q_norm / k_norm (qk_norms) when `names` has them. `inter` = the
+        checkpoint's FFN inter size (needed for padding + fusion).
 
         Act-order: qkv, o and w13 carry their row order (the GEMM gathers x). w2's order P2 is folded into w13 instead: column i
         of w2's input is SiLU(gate_i) * up_i, so w13 with its gate and up columns permuted by P2 emits act[:, P2] directly and
         the sorted w2 needs no gather."""
-        out = {"qkv": self._load([names["q"], names["k"], names["v"]]), "o": self._load([names["o"]])}
+        norms = self.qk_norms(names)      # first: a missing norm fails before any weight is packed
+        out = {"qkv": self._load([names["q"], names["k"], names["v"]]), "o": self._load([names["o"]]), **norms}
         pad = self.align
         inter_p = inter if inter is None or not pad else (inter + pad - 1) // pad * pad
         fuse = self.fuse_silu and inter_p is not None and inter_p % 64 == 0

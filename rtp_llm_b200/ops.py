@@ -414,6 +414,55 @@ def rope_append_ex(qkv, kv_cache_base, page_list, sequence_lengths, head_num, ro
     return q_out
 
 
+def _qk_norm_checks(what, qkv, q_gamma, k_gamma, D, q_len):
+    _cuda_contig(q_gamma, k_gamma)
+    rows = qkv.shape[0]
+    if q_len < 1 or rows % q_len:
+        raise B200Error(f"{what}: {rows} qkv rows are not a multiple of q_len {q_len}")
+    for name, g in (("q_gamma", q_gamma), ("k_gamma", k_gamma)):
+        if g is None or g.dtype != qkv.dtype or g.numel() != D:
+            raise B200Error(f"{what}: {name} must be a [{D}] tensor of qkv's dtype {qkv.dtype}")
+
+
+def qk_norm_rope_append(qkv, q_gamma, k_gamma, eps, kv_cache_base, page_list, sequence_lengths, head_num, rope_base, q_out=None,
+                        q_len: int = 1):
+    """rope_append after Qwen3's QK-RMSNorm, in one launch: each q and k head of qkv is RMS-normalised with q_gamma / k_gamma
+    [D] first, with the bits of qk_rmsnorm on a copy of qkv followed by rope_append (b200_qk_norm_rope_append). qkv is only
+    read. Returns q [B*q_len, Hq*D]."""
+    _cuda_contig(qkv, kv_cache_base, page_list, sequence_lengths, q_out)
+    P, two, Hkv, T, D = kv_cache_base.shape
+    _qk_norm_checks("qk_norm_rope_append", qkv, q_gamma, k_gamma, D, q_len)
+    rows = qkv.shape[0]
+    if q_out is None:
+        q_out = torch.empty((rows, head_num * D), dtype=qkv.dtype, device=qkv.device)
+    check(_lib.load().b200_qk_norm_rope_append(_p(qkv), _p(q_gamma), _p(k_gamma), eps, _p(q_out), _p(kv_cache_base), _p(page_list),
+                                               _p(sequence_lengths), _is_bf16(qkv), rows // q_len, head_num, Hkv, D,
+                                               page_list.shape[-1], T, rope_base, q_len, _stream()), "b200_qk_norm_rope_append")
+    return q_out
+
+
+def qk_norm_rope_append_ex(qkv, q_gamma, k_gamma, eps, kv_cache_base, page_list, sequence_lengths, head_num,
+                           rope_cfg: "_lib.RopeConfig", q_out=None, position_ids=None, cos_sin_cache=None, use_logn_attn=False,
+                           q_len: int = 1):
+    """rope_append_ex (no bias) after Qwen3's QK-RMSNorm, in one launch (b200_qk_norm_rope_append_ex): the bits of qk_rmsnorm
+    on a copy of qkv followed by rope_append_ex. qkv is only read. Returns q [B*q_len, Hq*D]."""
+    import ctypes
+    _cuda_contig(qkv, kv_cache_base, page_list, sequence_lengths, q_out, position_ids, cos_sin_cache)
+    P, two, Hkv, T, D = kv_cache_base.shape
+    _qk_norm_checks("qk_norm_rope_append_ex", qkv, q_gamma, k_gamma, D, q_len)
+    rows = qkv.shape[0]
+    if position_ids is not None and position_ids.numel() != rows:
+        raise B200Error(f"qk_norm_rope_append_ex: {position_ids.numel()} position ids for {rows} qkv rows")
+    if q_out is None:
+        q_out = torch.empty((rows, head_num * D), dtype=qkv.dtype, device=qkv.device)
+    check(_lib.load().b200_qk_norm_rope_append_ex(
+        _p(qkv), _p(q_gamma), _p(k_gamma), eps, _p(q_out), _p(kv_cache_base), _p(page_list), _p(sequence_lengths),
+        _p(position_ids), _p(cos_sin_cache), cos_sin_cache.shape[0] if cos_sin_cache is not None else 0,
+        ctypes.cast(ctypes.pointer(rope_cfg), ctypes.c_void_p), 1 if use_logn_attn else 0, _is_bf16(qkv), rows // q_len, head_num,
+        Hkv, D, page_list.shape[-1], T, q_len, _stream()), "b200_qk_norm_rope_append_ex")
+    return q_out
+
+
 def embedding(ids, table, out=None):
     _cuda_contig(ids, table, out)
     rows, hidden = ids.shape[0], table.shape[1]

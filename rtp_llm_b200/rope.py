@@ -113,14 +113,21 @@ def table(spec: RopeSpec, device) -> Optional[torch.Tensor]:
 
 
 def rope_append(spec: RopeSpec, qkv, kv_cache_base, page_list, sequence_lengths, head_num: int, q_out=None, q_len: int = 1,
-                use_logn_attn: bool = False, position_ids=None):
+                use_logn_attn: bool = False, position_ids=None, qk_norm=None):
     """Rotate q and k of qkv [B*q_len, (Hq+2Hkv)*D] and append K/V for any served config. A plain Base config without logn
     and position ids runs b200_rope_append(_multi) -- the bits callers that only set `base` have always had -- and every other
-    config runs b200_rope_append_ex(_multi), with the cos/sin table for Base and Yarn."""
+    config runs b200_rope_append_ex(_multi), with the cos/sin table for Base and Yarn.
+    qk_norm = (q_gamma, k_gamma, eps): Qwen3's QK-RMSNorm of each q and k head first, in the same launch
+    (b200_qk_norm_rope_append(_ex), picked by the same rule); qkv is then only read."""
     from . import ops
     D = kv_cache_base.shape[-1]
     if is_plain_base(spec, D) and not use_logn_attn and position_ids is None:
+        if qk_norm is not None:
+            return ops.qk_norm_rope_append(qkv, *qk_norm, kv_cache_base, page_list, sequence_lengths, head_num, spec.base,
+                                           q_out=q_out, q_len=q_len)
         return ops.rope_append(qkv, kv_cache_base, page_list, sequence_lengths, head_num, spec.base, q_out=q_out, q_len=q_len)
-    return ops.rope_append_ex(qkv, kv_cache_base, page_list, sequence_lengths, head_num, c_config(spec), q_out=q_out,
-                              position_ids=position_ids, cos_sin_cache=table(spec, qkv.device), use_logn_attn=use_logn_attn,
-                              q_len=q_len)
+    ex = dict(q_out=q_out, position_ids=position_ids, cos_sin_cache=table(spec, qkv.device), use_logn_attn=use_logn_attn,
+              q_len=q_len)
+    if qk_norm is not None:
+        return ops.qk_norm_rope_append_ex(qkv, *qk_norm, kv_cache_base, page_list, sequence_lengths, head_num, c_config(spec), **ex)
+    return ops.rope_append_ex(qkv, kv_cache_base, page_list, sequence_lengths, head_num, c_config(spec), **ex)

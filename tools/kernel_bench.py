@@ -173,6 +173,37 @@ def bench_rope(kind, B, Hq, Hkv, q_len, S=2048, T=64, D=128, nrot=4):
     return us
 
 
+def bench_qknorm_rope(kind, fused, B, Hq, Hkv, q_len, S=2048, T=64, D=128, nrot=4):
+    """Qwen3's QK-RMSNorm + RoPE + K/V append of q_len tokens per sequence at cached length S - q_len, plain Base at base 1e6
+    ("base") or Qwen3's Yarn cos/sin table ("yarn table"): the one-launch b200_qk_norm_rope_append(_ex) (fused) against
+    b200_qk_rmsnorm in place on qkv followed by b200_rope_append(_ex) (two launches). Bytes = those of the fused kernel, qkv
+    read + q and K/V written (+ the table rows); the composition moves the q and k heads once more."""
+    from rtp_llm_b200 import rope
+    M = math.ceil(S / T)
+    P = B * M + 1
+    pools = [torch.zeros(P, 2, Hkv, T, D, device=dev).half() for _ in range(nrot)]
+    qkv = torch.randn(B * q_len, (Hq + 2 * Hkv) * D, device=dev).half()
+    q = torch.empty(B * q_len, Hq * D, device=dev).half()
+    qg, kg = (1 + 0.1 * torch.randn(D, device=dev)).half(), (1 + 0.1 * torch.randn(D, device=dev)).half()
+    pl = ops.convert_block_table((torch.randperm(P - 1, device=dev).to(torch.int32) + 1).reshape(B, M))
+    seq = torch.full((B,), S - q_len, dtype=torch.int32, device=dev)
+    spec = (rope.RopeSpec(dim=D, base=1000000.0) if kind == "base" else
+            rope.RopeSpec(style=rope.YARN, dim=D, base=1000000.0, scale=4.0, factor1=1.0, factor2=32.0, max_pos=32768, mscale=1.14))
+    rope.table(spec, dev)
+
+    def fn(i):
+        if fused:
+            rope.rope_append(spec, qkv, pools[i], pl, seq, Hq, q_out=q, q_len=q_len, qk_norm=(qg, kg, 1e-6))
+        else:
+            ops.qk_rmsnorm(qkv, qg, kg, Hq, Hkv, D, 1e-6)
+            rope.rope_append(spec, qkv, pools[i], pl, seq, Hq, q_out=q, q_len=q_len)
+    us = timeit(fn, nrot)
+    byt = B * q_len * 2 * (Hq + 2 * Hkv) * D * 2 + (B * q_len * D * 4 if kind != "base" else 0)
+    print(f"qknorm-rope {kind:10s} {'fused' if fused else 'norm + rope':11s} B{B} Hq{Hq} Hkv{Hkv} D{D} q_len {q_len}: {us:7.2f} us  "
+          f"{byt / us / 1e3:7.0f} GB/s", flush=True)
+    return us
+
+
 def bench_permute(B, K, nrot=4):
     """b200_permute_cols on [B, K] fp16; bytes = the row read and written, plus the perm."""
     xs = [torch.randn(B, K, device=dev).half() for _ in range(nrot)]
@@ -287,6 +318,16 @@ if __name__ == "__main__":
         for n in (1, 4):
             t = {k: bench_rope(k, 32, 32, 8, n) for k in ("base", "llama3", "yarn table")}
             print(f"rope q_len {n} relative to base: " + ", ".join(f"{k}: {t[k] / t['base']:.2f}x" for k in t), flush=True)
+    if "qknorm-rope" in which:
+        # Qwen3-8B's attention shape (Hq 32, Hkv 8, D 128) at B 32: the fused QK-norm + rope against the two launches, alternating
+        for kind in ("base", "yarn table"):
+            for n in (1, 4):
+                t = {f: [] for f in (True, False)}
+                for _ in range(3):
+                    for f in t:
+                        t[f].append(bench_qknorm_rope(kind, f, 32, 32, 8, n))
+                fu, co = sorted(t[True])[1], sorted(t[False])[1]
+                print(f"qknorm-rope {kind} q_len {n} median: fused {fu:.2f} us, norm + rope {co:.2f} us ({fu / co:.2f}x)", flush=True)
     if "gemm" in which:
         for B in (32,):
             bench_gemm(B200_FMT_INT4, B, 4096, 6144)
