@@ -1,5 +1,6 @@
 """Float64 numpy reference of one beam-search step (b200_beam_search_step) and of the no-repeat-n-gram ban
-(b200_ban_repeat_ngram), restated from the Hugging Face / TensorRT-LLM beam-search convention."""
+(b200_ban_repeat_ngram), restated from the Hugging Face / TensorRT-LLM beam-search convention, and the pass rule of a kernel's
+selection against it (check_beam)."""
 import numpy as np
 
 
@@ -48,6 +49,38 @@ def next_from_candidates(cand_token, cand_parent, cand_score, W, eos_id=-1):
     keep = [np.nonzero(cand_token[b] != eos_id)[0][:W] for b in range(cand_token.shape[0])]
     return (np.stack([cand_token[b, k] for b, k in enumerate(keep)]), np.stack([cand_parent[b, k] for b, k in enumerate(keep)]),
             np.stack([cand_score[b, k] for b, k in enumerate(keep)]))
+
+
+def score_tol(score):
+    return 1e-5 * (1.0 + np.abs(score))
+
+
+def check_beam(got, exp, W, eos_id):
+    """The pass rule against the float64 reference: scores within 1e-5 * (1 + |score|) rank by rank; tokens and parents
+    equal at every rank whose reference score is clear of its neighbours by that bound (or exactly tied, which both rank by
+    flat index); the next_* arrays follow from the kernel's own candidates by the EOS rule exactly."""
+    es, rs = exp["cand_score"], exp["ranked_scores"]
+    gs = got["cand_score"].astype(np.float64)
+    fin = np.isfinite(es)
+    assert (np.isneginf(gs) == np.isneginf(es)).all(), (gs, es)
+    assert (np.abs(gs[fin] - es[fin]) <= score_tol(es[fin])).all(), np.abs(gs - es)[fin].max()
+    B = es.shape[0]
+    for b in range(B):
+        for r in range(2 * W):
+            def clear(a, c):
+                if np.isneginf(a) and np.isneginf(c):
+                    return True                                  # both -inf: an exact tie, ranked by index
+                d = abs(a - c)
+                return d == 0 or d > score_tol(a)
+            ok = clear(rs[b, r], rs[b, r + 1]) and (r == 0 or clear(rs[b, r - 1], rs[b, r]))
+            tied = (r > 0 and rs[b, r - 1] == rs[b, r]) or rs[b, r] == rs[b, r + 1]
+            if ok or tied and np.isneginf(rs[b, r]):
+                assert got["cand_token"][b, r] == exp["cand_token"][b, r], (b, r, got["cand_token"][b], exp["cand_token"][b])
+                assert got["cand_parent"][b, r] == exp["cand_parent"][b, r], (b, r)
+    nt, npar, nc = next_from_candidates(got["cand_token"], got["cand_parent"], got["cand_score"], W, eos_id)
+    np.testing.assert_array_equal(got["next_token"], nt)
+    np.testing.assert_array_equal(got["next_parent"], npar)
+    np.testing.assert_array_equal(got["next_cum"], nc)
 
 
 def banned_np(history, hist_len, ngram_size, vocab):

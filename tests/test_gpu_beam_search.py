@@ -3,7 +3,6 @@
 selections, the page-table fork (bit-exact K/V histories), a re-score of the surviving beams through plain steps, and
 beam_width 1 against the greedy step."""
 import dataclasses
-import types
 
 import numpy as np
 import pytest
@@ -13,8 +12,8 @@ pytestmark = pytest.mark.gpu
 
 from rtp_llm_b200 import ops  # noqa: E402
 from rtp_llm_b200.decode_step import TINY, DecodeStep  # noqa: E402
-from tests.beam_oracle import banned_np, beam_step_np, next_from_candidates  # noqa: E402
-from tests.step_oracle import bits, oracle_step  # noqa: E402
+from tests.beam_oracle import banned_np, beam_step_np, check_beam, score_tol  # noqa: E402
+from tests.step_oracle import bits, check_logits, device_state, oracle_step  # noqa: E402
 
 DEV = torch.device("cuda")
 DTYPES = {"fp16": torch.float16, "bf16": torch.bfloat16, "fp32": torch.float32}
@@ -22,38 +21,6 @@ DTYPES = {"fp16": torch.float16, "bf16": torch.bfloat16, "fp32": torch.float32}
 
 def _bits(t):
     return t.contiguous().view(torch.int16 if t.element_size() == 2 else torch.int32)
-
-
-def _tol(score):
-    return 1e-5 * (1.0 + np.abs(score))
-
-
-def check_beam(got, exp, W, eos_id):
-    """The pass rule against the float64 reference: scores within 1e-5 * (1 + |score|) rank by rank; tokens and parents
-    equal at every rank whose reference score is clear of its neighbours by that bound (or exactly tied, which both rank by
-    flat index); the next_* arrays follow from the kernel's own candidates by the EOS rule exactly."""
-    es, rs = exp["cand_score"], exp["ranked_scores"]
-    gs = got["cand_score"].astype(np.float64)
-    fin = np.isfinite(es)
-    assert (np.isneginf(gs) == np.isneginf(es)).all(), (gs, es)
-    assert (np.abs(gs[fin] - es[fin]) <= _tol(es[fin])).all(), np.abs(gs - es)[fin].max()
-    B = es.shape[0]
-    for b in range(B):
-        for r in range(2 * W):
-            def clear(a, c):
-                if np.isneginf(a) and np.isneginf(c):
-                    return True                                  # both -inf: an exact tie, ranked by index
-                d = abs(a - c)
-                return d == 0 or d > _tol(a)
-            ok = clear(rs[b, r], rs[b, r + 1]) and (r == 0 or clear(rs[b, r - 1], rs[b, r]))
-            tied = (r > 0 and rs[b, r - 1] == rs[b, r]) or rs[b, r] == rs[b, r + 1]
-            if ok or tied and np.isneginf(rs[b, r]):
-                assert got["cand_token"][b, r] == exp["cand_token"][b, r], (b, r, got["cand_token"][b], exp["cand_token"][b])
-                assert got["cand_parent"][b, r] == exp["cand_parent"][b, r], (b, r)
-    nt, npar, nc = next_from_candidates(got["cand_token"], got["cand_parent"], got["cand_score"], W, eos_id)
-    np.testing.assert_array_equal(got["next_token"], nt)
-    np.testing.assert_array_equal(got["next_parent"], npar)
-    np.testing.assert_array_equal(got["next_cum"], nc)
 
 
 def _case(B, W, V, dtype, seed):
@@ -107,7 +74,7 @@ def test_width_one_picks_the_argmax_token():
     x64 = x.double().numpy()
     ls = x64[np.arange(B), am] - (x64.max(1) + np.log(np.exp(x64 - x64.max(1, keepdims=True)).sum(1)))
     e = cum.numpy()[:, 0] + ls
-    assert (np.abs(nc - e)[clear] <= _tol(e)[clear]).all()
+    assert (np.abs(nc - e)[clear] <= score_tol(e)[clear]).all()
 
 
 @pytest.mark.parametrize("dt", list(DTYPES))
@@ -181,14 +148,6 @@ def test_both_ops_give_the_same_bits_under_graph_replay_with_pdl():
 
 
 # ---------------------------------------------------------------------------------------------------- decode step
-def _state(model):
-    """The fields oracle_step reads, from the step's forked device state (B = the step's rows)."""
-    return types.SimpleNamespace(cfg=model.cfg, B=model.B, q_len=1, Hq=model.Hq, Hkv=model.Hkv, D=model.D,
-                                 rope_spec=model.rope_spec, seq_lens_h=model.seq_lens.cpu(), block_ids_h=model.block_ids.cpu(),
-                                 ids_h=model.ids.cpu(), embed=model.embed, layers=model.layers, final_ln=model.final_ln,
-                                 lm_head_ref=model.lm_head_ref)
-
-
 def _seed_history(model, n):
     """A prompt history whose last n - 1 ids (ending in each row's input token) occurred once before, followed by a row-specific
     token: with the n-gram ban on, step 1 must ban that token in every row (n == 1 bans the input token itself)."""
@@ -229,7 +188,7 @@ def test_beam_step_vs_oracle(case):
         bans = []
         for t in range(steps):
             torch.cuda.synchronize()
-            state, kv_before = _state(model), [bits(L["kv"]) for L in model.layers]
+            state, kv_before = device_state(model), [bits(L["kv"]) for L in model.layers]
             cum = model.beam_cum.cpu().numpy()
             hist, hist_len = model.hist.cpu().numpy(), model.hist_len.cpu().numpy()
             model.replay() if "graph" in mode else model.run()
@@ -242,9 +201,7 @@ def test_beam_step_vs_oracle(case):
             for r in range(R):
                 np.testing.assert_array_equal(np.nonzero(np.isneginf(got[r]))[0], banned[r], err_msg=f"step {t} row {r}: banned set")
                 fin[r, banned[r]] = False
-            scale = float(np.sqrt((exp[fin] ** 2).mean()))
-            err = float(np.abs(got[fin] - exp[fin]).max())
-            assert np.isfinite(got[fin]).all() and err <= 3e-2 * scale + 3e-2, f"logits differ: max err {err} vs rms {scale}"
+            check_logits(got, exp, mask=fin)
             sel = {k: v.cpu().numpy() for k, v in model.beam_out.items()}
             check_beam(sel, beam_step_np(got, cum), W, -1)
             par = (np.arange(R) // W * W + sel["next_parent"].reshape(-1)).tolist()

@@ -3,9 +3,7 @@ oracle in every mode (eager, CUDA graph + PDL, decode program, verification step
 modes, the step's logits bit for bit against a two-launch composition (qk_rmsnorm, then the plain rope launch), and the
 launch count of a QK-norm step."""
 import dataclasses
-import types
 
-import numpy as np
 import pytest
 import torch
 
@@ -13,24 +11,14 @@ pytestmark = pytest.mark.gpu
 
 from rtp_llm_b200 import ops, rope  # noqa: E402
 from rtp_llm_b200.decode_step import TINY_QWEN3, DecodeStep, SamplingParams, sampling_uniforms  # noqa: E402
-from tests.beam_oracle import beam_step_np  # noqa: E402
-from tests.qwen3_oracle import check_step, oracle_step  # noqa: E402
-from tests.step_oracle import bits  # noqa: E402
-from tests.test_gpu_beam_search import check_beam  # noqa: E402
+from tests.beam_oracle import beam_step_np, check_beam  # noqa: E402
+from tests.step_oracle import TwoLaunchStep, bits, check_logits, check_step, device_state, oracle_step  # noqa: E402
 
 DEV = torch.device("cuda")
 # Qwen3's YaRN (rope_scaling factor 4, beta_fast 32, beta_slow 1, mscale 0.1 ln 4 + 1) with original max positions 16, so the
 # tiny contexts (positions 20..70) sit in the scaled band and the cos/sin table covers them
 YARN = rope.RopeSpec(style=rope.YARN, dim=128, base=1000000.0, scale=4.0, factor1=1.0, factor2=32.0, max_pos=16, mscale=1.1386)
 TINY_QWEN3_YARN = dataclasses.replace(TINY_QWEN3, rope=YARN)
-
-
-class TwoLaunchStep(DecodeStep):
-    """The composition the fused launch replaces: qk_rmsnorm in place on qkv, then rope.rope_append without QK-norm."""
-
-    def _rope_append(self, L):
-        ops.qk_rmsnorm(self.qkv, L["q_norm"], L["k_norm"], self.Hq, self.Hkv, self.D, self.cfg.eps)
-        rope.rope_append(self.rope_spec, self.qkv, L["kv"], self.page_list, self.seq_lens, self.Hq, q_out=self.q, q_len=self.q_len)
 
 
 @pytest.mark.parametrize("quant", ["int4", "f16", "int8", "int8g"])
@@ -92,19 +80,6 @@ def test_launches_per_step_equal_those_without_qk_norm():
     assert progs[True] == progs[False]
 
 
-def _state(model, q_len=1):
-    return types.SimpleNamespace(cfg=model.cfg, B=model.B, q_len=q_len, Hq=model.Hq, Hkv=model.Hkv, D=model.D,
-                                 rope_spec=model.rope_spec, seq_lens_h=model.seq_lens.cpu(), block_ids_h=model.block_ids.cpu(),
-                                 ids_h=model.ids.cpu(), embed=model.embed, layers=model.layers, final_ln=model.final_ln,
-                                 lm_head_ref=model.lm_head_ref)
-
-
-def _check_logits(got, exp):
-    scale = float(np.sqrt((exp ** 2).mean()))
-    err = float(np.abs(got - exp).max())
-    assert np.isfinite(got).all() and err <= 3e-2 * scale + 3e-2, f"logits differ: max err {err} vs rms {scale}"
-
-
 def test_qwen3_sampling_steps():
     """Three sampled steps under a CUDA graph with PDL: every step's logits against the oracle, the same logits, tokens and state
     as the two-launch composition, and the greedy (top_k 1) request's token the argmax of the logits."""
@@ -116,11 +91,11 @@ def test_qwen3_sampling_steps():
             m.capture()
         for t in range(3):
             torch.cuda.synchronize()
-            state, kv_before = _state(fused), [bits(L["kv"]) for L in fused.layers]
+            state, kv_before = device_state(fused), [bits(L["kv"]) for L in fused.layers]
             for m in (fused, two):
                 m.replay()
             torch.cuda.synchronize()
-            _check_logits(fused.logits.float().cpu().numpy(), oracle_step(state, kv_before))
+            check_logits(fused.logits.float().cpu().numpy(), oracle_step(state, kv_before))
             assert torch.equal(fused.logits, two.logits) and torch.equal(fused.next_ids, two.next_ids)
             assert torch.equal(fused.uniform.cpu(), sampling_uniforms(sp.seed, t, fused.B))
             assert int(fused.next_ids[0]) == int(fused.logits[0].float().argmax())
@@ -139,13 +114,13 @@ def test_qwen3_beam_steps():
     two = TwoLaunchStep(fused.cfg, 2, 40, DEV, keep_reference=True, ragged=True, seed=6, beam_width=4)
     for t in range(3):
         torch.cuda.synchronize()
-        state, kv_before = _state(fused), [bits(L["kv"]) for L in fused.layers]
+        state, kv_before = device_state(fused), [bits(L["kv"]) for L in fused.layers]
         cum = fused.beam_cum.cpu().numpy()
         for m in (fused, two):
             m.run()
         torch.cuda.synchronize()
         got = fused.logits.float().cpu().numpy()
-        _check_logits(got, oracle_step(state, kv_before))
+        check_logits(got, oracle_step(state, kv_before))
         sel = {k: v.cpu() for k, v in fused.beam_out.items()}
         check_beam({k: v.numpy() for k, v in sel.items()}, beam_step_np(got, cum), 4, -1)
         assert torch.equal(fused.logits, two.logits)

@@ -3,7 +3,6 @@ bits under CUDA-graph replay with PDL; DecodeStep's sampling mode step by step a
 (pinned to the reference's CudaSamplerTest vectors) on the step's own logits, params, history and uniforms; and sampled
 verification of speculative tokens against spec_verify_np on the step's own probabilities and uniforms."""
 import dataclasses
-import types
 
 import numpy as np
 import pytest
@@ -17,7 +16,7 @@ from rtp_llm_b200.decode_step import TINY, DecodeStep, SamplingParams, sampling_
 from tests.beam_oracle import banned_np  # noqa: E402
 from tests.logprob_oracle import log_softmax_np, token_logprobs_np  # noqa: E402
 from tests.spec_oracle import spec_verify_np  # noqa: E402
-from tests.step_oracle import bits, oracle_step  # noqa: E402
+from tests.step_oracle import bits, check_logits, device_state, oracle_step  # noqa: E402
 
 DEV = torch.device("cuda")
 DTYPES = {"fp16": torch.float16, "bf16": torch.bfloat16, "fp32": torch.float32}
@@ -128,20 +127,6 @@ def test_logprobs_give_the_same_bits_under_graph_replay_with_pdl():
 
 
 # ---------------------------------------------------------------------------------------------------- decode step
-def _state(model):
-    """The fields oracle_step reads, from the step's advanced device state."""
-    return types.SimpleNamespace(cfg=model.cfg, B=model.B, q_len=model.q_len, Hq=model.Hq, Hkv=model.Hkv, D=model.D,
-                                 rope_spec=model.rope_spec, seq_lens_h=model.seq_lens.cpu(), block_ids_h=model.block_ids.cpu(),
-                                 ids_h=model.ids.cpu(), embed=model.embed, layers=model.layers, final_ln=model.final_ln,
-                                 lm_head_ref=model.lm_head_ref)
-
-
-def _check_logits(got, exp):
-    scale = float(np.sqrt((exp ** 2).mean()))
-    err = float(np.abs(got - exp).max())
-    assert np.isfinite(got).all() and err <= 3e-2 * scale + 3e-2, f"logits differ: max err {err} vs rms {scale}"
-
-
 # request 0: top_k 1 (greedy); 1: repetition 2 + presence 1, certain to move every history logit; 2: frequency; 3: top-k + top-p
 PARAMS = SamplingParams(temperature=[0.7, 1.0, 1.3, 0.9], top_k=[1, 50, 0, 20], top_p=[1.0, 0.9, 0.8, 0.95],
                         repetition=[1.0, 2.0, 1.0, 1.3], presence=[0.0, 1.0, 0.0, 0.0], frequency=[0.0, 0.0, 0.5, 0.0], seed=11)
@@ -178,12 +163,12 @@ def test_sampling_step_vs_oracles(case):
         moved = 0
         for t in range(steps):
             torch.cuda.synchronize()
-            state, kv_before = _state(model), [bits(L["kv"]) for L in model.layers]
+            state, kv_before = device_state(model), [bits(L["kv"]) for L in model.layers]
             hist, hist_len = model.hist.cpu().numpy(), model.hist_len.cpu().numpy()
             model.replay() if "graph" in mode else model.run()
             torch.cuda.synchronize()
             raw = model.logits.float().cpu().numpy()
-            _check_logits(raw, oracle_step(state, kv_before))
+            check_logits(raw, oracle_step(state, kv_before))
             u = model.uniform.cpu()
             assert torch.equal(u, sampling_uniforms(PARAMS.seed, t, R)), f"step {t}: uniforms"
             lg = raw.copy()
@@ -256,11 +241,11 @@ def test_sampled_verification_vs_reference(q_len, mode):
             model.upload_inputs()
             torch.cuda.synchronize()
             kv_before = [bits(L["kv"]) for L in model.layers]
-            state = _state(model)
+            state = device_state(model)
             model.replay() if "graph" in mode else model.run()
             torch.cuda.synchronize()
             raw = model.logits.float().cpu().numpy()
-            _check_logits(raw, oracle_step(state, kv_before))
+            check_logits(raw, oracle_step(state, kv_before))
             u = model.uniform.cpu()
             assert torch.equal(u, sampling_uniforms(sp.seed, 0, 2 * R)), "uniforms restart with upload_inputs()"
             rep = lambda v, dt: np.repeat(np.asarray(v, dt), q_len)  # noqa: E731
@@ -299,8 +284,7 @@ def test_sampled_verification_accepts_near_greedy_drafts():
     torch.cuda.synchronize()
     got = spec.logits.float().cpu().numpy().reshape(spec.B, k + 1, -1)
     exp = np.stack(logits, axis=1)
-    err = float(np.abs(got - exp).max())
-    assert err <= 3e-2 * float(np.sqrt((exp ** 2).mean())) + 3e-2
+    err = check_logits(got, exp)
     srt = np.sort(exp, axis=-1)
     sure = ((srt[..., -1] - srt[..., -2]) > 2 * err + 1e-3).all(axis=1)
     assert sure.any(), "no sequence with a clear margin at every step"

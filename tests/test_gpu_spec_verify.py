@@ -13,7 +13,7 @@ from rtp_llm_b200 import ops  # noqa: E402
 from rtp_llm_b200.decode_step import TINY, DecodeStep  # noqa: E402
 from tests import gpu_probe as probe  # noqa: E402
 from tests.spec_oracle import spec_verify_np  # noqa: E402
-from tests.step_oracle import TINY31, check_step  # noqa: E402
+from tests.step_oracle import TINY31, check_logits, check_step  # noqa: E402
 
 DEV = torch.device("cuda")
 TILES = "B200_ATTN_TILES_PER_SPLIT"
@@ -234,9 +234,7 @@ def test_verification_step_accepts_the_tokens_plain_steps_produce(cfg, k):
     torch.cuda.synchronize()
     got = spec.logits.float().cpu().numpy().reshape(spec.B, k + 1, -1)
     exp = np.stack(logits, axis=1)
-    scale = float(np.sqrt((exp ** 2).mean()))
-    err = float(np.abs(got - exp).max())
-    assert err <= 3e-2 * scale + 3e-2, f"logits differ: max err {err} vs rms {scale}"
+    err = check_logits(got, exp)
     srt = np.sort(exp, axis=-1)
     sure = ((srt[..., -1] - srt[..., -2]) > 2 * err + 1e-6).all(axis=1)
     assert sure.any(), "no sequence with a clear margin at every step"
