@@ -287,13 +287,52 @@ int b200_spec_verify(const float* target_probs, const int32_t* target_ids, const
  * Outputs: the top 2W candidates in rank order, cand_token / cand_parent (beam index 0..W-1) / cand_score [batch][2W]; the next
  * beams next_token / next_parent / next_cum [batch][W] = the first W ranked candidates whose token is not eos_id (-1: none). Each
  * row adds at most one EOS candidate, so W of the 2W are never EOS; the EOS candidates among the first W ranks are the finished
- * hypotheses (length penalty, early stopping and the finished-hypothesis set stay the caller's).
+ * hypotheses, which b200_beam_hypotheses_update keeps on the device.
  * workspace: b200_beam_search_step_workspace_bytes(batch, W, vocab) bytes, ZERO on first use; every call leaves it zero-ready
  * (self-resetting arrival counters). One launch, deterministic, graph-capturable; under PDL it waits before reading logits / cum. */
 size_t b200_beam_search_step_workspace_bytes(int batch, int beam_width, int vocab);
 int b200_beam_search_step(const void* logits, int dtype, const float* cum_log_probs, int batch, int beam_width, int vocab, int eos_id,
                           int32_t* cand_token, int32_t* cand_parent, float* cand_score, int32_t* next_token, int32_t* next_parent,
                           float* next_cum, void* workspace, size_t workspace_bytes, void* stream);
+
+/* The finished-hypothesis set of beam search, per request, on the device (Hugging Face BeamHypotheses / BeamSearchScorer and
+ * TRT-LLM's device-side finished candidates, restated; parity with the reference's kernels unpinned). W = beam_width in 1..32.
+ * State: b200_beam_hypotheses_state_bytes(batch, W, max_len) bytes owned by the caller; request b owns the stride
+ * = 16 + 16*W + 4*W*max_len bytes at b * stride:
+ *   int32 count (filled slots, 0..W), int32 next_order (insertion order of the next hypothesis), int32 pad[2];
+ *   W slots of {float cum (raw log-prob), float score, int32 len (generated tokens), int32 order}; slots 0..count-1 are filled;
+ *   int32 tokens [W][max_len]: slot k's path, its first min(len, max_len) entries (the rest is undefined).
+ * All-zero bytes are the empty set, so restarting from the prompt is a memset. done int32 [batch], also caller-owned and zeroed
+ * with the state: set once a request is done and never cleared.
+ * A hypothesis of raw log-prob cum and L generated tokens scores s = cum / L^alpha in fp32 (exactly cum at alpha 0), alpha =
+ * length_penalty[b]. It enters a set of fewer than W, or a full set when s > the set's lowest score (strictly), evicting the
+ * lowest (the earliest inserted among equal lowest scores).
+ * history [batch*W][hist_stride], hist_len [batch*W] (clamped to hist_stride): each beam's token history; its generated tokens
+ * are history[row][gen_start : hist_len[row]] (none when hist_len <= gen_start).
+ *
+ * b200_beam_hypotheses_update: after b200_beam_search_step (its cand_token / cand_parent / cand_score [batch][2W]) and before
+ * the history rows are forked. One CTA per request; a request with done[b] set is skipped entirely. Ranks r = 0..W-1 in order:
+ * a candidate whose token is eos_id and whose score is finite becomes a hypothesis with cum = its score, the path of row
+ * b*W + cand_parent followed by eos_id (kept up to max_len tokens) and L = that row's generated tokens + 1. EOS at rank >= W is
+ * ignored. Then, with a full set, the request is done when early_stopping[b] is 1, or (0, and 2 at alpha <= 0) when
+ * worst >= cand_score[b][0] / L^alpha, L the generated length of rank 0's candidate (its parent row's + 1), or (2 = "never",
+ * alpha > 0) when worst >= cand_score[b][0] / max_len^alpha. Any other early_stopping value counts as 0. eos_id >= 0.
+ * b200_beam_hypotheses_finalize: the n (1..W) best of each request's set into out_tokens [batch][n][max_len], out_len,
+ * out_score (= s), out_cum [batch][n], sorted by score descending, the earlier inserted first among equal scores. For a request
+ * that is not done, the W live beams are merged in first by the same rule, in rank order: beam i has cum beam_cum[b][i]
+ * ([batch][W]) and the path history[b*W + i][gen_start : hist_len] without EOS (a beam with a non-finite cum or no generated
+ * token is left out). Token slots past a path are -1; a missing hypothesis has tokens -1, len -1, score and cum -inf. The state
+ * and done are only read, so it may run after any step and again later.
+ * Both: deterministic, graph-capturable, allocate nothing; under PDL they wait before reading anything. */
+size_t b200_beam_hypotheses_state_bytes(int batch, int beam_width, int max_len);
+int b200_beam_hypotheses_update(const int32_t* cand_token, const int32_t* cand_parent, const float* cand_score, const int32_t* history,
+                                const int32_t* hist_len, int hist_stride, int gen_start, int batch, int beam_width, int eos_id,
+                                const float* length_penalty, const int32_t* early_stopping, int max_len, void* state,
+                                size_t state_bytes, int32_t* done, void* stream);
+int b200_beam_hypotheses_finalize(const void* state, size_t state_bytes, const int32_t* done, const float* beam_cum,
+                                  const int32_t* history, const int32_t* hist_len, int hist_stride, int gen_start, int batch,
+                                  int beam_width, int n, int max_len, const float* length_penalty, int32_t* out_tokens,
+                                  int32_t* out_len, float* out_score, float* out_cum, void* stream);
 
 /* Per-token log-probabilities of the lm_head output (OpenAI-style logprobs / top_logprobs), without copying the probabilities
  * to the host. logits [rows][vocab], dtype 0 fp16, 1 bf16, 2 fp32, read as they are. Each row's lp(i) = (x_i - m) - log sum_v

@@ -55,6 +55,10 @@ SIGNATURES = {
     "b200_spec_verify": (c_int, [c_void_p] * 5 + [c_int] * 3 + [c_void_p] * 3),
     "b200_beam_search_step_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "b200_beam_search_step": (c_int, [c_void_p, c_int, c_void_p] + [c_int] * 4 + [c_void_p] * 7 + [c_size_t, c_void_p]),
+    "b200_beam_hypotheses_state_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "b200_beam_hypotheses_update": (c_int, [c_void_p] * 5 + [c_int] * 5 + [c_void_p, c_void_p, c_int, c_void_p, c_size_t, c_void_p,
+                                                                         c_void_p]),
+    "b200_beam_hypotheses_finalize": (c_int, [c_void_p, c_size_t] + [c_void_p] * 4 + [c_int] * 6 + [c_void_p] * 6),
     "b200_token_logprobs_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "b200_token_logprobs": (c_int, [c_void_p] + [c_int] * 4 + [c_void_p] * 5 + [c_size_t, c_void_p]),
     "b200_ban_repeat_ngram": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),

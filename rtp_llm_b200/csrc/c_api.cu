@@ -1162,6 +1162,97 @@ int b200_beam_search_step(const void* logits, int dtype, const float* cum_log_pr
     return dtype == 2 ? launch(0.f) : by_dtype(dtype == 1, launch);
 }
 
+size_t b200_beam_hypotheses_state_bytes(int batch, int beam_width, int max_len) {
+    if (batch < 0 || beam_width < 1 || beam_width > kBeamMaxWidth || max_len < 1 || max_len > (1 << 24)) return 0;
+    return (size_t)batch * beam_hyps_stride(beam_width, max_len);
+}
+
+// The checks both beam-hypothesis entries share
+#define BEAM_HYPS_CHECKS(who)                                                                                                   \
+    ARG_CHECK(beam_width >= 1 && beam_width <= kBeamMaxWidth, who ": beam_width %d unsupported (1..%d)", beam_width,          \
+              kBeamMaxWidth);                                                                                                 \
+    ARG_CHECK(max_len >= 1 && max_len <= (1 << 24), who ": max_len %d unsupported (1..%d)", max_len, 1 << 24);                \
+    ARG_CHECK(batch >= 0 && batch <= 65535, who ": batch %d unsupported (0..65535)", batch);                                  \
+    ARG_CHECK(hist_stride >= 1 && gen_start >= 0, who ": hist_stride %d must be >= 1 and gen_start %d >= 0", hist_stride,     \
+              gen_start)
+
+int b200_beam_hypotheses_update(const int32_t* cand_token, const int32_t* cand_parent, const float* cand_score, const int32_t* history,
+                                const int32_t* hist_len, int hist_stride, int gen_start, int batch, int beam_width, int eos_id,
+                                const float* length_penalty, const int32_t* early_stopping, int max_len, void* state,
+                                size_t state_bytes, int32_t* done, void* stream) {
+    BEAM_HYPS_CHECKS("beam_hypotheses_update");
+    ARG_CHECK(eos_id >= 0, "beam_hypotheses_update: eos_id %d must be >= 0", eos_id);
+    if (batch == 0) return B200_OK;
+    ARG_CHECK(cand_token && cand_parent && cand_score && history && hist_len && length_penalty && early_stopping && state && done,
+              "beam_hypotheses_update: null pointer");
+    const size_t need = b200_beam_hypotheses_state_bytes(batch, beam_width, max_len);
+    ARG_CHECK(state_bytes >= need, "beam_hypotheses_update: state too small (%zu < %zu bytes, see b200_beam_hypotheses_state_bytes)",
+              state_bytes, need);
+    if (g_rec)
+        return rec_call([=](void* st) {
+            return b200_beam_hypotheses_update(cand_token, cand_parent, cand_score, history, hist_len, hist_stride, gen_start, batch,
+                                               beam_width, eos_id, length_penalty, early_stopping, max_len, state, state_bytes, done,
+                                               st);
+        });
+    BeamHypsParams p{};
+    p.cand_token = cand_token;
+    p.cand_parent = cand_parent;
+    p.cand_score = cand_score;
+    p.history = history;
+    p.hist_len = hist_len;
+    p.length_penalty = length_penalty;
+    p.early_stopping = early_stopping;
+    p.state = static_cast<char*>(state);
+    p.done = done;
+    p.W = beam_width;
+    p.max_len = max_len;
+    p.hist_stride = hist_stride;
+    p.gen_start = gen_start;
+    p.eos = eos_id;
+    CUDA_CHECK(launch_ex(beam_hyps_update_kernel, {dim3(batch), dim3(kBeamHypThreads), 0, (cudaStream_t)stream, g_pdl.load() != 0},
+                         p));
+    return launched("beam_hyps_update_kernel");
+}
+
+int b200_beam_hypotheses_finalize(const void* state, size_t state_bytes, const int32_t* done, const float* beam_cum,
+                                  const int32_t* history, const int32_t* hist_len, int hist_stride, int gen_start, int batch,
+                                  int beam_width, int n, int max_len, const float* length_penalty, int32_t* out_tokens,
+                                  int32_t* out_len, float* out_score, float* out_cum, void* stream) {
+    BEAM_HYPS_CHECKS("beam_hypotheses_finalize");
+    ARG_CHECK(n >= 1 && n <= beam_width, "beam_hypotheses_finalize: n %d unsupported (1..beam_width %d)", n, beam_width);
+    if (batch == 0) return B200_OK;
+    ARG_CHECK(state && done && beam_cum && history && hist_len && length_penalty && out_tokens && out_len && out_score && out_cum,
+              "beam_hypotheses_finalize: null pointer");
+    const size_t need = b200_beam_hypotheses_state_bytes(batch, beam_width, max_len);
+    ARG_CHECK(state_bytes >= need, "beam_hypotheses_finalize: state too small (%zu < %zu bytes, see b200_beam_hypotheses_state_bytes)",
+              state_bytes, need);
+    if (g_rec)
+        return rec_call([=](void* st) {
+            return b200_beam_hypotheses_finalize(state, state_bytes, done, beam_cum, history, hist_len, hist_stride, gen_start, batch,
+                                                 beam_width, n, max_len, length_penalty, out_tokens, out_len, out_score, out_cum, st);
+        });
+    BeamHypsParams p{};
+    p.beam_cum = beam_cum;
+    p.history = history;
+    p.hist_len = hist_len;
+    p.length_penalty = length_penalty;
+    p.state = const_cast<char*>(static_cast<const char*>(state));
+    p.done = const_cast<int32_t*>(done);
+    p.out_tokens = out_tokens;
+    p.out_len = out_len;
+    p.out_score = out_score;
+    p.out_cum = out_cum;
+    p.W = beam_width;
+    p.n = n;
+    p.max_len = max_len;
+    p.hist_stride = hist_stride;
+    p.gen_start = gen_start;
+    CUDA_CHECK(launch_ex(beam_hyps_finalize_kernel, {dim3(batch), dim3(kBeamHypThreads), 0, (cudaStream_t)stream, g_pdl.load() != 0},
+                         p));
+    return launched("beam_hyps_finalize_kernel");
+}
+#undef BEAM_HYPS_CHECKS
+
 namespace {
 // Byte offsets of the log-prob kernel's workspace arrays (LogprobParams), each 256-byte aligned; total = 0 for an unsupported
 // shape.

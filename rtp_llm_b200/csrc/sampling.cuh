@@ -583,6 +583,210 @@ __global__ void __launch_bounds__(kBeamThreads) beam_search_kernel(const BeamPar
     }
 }
 
+// ------------------------------------------------------------------------------------------------ beam hypotheses
+// The finished-hypothesis set of beam search (Hugging Face BeamHypotheses / TRT-LLM's device-side finished candidates), kept
+// on the device so that a step under graph replay needs no host round trip. Request b owns the bytes
+// [b * stride, (b + 1) * stride) of the caller's state, stride = beam_hyps_stride(W, max_len): a BeamHypHeader, W BeamHyp
+// slots, then W token rows of max_len int32. Slots 0 .. count-1 are filled; all-zero bytes are the empty set.
+// A hypothesis of raw log-prob cum and L generated tokens scores s = cum / L^alpha (fp32; exactly cum at alpha 0). It enters a
+// set of fewer than W, or replaces the full set's lowest s (the earliest inserted among equal ones) when its s is strictly
+// greater. Every decision runs in thread 0 in a fixed order and the CTA only copies paths: deterministic.
+constexpr int kBeamHypThreads = 128;
+
+struct BeamHypHeader {
+    int32_t count, next_order, pad[2];   // filled slots; insertion order of the next hypothesis
+};
+struct BeamHyp {
+    float cum, score;                    // raw cum log-prob, cum / len^alpha
+    int32_t len, order;                  // generated tokens (EOS included for a finished one), insertion order
+};
+
+__host__ __device__ inline size_t beam_hyps_stride(int W, int max_len) {
+    return sizeof(BeamHypHeader) + (size_t)W * sizeof(BeamHyp) + (size_t)W * max_len * sizeof(int32_t);
+}
+
+struct BeamHypsParams {
+    const int32_t* cand_token;       // [B][2W] (update)
+    const int32_t* cand_parent;      // [B][2W] (update)
+    const float* cand_score;         // [B][2W] (update)
+    const float* beam_cum;           // [B][W] (finalize)
+    const int32_t* history;          // [B*W][hist_stride]
+    const int32_t* hist_len;         // [B*W], clamped to hist_stride
+    const float* length_penalty;     // [B]
+    const int32_t* early_stopping;   // [B] (update): 1 true, 2 never, anything else false
+    char* state;                     // [B][stride]; finalize only reads it
+    int32_t* done;                   // [B]
+    int32_t* out_tokens;             // [B][n][max_len] (finalize)
+    int32_t* out_len;                // [B][n]
+    float* out_score;                // [B][n]
+    float* out_cum;                  // [B][n]
+    int W, n, max_len, hist_stride, gen_start, eos;
+};
+
+// Not inlined: the update and the finalize kernel run this one code, so equal (cum, L) give equal bits in both (an inlined copy
+// may be contracted into FMAs differently in each kernel, and a 1-ulp difference would reorder equal hypotheses).
+__device__ __noinline__ float beam_hyp_norm(float cum, int L, float alpha) {
+    return alpha == 0.f ? cum : cum / powf((float)L, alpha);
+}
+
+// Generated tokens in a history row: history[row][gen_start : hist_len[row]] (empty when hist_len <= gen_start)
+__device__ __forceinline__ int beam_hyp_gen(const BeamHypsParams& p, int row) {
+    return max(0, min(p.hist_len[row], p.hist_stride) - p.gen_start);
+}
+
+// The slot a hypothesis of score s takes among the `count` filled slots of h [W]: the next free one, or in a full set the one
+// with the lowest score (the earliest inserted among equal ones) when s is strictly greater; -1 when it does not enter.
+__device__ __forceinline__ int beam_hyp_slot(const BeamHyp* h, int count, int W, float s) {
+    if (count < W) return count;
+    int w = 0;
+    for (int k = 1; k < W; ++k)
+        if (h[k].score < h[w].score || (h[k].score == h[w].score && h[k].order < h[w].order)) w = k;
+    return s > h[w].score ? w : -1;
+}
+
+// After b200_beam_search_step, before the fork: the EOS candidates among ranks 0..W-1 of request b (one CTA each) enter its
+// set, then the done test. Their path is the parent row's generated history followed by EOS (truncated to max_len tokens;
+// len and the score count them all). Every input thread 0's decisions read is staged in shared memory first, by all threads at
+// once, so the serial part issues no global load.
+__global__ void __launch_bounds__(kBeamHypThreads) beam_hyps_update_kernel(const BeamHypsParams p) {
+    __shared__ BeamHyp sh[kBeamMaxWidth];
+    __shared__ int s_src[kBeamMaxWidth];     // per slot: the rank whose path it takes in this call, -1 none
+    __shared__ int s_tok[kBeamMaxWidth], s_par[kBeamMaxWidth], s_gen[kBeamMaxWidth];   // rank r: token, parent, its generated
+    __shared__ float s_score[kBeamMaxWidth];                                           // tokens (-1: parent out of range), score
+    const int b = blockIdx.x, W = p.W, K = 2 * W, tid = threadIdx.x;
+    pdl_wait();                              // under PDL the candidates and the history come from the kernels before this one
+    const bool was_done = p.done[b] != 0;
+    char* st = p.state + (size_t)b * beam_hyps_stride(W, p.max_len);
+    BeamHypHeader* hd = reinterpret_cast<BeamHypHeader*>(st);
+    BeamHyp* meta = reinterpret_cast<BeamHyp*>(st + sizeof(BeamHypHeader));
+    int32_t* tok = reinterpret_cast<int32_t*>(meta + W);
+    const int count0 = min(max(hd->count, 0), W), order0 = hd->next_order;
+    const float alpha = p.length_penalty[b];
+    const int es = p.early_stopping[b];
+    for (int r = tid; r < W; r += kBeamHypThreads) {
+        const size_t c = (size_t)b * K + r;
+        const int par = p.cand_parent[c];
+        s_tok[r] = p.cand_token[c];
+        s_score[r] = p.cand_score[c];
+        s_par[r] = par;
+        s_gen[r] = (par >= 0 && par < W) ? beam_hyp_gen(p, b * W + par) : -1;
+        if (r < count0) sh[r] = meta[r];
+        s_src[r] = -1;
+    }
+    __syncthreads();                         // the staging, and every thread has read done before thread 0 may set it
+    if (was_done) return;
+    if (tid == 0) {
+        int count = count0, order = order0;
+        for (int r = 0; r < W; ++r) {
+            const float c = s_score[r];
+            if (s_tok[r] != p.eos || !isfinite(c) || s_gen[r] < 0) continue;
+            const int L = s_gen[r] + 1;
+            const float s = beam_hyp_norm(c, L, alpha);
+            const int k = beam_hyp_slot(sh, count, W, s);
+            if (k < 0) continue;
+            sh[k] = BeamHyp{c, s, L, order++};
+            s_src[k] = r;
+            if (k == count) ++count;
+        }
+        bool done = false;
+        if (count == W) {
+            if (es == 1) {
+                done = true;
+            } else {
+                float worst = sh[0].score;
+                for (int k = 1; k < W; ++k) worst = fminf(worst, sh[k].score);
+                const int L = (es == 2 && alpha > 0.f) ? p.max_len : max(s_gen[0], 0) + 1;
+                done = worst >= beam_hyp_norm(s_score[0], L, alpha);
+            }
+        }
+        for (int k = 0; k < count; ++k)
+            if (s_src[k] >= 0) meta[k] = sh[k];
+        hd->count = count;
+        hd->next_order = order;
+        if (done) p.done[b] = 1;
+    }
+    __syncthreads();
+    for (int k = 0; k < W; ++k) {
+        const int r = s_src[k];
+        if (r < 0) continue;
+        const int row = b * W + s_par[r], g = s_gen[r], L = min(g + 1, p.max_len);
+        const int32_t* src = p.history + (size_t)row * p.hist_stride + p.gen_start;
+        int32_t* dst = tok + (size_t)k * p.max_len;
+        for (int j = tid; j < L; j += kBeamHypThreads) dst[j] = j < g ? src[j] : p.eos;
+    }
+}
+
+// The n best of request b's set (one CTA each), with the W live beams merged in first when the request is not done: beam i
+// (rank order) has cum beam_cum[b][i] and the path history[b*W + i][gen_start : hist_len] without EOS; a beam with a non-finite
+// cum or no generated token is left out. Sorted by score descending, the earlier inserted first among equal ones; token slots
+// past a path and missing hypotheses are -1 (len -1, score and cum -inf). The state is only read.
+__global__ void __launch_bounds__(kBeamHypThreads) beam_hyps_finalize_kernel(const BeamHypsParams p) {
+    __shared__ BeamHyp sh[kBeamMaxWidth];
+    __shared__ int s_src[kBeamMaxWidth];     // per slot: -1 the state's path, i >= 0 live beam i
+    __shared__ int s_pick[kBeamMaxWidth];    // output j -> slot
+    __shared__ int s_gen[kBeamMaxWidth];     // live beam i: generated tokens
+    __shared__ float s_cum[kBeamMaxWidth];   // live beam i: cum
+    __shared__ int s_found;
+    const int b = blockIdx.x, W = p.W, n = p.n, tid = threadIdx.x;
+    pdl_wait();                              // under PDL the state, the beams and the history come from the kernels before this one
+    const char* st = p.state + (size_t)b * beam_hyps_stride(W, p.max_len);
+    const BeamHypHeader* hd = reinterpret_cast<const BeamHypHeader*>(st);
+    const BeamHyp* meta = reinterpret_cast<const BeamHyp*>(st + sizeof(BeamHypHeader));
+    const int32_t* tok = reinterpret_cast<const int32_t*>(meta + W);
+    const int count0 = min(max(hd->count, 0), W), order0 = hd->next_order;
+    const float alpha = p.length_penalty[b];
+    const bool done = p.done[b] != 0;
+    for (int i = tid; i < W; i += kBeamHypThreads) {     // staged by all threads at once, as in the update
+        s_cum[i] = p.beam_cum[(size_t)b * W + i];
+        s_gen[i] = beam_hyp_gen(p, b * W + i);
+        if (i < count0) sh[i] = meta[i];
+        s_src[i] = -1;
+    }
+    __syncthreads();
+    if (tid == 0) {
+        int count = count0, order = order0;
+        if (!done) {
+            for (int i = 0; i < W; ++i) {
+                const float c = s_cum[i];
+                const int L = s_gen[i];
+                if (!isfinite(c) || L < 1) continue;
+                const float s = beam_hyp_norm(c, L, alpha);
+                const int k = beam_hyp_slot(sh, count, W, s);
+                if (k < 0) continue;
+                sh[k] = BeamHyp{c, s, L, order++};
+                s_src[k] = i;
+                if (k == count) ++count;
+            }
+        }
+        for (int k = 0; k < count; ++k) {
+            int r = 0;
+            for (int m = 0; m < count; ++m)
+                r += (sh[m].score > sh[k].score || (sh[m].score == sh[k].score && sh[m].order < sh[k].order)) ? 1 : 0;
+            if (r < n) s_pick[r] = k;
+        }
+        s_found = min(count, n);
+        for (int j = 0; j < n; ++j) {
+            const size_t o = (size_t)b * n + j;
+            const bool have = j < s_found;
+            p.out_len[o] = have ? sh[s_pick[j]].len : -1;
+            p.out_score[o] = have ? sh[s_pick[j]].score : -INFINITY;
+            p.out_cum[o] = have ? sh[s_pick[j]].cum : -INFINITY;
+        }
+    }
+    __syncthreads();
+    for (int j = 0; j < n; ++j) {
+        int32_t* dst = p.out_tokens + ((size_t)b * n + j) * p.max_len;
+        int L = 0;
+        const int32_t* src = nullptr;
+        if (j < s_found) {
+            const int k = s_pick[j], i = s_src[k];
+            L = min(sh[k].len, p.max_len);
+            src = i < 0 ? tok + (size_t)k * p.max_len : p.history + (size_t)(b * W + i) * p.hist_stride + p.gen_start;
+        }
+        for (int t = tid; t < p.max_len; t += kBeamHypThreads) dst[t] = t < L ? src[t] : -1;
+    }
+}
+
 // ------------------------------------------------------------------------------------------------ token log-probabilities
 // Per row of the [rows][V] lm_head logits, in fp32, lp(i) = (x_i - m) - log sum_v exp(x_v - m) with m the row max: the log-softmax
 // of the logits as given, i.e. the raw model distribution before temperature, penalties and top-k / top-p. Outputs the drawn

@@ -163,6 +163,13 @@ class DecodeStep:
     become next_token and the lengths grow by one: the next call runs the next step. upload_inputs() restarts from the prompt;
     a step past max_new_tokens since then raises ValueError (the page-table rows end there), in run() and in replay().
     The device state: beam_cum [B, W], hist [B*W, ctx] / hist_len [B*W], beam_out (the beam_search_step outputs).
+    With eos_id, finished hypotheses are kept on the device: beam_search_step runs with that EOS (the next beams skip it), then
+    beam_hypotheses_update moves the EOS candidates among the first W ranks into each request's set (hyp_state, up to W paths
+    of max_new_tokens; history from hist[:, 1:], hist[:, 0] being the input token) before the fork. length_penalty (alpha,
+    score = cum / len^alpha) and early_stopping (False, True or "never") take one value for every request or one per request.
+    done [B] (int32, device) is set when a request's set is done; its beams keep computing (the graph is static) but its
+    hypotheses stay as they are. beam_results(n) returns the n best per request, the live beams merged in for requests that are
+    not done. upload_inputs() empties the sets and done. With eos_id None the step is the beam step without EOS.
 
     sampling=SamplingParams (TP 1, beam_width 1, batch * q_len <= 128, op by op or under a CUDA graph; not in a decode program):
     sampled decoding. The per-request parameters sit in static device buffers; after the lm_head the step copies the logits to a
@@ -184,7 +191,9 @@ class DecodeStep:
                  pdl: bool = False, comm=None, fuse_silu: bool = True, fuse_ar_norm: bool = True, fuse_rope: Optional[bool] = None,
                  fuse_gemm_rs: Optional[bool] = None, act_order: bool = False, q_len: int = 1, beam_width: int = 1,
                  no_repeat_ngram: int = 0, max_new_tokens: int = 16, sampling: Optional[SamplingParams] = None,
-                 logprobs: Optional[int] = None):
+                 logprobs: Optional[int] = None, eos_id: Optional[int] = None,
+                 length_penalty: Union[float, Sequence[float]] = 1.0,
+                 early_stopping: Union[bool, str, Sequence[Union[bool, str]]] = False):
         assert cfg.head_num % tp_size == 0 and cfg.inter % tp_size == 0
         if q_len < 1:
             raise ValueError(f"q_len must be >= 1 (got {q_len})")
@@ -215,6 +224,23 @@ class DecodeStep:
         if no_repeat_ngram != 0 and beam_width == 1 and sampling is None:
             raise ValueError(f"no_repeat_ngram {no_repeat_ngram} needs beam search (beam_width > 1); the greedy step has no ban")
         self.W, self.ngram, self.max_new_tokens = beam_width, no_repeat_ngram, max_new_tokens
+        if eos_id is not None:
+            if beam_width == 1 or not 0 <= eos_id < cfg.vocab:
+                raise ValueError(f"eos_id needs beam search (beam_width > 1) and must be in 0..vocab-1 (got eos_id {eos_id}, "
+                                 f"beam_width {beam_width})")
+
+            def per_request(v, name):
+                vals = list(v) if isinstance(v, (list, tuple)) else [v] * batch
+                if len(vals) != batch:
+                    raise ValueError(f"{name}: {len(vals)} values for {batch} requests")
+                return vals
+            alphas = [float(a) for a in per_request(length_penalty, "length_penalty")]
+            modes = per_request(early_stopping, "early_stopping")
+            for m in modes:
+                if m not in (False, True, "never"):
+                    raise ValueError(f"early_stopping must be False, True or \"never\" (got {m!r})")
+            modes = [2 if m == "never" else int(bool(m)) for m in modes]
+        self.eos_id = eos_id
         self.beam_steps = 0                             # beam / sampled steps run since the prompt (upload_inputs)
         self.requests = batch
         batch = batch * beam_width                      # sequences (page-table rows) of the step
@@ -451,6 +477,11 @@ class DecodeStep:
             self.hist_parent = buf(R, ctx, dt=torch.int32)
             self.len_parent = buf(R, dt=torch.int32)
             self.page_scratch = buf(R, 2, self.Hkv, T, self.D)
+            if eos_id is not None:    # the finished-hypothesis sets (emptied by upload_inputs)
+                self.hyp_state = ops.beam_hypotheses_state(B, W, max_new_tokens, device)
+                self.done = torch.zeros(B, dtype=torch.int32, device=device)
+                self.length_penalty = torch.tensor(alphas, dtype=torch.float32, device=device)
+                self.early_stopping = torch.tensor(modes, dtype=torch.int32, device=device)
         if sampling is not None:
             def per_row(v, dt):
                 t = torch.tensor(v if isinstance(v, (list, tuple)) else [v] * batch, dtype=dt)
@@ -509,6 +540,9 @@ class DecodeStep:
             self.hist[:, 0].copy_(self.ids)
             self.hist_len.fill_(1)
             self.beam_steps = 0
+            if self.eos_id is not None:
+                self.hyp_state.zero_()
+                self.done.zero_()
         if self.samp is not None:  # back to the prompt: step 0 of the uniforms; at q_len 1 the input token as the whole history
             self.draw_step.zero_()
             if self.q_len == 1:
@@ -612,7 +646,11 @@ class DecodeStep:
         if self.W > 1:
             if self.ngram > 0:
                 ops.ban_repeat_ngram(self.logits, self.hist, self.hist_len, self.ngram_size)
-            ops.beam_search_step(self.logits, self.beam_cum, self.W, workspace=self.beam_ws, out=self.beam_out)
+            ops.beam_search_step(self.logits, self.beam_cum, self.W, eos_id=-1 if self.eos_id is None else self.eos_id,
+                                 workspace=self.beam_ws, out=self.beam_out)
+            if self.eos_id is not None:    # between the beam step and the fork: the history rows are still the parents'
+                ops.beam_hypotheses_update(self.beam_out, self.hist, self.hist_len, self.eos_id, self.length_penalty,
+                                           self.early_stopping, self.hyp_state, self.done, self.max_new_tokens, gen_start=1)
             self.fork()
         elif self.samp is not None:
             self.sample()
@@ -662,6 +700,16 @@ class DecodeStep:
             L["kv"].index_copy_(0, self.dst_page, self.page_scratch)
         self.ids.copy_(o["next_token"].view(-1))
         self.seq_lens.add_(1)
+
+    def beam_results(self, n: int) -> Dict[str, torch.Tensor]:
+        """Beam mode with eos_id: the n (1..W) best hypotheses of each request now (beam_hypotheses_finalize on the current state,
+        which it leaves as it is), as host tensors: tokens int32 [B, n, max_new_tokens] (the generated tokens, -1 past each
+        path), len int32 [B, n], score / cum fp32 [B, n]."""
+        if self.W == 1 or self.eos_id is None:
+            raise ValueError("beam_results needs the beam mode with an eos_id")
+        out = ops.beam_hypotheses_finalize(self.hyp_state, self.done, self.beam_cum, self.hist, self.hist_len, n, self.max_new_tokens,
+                                           self.length_penalty, gen_start=1)
+        return {k: v.cpu() for k, v in out.items()}
 
     def sample(self):
         """Sampling mode, after the lm_head (see the class docstring). b200 kernels and torch ops on static buffers only, so a CUDA

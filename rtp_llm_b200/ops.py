@@ -599,6 +599,86 @@ def beam_search_step(logits: torch.Tensor, cum_log_probs: torch.Tensor, beam_wid
     return out
 
 
+def beam_hypotheses_state(batch: int, beam_width: int, max_len: int, device) -> torch.Tensor:
+    """Empty finished-hypothesis sets (all-zero bytes) of `batch` requests, W = beam_width slots of up to max_len tokens each:
+    the state of beam_hypotheses_update / beam_hypotheses_finalize (layout in include/b200_decode_ops.h). zero_() restarts it."""
+    n = int(_lib.load().b200_beam_hypotheses_state_bytes(batch, beam_width, max_len))
+    if n == 0 and batch != 0:
+        raise B200Error(f"beam_hypotheses: unsupported shape batch {batch}, beam_width {beam_width}, max_len {max_len}")
+    return torch.zeros(n, dtype=torch.uint8, device=device)
+
+
+def _beam_hyps_checks(who: str, B: int, W: int, max_len: int, history, hist_len, length_penalty, state, done) -> None:
+    if not 1 <= W <= 32:
+        raise B200Error(f"{who}: beam_width {W} unsupported (1..32)")
+    if history.dtype != torch.int32 or history.dim() != 2 or history.shape[0] != B * W or history.shape[1] < 1:
+        raise B200Error(f"{who}: history must be int32 [{B * W}, stride >= 1]")
+    if hist_len.dtype != torch.int32 or hist_len.numel() != B * W:
+        raise B200Error(f"{who}: hist_len must be int32 [{B * W}]")
+    if length_penalty.dtype != torch.float32 or length_penalty.numel() != B:
+        raise B200Error(f"{who}: length_penalty must be fp32 [{B}]")
+    if done.dtype != torch.int32 or done.numel() != B:
+        raise B200Error(f"{who}: done must be int32 [{B}]")
+    need = int(_lib.load().b200_beam_hypotheses_state_bytes(B, W, max_len))
+    if state.dtype != torch.uint8 or (need == 0 and B != 0) or state.numel() < need:
+        raise B200Error(f"{who}: state must be uint8 of at least {need} bytes (beam_hypotheses_state({B}, {W}, {max_len}))")
+
+
+def beam_hypotheses_update(beam_out: dict, history: torch.Tensor, hist_len: torch.Tensor, eos_id: int, length_penalty: torch.Tensor,
+                           early_stopping: torch.Tensor, state: torch.Tensor, done: torch.Tensor, max_len: int,
+                           gen_start: int = 0) -> None:
+    """b200_beam_hypotheses_update, after beam_search_step and before the fork: the EOS candidates among the first W ranks of
+    beam_out (beam_search_step's cand_token / cand_parent / cand_score [B, 2W]) enter each request's finished set in `state`
+    (beam_hypotheses_state(B, W, max_len)), with the path history[B*W, stride][gen_start : hist_len] + eos_id. length_penalty
+    fp32 [B]; early_stopping int32 [B] (0 False, 1 True, 2 "never"); done int32 [B] is set once a request is done, and a done
+    request is left alone."""
+    ct = beam_out["cand_token"]
+    if ct.dim() != 2 or ct.shape[1] % 2:
+        raise B200Error(f"beam_hypotheses_update: cand_token must be [B, 2W] (got {tuple(ct.shape)})")
+    B, W = ct.shape[0], ct.shape[1] // 2
+    _beam_hyps_checks("beam_hypotheses_update", B, W, max_len, history, hist_len, length_penalty, state, done)
+    for k, dt in (("cand_token", torch.int32), ("cand_parent", torch.int32), ("cand_score", torch.float32)):
+        if beam_out[k].dtype != dt or beam_out[k].numel() != B * 2 * W:
+            raise B200Error(f"beam_hypotheses_update: {k} must be {dt} [{B}, {2 * W}]")
+    if early_stopping.dtype != torch.int32 or early_stopping.numel() != B:
+        raise B200Error(f"beam_hypotheses_update: early_stopping must be int32 [{B}]")
+    if eos_id < 0:
+        raise B200Error(f"beam_hypotheses_update: eos_id {eos_id} must be >= 0")
+    _cuda_contig(ct, beam_out["cand_parent"], beam_out["cand_score"], history, hist_len, length_penalty, early_stopping, state, done)
+    check(_lib.load().b200_beam_hypotheses_update(_p(ct), _p(beam_out["cand_parent"]), _p(beam_out["cand_score"]), _p(history),
+                                                  _p(hist_len), history.shape[1], gen_start, B, W, eos_id, _p(length_penalty),
+                                                  _p(early_stopping), max_len, _p(state), state.numel(), _p(done), _stream()),
+          "b200_beam_hypotheses_update")
+
+
+def beam_hypotheses_finalize(state: torch.Tensor, done: torch.Tensor, beam_cum: torch.Tensor, history: torch.Tensor,
+                             hist_len: torch.Tensor, n: int, max_len: int, length_penalty: torch.Tensor, gen_start: int = 0,
+                             out: Optional[dict] = None) -> dict:
+    """b200_beam_hypotheses_finalize: the n (1..W) best hypotheses of each request, the live beams (beam_cum fp32 [B, W] and
+    their history rows) merged in for a request that is not done. Returns dict(tokens int32 [B, n, max_len] (-1 past the
+    path), len int32 [B, n], score fp32 [B, n] (cum / len^length_penalty, descending), cum fp32 [B, n]); a missing
+    hypothesis has tokens and len -1, score and cum -inf. The state is not modified."""
+    if beam_cum.dtype != torch.float32 or beam_cum.dim() != 2:
+        raise B200Error(f"beam_hypotheses_finalize: beam_cum must be fp32 [B, W] (got {beam_cum.dtype} {tuple(beam_cum.shape)})")
+    B, W = beam_cum.shape
+    _beam_hyps_checks("beam_hypotheses_finalize", B, W, max_len, history, hist_len, length_penalty, state, done)
+    if not 1 <= n <= W:
+        raise B200Error(f"beam_hypotheses_finalize: n {n} unsupported (1..beam_width {W})")
+    shapes = dict(tokens=(torch.int32, (B, n, max_len)), len=(torch.int32, (B, n)), score=(torch.float32, (B, n)),
+                  cum=(torch.float32, (B, n)))
+    out = dict(out or {})
+    for k, (dtype, shape) in shapes.items():
+        if k not in out:
+            out[k] = torch.empty(shape, dtype=dtype, device=beam_cum.device)
+        elif out[k].dtype != dtype or out[k].numel() != math.prod(shape):
+            raise B200Error(f"beam_hypotheses_finalize: {k} must be {dtype} {list(shape)}")
+    _cuda_contig(state, done, beam_cum, history, hist_len, length_penalty, *out.values())
+    check(_lib.load().b200_beam_hypotheses_finalize(_p(state), state.numel(), _p(done), _p(beam_cum), _p(history), _p(hist_len),
+                                                    history.shape[1], gen_start, B, W, n, max_len, _p(length_penalty),
+                                                    *(_p(out[k]) for k in shapes), _stream()), "b200_beam_hypotheses_finalize")
+    return out
+
+
 LOGPROB_MAX_TOP_N = 64
 
 

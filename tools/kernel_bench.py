@@ -111,6 +111,45 @@ def bench_beam(B, W, V=128256, ngram=0, hist=2048, nrot=8):
     return us
 
 
+def bench_beam_hyps(B, W, max_len, nrot=8):
+    """b200_beam_hypotheses_update and b200_beam_hypotheses_finalize (n = W), each timed on its own. The update sees a
+    non-EOS best candidate of score 0 (so no request is ever done: every hypothesis scores below it), then EOS at ranks
+    1..2W-1 with fresh scores (rotated through nrot candidate sets), parent paths of max_len - 1 tokens, length penalty 1. "steady" keeps the state across calls: the sets are
+    full and a candidate enters only when it beats the worst. "empty" zeroes the state before every call (the memset is in the
+    time), so every call inserts W - 1 hypotheses and copies their paths of max_len tokens. Finalize merges W live beams of max_len - 1
+    tokens into the full sets and writes n = W."""
+    g = torch.Generator(device=dev).manual_seed(4)
+    K, R = 2 * W, B * W
+    cands = []
+    for _ in range(nrot):
+        score = -torch.rand(B, K, generator=g, device=dev).mul_(8.0).sort(dim=1).values
+        score[:, 0] = 0.0
+        token = torch.full((B, K), 2, dtype=torch.int32, device=dev)
+        token[:, 0] = 3
+        cands.append(dict(cand_token=token,
+                          cand_parent=torch.randint(0, W, (B, K), generator=g, device=dev, dtype=torch.int32), cand_score=score))
+    hist = torch.randint(0, 128256, (R, max_len), generator=g, device=dev, dtype=torch.int32)
+    hl = torch.full((R,), max_len, dtype=torch.int32, device=dev)
+    lp = torch.ones(B, device=dev)
+    es = torch.full((B,), 2, dtype=torch.int32, device=dev)
+    state = ops.beam_hypotheses_state(B, W, max_len, dev)
+    done = torch.zeros(B, dtype=torch.int32, device=dev)
+    cum = -torch.rand(B, W, generator=g, device=dev)
+    out = ops.beam_hypotheses_finalize(state, done, cum, hist, hl, W, max_len, lp, gen_start=1)
+
+    def update(i, empty):
+        if empty:
+            state.zero_()
+        ops.beam_hypotheses_update(cands[i], hist, hl, 2, lp, es, state, done, max_len, gen_start=1)
+    empty = timeit(lambda i: update(i, True), nrot)
+    up = timeit(lambda i: update(i, False), nrot)
+    fin = timeit(lambda i: ops.beam_hypotheses_finalize(state, done, cum, hist, hl, W, max_len, lp, gen_start=1, out=out), nrot)
+    assert int(done.sum()) == 0
+    print(f"beam-hyps B{B} W{W} max_len {max_len}: update steady {up:7.2f} us, empty (+ memset) {empty:7.2f} us, "
+          f"finalize {fin:7.2f} us", flush=True)
+    return up, empty, fin
+
+
 def bench_logprobs(B, top_n, V=128256, nrot=8):
     """b200_token_logprobs on fp16 logits [B, V] (rotated through nrot sets, > L2): the drawn token's log-prob and the top_n."""
     g = torch.Generator(device=dev).manual_seed(2)
@@ -300,6 +339,14 @@ if __name__ == "__main__":
                 for n in t:
                     t[n].append(bench_beam(B, W, ngram=n))
             print(f"beam B{B} W{W} V128256 median: step {sorted(t[0])[1]:.1f} us, ban n3 + step {sorted(t[3])[1]:.1f} us", flush=True)
+    if "beam-hyps" in which:
+        # the finished-hypothesis update and finalize at the beam step's shapes, short and long paths; medians of 3
+        for B, W in ((8, 4), (32, 4), (4, 16)):
+            for L in (16, 512):
+                t = [bench_beam_hyps(B, W, L) for _ in range(3)]
+                m = [sorted(x[k] for x in t)[1] for k in range(3)]
+                print(f"beam-hyps B{B} W{W} max_len {L} median: update steady {m[0]:.2f} us, empty (+ memset) {m[1]:.2f} us, "
+                      f"finalize {m[2]:.2f} us", flush=True)
     if "logprobs" in which:
         # the log-prob kernel over Llama-3's vocabulary at B 32: the drawn token's log-prob alone, and with the top 5 / 20
         t = {n: sorted(bench_logprobs(32, n) for _ in range(3))[1] for n in (0, 5, 20)}

@@ -4,8 +4,9 @@ each a step captured in a CUDA graph with PDL at --ctx tokens; the first arm is 
 
   act-order  Llama-3-8B INT4: plain, then act_order=True (three gathers per layer; w2's order is folded into w13)
   spec       Llama-3-8B INT4 (--model llama31: Llama-3.1-8B with its Llama3 rope): q_len 1, 2, 4 with batch * q_len <= 128
-  beam       Llama-3-8B INT4: the greedy step at batch * W rows, the beam step (W beams per request, --ngram ban), and the
-             fork alone as a graph of DecodeStep.fork()
+  beam       Llama-3-8B INT4: the greedy step at batch * W rows, the beam step (W beams per request, --ngram ban), with --eos
+             the beam step that also keeps the finished hypotheses (eos_id set), and the fork alone as a graph of
+             DecodeStep.fork()
   sample     Llama-3-8B INT4: greedy, then sampled (temperature 0.8, top-k 50, top-p 0.9, repetition 1.1, the drawn token's
              log-prob and the top 5)
   qwen3      Qwen3-8B INT4: qk_rmsnorm, then the plain rope launch (TwoLaunchStep), against the fused QK-norm append
@@ -69,6 +70,12 @@ def beam_arms(a, cfg, B, dev):
     model = DecodeStep(cfg, B, a.ctx, dev, pdl=True, beam_width=W, no_repeat_ngram=a.ngram, max_new_tokens=max_new_tokens(a))
     beam = step_arm(f"beam W{W}", model)
     model.replay()                          # beam_out holds a real selection for the fork graph to replay
+    hyps = []
+    if a.eos:                               # EOS = request 0's best candidate at step 1: hypotheses enter from the first step
+        eos = int(model.beam_out["cand_token"][0, 0])
+        print(f"B{B} beam W{W} + hyps: eos_id {eos}", flush=True)
+        hyps = [step_arm(f"beam W{W} + hyps", DecodeStep(cfg, B, a.ctx, dev, pdl=True, beam_width=W, no_repeat_ngram=a.ngram,
+                                                         max_new_tokens=max_new_tokens(a), eos_id=eos))]
     s = torch.cuda.Stream()
     s.wait_stream(torch.cuda.current_stream())
     with torch.cuda.stream(s):
@@ -79,7 +86,7 @@ def beam_arms(a, cfg, B, dev):
         model.fork()
     model.upload_inputs()
     torch.cuda.synchronize()
-    return [greedy, beam, Arm("fork", fork.replay, None, (model,))]
+    return [greedy, beam] + hyps + [Arm("fork", fork.replay, None, (model,))]
 
 
 def sample_arms(a, cfg, B, dev):
@@ -116,6 +123,8 @@ def parse(argv=None):
         if name == "beam":
             p.add_argument("--beam-width", type=int, default=4)
             p.add_argument("--ngram", type=int, default=0, help="no-repeat-ngram size of the beam step (default 0: off)")
+            p.add_argument("--eos", action="store_true", help="add the beam step with finished-hypothesis tracking (eos_id: "
+                                                              "request 0's best candidate at step 1)")
         p.set_defaults(arms=arms)
     a = ap.parse_args(argv)
     a.cfg = QWEN3_8B if a.preset == "qwen3" else MODELS[getattr(a, "model", "llama3")]
@@ -156,7 +165,7 @@ def main(argv=None):
     res = dict(device=torch.cuda.get_device_name(0), nvidia_smi_name_power_limit_sm_clock=card, preset=a.preset,
                model=a.cfg.name, ctx=a.ctx, runs=a.runs, iters=a.iters, warmup=a.warmup, batches=[])
     if a.preset == "beam":
-        res.update(beam_width=a.beam_width, ngram=a.ngram)
+        res.update(beam_width=a.beam_width, ngram=a.ngram, eos=a.eos)
     try:
         for B in a.batch:
             arms = a.arms(a, a.cfg, B, dev)
