@@ -119,6 +119,24 @@ int b200_paged_decode_attn_rope(const void* qkv, int is_bf16, void* out, size_t 
                                 const int32_t* page_list, const uint32_t* sequence_lengths, float q_scale, float rope_base,
                                 void* workspace, size_t workspace_bytes, void* stream);
 
+/* Beam search: the attention of `requests` requests with beam_width beams each, reading what a request's beams share once for all
+ * of them. Replaces runXqa with XQAParams::beam_width > 1 (CudaXqa.h:10-16, 65-84; XQA's beamWidth, 3rdparty/xqa/mha_sm90.cu:
+ * ctaNbValidQHeads = headGrpSize * beamWidth), which b200_paged_decode_attn serves as requests * beam_width unrelated sequences.
+ *   q, out, page_list, sequence_lengths   those of b200_paged_decode_attn with batch = requests * beam_width; row
+ *                b * beam_width + i is beam i of request b. Beams of a request may differ in length.
+ *   shared_lengths [requests] int32 (device-accessible): tokens of each request that all its beams share. Over the first
+ *                shared_lengths[b] / page_size pages the request's beam_width page_list rows must be equal; beam 0's are read.
+ *                The kernel rounds the value down to a multiple of 64 and keeps it at or below the shortest beam's
+ *                sequence_lengths (the token a step appends is never shared), so any value is safe under that contract and
+ *                0 shares nothing.
+ * Every output row has the bits it has with shared_lengths = 0, whatever is shared, and beam_width == 1 gives the bits of
+ * b200_paged_decode_attn. (head_num / kv_head_num) * beam_width <= 64; requests * kv_head_num <= 65535; max_seq_len bounds
+ * sequence_lengths[.] + 1; size the workspace with b200_paged_decode_attn_workspace_bytes(requests * beam_width, ...). */
+int b200_paged_decode_attn_beam(const void* q, int is_bf16, void* out, size_t head_num, size_t kv_head_num, size_t head_dim,
+                                size_t requests, size_t beam_width, size_t max_blocks_per_seq, size_t max_seq_len, size_t page_size,
+                                const void* kv_pool, const int32_t* page_list, const uint32_t* sequence_lengths,
+                                const int32_t* shared_lengths, float q_scale, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------------ weight-only GEMM */
 
 /* Load-time weight re-layout.  Replace CudaImpl.preprocess_weights_for_mixed_gemm (rtp_llm/device/device_impl.py:392-479):

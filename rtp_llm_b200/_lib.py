@@ -29,6 +29,8 @@ SIGNATURES = {
                                              c_float, c_void_p, c_size_t, c_void_p]),
     "b200_paged_decode_attn_rope": (c_int, [c_void_p, c_int, c_void_p] + [c_size_t] * 7 + [c_void_p, c_void_p, c_void_p,
                                             c_float, c_float, c_void_p, c_size_t, c_void_p]),
+    "b200_paged_decode_attn_beam": (c_int, [c_void_p, c_int, c_void_p] + [c_size_t] * 8 + [c_void_p, c_void_p, c_void_p, c_void_p,
+                                            c_float, c_void_p, c_size_t, c_void_p]),
     "b200_wo_gemm_packed_bytes": (c_size_t, [c_int, c_int, c_int]),
     "b200_pack_w4": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "b200_pack_w8": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),

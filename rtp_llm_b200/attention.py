@@ -55,6 +55,19 @@ class B200AttnParams:
 
 
 _MAX_ROWS = 64       # query rows (group x q_len) per (sequence, kv head) of b200_paged_decode_attn(_multi)
+_BEAM_MIN_UNITS = 128   # (request, kv head) pairs from which b200_paged_decode_attn_beam wins (measured, see beam_rows_fit)
+
+
+def beam_rows_fit(head_num: int, kv_head_num: int, beam_width: int, requests: int) -> bool:
+    """When a request's beams take the seat of one (sequence, kv head) in b200_paged_decode_attn_beam, which reads the K/V they
+    share once: there is more than one beam, their group x beam_width query rows fit the kernel's row limit, and there are
+    enough (request, kv head) pairs to fill the GPU with that many fewer, heavier CTAs. Everything else runs
+    b200_paged_decode_attn on every beam.
+    The boundary is measured (H100 80GB HBM3, 700 W; Hkv 8, D 128, ctx 2048, tools/kernel_bench.py attn-beam, beam / per row):
+    256 pairs W 4 0.73; 128 pairs W 8 0.48 (group 4) and 0.72 (group 8); 64 pairs W 8 0.86, W 4 0.96, W 2 1.21; 32 pairs
+    W 16 1.32 -- and at 64 pairs W 4 the whole step was 5 % slower with the beam kernel (tools/step_ab.py beam)."""
+    group = head_num // max(kv_head_num, 1)
+    return beam_width > 1 and group * beam_width <= _MAX_ROWS and requests * kv_head_num >= _BEAM_MIN_UNITS
 
 
 def _q_len(attn_inputs) -> int:

@@ -418,10 +418,12 @@ size_t b200_paged_decode_attn_workspace_bytes(size_t batch, size_t head_num, siz
     return w.sem + w.ml + w.o;
 }
 
+// beam_width > 0: the beam instance. `batch` then counts requests, each with beam_width sequences (rows of q, out, page_list and
+// sequence_lengths), and shared_lengths [batch] says how much of a request's K/V its beams share; q_len is 1.
 static int attn_impl(const void* q, const void* qkv, float rope_base, int q_len, int is_bf16, void* out, size_t head_num, size_t kv_head_num,
                      size_t head_dim, size_t batch, size_t max_blocks_per_seq, size_t max_seq_len, size_t page_size, const void* kv_pool,
                      const int32_t* page_list, const uint32_t* sequence_lengths, float q_scale, void* workspace, size_t workspace_bytes,
-                     void* stream) {
+                     void* stream, int beam_width = 0, const int32_t* shared_lengths = nullptr) {
     if (batch == 0) return B200_OK;
     ARG_CHECK((q || qkv) && out && kv_pool && page_list && sequence_lengths, "paged_decode_attn: null pointer");
     ARG_CHECK(head_dim == 64 || head_dim == 128 || head_dim == 256, "paged_decode_attn: head_dim %zu unsupported (64 / 128 / 256)", head_dim);
@@ -434,6 +436,9 @@ static int attn_impl(const void* q, const void* qkv, float rope_base, int q_len,
     ARG_CHECK(group >= 1 && group <= kAttnMaxRows, "paged_decode_attn: group size %d unsupported (1..%d)", group, kAttnMaxRows);
     ARG_CHECK(group * q_len <= kAttnMaxRows, "paged_decode_attn: group %d x q_len %d exceeds the limit of %d query rows per (sequence, kv head)",
               group, q_len, kAttnMaxRows);
+    ARG_CHECK(group * beam_width <= kAttnMaxRows,
+              "paged_decode_attn_beam: group %d x beam_width %d exceeds the limit of %d query rows per (request, kv head)", group,
+              beam_width, kAttnMaxRows);
     ARG_CHECK(page_size == 16 || page_size == 32 || page_size == 64 || page_size == 128,
               "paged_decode_attn: page_size %zu unsupported (16/32/64/128)", page_size);
     ARG_CHECK(max_seq_len >= 1, "paged_decode_attn: max_seq_len must be >= 1");
@@ -444,10 +449,14 @@ static int attn_impl(const void* q, const void* qkv, float rope_base, int q_len,
     if (g_rec)
         return rec_call([=](void* st) {
             return attn_impl(q, qkv, rope_base, q_len, is_bf16, out, head_num, kv_head_num, head_dim, batch, max_blocks_per_seq, max_seq_len,
-                             page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, st);
+                             page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, st, beam_width,
+                             shared_lengths);
         });
 
-    AttnParams p{};
+    const int slots = beam_width ? beam_width : q_len;   // query tokens or beams that share a CTA
+    AttnBeamParams p{};
+    p.beam_width = beam_width;
+    p.shared_lens = shared_lengths;
     p.q = q;
     p.qkv = qkv;
     p.kv_pool_rw = const_cast<void*>(kv_pool);
@@ -470,7 +479,7 @@ static int attn_impl(const void* q, const void* qkv, float rope_base, int q_len,
     attn_split((int)(batch * kv_head_num), max_tiles, &p.nsplit, &p.tiles_per_split, (int)head_dim);
 
     if (p.nsplit > 8) {
-        const AttnWorkspace w = attn_workspace(batch, head_num, kv_head_num, q_len, p.nsplit, head_dim);
+        const AttnWorkspace w = attn_workspace(batch, head_num, kv_head_num, slots, p.nsplit, head_dim);
         ARG_CHECK(workspace && workspace_bytes >= w.sem + w.ml + w.o,
                   "paged_decode_attn: workspace too small (%zu < %zu)", workspace_bytes, w.sem + w.ml + w.o);
         p.sem = reinterpret_cast<int*>(workspace);
@@ -490,20 +499,25 @@ static int attn_impl(const void* q, const void* qkv, float rope_base, int q_len,
     const dim3 grid(p.nsplit, (unsigned)(batch * kv_head_num), 1);
     p.cluster_merge = (p.nsplit >= 2 && p.nsplit <= 8) ? 1 : 0;   // 2..8 splits merge in a cluster, more through the workspace
     const dim3 cluster(p.cluster_merge ? p.nsplit : 1);
-    auto launch = [&](auto t, auto hd, auto rt) {
-        constexpr auto kern = paged_decode_attn_kernel<decltype(t), decltype(hd)::value, decltype(rt)::value>;
+    auto launch = [&](auto t, auto hd, auto rt, auto beam) {
+        constexpr auto kern = paged_decode_attn_kernel<decltype(t), decltype(hd)::value, decltype(rt)::value, decltype(beam)::value>;
         const int smem = attn_smem_bytes(decltype(hd)::value);
         int rc = configure_once<kern>(smem);
         if (rc) return rc;
+        // (launch_ex converts p to the kernel's parameter type: the plain instances take its AttnParams part)
         CUDA_CHECK(launch_ex(kern, {grid, dim3(kAttnThreads), (size_t)smem, (cudaStream_t)stream, g_pdl.load() != 0, cluster}, map, p));
         return launched("paged_decode_attn_kernel");
     };
-    // query rows in 16-row tiles: 1, 2 or 4 per (sequence, kv head)
-    const int rows = group * q_len;
+    // query rows in 16-row tiles: 1, 2 or 4 per (sequence or request, kv head)
+    const int rows = group * slots;
     auto by_rows = [&](auto t, auto hd) {
-        if (rows <= 16) return launch(t, hd, std::integral_constant<int, 1>());
-        if (rows <= 32) return launch(t, hd, std::integral_constant<int, 2>());
-        return launch(t, hd, std::integral_constant<int, 4>());
+        auto by_beam = [&](auto rt) {
+            if (beam_width) return launch(t, hd, rt, std::true_type());
+            return launch(t, hd, rt, std::false_type());
+        };
+        if (rows <= 16) return by_beam(std::integral_constant<int, 1>());
+        if (rows <= 32) return by_beam(std::integral_constant<int, 2>());
+        return by_beam(std::integral_constant<int, 4>());
     };
     return by_dtype(is_bf16, [&](auto t) {
         if (head_dim == 64) return by_rows(t, std::integral_constant<int, 64>());
@@ -539,6 +553,19 @@ int b200_paged_decode_attn_rope(const void* qkv, int is_bf16, void* out, size_t 
     ARG_CHECK(rope_base > 1.f, "paged_decode_attn_rope: rope_base must be > 1");
     return attn_impl(nullptr, qkv, rope_base, 1, is_bf16, out, head_num, kv_head_num, head_dim, batch, max_blocks_per_seq, max_seq_len,
                      page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, stream);
+}
+
+int b200_paged_decode_attn_beam(const void* q, int is_bf16, void* out, size_t head_num, size_t kv_head_num, size_t head_dim,
+                                size_t requests, size_t beam_width, size_t max_blocks_per_seq, size_t max_seq_len, size_t page_size,
+                                const void* kv_pool, const int32_t* page_list, const uint32_t* sequence_lengths,
+                                const int32_t* shared_lengths, float q_scale, void* workspace, size_t workspace_bytes, void* stream) {
+    ARG_CHECK(beam_width >= 1 && beam_width <= (size_t)kAttnMaxRows, "paged_decode_attn_beam: beam_width %zu unsupported (1..%d)",
+              beam_width, kAttnMaxRows);
+    ARG_CHECK(requests * kv_head_num <= 65535, "paged_decode_attn_beam: requests*kv_heads %zu exceeds grid limit", requests * kv_head_num);
+    ARG_CHECK((q && shared_lengths) || requests == 0, "paged_decode_attn_beam: null pointer (q or shared_lengths)");
+    return attn_impl(q, nullptr, 0.f, 1, is_bf16, out, head_num, kv_head_num, head_dim, requests, max_blocks_per_seq, max_seq_len,
+                     page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, stream, (int)beam_width,
+                     shared_lengths);
 }
 
 // ------------------------------------------------------------------------------------------------ GEMM

@@ -18,6 +18,8 @@
 //   HBM once per (sequence, kv head) and a warp's registers are those of one row tile. RT == 1 is the single-tile kernel.
 //   The kernel is HBM-bound: per CTA 96 KB of K/V in flight, two CTAs per SM.
 #pragma once
+#include <type_traits>
+
 #include "ptx.cuh"
 
 namespace b200 {
@@ -63,10 +65,24 @@ struct AttnParams {
                               //    their partial (m, l, O) through distributed shared memory; no workspace, no semaphore
 };
 
+// The beam instance's parameters (XQA's beamWidth, 3rdparty/xqa/mha_sm90.cu: ctaNbValidQHeads = headGrpSize * beamWidth). B is the
+// number of requests; request b owns the beam_width sequences b * beam_width + i of q / out / page_list / seq_lens, and its
+// group * beam_width <= 64 query rows share one CTA: MMA row i * group + g is beam i, head kvh * group + g. q_len is 1.
+struct AttnBeamParams : AttnParams {
+    int beam_width;
+    const int32_t* shared_lens;   // [B] tokens of request b that all its beams share: over the first shared_lens[b] / T pages the
+                                  // request's page_list rows are equal (the caller's contract). The kernel rounds it down to whole
+                                  // 64-token tiles below the shortest beam's cached length, so a wrong value can only cost sharing.
+};
+
 // RT: 16-row tiles of query rows (rows = group * q_len rounded up to 16 / 32 / 64)
-template <typename T, int D = kAttnD, int RT = 1>
+// BEAM: a request's beams in one CTA. Tile t below the shared length is one pipeline stage, loaded once through beam 0's pages with
+// every row live; a tile from there on is one stage per beam that reaches it, in beam order, each loaded through that beam's pages
+// and masked to that beam's rows. A row so meets the tiles of its own sequence in order with the arithmetic of the plain instance;
+// another beam's stage leaves its (m, l, O) bit for bit as they were.
+template <typename T, int D = kAttnD, int RT = 1, bool BEAM = false>
 __global__ void __launch_bounds__(kAttnThreads, D <= 128 ? 2 : 1)
-paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const AttnParams p) {
+paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const std::conditional_t<BEAM, AttnBeamParams, AttnParams> p) {
     constexpr int NH = D / 64;                       // 64-channel halves per K / V row
     constexpr int STAGE = attn_stage_bytes(D);
     constexpr int OROW = D + 8;                      // floats; +8 banks per row -> conflict-free float2 stores
@@ -92,8 +108,37 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const AttnP
 
     // the host sized the split for max_seq_len: a longer sequence is clamped to that bound (never more tiles than the
     // splits cover, so the last-arriver count below always matches the CTAs that really contribute)
-    const int len = min(p.seq_lens[b] + p.q_len, p.nsplit * p.tiles_per_split * kAttnTile);
-    const int rows = p.group * p.q_len;
+    // query slots per CTA: tokens of a verification step, or the request's beams
+    auto nq = [&] {
+        if constexpr (BEAM) return p.beam_width;
+        else return p.q_len;
+    };
+    int len_v, sh_tiles = 0;     // BEAM: len is the longest beam's, tiles [0, sh_tiles) are shared
+    // BEAM: every beam's clamped length, then the shared tile count (in the fused rope's table: the beam instance has no rope)
+    int* s_len = reinterpret_cast<int*>(cs_tab);
+    if constexpr (BEAM) {
+        const int cap = p.nsplit * p.tiles_per_split * kAttnTile;
+        int lmax = 0, cmin = cap;
+        for (int i = lane; i < nq(); i += 32) {
+            const int cached = min(p.seq_lens[b * nq() + i], cap);
+            const int l = min(cached + 1, cap);
+            if (warp == 0) s_len[i] = l;     // (read after the barrier below)
+            lmax = max(lmax, l);
+            cmin = min(cmin, cached);   // the token appended this step is never shared
+        }
+#pragma unroll
+        for (int o = 16; o; o >>= 1) {
+            lmax = max(lmax, __shfl_xor_sync(0xffffffffu, lmax, o));
+            cmin = min(cmin, __shfl_xor_sync(0xffffffffu, cmin, o));
+        }
+        len_v = lmax;
+        sh_tiles = min(max(p.shared_lens[b], 0), cmin) / kAttnTile;
+        if (threadIdx.x == 0) s_len[kAttnMaxRows] = sh_tiles;   // the stage loops read it from there: a register less to hold
+    } else {
+        len_v = min(p.seq_lens[b] + p.q_len, p.nsplit * p.tiles_per_split * kAttnTile);
+    }
+    const int len = len_v;
+    const int rows = p.group * nq();
     const int ntiles = (len + kAttnTile - 1) / kAttnTile;
     const int t0 = split * p.tiles_per_split;
     const int t1 = min(t0 + p.tiles_per_split, ntiles);
@@ -110,15 +155,34 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const AttnP
     }
     __syncthreads();
 
+    // BEAM: the stage sequence, derived alike by the producer and the consumers. live_from: the first beam >= from with a stage
+    // at tile t (nq() when none); a shared tile has the one stage, filed under beam 0, whose pages it is loaded through.
+    auto live_from = [&](int t, int from) {
+        if (t < s_len[kAttnMaxRows]) return from == 0 ? 0 : nq();
+        while (from < nq() && s_len[from] <= t * kAttnTile) ++from;
+        return from;
+    };
+
     if (warp == kAttnConsumerWarps) {
         // ------------------------------------------------------------------ TMA producer
         // Tile issue is split in two so that, with the fused rope, the append of the new token (all 32 lanes) overlaps the first
         // loads in flight: lane 0 first fills the ring with tiles that cannot contain the new token, the warp appends, then
         // lane 0 streams the rest (the token's tile is the sequence's last tile).
-        const int32_t* kpl = p.page_list + (size_t)(b * 2 + 0) * p.M;
-        const int32_t* vpl = p.page_list + (size_t)(b * 2 + 1) * p.M;
-        auto issue = [&](int i) {
-            const int it = i - t0, s = it % kAttnStages;
+        int seq = b;                                  // page_list row
+        if constexpr (BEAM) seq = b * nq();             // beam 0's; beam i's rows lie 2 * M * i further on
+        const int32_t* kpl = p.page_list + (size_t)(seq * 2 + 0) * p.M;
+        const int32_t* vpl = p.page_list + (size_t)(seq * 2 + 1) * p.M;
+        // BEAM: stage n of this CTA is tile i through beam `beam`'s pages, up to that beam's length when the tile is private
+        auto issue = [&](int i, int n = 0, int beam = 0) {
+            int it = i - t0, len_s = len;
+            const int32_t *kp = kpl, *vp = vpl;
+            if constexpr (BEAM) {
+                it = n;
+                kp += (size_t)beam * 2 * p.M;
+                vp += (size_t)beam * 2 * p.M;
+                if (i >= s_len[kAttnMaxRows]) len_s = s_len[beam];
+            }
+            const int s = it % kAttnStages;
             const uint32_t ph = (it / kAttnStages) & 1;
             // page ids first (global loads overlap the wait below)
             int kpage[4], vpage[4], inpage[4];
@@ -126,10 +190,10 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const AttnP
 #pragma unroll
             for (int bx = 0; bx < 4; ++bx) {
                 const int tok = i * kAttnTile + bx * p.box_h;
-                if (bx < p.boxes_per_tile && tok < len) {
+                if (bx < p.boxes_per_tile && tok < len_s) {
                     const int pidx = tok >> p.log2T;
-                    kpage[bx] = kpl[pidx];
-                    vpage[bx] = vpl[pidx];
+                    kpage[bx] = kp[pidx];
+                    vpage[bx] = vp[pidx];
                     inpage[bx] = tok & (p.T - 1);
                     nbox = bx + 1;
                 }
@@ -152,14 +216,20 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const AttnP
         int first_end = t1;                               // tiles [t0, first_end) are issued before the append
         bool own = false;
         int pos = 0;
-        if (D == 128 && RT == 1 && p.qkv != nullptr) {   // fused rope: head_dim 128, one row tile (the host rejects others)
+        if (!BEAM && D == 128 && RT == 1 && p.qkv != nullptr) {   // fused rope: head_dim 128, one row tile (the host rejects others)
             pos = p.seq_lens[b];
             own = pos < len && (pos / kAttnTile) >= t0 && (pos / kAttnTile) < t1;      // this CTA streams the new token's tile
             if (own) first_end = min(min(t0 + kAttnStages, t1), pos / kAttnTile);
         }
         if (lane == 0) {
             tma_prefetch_desc(&kv_map);
-            for (int i = t0; i < first_end; ++i) issue(i);
+            if constexpr (BEAM) {
+                int n = 0;
+                for (int i = t0; i < t1; ++i)
+                    for (int beam = live_from(i, 0); beam < nq(); beam = live_from(i, beam + 1)) issue(i, n++, beam);
+            } else {
+                for (int i = t0; i < first_end; ++i) issue(i);
+            }
         }
         __syncwarp();
         if (own) {
@@ -207,7 +277,7 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const AttnP
     // Q fragments for the whole head dim: 8 k-steps x 4 regs. Rows >= group are zero.
     uint32_t qf[D / 16][4];
     bool q_loaded = false;
-    if constexpr (D == 128 && RT == 1) {
+    if constexpr (D == 128 && RT == 1 && !BEAM) {
       if (p.qkv) {
         q_loaded = true;
         // un-rotated q straight from the qkv GEMM output; the NeoX partner of column c < 64 is column c + 64 = the same
@@ -251,11 +321,11 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const AttnP
       }
     }
     if (!q_loaded) {
-        // MMA row R = j * group + g  <->  query token j, head kvh * group + g
+        // MMA row R = j * group + g  <->  query token (BEAM: beam) j, head kvh * group + g
         const bool v0 = row0 < rows, v1 = row1 < rows;
         const T* qall = reinterpret_cast<const T*>(p.q);
-        const T* q0 = qall + (((size_t)b * p.q_len + row0 / p.group) * p.Hq + (size_t)kvh * p.group + row0 % p.group) * D;
-        const T* q1 = qall + (((size_t)b * p.q_len + row1 / p.group) * p.Hq + (size_t)kvh * p.group + row1 % p.group) * D;
+        const T* q0 = qall + (((size_t)b * nq() + row0 / p.group) * p.Hq + (size_t)kvh * p.group + row0 % p.group) * D;
+        const T* q1 = qall + (((size_t)b * nq() + row1 / p.group) * p.Hq + (size_t)kvh * p.group + row1 % p.group) * D;
 #pragma unroll
         for (int kk = 0; kk < D / 16; ++kk) {
             const int c = kk * 16 + qcol;
@@ -272,7 +342,11 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const AttnP
     float m0 = -INFINITY, m1 = -INFINITY;  // running max (raw score units) for rows qrow / qrow+8
     float l0 = 0.f, l1 = 0.f;              // per-thread partial row sums (quad-reduced at the end)
     const float sl2 = p.scale_log2;
-    const int off0 = p.q_len - 1 - min(row0 / p.group, p.q_len - 1), off1 = p.q_len - 1 - min(row1 / p.group, p.q_len - 1);
+    int off0 = 0, off1 = 0;   // (BEAM: one query token per beam)
+    if constexpr (!BEAM) {
+        off0 = p.q_len - 1 - min(row0 / p.group, p.q_len - 1);
+        off1 = p.q_len - 1 - min(row1 / p.group, p.q_len - 1);
+    }
 
     // ldmatrix lane geometry
     const int mi = lane >> 3, mr = lane & 7;
@@ -281,19 +355,48 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const AttnP
     const int v_tokrow0 = warp / RT * 16 + (mi & 1) * 8 + mr;   // V (trans): (tok0-7,c),(tok8-15,c),(tok0-7,c+1),(tok8-15,c+1)
     const int v_chunk_add = mi >> 1;
 
+    // BEAM: the stage's beam and count; in a private stage only the beam's own rows are kept (row0 / row1 of this thread)
+    int nstage = 0;
     for (int i = t0; i < t1; ++i) {
-        const int it = i - t0, s = it % kAttnStages;
+      int beam = 0;
+      if constexpr (BEAM) beam = live_from(i, 0);
+      do {      // (one pass unless BEAM)
+        int it = i - t0, len_s = len;
+        bool keep0 = true, keep1 = true;
+        if constexpr (BEAM) {
+            it = nstage++;
+            len_s = (i + 1) * kAttnTile;   // a shared tile is whole in every beam
+        }
+        const int s = it % kAttnStages;
         const uint32_t ph = (it / kAttnStages) & 1;
         mbar_wait(&full_bar[s], ph);
         uint8_t* stage = smem + s * STAGE;
         const uint32_t k_base = smem_u32(stage), v_base = k_base + NH * 8192;
+        if constexpr (BEAM) {
+            if (i >= s_len[kAttnMaxRows]) {
+                len_s = s_len[beam];
+                const int r0 = rt * 16 + qrow - beam * p.group;   // row0, counted from the beam's first row
+                keep0 = r0 >= 0 && r0 < p.group;
+                keep1 = r0 + 8 >= 0 && r0 + 8 < p.group;
+                // no row of this beam in the warp's row tile: nothing to compute, but the stage is still this warp's to release
+                if (beam * p.group >= rt * 16 + 16 || (beam + 1) * p.group <= rt * 16) {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&empty_bar[s]);
+                    continue;
+                }
+            }
+        }
 
+      int nks = RT;
+      // The beam instances of two and four row tiles keep their slice passes a loop (the count is hidden from the compiler):
+      // unrolled, the accumulators a private stage sets aside push them over the register budget of two CTAs per SM (spills).
+      if constexpr (BEAM && RT > 1) asm volatile("" : "+r"(nks));
 #pragma unroll
-      for (int ks = 0; ks < RT; ++ks) {
+      for (int ks = 0; ks < nks; ++ks) {
         const int slice = warp / RT + ks * NW;           // 16-token slice of the stage
         const int k_tokrow = k_tokrow0 + ks * NW * 16, v_tokrow = v_tokrow0 + ks * NW * 16;
         const int tok0 = i * kAttnTile + slice * 16;
-        const int valid = len - tok0;  // tokens of this slice that exist (may be <= 0)
+        const int valid = len_s - tok0;  // tokens of this slice that exist (may be <= 0)
         if (valid < 16) {
             // Rows past the end of the sequence hold stale / never-written bytes: P is 0 there but 0 * NaN = NaN,
             // so the V rows are zeroed before use (K garbage is masked on the scores below). With RT > 1 the warps of the
@@ -322,12 +425,17 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const AttnP
 
         // ---- mask + online softmax (rows qrow and qrow+8)
         float mx0 = -INFINITY, mx1 = -INFINITY;
+        int lim0 = valid - off0, lim1 = valid - off1;
+        if constexpr (BEAM) {   // another beam's stage: every score of the row is masked
+            if (!keep0) lim0 = 0;
+            if (!keep1) lim1 = 0;
+        }
 #pragma unroll
         for (int j = 0; j < 2; ++j) {
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
                 // query j of a q_len-token step sees q_len - 1 - j fewer tokens than the last one (causal among the new tokens)
-                const bool ok0 = (j * 8 + qcol + e) < valid - off0, ok1 = (j * 8 + qcol + e) < valid - off1;
+                const bool ok0 = (j * 8 + qcol + e) < lim0, ok1 = (j * 8 + qcol + e) < lim1;
                 sc[j][e] = ok0 ? sc[j][e] : -INFINITY;
                 sc[j][2 + e] = ok1 ? sc[j][2 + e] : -INFINITY;
                 mx0 = fmaxf(mx0, sc[j][e]);
@@ -341,7 +449,13 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const AttnP
         const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);
         // a fully masked slice keeps m = -inf; use 0 as the subtrahend so exp2(-inf - 0) = 0 (no NaN)
         const float ms0 = (mn0 == -INFINITY) ? 0.f : mn0 * sl2, ms1 = (mn1 == -INFINITY) ? 0.f : mn1 * sl2;
-        const float a0 = fast_exp2(m0 * sl2 - ms0), a1 = fast_exp2(m1 * sl2 - ms1);  // m = -inf -> 0
+        float a0 = fast_exp2(m0 * sl2 - ms0), a1 = fast_exp2(m1 * sl2 - ms1);  // m = -inf -> 0
+        if constexpr (BEAM) {
+            // A masked row has mn = m and p = 0, but m * sl2 - ms may contract to an fma and leave the product's rounding error in
+            // the exponent. Another beam's stage must not rescale the row at all: the sharing a caller declares never changes bits.
+            if (!keep0) a0 = 1.f;
+            if (!keep1) a1 = 1.f;
+        }
         m0 = mn0;
         m1 = mn1;
         float ps0 = 0.f, ps1 = 0.f;
@@ -379,12 +493,26 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const AttnP
             const int half = n2 >> 2, c = (n2 & 3) * 2 + v_chunk_add;
             uint32_t vb[4];
             ldmatrix_x4_trans(vb, v_base + half * 8192 + v_tokrow * 128 + ((c ^ (v_tokrow & 7)) << 4));
-            mma_m16n8k16<T>(o[2 * n2], pf, vb[0], vb[1]);
-            mma_m16n8k16<T>(o[2 * n2 + 1], pf, vb[2], vb[3]);
+            if constexpr (BEAM) {
+                // p = 0 does not shield a row from another beam's V: 0 * inf and 0 * NaN are NaN. A row the stage does not keep
+                // takes its accumulators back as they were.
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    float(&acc)[4] = o[2 * n2 + h];
+                    const float old[4] = {acc[0], acc[1], acc[2], acc[3]};
+                    mma_m16n8k16<T>(acc, pf, vb[2 * h], vb[2 * h + 1]);
+                    if (!keep0) acc[0] = old[0], acc[1] = old[1];
+                    if (!keep1) acc[2] = old[2], acc[3] = old[3];
+                }
+            } else {
+                mma_m16n8k16<T>(o[2 * n2], pf, vb[0], vb[1]);
+                mma_m16n8k16<T>(o[2 * n2 + 1], pf, vb[2], vb[3]);
+            }
         }
       }
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty_bar[s]);
+      } while (BEAM && (beam = live_from(i, beam + 1)) < nq());
     }
 
     // quad-reduce the row sums
@@ -418,9 +546,9 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const AttnP
     constexpr int DPT = (D + 127) / 128;
     const int d0 = threadIdx.x;
     const size_t ws_base = ((size_t)bh * p.nsplit + split) * rows;
-    // output row of MMA row r: token r / group, head kvh * group + r % group of out [B][q_len][Hq * D]
+    // output row of MMA row r: token (BEAM: beam) r / group, head kvh * group + r % group of out [B][q_len][Hq * D]
     auto out_row = [&](int r) {
-        return reinterpret_cast<T*>(p.out) + (((size_t)b * p.q_len + r / p.group) * p.Hq + (size_t)kvh * p.group + r % p.group) * D;
+        return reinterpret_cast<T*>(p.out) + (((size_t)b * nq() + r / p.group) * p.Hq + (size_t)kvh * p.group + r % p.group) * D;
     };
     // per-CTA partial of the cluster merge: [rows][D] fp32 + (m, l) per row, behind the per-warp staging area
     float* part_o = l_s + kAttnConsumerWarps * 16;

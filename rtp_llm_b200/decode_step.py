@@ -19,6 +19,7 @@ import torch
 
 from . import ops, rope
 from ._lib import B200_FMT_F16, B200_FMT_INT4, B200_FMT_INT8, B200_FMT_INT8G
+from .attention import beam_rows_fit
 from .rope import LLAMA3, RopeSpec
 
 
@@ -162,6 +163,12 @@ class DecodeStep:
     gathered into scratch first, then scattered, since a beam can be a parent and a child in the same step). Then the ids
     become next_token and the lengths grow by one: the next call runs the next step. upload_inputs() restarts from the prompt;
     a step past max_new_tokens since then raises ValueError (the page-table rows end there), in run() and in replay().
+    The attention reads that shared prompt once per request: when attention.beam_rows_fit holds (group * W <= 64 query rows and
+    at least 128 (request, kv head) pairs, from where the kernel was measured to win) the layers call paged_decode_attn_beam with shared_lens [B] = the prompt's full pages * tokens_per_block, a static buffer
+    that upload_inputs() refreshes (the prompt is fixed between two uploads, so a graph replays it); a wider search runs
+    paged_decode_attn on the B * W rows. The invariant this rests on: the fork gives a new beam its parent's page-table entries
+    for every page the step has filled, and all parents descend from the prompt's beams, so at every step the W page-table rows
+    of a request are equal over the first shared_lens[b] / tokens_per_block pages.
     The device state: beam_cum [B, W], hist [B*W, ctx] / hist_len [B*W], beam_out (the beam_search_step outputs).
     With eos_id, finished hypotheses are kept on the device: beam_search_step runs with that EOS (the next beams skip it), then
     beam_hypotheses_update moves the EOS candidates among the first W ranks into each request's set (hyp_state, up to W paths
@@ -424,6 +431,7 @@ class DecodeStep:
                     for L in self.layers:
                         L["kv"][blk[b, 1:, f].long().to(device)] = L["kv"][int(blk[b, 0, f])].clone()
             self.ids_h.copy_(self.ids_h.view(-1, beam_width)[:, :1].expand(-1, beam_width).reshape(-1))
+            self.shared_lens_h = (full * T).to(torch.int32).pin_memory()
         self.next_h = torch.zeros(batch, dtype=torch.int32).pin_memory()
         if q_len > 1:
             self.drafts_h = torch.zeros(batch, q_len - 1, dtype=torch.int32).pin_memory()
@@ -477,6 +485,7 @@ class DecodeStep:
             self.hist_parent = buf(R, ctx, dt=torch.int32)
             self.len_parent = buf(R, dt=torch.int32)
             self.page_scratch = buf(R, 2, self.Hkv, T, self.D)
+            self.shared_lens = buf(B, dt=torch.int32)
             if eos_id is not None:    # the finished-hypothesis sets (emptied by upload_inputs)
                 self.hyp_state = ops.beam_hypotheses_state(B, W, max_new_tokens, device)
                 self.done = torch.zeros(B, dtype=torch.int32, device=device)
@@ -535,6 +544,7 @@ class DecodeStep:
             self.drafts_h.copy_(self.ids_h[:, 1:])
             self.drafts.copy_(self.drafts_h, non_blocking=True)
         if self.W > 1:        # back to the prompt: beam 0 alone live (cum 0), the input token as the whole history
+            self.shared_lens.copy_(self.shared_lens_h, non_blocking=True)
             self.beam_cum.fill_(-math.inf)
             self.beam_cum[:, 0] = 0.0
             self.hist[:, 0].copy_(self.ids)
@@ -609,6 +619,19 @@ class DecodeStep:
         rope.rope_append(self.rope_spec, self.qkv, L["kv"], self.page_list, self.seq_lens, self.Hq, q_out=self.q, q_len=self.q_len,
                          qk_norm=qk_norm)
 
+    def _attention(self, L):
+        """self.attn = the attention of the step's rows over layer L's cache, after _rope_append. In beam mode a request's beams
+        share one pass over its prompt when their rows fit (attention.beam_rows_fit)."""
+        if self.q_len > 1:    # each query token attends up to its own position
+            ops.paged_decode_attn_multi(self.q.view(self.B, self.q_len, self.Hq, self.D), L["kv"], self.page_list, self.seq_lens,
+                                        self.ctx, self.attn_ws, out=self.attn.view(self.B, self.q_len, self.Hq * self.D))
+        elif beam_rows_fit(self.Hq, self.Hkv, self.W, self.requests):
+            ops.paged_decode_attn_beam(self.q.view(self.requests, self.W, self.Hq, self.D), L["kv"], self.page_list, self.seq_lens,
+                                       self.shared_lens, self.ctx, self.attn_ws,
+                                       out=self.attn.view(self.requests, self.W, self.Hq * self.D))
+        else:
+            ops.paged_decode_attn(self.q, L["kv"], self.page_list, self.seq_lens, self.ctx, self.attn_ws, out=self.attn)
+
     def step_core(self):
         """Everything up to the sampled token (TP1 / peer communicator) or the local logits (NCCL): C-ABI calls only, so it
         can be recorded into a decode program."""
@@ -626,13 +649,9 @@ class DecodeStep:
             if self.fuse_rope:    # RoPE + K/V append inside the attention kernel (one launch instead of two)
                 ops.paged_decode_attn_rope(self.qkv, L["kv"], self.page_list, self.seq_lens, self.Hq, self.ctx,
                                            self.rope_spec.base, self.attn_ws, out=self.attn)
-            elif self.q_len > 1:  # K/V of all q_len tokens appended, then each query token attends up to its own position
+            else:                 # K/V of the step's tokens appended, then the attention over the cache
                 self._rope_append(L)
-                ops.paged_decode_attn_multi(self.q.view(self.B, self.q_len, self.Hq, self.D), L["kv"], self.page_list, self.seq_lens,
-                                            self.ctx, self.attn_ws, out=self.attn.view(self.B, self.q_len, self.Hq * self.D))
-            else:
-                self._rope_append(L)
-                ops.paged_decode_attn(self.q, L["kv"], self.page_list, self.seq_lens, self.ctx, self.attn_ws, out=self.attn)
+                self._attention(L)
             self._row_gemm(self.attn, L["o"])
             self._ar_norm(self.proj, L["ln2"])
             if self.fuse_silu:     # SiLU(gate)*up in the GEMM epilogue (gate/up columns interleaved at load time)
@@ -813,6 +832,8 @@ class DecodeStep:
         w = (weight_bytes(cfg, H, qkv_n) + weight_bytes(cfg, self.Hq * self.D, H) + weight_bytes(cfg, H, 2 * self.inter)
              + weight_bytes(cfg, self.inter, H)) * cfg.layers
         lens = (self.seq_lens_h.to(torch.int64) + self.q_len).sum().item()
+        if self.W > 1:    # a request's shared prompt pages are one copy of K/V, whichever kernel reads them
+            lens -= (self.W - 1) * self.shared_lens_h.to(torch.int64).sum().item()
         kv = 2.0 * lens * self.Hkv * self.D * 2 * cfg.layers
         lm = 2.0 * H * self.vocab
         return dict(weights=w, kv=kv, lm_head=lm, total=w + kv + lm)

@@ -114,6 +114,23 @@ def paged_decode_attn_multi(q: torch.Tensor, kv_cache_base: torch.Tensor, page_l
     return out
 
 
+def paged_decode_attn_beam(q: torch.Tensor, kv_cache_base: torch.Tensor, page_list: torch.Tensor, sequence_lengths: torch.Tensor,
+                           shared_lengths: torch.Tensor, max_seq_len: int, workspace: torch.Tensor, out: Optional[torch.Tensor] = None,
+                           q_scale: float = 1.0) -> torch.Tensor:
+    """q [B, W, Hq, D]: beam i of request b is sequence b * W + i of page_list [B*W, 1, 2, M] and sequence_lengths [B*W];
+    shared_lengths [B] int32 = tokens of each request that all its W beams share (their page_list rows are equal over those
+    pages), read once for the W beams. The bits of paged_decode_attn on the B * W rows. Returns [B, W, Hq*D]."""
+    _cuda_contig(q, kv_cache_base, page_list, shared_lengths, workspace, out)
+    P, two, Hkv, T, D = kv_cache_base.shape
+    B, W, Hq = q.shape[0], q.shape[1], q.shape[2]
+    if out is None:
+        out = torch.empty((B, W, Hq * D), dtype=q.dtype, device=q.device)
+    check(_lib.load().b200_paged_decode_attn_beam(_p(q), _is_bf16(q), _p(out), Hq, Hkv, D, B, W, page_list.shape[-1], max_seq_len,
+                                                  T, _p(kv_cache_base), _p(page_list), _p(sequence_lengths), _p(shared_lengths),
+                                                  q_scale, _p(workspace), workspace.numel(), _stream()), "b200_paged_decode_attn_beam")
+    return out
+
+
 def paged_decode_attn_rope(qkv: torch.Tensor, kv_cache_base: torch.Tensor, page_list: torch.Tensor, sequence_lengths: torch.Tensor,
                            head_num: int, max_seq_len: int, rope_base: float, workspace: torch.Tensor,
                            out: Optional[torch.Tensor] = None, q_scale: float = 1.0) -> torch.Tensor:

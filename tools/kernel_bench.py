@@ -89,6 +89,44 @@ def bench_attn_multi(B, Hq, Hkv, S, q_len, T=64, nrot=3):
     return us
 
 
+def bench_attn_beam(B, W, Hq, Hkv, S=2048, T=64, private=28, nrot=3, runs=3):
+    """b200_paged_decode_attn_beam against b200_paged_decode_attn on the same B * W rows and the same page tables, whose beams
+    share the full pages of the first S - private tokens and own the pages after them (the beam step's tables), the arms
+    alternating; and the beam kernel with shared_lengths 0 on those tables: what the expansion into one stage per beam costs
+    by itself. GB/s is distinct bytes over kernel time, the K/V bytes that differ between rows (a request's shared pages
+    once): HBM traffic of the beam arm, not of the per-row arm, which reads the shared pages once per beam from HBM or L2."""
+    M, R = math.ceil(S / T), B * W
+    shared_pages = (S - private) // T
+    P = B * shared_pages + R * (M - shared_pages) + 1
+    pools = [torch.randn(P, 2, Hkv, T, 128, device=dev).half() for _ in range(nrot)]
+    q = torch.randn(B, W, Hq, 128, device=dev).half()
+    ids = iter((torch.randperm(P - 1) + 1).tolist())
+    bid = torch.zeros(R, M, dtype=torch.int32)
+    for b in range(B):
+        common = [next(ids) for _ in range(shared_pages)]
+        for i in range(W):
+            bid[b * W + i] = torch.tensor(common + [next(ids) for _ in range(M - shared_pages)], dtype=torch.int32)
+    pl = ops.convert_block_table(bid.to(dev))
+    seq = torch.full((R,), S - 1, dtype=torch.int32, device=dev)
+    shared = torch.full((B,), shared_pages * T, dtype=torch.int32, device=dev)
+    zero = torch.zeros_like(shared)
+    ws = ops.attn_workspace(R, Hq, Hkv, S, dev)
+    out = torch.empty(B, W, Hq * 128, device=dev).half()
+    arms = {"per row": lambda i: ops.paged_decode_attn(q.view(R, Hq, 128), pools[i], pl, seq, S, ws, out=out.view(R, -1)),
+            "beam": lambda i: ops.paged_decode_attn_beam(q, pools[i], pl, seq, shared, S, ws, out=out),
+            "beam shared 0": lambda i: ops.paged_decode_attn_beam(q, pools[i], pl, seq, zero, S, ws, out=out)}
+    t = {k: [] for k in arms}
+    for _ in range(runs):
+        for k, fn in arms.items():
+            t[k].append(timeit(fn, nrot))
+    byt = 2 * (B * shared_pages * T + R * (S - shared_pages * T)) * Hkv * 128 * 2
+    med = {k: sorted(v)[len(v) // 2] for k, v in t.items()}
+    print(f"attn-beam B{B} W{W} Hq{Hq} Hkv{Hkv} S{S} (rows {Hq // Hkv * W}, {byt / 1e6:.0f} MB distinct K/V): " + ", ".join(
+        f"{k} {med[k]:.1f} us (min {min(t[k]):.1f}, max {max(t[k]):.1f}; distinct bytes over kernel time {byt / med[k] / 1e3:.0f} GB/s)"
+        for k in arms) + f"; beam / per row = {med['beam'] / med['per row']:.2f}", flush=True)
+    return med
+
+
 def bench_beam(B, W, V=128256, ngram=0, hist=2048, nrot=8):
     """b200_beam_search_step on fp16 logits [B*W, V] (rotated through nrot sets, > L2), preceded by b200_ban_repeat_ngram
     over `hist` history tokens per row when ngram > 0."""
@@ -331,6 +369,14 @@ if __name__ == "__main__":
         # speculative-token verification at group 8 (Qwen2-72B / Llama-3-70B): 8, 16, 32, 64 query rows per kv head
         t = {n: bench_attn_multi(32, 64, 8, 2048, n) for n in (1, 2, 4, 8)}
         print("attn-multi time relative to q_len 2 (16 rows): " + ", ".join(f"q_len {n}: {t[n] / t[2]:.2f}x" for n in t), flush=True)
+    if "attn-beam" in which:
+        # a request's beams in one CTA against one CTA per beam, Llama-3-8B heads (group 4) and group 8 at W 8
+        import subprocess
+        print("attn-beam on " + (subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader",
+                                                 "-i", "0"], capture_output=True, text=True).stdout.strip() or "unknown card")
+              + " (name, power limit, SM clock, max SM clock)", flush=True)
+        for B, W, Hq in ((8, 4, 32), (32, 4, 32), (4, 16, 32), (16, 8, 32), (16, 8, 64), (8, 2, 32), (8, 8, 32)):
+            bench_attn_beam(B, W, Hq, 8)
     if "beam" in which:
         # beam search over Llama-3's vocabulary, with and without the 3-gram ban over 2048 history tokens, alternating
         for B, W in ((8, 4), (32, 4), (4, 16)):

@@ -4,9 +4,10 @@ each a step captured in a CUDA graph with PDL at --ctx tokens; the first arm is 
 
   act-order  Llama-3-8B INT4: plain, then act_order=True (three gathers per layer; w2's order is folded into w13)
   spec       Llama-3-8B INT4 (--model llama31: Llama-3.1-8B with its Llama3 rope): q_len 1, 2, 4 with batch * q_len <= 128
-  beam       Llama-3-8B INT4: the greedy step at batch * W rows, the beam step (W beams per request, --ngram ban), with --eos
-             the beam step that also keeps the finished hypotheses (eos_id set), and the fork alone as a graph of
-             DecodeStep.fork()
+  beam       Llama-3-8B INT4: the greedy step at batch * W rows, the beam step with b200_paged_decode_attn on every beam's row
+             (PerRowBeamStep), the beam step as it is (W beams per request, --ngram ban; the beam attention kernel when the
+             rows fit), with --eos the beam step that also keeps the finished hypotheses (eos_id set), and the fork alone as a
+             graph of DecodeStep.fork()
   sample     Llama-3-8B INT4: greedy, then sampled (temperature 0.8, top-k 50, top-p 0.9, repetition 1.1, the drawn token's
              log-prob and the top 5)
   qwen3      Qwen3-8B INT4: qk_rmsnorm, then the plain rope launch (TwoLaunchStep), against the fused QK-norm append
@@ -35,6 +36,7 @@ sys.path.insert(0, ROOT)
 from rtp_llm_b200 import ops  # noqa: E402
 from rtp_llm_b200.decode_step import LLAMA3_8B, LLAMA31_8B, QWEN3_8B, DecodeStep, SamplingParams  # noqa: E402
 from tests.step_oracle import TwoLaunchStep  # noqa: E402
+from tests.test_gpu_beam_attn import PerRowBeamStep  # noqa: E402
 
 
 @dataclasses.dataclass
@@ -67,7 +69,9 @@ def spec_arms(a, cfg, B, dev):
 def beam_arms(a, cfg, B, dev):
     W = a.beam_width
     greedy = step_arm(f"greedy B{B * W}", DecodeStep(cfg, B * W, a.ctx, dev, pdl=True))
-    model = DecodeStep(cfg, B, a.ctx, dev, pdl=True, beam_width=W, no_repeat_ngram=a.ngram, max_new_tokens=max_new_tokens(a))
+    kw = dict(pdl=True, beam_width=W, no_repeat_ngram=a.ngram, max_new_tokens=max_new_tokens(a))
+    per_row = step_arm(f"beam W{W} per row", PerRowBeamStep(cfg, B, a.ctx, dev, **kw))
+    model = DecodeStep(cfg, B, a.ctx, dev, **kw)
     beam = step_arm(f"beam W{W}", model)
     model.replay()                          # beam_out holds a real selection for the fork graph to replay
     hyps = []
@@ -86,7 +90,7 @@ def beam_arms(a, cfg, B, dev):
         model.fork()
     model.upload_inputs()
     torch.cuda.synchronize()
-    return [greedy, beam] + hyps + [Arm("fork", fork.replay, None, (model,))]
+    return [greedy, per_row, beam] + hyps + [Arm("fork", fork.replay, None, (model,))]
 
 
 def sample_arms(a, cfg, B, dev):
@@ -183,7 +187,7 @@ def main(argv=None):
                 launches = "torch ops only" if arm.launches is None else f"{arm.launches} launches/step"
                 diff = "" if arm is arms[0] else (f"; vs {arms[0].name} {rows[-1]['minus_baseline_us']:+.1f} us/step, "
                                                   f"t/t0 - 1 = {rows[-1]['over_baseline']:+.4f}")
-                print(f"B{B:<3d} {arm.name:12s}: {med:.3f} ms/step (min {min(t):.3f}, max {max(t):.3f}), {launches}{diff}",
+                print(f"B{B:<3d} {arm.name:16s}: {med:.3f} ms/step (min {min(t):.3f}, max {max(t):.3f}), {launches}{diff}",
                       flush=True)
             res["batches"].append(dict(batch=B, arms=rows))
             del arms, arm
