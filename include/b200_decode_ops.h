@@ -429,12 +429,16 @@ int b200_peer_argmax(const void* logits, int is_bf16, int rows, int vocab_local,
 /* A decode program is a recorded sequence of the op calls above, replayed with far fewer launches -- this library's counterpart
  * of the reference's CUDA-graph capture of the decode step (rtp_llm/cpp/cuda_graph/cuda_graph_runner.cc: capture once per
  * batch size, replay every step).  Between b200_program_begin and b200_program_end every op call of the CALLING THREAD is
- * appended to the program instead of being launched (arguments are checked and launch shapes planned at record time;
- * pointers and sizes are frozen, exactly as under stream capture).  Consecutive weight-only GEMMs, norms, rope+append,
- * embedding and block-table ops are fused into ONE persistent kernel (2 CTAs per SM, grid-wide barriers between ops,
- * stream-K GEMMs, weights prefetched across op boundaries -- csrc/decode_program.cuh); attention, FP16 GEMMs, argmax and
- * all-reduce calls are replayed as their own launches in order.  b200_program_launch never allocates or synchronises and
- * may itself be captured into a CUDA graph.  b200_program_end allocates the device-side op table (once).
+ * appended to the program instead of being launched.  Consecutive weight-only GEMMs, norms, rope+append, embedding and
+ * block-table ops are fused into ONE persistent kernel (2 CTAs per SM, grid-wide barriers between ops, stream-K GEMMs,
+ * weights prefetched across op boundaries -- csrc/decode_program.cuh); attention, FP16 GEMMs, argmax, sampling and
+ * all-reduce calls keep their own launches, in order.  Everything an op call decides is decided when it is recorded and
+ * never evaluated again by b200_program_launch: its argument checks, launch-shape plans and tensor maps, the B200_* test-hook
+ * environment variables, and for the launches outside the persistent kernel the b200_set_pdl setting (the persistent
+ * kernel's launches take the setting current at b200_program_launch; PDL never changes results).  Pointers and sizes are
+ * frozen, exactly as under stream capture, and structs passed by pointer (b200_rope_config, the peer region array) are
+ * copied, so the caller may reuse them.  b200_program_launch never allocates or synchronises and may itself be captured
+ * into a CUDA graph.  b200_program_end allocates the device-side op table (once).
  * Results are identical to issuing the same calls one by one (same kernels' arithmetic; tests compare bit for bit). */
 typedef struct b200_program b200_program;
 int b200_program_create(b200_program** out);

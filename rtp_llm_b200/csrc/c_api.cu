@@ -5,14 +5,12 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <array>
 #include <atomic>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <functional>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -261,13 +259,6 @@ int fill_ar_params(PeerArParams& p, void* const* regions, size_t max_message_byt
     return set_peers(p, "peer collective", regions, max_message_bytes, rank, world);
 }
 
-// A recorded peer call keeps its own copy of the region list: the caller's array need not outlive the recording.
-std::array<void*, kArMaxWorld> copy_regions(void* const* regions, int world) {
-    std::array<void*, kArMaxWorld> c{};
-    std::copy(regions, regions + world, c.begin());
-    return c;
-}
-
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------ decode program recorder
@@ -275,13 +266,14 @@ std::array<void*, kArMaxWorld> copy_regions(void* const* regions, int world) {
 // cudaStreamBeginCapture in cpp/cuda_graph/cuda_graph_runner.cc): between b200_program_begin and b200_program_end the
 // calling thread's op calls are appended to the program instead of being launched. Consecutive ops the persistent kernel
 // implements (weight-only GEMMs, norms, rope + append, embedding, block-table conversion) become ONE launch; every other
-// op (attention, FP16 GEMMs, argmax, all-reduce) is replayed as its own launch in between.
+// op's launch (attention, FP16 GEMMs, argmax, all-reduce) is kept with its arguments and issued as its own launch in between.
 struct b200_program {
     struct Item {
         bool segment = false;
         int first = 0, count = 0;          // ops[first, first+count)
         int bf16 = -1, bpad = -1, qfmt = -1;
-        std::function<int(void*)> fn;      // non-segment: replays the recorded call on a stream
+        const char* name = nullptr;        // non-segment: the kernel and its recorded launch on a given stream
+        std::function<cudaError_t(cudaStream_t)> issue;
     };
     std::vector<ProgOp> ops;
     std::vector<Item> items;
@@ -291,9 +283,17 @@ struct b200_program {
     bool finalized = false;
 };
 
-namespace {
+thread_local b200_program* b200_host::g_rec = nullptr;
 
-thread_local b200_program* g_rec = nullptr;
+int b200_host::record_launch(const char* name, std::function<cudaError_t(cudaStream_t)> issue) {
+    b200_program::Item it;
+    it.name = name;
+    it.issue = std::move(issue);
+    g_rec->items.push_back(std::move(it));
+    return B200_OK;
+}
+
+namespace {
 
 int rec_segment_op(const ProgOp& op, int bf16, int bpad, int qfmt) {
     b200_program* P = g_rec;
@@ -318,13 +318,6 @@ int rec_segment_op(const ProgOp& op, int bf16, int bpad, int qfmt) {
     it.qfmt = qfmt;
     P->ops.push_back(op);
     P->items.push_back(std::move(it));
-    return B200_OK;
-}
-
-int rec_call(std::function<int(void*)> fn) {
-    b200_program::Item it;
-    it.fn = std::move(fn);
-    g_rec->items.push_back(std::move(it));
     return B200_OK;
 }
 }  // namespace
@@ -379,9 +372,10 @@ int b200_convert_block_table(int32_t* page_list, const int32_t* block_ids, int b
     }
     const int total = batch * max_blocks;
     const int threads = 256, blocks = (total + threads - 1) / threads;
-    convert_block_table_kernel<<<blocks < 1024 ? blocks : 1024, threads, 0, (cudaStream_t)stream>>>(page_list, block_ids,
-                                                                                                  batch, max_blocks);
-    return launched("convert_block_table_kernel");
+    return launch_or_record("convert_block_table_kernel", stream, [=](cudaStream_t s) {
+        convert_block_table_kernel<<<blocks < 1024 ? blocks : 1024, threads, 0, s>>>(page_list, block_ids, batch, max_blocks);
+        return cudaGetLastError();
+    });
 }
 
 int b200_paged_attn_plan(const int32_t* input_lengths, const int32_t* sequence_lengths, const int32_t* prefix_lengths,
@@ -395,18 +389,13 @@ int b200_paged_attn_plan(const int32_t* input_lengths, const int32_t* sequence_l
     ARG_CHECK(tokens_per_block > 0, "paged_attn_plan: tokens_per_block must be positive");
     ARG_CHECK(paged_kv_last_page_len && decode_page_indptr && batch_indice && positions, "paged_attn_plan: null output");
     ARG_CHECK(!block_ids || page_indice, "paged_attn_plan: block_ids given but page_indice is null");
-    if (g_rec)
-        return rec_call([=](void* st) {
-            return b200_paged_attn_plan(input_lengths, sequence_lengths, prefix_lengths, block_ids, batch, max_blocks,
-                                        tokens_per_block, paged_kv_last_page_len, decode_page_indptr, page_indice, batch_indice,
-                                        positions, st);
-        });
     const int threads = (batch + 31) / 32 * 32;
-    paged_attn_plan_kernel<<<1, threads, 0, (cudaStream_t)stream>>>(input_lengths, sequence_lengths, prefix_lengths,
-                                                                    block_ids, batch, max_blocks, tokens_per_block,
-                                                                    paged_kv_last_page_len, decode_page_indptr,
-                                                                    page_indice, batch_indice, positions);
-    return launched("paged_attn_plan_kernel");
+    return launch_or_record("paged_attn_plan_kernel", stream, [=](cudaStream_t s) {
+        paged_attn_plan_kernel<<<1, threads, 0, s>>>(input_lengths, sequence_lengths, prefix_lengths, block_ids, batch, max_blocks,
+                                                     tokens_per_block, paged_kv_last_page_len, decode_page_indptr, page_indice,
+                                                     batch_indice, positions);
+        return cudaGetLastError();
+    });
 }
 
 // ------------------------------------------------------------------------------------------------ attention
@@ -446,12 +435,6 @@ static int attn_impl(const void* q, const void* qkv, float rope_base, int q_len,
               max_seq_len, max_blocks_per_seq * page_size);
     ARG_CHECK(batch * kv_head_num <= 65535, "paged_decode_attn: batch*kv_heads %zu exceeds grid limit", batch * kv_head_num);
     ARG_CHECK(((uintptr_t)kv_pool & 15) == 0 && (((uintptr_t)q | (uintptr_t)qkv) & 3) == 0, "paged_decode_attn: misaligned pointer");
-    if (g_rec)
-        return rec_call([=](void* st) {
-            return attn_impl(q, qkv, rope_base, q_len, is_bf16, out, head_num, kv_head_num, head_dim, batch, max_blocks_per_seq, max_seq_len,
-                             page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, st, beam_width,
-                             shared_lengths);
-        });
 
     const int slots = beam_width ? beam_width : q_len;   // query tokens or beams that share a CTA
     AttnBeamParams p{};
@@ -505,8 +488,9 @@ static int attn_impl(const void* q, const void* qkv, float rope_base, int q_len,
         int rc = configure_once<kern>(smem);
         if (rc) return rc;
         // (launch_ex converts p to the kernel's parameter type: the plain instances take its AttnParams part)
-        CUDA_CHECK(launch_ex(kern, {grid, dim3(kAttnThreads), (size_t)smem, (cudaStream_t)stream, g_pdl.load() != 0, cluster}, map, p));
-        return launched("paged_decode_attn_kernel");
+        return launch_or_record("paged_decode_attn_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+            return launch_ex(kern, {grid, dim3(kAttnThreads), (size_t)smem, s, pdl, cluster}, map, p);
+        });
     };
     // query rows in 16-row tiles: 1, 2 or 4 per (sequence or request, kv head)
     const int rows = group * slots;
@@ -692,14 +676,6 @@ static int wo_gemm_impl(int fmt, int is_bf16, const void* x, int B, int K, int N
         g.silu_mul = silu_mul ? 1 : 0;
         return rec_segment_op(op, is_bf16 ? 1 : 0, bpad, fmt);
     }
-    if (g_rec) {
-        const bool has_rs = rs != nullptr;
-        const RsPush d = has_rs ? *rs : RsPush{};
-        return rec_call([=](void* st) {
-            return wo_gemm_impl(fmt, is_bf16, x, B, K, N, w, col_scale, bias, y, workspace, workspace_bytes, flags,
-                                has_rs ? &d : nullptr, st);
-        });
-    }
 
     // ---- one kernel per GEMM, split-K merged by the last split CTA of a tile (gemm_cluster.cu)
     GemmParams p{};
@@ -779,15 +755,14 @@ int b200_add_rmsnorm(const void* x, void* residual, const void* gamma, void* y, 
         op.n.eps = eps;
         return rec_segment_op(op, is_bf16 ? 1 : 0, -1, -1);
     }
-    if (g_rec) return rec_call([=](void* st) { return b200_add_rmsnorm(x, residual, gamma, y, is_bf16, rows, hidden, eps, st); });
     const int threads = hidden / 8 >= 512 ? 512 : (hidden / 8 >= 256 ? 256 : 128);
     const size_t smem = (size_t)hidden * sizeof(float);
-    const bool pdl = g_pdl.load() != 0;
     return by_dtype(is_bf16, [&](auto t) {
         using T = decltype(t);
-        CUDA_CHECK(launch_ex(add_rmsnorm_kernel<T>, {dim3(rows), dim3(threads), smem, (cudaStream_t)stream, pdl}, (const T*)x,
-                             (T*)residual, (const T*)gamma, (T*)y, hidden, eps));
-        return launched("add_rmsnorm_kernel");
+        return launch_or_record("add_rmsnorm_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+            return launch_ex(add_rmsnorm_kernel<T>, {dim3(rows), dim3(threads), smem, s, pdl}, (const T*)x, (T*)residual,
+                             (const T*)gamma, (T*)y, hidden, eps);
+        });
     });
 }
 
@@ -798,18 +773,14 @@ int b200_qk_rmsnorm(void* qkv, const void* q_gamma, const void* k_gamma, const v
     ARG_CHECK((q_bias == nullptr) == (k_bias == nullptr), "qk_rmsnorm: give both biases or none");
     ARG_CHECK(head_dim > 0 && head_dim % 64 == 0, "qk_rmsnorm: head_dim %d must be a multiple of 64 (fused_qk_rmsnorm.cu:104-106)", head_dim);
     ARG_CHECK(rows > 0 && head_num > 0 && kv_head_num > 0, "qk_rmsnorm: bad shape");
-    if (g_rec)
-        return rec_call([=](void* st) {
-            return b200_qk_rmsnorm(qkv, q_gamma, k_gamma, q_bias, k_bias, is_bf16, rows, head_num, kv_head_num, head_dim, eps, st);
-        });
     const int units = rows * (head_num + kv_head_num), wpb = 8;
     const dim3 grid((units + wpb - 1) / wpb);
-    const bool pdl = g_pdl.load() != 0;
     return by_dtype(is_bf16, [&](auto t) {
         using T = decltype(t);
-        CUDA_CHECK(launch_ex(qk_rmsnorm_kernel<T>, {grid, dim3(wpb * 32), 0, (cudaStream_t)stream, pdl}, (T*)qkv, (const T*)q_gamma,
-                             (const T*)k_gamma, (const T*)q_bias, (const T*)k_bias, rows, head_num, kv_head_num, head_dim, eps));
-        return launched("qk_rmsnorm_kernel");
+        return launch_or_record("qk_rmsnorm_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+            return launch_ex(qk_rmsnorm_kernel<T>, {grid, dim3(wpb * 32), 0, s, pdl}, (T*)qkv, (const T*)q_gamma, (const T*)k_gamma,
+                             (const T*)q_bias, (const T*)k_bias, rows, head_num, kv_head_num, head_dim, eps);
+        });
     });
 }
 
@@ -817,17 +788,15 @@ int b200_silu_and_mul(const void* gate_up, void* y, int is_bf16, int rows, int i
     if (rows == 0) return B200_OK;
     ARG_CHECK(gate_up && y, "silu_and_mul: null pointer");
     ARG_CHECK(inter > 0 && inter % 2 == 0, "silu_and_mul: inter=%d must be positive and even", inter);
-    if (g_rec) return rec_call([=](void* st) { return b200_silu_and_mul(gate_up, y, is_bf16, rows, inter, st); });
     const size_t total = (size_t)rows * inter / 2;
     const int threads = 256;
     const size_t blocks = (total + threads - 1) / threads;
     const unsigned g = (unsigned)(blocks < 4 * num_sms() * 8 ? blocks : 4 * num_sms() * 8);
-    const bool pdl = g_pdl.load() != 0;
     return by_dtype(is_bf16, [&](auto t) {
         using T = decltype(t);
-        CUDA_CHECK(launch_ex(silu_and_mul_kernel<T>, {dim3(g), dim3(threads), 0, (cudaStream_t)stream, pdl}, (const T*)gate_up, (T*)y,
-                             rows, inter));
-        return launched("silu_and_mul_kernel");
+        return launch_or_record("silu_and_mul_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+            return launch_ex(silu_and_mul_kernel<T>, {dim3(g), dim3(threads), 0, s, pdl}, (const T*)gate_up, (T*)y, rows, inter);
+        });
     });
 }
 
@@ -842,13 +811,13 @@ int b200_permute_cols(const void* x, const int32_t* perm, void* y, int is_bf16, 
     ARG_CHECK(rows > 0, "permute_cols: rows=%d must be positive", rows);
     ARG_CHECK(K > 0 && K % 8 == 0 && K <= kPermuteMaxK, "permute_cols: K=%d must be a positive multiple of 8, <= %d", K, kPermuteMaxK);
     ARG_CHECK((((uintptr_t)x | (uintptr_t)y | (uintptr_t)perm) & 15) == 0, "permute_cols: x / perm / y must be 16-byte aligned");
-    if (g_rec) return rec_call([=](void* st) { return b200_permute_cols(x, perm, y, is_bf16, rows, K, st); });
     const int rc = configure_once<permute_cols_kernel>(kPermuteMaxK * 2);
     if (rc) return rc;
     const int threads = K / 8 >= 512 ? 512 : (K / 8 >= 256 ? 256 : 128);
-    CUDA_CHECK(launch_ex(permute_cols_kernel, {dim3(rows), dim3(threads), (size_t)K * 2, (cudaStream_t)stream, g_pdl.load() != 0},
-                         (const uint16_t*)x, perm, (uint16_t*)y, K));
-    return launched("permute_cols_kernel");
+    return launch_or_record("permute_cols_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+        return launch_ex(permute_cols_kernel, {dim3(rows), dim3(threads), (size_t)K * 2, s, pdl}, (const uint16_t*)x, perm,
+                         (uint16_t*)y, K);
+    });
 }
 
 // q_gamma / k_gamma non-null: QK-RMSNorm first (qk_norm_rope_append_kernel), always its own launch inside a decode program.
@@ -862,12 +831,7 @@ static int rope_append_impl(const void* qkv, void* q_out, void* kv_pool, const i
     ARG_CHECK(batch > 0 && q_len >= 1 && (long)batch * q_len <= 0x7fffffffL, "rope_append: bad shape batch %d x q_len %d", batch, q_len);
     const bool qkn = q_gamma != nullptr;
     const float l2b = std::log2(rope_base);
-    if (g_rec && (q_len > 1 || qkn))   // its own launch: the persistent kernel's rope op appends one token per sequence, unnormed
-        return rec_call([=](void* st) {
-            return rope_append_impl(qkv, q_out, kv_pool, page_list, sequence_lengths, is_bf16, batch, q_len, head_num, kv_head_num,
-                                    head_dim, max_blocks_per_seq, page_size, rope_base, q_gamma, k_gamma, eps, st);
-        });
-    if (g_rec) {
+    if (g_rec && q_len == 1 && !qkn) {   // the persistent kernel's rope op appends one token per sequence, unnormed
         ProgOp op{};
         op.type = kOpRope;
         op.r.qkv = qkv;
@@ -885,20 +849,20 @@ static int rope_append_impl(const void* qkv, void* q_out, void* kv_pool, const i
         return rec_segment_op(op, is_bf16 ? 1 : 0, -1, -1);
     }
     const dim3 grid(batch * q_len, head_num + 2 * kv_head_num);
-    const bool pdl = g_pdl.load() != 0;
     return by_dtype(is_bf16, [&](auto t) {
         using T = decltype(t);
-        const LaunchCfg lc{grid, dim3(head_dim / 2), 0, (cudaStream_t)stream, pdl};
-        if (qkn) {
-            CUDA_CHECK(launch_ex(q_len > 1 ? qk_norm_rope_append_kernel<T, true> : qk_norm_rope_append_kernel<T, false>, lc,
-                                 (const T*)qkv, (T*)q_out, (T*)kv_pool, page_list, sequence_lengths, head_num, kv_head_num, head_dim,
-                                 (int)max_blocks_per_seq, page_size, l2b, q_len, (const T*)q_gamma, (const T*)k_gamma, eps));
-            return launched("qk_norm_rope_append_kernel");
-        }
-        CUDA_CHECK(launch_ex(q_len > 1 ? rope_append_kernel<T, true> : rope_append_kernel<T, false>, lc, (const T*)qkv,
-                             (T*)q_out, (T*)kv_pool, page_list, sequence_lengths, head_num, kv_head_num, head_dim,
-                             (int)max_blocks_per_seq, page_size, l2b, q_len));
-        return launched("rope_append_kernel");
+        if (qkn)
+            return launch_or_record("qk_norm_rope_append_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+                return launch_ex(q_len > 1 ? qk_norm_rope_append_kernel<T, true> : qk_norm_rope_append_kernel<T, false>,
+                                 {grid, dim3(head_dim / 2), 0, s, pdl}, (const T*)qkv, (T*)q_out, (T*)kv_pool, page_list,
+                                 sequence_lengths, head_num, kv_head_num, head_dim, (int)max_blocks_per_seq, page_size, l2b, q_len,
+                                 (const T*)q_gamma, (const T*)k_gamma, eps);
+            });
+        return launch_or_record("rope_append_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+            return launch_ex(q_len > 1 ? rope_append_kernel<T, true> : rope_append_kernel<T, false>, {grid, dim3(head_dim / 2), 0, s, pdl},
+                             (const T*)qkv, (T*)q_out, (T*)kv_pool, page_list, sequence_lengths, head_num, kv_head_num, head_dim,
+                             (int)max_blocks_per_seq, page_size, l2b, q_len);
+        });
     });
 }
 
@@ -943,31 +907,25 @@ static int rope_append_ex_impl(const void* qkv, const void* qkv_bias, void* q_ou
     ARG_CHECK(!cos_sin_cache || cache_positions > 0, "rope_append_ex: a cos/sin cache needs its number of positions");
     ARG_CHECK(!use_logn_attn || cfg->max_pos > 1, "rope_append_ex: logn attention needs max_pos > 1");
     ARG_CHECK(batch > 0 && q_len >= 1 && q_len <= 65535, "rope_append_ex: bad shape batch %d x q_len %d", batch, q_len);
-    const b200_rope_config cc = *cfg;
-    if (g_rec)
-        return rec_call([=](void* st) {
-            return rope_append_ex_impl(qkv, qkv_bias, q_out, kv_pool, page_list, sequence_lengths, position_ids, cos_sin_cache,
-                                       cache_positions, &cc, use_logn_attn, is_bf16, batch, q_len, head_num, kv_head_num, head_dim,
-                                       max_blocks_per_seq, page_size, q_gamma, k_gamma, eps, st);
-        });
-    RopeCfg rc{cc.style, cc.dim, cc.base, cc.scale, cc.factor1, cc.factor2, cc.max_pos, cc.extrapolation_factor, cc.mscale};
+    const RopeCfg rc{cfg->style, cfg->dim, cfg->base, cfg->scale, cfg->factor1, cfg->factor2, cfg->max_pos, cfg->extrapolation_factor,
+                     cfg->mscale};
     const dim3 grid(batch, head_num + 2 * kv_head_num, q_len);
-    const bool pdl = g_pdl.load() != 0;
     const float2* cache = reinterpret_cast<const float2*>(cos_sin_cache);
     return by_dtype(is_bf16, [&](auto t) {
         using T = decltype(t);
-        const LaunchCfg lc{grid, dim3(head_dim / 2), 0, (cudaStream_t)stream, pdl};
-        if (q_gamma) {
-            CUDA_CHECK(launch_ex(q_len > 1 ? qk_norm_rope_append_ex_kernel<T, true> : qk_norm_rope_append_ex_kernel<T, false>, lc,
-                                 (const T*)qkv, (T*)q_out, (T*)kv_pool, page_list, sequence_lengths, position_ids, cache,
-                                 cache_positions, rc, use_logn_attn, head_num, kv_head_num, head_dim, max_blocks_per_seq, page_size,
-                                 (const T*)q_gamma, (const T*)k_gamma, eps));
-            return launched("qk_norm_rope_append_ex_kernel");
-        }
-        CUDA_CHECK(launch_ex(q_len > 1 ? rope_append_ex_kernel<T, true> : rope_append_ex_kernel<T, false>, lc, (const T*)qkv,
-                             (const T*)qkv_bias, (T*)q_out, (T*)kv_pool, page_list, sequence_lengths, position_ids, cache,
-                             cache_positions, rc, use_logn_attn, head_num, kv_head_num, head_dim, max_blocks_per_seq, page_size));
-        return launched("rope_append_ex_kernel");
+        if (q_gamma)
+            return launch_or_record("qk_norm_rope_append_ex_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+                return launch_ex(q_len > 1 ? qk_norm_rope_append_ex_kernel<T, true> : qk_norm_rope_append_ex_kernel<T, false>,
+                                 {grid, dim3(head_dim / 2), 0, s, pdl}, (const T*)qkv, (T*)q_out, (T*)kv_pool, page_list,
+                                 sequence_lengths, position_ids, cache, cache_positions, rc, use_logn_attn, head_num, kv_head_num,
+                                 head_dim, max_blocks_per_seq, page_size, (const T*)q_gamma, (const T*)k_gamma, eps);
+            });
+        return launch_or_record("rope_append_ex_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+            return launch_ex(q_len > 1 ? rope_append_ex_kernel<T, true> : rope_append_ex_kernel<T, false>,
+                             {grid, dim3(head_dim / 2), 0, s, pdl}, (const T*)qkv, (const T*)qkv_bias, (T*)q_out, (T*)kv_pool, page_list,
+                             sequence_lengths, position_ids, cache, cache_positions, rc, use_logn_attn, head_num, kv_head_num, head_dim,
+                             max_blocks_per_seq, page_size);
+        });
     });
 }
 
@@ -1019,8 +977,10 @@ int b200_embedding(const int32_t* ids, const void* table, void* out, int is_bf16
         op.e.hidden = hidden;
         return rec_segment_op(op, -1, -1, -1);
     }
-    embedding_kernel<__half><<<rows, 128, 0, (cudaStream_t)stream>>>(ids, (const __half*)table, (__half*)out, hidden);
-    return launched("embedding_kernel");
+    return launch_or_record("embedding_kernel", stream, [=](cudaStream_t s) {
+        embedding_kernel<__half><<<rows, 128, 0, s>>>(ids, (const __half*)table, (__half*)out, hidden);
+        return cudaGetLastError();
+    });
 }
 
 int b200_argmax(const void* logits, int dtype, int rows, int vocab, int32_t* out, void* stream) {
@@ -1028,11 +988,12 @@ int b200_argmax(const void* logits, int dtype, int rows, int vocab, int32_t* out
     ARG_CHECK(logits && out, "argmax: null pointer");
     ARG_CHECK(vocab > 0, "argmax: vocab must be positive");
     ARG_CHECK(dtype >= 0 && dtype <= 2, "argmax: dtype %d unknown (0 fp16, 1 bf16, 2 fp32)", dtype);
-    if (g_rec) return rec_call([=](void* st) { return b200_argmax(logits, dtype, rows, vocab, out, st); });
     auto launch = [&](auto t) {
         using T = decltype(t);
-        argmax_kernel<T><<<rows, 1024, 0, (cudaStream_t)stream>>>((const T*)logits, vocab, out);
-        return launched("argmax_kernel");
+        return launch_or_record("argmax_kernel", stream, [=](cudaStream_t s) {
+            argmax_kernel<T><<<rows, 1024, 0, s>>>((const T*)logits, vocab, out);
+            return cudaGetLastError();
+        });
     };
     return dtype == 2 ? launch(0.f) : by_dtype(dtype == 1, launch);
 }
@@ -1046,11 +1007,6 @@ int b200_sample(float* logits, int rows, int vocab, const int32_t* history, cons
     ARG_CHECK(rows > 0 && rows <= 65535 && vocab > 0, "sample: bad shape [%d, %d]", rows, vocab);
     ARG_CHECK(!history || (hist_len && hist_stride > 0), "sample: history needs hist_len and a positive stride");
     ARG_CHECK(!(repetition || presence || frequency) || (history && count_ws), "sample: penalties need history and count_ws");
-    if (g_rec)
-        return rec_call([=](void* st) {
-            return b200_sample(logits, rows, vocab, history, hist_len, hist_stride, count_ws, temperature, repetition, presence,
-                               frequency, top_k, top_p, uniform, process, token_out, token_prob_out, probs_out, st);
-        });
     SampleParams p{};
     p.logits = logits;
     p.probs_out = probs_out;
@@ -1070,8 +1026,9 @@ int b200_sample(float* logits, int rows, int vocab, const int32_t* history, cons
     p.rows = rows;
     p.vocab = vocab;
     p.hist_stride = hist_stride;
-    CUDA_CHECK(launch_ex(sample_kernel, {dim3(rows), dim3(kSampleThreads), 0, (cudaStream_t)stream, g_pdl.load() != 0}, p));
-    return launched("sample_kernel");
+    return launch_or_record("sample_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+        return launch_ex(sample_kernel, {dim3(rows), dim3(kSampleThreads), 0, s, pdl}, p);
+    });
 }
 
 int b200_spec_verify(const float* target_probs, const int32_t* target_ids, const float* draft_probs, const int32_t* draft_tokens,
@@ -1084,11 +1041,6 @@ int b200_spec_verify(const float* target_probs, const int32_t* target_ids, const
     ARG_CHECK(target_probs || target_ids, "spec_verify: need target_probs (sampling) or target_ids (greedy)");
     ARG_CHECK(!target_probs || uniform, "spec_verify: sampling mode needs uniform");
     ARG_CHECK(!draft_probs || target_probs, "spec_verify: draft_probs need target_probs");
-    if (g_rec)
-        return rec_call([=](void* st) {
-            return b200_spec_verify(target_probs, target_ids, draft_probs, draft_tokens, uniform, batch, num_draft, vocab, out_tokens,
-                                    accepted, st);
-        });
     SpecVerifyParams p{};
     p.target_probs = target_probs;
     p.target_ids = target_ids;
@@ -1099,8 +1051,9 @@ int b200_spec_verify(const float* target_probs, const int32_t* target_ids, const
     p.accepted = accepted;
     p.num_draft = num_draft;
     p.vocab = vocab;
-    CUDA_CHECK(launch_ex(spec_verify_kernel, {dim3(batch), dim3(kSampleThreads), 0, (cudaStream_t)stream, g_pdl.load() != 0}, p));
-    return launched("spec_verify_kernel");
+    return launch_or_record("spec_verify_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+        return launch_ex(spec_verify_kernel, {dim3(batch), dim3(kSampleThreads), 0, s, pdl}, p);
+    });
 }
 
 namespace {
@@ -1155,11 +1108,6 @@ int b200_beam_search_step(const void* logits, int dtype, const float* cum_log_pr
     ARG_CHECK(workspace && workspace_bytes >= w.total,
               "beam_search_step: workspace too small (%zu < %zu bytes, see b200_beam_search_step_workspace_bytes)",
               workspace ? workspace_bytes : (size_t)0, w.total);
-    if (g_rec)
-        return rec_call([=](void* st) {
-            return b200_beam_search_step(logits, dtype, cum_log_probs, batch, beam_width, vocab, eos_id, cand_token, cand_parent,
-                                         cand_score, next_token, next_parent, next_cum, workspace, workspace_bytes, st);
-        });
     char* ws = static_cast<char*>(workspace);
     BeamParams p{};
     p.logits = logits;
@@ -1181,10 +1129,10 @@ int b200_beam_search_step(const void* logits, int dtype, const float* cum_log_pr
     p.V = vocab;
     p.S = (vocab + kBeamChunk - 1) / kBeamChunk;
     p.eos = eos_id;
-    const LaunchCfg cfg{dim3(p.S, batch * beam_width), dim3(kBeamThreads), 0, (cudaStream_t)stream, g_pdl.load() != 0};
     auto launch = [&](auto t) {
-        CUDA_CHECK(launch_ex(beam_search_kernel<decltype(t)>, cfg, p));
-        return launched("beam_search_kernel");
+        return launch_or_record("beam_search_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+            return launch_ex(beam_search_kernel<decltype(t)>, {dim3(p.S, batch * beam_width), dim3(kBeamThreads), 0, s, pdl}, p);
+        });
     };
     return dtype == 2 ? launch(0.f) : by_dtype(dtype == 1, launch);
 }
@@ -1215,12 +1163,6 @@ int b200_beam_hypotheses_update(const int32_t* cand_token, const int32_t* cand_p
     const size_t need = b200_beam_hypotheses_state_bytes(batch, beam_width, max_len);
     ARG_CHECK(state_bytes >= need, "beam_hypotheses_update: state too small (%zu < %zu bytes, see b200_beam_hypotheses_state_bytes)",
               state_bytes, need);
-    if (g_rec)
-        return rec_call([=](void* st) {
-            return b200_beam_hypotheses_update(cand_token, cand_parent, cand_score, history, hist_len, hist_stride, gen_start, batch,
-                                               beam_width, eos_id, length_penalty, early_stopping, max_len, state, state_bytes, done,
-                                               st);
-        });
     BeamHypsParams p{};
     p.cand_token = cand_token;
     p.cand_parent = cand_parent;
@@ -1236,9 +1178,9 @@ int b200_beam_hypotheses_update(const int32_t* cand_token, const int32_t* cand_p
     p.hist_stride = hist_stride;
     p.gen_start = gen_start;
     p.eos = eos_id;
-    CUDA_CHECK(launch_ex(beam_hyps_update_kernel, {dim3(batch), dim3(kBeamHypThreads), 0, (cudaStream_t)stream, g_pdl.load() != 0},
-                         p));
-    return launched("beam_hyps_update_kernel");
+    return launch_or_record("beam_hyps_update_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+        return launch_ex(beam_hyps_update_kernel, {dim3(batch), dim3(kBeamHypThreads), 0, s, pdl}, p);
+    });
 }
 
 int b200_beam_hypotheses_finalize(const void* state, size_t state_bytes, const int32_t* done, const float* beam_cum,
@@ -1253,11 +1195,6 @@ int b200_beam_hypotheses_finalize(const void* state, size_t state_bytes, const i
     const size_t need = b200_beam_hypotheses_state_bytes(batch, beam_width, max_len);
     ARG_CHECK(state_bytes >= need, "beam_hypotheses_finalize: state too small (%zu < %zu bytes, see b200_beam_hypotheses_state_bytes)",
               state_bytes, need);
-    if (g_rec)
-        return rec_call([=](void* st) {
-            return b200_beam_hypotheses_finalize(state, state_bytes, done, beam_cum, history, hist_len, hist_stride, gen_start, batch,
-                                                 beam_width, n, max_len, length_penalty, out_tokens, out_len, out_score, out_cum, st);
-        });
     BeamHypsParams p{};
     p.beam_cum = beam_cum;
     p.history = history;
@@ -1274,9 +1211,9 @@ int b200_beam_hypotheses_finalize(const void* state, size_t state_bytes, const i
     p.max_len = max_len;
     p.hist_stride = hist_stride;
     p.gen_start = gen_start;
-    CUDA_CHECK(launch_ex(beam_hyps_finalize_kernel, {dim3(batch), dim3(kBeamHypThreads), 0, (cudaStream_t)stream, g_pdl.load() != 0},
-                         p));
-    return launched("beam_hyps_finalize_kernel");
+    return launch_or_record("beam_hyps_finalize_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+        return launch_ex(beam_hyps_finalize_kernel, {dim3(batch), dim3(kBeamHypThreads), 0, s, pdl}, p);
+    });
 }
 #undef BEAM_HYPS_CHECKS
 
@@ -1325,11 +1262,6 @@ int b200_token_logprobs(const void* logits, int dtype, int rows, int vocab, int 
     ARG_CHECK(workspace && workspace_bytes >= w.total,
               "token_logprobs: workspace too small (%zu < %zu bytes, see b200_token_logprobs_workspace_bytes)",
               workspace ? workspace_bytes : (size_t)0, w.total);
-    if (g_rec)
-        return rec_call([=](void* st) {
-            return b200_token_logprobs(logits, dtype, rows, vocab, top_n, tokens, token_logprob, top_ids, top_logprobs, workspace,
-                                       workspace_bytes, st);
-        });
     char* ws = static_cast<char*>(workspace);
     LogprobParams p{};
     p.logits = logits;
@@ -1344,10 +1276,10 @@ int b200_token_logprobs(const void* logits, int dtype, int rows, int vocab, int 
     p.V = vocab;
     p.S = (vocab + kBeamChunk - 1) / kBeamChunk;
     p.top_n = top_n;
-    const LaunchCfg cfg{dim3(p.S, rows), dim3(kBeamThreads), 0, (cudaStream_t)stream, g_pdl.load() != 0};
     auto launch = [&](auto t) {
-        CUDA_CHECK(launch_ex(token_logprobs_kernel<decltype(t)>, cfg, p));
-        return launched("token_logprobs_kernel");
+        return launch_or_record("token_logprobs_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+            return launch_ex(token_logprobs_kernel<decltype(t)>, {dim3(p.S, rows), dim3(kBeamThreads), 0, s, pdl}, p);
+        });
     };
     return dtype == 2 ? launch(0.f) : by_dtype(dtype == 1, launch);
 }
@@ -1360,10 +1292,6 @@ int b200_ban_repeat_ngram(void* logits, int dtype, int rows, int vocab, const in
     ARG_CHECK(hist_stride > 0, "ban_repeat_ngram: hist_stride must be positive");
     if (rows == 0) return B200_OK;
     ARG_CHECK(logits && history && hist_len && ngram_size, "ban_repeat_ngram: null pointer");
-    if (g_rec)
-        return rec_call([=](void* st) {
-            return b200_ban_repeat_ngram(logits, dtype, rows, vocab, history, hist_len, hist_stride, ngram_size, st);
-        });
     BanNgramParams p{};
     p.logits = logits;
     p.history = history;
@@ -1371,10 +1299,10 @@ int b200_ban_repeat_ngram(void* logits, int dtype, int rows, int vocab, const in
     p.ngram_size = ngram_size;
     p.vocab = vocab;
     p.hist_stride = hist_stride;
-    const LaunchCfg cfg{dim3(rows), dim3(256), 0, (cudaStream_t)stream, g_pdl.load() != 0};
     auto launch = [&](auto t) {
-        CUDA_CHECK(launch_ex(ban_repeat_ngram_kernel<decltype(t)>, cfg, p));
-        return launched("ban_repeat_ngram_kernel");
+        return launch_or_record("ban_repeat_ngram_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+            return launch_ex(ban_repeat_ngram_kernel<decltype(t)>, {dim3(rows), dim3(256), 0, s, pdl}, p);
+        });
     };
     return dtype == 2 ? launch(0.f) : by_dtype(dtype == 1, launch);
 }
@@ -1415,35 +1343,25 @@ int b200_peer_allreduce(const void* in, void* out, size_t bytes, int is_bf16, vo
     ARG_CHECK(valid_peer_group(rank, world), "peer_allreduce: bad rank/world %d/%d", rank, world);
     ARG_CHECK(bytes > 0 && bytes % 16 == 0 && bytes <= max_message_bytes, "peer_allreduce: message of %zu bytes unsupported", bytes);
     ARG_CHECK((((uintptr_t)in | (uintptr_t)out) & 15) == 0, "peer_allreduce: in/out must be 16-byte aligned");
-    if (g_rec) {
-        const auto regs = copy_regions(regions, world);
-        return rec_call([=](void* st) {
-            return b200_peer_allreduce(in, out, bytes, is_bf16, regs.data(), max_message_bytes, 0, rank, world, st);
-        });
-    }
     PeerArParams p{};
     p.in = in;
     p.out = out;
     int rc = fill_ar_params(p, regions, max_message_bytes, rank, world);
     if (rc) return rc;
     p.n16 = (int)(bytes / 16);
-    int ctas = (p.n16 + 2 * kArThreads - 1) / (2 * kArThreads);   // ~2 chunks (32 B of payload) per thread
-    if (ctas < 1) ctas = 1;
-    if (ctas > kArMaxCtas) ctas = kArMaxCtas;
-    const bool pdl = g_pdl.load() != 0;
     // W >= 3: reduce-scatter + all-gather (2 hops, (W-1)/W of the volume twice); W == 2: one hop. Env override for tests.
     const int two_shot = env_int("B200_AR_TWOSHOT", world >= 3 ? 1 : 0) && (p.n16 % world == 0);
+    // one shot: ~2 chunks (32 B of payload) per thread; two shots: one chunk of the rank's 1/W share per thread
+    int ctas = two_shot ? (p.n16 / world + kArThreads - 1) / kArThreads : (p.n16 + 2 * kArThreads - 1) / (2 * kArThreads);
+    if (ctas < 1) ctas = 1;
+    if (ctas > kArMaxCtas) ctas = kArMaxCtas;
     return by_dtype(is_bf16, [&](auto t) {
         using T = decltype(t);
-        if (two_shot) {
-            int c2 = (p.n16 / world + kArThreads - 1) / kArThreads;
-            if (c2 < 1) c2 = 1;
-            if (c2 > kArMaxCtas) c2 = kArMaxCtas;
-            CUDA_CHECK(launch_ex(peer_allreduce_twoshot_kernel<T>, {dim3(c2), dim3(kArThreads), 0, (cudaStream_t)stream, pdl}, p));
-            return launched("peer_allreduce_twoshot_kernel");
-        }
-        CUDA_CHECK(launch_ex(peer_allreduce_kernel<T>, {dim3(ctas), dim3(kArThreads), 0, (cudaStream_t)stream, pdl}, p));
-        return launched("peer_allreduce_kernel");
+        return launch_or_record(two_shot ? "peer_allreduce_twoshot_kernel" : "peer_allreduce_kernel", stream,
+                                [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+            return launch_ex(two_shot ? peer_allreduce_twoshot_kernel<T> : peer_allreduce_kernel<T>,
+                             {dim3(ctas), dim3(kArThreads), 0, s, pdl}, p);
+        });
     });
 }
 
@@ -1456,12 +1374,6 @@ static int allreduce_norm_impl(const void* in, void* residual, const void* gamma
     ARG_CHECK(hidden > 0 && hidden % (8 * world) == 0 && hidden <= 8192, "peer_allreduce_norm: hidden %d must be a multiple of 8*world and <= 8192", hidden);
     ARG_CHECK((size_t)rows * hidden * 2 <= max_message_bytes, "peer_allreduce_norm: message of %zu bytes exceeds the region", (size_t)rows * hidden * 2);
     ARG_CHECK((((uintptr_t)in | (uintptr_t)residual | (uintptr_t)gamma | (uintptr_t)y) & 15) == 0, "peer_allreduce_norm: pointers must be 16-byte aligned");
-    if (g_rec) {
-        const auto regs = copy_regions(regions, world);
-        return rec_call([=](void* st) {
-            return allreduce_norm_impl(in, residual, gamma, y, is_bf16, rows, hidden, eps, regs.data(), max_message_bytes, rank, world, pushed, st);
-        });
-    }
     PeerArParams p{};
     p.in = in;
     int rc = fill_ar_params(p, regions, max_message_bytes, rank, world);
@@ -1474,10 +1386,10 @@ static int allreduce_norm_impl(const void* in, void* residual, const void* gamma
     p.eps = eps;
     p.pushed = pushed;
     const size_t smem = (size_t)hidden * sizeof(float) + (size_t)(hidden / 8 / world) * 16;
-    const bool pdl = g_pdl.load() != 0;
     return by_dtype(is_bf16, [&](auto t) {
-        CUDA_CHECK(launch_ex(peer_allreduce_norm_kernel<decltype(t)>, {dim3(rows), dim3(kArThreads), smem, (cudaStream_t)stream, pdl}, p));
-        return launched("peer_allreduce_norm_kernel");
+        return launch_or_record("peer_allreduce_norm_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+            return launch_ex(peer_allreduce_norm_kernel<decltype(t)>, {dim3(rows), dim3(kArThreads), smem, s, pdl}, p);
+        });
     });
 }
 
@@ -1495,12 +1407,6 @@ int b200_peer_argmax(const void* logits, int is_bf16, int rows, int vocab_local,
     ARG_CHECK(logits && out && regions, "peer_argmax: null pointer");
     ARG_CHECK(valid_peer_group(rank, world), "peer_argmax: bad rank/world %d/%d", rank, world);
     ARG_CHECK(rows > 0 && (size_t)rows * 16 <= max_message_bytes && vocab_local > 0 && vocab_total > 0, "peer_argmax: bad shape");
-    if (g_rec) {
-        const auto regs = copy_regions(regions, world);
-        return rec_call([=](void* st) {
-            return b200_peer_argmax(logits, is_bf16, rows, vocab_local, vocab_total, out, regs.data(), max_message_bytes, rank, world, st);
-        });
-    }
     PeerArParams p{};
     int rc = fill_ar_params(p, regions, max_message_bytes, rank, world);
     if (rc) return rc;
@@ -1509,10 +1415,10 @@ int b200_peer_argmax(const void* logits, int is_bf16, int rows, int vocab_local,
     p.rows = rows;
     p.vocab_local = vocab_local;
     p.vocab_total = vocab_total;
-    const bool pdl = g_pdl.load() != 0;
     return by_dtype(is_bf16, [&](auto t) {
-        CUDA_CHECK(launch_ex(peer_argmax_kernel<decltype(t)>, {dim3(rows), dim3(kArThreads), 0, (cudaStream_t)stream, pdl}, p));
-        return launched("peer_argmax_kernel");
+        return launch_or_record("peer_argmax_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+            return launch_ex(peer_argmax_kernel<decltype(t)>, {dim3(rows), dim3(kArThreads), 0, s, pdl}, p);
+        });
     });
 }
 
@@ -1576,7 +1482,7 @@ int b200_program_launch(b200_program* p, void* stream) {
             });
             g_ftrace_next = nullptr;
         } else {
-            rc = it.fn(stream);
+            rc = launch_or_record(it.name, stream, it.issue);   // not recording (checked above): launches now
         }
         if (rc) return rc;
     }

@@ -22,8 +22,9 @@ int launch_one(const CUtensorMap& xmap, const CUtensorMap& wmap, const ParamsT& 
     if (rc) return rc;
     // VAR 1, nsplit > 1: the nsplit CTAs of a tile form one cluster along y; the plain kernels launch single CTAs
     const dim3 grid(n_tiles, p.nsplit), cluster(1, B200_GEMM_VAR == 1 ? p.nsplit : 1);
-    CUDA_CHECK(launch_ex(kern, {grid, dim3(gemm_threads()), smem, st, p.use_pdl != 0, cluster}, xmap, wmap, p));
-    return launched("wo_gemm_kernel");
+    return launch_or_record("wo_gemm_kernel", st, [=](cudaStream_t s) {
+        return launch_ex(kern, {grid, dim3(gemm_threads()), smem, s, p.use_pdl != 0, cluster}, xmap, wmap, p);
+    });
 }
 
 template <int FMT, typename T>

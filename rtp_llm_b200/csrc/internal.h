@@ -7,7 +7,9 @@
 
 #include <cstdarg>
 #include <cstdio>
+#include <functional>
 #include <string>
+#include <utility>
 
 #include "../../include/b200_decode_ops.h"
 
@@ -94,6 +96,20 @@ static cudaError_t launch_ex(void (*kern)(KArgs...), const LaunchCfg& c, Args...
     cfg.attrs = attr;
     cfg.numAttrs = na;
     return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
+}
+
+extern thread_local b200_program* g_rec;   // the program this thread is recording, or null
+int record_launch(const char* name, std::function<cudaError_t(cudaStream_t)> issue);   // appends a launch to g_rec
+
+// Every launch of an op goes through here. `issue` makes one launch of kernel `name` on the stream it is given, with the
+// arguments it holds by value, and returns its error. Outside a recording it runs now; while recording, the program keeps it
+// and runs it at every b200_program_launch, where nothing else of the op is evaluated again.
+template <typename F>
+static int launch_or_record(const char* name, void* stream, F&& issue) {
+    if (g_rec) return record_launch(name, std::forward<F>(issue));
+    const cudaError_t e = issue((cudaStream_t)stream);
+    if (e != cudaSuccess) return fail(B200_ECUDA, "launch of %s failed: %s", name, cudaGetErrorString(e));
+    return launched(name);
 }
 
 // gemm_cluster.cu: the one-kernel-per-GEMM path (split-K merged through L2); FP16 weights and batches > 64 use it

@@ -60,8 +60,9 @@ int launch_segment(int bpad, int qfmt, const ProgOp* d_ops, int nops, unsigned* 
                    unsigned long long* trace, cudaStream_t st) {
     unsigned long long* ftrace = g_ftrace_next;   // developer fine timeline of the next launch (b200_program_set_trace)
     return seg_dispatch<T>(bpad, qfmt, [&](auto kern, int smem) {
-        CUDA_CHECK(launch_ex(kern, {dim3(grid), dim3(kSegThreads), (size_t)smem, st, pdl}, d_ops, nops, gbar, pdl ? 1 : 0, trace, ftrace));
-        return launched("decode_segment_kernel");
+        return launch_or_record("decode_segment_kernel", st, [=](cudaStream_t s) {
+            return launch_ex(kern, {dim3(grid), dim3(kSegThreads), (size_t)smem, s, pdl}, d_ops, nops, gbar, pdl ? 1 : 0, trace, ftrace);
+        });
     });
 }
 
