@@ -338,6 +338,228 @@ def silu_mul_budget(g, Ag, u, Au, K: int, nsplit: int, is_bf16: bool) -> np.ndar
 
 
 # ----------------------------------------------------------------------------------------------
+# Glue ops: float64 references and error budgets (RMSNorm, QK-RMSNorm, RoPE); SiLU*mul reuses silu_mul_np / _budget
+# ----------------------------------------------------------------------------------------------
+def rmsnorm_np(x, residual, gamma, eps, bias=None) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """Float64 RMSNorm of the rows of x (+ residual), flashinfer's fused-add contract (DESIGN section 3.3): s = x + r exact,
+    y = s * g / sqrt(mean(s^2) + eps) (+ bias), and the stored residual round_T(s) is round_t(s) by the caller.
+    x, residual [rows, n] (residual may be None), gamma / bias [n]: T values as floats (or anything float). eps is taken
+    as the fp32 value the kernels receive. Returns (y, s, A): A = |s * g / rms| + |bias|, the size of the terms of y that
+    norm_error_budget scales. QK-RMSNorm is this per head, with the bias added before the one rounding to T."""
+    s = np.asarray(x, np.float64)
+    if residual is not None:
+        s = s + np.asarray(residual, np.float64)
+    inv = 1.0 / np.sqrt(np.mean(s * s, axis=-1, keepdims=True) + float(np.float32(eps)))
+    y = s * inv * np.asarray(gamma, np.float64)
+    A = np.abs(y)
+    if bias is not None:
+        b = np.asarray(bias, np.float64)
+        y, A = y + b, A + np.abs(b)
+    return y, s, A
+
+
+def norm_chain(hidden: int, threads: int) -> int:
+    """The longest fp32 add chain of a norm kernel's sum of squares: the per-thread fmaf chain (8 elements per 16-byte
+    vector, ceil(hidden / 8 / threads) vectors) plus 16 for the warp butterfly and the cross-warp sum (5 + at most 8 adds in
+    the persistent kernel, 5 + 5 in the stand-alone one)."""
+    return 8 * (-(-hidden // (8 * threads))) + 16
+
+
+def norm_error_budget(ref: np.ndarray, A: np.ndarray, chain: int, is_bf16: bool) -> np.ndarray:
+    """Per-element bound on |y - ref| for an RMSNorm kernel in T = fp16 / bf16 against rmsnorm_np's (ref, A):
+    ulp_T(ref) + 2^-24 * (chain / 2 + 12) * A, chain = norm_chain(...) (QK-RMSNorm: head_dim / 32 + 5).
+
+    Why (u = 2^-24, the relative error of one fp32 rounding to nearest): s = x + r rounds once in fp32 (u |s|; exact
+    unless the two exponents are more than 13 apart). The sum of squares is a tree of nonnegative terms whose deepest path
+    is `chain` roundings (each fmaf of the per-thread chain rounds once, each butterfly or cross-warp add once), so it is
+    within chain * u of the exact sum, relatively. The mean (a division by hidden) and + eps round once each; rsqrtf is
+    within 2 ulp (CUDA C Programming Guide, table of single-precision functions), 4 u relatively; the square root halves
+    the relative error of its argument, so 1 / rms is within ((chain + 2) / 2 + 4 + 1) u. The two products s * inv * g round
+    once each (2 u), the optional bias add once more (u relative to A). In all, (chain / 2 + 9) u of A; 12 leaves room for
+    the first-order terms dropped. The one final rounding to T is half an ulp_T; ulp_T(ref) leaves room for the value
+    crossing a binade. eps is inside the square root, so a row whose mean square is near eps is no harder: the bound is
+    relative to the output, and a kernel that adds eps after the square root misses it by far on such rows."""
+    return ulp(ref, is_bf16) + 2.0 ** -24 * (chain / 2 + 12) * np.asarray(A, np.float64)
+
+
+# Thresholds of gemm_rounded_fractions for the glue ops on random data (correctly rounded, within one T step), set below
+# what the kernels gave on an H100 80GB HBM3 (700 W power limit) over the cases of tests/test_gpu_glue_exact.py and above
+# the CPU mutants of tests/test_glue_budget.py.
+# Norms (stand-alone, persistent kernel, QK-RMSNorm): at least 0.99951 / 1.0 measured; rounding y twice or s before the
+# variance gives 0.74-0.80 correctly rounded.
+NORM_MIN_ROUNDED = 0.99
+NORM_MIN_WITHIN_ONE = 0.9999
+# SiLU*mul (one fp32 evaluation of a few ulps, rounded once): at least 0.99991 / 1.0 measured.
+SILU_MIN_ROUNDED = 0.99
+SILU_MIN_WITHIN_ONE = 0.9999
+# RoPE, over the outputs whose fp32 error bound is below an eighth of ulp_T (rope_fraction_mask: the short positions, where
+# the angle is nearly exact): at least 0.99898 / 1.0 measured; a bias added without rounding it to T first gives 0.79-0.81
+# / 0.978-0.987 there.
+ROPE_MIN_ROUNDED = 0.99
+ROPE_MIN_WITHIN_ONE = 0.9999
+
+ROPE_PI32 = float(np.float32(3.141592654))       # the kernels' fp32 pi (Yarn's correction range, Llama3's wavelength)
+
+
+def yarn_ramp_bounds(cfg) -> Tuple[float, float]:
+    """Yarn's ramp bounds (lo, hi) as aux_kernels.cuh rope_coef computes them: from (int)base, floor / ceil to integers,
+    clamped to [0, dim - 1], hi nudged by 0.001 when they meet. They do not depend on the position."""
+    dim, mp = int(cfg["dim"]), float(np.float32(cfg["max_pos"]))
+    t1 = 2.0 * np.log(float(int(np.float32(cfg["base"]))))
+    f1, f2 = float(np.float32(cfg["factor1"])), float(np.float32(cfg["factor2"]))
+    low = int(np.floor(dim * np.log(mp / (f2 * 2 * ROPE_PI32)) / t1))
+    high = int(np.ceil(dim * np.log(mp / (f1 * 2 * ROPE_PI32)) / t1))
+    lo, hi = float(max(low, 0)), float(min(high, dim - 1))
+    if lo == hi:
+        hi += 0.001
+    return lo, hi
+
+
+def rope_angle_np(cfg, zid, pos, seq_len=None) -> Tuple[np.ndarray, float, np.ndarray]:
+    """Float64 angle of channel pair zid / 2 (zid = 2i) at integer position pos, and the coefficient scale, for the rope
+    contract of b200_rope_append_ex (aux_kernels.cuh rope_coef, DESIGN section 4), and dA, a bound on how far the kernel's
+    fp32 angle may be from it. cfg: the RopeConfig fields (its floats taken as the fp32 values the kernel holds); the plain
+    kernels' angle is rope_plain_angle_np. seq_len defaults to pos + 1 (the NTK styles' step uses it; a test may move it).
+    Returns (a, sc, dA), a / dA broadcast over zid and pos.
+
+    dA, in units of u = 2^-24 times |a|: powf is within 4 ulp (8 u) and its exponent zid / dim rounds once (u times
+    |log(base')| times zid / dim); the division pos / powf rounds once; every later fp32 step (/ scale, Yarn's blend of
+    three roundings, Llama3's smooth factor, whose relative error ~6 u * (max_pos / wavelen + factor1) / (factor2 - factor1)
+    moves a by that times |a - a / scale| <= |a|) adds its own. For the NTK styles past max_pos the rescaled base' =
+    base * powf(X, dim / (dim - 2)) carries powf's 8 u, the exponent's rounding times |log X| and X's own three or four
+    roundings amplified by dim / (dim - 2) <= 2: bounded by 64 u here, and it reaches a through the exponent zid / dim <= 1."""
+    c = {k: float(np.float32(v)) if isinstance(v, float) else v for k, v in cfg.items()}
+    style, dim, mp = int(c["style"]), int(c["dim"]), int(c["max_pos"])
+    zid = np.asarray(zid, np.float64)
+    pos = np.asarray(pos, np.float64)
+    sl = pos + 1 if seq_len is None else np.asarray(seq_len, np.float64)
+    base = np.full(np.broadcast(zid, pos).shape, c["base"])
+    eb = np.zeros_like(base)
+    if style == 3:
+        X = c["scale"] * sl / mp - (c["scale"] - 1.0)
+        step = sl > mp
+        base = np.where(step, c["base"] * np.abs(X) ** (dim / (dim - 2.0)), base)
+        eb = np.where(step, 64.0, 0.0) + eb
+    if style == 4:
+        ctx = np.log2(sl / mp) + 1.0
+        ntk = np.maximum(2.0 ** np.ceil(ctx) - 1.0, 1.0)
+        step = sl > mp
+        base = np.where(step, c["base"] * ntk ** (dim / (dim - 2.0)), base)
+        eb = np.where(step, 64.0, 0.0) + eb
+    t = zid / dim
+    a = pos / base ** t
+    da = 8.0 + 1.0 + t * eb + t * np.abs(np.log(base)) + 1.0
+    sc = 1.0
+    if style in (1, 7):
+        a = a / c["scale"]
+        da = da + 1.0
+    elif style == 5:
+        lo, hi = yarn_ramp_bounds(c)
+        ramp = np.clip((np.floor(zid / 2) - lo) / (hi - lo), 0.0, 1.0)
+        mask = (1.0 - ramp) * c["extrapolation_factor"]
+        a = (a / c["scale"]) * (1.0 - mask) + a * mask
+        da = da + 8.0
+        sc = c["mscale"]
+    elif style == 6:
+        wavelen = np.where(a == 0, np.inf, 2 * np.pi / np.where(a == 0, 1.0, a))
+        low_w, high_w = mp / c["factor1"], mp / c["factor2"]
+        smooth = (mp / wavelen - c["factor1"]) / (c["factor2"] - c["factor1"])
+        mid = (1 - smooth) * a / c["scale"] + smooth * a
+        a = np.where(wavelen < high_w, a, np.where(wavelen > low_w, a / c["scale"], mid))
+        da = da + 4.0 + 6.0 * (mp / wavelen + c["factor1"]) / (c["factor2"] - c["factor1"])
+    return a, sc, np.abs(a) * da * 2.0 ** -24
+
+
+def rope_plain_angle_np(base, head_dim, i, pos) -> Tuple[np.ndarray, np.ndarray]:
+    """Float64 angle pos * base^(-2i/D) of the plain RoPE kernels (rope_append_kernel, the persistent kernel's rope op, the
+    attention kernel's fused rope) and dA, a bound on their fp32 angle's distance from it. The kernel forms
+    e = fl(fl(-2i / D) * l2b), l2b = log2(base) rounded to fp32 on the host (within 1 ulp), then exp2f(e) (2 ulp) and
+    fl(pos * that). e is within 3 u |e| of the exact exponent (u = 2^-24), which moves 2^e by ln 2 * 3 u |e| relatively;
+    exp2f adds 4 u, the product u: dA = |a| * u * (5 + 2.08 |e|). At i = 0 the kernel's angle is exact (e = -0, 2^e = 1),
+    everywhere else dA grows like |a|: about 0.04 rad at position 131071 for the first pairs, which no fp32 RoPE avoids."""
+    base = float(np.float32(base))
+    i = np.asarray(i, np.float64)
+    pos = np.asarray(pos, np.float64)
+    e = -2.0 * i / head_dim * np.log2(base)
+    a = pos * 2.0 ** e
+    return a, np.abs(a) * 2.0 ** -24 * (5.0 + 3.0 * np.log(2.0) * np.abs(e))
+
+
+def rope_np(qkv, head_num, kv_head_num, head_dim, positions, base=None, cfg=None, bias=None, cos_sin_cache=None,
+            use_logn=False, is_bf16=False) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """Float64 RoPE of one token per row: qkv [B, (Hq + 2 Hkv) * D] T values (or bits), positions [B] (already resolved:
+    position_ids where > 0, else the slot). The plain kernels: base given, cfg None (Base style, rotary dim = D). The
+    rope_append_ex contract: cfg (RopeConfig fields), optional bias [(Hq + 2 Hkv) * D] added and rounded to T first,
+    cos_sin_cache fp32 [P, dim] interleaved (cos, sin) used for pos < P, logn on q heads past max_pos.
+    NeoX pairing (i, i + dim / 2) inside the first `dim` channels; the rest pass through.
+
+    Returns (out, R, dA), each [B, Hq + 2 Hkv, D]: out the rotated q / k heads and the v heads (as stored: the input,
+    with the bias rounded in); R = |logn| * ||(x_i, x_(i + dim/2))|| of each element's pair (|x| past the rotary dim), dA
+    the pair's angle bound (0 from the cache: the kernel uses those fp32 values as given). rope_error_budget takes them."""
+    x = _vals(qkv, is_bf16)
+    B = x.shape[0]
+    H = head_num + 2 * kv_head_num
+    x = x.reshape(B, H, head_dim).copy()
+    if bias is not None:
+        x = round_t(x + _vals(bias, is_bf16).reshape(1, H, head_dim), is_bf16)
+    dim = head_dim if cfg is None else int(cfg["dim"])
+    rot = cfg is None or int(cfg["style"]) != 0
+    half = dim // 2
+    pos = np.asarray(positions, np.int64)
+    i = np.arange(half)
+    if cfg is None:
+        a, dA = rope_plain_angle_np(base, head_dim, i[None, :], pos[:, None])
+        sc = 1.0
+    else:
+        a, sc, dA = rope_angle_np(cfg, 2 * i[None, :], pos[:, None])
+    cs, sn = sc * np.cos(a), sc * np.sin(a)
+    if cos_sin_cache is not None and cfg is not None:
+        cache = np.asarray(cos_sin_cache, np.float64).reshape(cos_sin_cache.shape[0], -1, 2)
+        hit = pos < cache.shape[0]
+        rows = cache[np.where(hit, pos, 0)]
+        cs = np.where(hit[:, None], rows[..., 0], cs)
+        sn = np.where(hit[:, None], rows[..., 1], sn)
+        dA = np.where(hit[:, None], 0.0, dA)
+    out = x.copy()
+    R = np.abs(x)
+    dAx = np.zeros_like(x)
+    qk = slice(0, head_num + kv_head_num)
+    if rot:
+        x0, x1 = x[:, qk, :half], x[:, qk, half:dim]
+        c, s = cs[:, None, :], sn[:, None, :]
+        out[:, qk, :half] = x0 * c - x1 * s
+        out[:, qk, half:dim] = x1 * c + x0 * s
+        nrm = np.hypot(x0, x1) * max(abs(sc), 1.0)
+        R[:, qk, :half] = nrm
+        R[:, qk, half:dim] = nrm
+        dAx[:, qk, :half] = dA[:, None, :]
+        dAx[:, qk, half:dim] = dA[:, None, :]
+    if use_logn and cfg is not None:
+        mp = int(cfg["max_pos"])
+        L = np.where(pos > mp, np.log(pos + 1.0) / np.log(float(mp)), 1.0)[:, None, None]
+        out[:, :head_num] *= L
+        R[:, :head_num] *= L
+    return out, R, dAx
+
+
+def rope_error_budget(ref, R, dA, is_bf16: bool) -> np.ndarray:
+    """Per-element bound on |y - ref| for a RoPE kernel in T against rope_np's (ref, R, dA): ulp_T(ref) + R * (dA + 16 u),
+    u = 2^-24. Why: an angle off by dA rotates the pair by dA, moving each output by at most ||(x0, x1)|| dA. sincosf is
+    within 2 ulp (<= 4 u absolute on cos and sin, so up to 4 sqrt(2) u ||x|| on an output), the rotation's product and
+    fma round once each (2 u ||x||), Yarn's mscale product and logn's factor (two logf of 1 ulp, a division, a product:
+    <= 8 u) the rest. The one final rounding to T is half an ulp_T. A position off by one moves the angle of pair 0 by
+    one radian, which no budget of this form allows; a bias not rounded to T first moves an output by a fraction of an ulp_T,
+    which the rounded fractions see (rope_fraction_mask)."""
+    return ulp(ref, is_bf16) + np.asarray(R, np.float64) * (np.asarray(dA, np.float64) + 16 * 2.0 ** -24)
+
+
+def rope_fraction_mask(ref, R, dA, is_bf16: bool) -> np.ndarray:
+    """The outputs where the fp32 part of rope_error_budget is below an eighth of ulp_T(ref): there a correct kernel rounds
+    almost every output correctly, so gemm_rounded_fractions against ROPE_MIN_* is a sharp check."""
+    return np.asarray(R) * (np.asarray(dA) + 16 * 2.0 ** -24) <= ulp(ref, is_bf16) / 8
+
+
+# ----------------------------------------------------------------------------------------------
 # Weight-only quantisation
 # ----------------------------------------------------------------------------------------------
 def unpack_groupwise_int4(qweight, qzeros, scales_f16, group: int, is_gptq: bool):

@@ -738,11 +738,14 @@ int b200_wo_gemm_rs(int fmt, int is_bf16, const void* x, int B, int K, int N, co
 }
 
 // ------------------------------------------------------------------------------------------------ glue ops
+static constexpr int kNormMaxHidden = 12288;   // the stand-alone norm stages its row in shared memory: 48 KB at the limit
+
 int b200_add_rmsnorm(const void* x, void* residual, const void* gamma, void* y, int is_bf16, int rows, int hidden,
                      float eps, void* stream) {
     if (rows == 0) return B200_OK;
     ARG_CHECK(x && gamma && y, "add_rmsnorm: null pointer");
-    ARG_CHECK(hidden > 0 && hidden % 8 == 0 && hidden <= 12288, "add_rmsnorm: hidden=%d must be a multiple of 8, <= 12288", hidden);
+    ARG_CHECK(hidden > 0 && hidden % 8 == 0 && hidden <= kNormMaxHidden, "add_rmsnorm: hidden=%d must be a multiple of 8, <= %d", hidden,
+              kNormMaxHidden);
     if (g_rec && hidden <= kSegNormMaxHidden) {
         ProgOp op{};
         op.type = kOpNorm;
@@ -759,6 +762,9 @@ int b200_add_rmsnorm(const void* x, void* residual, const void* gamma, void* y, 
     const size_t smem = (size_t)hidden * sizeof(float);
     return by_dtype(is_bf16, [&](auto t) {
         using T = decltype(t);
+        // the staged row is 48 KB at the limit: with the kernel's static s_red that is past the default dynamic limit
+        const int rc = configure_once<add_rmsnorm_kernel<T>>(kNormMaxHidden * (int)sizeof(float));
+        if (rc) return rc;
         return launch_or_record("add_rmsnorm_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
             return launch_ex(add_rmsnorm_kernel<T>, {dim3(rows), dim3(threads), smem, s, pdl}, (const T*)x, (T*)residual,
                              (const T*)gamma, (T*)y, hidden, eps);
