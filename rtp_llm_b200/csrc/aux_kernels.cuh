@@ -248,84 +248,27 @@ __device__ __forceinline__ float qk_norm_apply(T v, float scale, T g) {
     return to_f32<T>(from_f32<T>(to_f32<T>(v) * scale * to_f32<T>(g)));
 }
 
-// Decode RoPE (NeoX pairing, RopeStyle::Base, angle = pos * base^(-2i/dim)) + K,V append into the paged cache.
-// Contract: SURVEY.md appendix C; call site /root/reference/rtp_llm/ops/fused_rope_kvcache_op.py:202-246.
-// q_len new tokens per sequence (speculative-token verification): row x of qkv [B*q_len] is token j = x % q_len of sequence
-// b = x / q_len, rotated and appended at position seq_lens[b] + j; q_out [B*q_len][Hq*D].
-// grid (B*q_len, Hq + 2*Hkv), D/2 threads. MULTI = false is the one-token instance (q_len == 1, no division by q_len).
-// QKN: q and k heads are RMS-normalised first (qk_norm_scale); the bits of b200_qk_rmsnorm followed by this kernel.
-template <typename T, bool MULTI, bool QKN>
-__device__ __forceinline__ void rope_append_body(const T* __restrict__ qkv, T* __restrict__ q_out, T* __restrict__ kv_pool,
-                                                 const int32_t* __restrict__ page_list, const int32_t* __restrict__ seq_lens,
-                                                 int head_num, int kv_head_num, int head_dim, int max_blocks, int tokens_per_block,
-                                                 float log2_base, int q_len, const T* __restrict__ q_gamma,
-                                                 const T* __restrict__ k_gamma, float eps) {
-    pdl_launch_dependents();
-    const int x = blockIdx.x, h = blockIdx.y, i = threadIdx.x, half = head_dim / 2;
-    T g0, g1;   // QKN: the gammas are weights, constant after load, so they are read before the PDL wait
-    if constexpr (QKN) {
-        if (h < head_num + kv_head_num) {
-            const T* gamma = h < head_num ? q_gamma : k_gamma;
-            g0 = gamma[i];
-            g1 = gamma[i + half];
-        }
-    }
-    pdl_wait();
-    const int b = MULTI ? x / q_len : x;
-    const int pos = seq_lens[b] + (MULTI ? x % q_len : 0);
-    const T* src = qkv + ((size_t)x * (head_num + 2 * kv_head_num) + h) * head_dim;
-    const size_t page_elems = (size_t)kv_head_num * tokens_per_block * head_dim;
-    T* dst;
-    bool rotate = true;
-    if (h < head_num) {
-        dst = q_out + ((size_t)x * head_num + h) * head_dim;
-    } else {
-        const bool is_v = h >= head_num + kv_head_num;
-        const int kvh = is_v ? h - head_num - kv_head_num : h - head_num;
-        const int32_t page = page_list[((size_t)b * 2 + (is_v ? 1 : 0)) * max_blocks + pos / tokens_per_block];
-        dst = kv_pool + (size_t)page * page_elems + ((size_t)kvh * tokens_per_block + pos % tokens_per_block) * head_dim;
-        rotate = !is_v;
-    }
-    float x0 = to_f32<T>(src[i]), x1 = to_f32<T>(src[i + half]);
-    if (rotate) {
-        const float inv_freq = exp2f(-2.0f * (float)i / (float)head_dim * log2_base);
-        float sn, cs;
-        sincosf((float)pos * inv_freq, &sn, &cs);
-        if constexpr (QKN) {   // q or k head (uniform over the CTA: the barrier inside is safe), after the angle
-            const float scale = qk_norm_scale<T>(src, head_dim, eps);
-            x0 = qk_norm_apply<T>(src[i], scale, g0);
-            x1 = qk_norm_apply<T>(src[i + half], scale, g1);
-        }
-        float r0, r1;
-        rope_rotate(x0, x1, cs, sn, r0, r1);
-        dst[i] = from_f32<T>(r0);
-        dst[i + half] = from_f32<T>(r1);
-    } else {
-        dst[i] = src[i];
-        dst[i + half] = src[i + half];
-    }
-}
+// The plain Base rope + K/V append of one token per sequence: the persistent kernel's rope op (seg_rope), and the part of
+// rope_append_kernel's parameters every mode uses.
+struct RopeParams {
+    const void* qkv;             // [B*q_len][(Hq + 2*Hkv) * D]
+    void* q_out;                 // [B*q_len][Hq * D]
+    void* kv_pool;               // [pages][Hkv][page_size][D]
+    const int32_t* page_list;    // [B][2][max_blocks]: K pages, then V pages
+    const int32_t* seq_lens;     // [B] tokens already cached
+    int B, head_num, kv_head_num, head_dim, max_blocks, page_size;
+    float log2_base;             // the plain Base rope: log2(base)
+};
 
-template <typename T, bool MULTI = false>
-__global__ void rope_append_kernel(const T* __restrict__ qkv, T* __restrict__ q_out, T* __restrict__ kv_pool,
-                                   const int32_t* __restrict__ page_list, const int32_t* __restrict__ seq_lens,
-                                   int head_num, int kv_head_num, int head_dim, int max_blocks, int tokens_per_block,
-                                   float log2_base, int q_len) {
-    rope_append_body<T, MULTI, false>(qkv, q_out, kv_pool, page_list, seq_lens, head_num, kv_head_num, head_dim, max_blocks,
-                                      tokens_per_block, log2_base, q_len, nullptr, nullptr, 0.f);
+// The cache slot of position pos of sequence b for head h of a qkv row, a k head (Hq <= h < Hq + Hkv) or a v head.
+template <typename T>
+__device__ __forceinline__ T* kv_slot(const RopeParams& p, int b, int h, int pos) {
+    const bool is_v = h >= p.head_num + p.kv_head_num;
+    const int kvh = is_v ? h - p.head_num - p.kv_head_num : h - p.head_num;
+    const int32_t page = p.page_list[((size_t)b * 2 + (is_v ? 1 : 0)) * p.max_blocks + pos / p.page_size];
+    const size_t page_elems = (size_t)p.kv_head_num * p.page_size * p.head_dim;
+    return reinterpret_cast<T*>(p.kv_pool) + (size_t)page * page_elems + ((size_t)kvh * p.page_size + pos % p.page_size) * p.head_dim;
 }
-
-// rope_append_kernel with QK-RMSNorm: q_gamma / k_gamma [head_dim], no bias.
-template <typename T, bool MULTI = false>
-__global__ void qk_norm_rope_append_kernel(const T* __restrict__ qkv, T* __restrict__ q_out, T* __restrict__ kv_pool,
-                                           const int32_t* __restrict__ page_list, const int32_t* __restrict__ seq_lens,
-                                           int head_num, int kv_head_num, int head_dim, int max_blocks, int tokens_per_block,
-                                           float log2_base, int q_len, const T* __restrict__ q_gamma,
-                                           const T* __restrict__ k_gamma, float eps) {
-    rope_append_body<T, MULTI, true>(qkv, q_out, kv_pool, page_list, seq_lens, head_num, kv_head_num, head_dim, max_blocks,
-                                     tokens_per_block, log2_base, q_len, q_gamma, k_gamma, eps);
-}
-
 
 // ---- the full decode RoPE contract of FusedRopeKVCacheDecodeOp (rtp_llm/ops/fused_rope_kvcache_op.py:202-246 ->
 // decode_fused_rope_kvcache; device code rtp_llm/models_py/bindings/common/kernels/rotary_position_embedding.h):
@@ -388,102 +331,94 @@ __device__ __forceinline__ float2 rope_coef(const RopeCfg& c, int zid, int pos) 
     return make_float2(sc * cs, sc * sn);
 }
 
-// q_len new tokens per sequence (MULTI, verification of speculative tokens): grid (B, Hq + 2*Hkv, q_len); row
-// x = b * q_len + j of qkv / q_out / position_ids is token j = blockIdx.z of sequence b, appended at slot seq_lens[b] + j and
-// rotated at position_ids[x] (when > 0) or that slot. q_len rides in gridDim.z so both instances share one parameter block.
-// Everything after the row / slot / position choice is the one-token arithmetic: token j gives the bits of a one-token call at
-// seq_lens + j.
-// QKN: q and k heads are RMS-normalised first (qk_norm_scale; no bias); the bits of b200_qk_rmsnorm followed by this kernel.
-template <typename T, bool MULTI, bool QKN>
-__device__ __forceinline__ void rope_append_ex_body(const T* __restrict__ qkv, const T* __restrict__ bias, T* __restrict__ q_out,
-                                                    T* __restrict__ kv_pool, const int32_t* __restrict__ page_list,
-                                                    const int32_t* __restrict__ seq_lens, const int32_t* __restrict__ position_ids,
-                                                    const float2* __restrict__ cos_sin_cache, int cache_positions, const RopeCfg& cfg,
-                                                    int use_logn, int head_num, int kv_head_num, int head_dim, int max_blocks,
-                                                    int tokens_per_block, const T* __restrict__ q_gamma,
-                                                    const T* __restrict__ k_gamma, float eps) {
+struct RopeAppendParams {
+    RopeParams r;                  // log2_base: PLAIN only
+    const void* bias;              // optional [(Hq + 2*Hkv) * D] qkv bias
+    const int32_t* position_ids;   // optional [B*q_len]
+    const float2* cos_sin_cache;   // optional [cache_positions][cfg.dim / 2] (cos, sin)
+    int cache_positions;
+    RopeCfg cfg;
+    int use_logn;
+    const void* q_gamma;           // QKN: [D] each
+    const void* k_gamma;
+    float eps;
+};
+
+// Decode RoPE (NeoX pairing) + K,V append into the paged cache, the one kernel of every rope + append entry point.
+// Contract: SURVEY.md appendix C; call site /root/reference/rtp_llm/ops/fused_rope_kvcache_op.py:202-246.
+// grid (B, Hq + 2*Hkv, q_len), D/2 threads. Row x = b * q_len + j of qkv / q_out / position_ids is token j = blockIdx.z of
+// sequence b, appended at slot seq_lens[b] + j and rotated at position_ids[x] (when > 0) or that slot. Everything after the
+// row / slot / position choice is the one-token arithmetic: token j gives the bits of a one-token call at seq_lens + j.
+// MULTI = false is the one-token instance (q_len == 1).
+// PLAIN: the plain Base rope (rope_base_cos_sin) over the whole head, v copied bit for bit; no table, position ids, bias or
+// logn (the host passes none). Otherwise the whole contract of cfg above.
+// QKN: q and k heads are RMS-normalised first (qk_norm_scale; no bias, it belongs to the qkv GEMM before the norm); the bits of
+// b200_qk_rmsnorm followed by this kernel.
+template <typename T, bool MULTI, bool QKN, bool PLAIN>
+__global__ void rope_append_kernel(const RopeAppendParams p) {
     pdl_launch_dependents();
+    const RopeParams& r = p.r;
+    const int b = blockIdx.x, h = blockIdx.y, i = threadIdx.x, half = r.head_dim / 2, rhalf = PLAIN ? half : p.cfg.dim / 2;
+    const bool is_q = h < r.head_num, is_v = h >= r.head_num + r.kv_head_num;
+    const bool norm = QKN && !is_v;   // q or k head (uniform over the CTA: the barrier inside qk_norm_scale is safe)
+    const T* gamma = reinterpret_cast<const T*>(is_q ? p.q_gamma : p.k_gamma);
+    T g0, g1;   // the gammas of the rotary pair are weights, constant after load, so they are read before the PDL wait
+    if (norm && i < rhalf) {
+        g0 = gamma[i];
+        g1 = gamma[i + rhalf];
+    }
     pdl_wait();
-    const int b = blockIdx.x, h = blockIdx.y, i = threadIdx.x, half = head_dim / 2, rhalf = cfg.dim / 2;
     const int x = MULTI ? b * (int)gridDim.z + (int)blockIdx.z : b;
-    const int slot = seq_lens[b] + (MULTI ? (int)blockIdx.z : 0);  // where K/V of the new token go (tokens already cached)
-    const int pos = (position_ids && position_ids[x] > 0) ? position_ids[x] : slot;
-    const T* src = qkv + ((size_t)x * (head_num + 2 * kv_head_num) + h) * head_dim;
-    const T* bsrc = bias ? bias + (size_t)h * head_dim : nullptr;
-    const size_t page_elems = (size_t)kv_head_num * tokens_per_block * head_dim;
-    T* dst;
-    bool rotate = cfg.style != 0, is_q = h < head_num;
-    if (is_q) {
-        dst = q_out + ((size_t)x * head_num + h) * head_dim;
-    } else {
-        const bool is_v = h >= head_num + kv_head_num;
-        const int kvh = is_v ? h - head_num - kv_head_num : h - head_num;
-        const int32_t page = page_list[((size_t)b * 2 + (is_v ? 1 : 0)) * max_blocks + slot / tokens_per_block];
-        dst = kv_pool + (size_t)page * page_elems + ((size_t)kvh * tokens_per_block + slot % tokens_per_block) * head_dim;
-        rotate = rotate && !is_v;
+    const int slot = r.seq_lens[b] + (MULTI ? (int)blockIdx.z : 0);   // where K/V of the new token go (tokens already cached)
+    const int pos = (!PLAIN && p.position_ids && p.position_ids[x] > 0) ? p.position_ids[x] : slot;
+    const T* src = reinterpret_cast<const T*>(r.qkv) + ((size_t)x * (r.head_num + 2 * r.kv_head_num) + h) * r.head_dim;
+    T* dst = is_q ? reinterpret_cast<T*>(r.q_out) + ((size_t)x * r.head_num + h) * r.head_dim : kv_slot<T>(r, b, h, slot);
+    if (PLAIN && is_v) {
+        dst[i] = src[i];
+        dst[i + half] = src[i + half];
+        return;
     }
-    // thread i owns the channel pair (i, i + dim/2) for i < dim/2, and the pass-through channels dim + i, dim + i + (head_dim-dim)/2 ...
+    const T* bias = (PLAIN || !p.bias) ? nullptr : reinterpret_cast<const T*>(p.bias) + (size_t)h * r.head_dim;
+    const bool rotate = PLAIN || (p.cfg.style != 0 && !is_v);
+    float2 cf;   // (cos, sin) of the rotary pair, before the QK-norm (its latency overlaps the norm's reduction)
+    if (rotate && i < rhalf) {
+        if constexpr (PLAIN)
+            cf = rope_base_cos_sin(i, r.head_dim, r.log2_base, pos);
+        else
+            cf = (p.cos_sin_cache && pos < p.cache_positions) ? p.cos_sin_cache[(size_t)pos * rhalf + i] : rope_coef(p.cfg, 2 * i, pos);
+    }
     float scale = 0.f;
-    const T* gamma = is_q ? q_gamma : k_gamma;
-    const bool norm = QKN && !(h >= head_num + kv_head_num);   // q or k head (uniform over the CTA: the barrier inside is safe)
     if constexpr (QKN) {
-        if (norm) scale = qk_norm_scale<T>(src, head_dim, eps);
+        if (norm) scale = qk_norm_scale<T>(src, r.head_dim, p.eps);
     }
-    auto load = [&](int c) {
+    auto load = [&](int c, T g) {   // channel c as the rotation takes it: QK-normed, or with the bias added in T
         if constexpr (QKN) {
-            if (norm) return qk_norm_apply<T>(src[c], scale, gamma[c]);
+            if (norm) return qk_norm_apply<T>(src[c], scale, g);
         }
         float v = to_f32<T>(src[c]);
-        if (bsrc) v = to_f32<T>(from_f32<T>(v + to_f32<T>(bsrc[c])));
+        if (bias) v = to_f32<T>(from_f32<T>(v + to_f32<T>(bias[c])));
         return v;
     };
+    const bool logn = !PLAIN && is_q && p.use_logn && pos > p.cfg.max_pos;
+    // thread i owns the channel pair (i, i + dim/2) for i < dim/2, and the pass-through channels dim + i, dim + i + D/2 ...
     if (i < rhalf) {
-        float x0 = load(i), x1 = load(i + rhalf);
-        if (rotate) {
-            const float2 cf = (cos_sin_cache && pos < cache_positions) ? cos_sin_cache[(size_t)pos * rhalf + i] : rope_coef(cfg, 2 * i, pos);
-            float r0, r1;
-            rope_rotate(x0, x1, cf.x, cf.y, r0, r1);
-            x0 = r0;
-            x1 = r1;
-        }
-        if (is_q && use_logn && pos > cfg.max_pos) {
-            const float logn = logf((float)(pos + 1)) / logf((float)cfg.max_pos);
-            x0 *= logn;
-            x1 *= logn;
+        float x0 = load(i, g0), x1 = load(i + rhalf, g1);
+        if (rotate) rope_rotate(x0, x1, cf.x, cf.y, x0, x1);
+        if (logn) {
+            const float s = logf((float)(pos + 1)) / logf((float)p.cfg.max_pos);
+            x0 *= s;
+            x1 *= s;
         }
         dst[i] = from_f32<T>(x0);
         dst[i + rhalf] = from_f32<T>(x1);
     }
-    for (int c = cfg.dim + i; c < head_dim; c += half) {            // channels beyond the rotary dim
-        float v = load(c);
-        if (is_q && use_logn && pos > cfg.max_pos) v *= logf((float)(pos + 1)) / logf((float)cfg.max_pos);
-        dst[c] = from_f32<T>(v);
+    if constexpr (!PLAIN) {
+        for (int c = p.cfg.dim + i; c < r.head_dim; c += half) {   // channels beyond the rotary dim
+            float v = load(c, norm ? gamma[c] : T());
+            if (logn) v *= logf((float)(pos + 1)) / logf((float)p.cfg.max_pos);
+            dst[c] = from_f32<T>(v);
+        }
     }
-}
-
-template <typename T, bool MULTI = false>
-__global__ void rope_append_ex_kernel(const T* __restrict__ qkv, const T* __restrict__ bias, T* __restrict__ q_out,
-                                      T* __restrict__ kv_pool, const int32_t* __restrict__ page_list,
-                                      const int32_t* __restrict__ seq_lens, const int32_t* __restrict__ position_ids,
-                                      const float2* __restrict__ cos_sin_cache, int cache_positions, RopeCfg cfg, int use_logn,
-                                      int head_num, int kv_head_num, int head_dim, int max_blocks, int tokens_per_block) {
-    rope_append_ex_body<T, MULTI, false>(qkv, bias, q_out, kv_pool, page_list, seq_lens, position_ids, cos_sin_cache,
-                                         cache_positions, cfg, use_logn, head_num, kv_head_num, head_dim, max_blocks,
-                                         tokens_per_block, nullptr, nullptr, 0.f);
-}
-
-// rope_append_ex_kernel with QK-RMSNorm: q_gamma / k_gamma [head_dim]; qkv carries no bias (it belongs to the qkv GEMM, before
-// the norm).
-template <typename T, bool MULTI = false>
-__global__ void qk_norm_rope_append_ex_kernel(const T* __restrict__ qkv, T* __restrict__ q_out, T* __restrict__ kv_pool,
-                                              const int32_t* __restrict__ page_list, const int32_t* __restrict__ seq_lens,
-                                              const int32_t* __restrict__ position_ids, const float2* __restrict__ cos_sin_cache,
-                                              int cache_positions, RopeCfg cfg, int use_logn, int head_num, int kv_head_num,
-                                              int head_dim, int max_blocks, int tokens_per_block, const T* __restrict__ q_gamma,
-                                              const T* __restrict__ k_gamma, float eps) {
-    rope_append_ex_body<T, MULTI, true>(qkv, nullptr, q_out, kv_pool, page_list, seq_lens, position_ids, cos_sin_cache,
-                                        cache_positions, cfg, use_logn, head_num, kv_head_num, head_dim, max_blocks,
-                                        tokens_per_block, q_gamma, k_gamma, eps);
 }
 
 // Column gather y[r][j] = x[r][perm[j]] (the activation side of a GPTQ act-order weight whose rows were sorted by g_idx).

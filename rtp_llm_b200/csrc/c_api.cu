@@ -826,48 +826,51 @@ int b200_permute_cols(const void* x, const int32_t* perm, void* y, int is_bf16, 
     });
 }
 
-// q_gamma / k_gamma non-null: QK-RMSNorm first (qk_norm_rope_append_kernel), always its own launch inside a decode program.
-static int rope_append_impl(const void* qkv, void* q_out, void* kv_pool, const int32_t* page_list, const int32_t* sequence_lengths,
-                            int is_bf16, int batch, int q_len, int head_num, int kv_head_num, int head_dim, int max_blocks_per_seq,
-                            int page_size, float rope_base, const void* q_gamma, const void* k_gamma, float eps, void* stream) {
-    if (batch == 0) return B200_OK;
-    ARG_CHECK(qkv && q_out && kv_pool && page_list && sequence_lengths, "rope_append: null pointer");
-    ARG_CHECK(head_dim > 0 && head_dim % 2 == 0 && head_dim <= 512, "rope_append: head_dim %d unsupported", head_dim);
-    ARG_CHECK(rope_base > 1.f, "rope_append: rope_base must be > 1");
-    ARG_CHECK(batch > 0 && q_len >= 1 && (long)batch * q_len <= 0x7fffffffL, "rope_append: bad shape batch %d x q_len %d", batch, q_len);
-    const bool qkn = q_gamma != nullptr;
-    const float l2b = std::log2(rope_base);
-    if (g_rec && q_len == 1 && !qkn) {   // the persistent kernel's rope op appends one token per sequence, unnormed
+// The one host path of the six rope + append entry points (rope_append_kernel). plain: the plain Base rope at rope_base (no
+// position ids, table, bias or logn); else the whole rope contract of *cfg. qkn: QK-RMSNorm first with p.q_gamma / p.k_gamma.
+// Inside a decode program the plain one-token rope without QK-norm is the persistent kernel's rope op; every other mode is its
+// own launch there.
+static int rope_append_impl(const char* what, RopeAppendParams p, bool plain, float rope_base, const b200_rope_config* cfg, bool qkn,
+                            int is_bf16, int q_len, void* stream) {
+    RopeParams& r = p.r;
+    ARG_CHECK(q_len >= 1, "%s: q_len %d must be >= 1", what, q_len);
+    if (qkn) {
+        ARG_CHECK(p.q_gamma && p.k_gamma, "%s: null gamma", what);
+        ARG_CHECK(r.head_dim % 64 == 0 && r.head_dim <= kQkNormMaxD, "%s: head_dim %d must be 64, 128 or 256", what, r.head_dim);
+    }
+    if (r.B == 0) return B200_OK;
+    ARG_CHECK(r.qkv && r.q_out && r.kv_pool && r.page_list && r.seq_lens && (plain || cfg), "%s: null pointer", what);
+    ARG_CHECK(r.head_dim > 0 && r.head_dim % 2 == 0 && r.head_dim <= 512, "%s: head_dim %d unsupported", what, r.head_dim);
+    ARG_CHECK(r.B > 0 && q_len <= 65535 && (long)r.B * q_len <= 0x7fffffffL, "%s: bad shape batch %d x q_len %d", what, r.B, q_len);
+    if (plain) {
+        ARG_CHECK(rope_base > 1.f, "%s: rope_base must be > 1", what);
+        r.log2_base = std::log2(rope_base);
+    } else {
+        ARG_CHECK(cfg->style == 0 || (cfg->style >= 1 && cfg->style <= 7 && cfg->style != 2), "%s: rope style %d unsupported (Glm2 is out of scope)", what, cfg->style);
+        ARG_CHECK(cfg->dim > 0 && cfg->dim % 2 == 0 && cfg->dim <= r.head_dim, "%s: rotary dim %d must be even and <= head_dim", what, cfg->dim);
+        ARG_CHECK(cfg->style == 0 || cfg->base > 1.f, "%s: rope base must be > 1", what);
+        ARG_CHECK(!p.cos_sin_cache || p.cache_positions > 0, "%s: a cos/sin cache needs its number of positions", what);
+        ARG_CHECK(!p.use_logn || cfg->max_pos > 1, "%s: logn attention needs max_pos > 1", what);
+        p.cfg = {cfg->style, cfg->dim, cfg->base, cfg->scale, cfg->factor1, cfg->factor2, cfg->max_pos, cfg->extrapolation_factor, cfg->mscale};
+    }
+    if (g_rec && plain && q_len == 1 && !qkn) {   // the persistent kernel's rope op appends one token per sequence, unnormed
         ProgOp op{};
         op.type = kOpRope;
-        op.r.qkv = qkv;
-        op.r.q_out = q_out;
-        op.r.kv_pool = kv_pool;
-        op.r.page_list = page_list;
-        op.r.seq_lens = sequence_lengths;
-        op.r.B = batch;
-        op.r.head_num = head_num;
-        op.r.kv_head_num = kv_head_num;
-        op.r.head_dim = head_dim;
-        op.r.max_blocks = max_blocks_per_seq;
-        op.r.page_size = page_size;
-        op.r.log2_base = l2b;
+        op.r = r;
         return rec_segment_op(op, is_bf16 ? 1 : 0, -1, -1);
     }
-    const dim3 grid(batch * q_len, head_num + 2 * kv_head_num);
+    const dim3 grid(r.B, r.head_num + 2 * r.kv_head_num, q_len), block(r.head_dim / 2);
     return by_dtype(is_bf16, [&](auto t) {
         using T = decltype(t);
-        if (qkn)
-            return launch_or_record("qk_norm_rope_append_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
-                return launch_ex(q_len > 1 ? qk_norm_rope_append_kernel<T, true> : qk_norm_rope_append_kernel<T, false>,
-                                 {grid, dim3(head_dim / 2), 0, s, pdl}, (const T*)qkv, (T*)q_out, (T*)kv_pool, page_list,
-                                 sequence_lengths, head_num, kv_head_num, head_dim, (int)max_blocks_per_seq, page_size, l2b, q_len,
-                                 (const T*)q_gamma, (const T*)k_gamma, eps);
-            });
+        using Kernel = void (*)(RopeAppendParams);
+        const Kernel kernels[2][2][2] = {   // [MULTI][QKN][PLAIN]
+            {{rope_append_kernel<T, false, false, false>, rope_append_kernel<T, false, false, true>},
+             {rope_append_kernel<T, false, true, false>, rope_append_kernel<T, false, true, true>}},
+            {{rope_append_kernel<T, true, false, false>, rope_append_kernel<T, true, false, true>},
+             {rope_append_kernel<T, true, true, false>, rope_append_kernel<T, true, true, true>}}};
+        const Kernel kern = kernels[q_len > 1][qkn][plain];
         return launch_or_record("rope_append_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
-            return launch_ex(q_len > 1 ? rope_append_kernel<T, true> : rope_append_kernel<T, false>, {grid, dim3(head_dim / 2), 0, s, pdl},
-                             (const T*)qkv, (T*)q_out, (T*)kv_pool, page_list, sequence_lengths, head_num, kv_head_num, head_dim,
-                             (int)max_blocks_per_seq, page_size, l2b, q_len);
+            return launch_ex(kern, {grid, block, 0, s, pdl}, p);
         });
     });
 }
@@ -875,73 +878,35 @@ static int rope_append_impl(const void* qkv, void* q_out, void* kv_pool, const i
 int b200_rope_append(const void* qkv, void* q_out, void* kv_pool, const int32_t* page_list,
                      const int32_t* sequence_lengths, int is_bf16, int batch, int head_num, int kv_head_num,
                      int head_dim, int max_blocks_per_seq, int page_size, float rope_base, void* stream) {
-    return rope_append_impl(qkv, q_out, kv_pool, page_list, sequence_lengths, is_bf16, batch, 1, head_num, kv_head_num, head_dim,
-                            max_blocks_per_seq, page_size, rope_base, nullptr, nullptr, 0.f, stream);
+    return b200_rope_append_multi(qkv, q_out, kv_pool, page_list, sequence_lengths, is_bf16, batch, head_num, kv_head_num, head_dim,
+                                  max_blocks_per_seq, page_size, rope_base, 1, stream);
 }
 
 int b200_rope_append_multi(const void* qkv, void* q_out, void* kv_pool, const int32_t* page_list,
                            const int32_t* sequence_lengths, int is_bf16, int batch, int head_num, int kv_head_num,
                            int head_dim, int max_blocks_per_seq, int page_size, float rope_base, int q_len, void* stream) {
-    ARG_CHECK(q_len >= 1, "rope_append_multi: q_len %d must be >= 1", q_len);
-    return rope_append_impl(qkv, q_out, kv_pool, page_list, sequence_lengths, is_bf16, batch, q_len, head_num, kv_head_num, head_dim,
-                            max_blocks_per_seq, page_size, rope_base, nullptr, nullptr, 0.f, stream);
+    const RopeAppendParams p{{qkv, q_out, kv_pool, page_list, sequence_lengths, batch, head_num, kv_head_num, head_dim, max_blocks_per_seq, page_size}};
+    return rope_append_impl("rope_append", p, true, rope_base, nullptr, false, is_bf16, q_len, stream);
 }
 
 int b200_qk_norm_rope_append(const void* qkv, const void* q_gamma, const void* k_gamma, float eps, void* q_out, void* kv_pool,
                              const int32_t* page_list, const int32_t* sequence_lengths, int is_bf16, int batch, int head_num,
                              int kv_head_num, int head_dim, int max_blocks_per_seq, int page_size, float rope_base, int q_len,
                              void* stream) {
-    ARG_CHECK(q_gamma && k_gamma, "qk_norm_rope_append: null gamma");
-    ARG_CHECK(head_dim % 64 == 0 && head_dim <= kQkNormMaxD, "qk_norm_rope_append: head_dim %d must be 64, 128 or 256", head_dim);
-    ARG_CHECK(q_len >= 1, "qk_norm_rope_append: q_len %d must be >= 1", q_len);
-    return rope_append_impl(qkv, q_out, kv_pool, page_list, sequence_lengths, is_bf16, batch, q_len, head_num, kv_head_num, head_dim,
-                            max_blocks_per_seq, page_size, rope_base, q_gamma, k_gamma, eps, stream);
-}
-
-// q_gamma / k_gamma non-null (qkv_bias null): QK-RMSNorm first (qk_norm_rope_append_ex_kernel).
-static int rope_append_ex_impl(const void* qkv, const void* qkv_bias, void* q_out, void* kv_pool, const int32_t* page_list,
-                               const int32_t* sequence_lengths, const int32_t* position_ids, const float* cos_sin_cache,
-                               int cache_positions, const b200_rope_config* cfg, int use_logn_attn, int is_bf16, int batch,
-                               int q_len, int head_num, int kv_head_num, int head_dim, int max_blocks_per_seq, int page_size,
-                               const void* q_gamma, const void* k_gamma, float eps, void* stream) {
-    if (batch == 0) return B200_OK;
-    ARG_CHECK(qkv && q_out && kv_pool && page_list && sequence_lengths && cfg, "rope_append_ex: null pointer");
-    ARG_CHECK(head_dim > 0 && head_dim % 2 == 0 && head_dim <= 512, "rope_append_ex: head_dim %d unsupported", head_dim);
-    ARG_CHECK(cfg->style == 0 || (cfg->style >= 1 && cfg->style <= 7 && cfg->style != 2), "rope_append_ex: rope style %d unsupported (Glm2 is out of scope)", cfg->style);
-    ARG_CHECK(cfg->dim > 0 && cfg->dim % 2 == 0 && cfg->dim <= head_dim, "rope_append_ex: rotary dim %d must be even and <= head_dim", cfg->dim);
-    ARG_CHECK(cfg->style == 0 || cfg->base > 1.f, "rope_append_ex: rope base must be > 1");
-    ARG_CHECK(!cos_sin_cache || cache_positions > 0, "rope_append_ex: a cos/sin cache needs its number of positions");
-    ARG_CHECK(!use_logn_attn || cfg->max_pos > 1, "rope_append_ex: logn attention needs max_pos > 1");
-    ARG_CHECK(batch > 0 && q_len >= 1 && q_len <= 65535, "rope_append_ex: bad shape batch %d x q_len %d", batch, q_len);
-    const RopeCfg rc{cfg->style, cfg->dim, cfg->base, cfg->scale, cfg->factor1, cfg->factor2, cfg->max_pos, cfg->extrapolation_factor,
-                     cfg->mscale};
-    const dim3 grid(batch, head_num + 2 * kv_head_num, q_len);
-    const float2* cache = reinterpret_cast<const float2*>(cos_sin_cache);
-    return by_dtype(is_bf16, [&](auto t) {
-        using T = decltype(t);
-        if (q_gamma)
-            return launch_or_record("qk_norm_rope_append_ex_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
-                return launch_ex(q_len > 1 ? qk_norm_rope_append_ex_kernel<T, true> : qk_norm_rope_append_ex_kernel<T, false>,
-                                 {grid, dim3(head_dim / 2), 0, s, pdl}, (const T*)qkv, (T*)q_out, (T*)kv_pool, page_list,
-                                 sequence_lengths, position_ids, cache, cache_positions, rc, use_logn_attn, head_num, kv_head_num,
-                                 head_dim, max_blocks_per_seq, page_size, (const T*)q_gamma, (const T*)k_gamma, eps);
-            });
-        return launch_or_record("rope_append_ex_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
-            return launch_ex(q_len > 1 ? rope_append_ex_kernel<T, true> : rope_append_ex_kernel<T, false>,
-                             {grid, dim3(head_dim / 2), 0, s, pdl}, (const T*)qkv, (const T*)qkv_bias, (T*)q_out, (T*)kv_pool, page_list,
-                             sequence_lengths, position_ids, cache, cache_positions, rc, use_logn_attn, head_num, kv_head_num, head_dim,
-                             max_blocks_per_seq, page_size);
-        });
-    });
+    RopeAppendParams p{{qkv, q_out, kv_pool, page_list, sequence_lengths, batch, head_num, kv_head_num, head_dim, max_blocks_per_seq, page_size}};
+    p.q_gamma = q_gamma;
+    p.k_gamma = k_gamma;
+    p.eps = eps;
+    return rope_append_impl("qk_norm_rope_append", p, true, rope_base, nullptr, true, is_bf16, q_len, stream);
 }
 
 int b200_rope_append_ex(const void* qkv, const void* qkv_bias, void* q_out, void* kv_pool, const int32_t* page_list,
                         const int32_t* sequence_lengths, const int32_t* position_ids, const float* cos_sin_cache,
                         int cache_positions, const b200_rope_config* cfg, int use_logn_attn, int is_bf16, int batch, int head_num,
                         int kv_head_num, int head_dim, int max_blocks_per_seq, int page_size, void* stream) {
-    return rope_append_ex_impl(qkv, qkv_bias, q_out, kv_pool, page_list, sequence_lengths, position_ids, cos_sin_cache,
-                               cache_positions, cfg, use_logn_attn, is_bf16, batch, 1, head_num, kv_head_num, head_dim,
-                               max_blocks_per_seq, page_size, nullptr, nullptr, 0.f, stream);
+    return b200_rope_append_ex_multi(qkv, qkv_bias, q_out, kv_pool, page_list, sequence_lengths, position_ids, cos_sin_cache,
+                                     cache_positions, cfg, use_logn_attn, is_bf16, batch, head_num, kv_head_num, head_dim,
+                                     max_blocks_per_seq, page_size, 1, stream);
 }
 
 int b200_rope_append_ex_multi(const void* qkv, const void* qkv_bias, void* q_out, void* kv_pool, const int32_t* page_list,
@@ -949,10 +914,9 @@ int b200_rope_append_ex_multi(const void* qkv, const void* qkv_bias, void* q_out
                               int cache_positions, const b200_rope_config* cfg, int use_logn_attn, int is_bf16, int batch,
                               int head_num, int kv_head_num, int head_dim, int max_blocks_per_seq, int page_size, int q_len,
                               void* stream) {
-    ARG_CHECK(q_len >= 1, "rope_append_ex_multi: q_len %d must be >= 1", q_len);
-    return rope_append_ex_impl(qkv, qkv_bias, q_out, kv_pool, page_list, sequence_lengths, position_ids, cos_sin_cache,
-                               cache_positions, cfg, use_logn_attn, is_bf16, batch, q_len, head_num, kv_head_num, head_dim,
-                               max_blocks_per_seq, page_size, nullptr, nullptr, 0.f, stream);
+    const RopeAppendParams p{{qkv, q_out, kv_pool, page_list, sequence_lengths, batch, head_num, kv_head_num, head_dim, max_blocks_per_seq, page_size},
+                             qkv_bias, position_ids, reinterpret_cast<const float2*>(cos_sin_cache), cache_positions, {}, use_logn_attn};
+    return rope_append_impl("rope_append_ex", p, false, 0.f, cfg, false, is_bf16, q_len, stream);
 }
 
 int b200_qk_norm_rope_append_ex(const void* qkv, const void* q_gamma, const void* k_gamma, float eps, void* q_out, void* kv_pool,
@@ -960,12 +924,10 @@ int b200_qk_norm_rope_append_ex(const void* qkv, const void* q_gamma, const void
                                 const float* cos_sin_cache, int cache_positions, const b200_rope_config* cfg, int use_logn_attn,
                                 int is_bf16, int batch, int head_num, int kv_head_num, int head_dim, int max_blocks_per_seq,
                                 int page_size, int q_len, void* stream) {
-    ARG_CHECK(q_gamma && k_gamma, "qk_norm_rope_append_ex: null gamma");
-    ARG_CHECK(head_dim % 64 == 0 && head_dim <= kQkNormMaxD, "qk_norm_rope_append_ex: head_dim %d must be 64, 128 or 256", head_dim);
-    ARG_CHECK(q_len >= 1, "qk_norm_rope_append_ex: q_len %d must be >= 1", q_len);
-    return rope_append_ex_impl(qkv, nullptr, q_out, kv_pool, page_list, sequence_lengths, position_ids, cos_sin_cache,
-                               cache_positions, cfg, use_logn_attn, is_bf16, batch, q_len, head_num, kv_head_num, head_dim,
-                               max_blocks_per_seq, page_size, q_gamma, k_gamma, eps, stream);
+    const RopeAppendParams p{{qkv, q_out, kv_pool, page_list, sequence_lengths, batch, head_num, kv_head_num, head_dim, max_blocks_per_seq, page_size},
+                             nullptr, position_ids, reinterpret_cast<const float2*>(cos_sin_cache), cache_positions, {}, use_logn_attn,
+                             q_gamma, k_gamma, eps};
+    return rope_append_impl("qk_norm_rope_append_ex", p, false, 0.f, cfg, true, is_bf16, q_len, stream);
 }
 
 int b200_embedding(const int32_t* ids, const void* table, void* out, int is_bf16, int rows, int hidden, void* stream) {

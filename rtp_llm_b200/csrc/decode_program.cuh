@@ -57,16 +57,6 @@ struct NormParams {
     float eps;
 };
 
-struct RopeParams {
-    const void* qkv;
-    void* q_out;
-    void* kv_pool;
-    const int32_t* page_list;
-    const int32_t* seq_lens;
-    int B, head_num, kv_head_num, head_dim, max_blocks, page_size;
-    float log2_base;
-};
-
 struct EmbedParams {
     const int32_t* ids;
     const void* table;
@@ -464,37 +454,23 @@ __device__ __forceinline__ void seg_norm(const NormParams& p, const SM& sm, int 
     }
 }
 
-// RoPE (NeoX pairing, RopeStyle::Base) + K/V append, same math as rope_append_kernel (aux_kernels.cuh); flattened over
-// (sequence, head, channel pair) so all CTAs share the work.
+// RoPE (NeoX pairing, RopeStyle::Base) + K/V append, the math of rope_append_kernel's PLAIN mode (aux_kernels.cuh); flattened
+// over (sequence, head, channel pair) so all CTAs share the work.
 template <typename T>
 __device__ __forceinline__ void seg_rope(const RopeParams& p, int cta, int nctas) {
     const int half = p.head_dim / 2, heads = p.head_num + 2 * p.kv_head_num;
     const int total = p.B * heads * half;
-    const size_t page_elems = (size_t)p.kv_head_num * p.page_size * p.head_dim;
     const T* qkv = reinterpret_cast<const T*>(p.qkv);
     for (int idx = cta * kSegDqThreads + threadIdx.x; idx < total; idx += nctas * kSegDqThreads) {
         const int i = idx % half, h = (idx / half) % heads, b = idx / (half * heads);
         const int pos = p.seq_lens[b];
         const T* src = qkv + ((size_t)b * heads + h) * p.head_dim;
-        T* dst;
-        bool rotate = true;
-        if (h < p.head_num) {
-            dst = reinterpret_cast<T*>(p.q_out) + ((size_t)b * p.head_num + h) * p.head_dim;
-        } else {
-            const bool is_v = h >= p.head_num + p.kv_head_num;
-            const int kvh = is_v ? h - p.head_num - p.kv_head_num : h - p.head_num;
-            const int32_t page = p.page_list[((size_t)b * 2 + (is_v ? 1 : 0)) * p.max_blocks + pos / p.page_size];
-            dst = reinterpret_cast<T*>(p.kv_pool) + (size_t)page * page_elems +
-                  ((size_t)kvh * p.page_size + pos % p.page_size) * p.head_dim;
-            rotate = !is_v;
-        }
+        T* dst = h < p.head_num ? reinterpret_cast<T*>(p.q_out) + ((size_t)b * p.head_num + h) * p.head_dim : kv_slot<T>(p, b, h, pos);
         const float x0 = to_f32<T>(__ldcg(src + i)), x1 = to_f32<T>(__ldcg(src + i + half));
-        if (rotate) {
-            const float inv_freq = exp2f(-2.0f * (float)i / (float)p.head_dim * p.log2_base);
-            float sn, cs;
-            sincosf((float)pos * inv_freq, &sn, &cs);
+        if (h < p.head_num + p.kv_head_num) {   // q or k head: rotated
+            const float2 cf = rope_base_cos_sin(i, p.head_dim, p.log2_base, pos);
             float r0, r1;
-            rope_rotate(x0, x1, cs, sn, r0, r1);
+            rope_rotate(x0, x1, cf.x, cf.y, r0, r1);
             dst[i] = from_f32<T>(r0);
             dst[i + half] = from_f32<T>(r1);
         } else {

@@ -245,11 +245,9 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const std::
             for (int j = 0; j < 2; ++j) {
                 const int i = lane + 32 * j;                        // channel pair (i, i + 64)
                 const float x0 = to_f32<T>(ksrc[i]), x1 = to_f32<T>(ksrc[i + 64]);
-                const float inv_freq = exp2f(-2.0f * (float)i / (float)kAttnD * p.log2_base);
-                float sn, cs;
-                sincosf((float)pos * inv_freq, &sn, &cs);
+                const float2 cf = rope_base_cos_sin(i, kAttnD, p.log2_base, pos);
                 float r0, r1;
-                rope_rotate(x0, x1, cs, sn, r0, r1);
+                rope_rotate(x0, x1, cf.x, cf.y, r0, r1);
                 kdst[i] = from_f32<T>(r0);
                 kdst[i + 64] = from_f32<T>(r1);
                 vdst[i] = vsrc[i];
@@ -285,12 +283,8 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const std::
         const T* qbase = reinterpret_cast<const T*>(p.qkv) + ((size_t)b * (p.Hq + 2 * p.Hkv) + (size_t)kvh * p.group) * kAttnD;
         const bool v0 = qrow < p.group, v1 = (qrow + 8) < p.group;
         const int pos = p.seq_lens[b];
-        if (threadIdx.x < 64) {                              // one sincosf per channel pair and CTA, shared through smem
-            const float inv_freq = exp2f(-2.0f * (float)threadIdx.x / (float)kAttnD * p.log2_base);
-            float sn, cs;
-            sincosf((float)pos * inv_freq, &sn, &cs);
-            cs_tab[threadIdx.x] = make_float2(cs, sn);
-        }
+        if (threadIdx.x < 64)                                // one sincosf per channel pair and CTA, shared through smem
+            cs_tab[threadIdx.x] = rope_base_cos_sin(threadIdx.x, kAttnD, p.log2_base, pos);
         asm volatile("bar.sync 1, 128;" ::: "memory");
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk) {

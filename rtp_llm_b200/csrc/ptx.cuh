@@ -225,11 +225,21 @@ template <>
 __device__ __forceinline__ float from_f32<float>(float v) { return v; }
 
 // The rotation of one RoPE channel pair with the rounding sequence PINNED (explicit mul / fma intrinsics): every kernel that
-// rotates (rope_append, rope_append_ex, the persistent kernel's rope op, the attention kernel's fused rope) produces the same
-// bits whatever the compiler would otherwise contract.
+// rotates (rope_append_kernel in every mode, the persistent kernel's rope op, the attention kernel's fused rope) produces the
+// same bits whatever the compiler would otherwise contract.
 __device__ __forceinline__ void rope_rotate(float x0, float x1, float cs, float sn, float& r0, float& r1) {
     r0 = __fmaf_rn(x0, cs, -__fmul_rn(x1, sn));
     r1 = __fmaf_rn(x1, cs, __fmul_rn(x0, sn));
+}
+
+// (cos, sin) of the plain Base RoPE angle pos * base^(-2i/head_dim) of channel pair i, base given as log2(base). The one
+// expression of that angle: rope_append_kernel's PLAIN mode, the persistent kernel's rope op and the attention kernel's fused
+// rope must give the same bits, so none of them restates it.
+__device__ __forceinline__ float2 rope_base_cos_sin(int i, int head_dim, float log2_base, int pos) {
+    const float inv_freq = exp2f(-2.0f * (float)i / (float)head_dim * log2_base);
+    float sn, cs;
+    sincosf((float)pos * inv_freq, &sn, &cs);
+    return make_float2(cs, sn);
 }
 
 __device__ __forceinline__ float fast_exp2(float x) {

@@ -381,25 +381,41 @@ def silu_and_mul(gate_up, out=None):
     return out
 
 
-def rope_append(qkv, kv_cache_base, page_list, sequence_lengths, head_num, rope_base, q_out=None, q_len: int = 1):
-    """qkv [B*q_len, (Hq+2Hkv)*D]: q_len new tokens per sequence (row b*q_len + j = token j of sequence b, rotated and
-    appended at sequence_lengths[b] + j). Returns q [B*q_len, Hq*D]."""
-    _cuda_contig(qkv, kv_cache_base, page_list, sequence_lengths, q_out)
+def _rope_args(what, qkv, kv_cache_base, page_list, sequence_lengths, head_num, q_out, q_len, qk_norm=None, bias=None,
+               rope_cfg=None, position_ids=None, cos_sin_cache=None, use_logn_attn=False):
+    """Checks and C arguments shared by the four rope + append ops: (q_out, (q_out, pool, page list, sequence lengths),
+    the _ex entries' (position ids, table, table positions, config, logn), (dtype, B, Hq, Hkv, D, max blocks, page size)).
+    qk_norm: (q_gamma, k_gamma), each a [D] tensor of qkv's dtype."""
+    _cuda_contig(qkv, kv_cache_base, page_list, sequence_lengths, q_out, bias, position_ids, cos_sin_cache, *(qk_norm or ()))
     P, two, Hkv, T, D = kv_cache_base.shape
     rows = qkv.shape[0]
     if q_len < 1 or rows % q_len:
-        raise B200Error(f"rope_append: {rows} qkv rows are not a multiple of q_len {q_len}")
+        raise B200Error(f"{what}: {rows} qkv rows are not a multiple of q_len {q_len}")
+    if position_ids is not None and position_ids.numel() != rows:
+        raise B200Error(f"{what}: {position_ids.numel()} position ids for {rows} qkv rows")
+    for name, g in zip(("q_gamma", "k_gamma"), qk_norm or ()):
+        if g is None or g.dtype != qkv.dtype or g.numel() != D:
+            raise B200Error(f"{what}: {name} must be a [{D}] tensor of qkv's dtype {qkv.dtype}")
     if q_out is None:
         q_out = torch.empty((rows, head_num * D), dtype=qkv.dtype, device=qkv.device)
+    ex = ()
+    if rope_cfg is not None:
+        import ctypes
+        ex = (_p(position_ids), _p(cos_sin_cache), cos_sin_cache.shape[0] if cos_sin_cache is not None else 0,
+              ctypes.cast(ctypes.pointer(rope_cfg), ctypes.c_void_p), 1 if use_logn_attn else 0)
+    return (q_out, (_p(q_out), _p(kv_cache_base), _p(page_list), _p(sequence_lengths)), ex,
+            (_is_bf16(qkv), rows // q_len, head_num, Hkv, D, page_list.shape[-1], T))
+
+
+def rope_append(qkv, kv_cache_base, page_list, sequence_lengths, head_num, rope_base, q_out=None, q_len: int = 1):
+    """qkv [B*q_len, (Hq+2Hkv)*D]: q_len new tokens per sequence (row b*q_len + j = token j of sequence b, rotated and
+    appended at sequence_lengths[b] + j). Returns q [B*q_len, Hq*D]."""
+    q_out, io, _, shape = _rope_args("rope_append", qkv, kv_cache_base, page_list, sequence_lengths, head_num, q_out, q_len)
     lib = _lib.load()
     if q_len == 1:
-        check(lib.b200_rope_append(_p(qkv), _p(q_out), _p(kv_cache_base), _p(page_list), _p(sequence_lengths),
-                                   _is_bf16(qkv), rows, head_num, Hkv, D, page_list.shape[-1], T, rope_base, _stream()),
-              "b200_rope_append")
+        check(lib.b200_rope_append(_p(qkv), *io, *shape, rope_base, _stream()), "b200_rope_append")
     else:
-        check(lib.b200_rope_append_multi(_p(qkv), _p(q_out), _p(kv_cache_base), _p(page_list), _p(sequence_lengths),
-                                         _is_bf16(qkv), rows // q_len, head_num, Hkv, D, page_list.shape[-1], T, rope_base, q_len,
-                                         _stream()), "b200_rope_append_multi")
+        check(lib.b200_rope_append_multi(_p(qkv), *io, *shape, rope_base, q_len, _stream()), "b200_rope_append_multi")
     return q_out
 
 
@@ -409,36 +425,15 @@ def rope_append_ex(qkv, kv_cache_base, page_list, sequence_lengths, head_num, ro
     logn): see b200_rope_append_ex in include/b200_decode_ops.h. cos_sin_cache: fp32 [positions, dim] interleaved (cos, sin).
     q_len > 1: qkv [B*q_len, ...] holds q_len new tokens per sequence (row b*q_len + j = token j of sequence b, appended at
     sequence_lengths[b] + j) and position_ids, when given, has one entry per row. Returns q [B*q_len, Hq*D]."""
-    import ctypes
-    _cuda_contig(qkv, kv_cache_base, page_list, sequence_lengths, q_out, bias, position_ids, cos_sin_cache)
-    P, two, Hkv, T, D = kv_cache_base.shape
-    rows = qkv.shape[0]
-    if q_len < 1 or rows % q_len:
-        raise B200Error(f"rope_append_ex: {rows} qkv rows are not a multiple of q_len {q_len}")
-    if position_ids is not None and position_ids.numel() != rows:
-        raise B200Error(f"rope_append_ex: {position_ids.numel()} position ids for {rows} qkv rows")
-    if q_out is None:
-        q_out = torch.empty((rows, head_num * D), dtype=qkv.dtype, device=qkv.device)
+    q_out, io, ex, shape = _rope_args("rope_append_ex", qkv, kv_cache_base, page_list, sequence_lengths, head_num, q_out, q_len,
+                                      bias=bias, rope_cfg=rope_cfg, position_ids=position_ids, cos_sin_cache=cos_sin_cache,
+                                      use_logn_attn=use_logn_attn)
     lib = _lib.load()
-    args = (_p(qkv), _p(bias), _p(q_out), _p(kv_cache_base), _p(page_list), _p(sequence_lengths), _p(position_ids),
-            _p(cos_sin_cache), cos_sin_cache.shape[0] if cos_sin_cache is not None else 0,
-            ctypes.cast(ctypes.pointer(rope_cfg), ctypes.c_void_p), 1 if use_logn_attn else 0, _is_bf16(qkv), rows // q_len, head_num,
-            Hkv, D, page_list.shape[-1], T)
     if q_len == 1:
-        check(lib.b200_rope_append_ex(*args, _stream()), "b200_rope_append_ex")
+        check(lib.b200_rope_append_ex(_p(qkv), _p(bias), *io, *ex, *shape, _stream()), "b200_rope_append_ex")
     else:
-        check(lib.b200_rope_append_ex_multi(*args, q_len, _stream()), "b200_rope_append_ex_multi")
+        check(lib.b200_rope_append_ex_multi(_p(qkv), _p(bias), *io, *ex, *shape, q_len, _stream()), "b200_rope_append_ex_multi")
     return q_out
-
-
-def _qk_norm_checks(what, qkv, q_gamma, k_gamma, D, q_len):
-    _cuda_contig(q_gamma, k_gamma)
-    rows = qkv.shape[0]
-    if q_len < 1 or rows % q_len:
-        raise B200Error(f"{what}: {rows} qkv rows are not a multiple of q_len {q_len}")
-    for name, g in (("q_gamma", q_gamma), ("k_gamma", k_gamma)):
-        if g is None or g.dtype != qkv.dtype or g.numel() != D:
-            raise B200Error(f"{what}: {name} must be a [{D}] tensor of qkv's dtype {qkv.dtype}")
 
 
 def qk_norm_rope_append(qkv, q_gamma, k_gamma, eps, kv_cache_base, page_list, sequence_lengths, head_num, rope_base, q_out=None,
@@ -446,15 +441,10 @@ def qk_norm_rope_append(qkv, q_gamma, k_gamma, eps, kv_cache_base, page_list, se
     """rope_append after Qwen3's QK-RMSNorm, in one launch: each q and k head of qkv is RMS-normalised with q_gamma / k_gamma
     [D] first, with the bits of qk_rmsnorm on a copy of qkv followed by rope_append (b200_qk_norm_rope_append). qkv is only
     read. Returns q [B*q_len, Hq*D]."""
-    _cuda_contig(qkv, kv_cache_base, page_list, sequence_lengths, q_out)
-    P, two, Hkv, T, D = kv_cache_base.shape
-    _qk_norm_checks("qk_norm_rope_append", qkv, q_gamma, k_gamma, D, q_len)
-    rows = qkv.shape[0]
-    if q_out is None:
-        q_out = torch.empty((rows, head_num * D), dtype=qkv.dtype, device=qkv.device)
-    check(_lib.load().b200_qk_norm_rope_append(_p(qkv), _p(q_gamma), _p(k_gamma), eps, _p(q_out), _p(kv_cache_base), _p(page_list),
-                                               _p(sequence_lengths), _is_bf16(qkv), rows // q_len, head_num, Hkv, D,
-                                               page_list.shape[-1], T, rope_base, q_len, _stream()), "b200_qk_norm_rope_append")
+    q_out, io, _, shape = _rope_args("qk_norm_rope_append", qkv, kv_cache_base, page_list, sequence_lengths, head_num, q_out, q_len,
+                                     qk_norm=(q_gamma, k_gamma))
+    check(_lib.load().b200_qk_norm_rope_append(_p(qkv), _p(q_gamma), _p(k_gamma), eps, *io, *shape, rope_base, q_len, _stream()),
+          "b200_qk_norm_rope_append")
     return q_out
 
 
@@ -463,20 +453,11 @@ def qk_norm_rope_append_ex(qkv, q_gamma, k_gamma, eps, kv_cache_base, page_list,
                            q_len: int = 1):
     """rope_append_ex (no bias) after Qwen3's QK-RMSNorm, in one launch (b200_qk_norm_rope_append_ex): the bits of qk_rmsnorm
     on a copy of qkv followed by rope_append_ex. qkv is only read. Returns q [B*q_len, Hq*D]."""
-    import ctypes
-    _cuda_contig(qkv, kv_cache_base, page_list, sequence_lengths, q_out, position_ids, cos_sin_cache)
-    P, two, Hkv, T, D = kv_cache_base.shape
-    _qk_norm_checks("qk_norm_rope_append_ex", qkv, q_gamma, k_gamma, D, q_len)
-    rows = qkv.shape[0]
-    if position_ids is not None and position_ids.numel() != rows:
-        raise B200Error(f"qk_norm_rope_append_ex: {position_ids.numel()} position ids for {rows} qkv rows")
-    if q_out is None:
-        q_out = torch.empty((rows, head_num * D), dtype=qkv.dtype, device=qkv.device)
-    check(_lib.load().b200_qk_norm_rope_append_ex(
-        _p(qkv), _p(q_gamma), _p(k_gamma), eps, _p(q_out), _p(kv_cache_base), _p(page_list), _p(sequence_lengths),
-        _p(position_ids), _p(cos_sin_cache), cos_sin_cache.shape[0] if cos_sin_cache is not None else 0,
-        ctypes.cast(ctypes.pointer(rope_cfg), ctypes.c_void_p), 1 if use_logn_attn else 0, _is_bf16(qkv), rows // q_len, head_num,
-        Hkv, D, page_list.shape[-1], T, q_len, _stream()), "b200_qk_norm_rope_append_ex")
+    q_out, io, ex, shape = _rope_args("qk_norm_rope_append_ex", qkv, kv_cache_base, page_list, sequence_lengths, head_num, q_out,
+                                      q_len, qk_norm=(q_gamma, k_gamma), rope_cfg=rope_cfg, position_ids=position_ids,
+                                      cos_sin_cache=cos_sin_cache, use_logn_attn=use_logn_attn)
+    check(_lib.load().b200_qk_norm_rope_append_ex(_p(qkv), _p(q_gamma), _p(k_gamma), eps, *io, *ex, *shape, q_len, _stream()),
+          "b200_qk_norm_rope_append_ex")
     return q_out
 
 
