@@ -265,8 +265,9 @@ int b200_argmax(const void* logits, int dtype, int rows, int vocab, int32_t* out
  * Per row, in this order: temperature (logit *= 1/(T+1e-6)), repetition / presence / frequency penalties over the DISTINCT
  * tokens of `history` (hist_len[r] valid ids of [rows][hist_stride]), softmax (the probabilities REPLACE the logits, as in the
  * reference), top-k (keep p >= the k-th largest; top_k <= 0 = no limit; top_k == 1 = argmax, lowest index on ties), top-p
- * within what is left (smallest set of largest p reaching top_p; |top_p| < 1e-7 or >= 1 = no limit), renormalise, and one
- * inverse-CDF draw in index order with the caller's uniform[r] in [0, 1), which always returns a kept token with p > 0
+ * within what is left (smallest set of largest p reaching top_p; |top_p| < 1e-7 or >= 1 = no limit), min-p within what is left
+ * (keep p >= fl32(min_p[r] * p_max), p_max the row's largest p; min_p optional [rows], clamped to [0, 1]; NULL or 0 = no limit,
+ * bit-identical to a call without it), renormalise, and one inverse-CDF draw in index order with the caller's uniform[r] in [0, 1), which always returns a kept token with p > 0
  * (token -1 and token_prob 0 only for a row without positive finite mass, i.e. NaN logits).  Same distribution as the
  * reference's flashinfer rejection sampler, different random stream: the caller owns the randomness, so the op is
  * deterministic and graph-replayable.
@@ -275,8 +276,8 @@ int b200_argmax(const void* logits, int dtype, int rows, int vocab, int32_t* out
  * for cum_log_probs += log p), probs_out [rows][vocab] (output_all_probs after renormalisation). logits fp32, contiguous. */
 int b200_sample(float* logits, int rows, int vocab, const int32_t* history, const int32_t* hist_len, int hist_stride,
                 int32_t* count_ws, const float* temperature, const float* repetition, const float* presence,
-                const float* frequency, const int32_t* top_k, const float* top_p, const float* uniform, const uint8_t* process,
-                int32_t* token_out, float* token_prob_out, float* probs_out, void* stream);
+                const float* frequency, const int32_t* top_k, const float* top_p, const float* min_p, const float* uniform,
+                const uint8_t* process, int32_t* token_out, float* token_prob_out, float* probs_out, void* stream);
 
 /* Verification of num_draft = n speculative tokens per sequence (the chain form of the reference's speculative-sampling kernel,
  * rtp_llm/models_py/bindings/cuda/kernels/speculative_sampling/sampling.cu), after a step over the batch*(n+1) rows
@@ -377,6 +378,24 @@ int b200_token_logprobs(const void* logits, int dtype, int rows, int vocab, int 
  * this op and those does not matter. One CTA per row; under PDL it waits before reading anything. */
 int b200_ban_repeat_ngram(void* logits, int dtype, int rows, int vocab, const int32_t* history, const int32_t* hist_len, int hist_stride,
                           const int32_t* ngram_size, void* stream);
+
+/* Constrained decoding, in place on logits [rows][vocab] (dtype 0 fp16, 1 bf16, 2 fp32), before b200_argmax, b200_sample or
+ * b200_beam_search_step: a grammar engine's token bitmask and OpenAI-style logit_bias.
+ *   bitmask [rows][mask_stride] int32, xgrammar's layout: token t of row r is allowed iff (bitmask[r][t >> 5] >> (t & 31)) & 1
+ *   (an all-ones word, -1, allows its 32 tokens); mask_stride >= ceil(vocab / 32); bits at t >= vocab are ignored; NULL = no
+ *   mask. A masked token becomes the dtype's -inf and is never read.
+ *   bias: a CSR over rows, bias_offsets [rows + 1] (offsets[0] = 0, non-decreasing) selects the entries [offsets[r],
+ *   offsets[r+1]) of bias_ids / bias_values. An allowed token t = ids[e] becomes round_T(float(x) + values[e]): one fp32 add and
+ *   one rounding to the logits' dtype (so fp16 can overflow to +-inf). Ids outside [0, vocab) are ignored, a bias on a masked
+ *   token has no effect, and the ids of a row must be distinct (not checked). NULL bias_offsets = no bias.
+ *   Every other logit keeps its bits, NaN included.
+ * rows in 1..65535; at least one of bitmask and bias_offsets. A row whose mask allows nothing becomes all -inf: b200_argmax
+ * then returns token 0, b200_sample token -1 with token_prob 0, and b200_beam_search_step scores the row's candidates -inf.
+ * Cost: the mask pass reads rows * ceil(vocab / 32) words and writes only the masked tokens (a fully masked word as 16-byte
+ * stores when the row is 16-byte aligned), so an all-ones mask writes nothing; only biased entries read logits. One launch,
+ * deterministic, graph-capturable, recorded by decode programs; under PDL it writes nothing before its grid dependency. */
+int b200_constrain_logits(void* logits, int dtype, int rows, int vocab, const int32_t* bitmask, int mask_stride,
+                          const int32_t* bias_offsets, const int32_t* bias_ids, const float* bias_values, void* stream);
 
 /* ------------------------------------------------------------------------------------------------ TP all-reduce over NVLink peer memory */
 

@@ -53,7 +53,7 @@ SIGNATURES = {
                                     + [c_void_p]),
     "b200_embedding": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "b200_argmax": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
-    "b200_sample": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int] + [c_void_p] * 13),
+    "b200_sample": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int] + [c_void_p] * 14),
     "b200_spec_verify": (c_int, [c_void_p] * 5 + [c_int] * 3 + [c_void_p] * 3),
     "b200_beam_search_step_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "b200_beam_search_step": (c_int, [c_void_p, c_int, c_void_p] + [c_int] * 4 + [c_void_p] * 7 + [c_size_t, c_void_p]),
@@ -64,6 +64,7 @@ SIGNATURES = {
     "b200_token_logprobs_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "b200_token_logprobs": (c_int, [c_void_p] + [c_int] * 4 + [c_void_p] * 5 + [c_size_t, c_void_p]),
     "b200_ban_repeat_ngram": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "b200_constrain_logits": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int] + [c_void_p] * 4),
     "b200_peer_ar_region_bytes": (c_size_t, [c_size_t]),
     "b200_peer_alloc": (c_int, [c_size_t, c_void_p, c_void_p]),
     "b200_peer_open": (c_int, [c_void_p, c_void_p]),

@@ -968,8 +968,8 @@ int b200_argmax(const void* logits, int dtype, int rows, int vocab, int32_t* out
 
 int b200_sample(float* logits, int rows, int vocab, const int32_t* history, const int32_t* hist_len, int hist_stride,
                 int32_t* count_ws, const float* temperature, const float* repetition, const float* presence,
-                const float* frequency, const int32_t* top_k, const float* top_p, const float* uniform, const uint8_t* process,
-                int32_t* token_out, float* token_prob_out, float* probs_out, void* stream) {
+                const float* frequency, const int32_t* top_k, const float* top_p, const float* min_p, const float* uniform,
+                const uint8_t* process, int32_t* token_out, float* token_prob_out, float* probs_out, void* stream) {
     if (rows == 0) return B200_OK;
     ARG_CHECK(logits && top_k && top_p && uniform && token_out, "sample: null pointer");
     ARG_CHECK(rows > 0 && rows <= 65535 && vocab > 0, "sample: bad shape [%d, %d]", rows, vocab);
@@ -987,6 +987,7 @@ int b200_sample(float* logits, int rows, int vocab, const int32_t* history, cons
     p.frequency = frequency;
     p.top_k = top_k;
     p.top_p = top_p;
+    p.min_p = min_p;
     p.uniform = uniform;
     p.process = process;
     p.token_out = token_out;
@@ -1270,6 +1271,33 @@ int b200_ban_repeat_ngram(void* logits, int dtype, int rows, int vocab, const in
     auto launch = [&](auto t) {
         return launch_or_record("ban_repeat_ngram_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
             return launch_ex(ban_repeat_ngram_kernel<decltype(t)>, {dim3(rows), dim3(256), 0, s, pdl}, p);
+        });
+    };
+    return dtype == 2 ? launch(0.f) : by_dtype(dtype == 1, launch);
+}
+
+int b200_constrain_logits(void* logits, int dtype, int rows, int vocab, const int32_t* bitmask, int mask_stride,
+                          const int32_t* bias_offsets, const int32_t* bias_ids, const float* bias_values, void* stream) {
+    ARG_CHECK(rows >= 1 && rows <= 65535, "constrain_logits: rows %d unsupported (1..65535)", rows);
+    ARG_CHECK(vocab > 0, "constrain_logits: vocab must be positive");
+    ARG_CHECK(dtype >= 0 && dtype <= 2, "constrain_logits: dtype %d unknown (0 fp16, 1 bf16, 2 fp32)", dtype);
+    ARG_CHECK(logits, "constrain_logits: null pointer (logits)");
+    ARG_CHECK(bitmask || bias_offsets, "constrain_logits: neither a bitmask nor a bias given");
+    ARG_CHECK(!bias_offsets || (bias_ids && bias_values), "constrain_logits: null pointer (bias_ids / bias_values with bias_offsets)");
+    const int words = (int)(((long long)vocab + 31) / 32);
+    ARG_CHECK(!bitmask || mask_stride >= words, "constrain_logits: mask_stride %d < ceil(vocab / 32) = %d", mask_stride, words);
+    ConstrainParams p{};
+    p.logits = logits;
+    p.bitmask = reinterpret_cast<const uint32_t*>(bitmask);
+    p.bias_offsets = bias_offsets;
+    p.bias_ids = bias_ids;
+    p.bias_values = bias_values;
+    p.vocab = vocab;
+    p.mask_stride = mask_stride;
+    const dim3 grid((words + kConstrainThreads - 1) / kConstrainThreads, rows);
+    auto launch = [&](auto t) {
+        return launch_or_record("constrain_logits_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+            return launch_ex(constrain_logits_kernel<decltype(t)>, {grid, dim3(kConstrainThreads), 0, s, pdl}, p);
         });
     };
     return dtype == 2 ? launch(0.f) : by_dtype(dtype == 1, launch);

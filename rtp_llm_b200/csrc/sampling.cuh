@@ -10,6 +10,7 @@
 //   top_k == 1       argmax, lowest index on ties                    (:330-331, :453)
 //   top_k            keep p >= (k-th largest p), renormalise         (flashinfer top_k_renorm_probs semantics)
 //   top_p            of what is left keep the smallest set of largest p whose mass reaches top_p, renormalise
+//   min_p            of what is left keep p >= min_p * p_max (Hugging Face MinPLogitsWarper, applied after top-p)
 //   draw             inverse CDF over the kept tokens in index order with a caller-supplied uniform u in [0, 1)
 // The reference draws through flashinfer's rejection sampler with a Philox stream; the DISTRIBUTION is the same
 // (its own accuracy test compares distributions, CudaSamplerTest.cc:143-147), the random stream is not: here the caller
@@ -39,6 +40,7 @@ struct SampleParams {
     const float* frequency;     // optional [rows] (0 = off)
     const int32_t* top_k;       // [rows]; <= 0: no limit
     const float* top_p;         // [rows]; >= 1 or ~0: no limit
+    const float* min_p;         // optional [rows] in [0, 1] (clamped): also keep only p >= min_p * p_max
     const float* uniform;       // [rows] in [0, 1)
     const uint8_t* process;     // optional [rows]: 0 = skip temperature / penalties for this row (do_sample == false)
     int32_t* token_out;         // [rows]
@@ -220,6 +222,9 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(const SamplePara
         }
         thr = __uint_as_float(lo);
     }
+    // min-p after top-p (the Hugging Face order). The bound is relative to the row's max, which top-k / top-p always keep, so
+    // it equals min-p on the renormalised top-k / top-p distribution. min_p 0 leaves thr (>= 0) as it is.
+    if (p.min_p) thr = fmaxf(thr, fminf(fmaxf(p.min_p[row], 0.f), 1.f) * pmax);
 
     // ---- draw: inverse CDF over the kept tokens in index order (contiguous chunk per thread, block scan of chunk sums)
     // top_k == 1: the lowest index among the maxima (argmax semantics)
@@ -871,6 +876,69 @@ __global__ void __launch_bounds__(256) ban_repeat_ngram_kernel(const BanNgramPar
         for (int k = 0; k < n - 1 && match; ++k) match = h[s + k] == h[L - n + 1 + k];
         const int t = h[s + n - 1];
         if (match && t >= 0 && t < p.vocab) lg[t] = from_f32<T>(-INFINITY);
+    }
+}
+
+// ------------------------------------------------------------------------------------------------ constrained decoding
+// Grammar bitmask and logit bias, in place on the logits, before any ending picks a token. Token t of row r is allowed iff
+// bit (t & 31) of bitmask[r][t >> 5] is set (xgrammar's layout; bits at t >= vocab are ignored). A masked token becomes -inf
+// without being read; an allowed token t = bias_ids[e], e in [bias_offsets[r], bias_offsets[r+1]), becomes
+// round_T(float(x) + bias_values[e]); every other logit keeps its bits. Grid (ceil(words / kConstrainThreads), rows): each warp
+// loads 32 consecutive mask words with one coalesced load, writes the fully masked ones as 16-byte stores (32 lanes, several
+// words per store) when the row is 16-byte aligned and the partly masked ones a word at a time (lane = token). The bias entries
+// are spread over the row's CTAs; each checks the mask bit first, so the two passes touch disjoint tokens and cannot race.
+constexpr int kConstrainThreads = 256;
+
+struct ConstrainParams {
+    void* logits;                  // [rows][vocab] fp16 / bf16 / fp32, edited in place
+    const uint32_t* bitmask;       // optional [rows][mask_stride]
+    const int32_t* bias_offsets;   // optional [rows + 1]
+    const int32_t* bias_ids;       // [bias_offsets[rows]]
+    const float* bias_values;      // [bias_offsets[rows]]
+    int vocab, mask_stride;
+};
+
+template <typename T>
+__global__ void __launch_bounds__(kConstrainThreads) constrain_logits_kernel(const ConstrainParams p) {
+    const int row = blockIdx.y, lane = threadIdx.x & 31, V = p.vocab;
+    pdl_wait();                        // under PDL the logits come from the kernel before this one
+    T* lg = reinterpret_cast<T*>(p.logits) + (size_t)row * V;
+    const uint32_t* mask = p.bitmask ? p.bitmask + (size_t)row * p.mask_stride : nullptr;
+    if (mask) {
+        const int w0 = blockIdx.x * kConstrainThreads + (threadIdx.x & ~31), w = w0 + lane;
+        uint32_t word = ~0u;                                   // past the last word: nothing to write
+        if (w <= (V - 1) >> 5) {
+            word = mask[w];
+            if (V - 32 * w < 32) word |= ~0u << (V - 32 * w);  // bits at t >= vocab count as allowed: never written
+        }
+        const bool aligned = (reinterpret_cast<uintptr_t>(lg) & 15) == 0;
+        const uint32_t full = __ballot_sync(~0u, aligned && word == 0u);
+        const uint32_t part = __ballot_sync(~0u, word != ~0u) & ~full;
+        constexpr int kPerWord = 32 * (int)sizeof(T) / 16;     // 16-byte stores per word: 4 (fp16 / bf16) or 8 (fp32)
+        uint4 ninf;
+        T* e = reinterpret_cast<T*>(&ninf);
+#pragma unroll
+        for (int k = 0; k < 16 / (int)sizeof(T); ++k) e[k] = from_f32<T>(-INFINITY);
+        for (uint32_t m = full; m;) {
+            uint32_t mine = m;                                 // lane's word: set bit number lane / kPerWord of m
+            for (int s = 0; s < lane / kPerWord; ++s) mine &= mine - 1;
+            if (mine)
+                reinterpret_cast<uint4*>(lg + 32 * (w0 + __ffs(mine) - 1))[lane % kPerWord] = ninf;
+            for (int s = 0; s < 32 / kPerWord; ++s) m &= m - 1;
+        }
+        for (uint32_t m = part; m; m &= m - 1) {
+            const int j = __ffs(m) - 1;
+            const uint32_t wj = __shfl_sync(~0u, word, j);
+            if (!((wj >> lane) & 1u)) lg[32 * (w0 + j) + lane] = from_f32<T>(-INFINITY);
+        }
+    }
+    if (p.bias_offsets) {
+        const int e1 = p.bias_offsets[row + 1];
+        for (int i = p.bias_offsets[row] + blockIdx.x * kConstrainThreads + threadIdx.x; i < e1; i += gridDim.x * kConstrainThreads) {
+            const int t = p.bias_ids[i];
+            if (t < 0 || t >= V || (mask && !((mask[t >> 5] >> (t & 31)) & 1u))) continue;   // masked: the mask pass writes it
+            lg[t] = from_f32<T>(to_f32<T>(lg[t]) + p.bias_values[i]);
+        }
     }
 }
 

@@ -13,7 +13,7 @@ from __future__ import annotations
 import dataclasses
 import math
 import os
-from typing import Dict, List, Optional, Sequence, Union
+from typing import Dict, List, Mapping, Optional, Sequence, Union
 
 import torch
 
@@ -64,7 +64,7 @@ TINY_QWEN3 = ModelConfig("tiny-qwen3", 512, 2, 8, 2, 128, 512, 1024, rope_base=1
 class SamplingParams:
     """Per-request sampling parameters of DecodeStep's sampling mode: each field is one value for every request or a sequence of
     one value per request, with b200_sample's meaning (top_k <= 0 and top_p >= 1: no limit; repetition 1, presence 0 and
-    frequency 0: off). seed fixes the step's uniforms (sampling_uniforms)."""
+    frequency 0: off; min_p in [0, 1], 0: off). seed fixes the step's uniforms (sampling_uniforms)."""
     temperature: Union[float, Sequence[float]] = 1.0
     top_k: Union[int, Sequence[int]] = 0
     top_p: Union[float, Sequence[float]] = 1.0
@@ -72,10 +72,14 @@ class SamplingParams:
     presence: Union[float, Sequence[float]] = 0.0
     frequency: Union[float, Sequence[float]] = 0.0
     seed: int = 0
+    min_p: Union[float, Sequence[float]] = 0.0
 
     def has_penalties(self) -> bool:
         return any(any(float(v) != off for v in (x if isinstance(x, (list, tuple)) else [x]))
                    for x, off in ((self.repetition, 1.0), (self.presence, 0.0), (self.frequency, 0.0)))
+
+    def has_min_p(self) -> bool:
+        return any(float(v) != 0.0 for v in (self.min_p if isinstance(self.min_p, (list, tuple)) else [self.min_p]))
 
 
 _U32 = 0xFFFFFFFF
@@ -191,7 +195,17 @@ class DecodeStep:
     At q_len > 1 it verifies drafts by sampling: b200_sample runs over the B * q_len rows with probs_out into target_probs
     [B, q_len, V], then spec_verify in sampling mode with deterministic drafts (draft_probs None) and its own uniforms [B, q_len].
     Like the greedy verification step it does not advance. Penalties and the n-gram ban are rejected there: row j's history
-    would have to hold drafts 0..j-1."""
+    would have to hold drafts 0..j-1. SamplingParams.min_p runs b200_sample with a min_p buffer when some value is not 0, and
+    without one (today's kernel call) when every value is 0.
+
+    token_bitmask=True and / or logit_bias_capacity=n > 0 (TP 1, every mode): constrained decoding. Static device buffers,
+    filled by set_constraints() from pinned host twins, hold one grammar bitmask row per logits row (int32 [R, ceil(V / 32)],
+    xgrammar's layout) and a logit-bias CSR of up to n entries; a graph replay applies what was set last, and upload_inputs()
+    resets them to unconstrained (all-ones mask, no bias entries). b200_constrain_logits runs once per step where the ending
+    reads the logits: on self.logits before argmax (greedy and greedy verification; row j of a verification step carries the
+    mask of position j), on samp_logits after the fp32 copy and before the n-gram ban and b200_sample (sampling and sampled
+    verification), on self.logits before the n-gram ban and beam_search_step (beam: one row per beam, before the
+    log-softmax). The log-probs keep scoring the raw lm_head output. Without these options the step's launches are unchanged."""
 
     def __init__(self, cfg: ModelConfig, batch: int, ctx: int, device: torch.device, tp_rank: int = 0, tp_size: int = 1,
                  dtype=torch.float16, seed: int = 0, keep_reference: bool = False, ragged: bool = False,
@@ -200,8 +214,18 @@ class DecodeStep:
                  no_repeat_ngram: int = 0, max_new_tokens: int = 16, sampling: Optional[SamplingParams] = None,
                  logprobs: Optional[int] = None, eos_id: Optional[int] = None,
                  length_penalty: Union[float, Sequence[float]] = 1.0,
-                 early_stopping: Union[bool, str, Sequence[Union[bool, str]]] = False):
+                 early_stopping: Union[bool, str, Sequence[Union[bool, str]]] = False,
+                 token_bitmask: bool = False, logit_bias_capacity: int = 0):
         assert cfg.head_num % tp_size == 0 and cfg.inter % tp_size == 0
+        if logit_bias_capacity < 0:
+            raise ValueError(f"logit_bias_capacity must be >= 0 (got {logit_bias_capacity})")
+        if (token_bitmask or logit_bias_capacity) and tp_size != 1:
+            raise ValueError(f"token_bitmask / logit_bias need tp_size 1 (got tp_size {tp_size}): the vocabulary-parallel argmax "
+                             "would need a mask sharded by vocabulary")
+        if sampling is not None:
+            mp = sampling.min_p if isinstance(sampling.min_p, (list, tuple)) else [sampling.min_p]
+            if not all(0.0 <= float(v) <= 1.0 for v in mp):
+                raise ValueError(f"sampling: min_p must be in [0, 1] (got {sampling.min_p})")
         if q_len < 1:
             raise ValueError(f"q_len must be >= 1 (got {q_len})")
         if q_len > 1 and (batch * q_len > 128 or tp_size != 1):
@@ -504,6 +528,8 @@ class DecodeStep:
                 self.samp_params.update(repetition=per_row(sp.repetition, torch.float32), presence=per_row(sp.presence, torch.float32),
                                         frequency=per_row(sp.frequency, torch.float32),
                                         count_ws=torch.zeros(R, self.vocab, dtype=torch.int32, device=device))
+            if sp.has_min_p():
+                self.samp_params["min_p"] = per_row(sp.min_p, torch.float32)
             self.samp_logits = buf(R, self.vocab, dt=torch.float32)
             self.token_prob = buf(R, dt=torch.float32)
             self.log_prob = buf(R, dt=torch.float32)
@@ -522,6 +548,15 @@ class DecodeStep:
                 self.lp_out = dict(token_logprob=buf(R, dt=torch.float32), top_ids=buf(R, logprobs, dt=torch.int32),
                                    top_logprobs=buf(R, logprobs, dt=torch.float32))
                 self.lp_ws = ops.token_logprobs_workspace(R, self.vocab, logprobs, device)
+        # constrained decoding: device buffers the step reads, pinned host twins set_constraints() fills
+        if token_bitmask:
+            self.bitmask_h = torch.full((R, (self.vocab + 31) // 32), -1, dtype=torch.int32).pin_memory()
+            self.bitmask = buf(R, self.bitmask_h.shape[1], dt=torch.int32)
+        if logit_bias_capacity:
+            self.bias_h = (torch.zeros(R + 1, dtype=torch.int32).pin_memory(),
+                           torch.zeros(logit_bias_capacity, dtype=torch.int32).pin_memory(),
+                           torch.zeros(logit_bias_capacity, dtype=torch.float32).pin_memory())
+            self.bias = tuple(torch.zeros_like(t, device=device) for t in self.bias_h)
         self.x_perm = buf(R, H) if act_order else None                        # x[:, perm] before qkv / w13
         self.attn_perm = buf(R, self.Hq * self.D) if act_order else None      # attn[:, perm] before o
         shapes = [(H, qkv_n), (self.Hq * self.D, H), (H, 2 * self.inter), (self.inter, H), (H, self.vocab)]
@@ -560,8 +595,59 @@ class DecodeStep:
                 self.hist[:, 0].copy_(self.ids)
                 self.hist_len.fill_(1)
                 self.beam_steps = 0
+        if self.bitmask is not None or self.bias is not None:
+            self.set_constraints()
+
+    def set_constraints(self, bitmask=None, logit_bias: Optional[Sequence[Mapping[int, float]]] = None):
+        """The constraints the next step (or graph replay) applies, from host data, copied non_blocking into the static
+        buffers: bitmask int32 [R, ceil(V / 32)] (numpy or CPU tensor, xgrammar's layout; None: every token allowed) and
+        logit_bias, one {token id: bias} mapping per logits row (None: no bias; at most logit_bias_capacity entries in all).
+        R is the step's logits rows: row b (greedy, sampling), b * q_len + j (verification: position j), b * W + i (beam i).
+        Like upload_inputs(), it rewrites pinned buffers a copy may still read: call it once the previous step has been
+        enqueued and its inputs are no longer needed, as between two replays."""
+        R, V = self.B * self.q_len, self.vocab
+        if bitmask is not None:
+            if self.bitmask is None:
+                raise ValueError("set_constraints: this step was built without token_bitmask=True")
+            m = torch.as_tensor(bitmask)
+            if m.dtype != torch.int32 or tuple(m.shape) != tuple(self.bitmask_h.shape) or m.device.type != "cpu":
+                raise ValueError(f"set_constraints: bitmask must be host int32 {list(self.bitmask_h.shape)} (got {m.dtype} "
+                                 f"{list(m.shape)} on {m.device})")
+        if logit_bias is not None:
+            if self.bias is None:
+                raise ValueError("set_constraints: this step was built without logit_bias_capacity")
+            if len(logit_bias) != R:
+                raise ValueError(f"set_constraints: logit_bias needs one mapping per logits row ({R}, got {len(logit_bias)})")
+            try:
+                offsets, ids, values = ops.logit_bias_csr(logit_bias, V)
+            except ops.B200Error as e:
+                raise ValueError(str(e)) from None
+            if ids.numel() > self.bias_h[1].numel():
+                raise ValueError(f"set_constraints: {ids.numel()} logit_bias entries exceed logit_bias_capacity "
+                                 f"{self.bias_h[1].numel()}")
+        if self.bitmask is not None:
+            if bitmask is None:
+                self.bitmask_h.fill_(-1)
+            else:
+                self.bitmask_h.copy_(m)
+            self.bitmask.copy_(self.bitmask_h, non_blocking=True)
+        if self.bias is not None:
+            if logit_bias is None:
+                self.bias_h[0].zero_()
+            else:
+                self.bias_h[0].copy_(offsets)
+                self.bias_h[1][:ids.numel()] = ids
+                self.bias_h[2][:ids.numel()] = values
+            for d, h in zip(self.bias, self.bias_h):
+                d.copy_(h, non_blocking=True)
+
+    def _constrain(self, logits: torch.Tensor):
+        """b200_constrain_logits on `logits` with the buffers set_constraints() filled (no launch when the step has none)."""
+        if self.bitmask is not None or self.bias is not None:
+            ops.constrain_logits(logits, bitmask=self.bitmask, logit_bias=self.bias)
 
     sample_advances = False
+    bitmask = bitmask_h = bias = bias_h = None     # no constraint buffers unless token_bitmask / logit_bias_capacity
 
     def _count_beam_step(self):
         if self.W > 1 or self.sample_advances:
@@ -579,7 +665,9 @@ class DecodeStep:
 
     def h2d_bytes(self) -> int:
         drafts = self.drafts_h.numel() * 4 if self.q_len > 1 else 0
-        return self.ids_h.numel() * 4 + self.seq_lens_h.numel() * 4 + self.block_ids_h.numel() * 4 + drafts
+        constraints = sum(t.numel() * 4 for t in ([self.bitmask_h] if self.bitmask is not None else [])
+                          + (list(self.bias_h) if self.bias is not None else []))
+        return self.ids_h.numel() * 4 + self.seq_lens_h.numel() * 4 + self.block_ids_h.numel() * 4 + drafts + constraints
 
     def d2h_bytes(self) -> int:
         if self.q_len > 1:
@@ -663,6 +751,7 @@ class DecodeStep:
         self._ar_norm(self.proj, self.final_ln)
         ops.wo_gemm(self.x, self.lm_head, self.gemm_ws, out=self.logits, pdl=self.pdl)
         if self.W > 1:
+            self._constrain(self.logits)
             if self.ngram > 0:
                 ops.ban_repeat_ngram(self.logits, self.hist, self.hist_len, self.ngram_size)
             ops.beam_search_step(self.logits, self.beam_cum, self.W, eos_id=-1 if self.eos_id is None else self.eos_id,
@@ -674,6 +763,7 @@ class DecodeStep:
         elif self.samp is not None:
             self.sample()
         elif self.tp_size == 1:
+            self._constrain(self.logits)
             ops.argmax(self.logits, out=self.next_ids)
             if self.q_len > 1:
                 ops.spec_verify(self.drafts, target_ids=self.next_ids.view(self.B, self.q_len), out_tokens=self.out_tokens,
@@ -737,13 +827,14 @@ class DecodeStep:
         self.uniforms.draw(self.draw_step, self.uniform)
         self.draw_step.add_(1)
         self.samp_logits.copy_(self.logits)
+        self._constrain(self.samp_logits)
         adv = self.q_len == 1
         if adv and self.ngram > 0:
             ops.ban_repeat_ngram(self.samp_logits, self.hist, self.hist_len, self.ngram_size)
         hist = dict(history=self.hist, hist_len=self.hist_len) if adv else {}
         ops.sample(self.samp_logits, sp["top_k"], sp["top_p"], self.uniform[:R], temperature=sp["temperature"],
                    repetition=sp.get("repetition"), presence=sp.get("presence"), frequency=sp.get("frequency"),
-                   count_ws=sp.get("count_ws"), out=dict(token=self.next_ids, token_prob=self.token_prob,
+                   count_ws=sp.get("count_ws"), min_p=sp.get("min_p"), out=dict(token=self.next_ids, token_prob=self.token_prob,
                                                          **({} if adv else dict(probs=self.target_probs))), **hist)
         if self.logprobs is not None:
             ops.token_logprobs(self.logits, self.logprobs, tokens=self.next_ids, workspace=self.lp_ws, out=self.lp_out)

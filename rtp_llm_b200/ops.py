@@ -3,7 +3,8 @@ libb200_decode.so. Every function launches on the current CUDA stream and is CUD
 from __future__ import annotations
 
 import math
-from typing import Optional
+import numbers
+from typing import Mapping, Optional, Sequence, Tuple
 
 import torch
 
@@ -485,17 +486,25 @@ def sample(logits: torch.Tensor, top_k: torch.Tensor, top_p: torch.Tensor, unifo
            hist_len: Optional[torch.Tensor] = None, repetition: Optional[torch.Tensor] = None,
            presence: Optional[torch.Tensor] = None, frequency: Optional[torch.Tensor] = None,
            process: Optional[torch.Tensor] = None, count_ws: Optional[torch.Tensor] = None, want_probs: bool = False,
-           out: Optional[dict] = None):
+           out: Optional[dict] = None, min_p: Optional[torch.Tensor] = None):
     """sampleGreedy's CUDA path (CudaSampleOp.cc:423-463) on fp32 logits [B, V], IN PLACE (logits become probabilities).
     Returns (tokens int32 [B], token_prob fp32 [B], renormalised probs [B, V] or None). `out` may hold preallocated
-    token int32 [B], token_prob fp32 [B] and probs fp32 [B, V] (graph capture); a given probs implies want_probs."""
+    token int32 [B], token_prob fp32 [B] and probs fp32 [B, V] (graph capture); a given probs implies want_probs.
+    min_p fp32 [B] in [0, 1] (None: off) keeps only p >= min_p * p_max of what top-k / top-p keep; its range is checked on the
+    host (a device read) except while a CUDA graph is being captured, where the kernel clamps it."""
     out = out or {}
     B, V = logits.shape
     for k, dtype, n in (("token", torch.int32, B), ("token_prob", torch.float32, B), ("probs", torch.float32, B * V)):
         if k in out and (out[k].dtype != dtype or out[k].numel() != n):
             raise B200Error(f"sample: out[{k!r}] must be {dtype} with {n} elements")
+    if min_p is not None:
+        if min_p.dtype != torch.float32 or min_p.numel() != B:
+            raise B200Error(f"sample: min_p must be fp32 [{B}]")
+        capturing = min_p.is_cuda and torch.cuda.is_current_stream_capturing()
+        if not capturing and not bool(((min_p >= 0) & (min_p <= 1)).all()):
+            raise B200Error("sample: min_p must be in [0, 1]")
     _cuda_contig(logits, top_k, top_p, uniform, temperature, history, hist_len, repetition, presence, frequency, process, count_ws,
-                 *out.values())
+                 min_p, *out.values())
     if logits.dtype != torch.float32:
         raise B200Error("sample: logits must be fp32 (the reference sampler runs on fp32 logits)")
     if (repetition is not None or presence is not None or frequency is not None) and count_ws is None:
@@ -505,7 +514,7 @@ def sample(logits: torch.Tensor, top_k: torch.Tensor, top_p: torch.Tensor, unifo
     probs = out.get("probs", torch.empty_like(logits) if want_probs else None)
     check(_lib.load().b200_sample(_p(logits), B, V, _p(history), _p(hist_len), history.shape[1] if history is not None else 0,
                                   _p(count_ws), _p(temperature), _p(repetition), _p(presence), _p(frequency), _p(top_k), _p(top_p),
-                                  _p(uniform), _p(process), _p(tok), _p(tprob), _p(probs), _stream()), "b200_sample")
+                                  _p(min_p), _p(uniform), _p(process), _p(tok), _p(tprob), _p(probs), _stream()), "b200_sample")
     return tok, tprob, probs
 
 
@@ -742,6 +751,61 @@ def ban_repeat_ngram(logits: torch.Tensor, history: torch.Tensor, hist_len: torc
     check(_lib.load().b200_ban_repeat_ngram(_p(logits), dt, rows, V, _p(history), _p(hist_len), history.shape[1], _p(ngram_size),
                                             _stream()), "b200_ban_repeat_ngram")
     return logits
+
+
+def constrain_logits(logits: torch.Tensor, bitmask: Optional[torch.Tensor] = None,
+                     logit_bias: Optional[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = None) -> torch.Tensor:
+    """Grammar mask and logit bias in place (b200_constrain_logits): logits [rows, V] fp16 / bf16 / fp32; bitmask int32
+    [rows, stride >= ceil(V / 32)] in xgrammar's layout (token t allowed iff bit t & 31 of word t >> 5 is set); logit_bias =
+    (offsets int32 [rows + 1], ids int32 [n], values fp32 [n]), a CSR over rows with offsets[rows] <= n (logit_bias_csr builds
+    it on the host; n = 0 is no bias, and without a bitmask then launches nothing). Masked tokens become -inf, allowed biased
+    ones round(x + bias). Returns logits."""
+    dt = _logit_dtype("constrain_logits", logits)
+    if logits.dim() != 2:
+        raise B200Error(f"constrain_logits: logits must be [rows, V] (got {tuple(logits.shape)})")
+    rows, V = logits.shape
+    if not 1 <= rows <= 65535:
+        raise B200Error(f"constrain_logits: rows {rows} unsupported (1..65535)")
+    if bitmask is None and logit_bias is None:
+        raise B200Error("constrain_logits: pass a bitmask, a logit_bias or both")
+    words = (V + 31) // 32
+    if bitmask is not None and (bitmask.dtype != torch.int32 or bitmask.dim() != 2 or bitmask.shape[0] != rows
+                                or bitmask.shape[1] < words):
+        raise B200Error(f"constrain_logits: bitmask must be int32 [{rows}, stride >= {words}] (got {bitmask.dtype} "
+                        f"{tuple(bitmask.shape)})")
+    offsets = ids = values = None
+    if logit_bias is not None:
+        offsets, ids, values = logit_bias
+        if offsets.dtype != torch.int32 or offsets.numel() != rows + 1:
+            raise B200Error(f"constrain_logits: bias offsets must be int32 [{rows + 1}]")
+        if ids.dtype != torch.int32 or values.dtype != torch.float32 or ids.numel() != values.numel():
+            raise B200Error("constrain_logits: bias ids must be int32 and values fp32, of one length")
+    _cuda_contig(logits, bitmask, offsets, ids, values)
+    if ids is not None and ids.numel() == 0:          # no entries: no bias (an empty tensor has no data pointer to pass)
+        if bitmask is None:
+            return logits
+        offsets = ids = values = None
+    check(_lib.load().b200_constrain_logits(_p(logits), dt, rows, V, _p(bitmask), 0 if bitmask is None else bitmask.shape[1],
+                                            _p(offsets), _p(ids), _p(values), _stream()), "b200_constrain_logits")
+    return logits
+
+
+def logit_bias_csr(per_row: Sequence[Mapping[int, float]], vocab: int) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """OpenAI-style logit_bias maps {token id: bias}, one per row, as the CSR constrain_logits takes: (offsets int32
+    [rows + 1], ids int32, values fp32), on the host. Rejects ids outside [0, vocab) and values that are not numbers or are
+    NaN; a mapping holds each id once, so the ids of a row are distinct."""
+    offsets, ids, values = [0], [], []
+    for r, m in enumerate(per_row):
+        for t, b in m.items():
+            if isinstance(t, bool) or not isinstance(t, numbers.Integral) or not 0 <= t < vocab:
+                raise B200Error(f"logit_bias_csr: row {r}: token id {t!r} outside [0, {vocab})")
+            if isinstance(b, bool) or not isinstance(b, numbers.Real) or math.isnan(b):
+                raise B200Error(f"logit_bias_csr: row {r}: bias {b!r} of token {t} is not a number")
+            ids.append(int(t))
+            values.append(float(b))
+        offsets.append(len(ids))
+    return (torch.tensor(offsets, dtype=torch.int32), torch.tensor(ids, dtype=torch.int32),
+            torch.tensor(values, dtype=torch.float32))
 
 
 # ------------------------------------------------------------------------------------------------ decode programs

@@ -200,9 +200,10 @@ def bench_logprobs(B, top_n, V=128256, nrot=8):
     return us
 
 
-def bench_sample(B, top_k, top_p, V=128256, nrot=4, copy_only=False):
-    """b200_sample on fp32 logits [B, V] at temperature 0.8 with every row's top_k / top_p. The op works in place, so each call
-    first copies fresh logits into its buffer (rotated through nrot sources); copy_only times that copy alone."""
+def bench_sample(B, top_k, top_p, V=128256, nrot=4, copy_only=False, min_p=None):
+    """b200_sample on fp32 logits [B, V] at temperature 0.8 with every row's top_k / top_p (and min_p when given). The op works
+    in place, so each call first copies fresh logits into its buffer (rotated through nrot sources); copy_only times that copy
+    alone."""
     g = torch.Generator(device=dev).manual_seed(3)
     src = [torch.randn(B, V, generator=g, device=dev) * 3 for _ in range(nrot)]
     x = torch.empty(B, V, device=dev)
@@ -211,14 +212,47 @@ def bench_sample(B, top_k, top_p, V=128256, nrot=4, copy_only=False):
     t = torch.full((B,), 0.8, device=dev)
     u = torch.rand(B, generator=g, device=dev)
     out = dict(token=torch.empty(B, dtype=torch.int32, device=dev), token_prob=torch.empty(B, device=dev))
+    mp = None if min_p is None else torch.full((B,), min_p, device=dev)
 
     def fn(i):
         x.copy_(src[i])
         if not copy_only:
-            ops.sample(x, k, p, u, temperature=t, out=out)
+            ops.sample(x, k, p, u, temperature=t, out=out, min_p=mp)
     us = timeit(fn, nrot)
-    what = "copy alone" if copy_only else f"copy + sample top_k {top_k} top_p {top_p}"
+    what = "copy alone" if copy_only else f"copy + sample top_k {top_k} top_p {top_p}" + ("" if min_p is None else f" min_p {min_p}")
     print(f"sample B{B} V{V} {what}: {us:8.1f} us", flush=True)
+    return us
+
+
+def bench_constrain(rows, V, mask, bias, dtype=torch.float16):
+    """b200_constrain_logits on logits [rows, V] (rotated through > L2 of sets) with an all-ones ("ones"), a 50 % random
+    ("half") or a single-token ("single") mask, and 0 or `bias` entries per row on random tokens. Bytes = the mask words read,
+    the masked logits written, and per bias entry its id and value read and its logit read and written when it is allowed."""
+    g = torch.Generator(device=dev).manual_seed(4)
+    es = torch.finfo(dtype).bits // 8
+    nrot = max(2, int(200e6 // (rows * V * es)) + 1)
+    xs = [torch.randn(rows, V, generator=g, device=dev).to(dtype) for _ in range(nrot)]
+    words = (V + 31) // 32
+    if mask == "ones":
+        ok = torch.ones(rows, words * 32, dtype=torch.bool, device=dev)
+    elif mask == "half":
+        ok = torch.rand(rows, words * 32, generator=g, device=dev) < 0.5
+    else:
+        ok = torch.zeros(rows, words * 32, dtype=torch.bool, device=dev)
+        ok[torch.arange(rows, device=dev), torch.randint(0, V, (rows,), generator=g, device=dev)] = True
+    ok[:, V:] = False
+    m = (ok.view(rows, words, 32).to(torch.int64) << torch.arange(32, device=dev)).sum(-1)
+    m = torch.where(m >= 2 ** 31, m - 2 ** 32, m).to(torch.int32)
+    lb = None
+    byt = rows * words * 4 + int((~ok[:, :V]).sum()) * es
+    if bias:
+        ids = torch.stack([torch.randperm(V, generator=g, device=dev)[:bias] for _ in range(rows)])
+        lb = (torch.arange(rows + 1, dtype=torch.int32, device=dev) * bias, ids.to(torch.int32).view(-1),
+              torch.randn(rows * bias, generator=g, device=dev))
+        byt += rows * bias * 8 + int(ok.gather(1, ids).sum()) * 2 * es
+    us = timeit(lambda i: ops.constrain_logits(xs[i], m, lb), nrot)
+    print(f"constrain {str(dtype)[6:]} rows {rows} V{V} mask {mask:6s} bias {bias:3d}/row: {us:7.2f} us  {byt / 1e6:7.3f} MB  "
+          f"{byt / us / 1e3:6.0f} GB/s", flush=True)
     return us
 
 
@@ -406,6 +440,25 @@ if __name__ == "__main__":
                 m = sorted(bench_sample(B, k, p) for _ in range(3))[1]
                 print(f"sample B{B} V128256 top_k {k} top_p {p} median: {m - c:.1f} us (copy + sample {m:.1f}, copy {c:.1f})",
                       flush=True)
+    if "sample-min-p" in which:
+        # b200_sample with and without a min_p buffer (top-p 0.9, min_p 0.05), alternating, minus the logit copy; medians of 3
+        for B in (8, 32):
+            c = sorted(bench_sample(B, 0, 1.0, copy_only=True) for _ in range(3))[1]
+            t = {m: [] for m in (None, 0.05)}
+            for _ in range(3):
+                for m in t:
+                    t[m].append(bench_sample(B, 0, 0.9, min_p=m))
+            off, on = sorted(t[None])[1] - c, sorted(t[0.05])[1] - c
+            print(f"sample B{B} V128256 top_p 0.9 median: min_p off {off:.1f} us, min_p 0.05 {on:.1f} us ({on - off:+.1f} us)",
+                  flush=True)
+    if "constrain" in which:
+        # the grammar mask and logit bias over Llama-3's and Qwen's vocabularies at B 32 / 128, fp16 logits; medians of 3
+        for V in (128256, 151936):
+            for rows in (32, 128):
+                for mask in ("ones", "half", "single"):
+                    for bias in (0, 300):
+                        m = sorted(bench_constrain(rows, V, mask, bias) for _ in range(3))[1]
+                        print(f"constrain rows {rows} V{V} mask {mask} bias {bias}/row median: {m:.2f} us", flush=True)
     if "rope" in which:
         # Llama-3 shape (Hq 32, Hkv 8, D 128) at B 32: the Base-only kernel against the full-contract kernel, 1 and 4 tokens
         for n in (1, 4):

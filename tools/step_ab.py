@@ -11,6 +11,8 @@ each a step captured in a CUDA graph with PDL at --ctx tokens; the first arm is 
   sample     Llama-3-8B INT4: greedy, then sampled (temperature 0.8, top-k 50, top-p 0.9, repetition 1.1, the drawn token's
              log-prob and the top 5)
   qwen3      Qwen3-8B INT4: qk_rmsnorm, then the plain rope launch (TwoLaunchStep), against the fused QK-norm append
+  constrain  Llama-3-8B INT4: greedy, greedy with a 50 % random token bitmask and 300 logit_bias entries per row, sampled
+             (temperature 0.8, top-k 50, top-p 0.9), sampled with the same constraints
 
 Every run visits the arms in turn. Per arm: restart the steps whose state advances (beam, sampled) from the prompt with
 upload_inputs(), replay --warmup times, restart again, then time --iters replays with CUDA events and synchronise. An
@@ -100,6 +102,33 @@ def sample_arms(a, cfg, B, dev):
                                            max_new_tokens=max_new_tokens(a)))]
 
 
+class ConstrainedStep(DecodeStep):
+    """A step that sets its A/B constraints (ab_constraints: set_constraints' arguments) again after every upload_inputs(),
+    which would otherwise reset it to unconstrained."""
+    ab_constraints = None
+
+    def upload_inputs(self):
+        super().upload_inputs()
+        if self.ab_constraints is not None:
+            self.set_constraints(*self.ab_constraints)
+
+
+def constrain_arms(a, cfg, B, dev):
+    sp = SamplingParams(temperature=0.8, top_k=50, top_p=0.9, seed=1)
+    arms = []
+    for name, kw in (("greedy", {}), ("sampled", dict(sampling=sp, max_new_tokens=max_new_tokens(a)))):
+        arms.append(step_arm(name, DecodeStep(cfg, B, a.ctx, dev, pdl=True, **kw)))
+        model = ConstrainedStep(cfg, B, a.ctx, dev, pdl=True, token_bitmask=True, logit_bias_capacity=300 * B, **kw)
+        g = torch.Generator().manual_seed(B)
+        mask = torch.randint(-2 ** 31, 2 ** 31, model.bitmask_h.shape, generator=g, dtype=torch.int64).to(torch.int32)
+        bias = [dict(zip(torch.randperm(model.vocab, generator=g)[:300].tolist(), torch.randn(300, generator=g).tolist()))
+                for _ in range(B)]
+        model.ab_constraints = (mask, bias)
+        model.upload_inputs()
+        arms.append(step_arm(f"{name} + constraints", model))
+    return arms
+
+
 def qwen3_arms(a, cfg, B, dev):
     return [step_arm("norm + rope", TwoLaunchStep(cfg, B, a.ctx, dev, pdl=True)),
             step_arm("fused", DecodeStep(cfg, B, a.ctx, dev, pdl=True))]
@@ -107,7 +136,8 @@ def qwen3_arms(a, cfg, B, dev):
 
 # name: arms, default batches, timed replays per run, warm-up replays
 PRESETS = {"act-order": (act_order_arms, [32], 100, 10), "spec": (spec_arms, [8, 16, 32], 50, 3),
-           "beam": (beam_arms, [8], 20, 3), "sample": (sample_arms, [8, 32], 20, 3), "qwen3": (qwen3_arms, [8, 16, 32], 100, 10)}
+           "beam": (beam_arms, [8], 20, 3), "sample": (sample_arms, [8, 32], 20, 3), "qwen3": (qwen3_arms, [8, 16, 32], 100, 10),
+           "constrain": (constrain_arms, [8, 32], 50, 5)}
 MODELS = {"llama3": LLAMA3_8B, "llama31": LLAMA31_8B}
 
 
