@@ -137,6 +137,20 @@ int b200_paged_decode_attn_beam(const void* q, int is_bf16, void* out, size_t he
                                 const void* kv_pool, const int32_t* page_list, const uint32_t* sequence_lengths,
                                 const int32_t* shared_lengths, float q_scale, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Verification of a speculative token TREE (EAGLE / Medusa drafts; TensorRT-LLM XQA's spec-decoding mask, restated: parity
+ * unpinned). The arguments of b200_paged_decode_attn_multi plus tree_parents [batch][q_len] int32 (device): the q_len new tokens of
+ * sequence b are nodes, node 0 the root (the last accepted token; its entry is not read), node j >= 1 under tree_parents[b][j] in
+ * [0, j). Node j's K/V sit at slot sequence_lengths[b] + j. Query j attends to positions 0 .. sequence_lengths[b] - 1 and to the
+ * slots of the nodes on its ancestor walk: j, its parent, ... up to the root or to a parent outside [0, i), which ends the walk.
+ * No value of tree_parents reads outside its row. A chain (parents[j] = j - 1) gives the bits of b200_paged_decode_attn_multi.
+ * A new token outside a query's ancestors never changes that query's bits, even when its K/V hold NaN or inf: its non-finite V
+ * elements are read as 0, and a query whose ancestors hold one gets a NaN output row. Same limits and workspace sizing as
+ * b200_paged_decode_attn_multi. */
+int b200_paged_decode_attn_tree(const void* q, int is_bf16, void* out, size_t head_num, size_t kv_head_num, size_t head_dim,
+                                size_t batch, size_t q_len, size_t max_blocks_per_seq, size_t max_seq_len, size_t page_size,
+                                const void* kv_pool, const int32_t* page_list, const uint32_t* sequence_lengths,
+                                const int32_t* tree_parents, float q_scale, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------------ weight-only GEMM */
 
 /* Load-time weight re-layout.  Replace CudaImpl.preprocess_weights_for_mixed_gemm (rtp_llm/device/device_impl.py:392-479):
@@ -294,6 +308,35 @@ int b200_sample(float* logits, int rows, int vocab, const int32_t* history, cons
  *   randomness. One CTA per sequence. */
 int b200_spec_verify(const float* target_probs, const int32_t* target_ids, const float* draft_probs, const int32_t* draft_tokens,
                      const float* uniform, int batch, int num_draft, int vocab, int32_t* out_tokens, int32_t* accepted, void* stream);
+
+/* Verification of a speculative token tree of n <= 64 nodes per sequence (the tree of b200_paged_decode_attn_tree), after a step
+ * over its batch*n rows; b200_spec_verify is the case of a chain, and the two share one kernel.
+ *   tree_parents [batch][n] (node 0 the root, node c >= 1 under parents[c] in [0, c); a child with a parent outside that range
+ *   is never reached), node_tokens [batch][n] (node c's draft token; entry 0 is not read), uniform [batch][n].
+ * The walk starts at the root and tries the current node's children in index order.
+ * Greedy (target_probs == NULL): move to the first child whose token equals target_ids[cur]; at none, emit target_ids[cur].
+ * Sampling (deterministic drafts, multi-round rejection after SpecInfer / EAGLE): with t = target_probs[cur], child c with token x
+ *   is accepted iff uniform[c - 1] * (1 - S) < r(x) in fp32, where r is t with the tokens of the siblings rejected before c
+ *   zeroed (a duplicate sibling token has mass 0) and S is the fp32 sum of r over those rejections. With every child rejected the
+ *   token is drawn from max(0, t - 1) on the rejected tokens and t elsewhere (from t when that has no mass); at a leaf the bonus
+ *   token is drawn from t; both with uniform[n - 1] as b200_spec_verify draws.
+ * Outputs: out_tokens [batch][n] the path's tokens at depths 1..a, then the correction or bonus token, then -1; accepted [batch]
+ * = a; accepted_path [batch][n] the node at depths 0..a (path[0] = 0), then -1. On a chain every output equals b200_spec_verify's
+ * (with out_tokens of n = num_draft + 1 entries). */
+int b200_spec_verify_tree(const float* target_probs, const int32_t* target_ids, const int32_t* tree_parents, const int32_t* node_tokens,
+                          const float* uniform, int batch, int n, int vocab, int32_t* out_tokens, int32_t* accepted,
+                          int32_t* accepted_path, void* stream);
+
+/* After b200_spec_verify_tree: the accepted path's K/V moved to consecutive cache slots. For d = 1 .. accepted[b] with
+ * path[d] != d (path = accepted_path [batch][n]), the K and V of slot sequence_lengths[b] + path[d] are bit-copied to slot
+ * sequence_lengths[b] + d in every layer and kv head; no other slot is written. Copies go in increasing d, each read before any
+ * later write (path [0, 2, 3] reads slot 2 before writing it). kv_pools: a HOST array of `layers` <= 128 per-layer pools
+ * [pages][kv_head_num][page_size][head_dim] of 16-bit elements, copied at the call; page_list [batch][2][max_blocks_per_seq] as
+ * for attention; sequence_lengths [batch] tokens cached before the step's nodes. accepted is clamped to [0, n - 1], and a path
+ * entry outside [0, n) or a slot past the page table is skipped. One launch for all layers; under PDL it waits before reading. */
+int b200_kv_compact_path(void* const* kv_pools, int layers, int kv_head_num, int head_dim, int page_size, const int32_t* page_list,
+                         int max_blocks_per_seq, const int32_t* sequence_lengths, const int32_t* accepted_path, const int32_t* accepted,
+                         int batch, int n, void* stream);
 
 /* One beam-search step over the lm_head logits of `batch` requests x W = beam_width beams. The semantics are restated from the
  * Hugging Face / TensorRT-LLM beam-search convention; the reference's vendored kernels (3rdparty/trt_beam_search) are not in

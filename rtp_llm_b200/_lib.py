@@ -31,6 +31,8 @@ SIGNATURES = {
                                             c_float, c_float, c_void_p, c_size_t, c_void_p]),
     "b200_paged_decode_attn_beam": (c_int, [c_void_p, c_int, c_void_p] + [c_size_t] * 8 + [c_void_p, c_void_p, c_void_p, c_void_p,
                                             c_float, c_void_p, c_size_t, c_void_p]),
+    "b200_paged_decode_attn_tree": (c_int, [c_void_p, c_int, c_void_p] + [c_size_t] * 8 + [c_void_p, c_void_p, c_void_p, c_void_p,
+                                            c_float, c_void_p, c_size_t, c_void_p]),
     "b200_wo_gemm_packed_bytes": (c_size_t, [c_int, c_int, c_int]),
     "b200_pack_w4": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "b200_pack_w8": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
@@ -55,6 +57,8 @@ SIGNATURES = {
     "b200_argmax": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "b200_sample": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int] + [c_void_p] * 14),
     "b200_spec_verify": (c_int, [c_void_p] * 5 + [c_int] * 3 + [c_void_p] * 3),
+    "b200_spec_verify_tree": (c_int, [c_void_p] * 5 + [c_int] * 3 + [c_void_p] * 4),
+    "b200_kv_compact_path": (c_int, [c_void_p] + [c_int] * 4 + [c_void_p, c_int] + [c_void_p] * 3 + [c_int, c_int, c_void_p]),
     "b200_beam_search_step_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "b200_beam_search_step": (c_int, [c_void_p, c_int, c_void_p] + [c_int] * 4 + [c_void_p] * 7 + [c_size_t, c_void_p]),
     "b200_beam_hypotheses_state_bytes": (c_size_t, [c_int, c_int, c_int]),

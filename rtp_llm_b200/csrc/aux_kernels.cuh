@@ -453,6 +453,45 @@ static __global__ void permute_cols_kernel(const uint16_t* __restrict__ x, const
     }
 }
 
+// The accepted path of a token-tree verification step moved to consecutive cache slots: for d = 1 .. accepted[b] with
+// path[d] != d, the K and V of slot seq + path[d] are bit-copied to slot seq + d, in every layer and kv head; no other slot is
+// written. A path is increasing (a node's index exceeds its parent's), so path[d] >= d: copy d reads a slot that only a later
+// copy (d' = path[d]) writes, and never one an earlier copy wrote. One thread owns the same 16 bytes of every slot of its
+// (sequence, layer, kv head) and copies in increasing d, so each read precedes the write that could clobber it. Entries a caller
+// could get wrong are checked: accepted is clamped to [0, n - 1], a path entry outside [0, n) or a slot past the page table is
+// skipped. Grid (B, Hkv, layers), D / 4 threads (K then V, 16 bytes each).
+constexpr int kCompactMaxLayers = 128;
+struct KvCompactParams {
+    void* pools[kCompactMaxLayers];   // per layer [pages][Hkv][page_size][D], 16-bit elements
+    const int32_t* page_list;         // [B][2][max_blocks]
+    const int32_t* seq_lens;          // [B] tokens cached before the step's nodes
+    const int32_t* path;              // [B][n]
+    const int32_t* accepted;          // [B]
+    int kv_head_num, head_dim, page_size, max_blocks, n;
+};
+
+static __global__ void kv_compact_path_kernel(const __grid_constant__ KvCompactParams p) {
+    pdl_launch_dependents();
+    pdl_wait();                       // the path and the K/V come from the kernels before this one
+    const int b = blockIdx.x, kvh = blockIdx.y, layer = blockIdx.z;
+    const int chunks = p.head_dim / 8, is_v = (int)threadIdx.x >= chunks, ch = threadIdx.x - is_v * chunks;
+    const int seq = p.seq_lens[b], cap = p.max_blocks * p.page_size;
+    const int acc = min(max(p.accepted[b], 0), p.n - 1);
+    const int32_t* path = p.path + (size_t)b * p.n;
+    const int32_t* pages = p.page_list + ((size_t)b * 2 + is_v) * p.max_blocks;
+    uint4* pool = reinterpret_cast<uint4*>(p.pools[layer]);
+    const size_t page_chunks = (size_t)p.kv_head_num * p.page_size * chunks;
+    auto slot = [&](int pos) {
+        return pool + (size_t)pages[pos / p.page_size] * page_chunks + ((size_t)kvh * p.page_size + pos % p.page_size) * chunks + ch;
+    };
+    if (seq < 0) return;
+    for (int d = 1; d <= acc; ++d) {
+        const int src = path[d];
+        if (src == d || src < 0 || src >= p.n || (long long)seq + max(src, d) >= cap) continue;
+        *slot(seq + d) = *slot(seq + src);
+    }
+}
+
 // token embedding gather: out[b][:] = table[ids[b]][:]
 template <typename T>
 __global__ void embedding_kernel(const int32_t* __restrict__ ids, const T* __restrict__ table, T* __restrict__ out,

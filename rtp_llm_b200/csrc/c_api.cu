@@ -409,10 +409,11 @@ size_t b200_paged_decode_attn_workspace_bytes(size_t batch, size_t head_num, siz
 
 // beam_width > 0: the beam instance. `batch` then counts requests, each with beam_width sequences (rows of q, out, page_list and
 // sequence_lengths), and shared_lengths [batch] says how much of a request's K/V its beams share; q_len is 1.
+// tree_parents != null: the tree instance, parents [batch][q_len] of each sequence's q_len new tokens.
 static int attn_impl(const void* q, const void* qkv, float rope_base, int q_len, int is_bf16, void* out, size_t head_num, size_t kv_head_num,
                      size_t head_dim, size_t batch, size_t max_blocks_per_seq, size_t max_seq_len, size_t page_size, const void* kv_pool,
                      const int32_t* page_list, const uint32_t* sequence_lengths, float q_scale, void* workspace, size_t workspace_bytes,
-                     void* stream, int beam_width = 0, const int32_t* shared_lengths = nullptr) {
+                     void* stream, int beam_width = 0, const int32_t* shared_lengths = nullptr, const int32_t* tree_parents = nullptr) {
     if (batch == 0) return B200_OK;
     ARG_CHECK((q || qkv) && out && kv_pool && page_list && sequence_lengths, "paged_decode_attn: null pointer");
     ARG_CHECK(head_dim == 64 || head_dim == 128 || head_dim == 256, "paged_decode_attn: head_dim %zu unsupported (64 / 128 / 256)", head_dim);
@@ -482,22 +483,33 @@ static int attn_impl(const void* q, const void* qkv, float rope_base, int q_len,
     const dim3 grid(p.nsplit, (unsigned)(batch * kv_head_num), 1);
     p.cluster_merge = (p.nsplit >= 2 && p.nsplit <= 8) ? 1 : 0;   // 2..8 splits merge in a cluster, more through the workspace
     const dim3 cluster(p.cluster_merge ? p.nsplit : 1);
-    auto launch = [&](auto t, auto hd, auto rt, auto beam) {
-        constexpr auto kern = paged_decode_attn_kernel<decltype(t), decltype(hd)::value, decltype(rt)::value, decltype(beam)::value>;
+    auto launch = [&](auto t, auto hd, auto rt, auto beam, auto tree) {
+        constexpr auto kern = paged_decode_attn_kernel<decltype(t), decltype(hd)::value, decltype(rt)::value, decltype(beam)::value,
+                                                       decltype(tree)::value>;
         const int smem = attn_smem_bytes(decltype(hd)::value);
         int rc = configure_once<kern>(smem);
         if (rc) return rc;
-        // (launch_ex converts p to the kernel's parameter type: the plain instances take its AttnParams part)
-        return launch_or_record("paged_decode_attn_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
-            return launch_ex(kern, {grid, dim3(kAttnThreads), (size_t)smem, s, pdl, cluster}, map, p);
-        });
+        if constexpr (decltype(tree)::value) {
+            AttnTreeParams pt{};
+            static_cast<AttnParams&>(pt) = p;
+            pt.tree_parents = tree_parents;
+            return launch_or_record("paged_decode_attn_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+                return launch_ex(kern, {grid, dim3(kAttnThreads), (size_t)smem, s, pdl, cluster}, map, pt);
+            });
+        } else {
+            // (launch_ex converts p to the kernel's parameter type: the plain instances take its AttnParams part)
+            return launch_or_record("paged_decode_attn_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+                return launch_ex(kern, {grid, dim3(kAttnThreads), (size_t)smem, s, pdl, cluster}, map, p);
+            });
+        }
     };
     // query rows in 16-row tiles: 1, 2 or 4 per (sequence or request, kv head)
     const int rows = group * slots;
     auto by_rows = [&](auto t, auto hd) {
         auto by_beam = [&](auto rt) {
-            if (beam_width) return launch(t, hd, rt, std::true_type());
-            return launch(t, hd, rt, std::false_type());
+            if (beam_width) return launch(t, hd, rt, std::true_type(), std::false_type());
+            if (tree_parents) return launch(t, hd, rt, std::false_type(), std::true_type());
+            return launch(t, hd, rt, std::false_type(), std::false_type());
         };
         if (rows <= 16) return by_beam(std::integral_constant<int, 1>());
         if (rows <= 32) return by_beam(std::integral_constant<int, 2>());
@@ -550,6 +562,17 @@ int b200_paged_decode_attn_beam(const void* q, int is_bf16, void* out, size_t he
     return attn_impl(q, nullptr, 0.f, 1, is_bf16, out, head_num, kv_head_num, head_dim, requests, max_blocks_per_seq, max_seq_len,
                      page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, stream, (int)beam_width,
                      shared_lengths);
+}
+
+int b200_paged_decode_attn_tree(const void* q, int is_bf16, void* out, size_t head_num, size_t kv_head_num, size_t head_dim,
+                                size_t batch, size_t q_len, size_t max_blocks_per_seq, size_t max_seq_len, size_t page_size,
+                                const void* kv_pool, const int32_t* page_list, const uint32_t* sequence_lengths,
+                                const int32_t* tree_parents, float q_scale, void* workspace, size_t workspace_bytes, void* stream) {
+    ARG_CHECK((q && tree_parents) || batch == 0, "paged_decode_attn_tree: null pointer (q or tree_parents)");
+    ARG_CHECK(q_len >= 1 && q_len <= (size_t)kAttnMaxRows, "paged_decode_attn_tree: q_len %zu unsupported (1..%d)", q_len, kAttnMaxRows);
+    return attn_impl(q, nullptr, 0.f, (int)q_len, is_bf16, out, head_num, kv_head_num, head_dim, batch, max_blocks_per_seq, max_seq_len,
+                     page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, stream, 0, nullptr,
+                     tree_parents);
 }
 
 // ------------------------------------------------------------------------------------------------ GEMM
@@ -1018,10 +1041,69 @@ int b200_spec_verify(const float* target_probs, const int32_t* target_ids, const
     p.uniform = uniform;
     p.out_tokens = out_tokens;
     p.accepted = accepted;
-    p.num_draft = num_draft;
+    p.num_nodes = num_draft + 1;
     p.vocab = vocab;
     return launch_or_record("spec_verify_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
         return launch_ex(spec_verify_kernel, {dim3(batch), dim3(kSampleThreads), 0, s, pdl}, p);
+    });
+}
+
+int b200_spec_verify_tree(const float* target_probs, const int32_t* target_ids, const int32_t* tree_parents, const int32_t* node_tokens,
+                          const float* uniform, int batch, int n, int vocab, int32_t* out_tokens, int32_t* accepted,
+                          int32_t* accepted_path, void* stream) {
+    ARG_CHECK(batch >= 0 && batch <= 65535, "spec_verify_tree: batch %d unsupported (0..65535)", batch);
+    ARG_CHECK(n >= 1 && n <= kSpecTreeMaxNodes, "spec_verify_tree: n %d unsupported (1..%d)", n, kSpecTreeMaxNodes);
+    ARG_CHECK(vocab > 0, "spec_verify_tree: vocab must be positive");
+    if (batch == 0) return B200_OK;
+    ARG_CHECK(tree_parents && node_tokens && out_tokens && accepted && accepted_path, "spec_verify_tree: null pointer");
+    ARG_CHECK(target_probs || target_ids, "spec_verify_tree: need target_probs (sampling) or target_ids (greedy)");
+    ARG_CHECK(!target_probs || uniform, "spec_verify_tree: sampling mode needs uniform");
+    SpecVerifyParams p{};
+    p.target_probs = target_probs;
+    p.target_ids = target_ids;
+    p.draft_tokens = node_tokens;
+    p.parents = tree_parents;
+    p.uniform = uniform;
+    p.out_tokens = out_tokens;
+    p.accepted = accepted;
+    p.accepted_path = accepted_path;
+    p.num_nodes = n;
+    p.vocab = vocab;
+    return launch_or_record("spec_verify_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+        return launch_ex(spec_verify_kernel, {dim3(batch), dim3(kSampleThreads), 0, s, pdl}, p);
+    });
+}
+
+int b200_kv_compact_path(void* const* kv_pools, int layers, int kv_head_num, int head_dim, int page_size, const int32_t* page_list,
+                         int max_blocks_per_seq, const int32_t* sequence_lengths, const int32_t* accepted_path, const int32_t* accepted,
+                         int batch, int n, void* stream) {
+    ARG_CHECK(layers >= 1 && layers <= kCompactMaxLayers, "kv_compact_path: layers %d unsupported (1..%d)", layers, kCompactMaxLayers);
+    ARG_CHECK(kv_head_num >= 1 && kv_head_num <= 65535, "kv_compact_path: kv_head_num %d unsupported (1..65535)", kv_head_num);
+    ARG_CHECK(head_dim == 64 || head_dim == 128 || head_dim == 256, "kv_compact_path: head_dim %d unsupported (64 / 128 / 256)", head_dim);
+    ARG_CHECK(page_size >= 1 && max_blocks_per_seq >= 1, "kv_compact_path: page_size and max_blocks_per_seq must be positive");
+    ARG_CHECK((long long)page_size * max_blocks_per_seq <= 0x7fffffffLL, "kv_compact_path: page table capacity exceeds 2^31 - 1");
+    ARG_CHECK(n >= 1 && n <= kSpecTreeMaxNodes, "kv_compact_path: n %d unsupported (1..%d)", n, kSpecTreeMaxNodes);
+    ARG_CHECK(batch >= 0, "kv_compact_path: batch %d must be >= 0", batch);
+    if (batch == 0) return B200_OK;
+    ARG_CHECK(kv_pools && page_list && sequence_lengths && accepted_path && accepted, "kv_compact_path: null pointer");
+    KvCompactParams p{};
+    for (int l = 0; l < layers; ++l) {
+        ARG_CHECK(kv_pools[l], "kv_compact_path: pool of layer %d is null", l);
+        ARG_CHECK(((uintptr_t)kv_pools[l] & 15) == 0, "kv_compact_path: pool of layer %d is not 16-byte aligned", l);
+        p.pools[l] = kv_pools[l];
+    }
+    p.page_list = page_list;
+    p.seq_lens = sequence_lengths;
+    p.path = accepted_path;
+    p.accepted = accepted;
+    p.kv_head_num = kv_head_num;
+    p.head_dim = head_dim;
+    p.page_size = page_size;
+    p.max_blocks = max_blocks_per_seq;
+    p.n = n;
+    const dim3 grid(batch, kv_head_num, layers);
+    return launch_or_record("kv_compact_path_kernel", stream, [=, pdl = g_pdl.load() != 0](cudaStream_t s) {
+        return launch_ex(kv_compact_path_kernel, {grid, dim3(head_dim / 4), 0, s, pdl}, p);
     });
 }
 

@@ -75,20 +75,34 @@ struct AttnBeamParams : AttnParams {
                                   // 64-token tiles below the shortest beam's cached length, so a wrong value can only cost sharing.
 };
 
+// The tree instance's parameters (a speculative token tree, XQA's spec-decoding mask in TensorRT-LLM). The q_len new tokens of
+// sequence b are the nodes of a tree: parents [B][q_len], node 0 the root, node j >= 1 under parents[b][j] in [0, j). Query j
+// attends to positions 0 .. seq_lens[b] - 1 and to the slots seq_lens[b] + i of the nodes i on its ancestor walk (itself, its
+// parent, ... until the root or a parent outside [0, i)). A chain (parents[j] = j - 1) is the causal q_len instance.
+struct AttnTreeParams : AttnParams {
+    const int32_t* tree_parents;
+};
+
 // RT: 16-row tiles of query rows (rows = group * q_len rounded up to 16 / 32 / 64)
 // BEAM: a request's beams in one CTA. Tile t below the shared length is one pipeline stage, loaded once through beam 0's pages with
 // every row live; a tile from there on is one stage per beam that reaches it, in beam order, each loaded through that beam's pages
 // and masked to that beam's rows. A row so meets the tiles of its own sequence in order with the arithmetic of the plain instance;
 // another beam's stage leaves its (m, l, O) bit for bit as they were.
-template <typename T, int D = kAttnD, int RT = 1, bool BEAM = false>
+// TREE: the q_len instance with each query's new-token columns masked to its ancestors. The ancestor sets are 64-bit masks built
+// once per CTA in shared memory. A 16-token slice wholly below seq_lens[b] runs the plain instance's code; a slice that reaches
+// the new tokens also tests the mask and reads the new tokens' non-finite V elements as 0, so a node outside a row's ancestors
+// never changes that row's bits (p = 0 does not stop 0 * NaN in the mma). A row whose ancestors hold such an element ends NaN.
+template <typename T, int D = kAttnD, int RT = 1, bool BEAM = false, bool TREE = false>
 __global__ void __launch_bounds__(kAttnThreads, D <= 128 ? 2 : 1)
-paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const std::conditional_t<BEAM, AttnBeamParams, AttnParams> p) {
+paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map,
+                         const std::conditional_t<BEAM, AttnBeamParams, std::conditional_t<TREE, AttnTreeParams, AttnParams>> p) {
     constexpr int NH = D / 64;                       // 64-channel halves per K / V row
     constexpr int STAGE = attn_stage_bytes(D);
     constexpr int OROW = D + 8;                      // floats; +8 banks per row -> conflict-free float2 stores
     constexpr int NW = kAttnConsumerWarps / RT;      // warps per row tile (each takes RT of a stage's 4 slices)
     static_assert(D == 64 || D == 128 || D == 256, "head_dim 64 / 128 / 256");
     static_assert(RT == 1 || RT == 2 || RT == 4, "1, 2 or 4 row tiles");
+    static_assert(!(BEAM && TREE), "a beam step has one query token");
     // the merge staging (per-warp o / m / l, then the cluster partial [rows][D] + (m, l)) reuses the K/V ring
     static_assert((kAttnConsumerWarps * 16 * (OROW + 2) + RT * 16 * (D + 2)) * 4 <= kAttnStages * STAGE,
                   "merge staging exceeds the K/V ring");
@@ -153,6 +167,22 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const std::
         }
         fence_mbar_init();
     }
+    // TREE: node j's ancestor set (bit i = node i, j's own bit included), in the fused rope's table (the tree instance has no rope)
+    uint64_t* s_anc = reinterpret_cast<uint64_t*>(cs_tab);
+    if constexpr (TREE) {
+        const int j = threadIdx.x;
+        if (j < p.q_len) {
+            const int32_t* par = p.tree_parents + (size_t)b * p.q_len;
+            uint64_t m = 1ull << j;
+            for (int i = j; i > 0;) {        // a parent outside [0, i) ends the walk: at most j steps, every read inside the row
+                const int pi = par[i];
+                if (pi < 0 || pi >= i) break;
+                m |= 1ull << pi;
+                i = pi;
+            }
+            s_anc[j] = m;
+        }
+    }
     __syncthreads();
 
     // BEAM: the stage sequence, derived alike by the producer and the consumers. live_from: the first beam >= from with a stage
@@ -216,7 +246,7 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const std::
         int first_end = t1;                               // tiles [t0, first_end) are issued before the append
         bool own = false;
         int pos = 0;
-        if (!BEAM && D == 128 && RT == 1 && p.qkv != nullptr) {   // fused rope: head_dim 128, one row tile (the host rejects others)
+        if (!BEAM && !TREE && D == 128 && RT == 1 && p.qkv != nullptr) {   // fused rope: head_dim 128, one row tile (the host rejects others)
             pos = p.seq_lens[b];
             own = pos < len && (pos / kAttnTile) >= t0 && (pos / kAttnTile) < t1;      // this CTA streams the new token's tile
             if (own) first_end = min(min(t0 + kAttnStages, t1), pos / kAttnTile);
@@ -275,7 +305,7 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const std::
     // Q fragments for the whole head dim: 8 k-steps x 4 regs. Rows >= group are zero.
     uint32_t qf[D / 16][4];
     bool q_loaded = false;
-    if constexpr (D == 128 && RT == 1 && !BEAM) {
+    if constexpr (D == 128 && RT == 1 && !BEAM && !TREE) {
       if (p.qkv) {
         q_loaded = true;
         // un-rotated q straight from the qkv GEMM output; the NeoX partner of column c < 64 is column c + 64 = the same
@@ -336,8 +366,11 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const std::
     float m0 = -INFINITY, m1 = -INFINITY;  // running max (raw score units) for rows qrow / qrow+8
     float l0 = 0.f, l1 = 0.f;              // per-thread partial row sums (quad-reduced at the end)
     const float sl2 = p.scale_log2;
-    int off0 = 0, off1 = 0;   // (BEAM: one query token per beam)
-    if constexpr (!BEAM) {
+    int off0 = 0, off1 = 0;   // (BEAM: one query token per beam; TREE: the ancestor masks stand for the causal offsets)
+    int tree_base = 0;        // TREE: seq_lens[b], the position of node 0
+    bool pois0 = false, pois1 = false;   // TREE: the row attends to a new token's non-finite V element
+    if constexpr (TREE) tree_base = p.seq_lens[b];
+    if constexpr (!BEAM && !TREE) {
         off0 = p.q_len - 1 - min(row0 / p.group, p.q_len - 1);
         off1 = p.q_len - 1 - min(row1 / p.group, p.q_len - 1);
     }
@@ -424,12 +457,26 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const std::
             if (!keep0) lim0 = 0;
             if (!keep1) lim1 = 0;
         }
+        // TREE: bit c of vis = column c of the slice is visible to the row (column c is new token rel + c, cached when < 0)
+        const int rel = tok0 - tree_base;
+        const bool tail = TREE && rel > -16 && rel < kAttnMaxRows;   // the slice reaches the new tokens
+        uint32_t vis0 = 0xffffu, vis1 = 0xffffu;
+        if constexpr (TREE) if (tail) {
+            const uint64_t a0 = s_anc[min(row0 / p.group, p.q_len - 1)], a1 = s_anc[min(row1 / p.group, p.q_len - 1)];
+            const uint64_t below = rel < 0 ? (1ull << -rel) - 1 : 0ull;
+            vis0 = (uint32_t)((rel >= 0 ? a0 >> rel : (a0 << -rel) | below) & 0xffffu);
+            vis1 = (uint32_t)((rel >= 0 ? a1 >> rel : (a1 << -rel) | below) & 0xffffu);
+        }
 #pragma unroll
         for (int j = 0; j < 2; ++j) {
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
                 // query j of a q_len-token step sees q_len - 1 - j fewer tokens than the last one (causal among the new tokens)
-                const bool ok0 = (j * 8 + qcol + e) < lim0, ok1 = (j * 8 + qcol + e) < lim1;
+                bool ok0 = (j * 8 + qcol + e) < lim0, ok1 = (j * 8 + qcol + e) < lim1;
+                if constexpr (TREE) {
+                    ok0 = ok0 && ((vis0 >> (j * 8 + qcol + e)) & 1u);
+                    ok1 = ok1 && ((vis1 >> (j * 8 + qcol + e)) & 1u);
+                }
                 sc[j][e] = ok0 ? sc[j][e] : -INFINITY;
                 sc[j][2 + e] = ok1 ? sc[j][2 + e] : -INFINITY;
                 mx0 = fmaxf(mx0, sc[j][e]);
@@ -482,6 +529,48 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const std::
         pf[3] = pack2<T>(sc[1][2], sc[1][3]);
 
         // ---- O += P V
+        if constexpr (TREE) {
+          // (two loops, so that a slice below the new tokens runs the plain loop without a branch between its loads and mmas)
+          if (tail) {
+            // register vb[r] holds slice tokens (r & 1) * 8 + 2 * (lane & 3) (low half) and + 1 (high half); newv[r & 1] selects the
+            // halves of new tokens, whose non-finite elements are read as 0 and recorded in `bad` (bit = slice token)
+            uint32_t newv[2], bad = 0u;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int t = h * 8 + 2 * (lane & 3);
+                newv[h] = (rel + t >= 0 ? 0x0000ffffu : 0u) | (rel + t + 1 >= 0 ? 0xffff0000u : 0u);
+            }
+            constexpr uint32_t E = std::is_same<T, __half>::value ? 0x7c00u : 0x7f80u;   // exponent all ones: inf / NaN
+#pragma unroll
+            for (int n2 = 0; n2 < D / 16; ++n2) {
+                const int half = n2 >> 2, c = (n2 & 3) * 2 + v_chunk_add;
+                uint32_t vb[4];
+                ldmatrix_x4_trans(vb, v_base + half * 8192 + v_tokrow * 128 + ((c ^ (v_tokrow & 7)) << 4));
+#pragma unroll
+                for (int r = 0; r < 4; ++r) {
+                    const uint32_t x = vb[r];
+                    const uint32_t nf = (((x & E) == E ? 0x0000ffffu : 0u) | (((x >> 16) & E) == E ? 0xffff0000u : 0u)) & newv[r & 1];
+                    const int t = (r & 1) * 8 + 2 * (lane & 3);
+                    bad |= ((nf & 0xffffu) ? 1u << t : 0u) | ((nf >> 16) ? 2u << t : 0u);
+                    vb[r] = x & ~nf;
+                }
+                mma_m16n8k16<T>(o[2 * n2], pf, vb[0], vb[1]);
+                mma_m16n8k16<T>(o[2 * n2 + 1], pf, vb[2], vb[3]);
+            }
+            bad = __reduce_or_sync(0xffffffffu, bad);
+            pois0 |= (bad & vis0) != 0u;
+            pois1 |= (bad & vis1) != 0u;
+          } else {
+#pragma unroll
+            for (int n2 = 0; n2 < D / 16; ++n2) {
+                const int half = n2 >> 2, c = (n2 & 3) * 2 + v_chunk_add;
+                uint32_t vb[4];
+                ldmatrix_x4_trans(vb, v_base + half * 8192 + v_tokrow * 128 + ((c ^ (v_tokrow & 7)) << 4));
+                mma_m16n8k16<T>(o[2 * n2], pf, vb[0], vb[1]);
+                mma_m16n8k16<T>(o[2 * n2 + 1], pf, vb[2], vb[3]);
+            }
+          }
+        } else {
 #pragma unroll
         for (int n2 = 0; n2 < D / 16; ++n2) {
             const int half = n2 >> 2, c = (n2 & 3) * 2 + v_chunk_add;
@@ -503,6 +592,7 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const std::
                 mma_m16n8k16<T>(o[2 * n2 + 1], pf, vb[2], vb[3]);
             }
         }
+        }
       }
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty_bar[s]);
@@ -514,6 +604,10 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map, const std::
     l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
     l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
     l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+    if constexpr (TREE) {   // (uniform over the quad: vis and bad are the row's and the warp's)
+        if (pois0) l0 = __int_as_float(0x7fffffff);
+        if (pois1) l1 = __int_as_float(0x7fffffff);
+    }
 
     // ---------------------------------------------------------------------- merge the NW warps of each row tile through smem
     asm volatile("bar.sync 1, 128;" ::: "memory");  // everyone is done reading the K/V ring

@@ -242,70 +242,136 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(const SamplePara
     }
 }
 
-// Verification of n = num_draft speculative tokens per sequence against the target model's rows of the same step
-// (the reference's speculative-sampling kernel, bindings/cuda/kernels/speculative_sampling/sampling.cu, chain form).
-// Greedy (target_probs == NULL): accept draft i while it equals target_ids[i]; emit target_ids[accepted].
-// Sampling: accept draft d_i iff uniform[i] * p(d_i) < q(d_i) (fp32; p = draft_probs, 1 for deterministic drafts), stop at the
-// first rejection and draw from the residual max(0, q - p) -- from q itself when the residual has no mass -- or, with every draft
-// accepted, the bonus token from the last row; both draws use uniform[n] and chunked_draw. One CTA of 1024 threads per sequence.
+// Verification of speculative tokens against the target model's rows of the same step (the reference's speculative-sampling
+// kernel, bindings/cuda/kernels/speculative_sampling/sampling.cu, and its tree form after SpecInfer / EAGLE). A sequence's N rows
+// are the nodes of a tree: node 0 the last accepted token, node c >= 1 a draft token under parent(c) in [0, c). A chain (no
+// parents given) is parent(c) = c - 1 with node c's token draft_tokens[c - 1]; a tree gives parents and node tokens [B][N].
+// The walk starts at the root and tries the current node's children in index order.
+// Greedy (target_probs == NULL): move to the first child whose token equals target_ids[cur]; at none, emit target_ids[cur].
+// Sampling: child c with token x is accepted iff uniform[c - 1] * p < r(x) (fp32). r is the row of cur with the tokens of the
+// siblings rejected before c zeroed, p = draft_probs (chain only) or 1 - S, S the fp32 sum of r over those rejections: the
+// multi-round rejection of several deterministic drafts, which on a chain (S = 0) is the one-draft test uniform * 1 < q. With
+// every child rejected the token is drawn from the residual max(0, q - p) -- q with the rejected tokens removed for
+// deterministic drafts, from q itself when the residual has no mass -- and at a leaf the bonus token from the leaf's row; both
+// draws use uniform[N - 1] and chunked_draw. One CTA of 1024 threads per sequence; every thread walks the same tree (the same
+// loads, the same fp32 compares), so the decisions are uniform.
+constexpr int kSpecTreeMaxNodes = 64;
 struct SpecVerifyParams {
-    const float* target_probs;    // optional [B][n+1][V]
-    const int32_t* target_ids;    // [B][n+1] (greedy mode)
-    const float* draft_probs;     // optional [B][n][V]
-    const int32_t* draft_tokens;  // [B][n]
-    const float* uniform;         // [B][n+1] (sampling mode)
-    int32_t* out_tokens;          // [B][n+1]: accepted drafts, one correction / bonus token, then -1
+    const float* target_probs;    // optional [B][N][V]
+    const int32_t* target_ids;    // [B][N] (greedy mode)
+    const float* draft_probs;     // optional [B][N-1][V] (chain only)
+    const int32_t* draft_tokens;  // chain: [B][N-1], node c's token at c - 1; tree: node tokens [B][N], entry 0 unread
+    const int32_t* parents;       // optional [B][N] (tree, N <= kSpecTreeMaxNodes); NULL: the chain
+    const float* uniform;         // [B][N] (sampling mode)
+    int32_t* out_tokens;          // [B][N]: accepted tokens, one correction / bonus token, then -1
     int32_t* accepted;            // [B]
-    int num_draft, vocab;
+    int32_t* accepted_path;       // optional [B][N]: the node at depth 0 .. accepted, then -1
+    int num_nodes, vocab;
 };
 
 __global__ void __launch_bounds__(kSampleThreads) spec_verify_kernel(const SpecVerifyParams p) {
     __shared__ float s_scan[kSampleThreads];
     __shared__ int s_pick, s_owner;
-    const int b = blockIdx.x, tid = threadIdx.x, n = p.num_draft, V = p.vocab;
+    __shared__ int s_path[kSpecTreeMaxNodes];   // tree: the accepted path (a chain's is the identity)
+    __shared__ int s_rej[kSpecTreeMaxNodes];    // the rejected children's tokens at the node the walk stopped at
+    const int b = blockIdx.x, tid = threadIdx.x, N = p.num_nodes, V = p.vocab;
     pdl_wait();                        // under PDL the target rows come from the kernels before this one
-    const int32_t* draft = p.draft_tokens + (size_t)b * n;
-    int acc = 0, tok;
+    const bool tree = p.parents != nullptr;
+    const int32_t* par = tree ? p.parents + (size_t)b * N : nullptr;
+    const int32_t* ntok = p.draft_tokens + (size_t)b * (tree ? N : N - 1);
+    auto token = [&](int c) { return tree ? ntok[c] : ntok[c - 1]; };
+    // the children of node cur are the c in (cur, N) with parent(c) == cur; a chain's only one is cur + 1
+    auto child_end = [&](int cur) { return tree ? N : min(cur + 2, N); };
+    auto is_child = [&](int c, int cur) { return !tree || par[c] == cur; };
+    int acc = 0, cur = 0, tok;
+    if (tid == 0 && tree) s_path[0] = 0;
+    auto step = [&](int c) {
+        cur = c;
+        ++acc;
+        if (tid == 0 && tree) s_path[acc] = c;
+    };
     if (!p.target_probs) {
-        const int32_t* ids = p.target_ids + (size_t)b * (n + 1);
-        while (acc < n && draft[acc] == ids[acc]) ++acc;
-        tok = ids[acc];
+        const int32_t* ids = p.target_ids + (size_t)b * N;
+        for (bool moved = true; moved;) {
+            moved = false;
+            for (int c = cur + 1; c < child_end(cur); ++c) {
+                if (is_child(c, cur) && token(c) == ids[cur]) {
+                    step(c);
+                    moved = true;
+                    break;
+                }
+            }
+        }
+        tok = ids[cur];
     } else {
-        const float* u = p.uniform + (size_t)b * (n + 1);
-        auto trow = [&](int i) { return p.target_probs + ((size_t)b * (n + 1) + i) * V; };
-        auto drow = [&](int i) { return p.draft_probs + ((size_t)b * n + i) * V; };
-        // every thread walks the same chain (the same loads, the same fp32 compares): a uniform decision
-        for (; acc < n; ++acc) {
-            const int d = draft[acc];
-            const bool in = d >= 0 && d < V;
-            const float q = in ? trow(acc)[d] : 0.f;
-            const float pd = p.draft_probs ? (in ? drow(acc)[d] : 0.f) : 1.f;
-            if (!(u[acc] * pd < q)) break;
+        const float* u = p.uniform + (size_t)b * N;
+        auto trow = [&](int i) { return p.target_probs + ((size_t)b * N + i) * V; };
+        auto drow = [&](int i) { return p.draft_probs + ((size_t)b * (N - 1) + i) * V; };
+        int last_rej = -1, nrej = 0;   // at the node the walk stops at: its last rejected child, and how many
+        for (bool moved = true; moved;) {
+            moved = false;
+            const float* t = trow(cur);
+            float S = 0.f;
+            last_rej = -1;
+            nrej = 0;
+            for (int c = cur + 1; c < child_end(cur); ++c) {
+                if (!is_child(c, cur)) continue;
+                const int d = token(c);
+                const bool in = d >= 0 && d < V;
+                bool seen = false;             // d is the token of a sibling rejected before c: r(d) = 0
+                for (int c2 = cur + 1; c2 < c; ++c2) seen |= is_child(c2, cur) && token(c2) == d;
+                const float q = in && !seen ? t[d] : 0.f;
+                const float pd = p.draft_probs ? (in ? drow(c - 1)[d] : 0.f) : 1.f - S;
+                if (u[c - 1] * pd < q) {
+                    step(c);
+                    moved = true;
+                    break;
+                }
+                S += q;
+                last_rej = c;
+                ++nrej;
+            }
         }
         float total;
-        if (acc < n) {
-            const float* t = trow(acc);
-            const int d = draft[acc];
+        const float* t = trow(cur);
+        if (last_rej >= 0) {
             if (p.draft_probs) {
-                const float* dp = drow(acc);
-                tok = chunked_draw([&](int x) { return fmaxf(0.f, t[x] - dp[x]); }, V, u[n], false, s_scan, &s_pick, &s_owner, &total);
+                const float* dp = drow(last_rej - 1);
+                tok = chunked_draw([&](int x) { return fmaxf(0.f, t[x] - dp[x]); }, V, u[N - 1], false, s_scan, &s_pick, &s_owner,
+                                   &total);
             } else {
-                tok = chunked_draw([&](int x) { return fmaxf(0.f, t[x] - (x == d ? 1.f : 0.f)); }, V, u[n], false, s_scan, &s_pick,
-                                   &s_owner, &total);
+                if (tid == 0) {
+                    int k = 0;
+                    for (int c = cur + 1; c < child_end(cur); ++c)
+                        if (is_child(c, cur)) s_rej[k++] = token(c);
+                }
+                __syncthreads();
+                auto rejected = [&](int x) {
+                    bool r = false;
+                    for (int k = 0; k < nrej; ++k) r |= x == s_rej[k];
+                    return r;
+                };
+                tok = chunked_draw([&](int x) { return fmaxf(0.f, t[x] - (rejected(x) ? 1.f : 0.f)); }, V, u[N - 1], false, s_scan,
+                                   &s_pick, &s_owner, &total);
             }
             if (!(total > 0.f)) {          // the residual has no mass (q <= p everywhere): draw from q
                 __syncthreads();           // every thread has read the first draw's shared result
-                tok = chunked_draw([&](int x) { return t[x] > 0.f ? t[x] : 0.f; }, V, u[n], false, s_scan, &s_pick, &s_owner, &total);
+                tok = chunked_draw([&](int x) { return t[x] > 0.f ? t[x] : 0.f; }, V, u[N - 1], false, s_scan, &s_pick, &s_owner,
+                                   &total);
             }
         } else {
-            const float* t = trow(n);
-            tok = chunked_draw([&](int x) { return t[x] > 0.f ? t[x] : 0.f; }, V, u[n], false, s_scan, &s_pick, &s_owner, &total);
+            tok = chunked_draw([&](int x) { return t[x] > 0.f ? t[x] : 0.f; }, V, u[N - 1], false, s_scan, &s_pick, &s_owner, &total);
         }
     }
     if (tid == 0) {
-        int32_t* out = p.out_tokens + (size_t)b * (n + 1);
-        for (int i = 0; i <= n; ++i) out[i] = i < acc ? draft[i] : (i == acc ? tok : -1);
+        auto path = [&](int i) { return tree ? s_path[i] : i; };
+        int32_t* out = p.out_tokens + (size_t)b * N;
+        for (int i = 0; i < N; ++i) out[i] = i < acc ? token(path(i + 1)) : (i == acc ? tok : -1);
         p.accepted[b] = acc;
+        if (p.accepted_path) {
+            int32_t* ap = p.accepted_path + (size_t)b * N;
+            for (int i = 0; i < N; ++i) ap[i] = i <= acc ? path(i) : -1;
+        }
     }
 }
 

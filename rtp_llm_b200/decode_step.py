@@ -198,6 +198,18 @@ class DecodeStep:
     would have to hold drafts 0..j-1. SamplingParams.min_p runs b200_sample with a min_p buffer when some value is not 0, and
     without one (today's kernel call) when every value is 0.
 
+    tree=parents (q_len = n >= 2 nodes, greedy or sampled verification; TP 1, op by op or under a CUDA graph, with or without
+    PDL; not in a decode program): verification of a speculative token tree. parents is one list of n entries for every request
+    or one per request (parents[0] = -1, node j under parents[j] < j); set_tree() replaces it between replays. ids_h [B, n] holds
+    the root (the last accepted token) and node j's draft token in column j. Node j's K/V go to slot seq + j and it is rotated at
+    position seq + depth(j): the positions are formed on the device from static parent / depth buffers and passed to
+    rope.rope_append as position_ids, so by the seams' rule even a plain Base config runs the _ex rope kernels there. The layers
+    call paged_decode_attn_tree; the ending is argmax (or b200_sample with probs_out) and spec_verify_tree, then one
+    kv_compact_path over every layer moves the accepted path's K/V to slots seq .. seq + accepted. Like the chain step it does
+    not advance; out_tokens [B, n], accepted [B] and accepted_path [B, n] hold the result, with one launch more than the chain
+    step (the compaction). Constraints apply per row (row j carries node j's mask); penalties and the n-gram ban are rejected
+    as for sampled chain verification.
+
     token_bitmask=True and / or logit_bias_capacity=n > 0 (TP 1, every mode): constrained decoding. Static device buffers,
     filled by set_constraints() from pinned host twins, hold one grammar bitmask row per logits row (int32 [R, ceil(V / 32)],
     xgrammar's layout) and a logit-bias CSR of up to n entries; a graph replay applies what was set last, and upload_inputs()
@@ -215,7 +227,7 @@ class DecodeStep:
                  logprobs: Optional[int] = None, eos_id: Optional[int] = None,
                  length_penalty: Union[float, Sequence[float]] = 1.0,
                  early_stopping: Union[bool, str, Sequence[Union[bool, str]]] = False,
-                 token_bitmask: bool = False, logit_bias_capacity: int = 0):
+                 token_bitmask: bool = False, logit_bias_capacity: int = 0, tree=None):
         assert cfg.head_num % tp_size == 0 and cfg.inter % tp_size == 0
         if logit_bias_capacity < 0:
             raise ValueError(f"logit_bias_capacity must be >= 0 (got {logit_bias_capacity})")
@@ -231,6 +243,8 @@ class DecodeStep:
         if q_len > 1 and (batch * q_len > 128 or tp_size != 1):
             raise ValueError(f"a verification step (q_len {q_len}) needs batch * q_len <= 128 (the GEMM row limit) and tp_size 1 "
                              f"(got batch {batch}, tp_size {tp_size})")
+        if tree is not None and q_len < 2:
+            raise ValueError(f"a token-tree step needs q_len >= 2 nodes (got q_len {q_len})")
         if not 1 <= beam_width <= 32:
             raise ValueError(f"beam_width must be in 1..32 (got {beam_width})")
         if beam_width > 1 and (batch * beam_width > 128 or tp_size != 1 or q_len != 1):
@@ -484,6 +498,14 @@ class DecodeStep:
             self.drafts = buf(batch, q_len - 1, dt=torch.int32)
             self.out_tokens = buf(batch, q_len, dt=torch.int32)
             self.accepted = buf(batch, dt=torch.int32)
+        if tree is not None:    # the token tree: parents and depths (pinned twins set_tree() fills), rotation positions, path
+            self.tree_parents_h = torch.zeros(batch, q_len, dtype=torch.int32).pin_memory()
+            self.tree_depth_h = torch.zeros(batch, q_len, dtype=torch.int32).pin_memory()
+            self.tree_parents = buf(batch, q_len, dt=torch.int32)
+            self.tree_depth = buf(batch, q_len, dt=torch.int32)
+            self.tree_pos = buf(R, dt=torch.int32)
+            self.accepted_path = buf(batch, q_len, dt=torch.int32)
+            self.accepted_path_h = torch.zeros(batch, q_len, dtype=torch.int32).pin_memory()
         if beam_width > 1:
             W, B = beam_width, self.requests
             self.beam_cum = buf(B, W, dt=torch.float32)
@@ -566,6 +588,8 @@ class DecodeStep:
         ops.set_pdl(pdl)
         self.graph: Optional[torch.cuda.CUDAGraph] = None
         self.prog = None
+        if tree is not None:
+            self.set_tree(tree)
         self.upload_inputs()
         torch.cuda.synchronize(device)
 
@@ -641,6 +665,29 @@ class DecodeStep:
             for d, h in zip(self.bias, self.bias_h):
                 d.copy_(h, non_blocking=True)
 
+    def set_tree(self, parents):
+        """The token tree the next step (or graph replay) verifies: one parent list for every request, or one per request, of
+        q_len entries (parents[0] = -1 for the root, 0 <= parents[j] < j). Fills the pinned twins of the static parent and depth
+        buffers and copies them non_blocking, like set_constraints(): call it between two replays."""
+        if self.tree_parents is None:
+            raise ValueError("set_tree: this step was built without tree=")
+        n, B = self.q_len, self.B
+        rows = [list(parents)] * B if len(parents) == 0 or not isinstance(parents[0], (list, tuple)) else [list(r) for r in parents]
+        if len(rows) != B:
+            raise ValueError(f"set_tree: {len(rows)} parent lists for {B} requests")
+        depth = []
+        for r in rows:
+            if len(r) != n or int(r[0]) != -1 or any(not 0 <= int(r[j]) < j for j in range(1, n)):
+                raise ValueError(f"set_tree: parents must hold {n} entries, -1 for the root and 0 <= parents[j] < j (got {r})")
+            d = [0] * n
+            for j in range(1, n):
+                d[j] = d[int(r[j])] + 1
+            depth.append(d)
+        self.tree_parents_h.copy_(torch.tensor(rows, dtype=torch.int32))
+        self.tree_depth_h.copy_(torch.tensor(depth, dtype=torch.int32))
+        self.tree_parents.copy_(self.tree_parents_h, non_blocking=True)
+        self.tree_depth.copy_(self.tree_depth_h, non_blocking=True)
+
     def _constrain(self, logits: torch.Tensor):
         """b200_constrain_logits on `logits` with the buffers set_constraints() filled (no launch when the step has none)."""
         if self.bitmask is not None or self.bias is not None:
@@ -648,6 +695,7 @@ class DecodeStep:
 
     sample_advances = False
     bitmask = bitmask_h = bias = bias_h = None     # no constraint buffers unless token_bitmask / logit_bias_capacity
+    tree_parents = None                             # no token tree unless tree=
 
     def _count_beam_step(self):
         if self.W > 1 or self.sample_advances:
@@ -660,6 +708,8 @@ class DecodeStep:
         if self.q_len > 1:
             self.out_tokens_h.copy_(self.out_tokens, non_blocking=True)
             self.accepted_h.copy_(self.accepted, non_blocking=True)
+            if self.tree_parents is not None:
+                self.accepted_path_h.copy_(self.accepted_path, non_blocking=True)
             return
         self.next_h.copy_(self.beam_out["next_token"].view(-1) if self.W > 1 else self.next_ids, non_blocking=True)
 
@@ -704,13 +754,17 @@ class DecodeStep:
         """q of the step's rows into self.q, their K/V into layer L's cache: rope.rope_append, with L's QK-norm when the config
         has one."""
         qk_norm = (L["q_norm"], L["k_norm"], self.cfg.eps) if self.cfg.qk_norm else None
+        pos = self.tree_pos if self.tree_parents is not None else None   # (tree mode: seq + depth, formed in step_core)
         rope.rope_append(self.rope_spec, self.qkv, L["kv"], self.page_list, self.seq_lens, self.Hq, q_out=self.q, q_len=self.q_len,
-                         qk_norm=qk_norm)
+                         qk_norm=qk_norm, position_ids=pos)
 
     def _attention(self, L):
         """self.attn = the attention of the step's rows over layer L's cache, after _rope_append. In beam mode a request's beams
         share one pass over its prompt when their rows fit (attention.beam_rows_fit)."""
-        if self.q_len > 1:    # each query token attends up to its own position
+        if self.tree_parents is not None:    # each node attends to the cache and its ancestors
+            ops.paged_decode_attn_tree(self.q.view(self.B, self.q_len, self.Hq, self.D), L["kv"], self.page_list, self.seq_lens,
+                                       self.tree_parents, self.ctx, self.attn_ws, out=self.attn.view(self.B, self.q_len, self.Hq * self.D))
+        elif self.q_len > 1:    # each query token attends up to its own position
             ops.paged_decode_attn_multi(self.q.view(self.B, self.q_len, self.Hq, self.D), L["kv"], self.page_list, self.seq_lens,
                                         self.ctx, self.attn_ws, out=self.attn.view(self.B, self.q_len, self.Hq * self.D))
         elif beam_rows_fit(self.Hq, self.Hkv, self.W, self.requests):
@@ -725,6 +779,8 @@ class DecodeStep:
         can be recorded into a decode program."""
         cfg = self.cfg
         ops.convert_block_table(self.block_ids, out=self.page_list)
+        if self.tree_parents is not None:    # node j is rotated at seq + depth(j) (its K/V still go to slot seq + j)
+            torch.add(self.seq_lens.view(-1, 1), self.tree_depth, out=self.tree_pos.view(self.B, self.q_len))
         ops.embedding(self.ids, self.embed, out=self.resid)
         first = True
         for L in self.layers:
@@ -765,7 +821,9 @@ class DecodeStep:
         elif self.tp_size == 1:
             self._constrain(self.logits)
             ops.argmax(self.logits, out=self.next_ids)
-            if self.q_len > 1:
+            if self.tree_parents is not None:
+                self._verify_tree(target_ids=self.next_ids.view(self.B, self.q_len))
+            elif self.q_len > 1:
                 ops.spec_verify(self.drafts, target_ids=self.next_ids.view(self.B, self.q_len), out_tokens=self.out_tokens,
                                 accepted=self.accepted)
         elif hasattr(self.comm, "argmax"):
@@ -839,8 +897,11 @@ class DecodeStep:
         if self.logprobs is not None:
             ops.token_logprobs(self.logits, self.logprobs, tokens=self.next_ids, workspace=self.lp_ws, out=self.lp_out)
         if not adv:
-            ops.spec_verify(self.drafts, target_probs=self.target_probs, uniform=self.uniform[R:], out_tokens=self.out_tokens,
-                            accepted=self.accepted)
+            if self.tree_parents is not None:
+                self._verify_tree(target_probs=self.target_probs, uniform=self.uniform[R:])
+            else:
+                ops.spec_verify(self.drafts, target_probs=self.target_probs, uniform=self.uniform[R:], out_tokens=self.out_tokens,
+                                accepted=self.accepted)
             return
         torch.log(self.token_prob, out=self.log_prob)
         self.cum_log_probs.add_(self.log_prob)
@@ -850,6 +911,13 @@ class DecodeStep:
         self.hist_len.add_(1)
         self.ids.copy_(self.next_ids)
         self.seq_lens.add_(1)
+
+    def _verify_tree(self, **target):
+        """Tree mode's ending: spec_verify_tree over the node tokens (the step's input ids; the root's is not read), then the
+        accepted path's K/V moved to slots seq .. seq + accepted in every layer (one kv_compact_path launch)."""
+        ops.spec_verify_tree(self.tree_parents, self.ids.view(self.B, self.q_len), out_tokens=self.out_tokens, accepted=self.accepted,
+                             accepted_path=self.accepted_path, **target)
+        ops.kv_compact_path([L["kv"] for L in self.layers], self.page_list, self.seq_lens, self.accepted_path, self.accepted)
 
     def step_tail(self):
         """TP > 1 with stock NCCL: gather the vocab-split logits and sample (torch plumbing, outside the program)."""

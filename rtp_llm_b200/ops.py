@@ -132,6 +132,26 @@ def paged_decode_attn_beam(q: torch.Tensor, kv_cache_base: torch.Tensor, page_li
     return out
 
 
+def paged_decode_attn_tree(q: torch.Tensor, kv_cache_base: torch.Tensor, page_list: torch.Tensor, sequence_lengths: torch.Tensor,
+                           tree_parents: torch.Tensor, max_seq_len: int, workspace: torch.Tensor, out: Optional[torch.Tensor] = None,
+                           q_scale: float = 1.0) -> torch.Tensor:
+    """q [B, n, Hq, D]: the n nodes of each sequence's speculative token tree (K/V already appended at slots
+    sequence_lengths[b] + j); tree_parents int32 [B, n] (node 0 the root, node j under parents[j] in [0, j)). Query j attends to
+    the cached positions and to the slots of its ancestors and itself. A chain gives the bits of paged_decode_attn_multi.
+    Returns [B, n, Hq*D]."""
+    _cuda_contig(q, kv_cache_base, page_list, tree_parents, workspace, out)
+    P, two, Hkv, T, D = kv_cache_base.shape
+    B, q_len, Hq = q.shape[0], q.shape[1], q.shape[2]
+    if tree_parents.dtype != torch.int32 or tuple(tree_parents.shape) != (B, q_len):
+        raise B200Error(f"paged_decode_attn_tree: tree_parents must be int32 [{B}, {q_len}]")
+    if out is None:
+        out = torch.empty((B, q_len, Hq * D), dtype=q.dtype, device=q.device)
+    check(_lib.load().b200_paged_decode_attn_tree(_p(q), _is_bf16(q), _p(out), Hq, Hkv, D, B, q_len, page_list.shape[-1], max_seq_len,
+                                                  T, _p(kv_cache_base), _p(page_list), _p(sequence_lengths), _p(tree_parents),
+                                                  q_scale, _p(workspace), workspace.numel(), _stream()), "b200_paged_decode_attn_tree")
+    return out
+
+
 def paged_decode_attn_rope(qkv: torch.Tensor, kv_cache_base: torch.Tensor, page_list: torch.Tensor, sequence_lengths: torch.Tensor,
                            head_num: int, max_seq_len: int, rope_base: float, workspace: torch.Tensor,
                            out: Optional[torch.Tensor] = None, q_scale: float = 1.0) -> torch.Tensor:
@@ -552,6 +572,75 @@ def spec_verify(draft_tokens: torch.Tensor, *, target_probs: Optional[torch.Tens
     check(_lib.load().b200_spec_verify(_p(target_probs), _p(target_ids), _p(draft_probs), _p(draft_tokens), _p(uniform), B, n, V,
                                        _p(out_tokens), _p(accepted), _stream()), "b200_spec_verify")
     return out_tokens, accepted
+
+
+def spec_verify_tree(tree_parents: torch.Tensor, node_tokens: torch.Tensor, *, target_probs: Optional[torch.Tensor] = None,
+                     target_ids: Optional[torch.Tensor] = None, uniform: Optional[torch.Tensor] = None,
+                     out_tokens: Optional[torch.Tensor] = None, accepted: Optional[torch.Tensor] = None,
+                     accepted_path: Optional[torch.Tensor] = None):
+    """Verify a speculative token tree of n = tree_parents.shape[1] <= 64 nodes per sequence (b200_spec_verify_tree).
+    tree_parents, node_tokens int32 [B, n] (node 0 the root; its token is not read). Greedy: target_ids int32 [B, n]. Sampling
+    (deterministic drafts): target_probs fp32 [B, n, V], uniform fp32 [B, n]. Returns (out_tokens int32 [B, n]: the accepted
+    path's tokens, then one correction or bonus token, then -1; accepted int32 [B]; accepted_path int32 [B, n]: the node at depth
+    0 .. accepted, then -1)."""
+    _cuda_contig(tree_parents, node_tokens, target_probs, target_ids, uniform, out_tokens, accepted, accepted_path)
+    if tree_parents.dim() != 2:
+        raise B200Error("spec_verify_tree: tree_parents must be [B, n]")
+    B, n = tree_parents.shape
+    if tree_parents.dtype != torch.int32 or node_tokens.dtype != torch.int32 or tuple(node_tokens.shape) != (B, n):
+        raise B200Error(f"spec_verify_tree: tree_parents and node_tokens must be int32 [{B}, {n}]")
+    if target_probs is None and target_ids is None:
+        raise B200Error("spec_verify_tree: pass target_probs (sampling) or target_ids (greedy)")
+    if target_probs is not None:
+        if target_probs.dtype != torch.float32 or target_probs.dim() != 3 or tuple(target_probs.shape[:2]) != (B, n):
+            raise B200Error(f"spec_verify_tree: target_probs must be fp32 [{B}, {n}, V]")
+        V = target_probs.shape[2]
+        if uniform is None or uniform.dtype != torch.float32 or uniform.numel() != B * n:
+            raise B200Error(f"spec_verify_tree: sampling mode needs uniform fp32 [{B}, {n}]")
+    else:
+        if target_ids.dtype != torch.int32 or tuple(target_ids.shape) != (B, n):
+            raise B200Error(f"spec_verify_tree: target_ids must be int32 [{B}, {n}]")
+        V = 1                                   # the vocabulary is not read in greedy mode
+    dev = tree_parents.device
+    if out_tokens is None:
+        out_tokens = torch.empty((B, n), dtype=torch.int32, device=dev)
+    if accepted is None:
+        accepted = torch.empty(B, dtype=torch.int32, device=dev)
+    if accepted_path is None:
+        accepted_path = torch.empty((B, n), dtype=torch.int32, device=dev)
+    check(_lib.load().b200_spec_verify_tree(_p(target_probs), _p(target_ids), _p(tree_parents), _p(node_tokens), _p(uniform), B, n, V,
+                                            _p(out_tokens), _p(accepted), _p(accepted_path), _stream()), "b200_spec_verify_tree")
+    return out_tokens, accepted, accepted_path
+
+
+def kv_compact_path(kv_caches: Sequence[torch.Tensor], page_list: torch.Tensor, sequence_lengths: torch.Tensor,
+                    accepted_path: torch.Tensor, accepted: torch.Tensor) -> None:
+    """Move the accepted path of a token-tree step to consecutive cache slots, in place, in one launch for every layer
+    (b200_kv_compact_path): for d = 1 .. accepted[b] the K/V of slot sequence_lengths[b] + accepted_path[b][d] go to slot
+    sequence_lengths[b] + d. kv_caches: one [P, 2, Hkv, T, D] cache per layer (fp16 / bf16, the same shape); page_list
+    [B, 1, 2, M]; sequence_lengths, accepted int32 [B]; accepted_path int32 [B, n]."""
+    kv_caches = list(kv_caches)
+    if not kv_caches:
+        raise B200Error("kv_compact_path: no layer caches given")
+    _cuda_contig(*kv_caches, page_list, sequence_lengths, accepted_path, accepted)
+    shape = tuple(kv_caches[0].shape)
+    if len(shape) != 5 or any(tuple(c.shape) != shape or c.dtype != kv_caches[0].dtype for c in kv_caches):
+        raise B200Error("kv_compact_path: every layer cache must be [P, 2, Hkv, T, D] of one shape and dtype")
+    _is_bf16(kv_caches[0])
+    P, two, Hkv, T, D = shape
+    if accepted_path.dim() != 2:
+        raise B200Error("kv_compact_path: accepted_path must be [B, n]")
+    B, n = accepted_path.shape
+    for name, t, shp in (("sequence_lengths", sequence_lengths, (B,)), ("accepted", accepted, (B,)),
+                         ("accepted_path", accepted_path, (B, n))):
+        if t.dtype != torch.int32 or tuple(t.shape) != shp:
+            raise B200Error(f"kv_compact_path: {name} must be int32 {list(shp)}")
+    if page_list.dtype != torch.int32 or page_list.dim() != 4 or page_list.shape[0] != B:
+        raise B200Error(f"kv_compact_path: page_list must be int32 [{B}, 1, 2, M]")
+    import ctypes
+    pools = (ctypes.c_void_p * len(kv_caches))(*[c.data_ptr() for c in kv_caches])
+    check(_lib.load().b200_kv_compact_path(pools, len(kv_caches), Hkv, D, T, _p(page_list), page_list.shape[-1], _p(sequence_lengths),
+                                           _p(accepted_path), _p(accepted), B, n, _stream()), "b200_kv_compact_path")
 
 
 _LOGIT_DTYPES = {torch.float16: 0, torch.bfloat16: 1, torch.float32: 2}

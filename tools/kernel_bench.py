@@ -89,6 +89,64 @@ def bench_attn_multi(B, Hq, Hkv, S, q_len, T=64, nrot=3):
     return us
 
 
+def bench_attn_tree(B, Hq, Hkv, S, q_len, kind, T=64, nrot=3, runs=3):
+    """b200_paged_decode_attn_tree against b200_paged_decode_attn_multi on the same rows and tables, alternating; kind: the
+    tree's shape (chain, star or binary). The mask only touches the slices that reach the new tokens."""
+    M = math.ceil(S / T)
+    P = B * M + 1
+    pools = [torch.randn(P, 2, Hkv, T, 128, device=dev).half() for _ in range(nrot)]
+    q = torch.randn(B, q_len, Hq, 128, device=dev).half()
+    bid = (torch.randperm(P - 1, device=dev).to(torch.int32) + 1).reshape(B, M)
+    pl = ops.convert_block_table(bid)
+    seq = torch.full((B,), S - q_len, dtype=torch.int32, device=dev)
+    par = [-1] + [{"chain": j - 1, "star": 0, "binary": (j - 1) // 2}[kind] for j in range(1, q_len)]
+    parents = torch.tensor([par] * B, dtype=torch.int32, device=dev)
+    ws = ops.attn_workspace(B * q_len, Hq, Hkv, S, dev)
+    out = torch.empty(B, q_len, Hq * 128, device=dev).half()
+    arms = {"multi": lambda i: ops.paged_decode_attn_multi(q, pools[i], pl, seq, S, ws, out=out),
+            "tree": lambda i: ops.paged_decode_attn_tree(q, pools[i], pl, seq, parents, S, ws, out=out)}
+    t = {k: [] for k in arms}
+    for _ in range(runs):
+        for k, fn in arms.items():
+            t[k].append(timeit(fn, nrot))
+    med = {k: sorted(v)[len(v) // 2] for k, v in t.items()}
+    print(f"attn-tree B{B} Hq{Hq} Hkv{Hkv} S{S} q_len {q_len} {kind} median: multi {med['multi']:.1f} us, tree {med['tree']:.1f} us "
+          f"({med['tree'] / med['multi']:.3f}x)", flush=True)
+    return med
+
+
+def bench_tree_verify(B, n, sampling, V=128256, nrot=4):
+    """b200_spec_verify_tree on binary trees of n nodes, greedy or sampled (target rows of temperature-0.25 softmaxes)."""
+    par = torch.tensor([[-1] + [(j - 1) // 2 for j in range(1, n)]] * B, dtype=torch.int32, device=dev)
+    ids = torch.randint(0, V, (B, n), dtype=torch.int32, device=dev)
+    toks = [ids.gather(1, par.clamp(min=0).long()).to(torch.int32).contiguous() for _ in range(nrot)]
+    probs = [torch.softmax(torch.randn(B, n, V, device=dev) / 0.25, dim=-1) for _ in range(nrot)] if sampling else None
+    u = torch.rand(B, n, device=dev)
+    if sampling:
+        fn = lambda i: ops.spec_verify_tree(par, toks[i], target_probs=probs[i], uniform=u)
+    else:
+        fn = lambda i: ops.spec_verify_tree(par, toks[i], target_ids=ids)
+    us = timeit(fn, nrot)
+    print(f"tree-verify B{B} n{n} {'sampled' if sampling else 'greedy'}: {us:.1f} us", flush=True)
+    return us
+
+
+def bench_kv_compact(B, layers=32, Hkv=8, T=64, n=8, S=2048, nrot=2):
+    """b200_kv_compact_path over the Llama-3-8B cache (32 layers, Hkv 8, D 128) with a path that moves every depth."""
+    M = math.ceil((S + n) / T)
+    P = B * M + 1
+    caches = [torch.randn(P, 2, Hkv, T, 128, device=dev).half() for _ in range(layers)]
+    pl = ops.convert_block_table((torch.randperm(P - 1, device=dev).to(torch.int32) + 1).reshape(B, M))
+    seq = torch.full((B,), S, dtype=torch.int32, device=dev)
+    a = n // 2
+    path = torch.tensor([[0] + [d + 1 for d in range(1, a + 1)] + [-1] * (n - a - 1)] * B, dtype=torch.int32, device=dev)
+    acc = torch.full((B,), a, dtype=torch.int32, device=dev)
+    us = timeit(lambda i: ops.kv_compact_path(caches, pl, seq, path, acc), nrot)
+    byt = 2 * 2 * B * layers * Hkv * a * 128 * 2
+    print(f"kv-compact B{B} layers {layers} accepted {a}: {us:.2f} us ({byt / 1e6:.2f} MB moved)", flush=True)
+    return us
+
+
 def bench_attn_beam(B, W, Hq, Hkv, S=2048, T=64, private=28, nrot=3, runs=3):
     """b200_paged_decode_attn_beam against b200_paged_decode_attn on the same B * W rows and the same page tables, whose beams
     share the full pages of the first S - private tokens and own the pages after them (the beam step's tables), the arms
@@ -403,6 +461,24 @@ if __name__ == "__main__":
         # speculative-token verification at group 8 (Qwen2-72B / Llama-3-70B): 8, 16, 32, 64 query rows per kv head
         t = {n: bench_attn_multi(32, 64, 8, 2048, n) for n in (1, 2, 4, 8)}
         print("attn-multi time relative to q_len 2 (16 rows): " + ", ".join(f"q_len {n}: {t[n] / t[2]:.2f}x" for n in t), flush=True)
+    if "attn-tree" in which or "tree-verify" in which or "kv-compact" in which:
+        import subprocess
+        print("tree benches on " + (subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader",
+                                                    "-i", "0"], capture_output=True, text=True).stdout.strip() or "unknown card")
+              + " (name, power limit, SM clock, max SM clock)", flush=True)
+    if "attn-tree" in which:
+        # Llama-3-8B heads (group 4) at B 32, S 2048: the tree instance against the q_len instance on the same rows
+        for n in (4, 8, 16):
+            for kind in ("chain", "star", "binary"):
+                bench_attn_tree(32, 32, 8, 2048, n, kind)
+    if "tree-verify" in which:
+        for B in (8, 32):
+            for n in (4, 8, 16):
+                for sampling in (False, True):
+                    bench_tree_verify(B, n, sampling)
+    if "kv-compact" in which:
+        for B in (8, 32):
+            bench_kv_compact(B)
     if "attn-beam" in which:
         # a request's beams in one CTA against one CTA per beam, Llama-3-8B heads (group 4) and group 8 at W 8
         import subprocess

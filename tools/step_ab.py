@@ -11,6 +11,8 @@ each a step captured in a CUDA graph with PDL at --ctx tokens; the first arm is 
   sample     Llama-3-8B INT4: greedy, then sampled (temperature 0.8, top-k 50, top-p 0.9, repetition 1.1, the drawn token's
              log-prob and the top 5)
   qwen3      Qwen3-8B INT4: qk_rmsnorm, then the plain rope launch (TwoLaunchStep), against the fused QK-norm append
+  tree       Llama-3-8B INT4: per q_len 4 and 8 with batch * q_len <= 128, the chain verification step, then the token-tree
+             step on a binary tree of q_len nodes (tree attention, spec_verify_tree and the K/V compaction)
   constrain  Llama-3-8B INT4: greedy, greedy with a 50 % random token bitmask and 300 logit_bias entries per row, sampled
              (temperature 0.8, top-k 50, top-p 0.9), sampled with the same constraints
 
@@ -129,6 +131,16 @@ def constrain_arms(a, cfg, B, dev):
     return arms
 
 
+def tree_arms(a, cfg, B, dev):
+    arms = []
+    for n in (4, 8):
+        if B * n <= 128:
+            binary = [-1] + [(j - 1) // 2 for j in range(1, n)]
+            arms.append(step_arm(f"chain q_len {n}", DecodeStep(cfg, B, a.ctx, dev, pdl=True, q_len=n)))
+            arms.append(step_arm(f"tree q_len {n}", DecodeStep(cfg, B, a.ctx, dev, pdl=True, q_len=n, tree=binary)))
+    return arms
+
+
 def qwen3_arms(a, cfg, B, dev):
     return [step_arm("norm + rope", TwoLaunchStep(cfg, B, a.ctx, dev, pdl=True)),
             step_arm("fused", DecodeStep(cfg, B, a.ctx, dev, pdl=True))]
@@ -137,7 +149,7 @@ def qwen3_arms(a, cfg, B, dev):
 # name: arms, default batches, timed replays per run, warm-up replays
 PRESETS = {"act-order": (act_order_arms, [32], 100, 10), "spec": (spec_arms, [8, 16, 32], 50, 3),
            "beam": (beam_arms, [8], 20, 3), "sample": (sample_arms, [8, 32], 20, 3), "qwen3": (qwen3_arms, [8, 16, 32], 100, 10),
-           "constrain": (constrain_arms, [8, 32], 50, 5)}
+           "constrain": (constrain_arms, [8, 32], 50, 5), "tree": (tree_arms, [8, 16, 32], 50, 3)}
 MODELS = {"llama3": LLAMA3_8B, "llama31": LLAMA31_8B}
 
 
