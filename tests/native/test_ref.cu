@@ -74,9 +74,99 @@ __global__ void ref_dequant_gemm_kernel(const T* __restrict__ x, int B, int K, i
     y[(size_t)b * N + n] = from_f32<T>(acc);
 }
 
+// ---- PDL hazard harness (tests/test_gpu_pdl_hazards.py). The writer is a slow predecessor launched without the PDL
+// attribute; the kernel launched after it with the attribute may become resident during the writer's delay and must not
+// touch dependent data until its griddepcontrol.wait returns, which is after the writer has finished.
+struct PdlCopy {
+    const void* src;
+    void* dst;
+    unsigned long long bytes;
+};
+
+__device__ __forceinline__ unsigned long long globaltimer() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
+    return t;
+}
+
+// One CTA: the same thread copies the same bytes of every range, so an in-place buffer is snapshotted before the staged
+// input lands on it. .cg loads read L2, where a dependent kernel's early store would be.
+__device__ void pdl_copy_range(const PdlCopy& c) {
+    const bool vec = (((uintptr_t)c.src | (uintptr_t)c.dst | c.bytes) & 15) == 0;
+    if (vec) {
+        const uint4* s = (const uint4*)c.src;
+        uint4* d = (uint4*)c.dst;
+        for (unsigned long long i = threadIdx.x; i < c.bytes / 16; i += blockDim.x) __stcg(d + i, __ldcg(s + i));
+    } else {
+        const volatile uint8_t* s = (const volatile uint8_t*)c.src;
+        volatile uint8_t* d = (volatile uint8_t*)c.dst;
+        for (unsigned long long i = threadIdx.x; i < c.bytes; i += blockDim.x) d[i] = s[i];
+    }
+}
+
+__global__ void pdl_writer_kernel(const PdlCopy* __restrict__ copies, int n_snap, int n_stage, unsigned long long delay_ns,
+                                  unsigned long long* __restrict__ times) {
+    pdl_launch_dependents();
+    const unsigned long long t0 = globaltimer();
+    while (globaltimer() - t0 < delay_ns) {
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) times[0] = globaltimer();
+    for (int i = 0; i < n_snap; ++i) pdl_copy_range(copies[i]);
+    __syncthreads();
+    for (int i = 0; i < n_stage; ++i) pdl_copy_range(copies[n_snap + i]);
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) times[1] = globaltimer();
+}
+
+// Each CTA records when it became resident, before its grid dependency resolves.
+__global__ void pdl_probe_kernel(unsigned long long* __restrict__ entry) {
+    const unsigned long long t = globaltimer();
+    if (threadIdx.x == 0) entry[blockIdx.x + (size_t)gridDim.x * blockIdx.y] = t;
+    pdl_wait();
+}
+
+// The harness's controls: mode 0 waits and then copies in -> out; mode 1 loads in before the wait; mode 2 stores to out
+// before the wait.
+__global__ void pdl_copy_kernel(const uint32_t* __restrict__ in, uint32_t* __restrict__ out, int n, int mode) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    uint32_t v = 0;
+    if (mode == 1 && i < n) v = __ldcg(in + i);
+    if (mode == 2 && i < n) __stcg(out + i, 0u);
+    pdl_wait();
+    if (mode != 1 && i < n) v = __ldcg(in + i);
+    if (i < n) out[i] = v;
+}
+
 }  // namespace b200
 
 using namespace b200;
+
+namespace {
+cudaError_t launch_pdl(void (*kern)(unsigned long long*), dim3 grid, dim3 block, size_t smem, dim3 cluster, void* stream,
+                       unsigned long long* entry) {
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = grid;
+    cfg.blockDim = block;
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = (cudaStream_t)stream;
+    cudaLaunchAttribute attr[2];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    int na = 1;
+    if (cluster.x > 1) {
+        attr[1].id = cudaLaunchAttributeClusterDimension;
+        attr[1].val.clusterDim.x = cluster.x;
+        attr[1].val.clusterDim.y = 1;
+        attr[1].val.clusterDim.z = 1;
+        na = 2;
+    }
+    cfg.attrs = attr;
+    cfg.numAttrs = na;
+    return cudaLaunchKernelEx(&cfg, kern, entry);
+}
+}  // namespace
 
 extern "C" {
 
@@ -111,6 +201,39 @@ int b200_ref_dequant_gemm(int fmt, int is_bf16, const void* x, int B, int K, int
             (const __half*)x, B, K, N, fmt, w, (const __half*)scales, (const __half*)zeros_x_scales, group,
             (const __half*)bias, (__half*)y);
     return cudaPeekAtLastError() == cudaSuccess ? 0 : -2;
+}
+
+// copies: device array of n_snap snapshot ranges then n_stage staging ranges; times: 2 device uint64 (before the copies,
+// after them). Launched plainly, so it runs after everything before it on the stream.
+int b200_ref_pdl_writer(const void* copies, int n_snap, int n_stage, unsigned long long delay_ns, void* times, void* stream) {
+    pdl_writer_kernel<<<1, 256, 0, (cudaStream_t)stream>>>((const PdlCopy*)copies, n_snap, n_stage, delay_ns,
+                                                           (unsigned long long*)times);
+    return cudaPeekAtLastError() == cudaSuccess ? 0 : -2;
+}
+
+// entry: grid_x * grid_y device uint64; cluster_x > 1 launches clusters along x.
+int b200_ref_pdl_probe(int grid_x, int grid_y, int block, int smem, int cluster_x, void* entry, void* stream) {
+    if (cudaFuncSetAttribute(pdl_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) return -1;
+    if (cudaFuncSetAttribute(pdl_probe_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
+                             cudaSharedmemCarveoutMaxShared) != cudaSuccess)
+        return -1;
+    const cudaError_t e = launch_pdl(pdl_probe_kernel, dim3(grid_x, grid_y), dim3(block), smem, dim3(cluster_x), stream,
+                                     (unsigned long long*)entry);
+    return e == cudaSuccess ? 0 : -2;
+}
+
+int b200_ref_pdl_copy(const void* in, void* out, int n_words, int mode, void* stream) {
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3((n_words + 255) / 256);
+    cfg.blockDim = dim3(256);
+    cfg.stream = (cudaStream_t)stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    const cudaError_t e = cudaLaunchKernelEx(&cfg, pdl_copy_kernel, (const uint32_t*)in, (uint32_t*)out, n_words, mode);
+    return e == cudaSuccess ? 0 : -2;
 }
 
 }  // extern "C"

@@ -2,7 +2,7 @@
 tensors. Test infrastructure (a second opinion next to the CPU oracle), never part of the product library."""
 import ctypes
 import os
-from ctypes import c_float, c_int, c_void_p
+from ctypes import c_float, c_int, c_uint64, c_void_p
 
 import torch
 
@@ -25,6 +25,12 @@ def load():
         lib.b200_ref_dequant_gemm.restype = c_int
         lib.b200_ref_dequant_gemm.argtypes = [c_int, c_int, c_void_p, c_int, c_int, c_int] + [c_void_p] * 3 + [c_int, c_void_p,
                                                                                                         c_void_p, c_void_p]
+        lib.b200_ref_pdl_writer.restype = c_int
+        lib.b200_ref_pdl_writer.argtypes = [c_void_p, c_int, c_int, c_uint64, c_void_p, c_void_p]
+        lib.b200_ref_pdl_probe.restype = c_int
+        lib.b200_ref_pdl_probe.argtypes = [c_int] * 5 + [c_void_p, c_void_p]
+        lib.b200_ref_pdl_copy.restype = c_int
+        lib.b200_ref_pdl_copy.argtypes = [c_void_p, c_void_p, c_int, c_int, c_void_p]
         _lib = lib
     return _lib
 
@@ -57,3 +63,22 @@ def ref_dequant_gemm(x, fmt, w, scales=None, zeros_x_scales=None, group=128, bia
                                       group, _p(bias), _p(out), _stream())
     assert rc == 0, rc
     return out
+
+
+def pdl_writer(copies, n_snap, n_stage, delay_ns, times):
+    """The PDL harness's slow predecessor on the current stream: copies int64 [n_snap + n_stage, 3] rows of (source, destination,
+    bytes), the snapshot ranges first; times int64 [2] receives %globaltimer before and after the copies."""
+    rc = load().b200_ref_pdl_writer(_p(copies), n_snap, n_stage, delay_ns, _p(times), _stream())
+    assert rc == 0, rc
+
+
+def pdl_probe(grid_x, grid_y, threads, smem, cluster_x, entry):
+    """A PDL-attributed kernel of that shape whose CTAs store %globaltimer at entry into entry int64 [grid_x * grid_y]."""
+    rc = load().b200_ref_pdl_probe(grid_x, grid_y, threads, smem, cluster_x, _p(entry), _stream())
+    assert rc == 0, rc
+
+
+def pdl_copy(x, out, mode):
+    """The harness's control (int32 x -> out, PDL attribute): 0 waits first, 1 loads x before the wait, 2 stores before it."""
+    rc = load().b200_ref_pdl_copy(_p(x), _p(out), x.numel(), mode, _stream())
+    assert rc == 0, rc
