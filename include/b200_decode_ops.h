@@ -137,6 +137,29 @@ int b200_paged_decode_attn_beam(const void* q, int is_bf16, void* out, size_t he
                                 const void* kv_pool, const int32_t* page_list, const uint32_t* sequence_lengths,
                                 const int32_t* shared_lengths, float q_scale, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Shared-prefix decode attention: rows of different requests that share cached leading pages (prefix-cache hits on one system
+ * prompt, n samples of one prompt) read those pages once per chunk instead of once per row. The beam instance above with the rows
+ * of a CTA taken from a list instead of b * beam_width + i.
+ *   q, out, page_list, sequence_lengths   those of b200_paged_decode_attn on `batch` rows.
+ *   chunk_offsets [chunks + 1], chunk_rows [batch] int32 (device): chunk c is the rows chunk_rows[chunk_offsets[c] ..
+ *                chunk_offsets[c + 1]), at most max_members of them, in any order and any positions of the batch.
+ *   shared_lengths [chunks] int32 (device): tokens that all rows of chunk c share. The caller's contract: each row appears in at
+ *                most one chunk, and the members' page_list rows are equal over the first shared_lengths[c] / page_size pages
+ *                (the first member's are read). The kernel rounds the value down to a multiple of 64 and keeps it at or below
+ *                the shortest member's sequence_lengths, so 0 shares nothing.
+ * Every row has the bits it has with shared_lengths all 0 in the same chunking and max_members, and one row per chunk with
+ * max_members 1 gives the bits of b200_paged_decode_attn. Bad chunk data cannot read or write outside q, out and page_list:
+ * offsets are clamped to [0, batch], a chunk's rows past max_members are cut off, a row index outside [0, batch) is skipped.
+ * A row that no chunk lists is not written. (head_num / kv_head_num) * max_members <= 64 picks 1, 2 or 4 row tiles per CTA;
+ * 1 <= chunks <= batch <= 65535; chunks * kv_head_num <= 65535; head_dim and page_size as b200_paged_decode_attn; size the workspace with
+ * b200_paged_decode_attn_workspace_bytes(batch, ...). */
+int b200_paged_decode_attn_prefix(const void* q, int is_bf16, void* out, size_t head_num, size_t kv_head_num, size_t head_dim,
+                                  size_t batch, size_t chunks, size_t max_members, const int32_t* chunk_offsets,
+                                  const int32_t* chunk_rows, const int32_t* shared_lengths, size_t max_blocks_per_seq,
+                                  size_t max_seq_len, size_t page_size, const void* kv_pool, const int32_t* page_list,
+                                  const uint32_t* sequence_lengths, float q_scale, void* workspace, size_t workspace_bytes,
+                                  void* stream);
+
 /* Verification of a speculative token TREE (EAGLE / Medusa drafts; TensorRT-LLM XQA's spec-decoding mask, restated: parity
  * unpinned). The arguments of b200_paged_decode_attn_multi plus tree_parents [batch][q_len] int32 (device): the q_len new tokens of
  * sequence b are nodes, node 0 the root (the last accepted token; its entry is not read), node j >= 1 under tree_parents[b][j] in

@@ -31,6 +31,8 @@ SIGNATURES = {
                                             c_float, c_float, c_void_p, c_size_t, c_void_p]),
     "b200_paged_decode_attn_beam": (c_int, [c_void_p, c_int, c_void_p] + [c_size_t] * 8 + [c_void_p, c_void_p, c_void_p, c_void_p,
                                             c_float, c_void_p, c_size_t, c_void_p]),
+    "b200_paged_decode_attn_prefix": (c_int, [c_void_p, c_int, c_void_p] + [c_size_t] * 6 + [c_void_p] * 3 + [c_size_t] * 3
+                                      + [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_size_t, c_void_p]),
     "b200_paged_decode_attn_tree": (c_int, [c_void_p, c_int, c_void_p] + [c_size_t] * 8 + [c_void_p, c_void_p, c_void_p, c_void_p,
                                             c_float, c_void_p, c_size_t, c_void_p]),
     "b200_wo_gemm_packed_bytes": (c_size_t, [c_int, c_int, c_int]),

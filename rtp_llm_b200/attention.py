@@ -70,6 +70,18 @@ def beam_rows_fit(head_num: int, kv_head_num: int, beam_width: int, requests: in
     return beam_width > 1 and group * beam_width <= _MAX_ROWS and requests * kv_head_num >= _BEAM_MIN_UNITS
 
 
+def prefix_rows_fit(kv_head_num: int, chunks: int, mean_shared_tokens: float, max_members: int) -> bool:
+    """When b200_paged_decode_attn_prefix on ops.prefix_chunks' chunking beats b200_paged_decode_attn on the same rows: chunks of
+    at most 8 rows, enough (chunk, kv head) pairs to fill the GPU with the fewer, heavier CTAs, and, at the smallest such count,
+    half a 2048 context shared. Measured (H100 80GB HBM3, 700 W; Hq 32, Hkv 8, D 128, T 64, ctx 2048; tools/kernel_bench.py
+    attn-prefix, prefix / per row, medians of 3): 512 pairs 0.54-0.91; 256 pairs 0.67-0.95 (512 shared tokens 0.88-0.95); 128
+    pairs 0.74-0.90 at 1024 or more shared tokens but 0.90-1.02 at 512; 64 pairs 1.05-1.35. Chunks of 16 rows lost wherever they
+    were measured (1.25-4.6 at 16 to 64 pairs): a private tile is one stage per member, so a 16-row chunk runs its members' tails
+    one after another."""
+    units = kv_head_num * chunks
+    return max_members <= 8 and (units >= 256 or (units >= 128 and mean_shared_tokens >= 1024))
+
+
 def _q_len(attn_inputs) -> int:
     """Tokens per sequence of a decode step: max(input_lengths) when the inputs carry them (speculative verification,
     uniform across the batch), else 1."""

@@ -436,11 +436,14 @@ size_t b200_paged_decode_attn_workspace_bytes(size_t batch, size_t head_num, siz
 
 // beam_width > 0: the beam instance. `batch` then counts requests, each with beam_width sequences (rows of q, out, page_list and
 // sequence_lengths), and shared_lengths [batch] says how much of a request's K/V its beams share; q_len is 1.
+// chunks > 0 (with beam_width > 0): the beam instance's prefix mode. `batch` counts rows; CTAs own the chunks of up to beam_width
+// rows that chunk_offsets / chunk_rows list, and shared_lengths [chunks] is per chunk.
 // tree_parents != null: the tree instance, parents [batch][q_len] of each sequence's q_len new tokens.
 static int attn_impl(const void* q, const void* qkv, float rope_base, int q_len, int is_bf16, void* out, size_t head_num, size_t kv_head_num,
                      size_t head_dim, size_t batch, size_t max_blocks_per_seq, size_t max_seq_len, size_t page_size, const void* kv_pool,
                      const int32_t* page_list, const uint32_t* sequence_lengths, float q_scale, void* workspace, size_t workspace_bytes,
-                     void* stream, int beam_width = 0, const int32_t* shared_lengths = nullptr, const int32_t* tree_parents = nullptr) {
+                     void* stream, int beam_width = 0, const int32_t* shared_lengths = nullptr, const int32_t* tree_parents = nullptr,
+                     size_t chunks = 0, const int32_t* chunk_offsets = nullptr, const int32_t* chunk_rows = nullptr) {
     if (batch == 0) return B200_OK;
     ARG_CHECK((q || qkv) && out && kv_pool && page_list && sequence_lengths, "paged_decode_attn: null pointer");
     ARG_CHECK(head_dim == 64 || head_dim == 128 || head_dim == 256, "paged_decode_attn: head_dim %zu unsupported (64 / 128 / 256)", head_dim);
@@ -461,13 +464,16 @@ static int attn_impl(const void* q, const void* qkv, float rope_base, int q_len,
     ARG_CHECK(max_seq_len >= 1, "paged_decode_attn: max_seq_len must be >= 1");
     ARG_CHECK(max_seq_len <= max_blocks_per_seq * page_size, "paged_decode_attn: max_seq_len %zu exceeds page table capacity %zu",
               max_seq_len, max_blocks_per_seq * page_size);
-    ARG_CHECK(batch * kv_head_num <= 65535, "paged_decode_attn: batch*kv_heads %zu exceeds grid limit", batch * kv_head_num);
+    const size_t units = chunks ? chunks : batch;   // sequences, requests or chunks: one CTA row of the grid each
+    ARG_CHECK(units * kv_head_num <= 65535, "paged_decode_attn: batch*kv_heads %zu exceeds grid limit", units * kv_head_num);
     ARG_CHECK(((uintptr_t)kv_pool & 15) == 0 && (((uintptr_t)q | (uintptr_t)qkv) & 3) == 0, "paged_decode_attn: misaligned pointer");
 
     const int slots = beam_width ? beam_width : q_len;   // query tokens or beams that share a CTA
     AttnBeamParams p{};
     p.beam_width = beam_width;
     p.shared_lens = shared_lengths;
+    p.chunk_offsets = chunk_offsets;
+    p.chunk_rows = chunk_rows;
     p.q = q;
     p.qkv = qkv;
     p.kv_pool_rw = const_cast<void*>(kv_pool);
@@ -487,10 +493,10 @@ static int attn_impl(const void* q, const void* qkv, float rope_base, int q_len,
     p.boxes_per_tile = kAttnTile / p.box_h;
     p.scale_log2 = q_scale / std::sqrt((float)head_dim) * 1.4426950408889634f;
     const int max_tiles = (int)((max_seq_len + kAttnTile - 1) / kAttnTile);
-    attn_split((int)(batch * kv_head_num), max_tiles, &p.nsplit, &p.tiles_per_split, (int)head_dim);
+    attn_split((int)(units * kv_head_num), max_tiles, &p.nsplit, &p.tiles_per_split, (int)head_dim);
 
     if (p.nsplit > 8) {
-        const AttnWorkspace w = attn_workspace(batch, head_num, kv_head_num, slots, p.nsplit, head_dim);
+        const AttnWorkspace w = attn_workspace(batch, head_num, kv_head_num, chunks ? 1 : slots, p.nsplit, head_dim);
         ARG_CHECK(workspace && workspace_bytes >= w.sem + w.ml + w.o,
                   "paged_decode_attn: workspace too small (%zu < %zu)", workspace_bytes, w.sem + w.ml + w.o);
         p.sem = reinterpret_cast<int*>(workspace);
@@ -507,7 +513,7 @@ static int attn_impl(const void* q, const void* qkv, float rope_base, int q_len,
         int rc = make_map(&map, is_bf16 != 0, 4, kv_pool, dims, strides, box);
         if (rc) return rc;
     }
-    const dim3 grid(p.nsplit, (unsigned)(batch * kv_head_num), 1);
+    const dim3 grid(p.nsplit, (unsigned)(units * kv_head_num), 1);
     p.cluster_merge = (p.nsplit >= 2 && p.nsplit <= 8) ? 1 : 0;   // 2..8 splits merge in a cluster, more through the workspace
     const dim3 cluster(p.cluster_merge ? p.nsplit : 1);
     auto launch = [&](auto t, auto hd, auto rt, auto beam, auto tree) {
@@ -586,6 +592,27 @@ int b200_paged_decode_attn_beam(const void* q, int is_bf16, void* out, size_t he
     return attn_impl(q, nullptr, 0.f, 1, is_bf16, out, head_num, kv_head_num, head_dim, requests, max_blocks_per_seq, max_seq_len,
                      page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, stream, (int)beam_width,
                      shared_lengths);
+}
+
+int b200_paged_decode_attn_prefix(const void* q, int is_bf16, void* out, size_t head_num, size_t kv_head_num, size_t head_dim,
+                                  size_t batch, size_t chunks, size_t max_members, const int32_t* chunk_offsets,
+                                  const int32_t* chunk_rows, const int32_t* shared_lengths, size_t max_blocks_per_seq,
+                                  size_t max_seq_len, size_t page_size, const void* kv_pool, const int32_t* page_list,
+                                  const uint32_t* sequence_lengths, float q_scale, void* workspace, size_t workspace_bytes,
+                                  void* stream) {
+    if (batch == 0) return B200_OK;
+    ARG_CHECK(q && chunk_offsets && chunk_rows && shared_lengths, "paged_decode_attn_prefix: null pointer (q or a chunk array)");
+    ARG_CHECK(chunks >= 1 && chunks <= batch, "paged_decode_attn_prefix: chunks %zu must be in 1..batch (%zu)", chunks, batch);
+    ARG_CHECK(batch <= 65535, "paged_decode_attn_prefix: batch %zu exceeds 65535 rows", batch);
+    ARG_CHECK(kv_head_num > 0 && head_num % kv_head_num == 0, "paged_decode_attn_prefix: head_num %zu not a multiple of kv_head_num %zu",
+              head_num, kv_head_num);
+    ARG_CHECK(max_members >= 1 && (head_num / kv_head_num) * max_members <= (size_t)kAttnMaxRows,
+              "paged_decode_attn_prefix: group %zu x max_members %zu exceeds the limit of %d query rows per (chunk, kv head)",
+              head_num / kv_head_num, max_members, kAttnMaxRows);
+    ARG_CHECK(chunks * kv_head_num <= 65535, "paged_decode_attn_prefix: chunks*kv_heads %zu exceeds grid limit", chunks * kv_head_num);
+    return attn_impl(q, nullptr, 0.f, 1, is_bf16, out, head_num, kv_head_num, head_dim, batch, max_blocks_per_seq, max_seq_len,
+                     page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, stream, (int)max_members,
+                     shared_lengths, nullptr, chunks, chunk_offsets, chunk_rows);
 }
 
 int b200_paged_decode_attn_tree(const void* q, int is_bf16, void* out, size_t head_num, size_t kv_head_num, size_t head_dim,

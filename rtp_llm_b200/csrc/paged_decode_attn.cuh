@@ -65,14 +65,19 @@ struct AttnParams {
                               //    their partial (m, l, O) through distributed shared memory; no workspace, no semaphore
 };
 
-// The beam instance's parameters (XQA's beamWidth, 3rdparty/xqa/mha_sm90.cu: ctaNbValidQHeads = headGrpSize * beamWidth). B is the
-// number of requests; request b owns the beam_width sequences b * beam_width + i of q / out / page_list / seq_lens, and its
-// group * beam_width <= 64 query rows share one CTA: MMA row i * group + g is beam i, head kvh * group + g. q_len is 1.
+// The beam instance's parameters (XQA's beamWidth, 3rdparty/xqa/mha_sm90.cu: ctaNbValidQHeads = headGrpSize * beamWidth). A CTA
+// owns a chunk: up to beam_width members, rows of q / out / page_list / seq_lens whose group * beam_width <= 64 query rows share
+// it; MMA row i * group + g is member i, head kvh * group + g. q_len is 1.
+// Beam mode (chunk_rows null): chunk b is request b, its members the beam_width rows b * beam_width + i; B counts requests.
+// Prefix mode: chunk c's members are the rows chunk_rows[chunk_offsets[c] .. chunk_offsets[c + 1]) of the B rows, at most
+// beam_width of them (more are cut off); a member row outside [0, B) is skipped (never read or written), and so is a row in no chunk.
 struct AttnBeamParams : AttnParams {
     int beam_width;
-    const int32_t* shared_lens;   // [B] tokens of request b that all its beams share: over the first shared_lens[b] / T pages the
-                                  // request's page_list rows are equal (the caller's contract). The kernel rounds it down to whole
-                                  // 64-token tiles below the shortest beam's cached length, so a wrong value can only cost sharing.
+    const int32_t* shared_lens;   // [chunks] tokens that all members of chunk c share: over the first shared_lens[c] / T pages the
+                                  // members' page_list rows are equal (the caller's contract). The kernel rounds it down to whole
+                                  // 64-token tiles below the shortest member's cached length, so a wrong value can only cost sharing.
+    const int32_t* chunk_offsets; // [chunks + 1]
+    const int32_t* chunk_rows;    // [B] (B <= 65535), or null (beam mode)
 };
 
 // The tree instance's parameters (a speculative token tree, XQA's spec-decoding mask in TensorRT-LLM). The q_len new tokens of
@@ -84,10 +89,11 @@ struct AttnTreeParams : AttnParams {
 };
 
 // RT: 16-row tiles of query rows (rows = group * q_len rounded up to 16 / 32 / 64)
-// BEAM: a request's beams in one CTA. Tile t below the shared length is one pipeline stage, loaded once through beam 0's pages with
-// every row live; a tile from there on is one stage per beam that reaches it, in beam order, each loaded through that beam's pages
-// and masked to that beam's rows. A row so meets the tiles of its own sequence in order with the arithmetic of the plain instance;
-// another beam's stage leaves its (m, l, O) bit for bit as they were.
+// BEAM: a chunk's members (a request's beams, or rows that share a prefix) in one CTA. Tile t below the shared length is one
+// pipeline stage, loaded once through member 0's pages with every row live; a tile from there on is one stage per member that
+// reaches it, in member order, each loaded through that member's pages and masked to that member's rows. A row so meets the tiles
+// of its own sequence in order with the arithmetic of the plain instance; another member's stage leaves its (m, l, O) bit for bit
+// as they were.
 // TREE: the q_len instance with each query's new-token columns masked to its ancestors. The ancestor sets are 64-bit masks built
 // once per CTA in shared memory. A 16-token slice wholly below seq_lens[b] runs the plain instance's code; a slice that reaches
 // the new tokens also tests the mask and reads the new tokens' non-finite V elements as 0, so a node outside a row's ancestors
@@ -122,20 +128,40 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map,
 
     // the host sized the split for max_seq_len: a longer sequence is clamped to that bound (never more tiles than the
     // splits cover, so the last-arriver count below always matches the CTAs that really contribute)
-    // query slots per CTA: tokens of a verification step, or the request's beams
+    // query slots per CTA: tokens of a verification step, or the chunk's member slots (BEAM)
     auto nq = [&] {
         if constexpr (BEAM) return p.beam_width;
         else return p.q_len;
     };
-    int len_v, sh_tiles = 0;     // BEAM: len is the longest beam's, tiles [0, sh_tiles) are shared
-    // BEAM: every beam's clamped length, then the shared tile count (in the fused rope's table: the beam instance has no rope)
+    int len_v, sh_tiles = 0;     // BEAM: len is the longest member's, tiles [0, sh_tiles) are shared
+    // BEAM: every member's clamped length, then the shared tile count, then (prefix mode) every member's row (kNoRow: a slot
+    // past the chunk's members or a row outside [0, B)), in the fused rope's table (the beam instance has no rope)
     int* s_len = reinterpret_cast<int*>(cs_tab);
+    uint16_t* s_row = reinterpret_cast<uint16_t*>(s_len + kAttnMaxRows + 1);
+    constexpr uint16_t kNoRow = 0xffff;   // (the host keeps B <= 65535 in prefix mode)
     if constexpr (BEAM) {
         const int cap = p.nsplit * p.tiles_per_split * kAttnTile;
         int lmax = 0, cmin = cap;
+        // prefix mode: the chunk's rows are chunk_rows[lo, hi), at most beam_width of them; every position read lies in [0, B)
+        int lo = 0, nmem = nq();
+        if (p.chunk_rows) {
+            lo = min(max(p.chunk_offsets[b], 0), p.B);
+            nmem = min(min(max(p.chunk_offsets[b + 1], lo), p.B) - lo, p.beam_width);
+            if (threadIdx.x == 0) s_flag[1] = lo;   // the workspace merge's position of member 0
+        }
         for (int i = lane; i < nq(); i += 32) {
-            const int cached = min(p.seq_lens[b * nq() + i], cap);
-            const int l = min(cached + 1, cap);
+            int row = b * nq() + i;
+            if (p.chunk_rows) {
+                row = i < nmem ? p.chunk_rows[lo + i] : -1;
+                if (row >= p.B) row = -1;
+                if (warp == 0) s_row[i] = row < 0 ? kNoRow : (uint16_t)row;
+                if (i >= nmem) {                    // an empty slot takes no part
+                    if (warp == 0) s_len[i] = 0;
+                    continue;
+                }
+            }
+            const int cached = row < 0 ? 0 : min(p.seq_lens[row], cap);
+            const int l = row < 0 ? 0 : min(cached + 1, cap);   // a skipped member has no tile of its own and shares nothing
             if (warp == 0) s_len[i] = l;     // (read after the barrier below)
             lmax = max(lmax, l);
             cmin = min(cmin, cached);   // the token appended this step is never shared
@@ -185,8 +211,8 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map,
     }
     __syncthreads();
 
-    // BEAM: the stage sequence, derived alike by the producer and the consumers. live_from: the first beam >= from with a stage
-    // at tile t (nq() when none); a shared tile has the one stage, filed under beam 0, whose pages it is loaded through.
+    // BEAM: the stage sequence, derived alike by the producer and the consumers. live_from: the first member >= from with a stage
+    // at tile t (nq() when none); a shared tile has the one stage, filed under member 0, whose pages it is loaded through.
     auto live_from = [&](int t, int from) {
         if (t < s_len[kAttnMaxRows]) return from == 0 ? 0 : nq();
         while (from < nq() && s_len[from] <= t * kAttnTile) ++from;
@@ -202,14 +228,20 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map,
         if constexpr (BEAM) seq = b * nq();             // beam 0's; beam i's rows lie 2 * M * i further on
         const int32_t* kpl = p.page_list + (size_t)(seq * 2 + 0) * p.M;
         const int32_t* vpl = p.page_list + (size_t)(seq * 2 + 1) * p.M;
-        // BEAM: stage n of this CTA is tile i through beam `beam`'s pages, up to that beam's length when the tile is private
+        // BEAM: stage n of this CTA is tile i through member `beam`'s pages (a live member's row is valid), up to that member's
+        // length when the tile is private
         auto issue = [&](int i, int n = 0, int beam = 0) {
             int it = i - t0, len_s = len;
             const int32_t *kp = kpl, *vp = vpl;
             if constexpr (BEAM) {
                 it = n;
-                kp += (size_t)beam * 2 * p.M;
-                vp += (size_t)beam * 2 * p.M;
+                if (p.chunk_rows) {
+                    kp = p.page_list + (size_t)s_row[beam] * 2 * p.M;
+                    vp = kp + p.M;
+                } else {
+                    kp += (size_t)beam * 2 * p.M;
+                    vp += (size_t)beam * 2 * p.M;
+                }
                 if (i >= s_len[kAttnMaxRows]) len_s = s_len[beam];
             }
             const int s = it % kAttnStages;
@@ -345,11 +377,19 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map,
       }
     }
     if (!q_loaded) {
-        // MMA row R = j * group + g  <->  query token (BEAM: beam) j, head kvh * group + g
-        const bool v0 = row0 < rows, v1 = row1 < rows;
+        // MMA row R = j * group + g  <->  query token (BEAM: member) j, head kvh * group + g
+        bool v0 = row0 < rows, v1 = row1 < rows;
+        if constexpr (BEAM) if (p.chunk_rows) {
+            v0 = v0 && s_row[row0 / p.group] != kNoRow;
+            v1 = v1 && s_row[row1 / p.group] != kNoRow;
+        }
         const T* qall = reinterpret_cast<const T*>(p.q);
         const T* q0 = qall + (((size_t)b * nq() + row0 / p.group) * p.Hq + (size_t)kvh * p.group + row0 % p.group) * D;
         const T* q1 = qall + (((size_t)b * nq() + row1 / p.group) * p.Hq + (size_t)kvh * p.group + row1 % p.group) * D;
+        if constexpr (BEAM) if (p.chunk_rows) {   // prefix mode: member j is row s_row[j]
+            q0 = qall + ((size_t)s_row[row0 / p.group] * p.Hq + (size_t)kvh * p.group + row0 % p.group) * D;
+            q1 = qall + ((size_t)s_row[row1 / p.group] * p.Hq + (size_t)kvh * p.group + row1 % p.group) * D;
+        }
 #pragma unroll
         for (int kk = 0; kk < D / 16; ++kk) {
             const int c = kk * 16 + qcol;
@@ -633,15 +673,26 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map,
     // thread t finishes the output channels t, t + 128, ... < D
     constexpr int DPT = (D + 127) / 128;
     const int d0 = threadIdx.x;
+    // workspace row of MMA row r and split sp. BEAM: member i's partials sit at its position (b * beam_width or chunk_offsets[b]) + i,
+    // [B][Hkv][nsplit][group]
+    // (B rows, so the workspace of a plain launch on the rows holds them, and a position lies in [0, B) whatever the chunks hold)
+    auto ws_row = [&](int r, int sp) -> size_t {
+        if constexpr (BEAM)
+            return (((size_t)((p.chunk_rows ? s_flag[1] : b * nq()) + r / p.group) * p.Hkv + kvh) * p.nsplit + sp) * p.group + r % p.group;
+        else return (size_t)0;   // (not called)
+    };
     const size_t ws_base = ((size_t)bh * p.nsplit + split) * rows;
-    // output row of MMA row r: token (BEAM: beam) r / group, head kvh * group + r % group of out [B][q_len][Hq * D]
+    // output row of MMA row r: token (BEAM: member) r / group, head kvh * group + r % group of out [B][q_len][Hq * D]
     auto out_row = [&](int r) {
+        if constexpr (BEAM) if (p.chunk_rows)
+            return reinterpret_cast<T*>(p.out) + ((size_t)s_row[r / p.group] * p.Hq + (size_t)kvh * p.group + r % p.group) * D;
         return reinterpret_cast<T*>(p.out) + (((size_t)b * nq() + r / p.group) * p.Hq + (size_t)kvh * p.group + r % p.group) * D;
     };
     // per-CTA partial of the cluster merge: [rows][D] fp32 + (m, l) per row, behind the per-warp staging area
     float* part_o = l_s + kAttnConsumerWarps * 16;
     float* part_ml = part_o + RT * 16 * D;
     for (int r = 0; r < rows; ++r) {
+        if constexpr (BEAM) if (p.chunk_rows && s_row[r / p.group] == kNoRow) continue;   // a skipped member's rows are not written
         // row r is row rr of row tile r / 16, staged by the warps w = r / 16 + RT * j (j < NW)
         const int wt = RT == 1 ? 0 : r >> 4, rr = RT == 1 ? r : r & 15;
         float m = -INFINITY;
@@ -658,8 +709,8 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map,
                 part_ml[r * 2 + 0] = m;
                 part_ml[r * 2 + 1] = l;
             } else if (nact > 1) {
-                p.ws_ml[(ws_base + r) * 2 + 0] = m;
-                p.ws_ml[(ws_base + r) * 2 + 1] = l;
+                p.ws_ml[(BEAM ? ws_row(r, split) : ws_base + r) * 2 + 0] = m;
+                p.ws_ml[(BEAM ? ws_row(r, split) : ws_base + r) * 2 + 1] = l;
             }
         }
 #pragma unroll
@@ -671,7 +722,7 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map,
             for (int w = 0; w < NW; ++w) acc = fmaf(f[w], o_s[((size_t)(wt + RT * w) * 16 + rr) * OROW + d], acc);
             if (p.cluster_merge) part_o[r * D + d] = acc;
             else if (nact == 1) out_row(r)[d] = from_f32<T>(acc / l);
-            else p.ws_o[(ws_base + r) * D + d] = acc;
+            else p.ws_o[(BEAM ? ws_row(r, split) : ws_base + r) * D + d] = acc;
         }
     }
     if (p.cluster_merge) {
@@ -682,6 +733,7 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map,
         const int S = p.nsplit;
         const uint32_t o_addr = smem_u32(part_o), ml_addr = smem_u32(part_ml);
         for (int r = (int)cluster_ctarank(); r < rows; r += S) {
+            if constexpr (BEAM) if (p.chunk_rows && s_row[r / p.group] == kNoRow) continue;
             float mm[8], ll[8];
             float m = -INFINITY;
 #pragma unroll
@@ -731,16 +783,17 @@ paged_decode_attn_kernel(const __grid_constant__ CUtensorMap kv_map,
     if (!*s_flag) return;
     __threadfence();
     for (int r = 0; r < rows; ++r) {
+        if constexpr (BEAM) if (p.chunk_rows && s_row[r / p.group] == kNoRow) continue;
         float m = -INFINITY;
         for (int sp = 0; sp < nact; ++sp)
-            m = fmaxf(m, __ldcg(&p.ws_ml[(((size_t)bh * p.nsplit + sp) * rows + r) * 2 + 0]));
+            m = fmaxf(m, __ldcg(&p.ws_ml[(BEAM ? ws_row(r, sp) : ((size_t)bh * p.nsplit + sp) * rows + r) * 2 + 0]));
 #pragma unroll
         for (int j = 0; j < DPT; ++j) {
             const int d = d0 + 128 * j;
             if (d >= D) break;
             float acc = 0.f, l = 0.f;
             for (int sp = 0; sp < nact; ++sp) {
-                const size_t row = ((size_t)bh * p.nsplit + sp) * rows + r;
+                const size_t row = BEAM ? ws_row(r, sp) : ((size_t)bh * p.nsplit + sp) * rows + r;
                 const float fsp = fast_exp2((__ldcg(&p.ws_ml[row * 2 + 0]) - m) * sl2);
                 acc = fmaf(fsp, __ldcg(&p.ws_o[row * D + d]), acc);
                 l = fmaf(fsp, __ldcg(&p.ws_ml[row * 2 + 1]), l);

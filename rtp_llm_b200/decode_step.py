@@ -19,7 +19,7 @@ import torch
 
 from . import ops, rope
 from ._lib import B200_FMT_F16, B200_FMT_INT4, B200_FMT_INT8, B200_FMT_INT8G
-from .attention import beam_rows_fit
+from .attention import beam_rows_fit, prefix_rows_fit
 from .rope import LLAMA3, RopeSpec
 
 
@@ -198,6 +198,12 @@ class DecodeStep:
     would have to hold drafts 0..j-1. SamplingParams.min_p runs b200_sample with a min_p buffer when some value is not 0, and
     without one (today's kernel call) when every value is 0.
 
+    shared_prefix=(n, prefix_tokens) (TP 1, q_len 1, greedy, beam_width 1; op by op or under a CUDA graph, with or without PDL;
+    not in a decode program; the fused rope is off): groups of n requests, on rows a seeded permutation scatters over the batch,
+    share the whole pages of their first prefix_tokens that every member has cached. upload_inputs() computes the chunking with
+    ops.prefix_chunks, and the attention runs b200_paged_decode_attn_prefix where attention.prefix_rows_fit holds, else
+    b200_paged_decode_attn.
+
     tree=parents (q_len = n >= 2 nodes, greedy or sampled verification; TP 1, op by op or under a CUDA graph, with or without
     PDL; not in a decode program): verification of a speculative token tree. parents is one list of n entries for every request
     or one per request (parents[0] = -1, node j under parents[j] < j); set_tree() replaces it between replays. ids_h [B, n] holds
@@ -227,8 +233,18 @@ class DecodeStep:
                  logprobs: Optional[int] = None, eos_id: Optional[int] = None,
                  length_penalty: Union[float, Sequence[float]] = 1.0,
                  early_stopping: Union[bool, str, Sequence[Union[bool, str]]] = False,
-                 token_bitmask: bool = False, logit_bias_capacity: int = 0, tree=None):
+                 token_bitmask: bool = False, logit_bias_capacity: int = 0, tree=None, shared_prefix=None):
         assert cfg.head_num % tp_size == 0 and cfg.inter % tp_size == 0
+        if shared_prefix is not None:
+            n_share, p_tokens = shared_prefix
+            if not (n_share >= 1 and p_tokens >= 0):
+                raise ValueError(f"shared_prefix: (requests_per_prefix >= 1, prefix_tokens >= 0) (got {shared_prefix})")
+            if q_len != 1 or tree is not None or beam_width != 1 or sampling is not None or tp_size != 1:
+                raise ValueError(f"shared_prefix needs the greedy step: q_len 1, no tree, beam_width 1, no sampling and tp_size 1 "
+                                 f"(got q_len {q_len}, tree {tree is not None}, beam_width {beam_width}, sampling "
+                                 f"{sampling is not None}, tp_size {tp_size})")
+            fuse_rope = False       # (the fused rope runs its own attention; the shared-prefix path needs the rope kernel)
+        self.shared_prefix = shared_prefix
         if logit_bias_capacity < 0:
             raise ValueError(f"logit_bias_capacity must be >= 0 (got {logit_bias_capacity})")
         if (token_bitmask or logit_bias_capacity) and tp_size != 1:
@@ -450,6 +466,16 @@ class DecodeStep:
                         L["kv"][blk[b, 1:, f].long().to(device)] = L["kv"][int(blk[b, 0, f])].clone()
             self.ids_h.copy_(self.ids_h.view(-1, beam_width)[:, :1].expand(-1, beam_width).reshape(-1))
             self.shared_lens_h = (full * T).to(torch.int32).pin_memory()
+        if shared_prefix is not None:
+            # groups of n_share requests on rows a seeded permutation scatters over the batch; each group's members point at the
+            # first member's pages over the whole pages of the prefix that every member has cached, and at their own after them
+            # (so the token a step appends never lands in a shared page)
+            rows = torch.randperm(batch, generator=torch.Generator().manual_seed(seed + 71)).tolist()
+            for k in range(0, batch, n_share):
+                grp = rows[k:k + n_share]
+                f = min([p_tokens // T] + [int(self.seq_lens_h[r]) // T for r in grp])
+                for r in grp[1:]:
+                    self.block_ids_h[r, :f] = self.block_ids_h[grp[0], :f]
         self.next_h = torch.zeros(batch, dtype=torch.int32).pin_memory()
         if q_len > 1:
             self.drafts_h = torch.zeros(batch, q_len - 1, dtype=torch.int32).pin_memory()
@@ -486,6 +512,9 @@ class DecodeStep:
             self.tree_pos = buf(R, dt=torch.int32)
             self.accepted_path = buf(batch, q_len, dt=torch.int32)
             self.accepted_path_h = torch.zeros(batch, q_len, dtype=torch.int32).pin_memory()
+        if shared_prefix is not None:   # the chunking (ops.prefix_chunks), filled by upload_inputs
+            self.chunk_offsets_d, self.chunk_rows_d, self.chunk_shared_d = (buf(n, dt=torch.int32) for n in (batch + 1, batch, batch))
+            self.use_prefix = False
         if beam_width > 1:
             W, B = beam_width, self.requests
             self.beam_cum = buf(B, W, dt=torch.float32)
@@ -582,6 +611,15 @@ class DecodeStep:
         if self.q_len > 1:
             self.drafts_h.copy_(self.ids_h[:, 1:])
             self.drafts.copy_(self.drafts_h, non_blocking=True)
+        if self.shared_prefix is not None:    # the chunking of this batch composition, and which attention serves it
+            offs, rows, shared, mm = ops.prefix_chunks(self.block_ids_h, self.seq_lens_h, self.cfg.tokens_per_block,
+                                                       self.Hq // self.Hkv)
+            C = shared.numel()
+            self.chunk_offsets_d[:C + 1].copy_(offs, non_blocking=True)
+            self.chunk_rows_d.copy_(rows, non_blocking=True)
+            self.chunk_shared_d[:C].copy_(shared, non_blocking=True)
+            self.chunks = (self.chunk_offsets_d[:C + 1], self.chunk_rows_d, self.chunk_shared_d[:C], mm)
+            self.use_prefix = prefix_rows_fit(self.Hkv, C, float(shared.float().mean()), mm)
         if self.W > 1:        # back to the prompt: beam 0 alone live (cum 0), the input token as the whole history
             self.shared_lens.copy_(self.shared_lens_h, non_blocking=True)
             self.beam_cum.fill_(-math.inf)
@@ -747,6 +785,10 @@ class DecodeStep:
         elif self.q_len > 1:    # each query token attends up to its own position
             ops.paged_decode_attn_multi(self.q.view(self.B, self.q_len, self.Hq, self.D), L["kv"], self.page_list, self.seq_lens,
                                         self.ctx, self.attn_ws, out=self.attn.view(self.B, self.q_len, self.Hq * self.D))
+        elif self.shared_prefix is not None and self.use_prefix:    # a chunk's shared pages read once (prefix_rows_fit)
+            offs, rows, shared, mm = self.chunks
+            ops.paged_decode_attn_prefix(self.q, L["kv"], self.page_list, self.seq_lens, offs, rows, shared, mm, self.ctx,
+                                         self.attn_ws, out=self.attn)
         elif beam_rows_fit(self.Hq, self.Hkv, self.W, self.requests):
             ops.paged_decode_attn_beam(self.q.view(self.requests, self.W, self.Hq, self.D), L["kv"], self.page_list, self.seq_lens,
                                        self.shared_lens, self.ctx, self.attn_ws,
@@ -925,6 +967,8 @@ class DecodeStep:
         if self.samp is not None:
             raise ValueError("a sampling step runs op by op or under a CUDA graph, not as a decode program (its uniforms and "
                              "state updates are torch ops, not C-ABI calls)")
+        if self.shared_prefix is not None:
+            raise ValueError("a shared-prefix step runs op by op or under a CUDA graph, not as a decode program")
         self.prog = ops.Program()
         with self.prog.record():
             self.step_core()

@@ -157,6 +157,82 @@ def paged_decode_attn_beam(q: torch.Tensor, kv_cache_base: torch.Tensor, page_li
                        tuple(q.shape[:2]), q.shape[2], (shared_lengths, q_scale))
 
 
+def paged_decode_attn_prefix(q: torch.Tensor, kv_cache_base: torch.Tensor, page_list: torch.Tensor, sequence_lengths: torch.Tensor,
+                             chunk_offsets: torch.Tensor, chunk_rows: torch.Tensor, shared_lengths: torch.Tensor, max_members: int,
+                             max_seq_len: int, workspace: torch.Tensor, out: Optional[torch.Tensor] = None,
+                             q_scale: float = 1.0) -> torch.Tensor:
+    """paged_decode_attn on q [B, Hq, D] with the rows grouped into chunks that read their shared leading pages once: chunk c is
+    the rows chunk_rows[chunk_offsets[c] : chunk_offsets[c + 1]] (int32 [chunks + 1] and [B], at most max_members rows each),
+    whose page_list rows are equal over the first shared_lengths[c] / T pages (int32 [chunks]). prefix_chunks builds the three
+    from a block table. Rows in no chunk are not written. Returns [B, Hq*D]."""
+    who = "paged_decode_attn_prefix"
+    _cuda_contig(q, kv_cache_base, page_list, sequence_lengths, chunk_offsets, chunk_rows, shared_lengths, workspace, out)
+    P, two, Hkv, T, D = kv_cache_base.shape
+    B = q.shape[0]
+    C = shared_lengths.numel()
+    _need(who, "chunk_offsets", chunk_offsets, torch.int32, (C + 1,), flat=True)
+    _need(who, "chunk_rows", chunk_rows, torch.int32, (B,), flat=True)
+    _need(who, "shared_lengths", shared_lengths, torch.int32, ("chunks",))
+    Hq = q.numel() // (B * D)
+    out = _outputs(who, {"attn_out": out}, q.device, attn_out=(q.dtype, (B, Hq * D)))["attn_out"]
+    check(_lib.load().b200_paged_decode_attn_prefix(
+        _p(q), _is_bf16(q), _p(out), Hq, Hkv, D, B, C, max_members, _p(chunk_offsets), _p(chunk_rows), _p(shared_lengths),
+        page_list.shape[-1], max_seq_len, T, _p(kv_cache_base), _p(page_list), _p(sequence_lengths), q_scale, _p(workspace),
+        workspace.numel(), _stream()), "b200_" + who)
+    return out
+
+
+def prefix_chunks(block_ids: torch.Tensor, sequence_lengths: torch.Tensor, tokens_per_block: int,
+                  group: int) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, int]:
+    """The chunking of paged_decode_attn_prefix for a batch, from host int32 tensors block_ids [B, M] and sequence_lengths [B]
+    (tokens cached) and the GQA group (head_num / kv_head_num). Rows whose block-table rows start with the same block are
+    candidates; only blocks a row has wholly cached count (the token a step appends never lands in a shared block). Among them,
+    the rows that agree with the first row on at least k whole blocks form a group sharing k * tokens_per_block tokens, k picked
+    to maximise the blocks read once fewer ((rows - 1) * k); the rest are grouped again the same way. A row that shares no whole
+    block with another becomes a chunk of one sharing 0 tokens, as does a row left alone after groups are cut, in row order,
+    into chunks of at most 64 // group rows. Returns (chunk_offsets [chunks + 1], chunk_rows [B], shared_lengths [chunks],
+    max_members), int32 host tensors and an int. Meant to run once per batch composition, not per step."""
+    if block_ids.dtype != torch.int32 or block_ids.dim() != 2 or block_ids.is_cuda:
+        raise B200Error("prefix_chunks: block_ids must be a host int32 [B, M] tensor")
+    B, M = block_ids.shape
+    _need("prefix_chunks", "sequence_lengths", sequence_lengths, torch.int32, (B,), flat=True)
+    if sequence_lengths.is_cuda or B == 0 or tokens_per_block < 1 or not 1 <= group <= 64:
+        raise B200Error(f"prefix_chunks: need host tensors, B >= 1, tokens_per_block >= 1 and group in 1..64 (got B {B}, "
+                        f"tokens_per_block {tokens_per_block}, group {group})")
+    ids = block_ids.tolist()
+    whole = [min(int(n) // tokens_per_block, M) for n in sequence_lengths.reshape(-1).tolist()]
+    candidates = {}
+    for r in range(B):
+        candidates.setdefault(ids[r][0] if M else -1 - r, []).append(r)
+    groups = []                                   # (rows, shared blocks)
+    for members in candidates.values():
+        first = ids[members[0]]
+        common = {members[0]: whole[members[0]]}  # whole blocks each member shares with the first
+        for r in members[1:]:
+            n = min(whole[r], whole[members[0]])
+            common[r] = next((j for j in range(n) if ids[r][j] != first[j]), n)
+        rest = members
+        while len(rest) > 1:
+            k = max(set(common[r] for r in rest), key=lambda k: (sum(common[r] >= k for r in rest) - 1) * k)
+            sub = [r for r in rest if common[r] >= k]
+            if k == 0 or len(sub) < 2:
+                break
+            groups.append((sub, k))
+            rest = [r for r in rest if common[r] < k]
+        groups += [([r], 0) for r in rest]
+    cap = 64 // group
+    offsets, rows, shared = [0], [], []
+    for members, k in groups:
+        for c in range(0, len(members), cap):
+            chunk = members[c:c + cap]
+            rows += chunk
+            offsets.append(len(rows))
+            shared.append(k * tokens_per_block if len(chunk) > 1 else 0)
+    max_members = max(b - a for a, b in zip(offsets, offsets[1:]))
+    i32 = dict(dtype=torch.int32)
+    return torch.tensor(offsets, **i32), torch.tensor(rows, **i32), torch.tensor(shared, **i32), max_members
+
+
 def paged_decode_attn_tree(q: torch.Tensor, kv_cache_base: torch.Tensor, page_list: torch.Tensor, sequence_lengths: torch.Tensor,
                            tree_parents: torch.Tensor, max_seq_len: int, workspace: torch.Tensor, out: Optional[torch.Tensor] = None,
                            q_scale: float = 1.0) -> torch.Tensor:

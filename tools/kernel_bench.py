@@ -185,6 +185,41 @@ def bench_attn_beam(B, W, Hq, Hkv, S=2048, T=64, private=28, nrot=3, runs=3):
     return med
 
 
+def bench_attn_prefix(B, n, shared, pools, Hq=32, Hkv=8, S=2048, T=64, runs=3):
+    """b200_paged_decode_attn_prefix against b200_paged_decode_attn on the same B rows and page tables: groups of n requests
+    share the pages of their first `shared` tokens and own the pages after them; the groups' rows are scattered over the batch.
+    The chunking is ops.prefix_chunks' (chunks of up to 64 / group rows). pools: the nrot K/V pools (> L2 together), reused
+    across calls. GB/s as in attn-beam: distinct K/V bytes (a group's shared pages once) over kernel time."""
+    M, nrot = math.ceil(S / T), len(pools)
+    g = torch.Generator().manual_seed(B * 1000 + n * 10 + shared)
+    ids = iter((torch.randperm(pools[0].shape[0] - 1, generator=g) + 1).tolist())
+    rows = torch.randperm(B, generator=g).tolist()
+    bid = torch.zeros(B, M, dtype=torch.int32)
+    for k in range(0, B, n):
+        common = [next(ids) for _ in range(shared // T)]
+        for r in rows[k:k + n]:
+            bid[r] = torch.tensor(common + [next(ids) for _ in range(M - len(common))], dtype=torch.int32)
+    seq_h = torch.full((B,), S - 1, dtype=torch.int32)
+    offs, crow, sh, mm = (t.to(dev) if torch.is_tensor(t) else t for t in ops.prefix_chunks(bid, seq_h, T, Hq // Hkv))
+    pl, seq = ops.convert_block_table(bid.to(dev)), seq_h.to(dev)
+    q = torch.randn(B, Hq, 128, device=dev).half()
+    ws = ops.attn_workspace(B, Hq, Hkv, S, dev)
+    out = torch.empty(B, Hq * 128, device=dev).half()
+    arms = {"per row": lambda i: ops.paged_decode_attn(q, pools[i], pl, seq, S, ws, out=out),
+            "prefix": lambda i: ops.paged_decode_attn_prefix(q, pools[i], pl, seq, offs, crow, sh, mm, S, ws, out=out)}
+    t = {k: [] for k in arms}
+    for _ in range(runs):
+        for k, fn in arms.items():
+            t[k].append(timeit(fn, nrot))
+    groups = math.ceil(B / n)
+    byt = 2 * (groups * shared + B * (S - shared)) * Hkv * 128 * 2
+    med = {k: sorted(v)[len(v) // 2] for k, v in t.items()}
+    print(f"attn-prefix B{B} group of {n} sharing {shared} (chunks {offs.numel() - 1}, max_members {mm}, {byt / 1e6:.0f} MB distinct "
+          f"K/V): " + ", ".join(f"{k} {med[k]:.1f} us (min {min(t[k]):.1f}, max {max(t[k]):.1f}; {byt / med[k] / 1e3:.0f} GB/s)"
+                                for k in arms) + f"; prefix / per row = {med['prefix'] / med['per row']:.2f}", flush=True)
+    return med
+
+
 def bench_beam(B, W, V=128256, ngram=0, hist=2048, nrot=8):
     """b200_beam_search_step on fp16 logits [B*W, V] (rotated through nrot sets, > L2), preceded by b200_ban_repeat_ngram
     over `hist` history tokens per row when ngram > 0."""
@@ -487,6 +522,20 @@ if __name__ == "__main__":
               + " (name, power limit, SM clock, max SM clock)", flush=True)
         for B, W, Hq in ((8, 4, 32), (32, 4, 32), (4, 16, 32), (16, 8, 32), (16, 8, 64), (8, 2, 32), (8, 8, 32)):
             bench_attn_beam(B, W, Hq, 8)
+    if "attn-prefix" in which:
+        # rows of different requests sharing a cached prompt, Llama-3-8B heads (group 4), ctx 2048, pages of 64 tokens, against
+        # one CTA per row; every row's tokens on distinct pages of three pools (1 GB each at B 128)
+        import subprocess
+        print("attn-prefix on " + (subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader",
+                                                   "-i", "0"], capture_output=True, text=True).stdout.strip() or "unknown card")
+              + " (name, power limit, SM clock, max SM clock)", flush=True)
+        for B in (32, 64, 128):
+            pools = [torch.randn(B * 32 + 1, 2, 8, 64, 128, device=dev, dtype=torch.float16) for _ in range(3)]
+            for n in (2, 4, 8, 16, 32):
+                for shared in (512, 1024, 1536):
+                    bench_attn_prefix(B, n, shared, pools)
+            del pools
+            torch.cuda.empty_cache()
     if "beam" in which:
         # beam search over Llama-3's vocabulary, with and without the 3-gram ban over 2048 history tokens, alternating
         for B, W in ((8, 4), (32, 4), (4, 16)):

@@ -13,6 +13,9 @@ each a step captured in a CUDA graph with PDL at --ctx tokens; the first arm is 
   qwen3      Qwen3-8B INT4: qk_rmsnorm, then the plain rope launch (TwoLaunchStep), against the fused QK-norm append
   tree       Llama-3-8B INT4: per q_len 4 and 8 with batch * q_len <= 128, the chain verification step, then the token-tree
              step on a binary tree of q_len nodes (tree attention, spec_verify_tree and the K/V compaction)
+  prefix     Llama-3-8B INT4: the shared-prefix step (1024 prompt tokens shared by groups of 8 requests) with
+             b200_paged_decode_attn on every row, then with b200_paged_decode_attn_prefix for groups of 8 and of 32
+             (PrefixStep forces the kernel either way); prints which kernel attention.prefix_rows_fit picks
   constrain  Llama-3-8B INT4: greedy, greedy with a 50 % random token bitmask and 300 logit_bias entries per row, sampled
              (temperature 0.8, top-k 50, top-p 0.9), sampled with the same constraints
 
@@ -38,6 +41,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from rtp_llm_b200 import ops  # noqa: E402
+from rtp_llm_b200.attention import prefix_rows_fit  # noqa: E402
 from rtp_llm_b200.decode_step import LLAMA3_8B, LLAMA31_8B, QWEN3_8B, DecodeStep, SamplingParams  # noqa: E402
 from tests.step_oracle import TwoLaunchStep  # noqa: E402
 from tests.test_gpu_beam_attn import PerRowBeamStep  # noqa: E402
@@ -131,6 +135,33 @@ def constrain_arms(a, cfg, B, dev):
     return arms
 
 
+class PrefixStep(DecodeStep):
+    """The shared-prefix step with its attention forced: b200_paged_decode_attn_prefix (prefix True) or b200_paged_decode_attn
+    on every row (False), whatever attention.prefix_rows_fit says."""
+
+    def __init__(self, *args, prefix: bool, **kw):
+        self.force_prefix = prefix
+        super().__init__(*args, **kw)
+
+    def upload_inputs(self):
+        super().upload_inputs()
+        self.use_prefix = self.force_prefix
+
+
+def prefix_arms(a, cfg, B, dev):
+    kw = dict(pdl=True)
+    models = [PrefixStep(cfg, B, a.ctx, dev, shared_prefix=(8, 1024), prefix=False, **kw)]
+    models += [PrefixStep(cfg, B, a.ctx, dev, shared_prefix=(n, 1024), prefix=True, **kw) for n in (8, 32)]
+    arms = [step_arm(name, m) for name, m in zip(("per row, groups of 8", "prefix kernel, groups of 8",
+                                                   "prefix kernel, groups of 32"), models)]
+    for m in models:
+        offs, _, shared, mm = m.chunks
+        fit = prefix_rows_fit(m.Hkv, shared.numel(), float(shared.float().mean()), mm)
+        print(f"B{B} {m.shared_prefix}: {shared.numel()} chunks of up to {mm} rows; attention.prefix_rows_fit picks "
+              f"{'the prefix kernel' if fit else 'the per-row kernel'}", flush=True)
+    return arms
+
+
 def tree_arms(a, cfg, B, dev):
     arms = []
     for n in (4, 8):
@@ -149,7 +180,7 @@ def qwen3_arms(a, cfg, B, dev):
 # name: arms, default batches, timed replays per run, warm-up replays
 PRESETS = {"act-order": (act_order_arms, [32], 100, 10), "spec": (spec_arms, [8, 16, 32], 50, 3),
            "beam": (beam_arms, [8], 20, 3), "sample": (sample_arms, [8, 32], 20, 3), "qwen3": (qwen3_arms, [8, 16, 32], 100, 10),
-           "constrain": (constrain_arms, [8, 32], 50, 5), "tree": (tree_arms, [8, 16, 32], 50, 3)}
+           "constrain": (constrain_arms, [8, 32], 50, 5), "tree": (tree_arms, [8, 16, 32], 50, 3), "prefix": (prefix_arms, [32, 64], 50, 5)}
 MODELS = {"llama3": LLAMA3_8B, "llama31": LLAMA31_8B}
 
 
