@@ -197,7 +197,7 @@ int b200_pack_w8g(const int8_t* q, const void* scales, const void* zeros_x_scale
 
 /* Scratch for split-K / stream-K partials + semaphores (+ the grid-barrier words of a stand-alone call); zero-fill once
  * after allocation (the kernels leave the semaphores at zero). Required for INT8 / INT4 weights, and for any weight format
- * whose split-K plan splits K (at least 24 KiB); b200_wo_gemm rejects a smaller one. */
+ * whose split-K plan splits K (at least 24 KiB); b200_wo_gemm rejects a smaller one. max_batch 1..256 (0 outside). */
 size_t b200_wo_gemm_workspace_bytes(int max_batch, int N, int K);
 
 /* Y[B][N] = X[B][K] . W' (+ bias).  The compute behind LinearBase.forward
@@ -206,7 +206,8 @@ size_t b200_wo_gemm_workspace_bytes(int max_batch, int N, int K);
  *   w         B200_FMT_INT4/INT4_G64/INT4_G32/INT8/INT8G: blob from b200_pack_w4/8/8g; B200_FMT_F16: W [N][K] (K contiguous)
  *   col_scale INT8 only: [N] per-column scale in the activation type
  *   bias      optional [N]
- * B <= 128, K % 128 == 0, x / y / w 16-byte aligned. */
+ * B 1..256 (129..256 rows run one CTA per 128 features over all of them: each weight block is read and dequantised once),
+ * K % 128 == 0, x / y / w 16-byte aligned. */
 int b200_wo_gemm(int fmt, int is_bf16, const void* x, int B, int K, int N, const void* w, const void* col_scale,
                  const void* bias, void* y, void* workspace, size_t workspace_bytes, int flags, void* stream);
 
@@ -494,7 +495,7 @@ int b200_peer_allreduce_norm(const void* in, void* residual, const void* gamma, 
  * registers; the columns this rank owns are stored to y. MUST be followed on the same stream by b200_peer_gather_norm over
  * the same y / regions with no other collective of this communicator in between (both derive the exchange epoch from the
  * communicator's device-side call counter). Bits are those of b200_wo_gemm + b200_peer_allreduce_norm.
- * N % 128 == 0, N % (8*world) == 0, N <= 8192, B*N*2 <= max_message_bytes, no SILU_MUL, not B200_FMT_INT4_G64 / _G32. */
+ * B <= 128, N % 128 == 0, N % (8*world) == 0, N <= 8192, B*N*2 <= max_message_bytes, no SILU_MUL, not B200_FMT_INT4_G64 / _G32. */
 int b200_wo_gemm_rs(int fmt, int is_bf16, const void* x, int B, int K, int N, const void* w, const void* col_scale,
                     const void* bias, void* y, void* workspace, size_t workspace_bytes, int flags, void* const* regions,
                     size_t max_message_bytes, int rank, int world, void* stream);

@@ -186,7 +186,8 @@ AttnWorkspace attn_workspace(size_t batch, size_t head_num, size_t kv_head_num, 
 }
 
 // ---- GEMM launch shape
-int gemm_bpad(int B) { return B <= 16 ? 16 : (B <= 32 ? 32 : (B <= 64 ? 64 : 128)); }
+constexpr int kGemmMaxRows = 256;   // rows per b200_wo_gemm call (batch pad 256); the reduce-scatter GEMM takes up to 128
+int gemm_bpad(int B) { return B <= 16 ? 16 : (B <= 32 ? 32 : (B <= 64 ? 64 : (B <= 128 ? 128 : 256))); }
 // one-kernel-per-GEMM path (gemm_cluster.cu): split-K so that one wave of 2*SMs CTAs is filled. The nsplit CTAs of a tile
 // merge their partials through L2 (at most 8 slots; the reduce-scatter GEMM merges them in a thread-block cluster, and 8 is
 // the portable cluster size). The GPC rule below stays from the cluster merge, which needs a cluster's CTAs in one GPC: it
@@ -681,12 +682,13 @@ int b200_pack_w8g(const int8_t* q, const void* scales, const void* zeros_x_scale
 }
 
 size_t b200_wo_gemm_workspace_bytes(int max_batch, int N, int K) {
-    if (max_batch <= 0 || N <= 0 || K <= 0 || K % kGemmBK) return 0;
-    const int n_tiles = (N + kGemmTileN - 1) / kGemmTileN;
+    if (max_batch <= 0 || max_batch > kGemmMaxRows || N <= 0 || K <= 0 || K % kGemmBK) return 0;
+    const int n_tiles = (N + kGemmTileN - 1) / kGemmTileN, bpad = gemm_bpad(max_batch);
     // partials of the plain kernel's split-K plan (any batch <= max_batch has a batch pad no larger) and of the persistent
-    // kernel's, sized for its largest grid (2 CTAs per SM); the two never run at once, so they share the room
-    const size_t plain = gemm_partial_bytes(n_tiles, K / kGemmBK, gemm_bpad(max_batch));
-    const size_t persistent = sk_ws_bytes(n_tiles, K / kGemmBK, 2 * num_sms(), gemm_bpad(max_batch));
+    // kernel's, sized for its largest grid (2 CTAs per SM); the two never run at once, so they share the room. The persistent
+    // kernel holds no GEMM at batch pad 256 (seg_capable), so none is sized there.
+    const size_t plain = gemm_partial_bytes(n_tiles, K / kGemmBK, bpad);
+    const size_t persistent = bpad <= 128 ? sk_ws_bytes(n_tiles, K / kGemmBK, 2 * num_sms(), bpad) : 0;
     return kGemmSemBytes + (plain > persistent ? plain : persistent);
 }
 
@@ -699,7 +701,7 @@ static int wo_gemm_impl(int fmt, int is_bf16, const void* x, int B, int K, int N
                   fmt == B200_FMT_INT4_G32,
               "wo_gemm: unknown weight format %d", fmt);
     ARG_CHECK(x && w && y, "wo_gemm: null pointer");
-    ARG_CHECK(B > 0 && B <= 128, "wo_gemm: batch %d unsupported (1..128 per call)", B);
+    ARG_CHECK(B > 0 && B <= kGemmMaxRows, "wo_gemm: batch %d unsupported (1..%d per call)", B, kGemmMaxRows);
     ARG_CHECK(K > 0 && K % kGemmBK == 0, "wo_gemm: K=%d must be a positive multiple of 128", K);
     ARG_CHECK(N > 0, "wo_gemm: N must be positive");
     ARG_CHECK(fmt != B200_FMT_INT8 || col_scale, "wo_gemm: INT8 needs col_scale");
@@ -800,6 +802,7 @@ int b200_wo_gemm_rs(int fmt, int is_bf16, const void* x, int B, int K, int N, co
                     const void* bias, void* y, void* workspace, size_t workspace_bytes, int flags, void* const* regions,
                     size_t max_message_bytes, int rank, int world, void* stream) {
     ARG_CHECK(regions, "wo_gemm_rs: null regions");
+    ARG_CHECK(B <= 128, "wo_gemm_rs: batch %d unsupported (1..128 per call; b200_wo_gemm takes up to %d rows)", B, kGemmMaxRows);
     ARG_CHECK(fmt != B200_FMT_INT4_G64 && fmt != B200_FMT_INT4_G32, "wo_gemm_rs: INT4 group-64 / group-32 weights (format %d) unsupported", fmt);
     ARG_CHECK(valid_peer_group(rank, world), "wo_gemm_rs: bad rank/world %d/%d", rank, world);
     ARG_CHECK(N % 128 == 0 && N % (8 * world) == 0 && N <= 8192, "wo_gemm_rs: N=%d must be a multiple of 128 and of 8*world, <= 8192", N);

@@ -16,7 +16,7 @@ int b200_wo_gemm_max_active_clusters(int cluster_size, int* num_clusters) {
     if (rc) return rc;
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(1, cluster_size);
-    cfg.blockDim = dim3(gemm_threads());
+    cfg.blockDim = dim3(gemm_threads(32));
     cfg.dynamicSmemBytes = smem;
     cudaLaunchAttribute attr;
     attr.id = cudaLaunchAttributeClusterDimension;

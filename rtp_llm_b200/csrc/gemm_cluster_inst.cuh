@@ -23,7 +23,7 @@ int launch_one(const CUtensorMap& xmap, const CUtensorMap& wmap, const ParamsT& 
     // VAR 1, nsplit > 1: the nsplit CTAs of a tile form one cluster along y; the plain kernels launch single CTAs
     const dim3 grid(n_tiles, p.nsplit), cluster(1, B200_GEMM_VAR == 1 ? p.nsplit : 1);
     return launch_or_record("wo_gemm_kernel", st, [=](cudaStream_t s) {
-        return launch_ex(kern, {grid, dim3(gemm_threads()), smem, s, p.use_pdl != 0, cluster}, xmap, wmap, p);
+        return launch_ex(kern, {grid, dim3(gemm_threads(BPAD)), smem, s, p.use_pdl != 0, cluster}, xmap, wmap, p);
     });
 }
 
@@ -33,6 +33,9 @@ int by_bpad(int bpad, const CUtensorMap& xmap, const CUtensorMap& wmap, const Pa
         case 16: return launch_one<FMT, T, 16>(xmap, wmap, p, n_tiles, st);
         case 32: return launch_one<FMT, T, 32>(xmap, wmap, p, n_tiles, st);
         case 64: return launch_one<FMT, T, 64>(xmap, wmap, p, n_tiles, st);
+#if B200_GEMM_VAR == 0   // batch pad 256: plain output only (b200_wo_gemm_rs takes up to 128 rows)
+        case 256: return launch_one<FMT, T, 256>(xmap, wmap, p, n_tiles, st);
+#endif
         default: return launch_one<FMT, T, 128>(xmap, wmap, p, n_tiles, st);
     }
 }

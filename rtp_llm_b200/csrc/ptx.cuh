@@ -264,6 +264,12 @@ __device__ __forceinline__ bool elect_one() {
 // d[4i+0..1] = (row g, columns 8i+2t, 8i+2t+1) and d[4i+2..3] = (row g+8, same columns). A from registers uses the
 // mma.m16n8k16 A fragment per warp: a[0] = (row g, k 2t..2t+1), a[1] = (row g+8, k 2t..), a[2] = (row g, k 2t+8..),
 // a[3] = (row g+8, k 2t+8..).
+// Moves registers between the warpgroups of a CTA (sm_90a): .dec returns this warpgroup's surplus to the CTA's pool, .inc
+// waits until the pool holds enough. Executed by all 128 threads of a warpgroup.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
@@ -420,6 +426,30 @@ __device__ __forceinline__ void wgmma_ss<128, __nv_bfloat16>(float (&d)[64], uin
         "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
         : "l"(a_desc), "l"(b_desc), "r"(scale_d));
+}
+// N 256: two m64n128k16 on the column halves of D that share A, which is what m64n256k16 computes (D's layout above puts
+// columns 128..255 in d[64..127]). B rows 128..255 of a K-major SW128 operand lie 128 rows x 128 B further, whole swizzle atoms
+// away: +1024 in the descriptor's start field.
+__device__ __forceinline__ float (&wgmma_d_half(float (&d)[128], int h))[64] { return *reinterpret_cast<float(*)[64]>(d + 64 * h); }
+template <>
+__device__ __forceinline__ void wgmma_rs<256, __half>(float (&d)[128], const uint32_t (&a)[4], uint64_t b_desc, uint32_t scale_d) {
+    wgmma_rs<128, __half>(wgmma_d_half(d, 0), a, b_desc, scale_d);
+    wgmma_rs<128, __half>(wgmma_d_half(d, 1), a, b_desc + 1024, scale_d);
+}
+template <>
+__device__ __forceinline__ void wgmma_rs<256, __nv_bfloat16>(float (&d)[128], const uint32_t (&a)[4], uint64_t b_desc, uint32_t scale_d) {
+    wgmma_rs<128, __nv_bfloat16>(wgmma_d_half(d, 0), a, b_desc, scale_d);
+    wgmma_rs<128, __nv_bfloat16>(wgmma_d_half(d, 1), a, b_desc + 1024, scale_d);
+}
+template <>
+__device__ __forceinline__ void wgmma_ss<256, __half>(float (&d)[128], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+    wgmma_ss<128, __half>(wgmma_d_half(d, 0), a_desc, b_desc, scale_d);
+    wgmma_ss<128, __half>(wgmma_d_half(d, 1), a_desc, b_desc + 1024, scale_d);
+}
+template <>
+__device__ __forceinline__ void wgmma_ss<256, __nv_bfloat16>(float (&d)[128], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+    wgmma_ss<128, __nv_bfloat16>(wgmma_d_half(d, 0), a_desc, b_desc, scale_d);
+    wgmma_ss<128, __nv_bfloat16>(wgmma_d_half(d, 1), a_desc, b_desc + 1024, scale_d);
 }
 
 }  // namespace b200

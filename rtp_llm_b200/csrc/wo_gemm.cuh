@@ -52,9 +52,15 @@ __host__ __device__ constexpr int gemm_w_bytes(int fmt) {
 // whole dequant -> MMA chain, and the bytes in flight per SM (Little's law: bandwidth per SM * latency) stay high.
 // 8 dequant warps = two warpgroups, each the MMA issuer of its 64 feature rows (see the dequant section of the kernel).
 __host__ __device__ constexpr int gemm_ndq_warps() { return 8; }
-__host__ __device__ constexpr int gemm_threads() { return (gemm_ndq_warps() + 2) * 32; }
+// + the two producer warps; at batch pad 256 they fill a warpgroup of their own (two warps idle), so that setmaxnreg can hand
+// the consumers the registers of 256 fp32 accumulator columns (kGemmConsumerRegs)
+__host__ __device__ constexpr int gemm_threads(int bpad) { return (gemm_ndq_warps() + (bpad <= 128 ? 2 : 4)) * 32; }
+// registers per thread after the rebalancing at batch pad 256: 2 x 128 consumers at 232 and 128 producers at 40 take the
+// 384 x 168 the launch allocates (64512 of the SM's 65536)
+constexpr int kGemmConsumerRegs = 232, kGemmProducerRegs = 40;
 __host__ __device__ constexpr int gemm_x_stage_bytes(int bpad) { return bpad * 256; }
-__host__ __device__ constexpr int gemm_x_stages(int bpad) { return bpad <= 32 ? 4 : 3; }
+// batch pad 256: a 64 KB activation stage per block, so two stages, next to a weight ring
+__host__ __device__ constexpr int gemm_x_stages(int bpad) { return bpad <= 32 ? 4 : (bpad <= 128 ? 3 : 2); }
 constexpr int kGemmSmemMisc = 1024 /*align*/ + 1024 /*barriers*/;
 __host__ __device__ constexpr int gemm_w_stages_for(int fmt, int bpad, int budget, int xs) {
     int n = (budget - kGemmSmemMisc - xs * gemm_x_stage_bytes(bpad)) / gemm_w_bytes(fmt);
@@ -70,8 +76,11 @@ __host__ __device__ constexpr int gemm_cluster_x_stages(int fmt, int bpad) {
 __host__ __device__ constexpr int gemm_min_ctas(int fmt, int bpad) {
     return gemm_w_stages_for(fmt, bpad, 106 * 1024, gemm_cluster_x_stages(fmt, bpad)) >= 4 ? 2 : 1;
 }
+// One CTA per SM takes 216 KB up to batch pad 128; batch pad 256 takes the 227 KB an SM allows one CTA, which keeps 3
+// FP16 weight stages (32 KB each) next to its two 64 KB activation stages.
 __host__ __device__ constexpr int gemm_w_stages(int fmt, int bpad) {
-    return gemm_w_stages_for(fmt, bpad, gemm_min_ctas(fmt, bpad) == 2 ? 106 * 1024 : 216 * 1024, gemm_cluster_x_stages(fmt, bpad));
+    return gemm_w_stages_for(fmt, bpad, gemm_min_ctas(fmt, bpad) == 2 ? 106 * 1024 : (bpad <= 128 ? 216 : 227) * 1024,
+                             gemm_cluster_x_stages(fmt, bpad));
 }
 __host__ __device__ constexpr int gemm_smem_bytes(int fmt, int bpad) {
     return gemm_cluster_x_stages(fmt, bpad) * gemm_x_stage_bytes(bpad) + gemm_w_stages(fmt, bpad) * gemm_w_bytes(fmt) + kGemmSmemMisc;
@@ -406,7 +415,7 @@ __device__ __forceinline__ bool l2_merge(const GemmParams& p, float (&acc)[NACC]
 }
 
 template <int FMT, typename T, int BPAD, int VAR>
-__global__ void __launch_bounds__(gemm_threads(), gemm_min_ctas(FMT, BPAD))
+__global__ void __launch_bounds__(gemm_threads(BPAD), gemm_min_ctas(FMT, BPAD))
 wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant__ CUtensorMap w_map,
                const typename GemmParamsOf<VAR>::type p) {
     constexpr int WS = gemm_w_stages(FMT, BPAD);           // weight ring depth
@@ -418,6 +427,7 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
     constexpr int W_BYTES = gemm_w_bytes(FMT);
     constexpr int NACC = BPAD / 2;                         // fp32 accumulators per thread (m64 x BPAD per warpgroup)
     static_assert(WS >= 3, "weight ring too shallow");
+    static_assert(gemm_smem_bytes(FMT, BPAD) <= 227 * 1024, "rings exceed an SM's shared memory");
 
     // 1024-byte alignment is required by the 128B-swizzled tiles. The array is DECLARED aligned (the kernel has no static
     // shared memory, so the dynamic segment starts at the aligned window base) and checked once; keeping the pointer's
@@ -449,6 +459,7 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
         fence_mbar_init();
     }
     __syncthreads();
+    if (BPAD == 256 && warp >= NDQ_WARPS) setmaxnreg_dec<kGemmProducerRegs>();
 
     if (warp == W_WTMA) {
         // ------------------------------------------------------------------ weight producer (HBM stream)
@@ -497,8 +508,9 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
                 }
             }
         }
-    } else {
+    } else if (BPAD <= 128 || warp < NDQ_WARPS) {   // (batch pad 256: warps 10 and 11 only pad the producer warpgroup)
         // ------------------------------------------------------------------ dequant + MMA warpgroups
+        if constexpr (BPAD == 256) setmaxnreg_inc<kGemmConsumerRegs>();   // (dominates the consumer code: ptxas allocates it 232)
         // Warpgroup g (warps 4g..4g+3) owns feature rows 64g..64g+63 of the tile: each warp dequantises its 16 rows of every
         // k-block into wgmma A fragments in registers and the warpgroup multiplies them with the activation block from
         // shared memory (wgmma, A from registers, B K-major SW128), fp32 accumulators in registers. The FP16-weight variant
@@ -619,7 +631,9 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant_
                     if (p.bias) bias[h] = to_f32<T>(reinterpret_cast<const T*>(p.bias)[n]);
                 }
             }
-            float* fin = reinterpret_cast<float*>(wring);       // [bpad][128] fp32 staging for the fused SiLU*mul (weight ring is idle)
+            // [bpad][128] fp32 staging for the fused SiLU*mul in an idle ring: the weight ring, or at batch pad 256 (128 KB, more
+            // than its weight ring holds) the activation ring, whose two 64 KB stages it fills exactly
+            float* fin = reinterpret_cast<float*>(BPAD == 256 ? xring : wring);
             RsLane rsl[2] = {};
             if constexpr (VAR == 1) {
                 rsl[0] = rs_lane(p, tile * kGemmTileN + rows[0]);

@@ -22,6 +22,10 @@ from ._lib import B200_FMT_F16, B200_FMT_INT4, B200_FMT_INT8, B200_FMT_INT8G
 from .attention import beam_rows_fit, prefix_rows_fit
 from .rope import LLAMA3, RopeSpec
 
+# token rows per step: b200_wo_gemm takes up to 256 per call; the TP exchange (b200_wo_gemm_rs and the peer collectives) is
+# built for up to 128, and so is DecodeStep's default max_rows of the verification, tree, beam and sampling modes
+GEMM_MAX_ROWS, TP_MAX_ROWS = 256, 128
+
 
 @dataclasses.dataclass
 class ModelConfig:
@@ -182,7 +186,7 @@ class DecodeStep:
     hypotheses stay as they are. beam_results(n) returns the n best per request, the live beams merged in for requests that are
     not done. upload_inputs() empties the sets and done. With eos_id None the step is the beam step without EOS.
 
-    sampling=SamplingParams (TP 1, beam_width 1, batch * q_len <= 128, op by op or under a CUDA graph; not in a decode program):
+    sampling=SamplingParams (TP 1, beam_width 1, batch * q_len <= max_rows, op by op or under a CUDA graph; not in a decode program):
     sampled decoding. The per-request parameters sit in static device buffers; after the lm_head the step copies the logits to a
     static fp32 buffer (samp_logits: b200_sample works in place and leaves the probabilities there), runs ban_repeat_ngram when
     no_repeat_ngram > 0, then b200_sample with the row's token history for the penalties. Its uniforms (one per row, `uniform`)
@@ -223,7 +227,12 @@ class DecodeStep:
     reads the logits: on self.logits before argmax (greedy and greedy verification; row j of a verification step carries the
     mask of position j), on samp_logits after the fp32 copy and before the n-gram ban and b200_sample (sampling and sampled
     verification), on self.logits before the n-gram ban and beam_search_step (beam: one row per beam, before the
-    log-softmax). The log-probs keep scoring the raw lm_head output. Without these options the step's launches are unchanged."""
+    log-softmax). The log-probs keep scoring the raw lm_head output. Without these options the step's launches are unchanged.
+
+    Token rows (batch * beam_width * q_len): every GEMM of the step takes up to 256 rows in one launch, so the greedy step runs
+    up to 256 rows (128 with tp_size > 1, the TP exchange's limit). The verification, tree, beam and sampling modes accept up
+    to max_rows rows: 128 by default, the limit those modes were built with, and up to 256 when the caller asks for it
+    (max_rows=256, TP 1); more raises ValueError, as before."""
 
     def __init__(self, cfg: ModelConfig, batch: int, ctx: int, device: torch.device, tp_rank: int = 0, tp_size: int = 1,
                  dtype=torch.float16, seed: int = 0, keep_reference: bool = False, ragged: bool = False,
@@ -233,7 +242,8 @@ class DecodeStep:
                  logprobs: Optional[int] = None, eos_id: Optional[int] = None,
                  length_penalty: Union[float, Sequence[float]] = 1.0,
                  early_stopping: Union[bool, str, Sequence[Union[bool, str]]] = False,
-                 token_bitmask: bool = False, logit_bias_capacity: int = 0, tree=None, shared_prefix=None):
+                 token_bitmask: bool = False, logit_bias_capacity: int = 0, tree=None, shared_prefix=None,
+                 max_rows: int = TP_MAX_ROWS):
         assert cfg.head_num % tp_size == 0 and cfg.inter % tp_size == 0
         if shared_prefix is not None:
             n_share, p_tokens = shared_prefix
@@ -254,21 +264,26 @@ class DecodeStep:
             mp = sampling.min_p if isinstance(sampling.min_p, (list, tuple)) else [sampling.min_p]
             if not all(0.0 <= float(v) <= 1.0 for v in mp):
                 raise ValueError(f"sampling: min_p must be in [0, 1] (got {sampling.min_p})")
+        if not 1 <= max_rows <= GEMM_MAX_ROWS:
+            raise ValueError(f"max_rows must be in 1..{GEMM_MAX_ROWS}, the GEMM row limit (got {max_rows})")
         if q_len < 1:
             raise ValueError(f"q_len must be >= 1 (got {q_len})")
-        if q_len > 1 and (batch * q_len > 128 or tp_size != 1):
-            raise ValueError(f"a verification step (q_len {q_len}) needs batch * q_len <= 128 (the GEMM row limit) and tp_size 1 "
+        if q_len > 1 and (batch * q_len > max_rows or tp_size != 1):
+            raise ValueError(f"a verification step (q_len {q_len}) needs batch * q_len <= {max_rows} (max_rows; the GEMM row limit "
+                             f"is {GEMM_MAX_ROWS}) and tp_size 1 "
                              f"(got batch {batch}, tp_size {tp_size})")
         if tree is not None and q_len < 2:
             raise ValueError(f"a token-tree step needs q_len >= 2 nodes (got q_len {q_len})")
         if not 1 <= beam_width <= 32:
             raise ValueError(f"beam_width must be in 1..32 (got {beam_width})")
-        if beam_width > 1 and (batch * beam_width > 128 or tp_size != 1 or q_len != 1):
-            raise ValueError(f"beam search (beam_width {beam_width}) needs batch * beam_width <= 128 (the GEMM row limit), tp_size 1 "
+        if beam_width > 1 and (batch * beam_width > max_rows or tp_size != 1 or q_len != 1):
+            raise ValueError(f"beam search (beam_width {beam_width}) needs batch * beam_width <= {max_rows} (max_rows; the GEMM row "
+                             f"limit is {GEMM_MAX_ROWS}), tp_size 1 "
                              f"and q_len 1 (got batch {batch}, tp_size {tp_size}, q_len {q_len})")
         if sampling is not None:
-            if tp_size != 1 or beam_width != 1 or batch * q_len > 128:
-                raise ValueError(f"sampling needs tp_size 1, beam_width 1 and batch * q_len <= 128 (the GEMM row limit) (got tp_size "
+            if tp_size != 1 or beam_width != 1 or batch * q_len > max_rows:
+                raise ValueError(f"sampling needs tp_size 1, beam_width 1 and batch * q_len <= {max_rows} (max_rows; the GEMM row limit "
+                                 f"is {GEMM_MAX_ROWS}) (got tp_size "
                                  f"{tp_size}, beam_width {beam_width}, batch {batch}, q_len {q_len})")
             if q_len > 1 and (sampling.has_penalties() or no_repeat_ngram != 0):
                 raise ValueError("sampled verification (q_len > 1) takes no penalties and no n-gram ban: row j's history would "
@@ -307,6 +322,9 @@ class DecodeStep:
         batch = batch * beam_width                      # sequences (page-table rows) of the step
         self.q_len = q_len
         R = batch * q_len                               # token rows of the step
+        if R > GEMM_MAX_ROWS or (R > TP_MAX_ROWS and tp_size != 1):
+            raise ValueError(f"a step runs at most {GEMM_MAX_ROWS} token rows (the GEMM row limit), and at most {TP_MAX_ROWS} with "
+                             f"tp_size > 1 (got {R} rows, tp_size {tp_size})")
         if act_order and (tp_size != 1 or cfg.quant not in ("int4", "int8g")):
             raise ValueError(f"act_order needs tp_size 1 and quant int4 / int8g (got tp_size {tp_size}, quant {cfg.quant})")
         self.act_order = act_order

@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """Per-kernel timing at the BASELINE shapes (developer tool, runs on the GPU). CUDA events on the launching stream,
 warm-up, inputs rotated through > L2-size working sets so nothing is served from the H100's 50 MB L2."""
+import itertools
 import json
 import math
 import os
@@ -451,6 +452,39 @@ def bench_gemm(fmt, B, K, N, env=None, pdl=False, group=128, act_order=False):
     return us
 
 
+def bench_gemm_rows(fmt, B, K, N, parts, silu=False, runs=3):
+    """One launch of B rows (one CTA over all of them: each weight block read and dequantised once) against the same rows cut
+    into `parts` launches, as the Linear seam's 128-row slabs do (each streams and dequantises the whole weight). CUDA-graph
+    replay, medians of `runs` alternating runs. Returns (us one launch, us parts)."""
+    nw = max(2, int(300e6 // (K * N / 2 if fmt == B200_FMT_INT4 else 2 * K * N)) + 1)
+    ws_ = []
+    for _ in range(nw):
+        if fmt == B200_FMT_INT4:
+            qp = torch.randint(0, 256, (K, N // 2), device=dev, dtype=torch.uint8)
+            s = (torch.randn(K // 128, N, device=dev).abs() * 0.01 + 1e-3).half()
+            ws_.append(ops.pack_w4(qp, s, s, 128))
+        else:
+            ws_.append(ops.PackedWeight(B200_FMT_F16, K, N, (torch.randn(N, K, device=dev) * 0.02).half()))
+    x = torch.randn(B, K, device=dev).half()
+    y = torch.empty(B, N // 2 if silu else N, device=dev).half()
+    wk = ops.gemm_workspace(B, [(K, N)], dev)
+    cuts = list(itertools.accumulate(parts, initial=0))
+
+    def sliced(i):
+        for a, b in zip(cuts[:-1], cuts[1:]):
+            ops.wo_gemm(x[a:b], ws_[i], wk, out=y[a:b], silu_mul=silu)
+    one, split = [], []
+    for _ in range(runs):
+        one.append(timeit(lambda i: ops.wo_gemm(x, ws_[i], wk, out=y, silu_mul=silu), nw))
+        split.append(timeit(sliced, nw))
+    one, split = sorted(one)[runs // 2], sorted(split)[runs // 2]
+    flop = 2.0 * B * K * N
+    nm = "int4 g128" if fmt == B200_FMT_INT4 else "f16"
+    print(f"gemm-rows {nm} B{B} K{K} N{N}{' silu' if silu else ''}: one launch {one:8.1f} us {flop / one / 1e6:6.1f} TFLOP/s | "
+          f"{' + '.join(map(str, parts))} rows {split:8.1f} us {flop / split / 1e6:6.1f} TFLOP/s | {one / split:.3f}x", flush=True)
+    return one, split
+
+
 if __name__ == "__main__":
     which = sys.argv[1:] or ["attn", "gemm"]
     if which[0] == "one_gemm":     # one_gemm fmt B K N  (for ncu)
@@ -599,6 +633,14 @@ if __name__ == "__main__":
                         t[f].append(bench_qknorm_rope(kind, f, 32, 32, 8, n))
                 fu, co = sorted(t[True])[1], sorted(t[False])[1]
                 print(f"qknorm-rope {kind} q_len {n} median: fused {fu:.2f} us, norm + rope {co:.2f} us ({fu / co:.2f}x)", flush=True)
+    if "gemm-rows256" in which:
+        # 129..256 rows: the batch-pad-256 instance against 128-row launches of the batch-pad-128 kernel (Llama-3-8B shapes)
+        for B, parts in ((256, (128, 128)), (192, (128, 64))):
+            bench_gemm_rows(B200_FMT_INT4, B, 4096, 6144, parts)
+            bench_gemm_rows(B200_FMT_INT4, B, 4096, 4096, parts)
+            bench_gemm_rows(B200_FMT_INT4, B, 4096, 28672, parts, silu=True)
+            bench_gemm_rows(B200_FMT_INT4, B, 14336, 4096, parts)
+            bench_gemm_rows(B200_FMT_F16, B, 4096, 128256, parts)
     if "gemm" in which:
         for B in (32,):
             bench_gemm(B200_FMT_INT4, B, 4096, 6144)
