@@ -110,6 +110,7 @@ class B200DecodeAttnOp:
         block_ids = attn_inputs.kv_cache_kernel_block_id_device
         if block_ids is None:
             raise B200Error("decode should have kv cache block id.")          # XQAAttnOp.cc:66-67
+        ops.check_lengths("B200DecodeAttnOp.prepare", attn_inputs.sequence_lengths, int(block_ids.shape[0]))
         B = int(attn_inputs.sequence_lengths.shape[0])
         if block_ids.shape[0] != B:
             raise B200Error(f"kv blocks batch size expected [{B}] but got [{block_ids.shape[0]}]")
@@ -125,6 +126,8 @@ class B200DecodeAttnOp:
     def update(self, params: B200AttnParams, attn_inputs) -> None:
         if params is None:
             raise B200Error("B200DecodeAttnOp::update received null params")
+        ops.check_lengths("B200DecodeAttnOp.update", attn_inputs.sequence_lengths,
+                          int(attn_inputs.kv_cache_kernel_block_id_device.shape[0]))
         self.update_kv_cache_offset(params.kv_cache_offset, attn_inputs.kv_cache_kernel_block_id_device)
         params.batch_size = int(attn_inputs.kv_cache_kernel_block_id_device.shape[0])
         params.sequence_lengths = attn_inputs.sequence_lengths
@@ -141,9 +144,7 @@ class B200DecodeAttnOp:
         if kv_cache is None:
             raise B200Error("decode should have kv cache.")                                  # XQAAttnOp.cc:138
         base = kv_cache.kv_cache_base if hasattr(kv_cache, "kv_cache_base") else kv_cache
-        seq = params.sequence_lengths
-        if not seq.is_cuda and not seq.is_pinned():
-            raise B200Error("sequence_lengths must be device-accessible (CUDA or pinned host memory)")
+        seq = params.sequence_lengths          # CUDA or pinned host int32: the ops wrappers check it
         q_scale = 1.0 / float(getattr(self.cfg, "q_scaling", 1.0) or 1.0)
         if params.q_len > 1:      # q [B*q_len, Hq*D] token-major -> [B, q_len, Hq, D]; out [B*q_len, Hq*D]
             D = base.shape[-1]

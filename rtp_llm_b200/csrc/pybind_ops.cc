@@ -173,6 +173,15 @@ static torch::Tensor rope_table(const RopeConfig& r, int dim, const torch::Devic
     return it->second;
 }
 
+// == ops.check_lengths: the sequence lengths a kernel reads through their pointer are int32, contiguous, at least `seqs` long, and
+// in device or pinned host memory. A pageable host tensor would hand the kernel a host pointer, an int64 one pairs of int32.
+static void check_lengths(const torch::Tensor& t, int64_t seqs, const char* who) {
+    B200_CHECK(t.defined() && t.scalar_type() == torch::kInt32 && t.is_contiguous() && t.numel() >= seqs &&
+                   (t.is_cuda() || t.is_pinned()),
+               std::string(who) + ": sequence_lengths must be a contiguous int32 tensor of at least " + std::to_string(seqs) +
+                   " entries in CUDA or pinned host memory");
+}
+
 static void update_offset_tensor(const torch::Tensor& kv_cache_offset, const torch::Tensor& block_ids) {
     B200_CHECK(block_ids.defined() && block_ids.is_cuda() && block_ids.scalar_type() == torch::kInt32 && block_ids.dim() == 2,
                "B200AttnOp expects a CUDA int32 block table [batch, blocks]");
@@ -208,7 +217,8 @@ public:
         auto params = std::make_shared<B200AttnParams>();
         const auto& block_ids = attn_inputs.kv_cache_kernel_block_id_device;
         B200_CHECK(block_ids.defined(), "decode should have kv cache block id.");
-        const int64_t batch = attn_inputs.sequence_lengths.size(0);
+        check_lengths(attn_inputs.sequence_lengths, block_ids.size(0), "B200AttnOp::prepare");
+        const int64_t batch = attn_inputs.sequence_lengths.numel();
         B200_CHECK(block_ids.size(0) == batch, "kv blocks batch size does not match sequence_lengths");
         params->kv_cache_offset = torch::empty({batch, 1, 2, block_ids.size(1)}, block_ids.options());
         update_offset_tensor(params->kv_cache_offset, block_ids);
@@ -229,6 +239,8 @@ public:
 
     void update(const B200AttnParamsPtr& params, PyAttentionInputs attn_inputs) {
         B200_CHECK(params != nullptr, "B200AttnOp::update received null params");
+        B200_CHECK(attn_inputs.kv_cache_kernel_block_id_device.defined(), "decode should have kv cache block id.");
+        check_lengths(attn_inputs.sequence_lengths, attn_inputs.kv_cache_kernel_block_id_device.size(0), "B200AttnOp::update");
         update_offset_tensor(params->kv_cache_offset, attn_inputs.kv_cache_kernel_block_id_device);
         params->batch_size = (size_t)attn_inputs.kv_cache_kernel_block_id_device.size(0);
         params->sequence_lengths = attn_inputs.sequence_lengths;
@@ -242,6 +254,7 @@ public:
     torch::Tensor forward(const torch::Tensor& input, std::optional<LayerKVCache> kv_cache, const B200AttnParamsPtr& params) {
         B200_CHECK(kv_cache.has_value(), "decode should have kv cache.");
         B200_CHECK(params != nullptr, "B200AttnOp::forward received null params");
+        check_lengths(params->sequence_lengths, (int64_t)params->batch_size, "B200AttnOp::forward");
         const auto& c = attn_configs_;
         const int64_t rows = input.size(0);
         torch::Tensor out = torch::empty({rows, (int64_t)(c.head_num * c.size_per_head)}, input.options());
@@ -281,6 +294,7 @@ static torch::Tensor b200_rope_kvcache_decode(const torch::Tensor& qkv, const La
     const auto& pool = kv_cache.kv_cache_base;
     const int q_len = (int)params->q_len, rows = (int)qkv.size(0), is_bf16 = qkv.scalar_type() == torch::kBFloat16;
     B200_CHECK(q_len >= 1 && rows % q_len == 0, "b200_rope_kvcache_decode: qkv rows must be a multiple of q_len");
+    check_lengths(params->sequence_lengths, rows / q_len, "b200_rope_kvcache_decode");
     torch::Tensor q = torch::empty({qkv.size(0), (int64_t)(c.head_num * c.size_per_head)}, qkv.options());
     const int32_t* seq = params->sequence_lengths.data_ptr<int>();
     const int M = (int)params->kv_cache_offset.size(3), T = (int)page_size_of(c);

@@ -81,6 +81,8 @@ class B200WeightOnlyLinear(LinearBase):
     def forward(self, input: torch.Tensor) -> torch.Tensor:
         lead = input.shape[:-1]
         x = input.reshape(-1, input.shape[-1])
+        if x.shape[0] == 0:                              # as F.linear: an empty [*lead, N], no launch
+            return input.new_empty((*lead, self.packed.N))
         if not x.is_contiguous():
             x = x.contiguous()
         if self.packed.col_scale is not None and self.packed.col_scale.dtype != x.dtype:

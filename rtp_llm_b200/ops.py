@@ -35,6 +35,18 @@ def _cuda_contig(*ts: Optional[torch.Tensor]) -> None:
             raise B200Error("expected contiguous CUDA tensors")
 
 
+def check_lengths(who: str, lengths: torch.Tensor, seqs: int) -> None:
+    """Raise unless `lengths` is what a kernel can read through its pointer: int32, contiguous, at least `seqs` entries, in
+    device memory or in pinned host memory (which the GPU reads in place). A pageable host tensor would hand the kernel a host
+    pointer, and an int64 one would be read as pairs of int32."""
+    if not (torch.is_tensor(lengths) and lengths.dtype == torch.int32 and lengths.is_contiguous() and lengths.numel() >= seqs
+            and (lengths.is_cuda or lengths.is_pinned())):
+        got = (f"{lengths.dtype} [{lengths.numel()}] on {lengths.device}{'' if lengths.is_cuda or lengths.is_pinned() else ', pageable'}"
+               if torch.is_tensor(lengths) else type(lengths).__name__)
+        raise B200Error(f"{who}: sequence_lengths must be a contiguous int32 tensor of at least {seqs} entries in CUDA or pinned "
+                        f"host memory (got {got})")
+
+
 _DTYPE_NAMES = {torch.int32: "int32", torch.float32: "fp32"}
 
 
@@ -110,14 +122,15 @@ def attn_workspace(batch: int, head_num: int, kv_head_num: int, max_seq_len: int
 
 
 def _paged_attn(entry: str, q: torch.Tensor, kv_cache_base: torch.Tensor, page_list: torch.Tensor, sequence_lengths: torch.Tensor,
-                max_seq_len: int, workspace: torch.Tensor, out: Optional[torch.Tensor], rows: tuple, Hq: Optional[int],
+                max_seq_len: int, workspace: torch.Tensor, out: Optional[torch.Tensor], rows: tuple, seqs: int, Hq: Optional[int],
                 extra: tuple) -> torch.Tensor:
     """The call of b200_<entry> that the paged_decode_attn* wrappers share. rows: the sizes before the heads, (B,) or (B, q_len
-    or W), passed after head_dim; out [*rows, Hq*D] of q's dtype is allocated when not given; Hq None: q's elements over
-    rows * D. extra: the arguments between sequence_lengths and the workspace (q_scale among them); tensors among them are
-    checked and passed as pointers."""
+    or W), passed after head_dim; seqs: the sequences whose lengths the kernel reads; out [*rows, Hq*D] of q's dtype is
+    allocated when not given; Hq None: q's elements over rows * D. extra: the arguments between sequence_lengths and the
+    workspace (q_scale among them); tensors among them are checked and passed as pointers."""
     tensors = [t for t in extra if isinstance(t, torch.Tensor)]
     _cuda_contig(q, kv_cache_base, page_list, *tensors, workspace, out)
+    check_lengths(entry, sequence_lengths, seqs)
     P, two, Hkv, T, D = kv_cache_base.shape
     if Hq is None:
         Hq = q.numel() // (math.prod(rows) * D)
@@ -136,7 +149,7 @@ def paged_decode_attn(q: torch.Tensor, kv_cache_base: torch.Tensor, page_list: t
     """q [B,Hq,D] (or [B,Hq*D]); kv_cache_base [P,2,Hkv,T,D]; page_list [B,1,2,M]; sequence_lengths [B] int32 = tokens
     already cached; max_seq_len = host bound on sequence_lengths+1. Returns [B, Hq*D]."""
     return _paged_attn("paged_decode_attn", q, kv_cache_base, page_list, sequence_lengths, max_seq_len, workspace, out, (q.shape[0],),
-                       None, (q_scale,))
+                       q.shape[0], None, (q_scale,))
 
 
 def paged_decode_attn_multi(q: torch.Tensor, kv_cache_base: torch.Tensor, page_list: torch.Tensor, sequence_lengths: torch.Tensor,
@@ -144,7 +157,7 @@ def paged_decode_attn_multi(q: torch.Tensor, kv_cache_base: torch.Tensor, page_l
     """q [B, q_len, Hq, D] (q_len speculative tokens per sequence, K/V already appended); sequence_lengths [B] = tokens cached
     before them; query j attends to positions 0 .. sequence_lengths[b] + j. Returns [B, q_len, Hq*D]."""
     return _paged_attn("paged_decode_attn_multi", q, kv_cache_base, page_list, sequence_lengths, max_seq_len, workspace, out,
-                       tuple(q.shape[:2]), q.shape[2], (q_scale,))
+                       tuple(q.shape[:2]), q.shape[0], q.shape[2], (q_scale,))
 
 
 def paged_decode_attn_beam(q: torch.Tensor, kv_cache_base: torch.Tensor, page_list: torch.Tensor, sequence_lengths: torch.Tensor,
@@ -154,7 +167,7 @@ def paged_decode_attn_beam(q: torch.Tensor, kv_cache_base: torch.Tensor, page_li
     shared_lengths [B] int32 = tokens of each request that all its W beams share (their page_list rows are equal over those
     pages), read once for the W beams. The bits of paged_decode_attn on the B * W rows. Returns [B, W, Hq*D]."""
     return _paged_attn("paged_decode_attn_beam", q, kv_cache_base, page_list, sequence_lengths, max_seq_len, workspace, out,
-                       tuple(q.shape[:2]), q.shape[2], (shared_lengths, q_scale))
+                       tuple(q.shape[:2]), q.shape[0] * q.shape[1], q.shape[2], (shared_lengths, q_scale))
 
 
 def paged_decode_attn_prefix(q: torch.Tensor, kv_cache_base: torch.Tensor, page_list: torch.Tensor, sequence_lengths: torch.Tensor,
@@ -166,9 +179,10 @@ def paged_decode_attn_prefix(q: torch.Tensor, kv_cache_base: torch.Tensor, page_
     whose page_list rows are equal over the first shared_lengths[c] / T pages (int32 [chunks]). prefix_chunks builds the three
     from a block table. Rows in no chunk are not written. Returns [B, Hq*D]."""
     who = "paged_decode_attn_prefix"
-    _cuda_contig(q, kv_cache_base, page_list, sequence_lengths, chunk_offsets, chunk_rows, shared_lengths, workspace, out)
+    _cuda_contig(q, kv_cache_base, page_list, chunk_offsets, chunk_rows, shared_lengths, workspace, out)
     P, two, Hkv, T, D = kv_cache_base.shape
     B = q.shape[0]
+    check_lengths(who, sequence_lengths, B)
     C = shared_lengths.numel()
     _need(who, "chunk_offsets", chunk_offsets, torch.int32, (C + 1,), flat=True)
     _need(who, "chunk_rows", chunk_rows, torch.int32, (B,), flat=True)
@@ -242,7 +256,7 @@ def paged_decode_attn_tree(q: torch.Tensor, kv_cache_base: torch.Tensor, page_li
     Returns [B, n, Hq*D]."""
     _need("paged_decode_attn_tree", "tree_parents", tree_parents, torch.int32, tuple(q.shape[:2]))
     return _paged_attn("paged_decode_attn_tree", q, kv_cache_base, page_list, sequence_lengths, max_seq_len, workspace, out,
-                       tuple(q.shape[:2]), q.shape[2], (tree_parents, q_scale))
+                       tuple(q.shape[:2]), q.shape[0], q.shape[2], (tree_parents, q_scale))
 
 
 def paged_decode_attn_rope(qkv: torch.Tensor, kv_cache_base: torch.Tensor, page_list: torch.Tensor, sequence_lengths: torch.Tensor,
@@ -251,7 +265,7 @@ def paged_decode_attn_rope(qkv: torch.Tensor, kv_cache_base: torch.Tensor, page_
     """RoPE + K/V append + paged decode attention in ONE launch: qkv [B, (Hq+2Hkv)*D] un-rotated (the qkv GEMM output);
     kv_cache_base receives the new token's K (rotated) and V. Bit-identical to rope_append() followed by paged_decode_attn()."""
     return _paged_attn("paged_decode_attn_rope", qkv, kv_cache_base, page_list, sequence_lengths, max_seq_len, workspace, out,
-                       (qkv.shape[0],), head_num, (q_scale, rope_base))
+                       (qkv.shape[0],), qkv.shape[0], head_num, (q_scale, rope_base))
 
 
 # ------------------------------------------------------------------------------------------------ weight-only GEMM
@@ -477,11 +491,17 @@ def wo_gemm(x: torch.Tensor, w: PackedWeight, workspace: torch.Tensor, bias: Opt
             out: Optional[torch.Tensor] = None, pdl: bool = False, silu_mul: bool = False,
             x_perm: Optional[torch.Tensor] = None) -> torch.Tensor:
     """y = x . W (+ bias). An act-order weight (w.perm set) needs x_perm, a scratch [>= B, K] of x's dtype: x[:, w.perm] is
-    gathered into it (b200_permute_cols) and the GEMM reads that."""
+    gathered into it (b200_permute_cols) and the GEMM reads that. bias: [N] of x's dtype; out: [B, N] ([B, N/2] with
+    silu_mul) of x's dtype."""
     _cuda_contig(x, w.data, workspace, bias, out)
     B, K = x.shape
     if K != w.K:
         raise B200Error(f"wo_gemm: x has K={K}, weight has K={w.K}")
+    n_out = w.N // 2 if silu_mul else w.N
+    if bias is not None and (bias.dtype != x.dtype or tuple(bias.shape) != (w.N,)):
+        raise B200Error(f"wo_gemm: bias must be [{w.N}] {x.dtype}, got {list(bias.shape)} {bias.dtype}")
+    if out is not None and (out.dtype != x.dtype or tuple(out.shape) != (B, n_out)):
+        raise B200Error(f"wo_gemm: out must be [{B}, {n_out}] {x.dtype}, got {list(out.shape)} {out.dtype}")
     if w.perm is not None:
         if x_perm is None:
             raise B200Error("wo_gemm: the weight is act-order (rows sorted by g_idx): pass x_perm, a [>= B, K] scratch for x[:, perm]")
@@ -489,7 +509,7 @@ def wo_gemm(x: torch.Tensor, w: PackedWeight, workspace: torch.Tensor, bias: Opt
             raise B200Error(f"wo_gemm: x_perm must be [>= {B}, {K}] {x.dtype}, got {tuple(x_perm.shape)} {x_perm.dtype}")
         x = permute_cols(x, w.perm, out=x_perm[:B])
     if out is None:
-        out = torch.empty((B, w.N // 2 if silu_mul else w.N), dtype=x.dtype, device=x.device)
+        out = torch.empty((B, n_out), dtype=x.dtype, device=x.device)
     check(_lib.load().b200_wo_gemm(w.fmt, _is_bf16(x), _p(x), B, K, w.N, _p(w.data), _p(w.col_scale), _p(bias), _p(out),
                                    _p(workspace), workspace.numel(),
                                    (_lib.B200_GEMM_PDL if pdl else 0) | (_lib.B200_GEMM_SILU_MUL if silu_mul else 0), _stream()),
@@ -531,11 +551,12 @@ def _rope_args(what, qkv, kv_cache_base, page_list, sequence_lengths, head_num, 
     """Checks and C arguments shared by the four rope + append ops: (q_out, (q_out, pool, page list, sequence lengths),
     the _ex entries' (position ids, table, table positions, config, logn), (dtype, B, Hq, Hkv, D, max blocks, page size)).
     qk_norm: (q_gamma, k_gamma), each a [D] tensor of qkv's dtype."""
-    _cuda_contig(qkv, kv_cache_base, page_list, sequence_lengths, q_out, bias, position_ids, cos_sin_cache, *(qk_norm or ()))
+    _cuda_contig(qkv, kv_cache_base, page_list, q_out, bias, position_ids, cos_sin_cache, *(qk_norm or ()))
     P, two, Hkv, T, D = kv_cache_base.shape
     rows = qkv.shape[0]
     if q_len < 1 or rows % q_len:
         raise B200Error(f"{what}: {rows} qkv rows are not a multiple of q_len {q_len}")
+    check_lengths(what, sequence_lengths, rows // q_len)
     if position_ids is not None and position_ids.numel() != rows:
         raise B200Error(f"{what}: {position_ids.numel()} position ids for {rows} qkv rows")
     for name, g in zip(("q_gamma", "k_gamma"), qk_norm or ()):
