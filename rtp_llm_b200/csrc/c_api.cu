@@ -185,6 +185,46 @@ AttnWorkspace attn_workspace(size_t batch, size_t head_num, size_t kv_head_num, 
             slots * head_dim * sizeof(float)};
 }
 
+// The six attention entries, one mode each of the one host path attn_impl
+enum class AttnMode { kPlain, kMulti, kRope, kBeam, kPrefix, kTree };
+
+// One call of an attention entry: the parameters every entry has, in their order, with `slots` where the multi, beam and tree
+// entries take theirs; then what only some modes use, left zero by the others.
+struct AttnCall {
+    const char* who;   // the entry's name, for messages
+    AttnMode mode;
+    const void* q;     // rope: the un-rotated qkv GEMM output
+    int is_bf16;
+    void* out;
+    size_t head_num, kv_head_num, head_dim;
+    size_t batch;      // sequences; beam: requests of `slots` sequences each
+    size_t slots;      // what shares a CTA: q_len query tokens (1 plain and rope), the beam width, or the largest chunk (prefix)
+    size_t max_blocks_per_seq, max_seq_len, page_size;
+    const void* kv_pool;
+    const int32_t* page_list;
+    const uint32_t* sequence_lengths;
+    float q_scale;
+    void* workspace;
+    size_t workspace_bytes;
+    void* stream;
+    const int32_t* shared_lengths;   // beam [batch], prefix [chunks]
+    size_t chunks;                   // prefix: chunk c is the rows chunk_rows[chunk_offsets[c] .. chunk_offsets[c + 1])
+    const int32_t *chunk_offsets, *chunk_rows;
+    const int32_t* tree_parents;     // [batch][slots]
+    float rope_base;
+};
+
+// A launch of the paged_decode_attn_kernel instance of dtype T, head_dim D and RT 16-row query tiles whose parameter struct is
+// P: AttnParams (plain, multi and rope modes), AttnBeamParams (beam and prefix) or AttnTreeParams (tree).
+template <typename T, int D, int RT, typename P>
+int launch_attn(const CUtensorMap& map, const P& p, dim3 grid, dim3 cluster, void* stream) {
+    constexpr auto kern = paged_decode_attn_kernel<T, D, RT, std::is_same_v<P, AttnBeamParams>, std::is_same_v<P, AttnTreeParams>>;
+    constexpr int smem = attn_smem_bytes(D);
+    int rc = configure_once<kern>(smem);
+    if (rc) return rc;
+    return launch_op("paged_decode_attn_kernel", stream, kern, {grid, dim3(kAttnThreads), (size_t)smem, cluster}, map, p);
+}
+
 // ---- GEMM launch shape
 constexpr int kGemmMaxRows = 256;   // rows per b200_wo_gemm call (batch pad 256); the reduce-scatter GEMM takes up to 128
 int gemm_bpad(int B) { return B <= 16 ? 16 : (B <= 32 ? 32 : (B <= 64 ? 64 : (B <= 128 ? 128 : 256))); }
@@ -435,164 +475,144 @@ size_t b200_paged_decode_attn_workspace_bytes(size_t batch, size_t head_num, siz
     return w.sem + w.ml + w.o;
 }
 
-// beam_width > 0: the beam instance. `batch` then counts requests, each with beam_width sequences (rows of q, out, page_list and
-// sequence_lengths), and shared_lengths [batch] says how much of a request's K/V its beams share; q_len is 1.
-// chunks > 0 (with beam_width > 0): the beam instance's prefix mode. `batch` counts rows; CTAs own the chunks of up to beam_width
-// rows that chunk_offsets / chunk_rows list, and shared_lengths [chunks] is per chunk.
-// tree_parents != null: the tree instance, parents [batch][q_len] of each sequence's q_len new tokens.
-static int attn_impl(const void* q, const void* qkv, float rope_base, int q_len, int is_bf16, void* out, size_t head_num, size_t kv_head_num,
-                     size_t head_dim, size_t batch, size_t max_blocks_per_seq, size_t max_seq_len, size_t page_size, const void* kv_pool,
-                     const int32_t* page_list, const uint32_t* sequence_lengths, float q_scale, void* workspace, size_t workspace_bytes,
-                     void* stream, int beam_width = 0, const int32_t* shared_lengths = nullptr, const int32_t* tree_parents = nullptr,
-                     size_t chunks = 0, const int32_t* chunk_offsets = nullptr, const int32_t* chunk_rows = nullptr) {
-    if (batch == 0) return B200_OK;
-    ARG_CHECK((q || qkv) && out && kv_pool && page_list && sequence_lengths, "paged_decode_attn: null pointer");
-    ARG_CHECK(head_dim == 64 || head_dim == 128 || head_dim == 256, "paged_decode_attn: head_dim %zu unsupported (64 / 128 / 256)", head_dim);
-    ARG_CHECK(!qkv || head_dim == 128, "paged_decode_attn_rope: the fused rope is built for head_dim 128 (got %zu)", head_dim);
-    ARG_CHECK(kv_head_num > 0 && head_num % kv_head_num == 0, "paged_decode_attn: head_num %zu not a multiple of kv_head_num %zu",
-              head_num, kv_head_num);
-    const int group = (int)(head_num / kv_head_num);
+// The one host path of the six attention entries: their checks, the launch plan, and the kernel instance of the call's mode.
+// Beam and prefix run the kernel's shared-K/V instance (a CTA owns a chunk of up to `slots` member rows: a request's beams, or
+// the rows chunk_rows lists), tree its tree instance, and plain, multi and rope its plain instance, rope with RoPE + K/V append.
+static int attn_impl(const AttnCall& c) {
+    const bool rope = c.mode == AttnMode::kRope, beam = c.mode == AttnMode::kBeam, prefix = c.mode == AttnMode::kPrefix,
+               tree = c.mode == AttnMode::kTree, shared = beam || prefix;
+    // how the messages name a CTA row of the grid and what shares it; the shared-K/V entries name themselves in those limits
+    const char* units = beam ? "requests" : prefix ? "chunks" : "batch";
+    const char* unit = beam ? "request" : prefix ? "chunk" : "sequence";
+    const char* slots = beam ? "beam_width" : prefix ? "max_members" : "q_len";
+    const char* limits = shared ? c.who : "paged_decode_attn";
+    // an empty call still has its query slots and its rope base checked; the largest chunk is checked with the rows it gives
+    ARG_CHECK(prefix || (c.slots >= 1 && c.slots <= (size_t)kAttnMaxRows), "%s: %s %zu unsupported (1..%d)", c.who, slots, c.slots,
+              kAttnMaxRows);
+    ARG_CHECK(!rope || c.rope_base > 1.f, "%s: rope_base must be > 1", c.who);
+    if (c.batch == 0) return B200_OK;
+    const char* own = beam ? " (q or shared_lengths)" : prefix ? " (q or a chunk array)" : tree ? " (q or tree_parents)" : "";
+    ARG_CHECK(c.q && (!shared || c.shared_lengths) && (!prefix || (c.chunk_offsets && c.chunk_rows)) && (!tree || c.tree_parents),
+              "%s: null pointer%s", c.who, own);
+    ARG_CHECK(!prefix || (c.chunks >= 1 && c.chunks <= c.batch), "%s: chunks %zu must be in 1..batch (%zu)", c.who, c.chunks, c.batch);
+    ARG_CHECK(!prefix || c.batch <= 65535, "%s: batch %zu exceeds 65535 rows", c.who, c.batch);
+    ARG_CHECK(c.out && c.kv_pool && c.page_list && c.sequence_lengths, "paged_decode_attn: null pointer");
+    ARG_CHECK(c.head_dim == 64 || c.head_dim == 128 || c.head_dim == 256, "paged_decode_attn: head_dim %zu unsupported (64 / 128 / 256)",
+              c.head_dim);
+    ARG_CHECK(!rope || c.head_dim == 128, "%s: the fused rope is built for head_dim 128 (got %zu)", c.who, c.head_dim);
+    ARG_CHECK(c.kv_head_num > 0 && c.head_num % c.kv_head_num == 0, "%s: head_num %zu not a multiple of kv_head_num %zu",
+              prefix ? c.who : "paged_decode_attn", c.head_num, c.kv_head_num);
+    const int group = (int)(c.head_num / c.kv_head_num);
     // the fused rope loads q into one 16-row tile; the plain q load takes up to four
-    ARG_CHECK(!qkv || group <= 16, "paged_decode_attn_rope: group size %d unsupported (1..16)", group);
+    ARG_CHECK(!rope || group <= 16, "%s: group size %d unsupported (1..16)", c.who, group);
     ARG_CHECK(group >= 1 && group <= kAttnMaxRows, "paged_decode_attn: group size %d unsupported (1..%d)", group, kAttnMaxRows);
-    ARG_CHECK(group * q_len <= kAttnMaxRows, "paged_decode_attn: group %d x q_len %d exceeds the limit of %d query rows per (sequence, kv head)",
-              group, q_len, kAttnMaxRows);
-    ARG_CHECK(group * beam_width <= kAttnMaxRows,
-              "paged_decode_attn_beam: group %d x beam_width %d exceeds the limit of %d query rows per (request, kv head)", group,
-              beam_width, kAttnMaxRows);
-    ARG_CHECK(page_size == 16 || page_size == 32 || page_size == 64 || page_size == 128,
-              "paged_decode_attn: page_size %zu unsupported (16/32/64/128)", page_size);
-    ARG_CHECK(max_seq_len >= 1, "paged_decode_attn: max_seq_len must be >= 1");
-    ARG_CHECK(max_seq_len <= max_blocks_per_seq * page_size, "paged_decode_attn: max_seq_len %zu exceeds page table capacity %zu",
-              max_seq_len, max_blocks_per_seq * page_size);
-    const size_t units = chunks ? chunks : batch;   // sequences, requests or chunks: one CTA row of the grid each
-    ARG_CHECK(units * kv_head_num <= 65535, "paged_decode_attn: batch*kv_heads %zu exceeds grid limit", units * kv_head_num);
-    ARG_CHECK(((uintptr_t)kv_pool & 15) == 0 && (((uintptr_t)q | (uintptr_t)qkv) & 3) == 0, "paged_decode_attn: misaligned pointer");
+    ARG_CHECK(c.slots >= 1 && c.slots <= (size_t)(kAttnMaxRows / group), "%s: group %d x %s %zu exceeds the limit of %d query rows per "
+              "(%s, kv head)", limits, group, slots, c.slots, kAttnMaxRows, unit);
+    ARG_CHECK(c.page_size == 16 || c.page_size == 32 || c.page_size == 64 || c.page_size == 128,
+              "paged_decode_attn: page_size %zu unsupported (16/32/64/128)", c.page_size);
+    ARG_CHECK(c.max_seq_len >= 1, "paged_decode_attn: max_seq_len must be >= 1");
+    ARG_CHECK(c.max_seq_len <= c.max_blocks_per_seq * c.page_size, "paged_decode_attn: max_seq_len %zu exceeds page table capacity %zu",
+              c.max_seq_len, c.max_blocks_per_seq * c.page_size);
+    const size_t ctas = (prefix ? c.chunks : c.batch) * c.kv_head_num;   // CTA rows of the grid: one per (unit, kv head)
+    ARG_CHECK(ctas <= 65535, "%s: %s*kv_heads %zu exceeds grid limit", limits, units, ctas);
+    ARG_CHECK(((uintptr_t)c.kv_pool & 15) == 0 && ((uintptr_t)c.q & 3) == 0, "paged_decode_attn: misaligned pointer");
 
-    const int slots = beam_width ? beam_width : q_len;   // query tokens or beams that share a CTA
-    AttnBeamParams p{};
-    p.beam_width = beam_width;
-    p.shared_lens = shared_lengths;
-    p.chunk_offsets = chunk_offsets;
-    p.chunk_rows = chunk_rows;
-    p.q = q;
-    p.qkv = qkv;
-    p.kv_pool_rw = const_cast<void*>(kv_pool);
-    p.log2_base = qkv ? std::log2(rope_base) : 0.f;
-    p.out = out;
-    p.page_list = page_list;
-    p.seq_lens = reinterpret_cast<const int32_t*>(sequence_lengths);
-    p.B = (int)batch;
-    p.Hq = (int)head_num;
-    p.Hkv = (int)kv_head_num;
+    AttnParams p{};
+    p.q = rope ? nullptr : c.q;
+    p.qkv = rope ? c.q : nullptr;
+    p.kv_pool_rw = const_cast<void*>(c.kv_pool);
+    p.log2_base = rope ? std::log2(c.rope_base) : 0.f;
+    p.out = c.out;
+    p.page_list = c.page_list;
+    p.seq_lens = reinterpret_cast<const int32_t*>(c.sequence_lengths);
+    p.B = (int)c.batch;
+    p.Hq = (int)c.head_num;
+    p.Hkv = (int)c.kv_head_num;
     p.group = group;
-    p.q_len = q_len;
-    p.M = (int)max_blocks_per_seq;
-    p.T = (int)page_size;
-    p.log2T = page_size == 16 ? 4 : page_size == 32 ? 5 : page_size == 64 ? 6 : 7;
-    p.box_h = page_size < (size_t)kAttnTile ? (int)page_size : kAttnTile;
+    p.q_len = shared ? 1 : (int)c.slots;
+    p.M = (int)c.max_blocks_per_seq;
+    p.T = (int)c.page_size;
+    p.log2T = c.page_size == 16 ? 4 : c.page_size == 32 ? 5 : c.page_size == 64 ? 6 : 7;
+    p.box_h = c.page_size < (size_t)kAttnTile ? (int)c.page_size : kAttnTile;
     p.boxes_per_tile = kAttnTile / p.box_h;
-    p.scale_log2 = q_scale / std::sqrt((float)head_dim) * 1.4426950408889634f;
-    const int max_tiles = (int)((max_seq_len + kAttnTile - 1) / kAttnTile);
-    attn_split((int)(units * kv_head_num), max_tiles, &p.nsplit, &p.tiles_per_split, (int)head_dim);
+    p.scale_log2 = c.q_scale / std::sqrt((float)c.head_dim) * 1.4426950408889634f;
+    const int max_tiles = (int)((c.max_seq_len + kAttnTile - 1) / kAttnTile);
+    attn_split((int)ctas, max_tiles, &p.nsplit, &p.tiles_per_split, (int)c.head_dim);
 
-    if (p.nsplit > 8) {
-        const AttnWorkspace w = attn_workspace(batch, head_num, kv_head_num, chunks ? 1 : slots, p.nsplit, head_dim);
-        ARG_CHECK(workspace && workspace_bytes >= w.sem + w.ml + w.o,
-                  "paged_decode_attn: workspace too small (%zu < %zu)", workspace_bytes, w.sem + w.ml + w.o);
-        p.sem = reinterpret_cast<int*>(workspace);
-        p.ws_ml = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + w.sem);
-        p.ws_o = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + w.sem + w.ml);
+    if (p.nsplit > 8) {   // query rows per sequence (or request) of the workspace; prefix mode counts rows in `batch`
+        const AttnWorkspace w = attn_workspace(c.batch, c.head_num, c.kv_head_num, prefix ? 1 : c.slots, p.nsplit, c.head_dim);
+        ARG_CHECK(c.workspace && c.workspace_bytes >= w.sem + w.ml + w.o,
+                  "paged_decode_attn: workspace too small (%zu < %zu)", c.workspace_bytes, w.sem + w.ml + w.o);
+        p.sem = reinterpret_cast<int*>(c.workspace);
+        p.ws_ml = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(c.workspace) + w.sem);
+        p.ws_o = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(c.workspace) + w.sem + w.ml);
     }
 
     CUtensorMap map;
     {
-        const cuuint64_t dims[4] = {(cuuint64_t)head_dim, (cuuint64_t)page_size, (cuuint64_t)kv_head_num, (cuuint64_t)1 << 31};
-        const cuuint64_t strides[3] = {(cuuint64_t)head_dim * 2, (cuuint64_t)page_size * head_dim * 2,
-                                       (cuuint64_t)kv_head_num * page_size * head_dim * 2};
+        const cuuint64_t dims[4] = {(cuuint64_t)c.head_dim, (cuuint64_t)c.page_size, (cuuint64_t)c.kv_head_num, (cuuint64_t)1 << 31};
+        const cuuint64_t strides[3] = {(cuuint64_t)c.head_dim * 2, (cuuint64_t)c.page_size * c.head_dim * 2,
+                                       (cuuint64_t)c.kv_head_num * c.page_size * c.head_dim * 2};
         const cuuint32_t box[4] = {64, (cuuint32_t)p.box_h, 1, 1};
-        int rc = make_map(&map, is_bf16 != 0, 4, kv_pool, dims, strides, box);
+        int rc = make_map(&map, c.is_bf16 != 0, 4, c.kv_pool, dims, strides, box);
         if (rc) return rc;
     }
-    const dim3 grid(p.nsplit, (unsigned)(units * kv_head_num), 1);
+    const dim3 grid(p.nsplit, (unsigned)ctas, 1);
     p.cluster_merge = (p.nsplit >= 2 && p.nsplit <= 8) ? 1 : 0;   // 2..8 splits merge in a cluster, more through the workspace
     const dim3 cluster(p.cluster_merge ? p.nsplit : 1);
-    auto launch = [&](auto t, auto hd, auto rt, auto beam, auto tree) {
-        constexpr auto kern = paged_decode_attn_kernel<decltype(t), decltype(hd)::value, decltype(rt)::value, decltype(beam)::value,
-                                                       decltype(tree)::value>;
-        const int smem = attn_smem_bytes(decltype(hd)::value);
-        int rc = configure_once<kern>(smem);
-        if (rc) return rc;
-        const OpShape sh{grid, dim3(kAttnThreads), (size_t)smem, cluster};
-        if constexpr (decltype(tree)::value) {
-            AttnTreeParams pt{};
-            static_cast<AttnParams&>(pt) = p;
-            pt.tree_parents = tree_parents;
-            return launch_op("paged_decode_attn_kernel", stream, kern, sh, map, pt);
-        } else {
-            // (launch_ex converts p to the kernel's parameter type: the plain instances take its AttnParams part)
-            return launch_op("paged_decode_attn_kernel", stream, kern, sh, map, p);
-        }
+    const int rows = group * (int)c.slots;   // query rows of a CTA, in 1, 2 or 4 16-row tiles
+    const int d = c.head_dim == 64 ? 0 : c.head_dim == 128 ? 1 : 2, rt = rows <= 16 ? 0 : rows <= 32 ? 1 : 2;
+    // the kernel instance of (dtype, head_dim, row tiles, mode), the mode given by the type of the parameter struct kp
+    auto launch = [&](const auto& kp) {
+        return by_dtype(c.is_bf16 != 0, [&](auto t) {
+            using T = decltype(t);
+            using P = std::decay_t<decltype(kp)>;
+            using Launch = int (*)(const CUtensorMap&, const P&, dim3, dim3, void*);
+            const Launch instances[3][3] = {   // [head_dim 64 / 128 / 256][row tiles 1 / 2 / 4]
+                {launch_attn<T, 64, 1, P>, launch_attn<T, 64, 2, P>, launch_attn<T, 64, 4, P>},
+                {launch_attn<T, 128, 1, P>, launch_attn<T, 128, 2, P>, launch_attn<T, 128, 4, P>},
+                {launch_attn<T, 256, 1, P>, launch_attn<T, 256, 2, P>, launch_attn<T, 256, 4, P>}};
+            return instances[d][rt](map, kp, grid, cluster, c.stream);
+        });
     };
-    // query rows in 16-row tiles: 1, 2 or 4 per (sequence or request, kv head)
-    const int rows = group * slots;
-    auto by_rows = [&](auto t, auto hd) {
-        auto by_beam = [&](auto rt) {
-            if (beam_width) return launch(t, hd, rt, std::true_type(), std::false_type());
-            if (tree_parents) return launch(t, hd, rt, std::false_type(), std::true_type());
-            return launch(t, hd, rt, std::false_type(), std::false_type());
-        };
-        if (rows <= 16) return by_beam(std::integral_constant<int, 1>());
-        if (rows <= 32) return by_beam(std::integral_constant<int, 2>());
-        return by_beam(std::integral_constant<int, 4>());
-    };
-    return by_dtype(is_bf16, [&](auto t) {
-        if (head_dim == 64) return by_rows(t, std::integral_constant<int, 64>());
-        if (head_dim == 128) return by_rows(t, std::integral_constant<int, 128>());
-        return by_rows(t, std::integral_constant<int, 256>());
-    });
+    if (shared) return launch(AttnBeamParams{p, (int)c.slots, c.shared_lengths, c.chunk_offsets, c.chunk_rows});
+    return tree ? launch(AttnTreeParams{p, c.tree_parents}) : launch(p);
 }
 
 int b200_paged_decode_attn(const void* q, int is_bf16, void* out, size_t head_num, size_t kv_head_num, size_t head_dim,
                            size_t batch, size_t max_blocks_per_seq, size_t max_seq_len, size_t page_size,
                            const void* kv_pool, const int32_t* page_list, const uint32_t* sequence_lengths,
                            float q_scale, void* workspace, size_t workspace_bytes, void* stream) {
-    ARG_CHECK(q || batch == 0, "paged_decode_attn: null pointer");
-    return attn_impl(q, nullptr, 0.f, 1, is_bf16, out, head_num, kv_head_num, head_dim, batch, max_blocks_per_seq, max_seq_len, page_size,
-                     kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, stream);
+    return attn_impl({"paged_decode_attn", AttnMode::kPlain, q, is_bf16, out, head_num, kv_head_num, head_dim, batch, 1, max_blocks_per_seq,
+                      max_seq_len, page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, stream});
 }
 
 int b200_paged_decode_attn_multi(const void* q, int is_bf16, void* out, size_t head_num, size_t kv_head_num, size_t head_dim,
                                  size_t batch, size_t q_len, size_t max_blocks_per_seq, size_t max_seq_len, size_t page_size,
                                  const void* kv_pool, const int32_t* page_list, const uint32_t* sequence_lengths, float q_scale,
                                  void* workspace, size_t workspace_bytes, void* stream) {
-    ARG_CHECK(q || batch == 0, "paged_decode_attn_multi: null pointer");
-    ARG_CHECK(q_len >= 1 && q_len <= (size_t)kAttnMaxRows, "paged_decode_attn_multi: q_len %zu unsupported (1..%d)", q_len, kAttnMaxRows);
-    return attn_impl(q, nullptr, 0.f, (int)q_len, is_bf16, out, head_num, kv_head_num, head_dim, batch, max_blocks_per_seq, max_seq_len,
-                     page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, stream);
+    return attn_impl({"paged_decode_attn_multi", AttnMode::kMulti, q, is_bf16, out, head_num, kv_head_num, head_dim, batch, q_len,
+                      max_blocks_per_seq, max_seq_len, page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace,
+                      workspace_bytes, stream});
 }
 
 int b200_paged_decode_attn_rope(const void* qkv, int is_bf16, void* out, size_t head_num, size_t kv_head_num, size_t head_dim,
                                 size_t batch, size_t max_blocks_per_seq, size_t max_seq_len, size_t page_size, void* kv_pool,
                                 const int32_t* page_list, const uint32_t* sequence_lengths, float q_scale, float rope_base,
                                 void* workspace, size_t workspace_bytes, void* stream) {
-    ARG_CHECK(qkv || batch == 0, "paged_decode_attn_rope: null pointer");
-    ARG_CHECK(rope_base > 1.f, "paged_decode_attn_rope: rope_base must be > 1");
-    return attn_impl(nullptr, qkv, rope_base, 1, is_bf16, out, head_num, kv_head_num, head_dim, batch, max_blocks_per_seq, max_seq_len,
-                     page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, stream);
+    AttnCall c{"paged_decode_attn_rope", AttnMode::kRope, qkv, is_bf16, out, head_num, kv_head_num, head_dim, batch, 1, max_blocks_per_seq,
+               max_seq_len, page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, stream};
+    c.rope_base = rope_base;
+    return attn_impl(c);
 }
 
 int b200_paged_decode_attn_beam(const void* q, int is_bf16, void* out, size_t head_num, size_t kv_head_num, size_t head_dim,
                                 size_t requests, size_t beam_width, size_t max_blocks_per_seq, size_t max_seq_len, size_t page_size,
                                 const void* kv_pool, const int32_t* page_list, const uint32_t* sequence_lengths,
                                 const int32_t* shared_lengths, float q_scale, void* workspace, size_t workspace_bytes, void* stream) {
-    ARG_CHECK(beam_width >= 1 && beam_width <= (size_t)kAttnMaxRows, "paged_decode_attn_beam: beam_width %zu unsupported (1..%d)",
-              beam_width, kAttnMaxRows);
-    ARG_CHECK(requests * kv_head_num <= 65535, "paged_decode_attn_beam: requests*kv_heads %zu exceeds grid limit", requests * kv_head_num);
-    ARG_CHECK((q && shared_lengths) || requests == 0, "paged_decode_attn_beam: null pointer (q or shared_lengths)");
-    return attn_impl(q, nullptr, 0.f, 1, is_bf16, out, head_num, kv_head_num, head_dim, requests, max_blocks_per_seq, max_seq_len,
-                     page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, stream, (int)beam_width,
-                     shared_lengths);
+    return attn_impl({"paged_decode_attn_beam", AttnMode::kBeam, q, is_bf16, out, head_num, kv_head_num, head_dim, requests, beam_width,
+                      max_blocks_per_seq, max_seq_len, page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace,
+                      workspace_bytes, stream, shared_lengths});
 }
 
 int b200_paged_decode_attn_prefix(const void* q, int is_bf16, void* out, size_t head_num, size_t kv_head_num, size_t head_dim,
@@ -601,30 +621,19 @@ int b200_paged_decode_attn_prefix(const void* q, int is_bf16, void* out, size_t 
                                   size_t max_seq_len, size_t page_size, const void* kv_pool, const int32_t* page_list,
                                   const uint32_t* sequence_lengths, float q_scale, void* workspace, size_t workspace_bytes,
                                   void* stream) {
-    if (batch == 0) return B200_OK;
-    ARG_CHECK(q && chunk_offsets && chunk_rows && shared_lengths, "paged_decode_attn_prefix: null pointer (q or a chunk array)");
-    ARG_CHECK(chunks >= 1 && chunks <= batch, "paged_decode_attn_prefix: chunks %zu must be in 1..batch (%zu)", chunks, batch);
-    ARG_CHECK(batch <= 65535, "paged_decode_attn_prefix: batch %zu exceeds 65535 rows", batch);
-    ARG_CHECK(kv_head_num > 0 && head_num % kv_head_num == 0, "paged_decode_attn_prefix: head_num %zu not a multiple of kv_head_num %zu",
-              head_num, kv_head_num);
-    ARG_CHECK(max_members >= 1 && (head_num / kv_head_num) * max_members <= (size_t)kAttnMaxRows,
-              "paged_decode_attn_prefix: group %zu x max_members %zu exceeds the limit of %d query rows per (chunk, kv head)",
-              head_num / kv_head_num, max_members, kAttnMaxRows);
-    ARG_CHECK(chunks * kv_head_num <= 65535, "paged_decode_attn_prefix: chunks*kv_heads %zu exceeds grid limit", chunks * kv_head_num);
-    return attn_impl(q, nullptr, 0.f, 1, is_bf16, out, head_num, kv_head_num, head_dim, batch, max_blocks_per_seq, max_seq_len,
-                     page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, stream, (int)max_members,
-                     shared_lengths, nullptr, chunks, chunk_offsets, chunk_rows);
+    return attn_impl({"paged_decode_attn_prefix", AttnMode::kPrefix, q, is_bf16, out, head_num, kv_head_num, head_dim, batch, max_members,
+                      max_blocks_per_seq, max_seq_len, page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace,
+                      workspace_bytes, stream, shared_lengths, chunks, chunk_offsets, chunk_rows});
 }
 
 int b200_paged_decode_attn_tree(const void* q, int is_bf16, void* out, size_t head_num, size_t kv_head_num, size_t head_dim,
                                 size_t batch, size_t q_len, size_t max_blocks_per_seq, size_t max_seq_len, size_t page_size,
                                 const void* kv_pool, const int32_t* page_list, const uint32_t* sequence_lengths,
                                 const int32_t* tree_parents, float q_scale, void* workspace, size_t workspace_bytes, void* stream) {
-    ARG_CHECK((q && tree_parents) || batch == 0, "paged_decode_attn_tree: null pointer (q or tree_parents)");
-    ARG_CHECK(q_len >= 1 && q_len <= (size_t)kAttnMaxRows, "paged_decode_attn_tree: q_len %zu unsupported (1..%d)", q_len, kAttnMaxRows);
-    return attn_impl(q, nullptr, 0.f, (int)q_len, is_bf16, out, head_num, kv_head_num, head_dim, batch, max_blocks_per_seq, max_seq_len,
-                     page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, stream, 0, nullptr,
-                     tree_parents);
+    AttnCall c{"paged_decode_attn_tree", AttnMode::kTree, q, is_bf16, out, head_num, kv_head_num, head_dim, batch, q_len, max_blocks_per_seq,
+               max_seq_len, page_size, kv_pool, page_list, sequence_lengths, q_scale, workspace, workspace_bytes, stream};
+    c.tree_parents = tree_parents;
+    return attn_impl(c);
 }
 
 // ------------------------------------------------------------------------------------------------ GEMM

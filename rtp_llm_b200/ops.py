@@ -123,23 +123,24 @@ def attn_workspace(batch: int, head_num: int, kv_head_num: int, max_seq_len: int
 
 def _paged_attn(entry: str, q: torch.Tensor, kv_cache_base: torch.Tensor, page_list: torch.Tensor, sequence_lengths: torch.Tensor,
                 max_seq_len: int, workspace: torch.Tensor, out: Optional[torch.Tensor], rows: tuple, seqs: int, Hq: Optional[int],
-                extra: tuple) -> torch.Tensor:
+                extra: tuple, sizes: Optional[tuple] = None) -> torch.Tensor:
     """The call of b200_<entry> that the paged_decode_attn* wrappers share. rows: the sizes before the heads, (B,) or (B, q_len
-    or W), passed after head_dim; seqs: the sequences whose lengths the kernel reads; out [*rows, Hq*D] of q's dtype is
-    allocated when not given; Hq None: q's elements over rows * D. extra: the arguments between sequence_lengths and the
-    workspace (q_scale among them); tensors among them are checked and passed as pointers."""
-    tensors = [t for t in extra if isinstance(t, torch.Tensor)]
-    _cuda_contig(q, kv_cache_base, page_list, *tensors, workspace, out)
+    or W), passed after head_dim unless `sizes` is passed there instead; seqs: the sequences whose lengths the kernel reads;
+    out [*rows, Hq*D] of q's dtype is allocated when not given; Hq None: q's elements over rows * D. extra: the arguments
+    between sequence_lengths and the workspace (q_scale among them). Tensors among sizes and extra are checked and passed as
+    pointers."""
+    sizes = rows if sizes is None else sizes
+    _cuda_contig(q, kv_cache_base, page_list, *(t for t in sizes + extra if isinstance(t, torch.Tensor)), workspace, out)
     check_lengths(entry, sequence_lengths, seqs)
     P, two, Hkv, T, D = kv_cache_base.shape
     if Hq is None:
         Hq = q.numel() // (math.prod(rows) * D)
     if out is None:
         out = torch.empty((*rows, Hq * D), dtype=q.dtype, device=q.device)
+    arg = lambda a: _p(a) if isinstance(a, torch.Tensor) else a   # tensors go to C as pointers
     check(getattr(_lib.load(), "b200_" + entry)(
-        _p(q), _is_bf16(q), _p(out), Hq, Hkv, D, *rows, page_list.shape[-1], max_seq_len, T, _p(kv_cache_base), _p(page_list),
-        _p(sequence_lengths), *(_p(a) if isinstance(a, torch.Tensor) else a for a in extra), _p(workspace), workspace.numel(),
-        _stream()), "b200_" + entry)
+        _p(q), _is_bf16(q), _p(out), Hq, Hkv, D, *map(arg, sizes), page_list.shape[-1], max_seq_len, T, _p(kv_cache_base),
+        _p(page_list), _p(sequence_lengths), *map(arg, extra), _p(workspace), workspace.numel(), _stream()), "b200_" + entry)
     return out
 
 
@@ -179,21 +180,13 @@ def paged_decode_attn_prefix(q: torch.Tensor, kv_cache_base: torch.Tensor, page_
     whose page_list rows are equal over the first shared_lengths[c] / T pages (int32 [chunks]). prefix_chunks builds the three
     from a block table. Rows in no chunk are not written. Returns [B, Hq*D]."""
     who = "paged_decode_attn_prefix"
-    _cuda_contig(q, kv_cache_base, page_list, chunk_offsets, chunk_rows, shared_lengths, workspace, out)
-    P, two, Hkv, T, D = kv_cache_base.shape
-    B = q.shape[0]
-    check_lengths(who, sequence_lengths, B)
-    C = shared_lengths.numel()
+    B, C, D = q.shape[0], shared_lengths.numel(), kv_cache_base.shape[-1]
     _need(who, "chunk_offsets", chunk_offsets, torch.int32, (C + 1,), flat=True)
     _need(who, "chunk_rows", chunk_rows, torch.int32, (B,), flat=True)
     _need(who, "shared_lengths", shared_lengths, torch.int32, ("chunks",))
-    Hq = q.numel() // (B * D)
-    out = _outputs(who, {"attn_out": out}, q.device, attn_out=(q.dtype, (B, Hq * D)))["attn_out"]
-    check(_lib.load().b200_paged_decode_attn_prefix(
-        _p(q), _is_bf16(q), _p(out), Hq, Hkv, D, B, C, max_members, _p(chunk_offsets), _p(chunk_rows), _p(shared_lengths),
-        page_list.shape[-1], max_seq_len, T, _p(kv_cache_base), _p(page_list), _p(sequence_lengths), q_scale, _p(workspace),
-        workspace.numel(), _stream()), "b200_" + who)
-    return out
+    out = _outputs(who, {"attn_out": out}, q.device, attn_out=(q.dtype, (B, q.numel() // (B * D) * D)))["attn_out"]
+    return _paged_attn(who, q, kv_cache_base, page_list, sequence_lengths, max_seq_len, workspace, out, (B,), B, None, (q_scale,),
+                       (B, C, max_members, chunk_offsets, chunk_rows, shared_lengths))
 
 
 def prefix_chunks(block_ids: torch.Tensor, sequence_lengths: torch.Tensor, tokens_per_block: int,

@@ -58,8 +58,10 @@ def _page_list(g, rows, M, P):
 
 
 # ---------------------------------------------------------------------------------------------- attention
-def _attn(fn, dtype=F16, D=128, B=3, Hq=16, Hkv=2, T=16, q_len=1, max_len=200, W=0):
+def _attn(fn, dtype=F16, D=128, B=3, Hq=16, Hkv=2, T=16, q_len=1, max_len=200, W=0, chunks=()):
+    """chunks (prefix): the sizes of the chunks over the B = sum(chunks) rows."""
     from rtp_llm_b200 import ops
+    B = sum(chunks) or B
     rows = B * W if W else B
     M = -(-max_len // T)
     P = rows * 2 * M + 1
@@ -80,6 +82,21 @@ def _attn(fn, dtype=F16, D=128, B=3, Hq=16, Hkv=2, T=16, q_len=1, max_len=200, W
                 shared[b] = s
                 pl[b * W + 1: (b + 1) * W, :, :, : s // T] = pl[b * W, :, :, : s // T]
             d["shared"] = shared.to(DEV)
+        elif fn == "prefix":
+            # the chunk sizes in a seeded order over a seeded permutation of the rows; a chunk's members share the first
+            # member's pages below their shortest cached length
+            d["q"] = _randn(g, B, Hq, D, dtype=dtype)
+            order = torch.randperm(B, generator=g).tolist()
+            offs, shared = [0], []
+            for n in (chunks[i] for i in torch.randperm(len(chunks), generator=g).tolist()):
+                members = order[offs[-1]: offs[-1] + n]
+                s = T * (int(seq[members].min()) // T) if n > 1 else 0
+                for r in members[1:]:
+                    pl[r, :, :, : s // T] = pl[members[0], :, :, : s // T]
+                offs.append(offs[-1] + n)
+                shared.append(s)
+            d.update(offs=torch.tensor(offs, dtype=I32).to(DEV), rows=torch.tensor(order, dtype=I32).to(DEV),
+                     shared=torch.tensor(shared, dtype=I32).to(DEV))
         elif fn == "single":
             d["q"] = _randn(g, B, Hq, D, dtype=dtype)
         else:
@@ -91,7 +108,7 @@ def _attn(fn, dtype=F16, D=128, B=3, Hq=16, Hkv=2, T=16, q_len=1, max_len=200, W
         d.update(pl=pl, seq=seq.to(DEV))
         return d
 
-    out_rows = (B,) if fn in ("single", "rope") else (B, W if W else q_len)
+    out_rows = (B,) if fn in ("single", "rope", "prefix") else (B, W if W else q_len)
 
     def call(b):
         kw = dict(out=b["out"])
@@ -103,6 +120,9 @@ def _attn(fn, dtype=F16, D=128, B=3, Hq=16, Hkv=2, T=16, q_len=1, max_len=200, W
             ops.paged_decode_attn_beam(b["q"], b["pool"], b["pl"], b["seq"], b["shared"], max_len, b["ws"], **kw)
         elif fn == "tree":
             ops.paged_decode_attn_tree(b["q"], b["pool"], b["pl"], b["seq"], b["parents"], max_len, b["ws"], **kw)
+        elif fn == "prefix":
+            ops.paged_decode_attn_prefix(b["q"], b["pool"], b["pl"], b["seq"], b["offs"], b["rows"], b["shared"], max(chunks), max_len,
+                                         b["ws"], **kw)
         else:
             ops.paged_decode_attn_rope(b["qkv"], b["pool"], b["pl"], b["seq"], Hq, max_len, 10000.0, b["ws"], **kw)
 
@@ -128,6 +148,8 @@ ATTN = [
     Case("attn multi rt4 f16 workspace merge", ("paged_decode_attn_kernel",), _attn("multi", q_len=8, max_len=700), WORKSPACE),
     Case("attn beam w4 bf16", ("paged_decode_attn_kernel",), _attn("beam", BF16, W=4, Hq=8, max_len=200), CLUSTER),
     Case("attn tree f16", ("paged_decode_attn_kernel",), _attn("tree", q_len=6, Hq=8, max_len=300), CLUSTER),
+    Case("attn prefix chunks 3 2 1 f16 workspace merge", ("paged_decode_attn_kernel",), _attn("prefix", chunks=(3, 2, 1), max_len=600),
+         WORKSPACE),
     Case("attn rope f16", ("paged_decode_attn_kernel",), _attn("rope", Hq=8, max_len=300)),
     Case("attn rope bf16 cluster merge", ("paged_decode_attn_kernel",), _attn("rope", BF16, Hq=8, max_len=300), CLUSTER),
 ]
