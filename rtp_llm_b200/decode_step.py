@@ -147,6 +147,89 @@ def weight_bytes(cfg: ModelConfig, K: int, N: int) -> float:
     return 2 * E
 
 
+def _per_request(v, n: int, name: str) -> list:
+    """One value for every request, or a sequence of one value per request, as a list of n values."""
+    vals = list(v) if isinstance(v, (list, tuple)) else [v] * n
+    if len(vals) != n:
+        raise ValueError(f"{name}: {len(vals)} values for {n} requests")
+    return vals
+
+
+def _check_options(cfg, batch, ctx, tp_size, act_order, q_len, beam_width, no_repeat_ngram, max_new_tokens, sampling, logprobs,
+                   eos_id, length_penalty, early_stopping, token_bitmask, logit_bias_capacity, tree, shared_prefix, max_rows,
+                   advances) -> None:
+    """DecodeStep's option checks, before anything is allocated: ValueError for the first fault, in this order."""
+    assert cfg.head_num % tp_size == 0 and cfg.inter % tp_size == 0
+    if shared_prefix is not None:
+        n_share, p_tokens = shared_prefix
+        if not (n_share >= 1 and p_tokens >= 0):
+            raise ValueError(f"shared_prefix: (requests_per_prefix >= 1, prefix_tokens >= 0) (got {shared_prefix})")
+        if q_len != 1 or tree is not None or beam_width != 1 or sampling is not None or tp_size != 1:
+            raise ValueError(f"shared_prefix needs the greedy step: q_len 1, no tree, beam_width 1, no sampling and tp_size 1 "
+                             f"(got q_len {q_len}, tree {tree is not None}, beam_width {beam_width}, sampling "
+                             f"{sampling is not None}, tp_size {tp_size})")
+    if logit_bias_capacity < 0:
+        raise ValueError(f"logit_bias_capacity must be >= 0 (got {logit_bias_capacity})")
+    if (token_bitmask or logit_bias_capacity) and tp_size != 1:
+        raise ValueError(f"token_bitmask / logit_bias need tp_size 1 (got tp_size {tp_size}): the vocabulary-parallel argmax "
+                         "would need a mask sharded by vocabulary")
+    if sampling is not None:
+        mp = sampling.min_p if isinstance(sampling.min_p, (list, tuple)) else [sampling.min_p]
+        if not all(0.0 <= float(v) <= 1.0 for v in mp):
+            raise ValueError(f"sampling: min_p must be in [0, 1] (got {sampling.min_p})")
+    if not 1 <= max_rows <= GEMM_MAX_ROWS:
+        raise ValueError(f"max_rows must be in 1..{GEMM_MAX_ROWS}, the GEMM row limit (got {max_rows})")
+    if q_len < 1:
+        raise ValueError(f"q_len must be >= 1 (got {q_len})")
+    # the verification, beam and sampling modes run TP 1 on at most max_rows token rows
+    rows = f"<= {max_rows} (max_rows; the GEMM row limit is {GEMM_MAX_ROWS})"
+    if q_len > 1 and (batch * q_len > max_rows or tp_size != 1):
+        raise ValueError(f"a verification step (q_len {q_len}) needs batch * q_len {rows} and tp_size 1 (got batch {batch}, "
+                         f"tp_size {tp_size})")
+    if tree is not None and q_len < 2:
+        raise ValueError(f"a token-tree step needs q_len >= 2 nodes (got q_len {q_len})")
+    if not 1 <= beam_width <= 32:
+        raise ValueError(f"beam_width must be in 1..32 (got {beam_width})")
+    if beam_width > 1 and (batch * beam_width > max_rows or tp_size != 1 or q_len != 1):
+        raise ValueError(f"beam search (beam_width {beam_width}) needs batch * beam_width {rows}, tp_size 1 and q_len 1 "
+                         f"(got batch {batch}, tp_size {tp_size}, q_len {q_len})")
+    if sampling is not None:
+        if tp_size != 1 or beam_width != 1 or batch * q_len > max_rows:
+            raise ValueError(f"sampling needs tp_size 1, beam_width 1 and batch * q_len {rows} (got tp_size {tp_size}, "
+                             f"beam_width {beam_width}, batch {batch}, q_len {q_len})")
+        if q_len > 1 and (sampling.has_penalties() or no_repeat_ngram != 0):
+            raise ValueError("sampled verification (q_len > 1) takes no penalties and no n-gram ban: row j's history would "
+                             "have to hold drafts 0..j-1")
+        if logprobs is not None and not 0 <= logprobs <= ops.LOGPROB_MAX_TOP_N:
+            raise ValueError(f"logprobs must be in 0..{ops.LOGPROB_MAX_TOP_N} (got {logprobs})")
+    elif logprobs is not None:
+        raise ValueError("logprobs needs the sampling mode (sampling=SamplingParams(...))")
+    if advances and not 1 <= max_new_tokens < ctx:
+        raise ValueError(f"max_new_tokens must be in 1..ctx-1 (got {max_new_tokens}, ctx {ctx})")
+    if no_repeat_ngram != 0 and beam_width == 1 and sampling is None:
+        raise ValueError(f"no_repeat_ngram {no_repeat_ngram} needs beam search (beam_width > 1); the greedy step has no ban")
+    if eos_id is not None:
+        if beam_width == 1 or not 0 <= eos_id < cfg.vocab:
+            raise ValueError(f"eos_id needs beam search (beam_width > 1) and must be in 0..vocab-1 (got eos_id {eos_id}, "
+                             f"beam_width {beam_width})")
+        for a in _per_request(length_penalty, batch, "length_penalty"):
+            float(a)                # (a value that is not a number raises here)
+        for m in _per_request(early_stopping, batch, "early_stopping"):
+            if m not in (False, True, "never"):
+                raise ValueError(f"early_stopping must be False, True or \"never\" (got {m!r})")
+    R = batch * beam_width * q_len
+    if R > GEMM_MAX_ROWS or (R > TP_MAX_ROWS and tp_size != 1):
+        raise ValueError(f"a step runs at most {GEMM_MAX_ROWS} token rows (the GEMM row limit), and at most {TP_MAX_ROWS} with "
+                         f"tp_size > 1 (got {R} rows, tp_size {tp_size})")
+    if act_order and (tp_size != 1 or cfg.quant not in ("int4", "int8g")):
+        raise ValueError(f"act_order needs tp_size 1 and quant int4 / int8g (got tp_size {tp_size}, quant {cfg.quant})")
+    if sampling is not None:        # the per-request parameters the step uploads
+        sp = sampling
+        for v in ([sp.temperature, sp.top_k, sp.top_p] + [sp.repetition, sp.presence, sp.frequency] * sp.has_penalties()
+                  + [sp.min_p] * sp.has_min_p()):
+            _per_request(v, batch, "sampling")
+
+
 class DecodeStep:
     """Synthetic decode step. tp_size > 1 shards exactly as the reference's TP split (utils/model_weight.py:1489-1580):
     qkv / w13 column-parallel, o / w2 row-parallel + all-reduce, lm_head vocab-parallel + all-gather.
@@ -244,89 +327,18 @@ class DecodeStep:
                  early_stopping: Union[bool, str, Sequence[Union[bool, str]]] = False,
                  token_bitmask: bool = False, logit_bias_capacity: int = 0, tree=None, shared_prefix=None,
                  max_rows: int = TP_MAX_ROWS):
-        assert cfg.head_num % tp_size == 0 and cfg.inter % tp_size == 0
-        if shared_prefix is not None:
-            n_share, p_tokens = shared_prefix
-            if not (n_share >= 1 and p_tokens >= 0):
-                raise ValueError(f"shared_prefix: (requests_per_prefix >= 1, prefix_tokens >= 0) (got {shared_prefix})")
-            if q_len != 1 or tree is not None or beam_width != 1 or sampling is not None or tp_size != 1:
-                raise ValueError(f"shared_prefix needs the greedy step: q_len 1, no tree, beam_width 1, no sampling and tp_size 1 "
-                                 f"(got q_len {q_len}, tree {tree is not None}, beam_width {beam_width}, sampling "
-                                 f"{sampling is not None}, tp_size {tp_size})")
-            fuse_rope = False       # (the fused rope runs its own attention; the shared-prefix path needs the rope kernel)
-        self.shared_prefix = shared_prefix
-        if logit_bias_capacity < 0:
-            raise ValueError(f"logit_bias_capacity must be >= 0 (got {logit_bias_capacity})")
-        if (token_bitmask or logit_bias_capacity) and tp_size != 1:
-            raise ValueError(f"token_bitmask / logit_bias need tp_size 1 (got tp_size {tp_size}): the vocabulary-parallel argmax "
-                             "would need a mask sharded by vocabulary")
-        if sampling is not None:
-            mp = sampling.min_p if isinstance(sampling.min_p, (list, tuple)) else [sampling.min_p]
-            if not all(0.0 <= float(v) <= 1.0 for v in mp):
-                raise ValueError(f"sampling: min_p must be in [0, 1] (got {sampling.min_p})")
-        if not 1 <= max_rows <= GEMM_MAX_ROWS:
-            raise ValueError(f"max_rows must be in 1..{GEMM_MAX_ROWS}, the GEMM row limit (got {max_rows})")
-        if q_len < 1:
-            raise ValueError(f"q_len must be >= 1 (got {q_len})")
-        if q_len > 1 and (batch * q_len > max_rows or tp_size != 1):
-            raise ValueError(f"a verification step (q_len {q_len}) needs batch * q_len <= {max_rows} (max_rows; the GEMM row limit "
-                             f"is {GEMM_MAX_ROWS}) and tp_size 1 "
-                             f"(got batch {batch}, tp_size {tp_size})")
-        if tree is not None and q_len < 2:
-            raise ValueError(f"a token-tree step needs q_len >= 2 nodes (got q_len {q_len})")
-        if not 1 <= beam_width <= 32:
-            raise ValueError(f"beam_width must be in 1..32 (got {beam_width})")
-        if beam_width > 1 and (batch * beam_width > max_rows or tp_size != 1 or q_len != 1):
-            raise ValueError(f"beam search (beam_width {beam_width}) needs batch * beam_width <= {max_rows} (max_rows; the GEMM row "
-                             f"limit is {GEMM_MAX_ROWS}), tp_size 1 "
-                             f"and q_len 1 (got batch {batch}, tp_size {tp_size}, q_len {q_len})")
-        if sampling is not None:
-            if tp_size != 1 or beam_width != 1 or batch * q_len > max_rows:
-                raise ValueError(f"sampling needs tp_size 1, beam_width 1 and batch * q_len <= {max_rows} (max_rows; the GEMM row limit "
-                                 f"is {GEMM_MAX_ROWS}) (got tp_size "
-                                 f"{tp_size}, beam_width {beam_width}, batch {batch}, q_len {q_len})")
-            if q_len > 1 and (sampling.has_penalties() or no_repeat_ngram != 0):
-                raise ValueError("sampled verification (q_len > 1) takes no penalties and no n-gram ban: row j's history would "
-                                 "have to hold drafts 0..j-1")
-            if logprobs is not None and not 0 <= logprobs <= ops.LOGPROB_MAX_TOP_N:
-                raise ValueError(f"logprobs must be in 0..{ops.LOGPROB_MAX_TOP_N} (got {logprobs})")
-        elif logprobs is not None:
-            raise ValueError("logprobs needs the sampling mode (sampling=SamplingParams(...))")
-        self.samp = sampling
-        self.logprobs = logprobs
-        self.sample_advances = sampling is not None and q_len == 1
-        if (beam_width > 1 or self.sample_advances) and not 1 <= max_new_tokens < ctx:
-            raise ValueError(f"max_new_tokens must be in 1..ctx-1 (got {max_new_tokens}, ctx {ctx})")
-        if no_repeat_ngram != 0 and beam_width == 1 and sampling is None:
-            raise ValueError(f"no_repeat_ngram {no_repeat_ngram} needs beam search (beam_width > 1); the greedy step has no ban")
+        self.advances = beam_width > 1 or (sampling is not None and q_len == 1)   # tokens join the history, lengths grow
+        self.redraws = sampling is not None     # every run moves the draw counter on, at any q_len, advancing or not
+        _check_options(cfg, batch, ctx, tp_size, act_order, q_len, beam_width, no_repeat_ngram, max_new_tokens, sampling,
+                       logprobs, eos_id, length_penalty, early_stopping, token_bitmask, logit_bias_capacity, tree, shared_prefix,
+                       max_rows, self.advances)
+        self.shared_prefix, self.samp, self.logprobs, self.eos_id = shared_prefix, sampling, logprobs, eos_id
         self.W, self.ngram, self.max_new_tokens = beam_width, no_repeat_ngram, max_new_tokens
-        if eos_id is not None:
-            if beam_width == 1 or not 0 <= eos_id < cfg.vocab:
-                raise ValueError(f"eos_id needs beam search (beam_width > 1) and must be in 0..vocab-1 (got eos_id {eos_id}, "
-                                 f"beam_width {beam_width})")
-
-            def per_request(v, name):
-                vals = list(v) if isinstance(v, (list, tuple)) else [v] * batch
-                if len(vals) != batch:
-                    raise ValueError(f"{name}: {len(vals)} values for {batch} requests")
-                return vals
-            alphas = [float(a) for a in per_request(length_penalty, "length_penalty")]
-            modes = per_request(early_stopping, "early_stopping")
-            for m in modes:
-                if m not in (False, True, "never"):
-                    raise ValueError(f"early_stopping must be False, True or \"never\" (got {m!r})")
-            modes = [2 if m == "never" else int(bool(m)) for m in modes]
-        self.eos_id = eos_id
-        self.beam_steps = 0                             # beam / sampled steps run since the prompt (upload_inputs)
+        self.new_tokens = 0                             # steps the step has advanced since the prompt (upload_inputs)
         self.requests = batch
         batch = batch * beam_width                      # sequences (page-table rows) of the step
         self.q_len = q_len
         R = batch * q_len                               # token rows of the step
-        if R > GEMM_MAX_ROWS or (R > TP_MAX_ROWS and tp_size != 1):
-            raise ValueError(f"a step runs at most {GEMM_MAX_ROWS} token rows (the GEMM row limit), and at most {TP_MAX_ROWS} with "
-                             f"tp_size > 1 (got {R} rows, tp_size {tp_size})")
-        if act_order and (tp_size != 1 or cfg.quant not in ("int4", "int8g")):
-            raise ValueError(f"act_order needs tp_size 1 and quant int4 / int8g (got tp_size {tp_size}, quant {cfg.quant})")
         self.act_order = act_order
         self.cfg, self.B, self.ctx, self.dev, self.dtype = cfg, batch, ctx, device, dtype
         self.tp_rank, self.tp_size, self.comm, self.pdl = tp_rank, tp_size, comm, pdl
@@ -355,9 +367,9 @@ class DecodeStep:
         if fuse_rope is None:
             fuse_rope = os.environ.get("B200_FUSE_ROPE", "0") == "1"
         self.rope_spec = RopeSpec(dim=self.D, base=cfg.rope_base) if cfg.rope is None else rope.spec_of(cfg.rope, self.D)
-        # the fused rope appends one token with plain Base rotation, and does not normalise q / k
-        self.fuse_rope = (bool(fuse_rope) and cfg.head_dim == 128 and q_len == 1 and rope.is_plain_base(self.rope_spec, self.D)
-                          and not cfg.qk_norm)
+        # the fused rope appends one token with plain Base rotation, does not normalise q / k and has no shared-prefix attention
+        self.fuse_rope = (shared_prefix is None and bool(fuse_rope) and cfg.head_dim == 128 and q_len == 1
+                          and rope.is_plain_base(self.rope_spec, self.D) and not cfg.qk_norm)
         g = torch.Generator(device="cpu").manual_seed(seed * 1000 + 17)
         H = cfg.hidden
 
@@ -466,9 +478,9 @@ class DecodeStep:
             lens = torch.randint(ctx // 2, ctx + 1, (batch,), generator=gl)
         else:
             lens = torch.full((batch,), ctx)
-        if beam_width > 1:    # one prompt per request, room for max_new_tokens
-            lens = (lens.view(-1, beam_width)[:, :1].expand(-1, beam_width).reshape(-1) - max_new_tokens + 1).clamp(min=1)
-        elif self.sample_advances:
+        if beam_width > 1:    # one prompt per request
+            lens = lens.view(-1, beam_width)[:, :1].expand(-1, beam_width).reshape(-1)
+        if self.advances:     # room for max_new_tokens
             lens = (lens - max_new_tokens + 1).clamp(min=1)
         self.seq_lens_h = (lens - q_len).to(torch.int32).pin_memory()   # tokens already cached (SURVEY a3)
         self.ids_h = torch.randint(0, cfg.vocab, (batch,) if q_len == 1 else (batch, q_len), generator=gp).to(torch.int32).pin_memory()
@@ -488,6 +500,7 @@ class DecodeStep:
             # groups of n_share requests on rows a seeded permutation scatters over the batch; each group's members point at the
             # first member's pages over the whole pages of the prefix that every member has cached, and at their own after them
             # (so the token a step appends never lands in a shared page)
+            n_share, p_tokens = shared_prefix
             rows = torch.randperm(batch, generator=torch.Generator().manual_seed(seed + 71)).tolist()
             for k in range(0, batch, n_share):
                 grp = rows[k:k + n_share]
@@ -495,10 +508,6 @@ class DecodeStep:
                 for r in grp[1:]:
                     self.block_ids_h[r, :f] = self.block_ids_h[grp[0], :f]
         self.next_h = torch.zeros(batch, dtype=torch.int32).pin_memory()
-        if q_len > 1:
-            self.drafts_h = torch.zeros(batch, q_len - 1, dtype=torch.int32).pin_memory()
-            self.out_tokens_h = torch.zeros(batch, q_len, dtype=torch.int32).pin_memory()
-            self.accepted_h = torch.zeros(batch, dtype=torch.int32).pin_memory()
 
         # ---- static device buffers (graph-capturable: nothing is allocated inside step())
         def buf(*shape, dt=dtype):
@@ -518,10 +527,14 @@ class DecodeStep:
         self.logits = buf(R, self.vocab)
         self.logits_all = buf(tp_size, batch, self.vocab) if tp_size > 1 else None
         self.next_ids = buf(R, dt=torch.int32)                                # each row's greedy token
-        if q_len > 1:
+        if q_len > 1:           # the drafts and the verification's outputs, with their pinned host twins
+            self.drafts_h = torch.zeros(batch, q_len - 1, dtype=torch.int32).pin_memory()
+            self.out_tokens_h = torch.zeros(batch, q_len, dtype=torch.int32).pin_memory()
+            self.accepted_h = torch.zeros(batch, dtype=torch.int32).pin_memory()
             self.drafts = buf(batch, q_len - 1, dt=torch.int32)
             self.out_tokens = buf(batch, q_len, dt=torch.int32)
             self.accepted = buf(batch, dt=torch.int32)
+        self.tree_parents = None
         if tree is not None:    # the token tree: parents and depths (pinned twins set_tree() fills), rotation positions, path
             self.tree_parents_h = torch.zeros(batch, q_len, dtype=torch.int32).pin_memory()
             self.tree_depth_h = torch.zeros(batch, q_len, dtype=torch.int32).pin_memory()
@@ -533,12 +546,14 @@ class DecodeStep:
         if shared_prefix is not None:   # the chunking (ops.prefix_chunks), filled by upload_inputs
             self.chunk_offsets_d, self.chunk_rows_d, self.chunk_shared_d = (buf(n, dt=torch.int32) for n in (batch + 1, batch, batch))
             self.use_prefix = False
+        if self.advances:       # the token history: upload_inputs() restarts it from the input token, _advance() appends
+            self.hist = buf(R, ctx, dt=torch.int32)
+            self.hist_len = buf(R, dt=torch.int32)
+            self.hist_pos = buf(R, dt=torch.int64)
+            self.ngram_size = torch.full((R,), no_repeat_ngram, dtype=torch.int32, device=device)
         if beam_width > 1:
             W, B = beam_width, self.requests
             self.beam_cum = buf(B, W, dt=torch.float32)
-            self.hist = buf(R, ctx, dt=torch.int32)
-            self.hist_len = buf(R, dt=torch.int32)
-            self.ngram_size = torch.full((R,), no_repeat_ngram, dtype=torch.int32, device=device)
             self.beam_out = {k: buf(B, n, dt=dt) for k, n, dt in (
                 ("cand_token", 2 * W, torch.int32), ("cand_parent", 2 * W, torch.int32), ("cand_score", 2 * W, torch.float32),
                 ("next_token", W, torch.int32), ("next_parent", W, torch.int32), ("next_cum", W, torch.float32))}
@@ -562,14 +577,13 @@ class DecodeStep:
             if eos_id is not None:    # the finished-hypothesis sets (emptied by upload_inputs)
                 self.hyp_state = ops.beam_hypotheses_state(B, W, max_new_tokens, device)
                 self.done = torch.zeros(B, dtype=torch.int32, device=device)
-                self.length_penalty = torch.tensor(alphas, dtype=torch.float32, device=device)
-                self.early_stopping = torch.tensor(modes, dtype=torch.int32, device=device)
+                lp, es = _per_request(length_penalty, B, "length_penalty"), _per_request(early_stopping, B, "early_stopping")
+                self.length_penalty = torch.tensor([float(a) for a in lp], dtype=torch.float32, device=device)
+                self.early_stopping = torch.tensor([2 if m == "never" else int(bool(m)) for m in es], dtype=torch.int32,
+                                                   device=device)
         if sampling is not None:
             def per_row(v, dt):
-                t = torch.tensor(v if isinstance(v, (list, tuple)) else [v] * batch, dtype=dt)
-                if t.numel() != batch:
-                    raise ValueError(f"sampling: {len(v)} values for {batch} requests")
-                return t.repeat_interleave(q_len).to(device)
+                return torch.tensor(_per_request(v, batch, "sampling"), dtype=dt).repeat_interleave(q_len).to(device)
             sp = sampling
             self.samp_params = dict(temperature=per_row(sp.temperature, torch.float32), top_k=per_row(sp.top_k, torch.int32),
                                     top_p=per_row(sp.top_p, torch.float32))
@@ -587,10 +601,6 @@ class DecodeStep:
             self.uniforms = _Uniforms(sp.seed, self.uniform.numel(), device)
             if q_len == 1:
                 self.cum_log_probs = buf(R, dt=torch.float32)
-                self.hist = buf(R, ctx, dt=torch.int32)
-                self.hist_len = buf(R, dt=torch.int32)
-                self.ngram_size = torch.full((R,), no_repeat_ngram, dtype=torch.int32, device=device)
-                self.hist_pos = buf(R, dt=torch.int64)
             else:
                 self.target_probs = buf(batch, q_len, self.vocab, dt=torch.float32)
             if logprobs is not None:
@@ -598,14 +608,12 @@ class DecodeStep:
                                    top_logprobs=buf(R, logprobs, dt=torch.float32))
                 self.lp_ws = ops.token_logprobs_workspace(R, self.vocab, logprobs, device)
         # constrained decoding: device buffers the step reads, pinned host twins set_constraints() fills
-        if token_bitmask:
-            self.bitmask_h = torch.full((R, (self.vocab + 31) // 32), -1, dtype=torch.int32).pin_memory()
-            self.bitmask = buf(R, self.bitmask_h.shape[1], dt=torch.int32)
-        if logit_bias_capacity:
-            self.bias_h = (torch.zeros(R + 1, dtype=torch.int32).pin_memory(),
-                           torch.zeros(logit_bias_capacity, dtype=torch.int32).pin_memory(),
-                           torch.zeros(logit_bias_capacity, dtype=torch.float32).pin_memory())
-            self.bias = tuple(torch.zeros_like(t, device=device) for t in self.bias_h)
+        self.bitmask_h = torch.full((R, (self.vocab + 31) // 32), -1, dtype=torch.int32).pin_memory() if token_bitmask else None
+        self.bitmask = buf(R, self.bitmask_h.shape[1], dt=torch.int32) if token_bitmask else None
+        self.bias_h = (torch.zeros(R + 1, dtype=torch.int32).pin_memory(),
+                       torch.zeros(logit_bias_capacity, dtype=torch.int32).pin_memory(),
+                       torch.zeros(logit_bias_capacity, dtype=torch.float32).pin_memory()) if logit_bias_capacity else None
+        self.bias = tuple(torch.zeros_like(t, device=device) for t in self.bias_h) if logit_bias_capacity else None
         self.x_perm = buf(R, H) if act_order else None                        # x[:, perm] before qkv / w13
         self.attn_perm = buf(R, self.Hq * self.D) if act_order else None      # attn[:, perm] before o
         shapes = [(H, qkv_n), (self.Hq * self.D, H), (H, 2 * self.inter), (self.inter, H), (H, self.vocab)]
@@ -638,23 +646,21 @@ class DecodeStep:
             self.chunk_shared_d[:C].copy_(shared, non_blocking=True)
             self.chunks = (self.chunk_offsets_d[:C + 1], self.chunk_rows_d, self.chunk_shared_d[:C], mm)
             self.use_prefix = prefix_rows_fit(self.Hkv, C, float(shared.float().mean()), mm)
-        if self.W > 1:        # back to the prompt: beam 0 alone live (cum 0), the input token as the whole history
+        if self.advances:     # back to the prompt: the input token as the whole history
+            self.hist[:, 0].copy_(self.ids)
+            self.hist_len.fill_(1)
+            self.new_tokens = 0
+        if self.W > 1:        # beam 0 alone live (cum 0), no finished hypotheses
             self.shared_lens.copy_(self.shared_lens_h, non_blocking=True)
             self.beam_cum.fill_(-math.inf)
             self.beam_cum[:, 0] = 0.0
-            self.hist[:, 0].copy_(self.ids)
-            self.hist_len.fill_(1)
-            self.beam_steps = 0
             if self.eos_id is not None:
                 self.hyp_state.zero_()
                 self.done.zero_()
-        if self.samp is not None:  # back to the prompt: step 0 of the uniforms; at q_len 1 the input token as the whole history
+        if self.redraws:      # step 0 of the uniforms; at q_len 1 no log-prob yet
             self.draw_step.zero_()
             if self.q_len == 1:
                 self.cum_log_probs.zero_()
-                self.hist[:, 0].copy_(self.ids)
-                self.hist_len.fill_(1)
-                self.beam_steps = 0
         if self.bitmask is not None or self.bias is not None:
             self.set_constraints()
 
@@ -729,16 +735,12 @@ class DecodeStep:
         if self.bitmask is not None or self.bias is not None:
             ops.constrain_logits(logits, bitmask=self.bitmask, logit_bias=self.bias)
 
-    sample_advances = False
-    bitmask = bitmask_h = bias = bias_h = None     # no constraint buffers unless token_bitmask / logit_bias_capacity
-    tree_parents = None                             # no token tree unless tree=
-
-    def _count_beam_step(self):
-        if self.W > 1 or self.sample_advances:
-            if self.beam_steps >= self.max_new_tokens:
-                raise ValueError(f"step {self.beam_steps + 1} since the prompt exceeds max_new_tokens {self.max_new_tokens}: "
+    def _count_new_token(self):
+        if self.advances:
+            if self.new_tokens >= self.max_new_tokens:
+                raise ValueError(f"step {self.new_tokens + 1} since the prompt exceeds max_new_tokens {self.max_new_tokens}: "
                                  "call upload_inputs() to restart from the prompt")
-            self.beam_steps += 1
+            self.new_tokens += 1
 
     def download_outputs(self):
         if self.q_len > 1:
@@ -872,18 +874,14 @@ class DecodeStep:
     def fork(self):
         """Beam mode, after beam_search_step: every row becomes the new beam of its slot (see the class docstring). Torch index
         ops on static buffers only, so a CUDA graph replays it."""
-        o, T, M, cap = self.beam_out, self.cfg.tokens_per_block, self.M, self.hist.shape[1]
+        o, T, M = self.beam_out, self.cfg.tokens_per_block, self.M
         torch.add(self.row_base, o["next_parent"].view(-1), out=self.parent_row)
         self.beam_cum.copy_(o["next_cum"])
-        # token history: the parent's row, then the new token
+        # token history: the parent's row (_advance appends the new token)
         torch.index_select(self.hist, 0, self.parent_row, out=self.hist_parent)
         torch.index_select(self.hist_len, 0, self.parent_row, out=self.len_parent)
         self.hist.copy_(self.hist_parent)
-        self.pos.copy_(self.len_parent)
-        self.pos.clamp_(max=cap - 1)
-        self.hist.scatter_(1, self.pos.view(-1, 1), o["next_token"].view(-1, 1))
-        self.hist_len.copy_(self.pos)
-        self.hist_len.add_(1)
+        self.hist_len.copy_(self.len_parent)
         # page table: the parent's entries for the pages the step filled (q = (seq + 1) // T of them), the own pages after them
         self.pos.copy_(self.seq_lens)
         self.pos.add_(1)
@@ -905,7 +903,16 @@ class DecodeStep:
         for L in self.layers:
             torch.index_select(L["kv"], 0, self.src_page, out=self.page_scratch)
             L["kv"].index_copy_(0, self.dst_page, self.page_scratch)
-        self.ids.copy_(o["next_token"].view(-1))
+        self._advance(o["next_token"])
+
+    def _advance(self, tokens: torch.Tensor):
+        """The end of an advancing step: each row's token joins its history and is its next input, and the lengths grow by one.
+        The history position is clamped to the buffer; the step count (max_new_tokens < ctx) keeps it from getting there."""
+        self.hist_pos.copy_(self.hist_len)
+        self.hist_pos.clamp_(max=self.hist.shape[1] - 1)
+        self.hist.scatter_(1, self.hist_pos.view(-1, 1), tokens.view(-1, 1))
+        self.hist_len.add_(1)
+        self.ids.copy_(tokens.view(-1))
         self.seq_lens.add_(1)
 
     def beam_results(self, n: int) -> Dict[str, torch.Tensor]:
@@ -926,17 +933,16 @@ class DecodeStep:
         self.draw_step.add_(1)
         self.samp_logits.copy_(self.logits)
         self._constrain(self.samp_logits)
-        adv = self.q_len == 1
-        if adv and self.ngram > 0:
+        if self.advances and self.ngram > 0:
             ops.ban_repeat_ngram(self.samp_logits, self.hist, self.hist_len, self.ngram_size)
-        hist = dict(history=self.hist, hist_len=self.hist_len) if adv else {}
+        hist = dict(history=self.hist, hist_len=self.hist_len) if self.advances else {}
         ops.sample(self.samp_logits, sp["top_k"], sp["top_p"], self.uniform[:R], temperature=sp["temperature"],
                    repetition=sp.get("repetition"), presence=sp.get("presence"), frequency=sp.get("frequency"),
                    count_ws=sp.get("count_ws"), min_p=sp.get("min_p"), out=dict(token=self.next_ids, token_prob=self.token_prob,
-                                                         **({} if adv else dict(probs=self.target_probs))), **hist)
+                                                         **({} if self.advances else dict(probs=self.target_probs))), **hist)
         if self.logprobs is not None:
             ops.token_logprobs(self.logits, self.logprobs, tokens=self.next_ids, workspace=self.lp_ws, out=self.lp_out)
-        if not adv:
+        if not self.advances:
             if self.tree_parents is not None:
                 self._verify_tree(target_probs=self.target_probs, uniform=self.uniform[R:])
             else:
@@ -945,12 +951,7 @@ class DecodeStep:
             return
         torch.log(self.token_prob, out=self.log_prob)
         self.cum_log_probs.add_(self.log_prob)
-        self.hist_pos.copy_(self.hist_len)
-        self.hist_pos.clamp_(max=self.hist.shape[1] - 1)
-        self.hist.scatter_(1, self.hist_pos.view(-1, 1), self.next_ids.view(-1, 1))
-        self.hist_len.add_(1)
-        self.ids.copy_(self.next_ids)
-        self.seq_lens.add_(1)
+        self._advance(self.next_ids)
 
     def _verify_tree(self, **target):
         """Tree mode's ending: spec_verify_tree over the node tokens (the step's input ids; the root's is not read), then the
@@ -968,7 +969,7 @@ class DecodeStep:
 
     def step(self):
         """One decode step, op by op (one kernel per call)."""
-        self._count_beam_step()
+        self._count_new_token()
         self.step_core()
         self.step_tail()
 
@@ -977,16 +978,13 @@ class DecodeStep:
         persistent-kernel launch. Requires every call in step_core to go through the C ABI (own peer all-reduce, not NCCL)."""
         from . import tp as tpmod
         assert self.tp_size == 1 or isinstance(self.comm, tpmod.PeerComm), "a program cannot record NCCL calls"
-        if self.q_len > 1:
-            raise ValueError("a verification step (q_len > 1) runs op by op or under a CUDA graph, not as a decode program")
-        if self.W > 1:
-            raise ValueError("a beam-search step runs op by op or under a CUDA graph, not as a decode program (its fork is "
-                             "torch index ops, not C-ABI calls)")
-        if self.samp is not None:
-            raise ValueError("a sampling step runs op by op or under a CUDA graph, not as a decode program (its uniforms and "
-                             "state updates are torch ops, not C-ABI calls)")
-        if self.shared_prefix is not None:
-            raise ValueError("a shared-prefix step runs op by op or under a CUDA graph, not as a decode program")
+        mode, why = (("a verification step (q_len > 1)", "") if self.q_len > 1
+                     else ("a beam-search step", " (its fork is torch index ops, not C-ABI calls)") if self.W > 1
+                     else ("a sampling step", " (its uniforms and state updates are torch ops, not C-ABI calls)")
+                     if self.samp is not None
+                     else ("a shared-prefix step", "") if self.shared_prefix is not None else (None, ""))
+        if mode is not None:    # the ending or the attention of these modes is not C-ABI calls only
+            raise ValueError(f"{mode} runs op by op or under a CUDA graph, not as a decode program{why}")
         self.prog = ops.Program()
         with self.prog.record():
             self.step_core()
@@ -994,7 +992,7 @@ class DecodeStep:
 
     def run(self):
         """One decode step through the program if one was built, else op by op."""
-        if getattr(self, "prog", None) is not None:
+        if self.prog is not None:
             self.prog.launch()
             self.step_tail()
         else:
@@ -1011,19 +1009,19 @@ class DecodeStep:
         with torch.cuda.stream(s):
             for _ in range(2):
                 self.run()
-                if self.W > 1 or self.samp is not None:   # the state / the draw counter advance: every warm-up starts from the prompt
+                if self.advances or self.redraws:   # the state moves on: every warm-up starts from the prompt
                     self.upload_inputs()
         torch.cuda.current_stream(self.dev).wait_stream(s)
         torch.cuda.synchronize(self.dev)
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
             self.run()
-        if self.W > 1 or self.samp is not None:
+        if self.advances or self.redraws:
             self.upload_inputs()            # the recorded step has not run: the first replay is step 1
         torch.cuda.synchronize(self.dev)
 
     def replay(self):
-        self._count_beam_step()
+        self._count_new_token()
         self.graph.replay()
 
     # ------------------------------------------------------------------ accounting (SURVEY 8d)

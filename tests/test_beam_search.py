@@ -102,15 +102,15 @@ def test_beam_steps_past_max_new_tokens_are_refused():
     """The page-table rows end max_new_tokens steps after the prompt: one more step raises before it launches anything."""
     from rtp_llm_b200.decode_step import DecodeStep
     step = DecodeStep.__new__(DecodeStep)
-    step.W, step.max_new_tokens, step.beam_steps = 4, 2, 0
-    step._count_beam_step()
-    step._count_beam_step()
+    step.advances, step.max_new_tokens, step.new_tokens = True, 2, 0
+    step._count_new_token()
+    step._count_new_token()
     with pytest.raises(ValueError, match="max_new_tokens 2"):
-        step._count_beam_step()
+        step._count_new_token()
     with pytest.raises(ValueError, match="max_new_tokens 2"):
         step.replay()                                              # the graph path counts too, before it replays
-    step.W, step.beam_steps = 1, 5                                 # the greedy step is never limited
-    step._count_beam_step()
+    step.advances, step.new_tokens = False, 5                      # the greedy step is never limited
+    step._count_new_token()
 
 
 def test_decode_step_beam_mode_is_not_a_program():

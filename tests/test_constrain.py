@@ -205,6 +205,7 @@ def _host_step(R=3, V=100, cap=4, mask=True):
     """A DecodeStep's constraint state with host tensors standing in for the device buffers."""
     s = DecodeStep.__new__(DecodeStep)
     s.B, s.q_len, s.vocab = R, 1, V
+    s.bitmask_h = s.bitmask = s.bias_h = s.bias = None
     if mask:
         s.bitmask_h = torch.full((R, (V + 31) // 32), -1, dtype=torch.int32)
         s.bitmask = torch.zeros_like(s.bitmask_h)

@@ -99,7 +99,7 @@ def _state(m) -> dict:
               "seq_lens"):
         if isinstance(getattr(m, k, None), torch.Tensor):
             s[k] = getattr(m, k)
-    if m.W > 1 or m.sample_advances:   # the token history up to each row's length (the rest of the buffer is never written)
+    if m.advances:                     # the token history up to each row's length (the rest of the buffer is never written)
         live = torch.arange(m.hist.shape[1], device=m.hist.device).view(1, -1) < m.hist_len.view(-1, 1)
         s["hist"] = torch.where(live, m.hist, torch.zeros_like(m.hist))
     for group in ("beam_out", "lp_out"):

@@ -160,11 +160,11 @@ def test_ban_without_beam_or_sampling_still_raises():
 
 def test_sampled_steps_past_max_new_tokens_are_refused():
     step = DecodeStep.__new__(DecodeStep)
-    step.W, step.sample_advances, step.max_new_tokens, step.beam_steps = 1, True, 2, 0
-    step._count_beam_step()
-    step._count_beam_step()
+    step.advances, step.max_new_tokens, step.new_tokens = True, 2, 0
+    step._count_new_token()
+    step._count_new_token()
     with pytest.raises(ValueError, match="max_new_tokens 2"):
-        step._count_beam_step()
+        step._count_new_token()
     with pytest.raises(ValueError, match="max_new_tokens 2"):
         step.replay()
 

@@ -58,7 +58,7 @@ class Arm:
 def step_arm(name: str, model: DecodeStep) -> Arm:
     launches = model.launches_per_step()    # one eager step; capture() then restarts an advancing step from its prompt
     model.capture()
-    return Arm(name, model.replay, launches, (model,) if model.W > 1 or model.sample_advances else ())
+    return Arm(name, model.replay, launches, (model,) if model.advances else ())
 
 
 def max_new_tokens(a) -> int:
