@@ -351,6 +351,28 @@ int b200_spec_verify_tree(const float* target_probs, const int32_t* target_ids, 
                           const float* uniform, int batch, int n, int vocab, int32_t* out_tokens, int32_t* accepted,
                           int32_t* accepted_path, void* stream);
 
+/* Sampled verification of a speculative token tree whose drafts were sampled from draft distributions: SpecInfer's multi-step
+ * speculative sampling (recursive rejection; also EAGLE-2/3's sampled trees), the tree form of the reference's chain kernel
+ * (rtp_llm/models_py/bindings/cuda/kernels/speculative_sampling/sampling.cu). The tree form is not in the reference: its
+ * semantics are restated here and parity with another implementation is unpinned. Emits tokens distributed as the target.
+ *   target_probs [batch][n][vocab] fp32 as for b200_spec_verify_tree; draft_probs [batch][n][vocab] fp32, row c the distribution
+ *   node c's token was drawn from given its parent (for siblings drawn without replacement: conditioned on the earlier
+ *   siblings); row 0 is not read. tree_parents, node_tokens, uniform [batch][n] as for b200_spec_verify_tree; 2 <= n <= 64.
+ * At the node cur, start from R = t = target_probs[cur] and Z = 1, and try cur's children c in index order, x = node_tokens[c],
+ * p = draft_probs[c]: accept c iff uniform[c - 1] * p(x) * Z < R(x) in fp32 (a token outside [0, vocab) has R(x) = 0 and is
+ * rejected). On a rejection R = max(0, R - Z * p) elementwise, whatever the token, then Z = sum R in fp32 in a fixed order
+ * (deterministic). With every child rejected the token is drawn from R (from t when R has no mass), at a leaf the bonus token
+ * from t, with uniform[n - 1] as b200_spec_verify draws. out_tokens, accepted, accepted_path as for b200_spec_verify_tree
+ * (b200_kv_compact_path takes them). On a chain this is b200_spec_verify with draft_probs, bit for bit.
+ * workspace: b200_spec_verify_tree_draft_workspace_bytes(batch, vocab) bytes (R, [batch][vocab] fp32), no initial contents.
+ * One CTA per sequence; each rejection is one pass over the vocabulary (read R or t and p, write R). Under PDL it waits before
+ * reading. */
+size_t b200_spec_verify_tree_draft_workspace_bytes(int batch, int vocab);
+int b200_spec_verify_tree_draft(const float* target_probs, const float* draft_probs, const int32_t* tree_parents,
+                                const int32_t* node_tokens, const float* uniform, int batch, int n, int vocab, void* workspace,
+                                size_t workspace_bytes, int32_t* out_tokens, int32_t* accepted, int32_t* accepted_path,
+                                void* stream);
+
 /* After b200_spec_verify_tree: the accepted path's K/V moved to consecutive cache slots. For d = 1 .. accepted[b] with
  * path[d] != d (path = accepted_path [batch][n]), the K and V of slot sequence_lengths[b] + path[d] are bit-copied to slot
  * sequence_lengths[b] + d in every layer and kv head; no other slot is written. Copies go in increasing d, each read before any

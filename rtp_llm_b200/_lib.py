@@ -60,6 +60,8 @@ SIGNATURES = {
     "b200_sample": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int] + [c_void_p] * 14),
     "b200_spec_verify": (c_int, [c_void_p] * 5 + [c_int] * 3 + [c_void_p] * 3),
     "b200_spec_verify_tree": (c_int, [c_void_p] * 5 + [c_int] * 3 + [c_void_p] * 4),
+    "b200_spec_verify_tree_draft_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "b200_spec_verify_tree_draft": (c_int, [c_void_p] * 5 + [c_int] * 3 + [c_void_p, c_size_t] + [c_void_p] * 4),
     "b200_kv_compact_path": (c_int, [c_void_p] + [c_int] * 4 + [c_void_p, c_int] + [c_void_p] * 3 + [c_int, c_int, c_void_p]),
     "b200_beam_search_step_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "b200_beam_search_step": (c_int, [c_void_p, c_int, c_void_p] + [c_int] * 4 + [c_void_p] * 7 + [c_size_t, c_void_p]),

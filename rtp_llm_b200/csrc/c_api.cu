@@ -1079,7 +1079,7 @@ static int spec_verify_launch(const float* target_probs, const int32_t* target_i
                               int32_t* accepted, int32_t* accepted_path, int batch, int num_nodes, int vocab, void* stream) {
     const SpecVerifyParams p{target_probs, target_ids, draft_probs, draft_tokens, parents, uniform,
                              out_tokens,   accepted,   accepted_path, num_nodes, vocab};
-    return launch_op("spec_verify_kernel", stream, spec_verify_kernel, {dim3(batch), dim3(kSampleThreads)}, p);
+    return launch_op("spec_verify_kernel", stream, spec_verify_kernel<false>, {dim3(batch), dim3(kSampleThreads)}, p);
 }
 
 int b200_spec_verify(const float* target_probs, const int32_t* target_ids, const float* draft_probs, const int32_t* draft_tokens,
@@ -1108,6 +1108,30 @@ int b200_spec_verify_tree(const float* target_probs, const int32_t* target_ids, 
     ARG_CHECK(!target_probs || uniform, "spec_verify_tree: sampling mode needs uniform");
     return spec_verify_launch(target_probs, target_ids, nullptr, node_tokens, tree_parents, uniform, out_tokens, accepted,
                               accepted_path, batch, n, vocab, stream);
+}
+
+size_t b200_spec_verify_tree_draft_workspace_bytes(int batch, int vocab) {
+    return batch > 0 && vocab > 0 ? (size_t)batch * vocab * sizeof(float) : 0;
+}
+
+int b200_spec_verify_tree_draft(const float* target_probs, const float* draft_probs, const int32_t* tree_parents,
+                                const int32_t* node_tokens, const float* uniform, int batch, int n, int vocab, void* workspace,
+                                size_t workspace_bytes, int32_t* out_tokens, int32_t* accepted, int32_t* accepted_path,
+                                void* stream) {
+    ARG_CHECK(batch >= 0 && batch <= 65535, "spec_verify_tree_draft: batch %d unsupported (0..65535)", batch);
+    ARG_CHECK(n >= 2 && n <= kSpecTreeMaxNodes, "spec_verify_tree_draft: n %d unsupported (2..%d)", n, kSpecTreeMaxNodes);
+    ARG_CHECK(vocab > 0, "spec_verify_tree_draft: vocab must be positive");
+    if (batch == 0) return B200_OK;
+    ARG_CHECK(target_probs && draft_probs && tree_parents && node_tokens && uniform && out_tokens && accepted && accepted_path,
+              "spec_verify_tree_draft: null pointer");
+    const size_t need = b200_spec_verify_tree_draft_workspace_bytes(batch, vocab);
+    ARG_CHECK(workspace && workspace_bytes >= need,
+              "spec_verify_tree_draft: workspace too small (%zu < %zu bytes, see b200_spec_verify_tree_draft_workspace_bytes)",
+              workspace ? workspace_bytes : (size_t)0, need);
+    const SpecVerifyTreeDraftParams p{{target_probs, nullptr, draft_probs, node_tokens, tree_parents, uniform, out_tokens, accepted,
+                                       accepted_path, n, vocab},
+                                      static_cast<float*>(workspace)};
+    return launch_op("spec_verify_kernel", stream, spec_verify_kernel<true>, {dim3(batch), dim3(kSampleThreads)}, p);
 }
 
 int b200_kv_compact_path(void* const* kv_pools, int layers, int kv_head_num, int head_dim, int page_size, const int32_t* page_list,

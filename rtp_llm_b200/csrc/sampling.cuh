@@ -22,6 +22,8 @@
 // beyond the chunk's own sum, takes the chunk's last kept token with p > 0. Token -1 (token_prob 0) only when the row has no
 // positive finite mass, i.e. NaN logits. Under PDL the kernel waits for its predecessor before it reads anything.
 #pragma once
+#include <type_traits>
+
 #include "ptx.cuh"
 
 namespace b200 {
@@ -255,6 +257,13 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(const SamplePara
 // deterministic drafts, from q itself when the residual has no mass -- and at a leaf the bonus token from the leaf's row; both
 // draws use uniform[N - 1] and chunked_draw. One CTA of 1024 threads per sequence; every thread walks the same tree (the same
 // loads, the same fp32 compares), so the decisions are uniform.
+// The draft-tree instance (kDraftTree, b200_spec_verify_tree_draft) runs SpecInfer's multi-step speculative sampling with draft
+// rows draft_probs [B][N][V] (row c: the distribution node c's token was drawn from). At the node cur, with R = t (its target
+// row) and Z = 1, child c with token x is accepted iff uniform[c - 1] * p_c(x) * Z < R(x) in fp32 (each product rounded, no
+// FMA); on a rejection R = max(0, R - Z * p_c) elementwise (again product and difference rounded apart) and Z = sum R, one
+// pass over the vocabulary (spec_residual_pass) into the caller's [B][V] workspace. With every child rejected the token is
+// drawn from R (from t when it has no mass), at a leaf from t. On a chain Z is 1 at every test and the rule is the chain's
+// draft_probs rule bit for bit.
 constexpr int kSpecTreeMaxNodes = 64;
 struct SpecVerifyParams {
     const float* target_probs;    // optional [B][N][V]
@@ -268,15 +277,60 @@ struct SpecVerifyParams {
     int32_t* accepted_path;       // optional [B][N]: the node at depth 0 .. accepted, then -1
     int num_nodes, vocab;
 };
+// The draft-tree instance's parameters: draft_probs is [B][N][V] there, parents and target_probs are set, target_ids is unread
+struct SpecVerifyTreeDraftParams : SpecVerifyParams {
+    float* residual;              // [B][V] workspace: the residual R of the node the walk stands on, written before it is read
+};
+template <bool kDraftTree>
+using SpecVerifyParamsOf = typename std::conditional<kDraftTree, SpecVerifyTreeDraftParams, SpecVerifyParams>::type;
 
-__global__ void __launch_bounds__(kSampleThreads) spec_verify_kernel(const SpecVerifyParams p) {
+// One rejection of the draft-tree walk: R = max(0, src - Z * p) over [0, V) (src: the target row at the node's first rejection,
+// R itself after it), returns the new Z = sum R, identical in every thread. Thread tid owns the 4-element groups g = tid + k *
+// 1024 and adds their elements in index order; block_reduce_sum adds the threads' sums in its fixed order, so Z is
+// deterministic (tests/draft_tree_oracle.py restates that order). float4 loads and stores when every row is 16-byte aligned.
+__device__ __forceinline__ float spec_residual_pass(const float* src, const float* dp, float* R, float Z, int V, bool vec,
+                                                    float* s_red) {
+    __syncthreads();                   // every thread has read R for its accept test before any thread rewrites it
+    const int G = (V + 3) >> 2;
+    float part = 0.f;
+    for (int g = threadIdx.x; g < G; g += kSampleThreads) {
+        float s[4], q[4], r[4];
+        if (vec) {
+            const float4 a = reinterpret_cast<const float4*>(src)[g], d = reinterpret_cast<const float4*>(dp)[g];
+            s[0] = a.x, s[1] = a.y, s[2] = a.z, s[3] = a.w;
+            q[0] = d.x, q[1] = d.y, q[2] = d.z, q[3] = d.w;
+        } else {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const int i = 4 * g + j;
+                s[j] = i < V ? src[i] : 0.f;
+                q[j] = i < V ? dp[i] : 0.f;
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < 4; ++j) r[j] = fmaxf(0.f, __fsub_rn(s[j], __fmul_rn(Z, q[j])));
+        if (vec) {
+            reinterpret_cast<float4*>(R)[g] = make_float4(r[0], r[1], r[2], r[3]);
+        } else {
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+                if (4 * g + j < V) R[4 * g + j] = r[j];
+        }
+#pragma unroll
+        for (int j = 0; j < 4; ++j) part = __fadd_rn(part, r[j]);
+    }
+    return block_reduce_sum(part, s_red);
+}
+
+template <bool kDraftTree>
+__global__ void __launch_bounds__(kSampleThreads) spec_verify_kernel(const SpecVerifyParamsOf<kDraftTree> p) {
     __shared__ float s_scan[kSampleThreads];
     __shared__ int s_pick, s_owner;
     __shared__ int s_path[kSpecTreeMaxNodes];   // tree: the accepted path (a chain's is the identity)
     __shared__ int s_rej[kSpecTreeMaxNodes];    // the rejected children's tokens at the node the walk stopped at
     const int b = blockIdx.x, tid = threadIdx.x, N = p.num_nodes, V = p.vocab;
     pdl_wait();                        // under PDL the target rows come from the kernels before this one
-    const bool tree = p.parents != nullptr;
+    const bool tree = kDraftTree || p.parents != nullptr;
     const int32_t* par = tree ? p.parents + (size_t)b * N : nullptr;
     const int32_t* ntok = p.draft_tokens + (size_t)b * (tree ? N : N - 1);
     auto token = [&](int c) { return tree ? ntok[c] : ntok[c - 1]; };
@@ -290,7 +344,45 @@ __global__ void __launch_bounds__(kSampleThreads) spec_verify_kernel(const SpecV
         ++acc;
         if (tid == 0 && tree) s_path[acc] = c;
     };
-    if (!p.target_probs) {
+    if constexpr (kDraftTree) {
+        __shared__ float s_red[kSampleThreads / 32];
+        const float* u = p.uniform + (size_t)b * N;
+        auto trow = [&](int i) { return p.target_probs + ((size_t)b * N + i) * V; };
+        auto drow = [&](int i) { return p.draft_probs + ((size_t)b * N + i) * V; };
+        float* R = p.residual + (size_t)b * V;
+        const bool vec = (V & 3) == 0 && ((reinterpret_cast<uintptr_t>(p.target_probs) | reinterpret_cast<uintptr_t>(p.draft_probs) |
+                                           reinterpret_cast<uintptr_t>(p.residual)) & 15) == 0;
+        int nrej = 0;                  // at the node the walk stands on: its rejected children (R is its residual when > 0)
+        for (bool moved = true; moved;) {
+            moved = false;
+            const float* t = trow(cur);
+            float Z = 1.f;
+            nrej = 0;
+            for (int c = cur + 1; c < N; ++c) {
+                if (par[c] != cur) continue;
+                const int x = ntok[c];
+                const bool in = x >= 0 && x < V;
+                const float r = in ? (nrej ? R[x] : t[x]) : 0.f;
+                const float px = in ? drow(c)[x] : 0.f;
+                if (__fmul_rn(__fmul_rn(u[c - 1], px), Z) < r) {
+                    step(c);
+                    moved = true;
+                    break;
+                }
+                Z = spec_residual_pass(nrej ? R : t, drow(c), R, Z, V, vec, s_red);
+                ++nrej;
+            }
+        }
+        float total;
+        const float* t = trow(cur);
+        tok = -1;
+        if (nrej) tok = chunked_draw([&](int x) { return R[x]; }, V, u[N - 1], false, s_scan, &s_pick, &s_owner, &total);
+        if (!nrej || !(total > 0.f)) {   // a leaf, or a residual without mass: draw from t
+            if (nrej) __syncthreads();     // every thread has read the first draw's shared result
+            tok = chunked_draw([&](int x) { return t[x] > 0.f ? t[x] : 0.f; }, V, u[N - 1], false, s_scan, &s_pick, &s_owner,
+                               &total);
+        }
+    } else if (!p.target_probs) {
         const int32_t* ids = p.target_ids + (size_t)b * N;
         for (bool moved = true; moved;) {
             moved = false;

@@ -157,7 +157,7 @@ def _per_request(v, n: int, name: str) -> list:
 
 def _check_options(cfg, batch, ctx, tp_size, act_order, q_len, beam_width, no_repeat_ngram, max_new_tokens, sampling, logprobs,
                    eos_id, length_penalty, early_stopping, token_bitmask, logit_bias_capacity, tree, shared_prefix, max_rows,
-                   advances) -> None:
+                   advances, draft_probs=False) -> None:
     """DecodeStep's option checks, before anything is allocated: ValueError for the first fault, in this order."""
     assert cfg.head_num % tp_size == 0 and cfg.inter % tp_size == 0
     if shared_prefix is not None:
@@ -204,6 +204,9 @@ def _check_options(cfg, batch, ctx, tp_size, act_order, q_len, beam_width, no_re
             raise ValueError(f"logprobs must be in 0..{ops.LOGPROB_MAX_TOP_N} (got {logprobs})")
     elif logprobs is not None:
         raise ValueError("logprobs needs the sampling mode (sampling=SamplingParams(...))")
+    if draft_probs and (sampling is None or q_len < 2):
+        raise ValueError(f"draft_probs needs sampled verification: sampling=SamplingParams(...) and q_len >= 2 (got sampling "
+                         f"{sampling is not None}, q_len {q_len})")
     if advances and not 1 <= max_new_tokens < ctx:
         raise ValueError(f"max_new_tokens must be in 1..ctx-1 (got {max_new_tokens}, ctx {ctx})")
     if no_repeat_ngram != 0 and beam_width == 1 and sampling is None:
@@ -284,6 +287,11 @@ class DecodeStep:
     Like the greedy verification step it does not advance. Penalties and the n-gram ban are rejected there: row j's history
     would have to hold drafts 0..j-1. SamplingParams.min_p runs b200_sample with a min_p buffer when some value is not 0, and
     without one (today's kernel call) when every value is 0.
+    draft_probs=True (sampled verification only: sampling and q_len >= 2, chain or tree) verifies drafts that were sampled from
+    draft distributions, with the drafter's rows in a static fp32 buffer that set_draft_probs() fills between replays (zero
+    until then): [B, q_len - 1, V] for a chain, passed to spec_verify as its draft_probs, and [B, q_len, V] for a tree, passed
+    to b200_spec_verify_tree_draft (recursive rejection) with a residual workspace allocated here. The step's launches are
+    those of the same step without it.
 
     shared_prefix=(n, prefix_tokens) (TP 1, q_len 1, greedy, beam_width 1; op by op or under a CUDA graph, with or without PDL;
     not in a decode program; the fused rope is off): groups of n requests, on rows a seeded permutation scatters over the batch,
@@ -326,12 +334,12 @@ class DecodeStep:
                  length_penalty: Union[float, Sequence[float]] = 1.0,
                  early_stopping: Union[bool, str, Sequence[Union[bool, str]]] = False,
                  token_bitmask: bool = False, logit_bias_capacity: int = 0, tree=None, shared_prefix=None,
-                 max_rows: int = TP_MAX_ROWS):
+                 max_rows: int = TP_MAX_ROWS, draft_probs: bool = False):
         self.advances = beam_width > 1 or (sampling is not None and q_len == 1)   # tokens join the history, lengths grow
         self.redraws = sampling is not None     # every run moves the draw counter on, at any q_len, advancing or not
         _check_options(cfg, batch, ctx, tp_size, act_order, q_len, beam_width, no_repeat_ngram, max_new_tokens, sampling,
                        logprobs, eos_id, length_penalty, early_stopping, token_bitmask, logit_bias_capacity, tree, shared_prefix,
-                       max_rows, self.advances)
+                       max_rows, self.advances, draft_probs)
         self.shared_prefix, self.samp, self.logprobs, self.eos_id = shared_prefix, sampling, logprobs, eos_id
         self.W, self.ngram, self.max_new_tokens = beam_width, no_repeat_ngram, max_new_tokens
         self.new_tokens = 0                             # steps the step has advanced since the prompt (upload_inputs)
@@ -581,6 +589,7 @@ class DecodeStep:
                 self.length_penalty = torch.tensor([float(a) for a in lp], dtype=torch.float32, device=device)
                 self.early_stopping = torch.tensor([2 if m == "never" else int(bool(m)) for m in es], dtype=torch.int32,
                                                    device=device)
+        self.draft_probs = None
         if sampling is not None:
             def per_row(v, dt):
                 return torch.tensor(_per_request(v, batch, "sampling"), dtype=dt).repeat_interleave(q_len).to(device)
@@ -603,6 +612,10 @@ class DecodeStep:
                 self.cum_log_probs = buf(R, dt=torch.float32)
             else:
                 self.target_probs = buf(batch, q_len, self.vocab, dt=torch.float32)
+            if draft_probs:     # the drafter's rows (set_draft_probs), and the tree verifier's residual workspace
+                self.draft_probs = torch.zeros(batch, q_len if tree is not None else q_len - 1, self.vocab, dtype=torch.float32,
+                                               device=device)
+                self.draft_ws = ops.spec_verify_tree_draft_workspace(batch, self.vocab, device) if tree is not None else None
             if logprobs is not None:
                 self.lp_out = dict(token_logprob=buf(R, dt=torch.float32), top_ids=buf(R, logprobs, dt=torch.int32),
                                    top_logprobs=buf(R, logprobs, dt=torch.float32))
@@ -729,6 +742,18 @@ class DecodeStep:
         self.tree_depth_h.copy_(torch.tensor(depth, dtype=torch.int32))
         self.tree_parents.copy_(self.tree_parents_h, non_blocking=True)
         self.tree_depth.copy_(self.tree_depth_h, non_blocking=True)
+
+    def set_draft_probs(self, rows) -> None:
+        """The draft distributions the next step (or graph replay) verifies with, copied non_blocking into the static buffer:
+        fp32 [B, q_len - 1, V] for a chain (row i: the distribution draft i was drawn from), [B, q_len, V] for a tree (row j: the
+        distribution node j's token was drawn from; row 0 is not read); a CUDA or host tensor. Like set_constraints(), call it
+        between two replays."""
+        if self.draft_probs is None:
+            raise ValueError("set_draft_probs: this step was built without draft_probs=True")
+        t = torch.as_tensor(rows)
+        if t.dtype != torch.float32 or tuple(t.shape) != tuple(self.draft_probs.shape):
+            raise ValueError(f"set_draft_probs: rows must be fp32 {list(self.draft_probs.shape)} (got {t.dtype} {list(t.shape)})")
+        self.draft_probs.copy_(t, non_blocking=True)
 
     def _constrain(self, logits: torch.Tensor):
         """b200_constrain_logits on `logits` with the buffers set_constraints() filled (no launch when the step has none)."""
@@ -944,10 +969,11 @@ class DecodeStep:
             ops.token_logprobs(self.logits, self.logprobs, tokens=self.next_ids, workspace=self.lp_ws, out=self.lp_out)
         if not self.advances:
             if self.tree_parents is not None:
-                self._verify_tree(target_probs=self.target_probs, uniform=self.uniform[R:])
+                draft = dict(draft_probs=self.draft_probs, workspace=self.draft_ws) if self.draft_probs is not None else {}
+                self._verify_tree(target_probs=self.target_probs, uniform=self.uniform[R:], **draft)
             else:
-                ops.spec_verify(self.drafts, target_probs=self.target_probs, uniform=self.uniform[R:], out_tokens=self.out_tokens,
-                                accepted=self.accepted)
+                ops.spec_verify(self.drafts, target_probs=self.target_probs, draft_probs=self.draft_probs, uniform=self.uniform[R:],
+                                out_tokens=self.out_tokens, accepted=self.accepted)
             return
         torch.log(self.token_prob, out=self.log_prob)
         self.cum_log_probs.add_(self.log_prob)

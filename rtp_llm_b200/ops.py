@@ -702,16 +702,28 @@ def spec_verify(draft_tokens: torch.Tensor, *, target_probs: Optional[torch.Tens
     return out["out_tokens"], out["accepted"]
 
 
+def spec_verify_tree_draft_workspace(batch: int, vocab: int, device) -> torch.Tensor:
+    """Workspace of b200_spec_verify_tree_draft (the residual rows; no initial contents needed)."""
+    n = int(_lib.load().b200_spec_verify_tree_draft_workspace_bytes(batch, vocab))
+    return torch.empty(max(n, 16), dtype=torch.uint8, device=device)
+
+
 def spec_verify_tree(tree_parents: torch.Tensor, node_tokens: torch.Tensor, *, target_probs: Optional[torch.Tensor] = None,
                      target_ids: Optional[torch.Tensor] = None, uniform: Optional[torch.Tensor] = None,
                      out_tokens: Optional[torch.Tensor] = None, accepted: Optional[torch.Tensor] = None,
-                     accepted_path: Optional[torch.Tensor] = None):
+                     accepted_path: Optional[torch.Tensor] = None, draft_probs: Optional[torch.Tensor] = None,
+                     workspace: Optional[torch.Tensor] = None):
     """Verify a speculative token tree of n = tree_parents.shape[1] <= 64 nodes per sequence (b200_spec_verify_tree).
     tree_parents, node_tokens int32 [B, n] (node 0 the root; its token is not read). Greedy: target_ids int32 [B, n]. Sampling
-    (deterministic drafts): target_probs fp32 [B, n, V], uniform fp32 [B, n]. Returns (out_tokens int32 [B, n]: the accepted
-    path's tokens, then one correction or bonus token, then -1; accepted int32 [B]; accepted_path int32 [B, n]: the node at depth
-    0 .. accepted, then -1)."""
-    _cuda_contig(tree_parents, node_tokens, target_probs, target_ids, uniform, out_tokens, accepted, accepted_path)
+    (deterministic drafts): target_probs fp32 [B, n, V], uniform fp32 [B, n]. Sampling with draft_probs fp32 [B, n, V] (row c:
+    the distribution node c's token was drawn from; n >= 2): recursive rejection (b200_spec_verify_tree_draft), in `workspace`
+    (spec_verify_tree_draft_workspace; allocated when not given). Returns (out_tokens int32 [B, n]: the accepted path's tokens,
+    then one correction or bonus token, then -1; accepted int32 [B]; accepted_path int32 [B, n]: the node at depth 0 ..
+    accepted, then -1)."""
+    if draft_probs is not None and target_probs is None:
+        raise B200Error("spec_verify_tree: draft_probs need the sampling mode (target_probs)")
+    _cuda_contig(tree_parents, node_tokens, target_probs, target_ids, uniform, out_tokens, accepted, accepted_path, draft_probs,
+                 workspace)
     if tree_parents.dim() != 2:
         raise B200Error("spec_verify_tree: tree_parents must be [B, n]")
     B, n = tree_parents.shape
@@ -727,9 +739,22 @@ def spec_verify_tree(tree_parents: torch.Tensor, node_tokens: torch.Tensor, *, t
     else:
         _need("spec_verify_tree", "target_ids", target_ids, torch.int32, (B, n))
         V = 1                                   # the vocabulary is not read in greedy mode
+    if draft_probs is not None:
+        _need("spec_verify_tree", "draft_probs", draft_probs, torch.float32, (B, n, V))
+        need = int(_lib.load().b200_spec_verify_tree_draft_workspace_bytes(B, V))
+        if workspace is None:
+            workspace = spec_verify_tree_draft_workspace(B, V, tree_parents.device)
+        elif workspace.dtype != torch.uint8 or workspace.numel() < need:
+            raise B200Error(f"spec_verify_tree: workspace must be uint8 of at least {need} bytes (spec_verify_tree_draft_workspace)")
     out = _outputs("spec_verify_tree", dict(out_tokens=out_tokens, accepted=accepted, accepted_path=accepted_path),
                    tree_parents.device, out_tokens=(torch.int32, (B, n)), accepted=(torch.int32, (B,)),
                    accepted_path=(torch.int32, (B, n)))
+    if draft_probs is not None:
+        check(_lib.load().b200_spec_verify_tree_draft(_p(target_probs), _p(draft_probs), _p(tree_parents), _p(node_tokens), _p(uniform),
+                                                      B, n, V, _p(workspace), workspace.numel(), _p(out["out_tokens"]),
+                                                      _p(out["accepted"]), _p(out["accepted_path"]), _stream()),
+              "b200_spec_verify_tree_draft")
+        return out["out_tokens"], out["accepted"], out["accepted_path"]
     check(_lib.load().b200_spec_verify_tree(_p(target_probs), _p(target_ids), _p(tree_parents), _p(node_tokens), _p(uniform), B, n, V,
                                             _p(out["out_tokens"]), _p(out["accepted"]), _p(out["accepted_path"]), _stream()),
           "b200_spec_verify_tree")

@@ -132,6 +132,49 @@ def bench_tree_verify(B, n, sampling, V=128256, nrot=4):
     return us
 
 
+def bench_tree_verify_draft(B, n, rejects, V=128256, nrot=4, runs=3):
+    """b200_spec_verify_tree_draft against b200_spec_verify_tree (deterministic drafts) on the same binary trees, target rows and
+    node tokens, the arms alternating; medians of `runs`. Every target row is a temperature-0.25 softmax with no mass on token
+    0. The draft rows force the decisions at each node the walk reaches: rejects "0" (first child token 1, its row without mass:
+    accepted), "1" (first child token 0: rejected, then the second child as in "0": accepted) or "all" (every child token 0:
+    the root's children rejected). A rejected child's row is a dense softmax, so each rejection is one full pass."""
+    par = torch.tensor([[-1] + [(j - 1) // 2 for j in range(1, n)]] * B, dtype=torch.int32, device=dev)
+    first = torch.tensor([j % 2 == 1 for j in range(n)], device=dev)       # node j is its parent's first child when j is odd
+    tok = torch.ones(B, n, dtype=torch.int32, device=dev)
+    if rejects == "1":
+        tok[:, first] = 0
+    elif rejects == "all":
+        tok.zero_()
+    probs, drafts = [], []
+    for _ in range(nrot):
+        t = torch.softmax(torch.randn(B, n, V, device=dev) / 0.25, dim=-1)
+        t[..., 0] = 0.0
+        probs.append(t)
+        d = torch.softmax(torch.randn(B, n, V, device=dev) / 0.25, dim=-1)
+        d[..., 1] = 0.0
+        d[tok == 1] = 0.0
+        drafts.append(d)
+    u = torch.rand(B, n, device=dev)
+    ws = ops.spec_verify_tree_draft_workspace(B, V, dev)
+    out = dict(out_tokens=torch.empty(B, n, dtype=torch.int32, device=dev), accepted=torch.empty(B, dtype=torch.int32, device=dev),
+               accepted_path=torch.empty(B, n, dtype=torch.int32, device=dev))
+    arms = {"deterministic": lambda i: ops.spec_verify_tree(par, tok, target_probs=probs[i], uniform=u, **out),
+            "draft rows": lambda i: ops.spec_verify_tree(par, tok, target_probs=probs[i], uniform=u, draft_probs=drafts[i],
+                                                         workspace=ws, **out)}
+    arms["draft rows"](0)
+    torch.cuda.synchronize()
+    acc = out["accepted"].float().mean().item()
+    t = {k: [] for k in arms}
+    for _ in range(runs):
+        for k, fn in arms.items():
+            t[k].append(timeit(fn, nrot))
+    med = {k: sorted(v)[len(v) // 2] for k, v in t.items()}
+    print(f"tree-verify-draft B{B} n{n} binary, {rejects} rejected per node, accepted {acc:.2f} (draft rows) median: "
+          f"deterministic {med['deterministic']:.1f} us, draft rows {med['draft rows']:.1f} us "
+          f"({med['draft rows'] - med['deterministic']:+.1f} us)", flush=True)
+    return med
+
+
 def bench_kv_compact(B, layers=32, Hkv=8, T=64, n=8, S=2048, nrot=2):
     """b200_kv_compact_path over the Llama-3-8B cache (32 layers, Hkv 8, D 128) with a path that moves every depth."""
     M = math.ceil((S + n) / T)
@@ -530,7 +573,7 @@ if __name__ == "__main__":
         # speculative-token verification at group 8 (Qwen2-72B / Llama-3-70B): 8, 16, 32, 64 query rows per kv head
         t = {n: bench_attn_multi(32, 64, 8, 2048, n) for n in (1, 2, 4, 8)}
         print("attn-multi time relative to q_len 2 (16 rows): " + ", ".join(f"q_len {n}: {t[n] / t[2]:.2f}x" for n in t), flush=True)
-    if "attn-tree" in which or "tree-verify" in which or "kv-compact" in which:
+    if "attn-tree" in which or "tree-verify" in which or "kv-compact" in which or "tree-verify-draft" in which:
         import subprocess
         print("tree benches on " + (subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader",
                                                     "-i", "0"], capture_output=True, text=True).stdout.strip() or "unknown card")
@@ -545,6 +588,11 @@ if __name__ == "__main__":
             for n in (4, 8, 16):
                 for sampling in (False, True):
                     bench_tree_verify(B, n, sampling)
+    if "tree-verify-draft" in which:
+        for B in (8, 32):
+            for n in (4, 8, 16):
+                for rejects in ("0", "1", "all"):
+                    bench_tree_verify_draft(B, n, rejects)
     if "kv-compact" in which:
         for B in (8, 32):
             bench_kv_compact(B)

@@ -12,7 +12,10 @@ each a step captured in a CUDA graph with PDL at --ctx tokens; the first arm is 
              log-prob and the top 5)
   qwen3      Qwen3-8B INT4: qk_rmsnorm, then the plain rope launch (TwoLaunchStep), against the fused QK-norm append
   tree       Llama-3-8B INT4: per q_len 4 and 8 with batch * q_len <= 128, the chain verification step, then the token-tree
-             step on a binary tree of q_len nodes (tree attention, spec_verify_tree and the K/V compaction)
+             step on a binary tree of q_len nodes (tree attention, spec_verify_tree and the K/V compaction); with
+             --draft-probs instead the sampled tree step (temperature 0.8, top-k 50, top-p 0.9) without and with draft rows
+             (draft_probs=True: b200_spec_verify_tree_draft; rows of dense random softmaxes, so the root's children are
+             rejected and each rejection is a pass over the vocabulary)
   prefix     Llama-3-8B INT4: the shared-prefix step (1024 prompt tokens shared by groups of 8 requests) with
              b200_paged_decode_attn on every row, then with b200_paged_decode_attn_prefix for groups of 8 and of 32
              (PrefixStep forces the kernel either way); prints which kernel attention.prefix_rows_fit picks
@@ -167,6 +170,15 @@ def tree_arms(a, cfg, B, dev):
     for n in (4, 8):
         if B * n <= 128:
             binary = [-1] + [(j - 1) // 2 for j in range(1, n)]
+            if a.draft_probs:
+                sp = SamplingParams(temperature=0.8, top_k=50, top_p=0.9, seed=1)
+                kw = dict(pdl=True, q_len=n, tree=binary, sampling=sp)
+                arms.append(step_arm(f"tree q_len {n} sampled", DecodeStep(cfg, B, a.ctx, dev, **kw)))
+                model = DecodeStep(cfg, B, a.ctx, dev, draft_probs=True, **kw)
+                g = torch.Generator(device=dev).manual_seed(n)
+                model.set_draft_probs(torch.softmax(torch.randn(B, n, model.vocab, generator=g, device=dev), -1))
+                arms.append(step_arm(f"tree q_len {n} sampled + draft rows", model))
+                continue
             arms.append(step_arm(f"chain q_len {n}", DecodeStep(cfg, B, a.ctx, dev, pdl=True, q_len=n)))
             arms.append(step_arm(f"tree q_len {n}", DecodeStep(cfg, B, a.ctx, dev, pdl=True, q_len=n, tree=binary)))
     return arms
@@ -197,6 +209,8 @@ def parse(argv=None):
         p.add_argument("--out", help="write the results as JSON to this file")
         if name == "spec":
             p.add_argument("--model", choices=sorted(MODELS), default="llama3")
+        if name == "tree":
+            p.add_argument("--draft-probs", action="store_true", help="the sampled tree step without and with draft rows")
         if name == "beam":
             p.add_argument("--beam-width", type=int, default=4)
             p.add_argument("--ngram", type=int, default=0, help="no-repeat-ngram size of the beam step (default 0: off)")
@@ -243,6 +257,8 @@ def main(argv=None):
                model=a.cfg.name, ctx=a.ctx, runs=a.runs, iters=a.iters, warmup=a.warmup, batches=[])
     if a.preset == "beam":
         res.update(beam_width=a.beam_width, ngram=a.ngram, eos=a.eos)
+    if a.preset == "tree":
+        res.update(draft_probs=a.draft_probs)
     try:
         for B in a.batch:
             arms = a.arms(a, a.cfg, B, dev)
