@@ -1073,65 +1073,86 @@ int b200_sample(float* logits, int rows, int vocab, const int32_t* history, cons
     return launch_op("sample_kernel", stream, sample_kernel, {dim3(rows), dim3(kSampleThreads)}, p);
 }
 
-// The launch both verification entries share: a chain has no parents and reports no path
-static int spec_verify_launch(const float* target_probs, const int32_t* target_ids, const float* draft_probs,
-                              const int32_t* draft_tokens, const int32_t* parents, const float* uniform, int32_t* out_tokens,
-                              int32_t* accepted, int32_t* accepted_path, int batch, int num_nodes, int vocab, void* stream) {
-    const SpecVerifyParams p{target_probs, target_ids, draft_probs, draft_tokens, parents, uniform,
-                             out_tokens,   accepted,   accepted_path, num_nodes, vocab};
-    return launch_op("spec_verify_kernel", stream, spec_verify_kernel<false>, {dim3(batch), dim3(kSampleThreads)}, p);
+// The three verification entries, one each of the one host path spec_verify_impl
+enum class VerifyEntry { kChain, kTree, kTreeDraft };
+
+// One call of a verification entry. A chain has no parents and reports no path; only the tree with draft rows has a workspace.
+struct VerifyCall {
+    const char* who;   // the entry's name, for messages
+    VerifyEntry entry;
+    const float* target_probs;
+    const int32_t* target_ids;
+    const float* draft_probs;
+    const int32_t* draft_tokens;     // chain: [batch][nodes - 1]; tree: node tokens [batch][nodes]
+    const int32_t* parents;
+    const float* uniform;
+    int batch;
+    long long nodes;                 // a chain's num_draft + 1 (no upper bound), a tree's n
+    int vocab;
+    int32_t *out_tokens, *accepted, *accepted_path;
+    void* workspace;
+    size_t workspace_bytes;
+    void* stream;
+};
+
+size_t b200_spec_verify_tree_draft_workspace_bytes(int batch, int vocab) {
+    return batch > 0 && vocab > 0 ? (size_t)batch * vocab * sizeof(float) : 0;
+}
+
+// The one host path of the three verification entries: their checks, and the kernel instance of the accept rule the inputs
+// select (greedy without target_probs, draft rows with draft_probs, deterministic drafts otherwise).
+static int spec_verify_impl(const VerifyCall& c) {
+    const bool chain = c.entry == VerifyEntry::kChain, tree_draft = c.entry == VerifyEntry::kTreeDraft;
+    ARG_CHECK(c.batch >= 0 && c.batch <= 65535, "%s: batch %d unsupported (0..65535)", c.who, c.batch);
+    ARG_CHECK(!chain || c.nodes >= 1, "%s: num_draft %lld must be >= 0", c.who, c.nodes - 1);
+    const int min_nodes = tree_draft ? 2 : 1;   // the tree's root and at least one draft node to test against it
+    ARG_CHECK(chain || (c.nodes >= min_nodes && c.nodes <= kSpecTreeMaxNodes), "%s: n %lld unsupported (%d..%d)", c.who, c.nodes,
+              min_nodes, kSpecTreeMaxNodes);
+    ARG_CHECK(c.vocab > 0, "%s: vocab must be positive", c.who);
+    if (c.batch == 0) return B200_OK;
+    ARG_CHECK(c.out_tokens && c.accepted && (c.draft_tokens || (chain && c.nodes == 1)) &&
+                  (chain || (c.parents && c.accepted_path)) && (!tree_draft || (c.target_probs && c.draft_probs && c.uniform)),
+              "%s: null pointer", c.who);
+    ARG_CHECK(c.target_probs || c.target_ids, "%s: need target_probs (sampling) or target_ids (greedy)", c.who);
+    ARG_CHECK(!c.target_probs || c.uniform, "%s: sampling mode needs uniform", c.who);
+    ARG_CHECK(!c.draft_probs || c.target_probs, "%s: draft_probs need target_probs", c.who);
+    const size_t need = tree_draft ? b200_spec_verify_tree_draft_workspace_bytes(c.batch, c.vocab) : 0;
+    ARG_CHECK(!tree_draft || (c.workspace && c.workspace_bytes >= need),
+              "%s: workspace too small (%zu < %zu bytes, see b200_spec_verify_tree_draft_workspace_bytes)", c.who,
+              c.workspace ? c.workspace_bytes : (size_t)0, need);
+    const SpecVerifyParams p{c.target_probs, c.target_ids, c.draft_probs, c.draft_tokens, c.parents, c.uniform,
+                             tree_draft ? static_cast<float*>(c.workspace) : nullptr, c.out_tokens, c.accepted, c.accepted_path,
+                             (int)c.nodes, c.vocab};
+    using Kernel = void (*)(SpecVerifyParams);
+    constexpr Kernel instances[2][3] = {   // [chain / tree][greedy / deterministic / draft rows]
+        {spec_verify_kernel<SpecRule::kGreedy, false>, spec_verify_kernel<SpecRule::kDeterministic, false>,
+         spec_verify_kernel<SpecRule::kDraftRows, false>},
+        {spec_verify_kernel<SpecRule::kGreedy, true>, spec_verify_kernel<SpecRule::kDeterministic, true>,
+         spec_verify_kernel<SpecRule::kDraftRows, true>}};
+    const Kernel kern = instances[chain ? 0 : 1][!c.target_probs ? 0 : c.draft_probs ? 2 : 1];
+    return launch_op("spec_verify_kernel", c.stream, kern, {dim3(c.batch), dim3(kSampleThreads)}, p);
 }
 
 int b200_spec_verify(const float* target_probs, const int32_t* target_ids, const float* draft_probs, const int32_t* draft_tokens,
                      const float* uniform, int batch, int num_draft, int vocab, int32_t* out_tokens, int32_t* accepted, void* stream) {
-    ARG_CHECK(batch >= 0 && batch <= 65535, "spec_verify: batch %d unsupported (0..65535)", batch);
-    ARG_CHECK(num_draft >= 0, "spec_verify: num_draft %d must be >= 0", num_draft);
-    ARG_CHECK(vocab > 0, "spec_verify: vocab must be positive");
-    if (batch == 0) return B200_OK;
-    ARG_CHECK(out_tokens && accepted && (draft_tokens || num_draft == 0), "spec_verify: null pointer");
-    ARG_CHECK(target_probs || target_ids, "spec_verify: need target_probs (sampling) or target_ids (greedy)");
-    ARG_CHECK(!target_probs || uniform, "spec_verify: sampling mode needs uniform");
-    ARG_CHECK(!draft_probs || target_probs, "spec_verify: draft_probs need target_probs");
-    return spec_verify_launch(target_probs, target_ids, draft_probs, draft_tokens, nullptr, uniform, out_tokens, accepted, nullptr,
-                              batch, num_draft + 1, vocab, stream);
+    return spec_verify_impl({"spec_verify", VerifyEntry::kChain, target_probs, target_ids, draft_probs, draft_tokens, nullptr, uniform,
+                             batch, num_draft + 1LL, vocab, out_tokens, accepted, nullptr, nullptr, 0, stream});
 }
 
 int b200_spec_verify_tree(const float* target_probs, const int32_t* target_ids, const int32_t* tree_parents, const int32_t* node_tokens,
                           const float* uniform, int batch, int n, int vocab, int32_t* out_tokens, int32_t* accepted,
                           int32_t* accepted_path, void* stream) {
-    ARG_CHECK(batch >= 0 && batch <= 65535, "spec_verify_tree: batch %d unsupported (0..65535)", batch);
-    ARG_CHECK(n >= 1 && n <= kSpecTreeMaxNodes, "spec_verify_tree: n %d unsupported (1..%d)", n, kSpecTreeMaxNodes);
-    ARG_CHECK(vocab > 0, "spec_verify_tree: vocab must be positive");
-    if (batch == 0) return B200_OK;
-    ARG_CHECK(tree_parents && node_tokens && out_tokens && accepted && accepted_path, "spec_verify_tree: null pointer");
-    ARG_CHECK(target_probs || target_ids, "spec_verify_tree: need target_probs (sampling) or target_ids (greedy)");
-    ARG_CHECK(!target_probs || uniform, "spec_verify_tree: sampling mode needs uniform");
-    return spec_verify_launch(target_probs, target_ids, nullptr, node_tokens, tree_parents, uniform, out_tokens, accepted,
-                              accepted_path, batch, n, vocab, stream);
-}
-
-size_t b200_spec_verify_tree_draft_workspace_bytes(int batch, int vocab) {
-    return batch > 0 && vocab > 0 ? (size_t)batch * vocab * sizeof(float) : 0;
+    return spec_verify_impl({"spec_verify_tree", VerifyEntry::kTree, target_probs, target_ids, nullptr, node_tokens, tree_parents,
+                             uniform, batch, n, vocab, out_tokens, accepted, accepted_path, nullptr, 0, stream});
 }
 
 int b200_spec_verify_tree_draft(const float* target_probs, const float* draft_probs, const int32_t* tree_parents,
                                 const int32_t* node_tokens, const float* uniform, int batch, int n, int vocab, void* workspace,
                                 size_t workspace_bytes, int32_t* out_tokens, int32_t* accepted, int32_t* accepted_path,
                                 void* stream) {
-    ARG_CHECK(batch >= 0 && batch <= 65535, "spec_verify_tree_draft: batch %d unsupported (0..65535)", batch);
-    ARG_CHECK(n >= 2 && n <= kSpecTreeMaxNodes, "spec_verify_tree_draft: n %d unsupported (2..%d)", n, kSpecTreeMaxNodes);
-    ARG_CHECK(vocab > 0, "spec_verify_tree_draft: vocab must be positive");
-    if (batch == 0) return B200_OK;
-    ARG_CHECK(target_probs && draft_probs && tree_parents && node_tokens && uniform && out_tokens && accepted && accepted_path,
-              "spec_verify_tree_draft: null pointer");
-    const size_t need = b200_spec_verify_tree_draft_workspace_bytes(batch, vocab);
-    ARG_CHECK(workspace && workspace_bytes >= need,
-              "spec_verify_tree_draft: workspace too small (%zu < %zu bytes, see b200_spec_verify_tree_draft_workspace_bytes)",
-              workspace ? workspace_bytes : (size_t)0, need);
-    const SpecVerifyTreeDraftParams p{{target_probs, nullptr, draft_probs, node_tokens, tree_parents, uniform, out_tokens, accepted,
-                                       accepted_path, n, vocab},
-                                      static_cast<float*>(workspace)};
-    return launch_op("spec_verify_kernel", stream, spec_verify_kernel<true>, {dim3(batch), dim3(kSampleThreads)}, p);
+    return spec_verify_impl({"spec_verify_tree_draft", VerifyEntry::kTreeDraft, target_probs, nullptr, draft_probs, node_tokens,
+                             tree_parents, uniform, batch, n, vocab, out_tokens, accepted, accepted_path, workspace, workspace_bytes,
+                             stream});
 }
 
 int b200_kv_compact_path(void* const* kv_pools, int layers, int kv_head_num, int head_dim, int page_size, const int32_t* page_list,

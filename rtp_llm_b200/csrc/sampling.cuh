@@ -248,43 +248,40 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(const SamplePara
 // kernel, bindings/cuda/kernels/speculative_sampling/sampling.cu, and its tree form after SpecInfer / EAGLE). A sequence's N rows
 // are the nodes of a tree: node 0 the last accepted token, node c >= 1 a draft token under parent(c) in [0, c). A chain (no
 // parents given) is parent(c) = c - 1 with node c's token draft_tokens[c - 1]; a tree gives parents and node tokens [B][N].
-// The walk starts at the root and tries the current node's children in index order.
-// Greedy (target_probs == NULL): move to the first child whose token equals target_ids[cur]; at none, emit target_ids[cur].
-// Sampling: child c with token x is accepted iff uniform[c - 1] * p < r(x) (fp32). r is the row of cur with the tokens of the
-// siblings rejected before c zeroed, p = draft_probs (chain only) or 1 - S, S the fp32 sum of r over those rejections: the
-// multi-round rejection of several deterministic drafts, which on a chain (S = 0) is the one-draft test uniform * 1 < q. With
-// every child rejected the token is drawn from the residual max(0, q - p) -- q with the rejected tokens removed for
-// deterministic drafts, from q itself when the residual has no mass -- and at a leaf the bonus token from the leaf's row; both
-// draws use uniform[N - 1] and chunked_draw. One CTA of 1024 threads per sequence; every thread walks the same tree (the same
-// loads, the same fp32 compares), so the decisions are uniform.
-// The draft-tree instance (kDraftTree, b200_spec_verify_tree_draft) runs SpecInfer's multi-step speculative sampling with draft
-// rows draft_probs [B][N][V] (row c: the distribution node c's token was drawn from). At the node cur, with R = t (its target
-// row) and Z = 1, child c with token x is accepted iff uniform[c - 1] * p_c(x) * Z < R(x) in fp32 (each product rounded, no
-// FMA); on a rejection R = max(0, R - Z * p_c) elementwise (again product and difference rounded apart) and Z = sum R, one
-// pass over the vocabulary (spec_residual_pass) into the caller's [B][V] workspace. With every child rejected the token is
-// drawn from R (from t when it has no mass), at a leaf from t. On a chain Z is 1 at every test and the rule is the chain's
-// draft_probs rule bit for bit.
+// One walk serves every rule: from the root it tests the current node's children in index order, moves to the first one
+// accepted, and stops at a node whose children are all rejected (or that has none). One kernel instance per shape (kTree) and
+// rule:
+// - kGreedy (target_ids): accept the first child whose token equals target_ids[cur]; emit target_ids[cur].
+// - kDeterministic (target_probs, drafts as fixed tokens): child c with token x is accepted iff uniform[c - 1] * (1 - S) < r(x)
+//   (fp32), r the row t of cur with the tokens of the siblings rejected before c zeroed and S the fp32 sum of r over those
+//   rejections: the multi-round rejection of several deterministic drafts, on a chain (S = 0) the one-draft test u * 1 < t.
+//   With every child rejected the token is drawn from max(0, t - 1) on the rejected tokens, t elsewhere.
+// - kDraftRows (target_probs and draft rows, node c's row p_c the distribution its token was drawn from): SpecInfer's
+//   multi-step speculative sampling. At cur, with R = t and Z = 1, child c is accepted iff uniform[c - 1] * p_c(x) * Z < R(x) in
+//   fp32 (each product rounded, no FMA); on a rejection R = max(0, R - Z * p_c) elementwise (product and difference rounded
+//   apart) and Z = sum R. On a tree every rejection is one pass over the vocabulary (spec_residual_pass) into the caller's
+//   [B][V] workspace, and with every child rejected the token is drawn from R there. A chain stops at its first rejection,
+//   where Z = 1 and R = t: it needs no workspace and draws from max(0, t - p_c) as it reads the rows.
+// A residual without mass falls back to t, and a leaf draws the bonus token from t; both draws use uniform[N - 1] and
+// chunked_draw. One CTA of 1024 threads per sequence; every thread walks the same tree (the same loads, the same fp32
+// compares), so the decisions are uniform.
 constexpr int kSpecTreeMaxNodes = 64;
+enum class SpecRule { kGreedy, kDeterministic, kDraftRows };
 struct SpecVerifyParams {
-    const float* target_probs;    // optional [B][N][V]
-    const int32_t* target_ids;    // [B][N] (greedy mode)
-    const float* draft_probs;     // optional [B][N-1][V] (chain only)
+    const float* target_probs;    // [B][N][V] (kDeterministic, kDraftRows)
+    const int32_t* target_ids;    // [B][N] (kGreedy)
+    const float* draft_probs;     // kDraftRows: chain [B][N-1][V], node c's row at c - 1; tree [B][N][V], row 0 unread
     const int32_t* draft_tokens;  // chain: [B][N-1], node c's token at c - 1; tree: node tokens [B][N], entry 0 unread
-    const int32_t* parents;       // optional [B][N] (tree, N <= kSpecTreeMaxNodes); NULL: the chain
-    const float* uniform;         // [B][N] (sampling mode)
+    const int32_t* parents;       // tree: [B][N] (N <= kSpecTreeMaxNodes); chain: unread
+    const float* uniform;         // [B][N] (kDeterministic, kDraftRows)
+    float* residual;              // kDraftRows on a tree: [B][V] workspace, the residual R of the node the walk stands on
     int32_t* out_tokens;          // [B][N]: accepted tokens, one correction / bonus token, then -1
     int32_t* accepted;            // [B]
     int32_t* accepted_path;       // optional [B][N]: the node at depth 0 .. accepted, then -1
     int num_nodes, vocab;
 };
-// The draft-tree instance's parameters: draft_probs is [B][N][V] there, parents and target_probs are set, target_ids is unread
-struct SpecVerifyTreeDraftParams : SpecVerifyParams {
-    float* residual;              // [B][V] workspace: the residual R of the node the walk stands on, written before it is read
-};
-template <bool kDraftTree>
-using SpecVerifyParamsOf = typename std::conditional<kDraftTree, SpecVerifyTreeDraftParams, SpecVerifyParams>::type;
 
-// One rejection of the draft-tree walk: R = max(0, src - Z * p) over [0, V) (src: the target row at the node's first rejection,
+// One rejection of the kDraftRows walk: R = max(0, src - Z * p) over [0, V) (src: the target row at the node's first rejection,
 // R itself after it), returns the new Z = sum R, identical in every thread. Thread tid owns the 4-element groups g = tid + k *
 // 1024 and adds their elements in index order; block_reduce_sum adds the threads' sums in its fixed order, so Z is
 // deterministic (tests/draft_tree_oracle.py restates that order). float4 loads and stores when every row is 16-byte aligned.
@@ -322,115 +319,91 @@ __device__ __forceinline__ float spec_residual_pass(const float* src, const floa
     return block_reduce_sum(part, s_red);
 }
 
-template <bool kDraftTree>
-__global__ void __launch_bounds__(kSampleThreads) spec_verify_kernel(const SpecVerifyParamsOf<kDraftTree> p) {
+// One CTA per SM (the minimum of 1): at ptxas' default target of two, 32 registers, the chain's two-row draw was 8 us slower
+// at B 32, V 128256 (DESIGN.md 3.3)
+template <SpecRule kRule, bool kTree>
+__global__ void __launch_bounds__(kSampleThreads, 1) spec_verify_kernel(const SpecVerifyParams p) {
+    constexpr bool kGreedy = kRule == SpecRule::kGreedy, kRows = kRule == SpecRule::kDraftRows, tree = kTree;
     __shared__ float s_scan[kSampleThreads];
+    __shared__ float s_red[kSampleThreads / 32];
     __shared__ int s_pick, s_owner;
     __shared__ int s_path[kSpecTreeMaxNodes];   // tree: the accepted path (a chain's is the identity)
-    __shared__ int s_rej[kSpecTreeMaxNodes];    // the rejected children's tokens at the node the walk stopped at
+    __shared__ int s_rej[kSpecTreeMaxNodes];    // kDeterministic: the rejected children's tokens at the node the walk stopped at
     const int b = blockIdx.x, tid = threadIdx.x, N = p.num_nodes, V = p.vocab;
     pdl_wait();                        // under PDL the target rows come from the kernels before this one
-    const bool tree = kDraftTree || p.parents != nullptr;
     const int32_t* par = tree ? p.parents + (size_t)b * N : nullptr;
-    const int32_t* ntok = p.draft_tokens + (size_t)b * (tree ? N : N - 1);
-    auto token = [&](int c) { return tree ? ntok[c] : ntok[c - 1]; };
+    const int rows = tree ? N : N - 1;                  // per sequence, of draft_tokens and draft_probs: a chain has no root row
+    auto row_of = [&](int c) { return tree ? c : c - 1; };
+    const int32_t* ntok = p.draft_tokens + (size_t)b * rows;
+    auto token = [&](int c) { return ntok[row_of(c)]; };
     // the children of node cur are the c in (cur, N) with parent(c) == cur; a chain's only one is cur + 1
     auto child_end = [&](int cur) { return tree ? N : min(cur + 2, N); };
     auto is_child = [&](int c, int cur) { return !tree || par[c] == cur; };
-    int acc = 0, cur = 0, tok;
+    const int32_t* ids = kGreedy ? p.target_ids + (size_t)b * N : nullptr;   // (each pointer formed only where it is set)
+    const float* u = kGreedy ? nullptr : p.uniform + (size_t)b * N;
+    auto trow = [&](int i) { return p.target_probs + ((size_t)b * N + i) * V; };
+    auto drow = [&](int c) { return p.draft_probs + ((size_t)b * rows + row_of(c)) * V; };
+    float* R = kRows && tree ? p.residual + (size_t)b * V : nullptr;
+    const bool vec = kRows && (V & 3) == 0 && ((reinterpret_cast<uintptr_t>(p.target_probs) |
+                                                reinterpret_cast<uintptr_t>(p.draft_probs) |
+                                                reinterpret_cast<uintptr_t>(p.residual)) & 15) == 0;
+    int acc = 0, cur = 0;
     if (tid == 0 && tree) s_path[0] = 0;
-    auto step = [&](int c) {
-        cur = c;
-        ++acc;
-        if (tid == 0 && tree) s_path[acc] = c;
-    };
-    if constexpr (kDraftTree) {
-        __shared__ float s_red[kSampleThreads / 32];
-        const float* u = p.uniform + (size_t)b * N;
-        auto trow = [&](int i) { return p.target_probs + ((size_t)b * N + i) * V; };
-        auto drow = [&](int i) { return p.draft_probs + ((size_t)b * N + i) * V; };
-        float* R = p.residual + (size_t)b * V;
-        const bool vec = (V & 3) == 0 && ((reinterpret_cast<uintptr_t>(p.target_probs) | reinterpret_cast<uintptr_t>(p.draft_probs) |
-                                           reinterpret_cast<uintptr_t>(p.residual)) & 15) == 0;
-        int nrej = 0;                  // at the node the walk stands on: its rejected children (R is its residual when > 0)
-        for (bool moved = true; moved;) {
-            moved = false;
-            const float* t = trow(cur);
-            float Z = 1.f;
-            nrej = 0;
-            for (int c = cur + 1; c < N; ++c) {
-                if (par[c] != cur) continue;
-                const int x = ntok[c];
-                const bool in = x >= 0 && x < V;
-                const float r = in ? (nrej ? R[x] : t[x]) : 0.f;
-                const float px = in ? drow(c)[x] : 0.f;
-                if (__fmul_rn(__fmul_rn(u[c - 1], px), Z) < r) {
-                    step(c);
-                    moved = true;
-                    break;
+    // at the node the walk stands on: its rejected children; kDeterministic: the mass S of their tokens; kDraftRows: Z, the row
+    // R the accept tests read (src: t until the first pass) and the row p_c of the child tested last
+    int nrej = 0;
+    float S = 0.f, Z = 1.f;
+    const float *src = nullptr, *pc = nullptr;
+    for (bool moved = true; moved;) {
+        moved = false;
+        nrej = 0;
+        S = 0.f;
+        Z = 1.f;
+        if constexpr (kRows) src = trow(cur);
+        for (int c = cur + 1; c < child_end(cur); ++c) {
+            if (!is_child(c, cur)) continue;
+            const int x = token(c);
+            const bool in = x >= 0 && x < V;
+            bool accept;
+            if constexpr (kGreedy) {
+                accept = x == ids[cur];
+            } else if constexpr (kRows) {
+                pc = drow(c);
+                accept = __fmul_rn(__fmul_rn(u[c - 1], in ? pc[x] : 0.f), Z) < (in ? src[x] : 0.f);
+                if (!accept && tree) {
+                    Z = spec_residual_pass(src, pc, R, Z, V, vec, s_red);
+                    src = R;
                 }
-                Z = spec_residual_pass(nrej ? R : t, drow(c), R, Z, V, vec, s_red);
-                ++nrej;
+            } else {
+                bool seen = false;     // x is the token of a sibling rejected before c: r(x) = 0
+                for (int c2 = cur + 1; c2 < c; ++c2) seen |= is_child(c2, cur) && token(c2) == x;
+                const float q = in && !seen ? trow(cur)[x] : 0.f;
+                accept = u[c - 1] * (1.f - S) < q;
+                S += q;
             }
-        }
-        float total;
-        const float* t = trow(cur);
-        tok = -1;
-        if (nrej) tok = chunked_draw([&](int x) { return R[x]; }, V, u[N - 1], false, s_scan, &s_pick, &s_owner, &total);
-        if (!nrej || !(total > 0.f)) {   // a leaf, or a residual without mass: draw from t
-            if (nrej) __syncthreads();     // every thread has read the first draw's shared result
-            tok = chunked_draw([&](int x) { return t[x] > 0.f ? t[x] : 0.f; }, V, u[N - 1], false, s_scan, &s_pick, &s_owner,
-                               &total);
-        }
-    } else if (!p.target_probs) {
-        const int32_t* ids = p.target_ids + (size_t)b * N;
-        for (bool moved = true; moved;) {
-            moved = false;
-            for (int c = cur + 1; c < child_end(cur); ++c) {
-                if (is_child(c, cur) && token(c) == ids[cur]) {
-                    step(c);
-                    moved = true;
-                    break;
-                }
+            if (accept) {
+                cur = c;
+                ++acc;
+                if (tid == 0 && tree) s_path[acc] = c;
+                moved = true;
+                break;
             }
+            ++nrej;
         }
+    }
+    int tok;
+    if constexpr (kGreedy) {
         tok = ids[cur];
     } else {
-        const float* u = p.uniform + (size_t)b * N;
-        auto trow = [&](int i) { return p.target_probs + ((size_t)b * N + i) * V; };
-        auto drow = [&](int i) { return p.draft_probs + ((size_t)b * (N - 1) + i) * V; };
-        int last_rej = -1, nrej = 0;   // at the node the walk stops at: its last rejected child, and how many
-        for (bool moved = true; moved;) {
-            moved = false;
-            const float* t = trow(cur);
-            float S = 0.f;
-            last_rej = -1;
-            nrej = 0;
-            for (int c = cur + 1; c < child_end(cur); ++c) {
-                if (!is_child(c, cur)) continue;
-                const int d = token(c);
-                const bool in = d >= 0 && d < V;
-                bool seen = false;             // d is the token of a sibling rejected before c: r(d) = 0
-                for (int c2 = cur + 1; c2 < c; ++c2) seen |= is_child(c2, cur) && token(c2) == d;
-                const float q = in && !seen ? t[d] : 0.f;
-                const float pd = p.draft_probs ? (in ? drow(c - 1)[d] : 0.f) : 1.f - S;
-                if (u[c - 1] * pd < q) {
-                    step(c);
-                    moved = true;
-                    break;
-                }
-                S += q;
-                last_rej = c;
-                ++nrej;
-            }
-        }
-        float total;
         const float* t = trow(cur);
-        if (last_rej >= 0) {
-            if (p.draft_probs) {
-                const float* dp = drow(last_rej - 1);
-                tok = chunked_draw([&](int x) { return fmaxf(0.f, t[x] - dp[x]); }, V, u[N - 1], false, s_scan, &s_pick, &s_owner,
-                                   &total);
+        float total = 0.f;
+        if (nrej) {                    // every child rejected: draw from the residual
+            if constexpr (kRows) {
+                if (tree)
+                    tok = chunked_draw([&](int x) { return R[x]; }, V, u[N - 1], false, s_scan, &s_pick, &s_owner, &total);
+                else           // a chain's one rejection (of node cur + 1), where Z = 1 and R = t
+                    tok = chunked_draw([&, dp = drow(cur + 1)](int x) { return fmaxf(0.f, t[x] - dp[x]); }, V, u[N - 1], false,
+                                       s_scan, &s_pick, &s_owner, &total);
             } else {
                 if (tid == 0) {
                     int k = 0;
@@ -446,12 +419,9 @@ __global__ void __launch_bounds__(kSampleThreads) spec_verify_kernel(const SpecV
                 tok = chunked_draw([&](int x) { return fmaxf(0.f, t[x] - (rejected(x) ? 1.f : 0.f)); }, V, u[N - 1], false, s_scan,
                                    &s_pick, &s_owner, &total);
             }
-            if (!(total > 0.f)) {          // the residual has no mass (q <= p everywhere): draw from q
-                __syncthreads();           // every thread has read the first draw's shared result
-                tok = chunked_draw([&](int x) { return t[x] > 0.f ? t[x] : 0.f; }, V, u[N - 1], false, s_scan, &s_pick, &s_owner,
-                                   &total);
-            }
-        } else {
+        }
+        if (!(total > 0.f)) {          // a leaf, or a residual without mass: draw from t
+            if (nrej) __syncthreads(); // every thread has read the first draw's shared result
             tok = chunked_draw([&](int x) { return t[x] > 0.f ? t[x] : 0.f; }, V, u[N - 1], false, s_scan, &s_pick, &s_owner, &total);
         }
     }

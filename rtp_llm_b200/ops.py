@@ -671,6 +671,27 @@ def sample(logits: torch.Tensor, top_k: torch.Tensor, top_p: torch.Tensor, unifo
     return out["token"], out["token_prob"], out.get("probs")
 
 
+def _spec_verify_args(who: str, device, B: int, nodes: int, draft_rows: int, target_probs, target_ids, uniform, draft_probs,
+                      outs: dict):
+    """The checks and outputs both verification wrappers share, for B sequences of `nodes` rows: the greedy (target_ids) or
+    sampling (target_probs, uniform) inputs, draft_probs [B, draft_rows, V] in sampling mode, and the outputs of `outs` (name:
+    tensor or None), out_tokens [B, nodes], accepted [B] and accepted_path [B, nodes]. Returns (V, outputs)."""
+    if target_probs is None and target_ids is None:
+        raise B200Error(f"{who}: pass target_probs (sampling) or target_ids (greedy)")
+    if target_probs is not None:
+        _need(who, "target_probs", target_probs, torch.float32, (B, nodes, "V"))
+        V = target_probs.shape[2]
+        if uniform is None or uniform.dtype != torch.float32 or uniform.numel() != B * nodes:
+            raise B200Error(f"{who}: sampling mode needs uniform fp32 [{B}, {nodes}]")
+        if draft_probs is not None:
+            _need(who, "draft_probs", draft_probs, torch.float32, (B, draft_rows, V))
+    else:
+        _need(who, "target_ids", target_ids, torch.int32, (B, nodes))
+        V = 1                                   # the vocabulary is not read in greedy mode
+    shapes = dict(out_tokens=(torch.int32, (B, nodes)), accepted=(torch.int32, (B,)), accepted_path=(torch.int32, (B, nodes)))
+    return V, _outputs(who, outs, device, **{k: shapes[k] for k in outs})
+
+
 def spec_verify(draft_tokens: torch.Tensor, *, target_probs: Optional[torch.Tensor] = None,
                 target_ids: Optional[torch.Tensor] = None, draft_probs: Optional[torch.Tensor] = None,
                 uniform: Optional[torch.Tensor] = None, out_tokens: Optional[torch.Tensor] = None,
@@ -681,22 +702,10 @@ def spec_verify(draft_tokens: torch.Tensor, *, target_probs: Optional[torch.Tens
     bonus token, then -1; accepted int32 [B])."""
     _cuda_contig(draft_tokens, target_probs, target_ids, draft_probs, uniform, out_tokens, accepted)
     B, n = draft_tokens.shape
-    if target_probs is None and target_ids is None:
-        raise B200Error("spec_verify: pass target_probs (sampling) or target_ids (greedy)")
-    if target_probs is not None:
-        _need("spec_verify", "target_probs", target_probs, torch.float32, (B, n + 1, "V"))
-        V = target_probs.shape[2]
-        if uniform is None or uniform.dtype != torch.float32 or uniform.numel() != B * (n + 1):
-            raise B200Error(f"spec_verify: sampling mode needs uniform fp32 [{B}, {n + 1}]")
-        if draft_probs is not None:
-            _need("spec_verify", "draft_probs", draft_probs, torch.float32, (B, n, V))
-    else:
-        _need("spec_verify", "target_ids", target_ids, torch.int32, (B, n + 1))
-        V = 1                                   # the vocabulary is not read in greedy mode
+    V, out = _spec_verify_args("spec_verify", draft_tokens.device, B, n + 1, n, target_probs, target_ids, uniform, draft_probs,
+                               dict(out_tokens=out_tokens, accepted=accepted))
     if draft_tokens.dtype != torch.int32:
         raise B200Error("spec_verify: draft_tokens must be int32")
-    out = _outputs("spec_verify", dict(out_tokens=out_tokens, accepted=accepted), draft_tokens.device,
-                   out_tokens=(torch.int32, (B, n + 1)), accepted=(torch.int32, (B,)))
     check(_lib.load().b200_spec_verify(_p(target_probs), _p(target_ids), _p(draft_probs), _p(draft_tokens), _p(uniform), B, n, V,
                                        _p(out["out_tokens"]), _p(out["accepted"]), _stream()), "b200_spec_verify")
     return out["out_tokens"], out["accepted"]
@@ -729,35 +738,20 @@ def spec_verify_tree(tree_parents: torch.Tensor, node_tokens: torch.Tensor, *, t
     B, n = tree_parents.shape
     if tree_parents.dtype != torch.int32 or node_tokens.dtype != torch.int32 or tuple(node_tokens.shape) != (B, n):
         raise B200Error(f"spec_verify_tree: tree_parents and node_tokens must be int32 [{B}, {n}]")
-    if target_probs is None and target_ids is None:
-        raise B200Error("spec_verify_tree: pass target_probs (sampling) or target_ids (greedy)")
-    if target_probs is not None:
-        _need("spec_verify_tree", "target_probs", target_probs, torch.float32, (B, n, "V"))
-        V = target_probs.shape[2]
-        if uniform is None or uniform.dtype != torch.float32 or uniform.numel() != B * n:
-            raise B200Error(f"spec_verify_tree: sampling mode needs uniform fp32 [{B}, {n}]")
-    else:
-        _need("spec_verify_tree", "target_ids", target_ids, torch.int32, (B, n))
-        V = 1                                   # the vocabulary is not read in greedy mode
-    if draft_probs is not None:
-        _need("spec_verify_tree", "draft_probs", draft_probs, torch.float32, (B, n, V))
-        need = int(_lib.load().b200_spec_verify_tree_draft_workspace_bytes(B, V))
-        if workspace is None:
-            workspace = spec_verify_tree_draft_workspace(B, V, tree_parents.device)
-        elif workspace.dtype != torch.uint8 or workspace.numel() < need:
-            raise B200Error(f"spec_verify_tree: workspace must be uint8 of at least {need} bytes (spec_verify_tree_draft_workspace)")
-    out = _outputs("spec_verify_tree", dict(out_tokens=out_tokens, accepted=accepted, accepted_path=accepted_path),
-                   tree_parents.device, out_tokens=(torch.int32, (B, n)), accepted=(torch.int32, (B,)),
-                   accepted_path=(torch.int32, (B, n)))
-    if draft_probs is not None:
-        check(_lib.load().b200_spec_verify_tree_draft(_p(target_probs), _p(draft_probs), _p(tree_parents), _p(node_tokens), _p(uniform),
-                                                      B, n, V, _p(workspace), workspace.numel(), _p(out["out_tokens"]),
-                                                      _p(out["accepted"]), _p(out["accepted_path"]), _stream()),
-              "b200_spec_verify_tree_draft")
+    V, out = _spec_verify_args("spec_verify_tree", tree_parents.device, B, n, n, target_probs, target_ids, uniform, draft_probs,
+                               dict(out_tokens=out_tokens, accepted=accepted, accepted_path=accepted_path))
+    outs = (_p(out["out_tokens"]), _p(out["accepted"]), _p(out["accepted_path"]), _stream())
+    if draft_probs is None:
+        check(_lib.load().b200_spec_verify_tree(_p(target_probs), _p(target_ids), _p(tree_parents), _p(node_tokens), _p(uniform), B, n,
+                                                V, *outs), "b200_spec_verify_tree")
         return out["out_tokens"], out["accepted"], out["accepted_path"]
-    check(_lib.load().b200_spec_verify_tree(_p(target_probs), _p(target_ids), _p(tree_parents), _p(node_tokens), _p(uniform), B, n, V,
-                                            _p(out["out_tokens"]), _p(out["accepted"]), _p(out["accepted_path"]), _stream()),
-          "b200_spec_verify_tree")
+    need = int(_lib.load().b200_spec_verify_tree_draft_workspace_bytes(B, V))
+    if workspace is None:
+        workspace = spec_verify_tree_draft_workspace(B, V, tree_parents.device)
+    elif workspace.dtype != torch.uint8 or workspace.numel() < need:
+        raise B200Error(f"spec_verify_tree: workspace must be uint8 of at least {need} bytes (spec_verify_tree_draft_workspace)")
+    check(_lib.load().b200_spec_verify_tree_draft(_p(target_probs), _p(draft_probs), _p(tree_parents), _p(node_tokens), _p(uniform),
+                                                  B, n, V, _p(workspace), workspace.numel(), *outs), "b200_spec_verify_tree_draft")
     return out["out_tokens"], out["accepted"], out["accepted_path"]
 
 

@@ -93,6 +93,22 @@ def test_tree_draft_verify_vs_fp32_oracle(kind, n, B):
         assert (ea < n - 1).any(), "no rejection"
 
 
+def _stop_children(par, ea, ep):
+    """How many children the node each sequence's walk stopped at has: all of them were rejected (0: a leaf)."""
+    return np.array([(par[b] == ep[b, ea[b]]).sum() for b in range(par.shape[0])])
+
+
+def test_cases_reach_every_kind_of_stop_node():
+    """The draw differs by where the walk stops: at a leaf (from t), after one rejected child (from the residual of one pass
+    from t), or after two or more (from the residual the passes rewrote in place). CASES reach all three."""
+    kinds = set()
+    for kind, n, B in CASES:
+        par, toks, t, dp, u = _case(n * 100 + B, kind, n, B)
+        _, ea, ep = tree_draft_verify_np(par, toks, t, dp, u)
+        kinds |= set(np.minimum(_stop_children(par, ea, ep), 2).tolist())
+    assert kinds == {0, 1, 2}, kinds
+
+
 @pytest.mark.parametrize("V", [1001, 4096])
 def test_tree_draft_verify_scalar_pass_vs_fp32_oracle(V):
     """The scalar pass (a vocabulary that is not a multiple of 4, or rows 4 bytes off 16-byte alignment) sums in the order of

@@ -175,6 +175,18 @@ def bench_tree_verify_draft(B, n, rejects, V=128256, nrot=4, runs=3):
     return med
 
 
+def bench_chain_verify_draft(B, n, V=128256, nrot=4):
+    """b200_spec_verify with draft rows on chains of n drafts: target and draft rows of temperature-0.25 softmaxes and random
+    draft tokens, so nearly every walk rejects its first draft and draws from the residual max(0, t - p)."""
+    toks = torch.randint(0, V, (B, n), dtype=torch.int32, device=dev)
+    probs = [torch.softmax(torch.randn(B, n + 1, V, device=dev) / 0.25, dim=-1) for _ in range(nrot)]
+    drafts = [torch.softmax(torch.randn(B, n, V, device=dev) / 0.25, dim=-1) for _ in range(nrot)]
+    u = torch.rand(B, n + 1, device=dev)
+    us = timeit(lambda i: ops.spec_verify(toks, target_probs=probs[i], draft_probs=drafts[i], uniform=u), nrot)
+    print(f"chain-verify-draft B{B} n{n}: {us:.1f} us", flush=True)
+    return us
+
+
 def bench_kv_compact(B, layers=32, Hkv=8, T=64, n=8, S=2048, nrot=2):
     """b200_kv_compact_path over the Llama-3-8B cache (32 layers, Hkv 8, D 128) with a path that moves every depth."""
     M = math.ceil((S + n) / T)
@@ -593,6 +605,9 @@ if __name__ == "__main__":
             for n in (4, 8, 16):
                 for rejects in ("0", "1", "all"):
                     bench_tree_verify_draft(B, n, rejects)
+    if "chain-verify-draft" in which:
+        for n in (4, 8):
+            bench_chain_verify_draft(32, n)
     if "kv-compact" in which:
         for B in (8, 32):
             bench_kv_compact(B)
