@@ -284,7 +284,7 @@ struct SpecVerifyParams {
 // One rejection of the kDraftRows walk: R = max(0, src - Z * p) over [0, V) (src: the target row at the node's first rejection,
 // R itself after it), returns the new Z = sum R, identical in every thread. Thread tid owns the 4-element groups g = tid + k *
 // 1024 and adds their elements in index order; block_reduce_sum adds the threads' sums in its fixed order, so Z is
-// deterministic (tests/draft_tree_oracle.py restates that order). float4 loads and stores when every row is 16-byte aligned.
+// deterministic (tests/verify_oracle.py restates that order). float4 loads and stores when every row is 16-byte aligned.
 __device__ __forceinline__ float spec_residual_pass(const float* src, const float* dp, float* R, float Z, int V, bool vec,
                                                     float* s_red) {
     __syncthreads();                   // every thread has read R for its accept test before any thread rewrites it

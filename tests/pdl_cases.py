@@ -102,7 +102,7 @@ def _attn(fn, dtype=F16, D=128, B=3, Hq=16, Hkv=2, T=16, q_len=1, max_len=200, W
         else:
             d["q"] = _randn(g, B, q_len, Hq, D, dtype=dtype)
         if fn == "tree":
-            from tests.tree_oracle import random_tree
+            from tests.verify_oracle import random_tree
             rng = np.random.default_rng(seed)
             d["parents"] = torch.from_numpy(np.stack([random_tree(rng, q_len, "random") for _ in range(B)])).to(I32).to(DEV)
         d.update(pl=pl, seq=seq.to(DEV))
@@ -312,7 +312,7 @@ def _rope(kind, dtype=F16, B=3, q_len=1, Hq=8, Hkv=2, D=128, T=16, qk_norm=False
 
 def _kv_compact(dtype=BF16, B=3, n=8, Hkv=2, D=128, T=16, layers=2):
     from rtp_llm_b200 import ops
-    from tests.tree_oracle import ancestors, random_tree
+    from tests.verify_oracle import ancestors, random_tree
     max_len = 256
     M = max_len // T
     P = B * 2 * M + 1
@@ -406,7 +406,7 @@ def _spec_verify(sampling, B=4, n=4, V=500):
 
 def _spec_verify_tree(B=4, n=8):
     from rtp_llm_b200 import ops
-    from tests.tree_oracle import random_tree
+    from tests.verify_oracle import random_tree
 
     def dyn(seed):
         g = _gen(seed)

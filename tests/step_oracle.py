@@ -10,7 +10,7 @@ import torch
 from oracle import oracle as orc
 from rtp_llm_b200 import ops, rope
 from rtp_llm_b200.decode_step import TINY, DecodeStep
-from tests.spec_oracle import spec_verify_np
+from tests.verify_oracle import chain_verify_np
 
 # Llama-3.1 rope on the tiny config. Llama3 keeps a rotary dim's angle below wavelength max_pos / factor2, divides it by scale
 # above max_pos / factor1 and blends in between. max_pos 16 puts about three quarters of the dims at the tiny contexts'
@@ -152,7 +152,7 @@ def check_step(cfg=TINY, quant=None, batch=3, ctx=40, mode="eager", q_len=1, act
     sure = srt[:, -1] - srt[:, -2] > 2 * err + 1e-6
     assert (nxt[sure] == oa[sure]).all(), (nxt, oa)
     if q_len > 1:
-        eo, ea = spec_verify_np(model.ids_h[:, 1:].numpy(), target_ids=nxt.reshape(model.B, q_len))
+        eo, ea = chain_verify_np(model.ids_h[:, 1:].numpy(), target_ids=nxt.reshape(model.B, q_len))[:2]
         np.testing.assert_array_equal(model.accepted.cpu().numpy(), ea)
         np.testing.assert_array_equal(model.out_tokens.cpu().numpy(), eo)
     return err

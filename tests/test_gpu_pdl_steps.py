@@ -18,7 +18,7 @@ pytestmark = pytest.mark.gpu
 from rtp_llm_b200 import ops  # noqa: E402
 from rtp_llm_b200.decode_step import TINY, TINY_QWEN3, DecodeStep  # noqa: E402
 from tests.test_gpu_sampling import PARAMS  # noqa: E402
-from tests.tree_oracle import random_tree  # noqa: E402
+from tests.verify_oracle import random_tree  # noqa: E402
 
 DEV = torch.device("cuda")
 STEPS, BATCH, CTX = 6, 4, 40

@@ -1,7 +1,7 @@
 """GPU tests (H100) of sampled decoding: b200_token_logprobs against the float64 reference (tests/logprob_oracle.py) and its
 bits under CUDA-graph replay with PDL; DecodeStep's sampling mode step by step against oracle_step and the sampler oracle
 (pinned to the reference's CudaSamplerTest vectors) on the step's own logits, params, history and uniforms; and sampled
-verification of speculative tokens against spec_verify_np on the step's own probabilities and uniforms."""
+verification of speculative tokens against chain_verify_np on the step's own probabilities and uniforms."""
 import dataclasses
 
 import numpy as np
@@ -15,8 +15,8 @@ from rtp_llm_b200 import ops  # noqa: E402
 from rtp_llm_b200.decode_step import TINY, DecodeStep, SamplingParams, sampling_uniforms  # noqa: E402
 from tests.beam_oracle import banned_np  # noqa: E402
 from tests.logprob_oracle import log_softmax_np, token_logprobs_np  # noqa: E402
-from tests.spec_oracle import spec_verify_np  # noqa: E402
 from tests.step_oracle import bits, check_logits, device_state, oracle_step  # noqa: E402
+from tests.verify_oracle import chain_verify_np  # noqa: E402
 
 DEV = torch.device("cuda")
 DTYPES = {"fp16": torch.float16, "bf16": torch.bfloat16, "fp32": torch.float32}
@@ -253,7 +253,8 @@ def test_sampled_verification_vs_reference(q_len, mode):
                                          temperature=rep(sp.temperature, np.float32))
             tp = model.target_probs.cpu().numpy()
             np.testing.assert_allclose(tp.reshape(R, -1), eprobs, rtol=1e-3, atol=1e-7)
-            eo, ea = spec_verify_np(model.ids_h[:, 1:].numpy(), target_probs=tp, uniform=u[R:].numpy().reshape(model.B, q_len))
+            eo, ea = chain_verify_np(model.ids_h[:, 1:].numpy(), target_probs=tp,
+                                     uniform=u[R:].numpy().reshape(model.B, q_len))[:2]
             np.testing.assert_array_equal(model.accepted.cpu().numpy(), ea)
             np.testing.assert_array_equal(model.out_tokens.cpu().numpy(), eo)
             check_logprobs({k: v.cpu().numpy() for k, v in model.lp_out.items()},

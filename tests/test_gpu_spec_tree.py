@@ -1,6 +1,6 @@
 """GPU tests (H100) of speculative token-tree verification: tree-masked paged attention against a float64 oracle that gathers each
 query's visible K/V into a contiguous sequence, bit equality with the q_len instance on chains and under NaN / inf in the slots a
-query does not see; the tree verifier against tests/tree_oracle.py and, on chains, against b200_spec_verify bit for bit; and the
+query does not see; the tree verifier against tests/verify_oracle.py and, on chains, against b200_spec_verify bit for bit; and the
 accepted-path K/V compaction, eagerly and under graph capture."""
 
 import numpy as np
@@ -12,8 +12,8 @@ pytestmark = pytest.mark.gpu
 from oracle import oracle as orc  # noqa: E402
 from rtp_llm_b200 import ops  # noqa: E402
 from tests import gpu_probe as probe  # noqa: E402
-from tests.test_gpu_spec_verify import ROWS, V_FULL, _check_draws, _probs  # noqa: E402
-from tests.tree_oracle import ancestors, compact_np, random_tree, tree_verify_np  # noqa: E402
+from tests.test_gpu_spec_verify import ROWS, V_FULL, _probs, check_verify  # noqa: E402
+from tests.verify_oracle import ancestors, compact_np, random_tree, verify_np  # noqa: E402
 
 DEV = torch.device("cuda")
 TREE_ROWS = [r for r in ROWS if r[3] > 1]          # the q_len > 1 rows: D 64 / 128 / 256, fp16 / bf16, pages 16..128, RT 1 / 2 / 4
@@ -145,28 +145,11 @@ def test_tree_verify_greedy_vs_oracle(n):
                 toks[b, c] = ids[b, par[b, c]]
     toks[:, 0] = -1
     out, acc, path = ops.spec_verify_tree(_T(par), _T(toks), target_ids=_T(ids))
-    eo, ea, ep = tree_verify_np(par, toks, target_ids=ids)
+    eo, ea, ep, _ = verify_np(par, toks, target_ids=ids)
     np.testing.assert_array_equal(acc.cpu().numpy(), ea)
     np.testing.assert_array_equal(out.cpu().numpy(), eo)
     np.testing.assert_array_equal(path.cpu().numpy(), ep)
     assert ea.max() >= min(2, n - 1)
-
-
-def _residual_masses(par, toks, t, path, acc):
-    """What the draw after the walk uses: the stop node's row with its (all rejected) children's tokens removed as the chain
-    removes its draft (max(0, t - 1)), or the row itself at a leaf or when that has no mass."""
-    def masses(b, a):
-        node = path[b, a]
-        row = t[b, node]
-        kids = [c for c in range(node + 1, par.shape[1]) if par[b, c] == node]
-        if kids:
-            sub = np.zeros_like(row)
-            sub[[int(toks[b, c]) for c in kids if 0 <= toks[b, c] < row.size]] = 1
-            r = np.maximum(np.float32(0), row - sub)
-            if r.astype(np.float64).sum() > 0:
-                return r
-        return np.where(row > 0, row, 0)
-    return masses
 
 
 @pytest.mark.parametrize("n", [2, 3, 5, 8, 12, 16])
@@ -191,11 +174,11 @@ def test_tree_verify_sampling_vs_oracle(n):
     u = rng.random((B, n)).astype(np.float32)
     u[0, :] = 0.999
     u[2, :] = 0.999                       # reject every child of row 2's root
-    out, acc, path = ops.spec_verify_tree(_T(par), _T(toks), target_probs=_T(t), uniform=_T(u))
-    eo, ea, ep = tree_verify_np(par, toks, target_probs=t, uniform=u)
-    got, acc_got, path_got = out.cpu().numpy(), acc.cpu().numpy(), path.cpu().numpy()
-    np.testing.assert_array_equal(path_got, ep)
-    _check_draws(got, eo, acc_got, ea, _residual_masses(par, toks, t, ep, ea), u[:, n - 1].astype(np.float64))
+    got = ops.spec_verify_tree(_T(par), _T(toks), target_probs=_T(t), uniform=_T(u))
+    exp = verify_np(par, toks, target_probs=t, uniform=u)
+    check_verify(got, exp, u[:, n - 1])
+    eo, ea = exp[:2]
+    got = got[0].cpu().numpy()
     assert ea[1] == 0 and eo[1, 0] == -1                 # mass-free row: every child rejected, nothing to draw
     assert ea[2] == 0 and got[2, 0] in set(toks[2, 1:3].tolist())   # empty residual: drawn from the row itself
     assert ea[0] == 0 and got[0, 0] != toks[0, 1]        # duplicate siblings: the token is rejected once for all of them

@@ -1,5 +1,5 @@
 """GPU tests (H100) of sampled tree verification with draft rows (b200_spec_verify_tree_draft): the kernel against the float32
-restatement of tests/draft_tree_oracle.py at Llama-3's vocabulary, bit for bit with b200_spec_verify(draft_probs) on chains,
+restatement of tests/verify_oracle.py at Llama-3's vocabulary, bit for bit with b200_spec_verify(draft_probs) on chains,
 the PDL grid dependency and graph replay through the slow-predecessor harness, and DecodeStep(draft_probs=True) for trees and
 chains."""
 import dataclasses
@@ -12,12 +12,10 @@ pytestmark = pytest.mark.gpu
 
 from rtp_llm_b200 import ops  # noqa: E402
 from rtp_llm_b200.decode_step import TINY, DecodeStep, SamplingParams, sampling_uniforms  # noqa: E402
-from tests.draft_tree_oracle import tree_draft_verify_np  # noqa: E402
 from tests.pdl_cases import I32, Case, Spec  # noqa: E402
-from tests.spec_oracle import spec_verify_np  # noqa: E402
 from tests.test_gpu_pdl_hazards import _run_case  # noqa: E402
-from tests.test_gpu_spec_verify import V_FULL, _check_draws, _probs  # noqa: E402
-from tests.tree_oracle import random_tree  # noqa: E402
+from tests.test_gpu_spec_verify import V_FULL, _probs, check_verify  # noqa: E402
+from tests.verify_oracle import chain_verify_np, random_tree, verify_np  # noqa: E402
 
 DEV = torch.device("cuda")
 
@@ -69,16 +67,6 @@ def _case(seed, kind, n, B, V=V_FULL):
     return par, toks, t, dp, u
 
 
-def _check(par, toks, t, dp, u, got):
-    out, acc, path = (x.cpu().numpy() for x in got)
-    eo, ea, ep, masses = tree_draft_verify_np(par, toks, t, dp, u, with_residuals=True)
-    np.testing.assert_array_equal(acc, ea)
-    np.testing.assert_array_equal(path, ep)
-    n = par.shape[1]
-    _check_draws(out, eo, acc, ea, lambda b, a: masses[b], u[:, n - 1].astype(np.float64))
-    return ea
-
-
 CASES = [("random", 2, 1), ("random", 5, 32), ("random", 16, 8), ("random", 64, 4), ("binary", 8, 32), ("binary", 31, 3),
          ("star", 3, 16), ("star", 12, 8), ("star", 64, 2), ("chain", 4, 32), ("chain", 17, 5)]
 
@@ -87,7 +75,9 @@ CASES = [("random", 2, 1), ("random", 5, 32), ("random", 16, 8), ("random", 64, 
 def test_tree_draft_verify_vs_fp32_oracle(kind, n, B):
     par, toks, t, dp, u = _case(n * 100 + B, kind, n, B)
     got = ops.spec_verify_tree(_T(par), _T(toks), target_probs=_T(t), uniform=_T(u), draft_probs=_T(dp))
-    ea = _check(par, toks, t, dp, u, got)
+    exp = verify_np(par, toks, target_probs=t, draft_probs=dp, uniform=u)
+    check_verify(got, exp, u[:, n - 1])
+    ea = exp[1]
     if n > 2 and B >= 8:
         assert 0 < ea.mean(), "no acceptance"
         assert (ea < n - 1).any(), "no rejection"
@@ -104,7 +94,7 @@ def test_cases_reach_every_kind_of_stop_node():
     kinds = set()
     for kind, n, B in CASES:
         par, toks, t, dp, u = _case(n * 100 + B, kind, n, B)
-        _, ea, ep = tree_draft_verify_np(par, toks, t, dp, u)
+        _, ea, ep, _ = verify_np(par, toks, target_probs=t, draft_probs=dp, uniform=u)
         kinds |= set(np.minimum(_stop_children(par, ea, ep), 2).tolist())
     assert kinds == {0, 1, 2}, kinds
 
@@ -115,7 +105,7 @@ def test_tree_draft_verify_scalar_pass_vs_fp32_oracle(V):
     the float4 pass: the oracle's decisions, and with misaligned rows the aligned launch's outputs bit for bit."""
     par, toks, t, dp, u = _case(V, "random", 12, 16, V=V)
     got = ops.spec_verify_tree(_T(par), _T(toks), target_probs=_T(t), uniform=_T(u), draft_probs=_T(dp))
-    _check(par, toks, t, dp, u, got)
+    check_verify(got, verify_np(par, toks, target_probs=t, draft_probs=dp, uniform=u), u[:, -1])
     if V % 4:
         return
     B, n = par.shape
@@ -220,13 +210,15 @@ def test_tree_step_with_its_own_rows_as_draft_rows_accepts_every_first_child(mod
     assert torch.equal(m.uniform[R:].cpu(), torch.from_numpy(u).view(-1))
     toks = m.ids_h.numpy()
     got = (m.out_tokens, m.accepted, m.accepted_path)
-    _check(np.tile(TREE, (B, 1)), toks, tp.cpu().numpy(), m.draft_probs.cpu().numpy(), u, got)
+    exp = verify_np(np.tile(TREE, (B, 1)), toks, target_probs=tp.cpu().numpy(), draft_probs=m.draft_probs.cpu().numpy(),
+                    uniform=u)
+    check_verify(got, exp, u[:, n - 1])
 
 
 @pytest.mark.parametrize("mode", ["eager", "graph pdl"])
 def test_chain_step_with_draft_rows_vs_oracle(mode):
     """The chain verification step with draft rows (a mix of the step's own target rows and a far distribution): out_tokens and
-    accepted are spec_verify_np's on the step's own target_probs, draft_probs and uniforms, for several drafts."""
+    accepted are chain_verify_np's on the step's own target_probs, draft_probs and uniforms, for several drafts."""
     cfg = dataclasses.replace(TINY, quant="int4")
     sp = SamplingParams(temperature=[0.7, 1.0, 1.3, 1.0], top_k=[0, 50, 0, 20], top_p=[1.0, 0.9, 0.95, 1.0], seed=11)
     q_len = 4
@@ -244,7 +236,7 @@ def test_chain_step_with_draft_rows_vs_oracle(mode):
         _run(m, mode)
         tp, dp = m.target_probs.cpu().numpy(), m.draft_probs.cpu().numpy()
         u = sampling_uniforms(sp.seed, 0, 2 * R)[R:].view(B, q_len).numpy()
-        eo, ea = spec_verify_np(m.ids_h[:, 1:].numpy(), target_probs=tp, draft_probs=dp, uniform=u)
+        eo, ea = chain_verify_np(m.ids_h[:, 1:].numpy(), target_probs=tp, draft_probs=dp, uniform=u)[:2]
         np.testing.assert_array_equal(m.accepted.cpu().numpy(), ea)
         np.testing.assert_array_equal(m.out_tokens.cpu().numpy(), eo)
         accepted.append(ea.mean())

@@ -12,8 +12,8 @@ from oracle import oracle as orc  # noqa: E402
 from rtp_llm_b200 import ops  # noqa: E402
 from rtp_llm_b200.decode_step import TINY, DecodeStep  # noqa: E402
 from tests import gpu_probe as probe  # noqa: E402
-from tests.spec_oracle import spec_verify_np  # noqa: E402
 from tests.step_oracle import TINY31, check_logits, check_step  # noqa: E402
+from tests.verify_oracle import chain_verify_np  # noqa: E402
 
 DEV = torch.device("cuda")
 TILES = "B200_ATTN_TILES_PER_SPLIT"
@@ -112,18 +112,26 @@ def test_rope_append_multi_equals_single_token_appends(case):
 V_FULL = 128256
 
 
-def _check_draws(got, exp, acc_got, acc_exp, masses, u):
-    """Accept decisions exact; a drawn token exact unless u * total lies within 1e-6 * total of a CDF boundary. There the
-    kernel's fp32 scan may pick another token with mass, whose CDF interval must then come within 1e-6 * total of u * total
-    (in a tail of tiny probabilities that can be a few tokens away, not only a neighbour)."""
-    np.testing.assert_array_equal(acc_got, acc_exp)
+def check_verify(got, expected, u):
+    """A verifier's outputs `got` (out_tokens, accepted[, accepted_path]) against verify_np's `expected`, u [B] the draw's
+    uniforms. Accept decisions and the path exact; a drawn token exact unless u * total lies within 1e-6 * total of a CDF
+    boundary of the mass the draw used. There the kernel's fp32 scan may pick another token with mass, whose CDF interval must
+    then come within 1e-6 * total of u * total (in a tail of tiny probabilities that can be a few tokens away, not only a
+    neighbour)."""
+    got = [x.cpu().numpy() for x in got]
+    exp, acc_exp, path_exp, masses = expected
+    u = np.asarray(u, np.float64)
+    np.testing.assert_array_equal(got[1], acc_exp)
+    if len(got) > 2:
+        np.testing.assert_array_equal(got[2], path_exp)
+    got = got[0]
     for b in range(got.shape[0]):
         a = acc_exp[b]
         np.testing.assert_array_equal(got[b, :a], exp[b, :a])
         assert (got[b, a + 1:] == -1).all()
         if got[b, a] == exp[b, a]:
             continue
-        m = masses(b, a).astype(np.float64)
+        m = masses[b].astype(np.float64)
         idx = np.nonzero(m > 0)[0]
         c = np.cumsum(m[idx])
         total, t = c[-1], u[b] * c[-1]
@@ -143,7 +151,7 @@ def test_spec_verify_greedy_vs_oracle(n):
     keep = rng.random((B, n)) < 0.8
     drafts = np.where(keep, ids[:, :n], rng.integers(0, V_FULL, (B, n))).astype(np.int32)
     out, acc = ops.spec_verify(torch.from_numpy(drafts).to(DEV), target_ids=torch.from_numpy(ids).to(DEV))
-    eo, ea = spec_verify_np(drafts, target_ids=ids)
+    eo, ea = chain_verify_np(drafts, target_ids=ids)[:2]
     np.testing.assert_array_equal(acc.cpu().numpy(), ea)
     np.testing.assert_array_equal(out.cpu().numpy(), eo)
 
@@ -174,17 +182,11 @@ def test_spec_verify_sampling_vs_oracle(n, with_draft_probs):
     u = rng.random((B, n + 1)).astype(np.float32)
     u[2, 0] = 0.9                                   # rejects row 2's first draft in both modes
     T = lambda a: None if a is None else torch.from_numpy(np.ascontiguousarray(a)).to(DEV)
-    out, acc = ops.spec_verify(T(drafts), target_probs=T(t), draft_probs=T(dp), uniform=T(u))
-    eo, ea = spec_verify_np(drafts, target_probs=t, draft_probs=dp, uniform=u)
-    got, acc_got = out.cpu().numpy(), acc.cpu().numpy()
-
-    def masses(b, a):
-        if a == n:
-            return np.where(t[b, n] > 0, t[b, n], 0)
-        draft = dp[b, a] if dp is not None else (np.arange(V_FULL) == drafts[b, a]).astype(np.float32)
-        r = np.maximum(np.float32(0), t[b, a] - draft)
-        return r if r.astype(np.float64).sum() > 0 else np.where(t[b, a] > 0, t[b, a], 0)
-    _check_draws(got, eo, acc_got, ea, masses, u[:, n].astype(np.float64))
+    got = ops.spec_verify(T(drafts), target_probs=T(t), draft_probs=T(dp), uniform=T(u))
+    exp = chain_verify_np(drafts, target_probs=t, draft_probs=dp, uniform=u)
+    check_verify(got, exp, u[:, n])
+    eo, ea = exp[:2]
+    got = got[0].cpu().numpy()
     assert ea[0] == 0 and eo[0, 0] == -1                   # mass-free row: rejected, nothing to draw
     assert ea[2] == 0 and got[2, 0] >= 0
     if with_draft_probs:
@@ -242,5 +244,5 @@ def test_verification_step_accepts_the_tokens_plain_steps_produce(cfg, k):
     assert (acc[sure] == k).all(), acc
     np.testing.assert_array_equal(out[sure, k], toks[k + 1].numpy()[sure])
     np.testing.assert_array_equal(out[sure, :k], torch.stack(toks[1:k + 1], dim=1).numpy()[sure])
-    eo, ea = spec_verify_np(spec.ids_h[:, 1:].numpy(), target_ids=spec.next_ids.view(spec.B, k + 1).cpu().numpy())
+    eo, ea = chain_verify_np(spec.ids_h[:, 1:].numpy(), target_ids=spec.next_ids.view(spec.B, k + 1).cpu().numpy())[:2]
     np.testing.assert_array_equal(acc, ea)

@@ -1,6 +1,6 @@
 """GPU tests (H100) of DecodeStep's token-tree mode: a chain tree is the chain verification step bit for bit; a tree whose greedy
 branch is not the first child accepts the plain steps' tokens along that branch; the verifier's decisions are those of
-tests/tree_oracle.py on the step's own rows; and after the step the accepted path's K/V sit at slots seq .. seq + accepted."""
+tests/verify_oracle.py on the step's own rows; and after the step the accepted path's K/V sit at slots seq .. seq + accepted."""
 import dataclasses
 
 import numpy as np
@@ -12,7 +12,7 @@ pytestmark = pytest.mark.gpu
 from rtp_llm_b200 import ops  # noqa: E402
 from rtp_llm_b200.decode_step import TINY, DecodeStep, SamplingParams  # noqa: E402
 from tests.step_oracle import TINY31, check_logits  # noqa: E402
-from tests.tree_oracle import tree_verify_np  # noqa: E402
+from tests.verify_oracle import verify_np  # noqa: E402
 
 DEV = torch.device("cuda")
 MODES = ["eager", "graph", "pdl", "graph pdl"]
@@ -60,7 +60,7 @@ def test_tree_step_follows_the_greedy_branch_of_plain_steps(cfg, mode):
     """Two greedy single-token steps on one model, then one tree step on an identical model whose second child of the root and
     second child of that node carry those tokens and whose first children are decoys. The path rows' logits match the plain
     steps; where every plain step's top-2 margin is clear of the error, the tree accepts 2 along [0, 2, 4] and emits plain step
-    2's token; everywhere the decisions are tree_verify_np's on the step's own rows; and the K/V of nodes 2 and 4 end at slots
+    2's token; everywhere the decisions are verify_np's on the step's own rows; and the K/V of nodes 2 and 4 end at slots
     seq + 1 and seq + 2."""
     plain = DecodeStep(cfg, 4, 40, DEV, ragged=True, seed=2)
     tree = DecodeStep(cfg, 4, 40, DEV, ragged=True, seed=2, q_len=5, tree=BRANCH, pdl="pdl" in mode)
@@ -89,7 +89,7 @@ def test_tree_step_follows_the_greedy_branch_of_plain_steps(cfg, mode):
     assert (acc[sure] == 2).all(), acc
     assert (path[sure] == [0, 2, 4, -1, -1]).all(), path
     np.testing.assert_array_equal(out[sure, :3], torch.stack(toks[1:4], dim=1).numpy()[sure])
-    eo, ea, ep = tree_verify_np(np.tile(BRANCH, (tree.B, 1)), tree.ids_h.numpy(), target_ids=tree.next_ids.view(tree.B, 5).cpu().numpy())
+    eo, ea, ep, _ = verify_np(np.tile(BRANCH, (tree.B, 1)), tree.ids_h.numpy(), target_ids=tree.next_ids.view(tree.B, 5).cpu().numpy())
     np.testing.assert_array_equal(acc, ea)
     np.testing.assert_array_equal(out, eo)
     np.testing.assert_array_equal(path, ep)

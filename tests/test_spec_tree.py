@@ -1,14 +1,12 @@
 """CPU tests of speculative token-tree verification: the argument checks of b200_paged_decode_attn_tree, b200_spec_verify_tree
-and b200_kv_compact_path (rejected on the host before any CUDA call), and the numpy references of tests/tree_oracle.py, which
-on a chain must be the chain verifier spec_verify_np."""
+and b200_kv_compact_path (rejected on the host before any CUDA call), and the numpy references of tests/verify_oracle.py."""
 import ctypes
 
 import numpy as np
 import pytest
 
 from rtp_llm_b200 import _lib
-from tests.spec_oracle import spec_verify_np
-from tests.tree_oracle import ancestors, compact_np, random_tree, tree_verify_np
+from tests.verify_oracle import ancestors, compact_np, verify_np
 
 
 @pytest.fixture(scope="module")
@@ -86,38 +84,11 @@ def test_ancestor_walk():
     assert ancestors([7, 0, 2, 5, 3]) == [[0], [0, 1], [2], [3], [3, 4]]
 
 
-@pytest.mark.parametrize("seed", range(4))
-def test_tree_oracle_is_the_chain_oracle_on_chains(seed):
-    rng = np.random.default_rng(seed)
-    B, n, V = 48, int(rng.integers(2, 9)), 30
-    par = np.tile(random_tree(rng, n, "chain"), (B, 1))
-    ids = rng.integers(0, V, (B, n))
-    toks = np.where(rng.random((B, n)) < 0.7, np.roll(ids, 1, axis=1), rng.integers(0, V, (B, n)))
-    toks[:, 0] = -5                                                          # the root's entry is never read
-    g_tree = tree_verify_np(par, toks, target_ids=ids)
-    g_chain = spec_verify_np(toks[:, 1:], target_ids=ids)
-    np.testing.assert_array_equal(g_tree[0], g_chain[0])
-    np.testing.assert_array_equal(g_tree[1], g_chain[1])
-    t = rng.random((B, n, V)).astype(np.float32) ** 3
-    t[:, :, rng.integers(0, V)] = 0                                          # some draft tokens without mass
-    t /= t.sum(-1, keepdims=True)
-    toks2 = np.concatenate([toks[:, :1], np.array([[rng.choice(V, p=t[b, i].astype(np.float64) / t[b, i].astype(np.float64).sum())
-                                                     for i in range(n - 1)] for b in range(B)])], axis=1)
-    u = rng.random((B, n)).astype(np.float32)
-    s_tree = tree_verify_np(par, toks2, target_probs=t, uniform=u)
-    s_chain = spec_verify_np(toks2[:, 1:], target_probs=t, uniform=u)
-    np.testing.assert_array_equal(s_tree[0], s_chain[0])
-    np.testing.assert_array_equal(s_tree[1], s_chain[1])
-    for b in range(B):
-        np.testing.assert_array_equal(s_tree[2][b], [i if i <= s_tree[1][b] else -1 for i in range(n)])
-    assert 0 < s_tree[1].mean() < n - 1
-
-
 def test_tree_oracle_greedy_takes_the_first_matching_child_and_stops_at_none():
     par = np.array([[-1, 0, 0, 2, 2, 1]])
     toks = np.array([[0, 5, 7, 9, 8, 4]])
     ids = np.array([[7, 0, 8, 0, 3, 0]])                                     # root wants 7 (node 2), node 2 wants 8 (node 4)
-    out, acc, path = tree_verify_np(par, toks, target_ids=ids)
+    out, acc, path, _ = verify_np(par, toks, target_ids=ids)
     assert acc[0] == 2 and list(path[0]) == [0, 2, 4, -1, -1, -1] and list(out[0]) == [7, 8, 3, -1, -1, -1]
 
 
@@ -134,7 +105,7 @@ def test_tree_oracle_multi_round_rejection_reproduces_the_target():
         P = np.zeros(4)
         for u0 in grid:
             for u1 in grid:
-                out, acc, _ = tree_verify_np(par, toks, target_probs=probs, uniform=np.array([[u0, u1, 0.5]], np.float32))
+                out, acc, _, _ = verify_np(par, toks, target_probs=probs, uniform=np.array([[u0, u1, 0.5]], np.float32))
                 if acc[0] == 1:
                     P[out[0, 0]] += 1
                 else:                                                    # both rejected: the residual, exactly

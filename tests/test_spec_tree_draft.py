@@ -1,7 +1,6 @@
-"""CPU tests of sampled tree verification with draft rows (b200_spec_verify_tree_draft): the rule of tests/draft_tree_oracle.py
-emits the target's distribution exactly (SpecInfer's theorem, in float64 over every draft and uniform), is the deterministic-
-draft rule with one-hot rows and the chain rule on chains; and the host checks of the C entry, of ops and of DecodeStep's
-draft_probs option."""
+"""CPU tests of sampled tree verification with draft rows (b200_spec_verify_tree_draft): the rule of tests/verify_oracle.py
+emits the target's distribution exactly (SpecInfer's theorem, in float64 over every draft and uniform) and is the deterministic-
+draft rule with one-hot rows; and the host checks of the C entry, of ops and of DecodeStep's draft_probs option."""
 import ctypes
 
 import numpy as np
@@ -10,10 +9,7 @@ import torch
 
 from rtp_llm_b200 import _lib, ops
 from rtp_llm_b200.decode_step import TINY, DecodeStep, SamplingParams
-from tests.draft_tree_oracle import (block_sum_f32, exact_emitted, extend, target_joint, tree_draft_verify_np,
-                                     verify_measure)
-from tests.spec_oracle import spec_verify_np
-from tests.tree_oracle import random_tree, tree_verify_np
+from tests.verify_oracle import block_sum_f32, exact_emitted, extend, random_tree, target_joint, verify_measure, verify_np
 
 
 def _row(key, V, zeros):
@@ -114,30 +110,11 @@ def test_fp32_oracle_with_one_hot_rows_decides_as_the_deterministic_oracle(seed)
         for c in range(1, n):
             dp[b, c, toks[b, c]] = 1.0
     u = rng.random((B, n)).astype(np.float32)
-    got = tree_draft_verify_np(par, toks, t, dp, u)
-    exp = tree_verify_np(par, toks, target_probs=t, uniform=u)
-    for g, e in zip(got, exp):
+    got = verify_np(par, toks, target_probs=t, draft_probs=dp, uniform=u)
+    exp = verify_np(par, toks, target_probs=t, uniform=u)
+    for g, e in zip(got[:3], exp[:3]):
         np.testing.assert_array_equal(g, e)
     assert 0 < got[1].mean()
-
-
-@pytest.mark.parametrize("seed", range(4))
-def test_fp32_oracle_on_chains_is_the_chain_oracle_with_draft_probs(seed):
-    rng = np.random.default_rng(10 + seed)
-    B, n, V = 48, int(rng.integers(2, 9)), 50
-    par = np.tile(random_tree(rng, n, "chain"), (B, 1))
-    t = _probs(rng, (B, n, V), 0.4, zeros=0.2)
-    dp = (0.5 * t + 0.5 * _probs(rng, (B, n, V), 0.4, zeros=0.3)).astype(np.float32)
-    toks = np.array([[-1] + [rng.choice(V, p=dp[b, c].astype(np.float64) / dp[b, c].astype(np.float64).sum())
-                             for c in range(1, n)] for b in range(B)])
-    toks[1, 1] = V + 3                                                       # a token outside the vocabulary: rejected
-    dp[2, 1, toks[2, 1]] = 0.0                                               # draft probability 0: accepted when q > 0
-    u = rng.random((B, n)).astype(np.float32)
-    got = tree_draft_verify_np(par, toks, t, dp, u)
-    exp = spec_verify_np(toks[:, 1:], target_probs=t, draft_probs=dp[:, 1:], uniform=u)
-    np.testing.assert_array_equal(got[0], exp[0])
-    np.testing.assert_array_equal(got[1], exp[1])
-    assert got[1][1] == 0 and 0 < got[1].mean() < n - 1
 
 
 def test_block_sum_order():

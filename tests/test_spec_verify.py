@@ -1,5 +1,5 @@
 """CPU tests of speculative-token verification: the argument checks of the new entry points (rejected on the host before any
-CUDA call), and the numpy reference spec_verify_np (tests/spec_oracle.py), whose chain rejection sampling must reproduce the
+CUDA call), and the numpy reference chain_verify_np (tests/verify_oracle.py), whose chain rejection sampling must reproduce the
 target distribution exactly (the property the reference's speculative-sampling kernel rests on)."""
 import ctypes
 
@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 
 from rtp_llm_b200 import _lib
-from tests.spec_oracle import spec_verify_np
+from tests.verify_oracle import chain_verify_np
 
 
 @pytest.fixture(scope="module")
@@ -70,7 +70,7 @@ def test_decode_step_rejects_unsupported_verification_shapes():
 def _first_token(d, target, draft_probs, u0, u1):
     t = np.stack([target, target]).astype(np.float32)[None]                  # [1, n+1 = 2, V]: row 1 is never reached here
     dp = None if draft_probs is None else draft_probs.astype(np.float32)[None, None]
-    out, _ = spec_verify_np(np.array([[d]]), target_probs=t, draft_probs=dp, uniform=np.array([[u0, u1]]))
+    out = chain_verify_np(np.array([[d]]), target_probs=t, draft_probs=dp, uniform=np.array([[u0, u1]]))[0]
     return int(out[0, 0])
 
 
@@ -157,8 +157,8 @@ def test_greedy_mode_equals_sampling_with_one_hot_targets():
     drafts = np.where(rng.random((B, n)) < 0.7, ids[:, :n], rng.integers(0, V, (B, n)))
     onehot = np.zeros((B, n + 1, V), np.float32)
     np.put_along_axis(onehot, ids[..., None], 1.0, axis=-1)
-    g = spec_verify_np(drafts, target_ids=ids)
-    s = spec_verify_np(drafts, target_probs=onehot, uniform=rng.random((B, n + 1)).astype(np.float32))
+    g = chain_verify_np(drafts, target_ids=ids)
+    s = chain_verify_np(drafts, target_probs=onehot, uniform=rng.random((B, n + 1)).astype(np.float32))
     np.testing.assert_array_equal(g[0], s[0])
     np.testing.assert_array_equal(g[1], s[1])
     assert 0 < g[1].mean() < n
@@ -171,8 +171,8 @@ def test_drafts_with_the_target_probabilities_are_all_accepted():
     t /= t.sum(-1, keepdims=True)
     t64 = t.astype(np.float64)
     drafts = np.array([[rng.choice(V, p=t64[b, i] / t64[b, i].sum()) for i in range(n)] for b in range(B)])
-    out, acc = spec_verify_np(drafts, target_probs=t, draft_probs=t[:, :n].copy(),
-                              uniform=(rng.random((B, n + 1)) * 0.999).astype(np.float32))
+    out, acc = chain_verify_np(drafts, target_probs=t, draft_probs=t[:, :n].copy(),
+                               uniform=(rng.random((B, n + 1)) * 0.999).astype(np.float32))[:2]
     assert (acc == n).all()
     np.testing.assert_array_equal(out[:, :n], drafts)
     assert (out[:, n] >= 0).all()
